@@ -374,7 +374,7 @@ int gib_seg_softmax(float* out, const float* EM, const float* EN, int ld, const 
 }
 int gib_gru_gates(float* hn, const float* gi, const float* gh, const float* h, int Hp, const int* ptr, long long S,
                   gib_stream stream) {
-  return gru_fwd(hn, gi, gh, h, Hp, ptr, S, ST(stream));
+  return gru_fwd(hn, gi, gh, h, Hp, ptr, S, nullptr, ST(stream));
 }
 int gib_graph_gather(float* g, float* att, const float* en, const float* em, int ld, const int* ptr, int N, int B,
                      float big, gib_stream stream) {

@@ -9,6 +9,16 @@ namespace gib {
 
 #define GIB_1D(total, threads) (unsigned)ceil_div_ll((long long)(total), (threads)), (threads)
 
+// Live rows of a buffer of `rows` bond rows.  Capacity mode passes the device int K0 wrote (the entry count of the
+// one untyped EMN group): the grid is sized from the capacity, and the threads at or past the live count exit before
+// any index load.  A count above the capacity (an overflowing batch) is clamped to it.  live == nullptr (exact mode):
+// every row is live.
+__device__ __forceinline__ long long live_rows(const int* live, long long rows) {
+  if (!live) return rows;
+  const long long n = __ldg(live);
+  return n < 0 ? 0 : (n < rows ? n : rows);
+}
+
 // ------------------------------------------------------------------------------------
 // concat2: dst[r, :] = [ a[r, :wa] | b[r, :wb] | 0 ... ]      (dst width = ldd)
 // reference: summation_mpnn.py:121-125 (zero-pad node features), modules.py:46 (cat(hidden, input))
@@ -124,38 +134,42 @@ int sum3_cols(float* dst, int ldd, int W, const float* a, int lda, int offa, con
   return 0;
 }
 
-// y = tanh(x) elementwise (EMN edge embedding, mpnn.py:469), and its backward
-__global__ void tanh_fwd_kernel(float* __restrict__ y, const float* __restrict__ x, long long n) {
+// y = tanh(x) elementwise over rows x ld (EMN edge embedding, mpnn.py:469), and its backward
+__global__ void tanh_fwd_kernel(float* __restrict__ y, const float* __restrict__ x, long long rows, int ld,
+                                const int* __restrict__ live) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n) y[i] = tanhf(x[i]);
+  if (i < live_rows(live, rows) * ld) y[i] = tanhf(x[i]);
 }
-int tanh_fwd(float* y, const float* x, long long n, cudaStream_t st) {
-  if (n <= 0) return 0;
-  tanh_fwd_kernel<<<GIB_1D(n, 256), 0, st>>>(y, x, n);
+int tanh_fwd(float* y, const float* x, long long rows, int ld, const int* live, cudaStream_t st) {
+  if (rows <= 0) return 0;
+  tanh_fwd_kernel<<<GIB_1D(rows * ld, 256), 0, st>>>(y, x, rows, ld, live);
   GIB_LAUNCH_CHECK();
   return 0;
 }
 // G = dy * (1 - y^2) * selu'(pre)   where pre is the SELU output that fed tanh
 __global__ void tanh_selu_bwd_kernel(float* __restrict__ G, const float* __restrict__ dy, const float* __restrict__ y,
-                                     const float* __restrict__ pre, long long n) {
+                                     const float* __restrict__ pre, long long rows, int ld,
+                                     const int* __restrict__ live) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n) G[i] = dy[i] * (1.f - y[i] * y[i]) * dselu_from_out(pre[i]);
+  if (i < live_rows(live, rows) * ld) G[i] = dy[i] * (1.f - y[i] * y[i]) * dselu_from_out(pre[i]);
 }
-int tanh_selu_bwd(float* G, const float* dy, const float* y, const float* pre, long long n, cudaStream_t st) {
-  if (n <= 0) return 0;
-  tanh_selu_bwd_kernel<<<GIB_1D(n, 256), 0, st>>>(G, dy, y, pre, n);
+int tanh_selu_bwd(float* G, const float* dy, const float* y, const float* pre, long long rows, int ld,
+                  const int* live, cudaStream_t st) {
+  if (rows <= 0) return 0;
+  tanh_selu_bwd_kernel<<<GIB_1D(rows * ld, 256), 0, st>>>(G, dy, y, pre, rows, ld, live);
   GIB_LAUNCH_CHECK();
   return 0;
 }
 
 // ------------------------------------------------------------------------------------
-// gather_rows: X0[p, :] = (scale ? w_p : 1) * h[src_p, :]      (pad rows -> 0)
+// gather_rows: X0[p, :] = (scale ? w_p : 1) * h[src_p, :]      (pad rows -> 0; rows at or past *live are not written)
 // reference: summation_mpnn.py:131 (`hidden_nodes[b, nghb]`) + mpnn.py:286-288 (edge-value scaling)
 // ------------------------------------------------------------------------------------
 __global__ void gather_rows_kernel(float4* __restrict__ dst, const float4* __restrict__ h, int ld4,
-                                   const int* __restrict__ src, const float* __restrict__ w, int scale, long long P) {
+                                   const int* __restrict__ src, const float* __restrict__ w, int scale, long long P,
+                                   const int* __restrict__ live) {
   const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (idx >= P * ld4) return;
+  if (idx >= live_rows(live, P) * ld4) return;
   const long long p = idx / ld4;
   const int c = (int)(idx % ld4);
   const int s = __ldg(src + p);
@@ -170,10 +184,11 @@ __global__ void gather_rows_kernel(float4* __restrict__ dst, const float4* __res
   dst[idx] = v;
 }
 int gather_rows(float* dst, const float* h, int ld, const int* src, const float* w, int scale, long long P,
-                cudaStream_t st) {
+                const int* live, cudaStream_t st) {
   if (P <= 0) return 0;
   gather_rows_kernel<<<GIB_1D(P * (ld / 4), 256), 0, st>>>(reinterpret_cast<float4*>(dst),
-                                                          reinterpret_cast<const float4*>(h), ld / 4, src, w, scale, P);
+                                                          reinterpret_cast<const float4*>(h), ld / 4, src, w, scale, P,
+                                                          live);
   GIB_LAUNCH_CHECK();
   return 0;
 }
@@ -404,12 +419,14 @@ int seg_softmax_bwd(float* GM, float* GN, const float* dM, const float* EM, cons
 // gi, gh: [S, 3*Hp] gate-blocked (gate g at columns g*Hp..).  h == nullptr means h = 0 and
 // gh is a single bias row (EMN: `self.gru(message)` with hx=None, mpnn.py:488).
 // Slots whose CSR row is empty keep their state (summation_mpnn.py:143-144 updates only
-// the nodes that have a bond).  ptr == nullptr: every row is active.
+// the nodes that have a bond).  ptr == nullptr: every row is active.  live (EMN bond rows, capacity mode): rows at or
+// past *live are neither read nor written.
 // ------------------------------------------------------------------------------------
 __global__ void gru_fwd_kernel(float* __restrict__ hn, const float* __restrict__ gi, const float* __restrict__ gh,
-                               const float* __restrict__ h, int Hp, const int* __restrict__ ptr, long long S) {
+                               const float* __restrict__ h, int Hp, const int* __restrict__ ptr, long long S,
+                               const int* __restrict__ live) {
   const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (idx >= S * Hp) return;
+  if (idx >= live_rows(live, S) * Hp) return;
   const long long s = idx / Hp;
   const int c = (int)(idx % Hp);
   const float hv = h ? h[idx] : 0.f;
@@ -426,9 +443,9 @@ __global__ void gru_fwd_kernel(float* __restrict__ hn, const float* __restrict__
   hn[idx] = res;
 }
 int gru_fwd(float* hn, const float* gi, const float* gh, const float* h, int Hp, const int* ptr, long long S,
-            cudaStream_t st) {
+            const int* live, cudaStream_t st) {
   if (S <= 0) return 0;
-  gru_fwd_kernel<<<GIB_1D(S * Hp, 256), 0, st>>>(hn, gi, gh, h, Hp, ptr, S);
+  gru_fwd_kernel<<<GIB_1D(S * Hp, 256), 0, st>>>(hn, gi, gh, h, Hp, ptr, S, live);
   GIB_LAUNCH_CHECK();
   return 0;
 }
@@ -436,9 +453,9 @@ int gru_fwd(float* hn, const float* gi, const float* gh, const float* h, int Hp,
 __global__ void gru_bwd_kernel(float* __restrict__ dgi, float* __restrict__ dgh, float* __restrict__ dh_direct,
                                const float* __restrict__ dhn, const float* __restrict__ gi,
                                const float* __restrict__ gh, const float* __restrict__ h, int Hp,
-                               const int* __restrict__ ptr, long long S) {
+                               const int* __restrict__ ptr, long long S, const int* __restrict__ live) {
   const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (idx >= S * Hp) return;
+  if (idx >= live_rows(live, S) * Hp) return;
   const long long s = idx / Hp;
   const int c = (int)(idx % Hp);
   const float d = dhn[idx];
@@ -469,20 +486,22 @@ __global__ void gru_bwd_kernel(float* __restrict__ dgi, float* __restrict__ dgh,
   if (dh_direct) dh_direct[idx] = dd;
 }
 int gru_bwd(float* dgi, float* dgh, float* dh_direct, const float* dhn, const float* gi, const float* gh,
-            const float* h, int Hp, const int* ptr, long long S, cudaStream_t st) {
+            const float* h, int Hp, const int* ptr, long long S, const int* live, cudaStream_t st) {
   if (S <= 0) return 0;
-  gru_bwd_kernel<<<GIB_1D(S * Hp, 256), 0, st>>>(dgi, dgh, dh_direct, dhn, gi, gh, h, Hp, ptr, S);
+  gru_bwd_kernel<<<GIB_1D(S * Hp, 256), 0, st>>>(dgi, dgh, dh_direct, dhn, gi, gh, h, Hp, ptr, S, live);
   GIB_LAUNCH_CHECK();
   return 0;
 }
 
-// column sums: out[r] += sum_m G[m, prow(r)]  (bias gradient when no dW GEMM runs alongside)
+// column sums: out[r] += sum_m G[m, prow(r)]  (bias gradient when no dW GEMM runs alongside).  live: sum over the
+// first *live of the M rows only, in the same order as an exact-size launch over those rows
 __global__ void colsum_kernel(float* __restrict__ out, const float* __restrict__ G, int ldg, long long M, int R,
-                              int Rb, int Rbp) {
+                              int Rb, int Rbp, const int* __restrict__ live) {
   // one CTA per 32 columns, 8 warps stride over rows; fixed-order tree at the end
   __shared__ float sm[8][33];
   const int r = blockIdx.x * 32 + (threadIdx.x & 31);
   const int wy = threadIdx.x >> 5;
+  M = live_rows(live, M);
   float s = 0.f;
   if (r < R) {
     const int prow = (r / Rb) * Rbp + (r % Rb);
@@ -496,9 +515,10 @@ __global__ void colsum_kernel(float* __restrict__ out, const float* __restrict__
     out[r] += t;
   }
 }
-int colsum_add(float* out, const float* G, int ldg, long long M, int R, int Rb, int Rbp, cudaStream_t st) {
+int colsum_add(float* out, const float* G, int ldg, long long M, int R, int Rb, int Rbp, const int* live,
+               cudaStream_t st) {
   if (M <= 0 || R <= 0) return 0;
-  colsum_kernel<<<ceil_div(R, 32), 256, 0, st>>>(out, G, ldg, M, R, Rb, Rbp);
+  colsum_kernel<<<ceil_div(R, 32), 256, 0, st>>>(out, G, ldg, M, R, Rb, Rbp, live);
   GIB_LAUNCH_CHECK();
   return 0;
 }
@@ -604,6 +624,9 @@ int bcast_nodes_add(float* dh, const float* dg, int ld, int N, long long S, cuda
 // EMN (edge memory network) kernels: edge_mpnn.py:104-192, mpnn.py:466-488
 // bond r = (b, i, j): ent_dst = slot of i, ent_src = slot of j.  Entries are untyped (one
 // group) and in reference order, so entry row == bond index r and dst_ent is the identity.
+// Capacity mode: E is the capacity and `live` the device-side bond count; rows [live, E) are pad rows (ent_src =
+// ent_dst = -1) or, after an overflow, bonds past the capacity.  The aggregation kernels skip them: the live rows
+// never read a row at or past the live count (K0 clamps dst_ptr / src_ptr to the capacity).
 // ------------------------------------------------------------------------------------
 // X[r, :] = [ nodes[i, :F] | nodes[j, :F] | edges[i, j, :Ef] | 0 ]
 __global__ void emn_input_kernel(float* __restrict__ X, int ld, const void* __restrict__ nodes,
@@ -638,9 +661,10 @@ __global__ void __launch_bounds__(256) emn_aggregate_fwd_kernel(float* __restric
                                                                 const float* __restrict__ ENm, int ld,
                                                                 const int* __restrict__ ent_dst,
                                                                 const int* __restrict__ ent_src,
-                                                                const int* __restrict__ dst_ptr, long long E) {
+                                                                const int* __restrict__ dst_ptr, long long E,
+                                                                const int* __restrict__ live) {
   const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (idx >= E * ld) return;
+  if (idx >= live_rows(live, E) * ld) return;
   const long long r = idx / ld;
   const int c = (int)(idx % ld);
   const int si = __ldg(ent_dst + r), sj = __ldg(ent_src + r);
@@ -660,9 +684,11 @@ __global__ void __launch_bounds__(256) emn_aggregate_fwd_kernel(float* __restric
   msg[idx] = num / den;
 }
 int emn_aggregate_fwd(float* msg, const float* EMx, const float* ENx, const float* EMm, const float* ENm, int ld,
-                      const int* ent_dst, const int* ent_src, const int* dst_ptr, long long E, cudaStream_t st) {
+                      const int* ent_dst, const int* ent_src, const int* dst_ptr, long long E, const int* live,
+                      cudaStream_t st) {
   if (E <= 0) return 0;
-  emn_aggregate_fwd_kernel<<<GIB_1D(E * ld, 256), 0, st>>>(msg, EMx, ENx, EMm, ENm, ld, ent_dst, ent_src, dst_ptr, E);
+  emn_aggregate_fwd_kernel<<<GIB_1D(E * ld, 256), 0, st>>>(msg, EMx, ENx, EMm, ENm, ld, ent_dst, ent_src, dst_ptr, E,
+                                                           live);
   GIB_LAUNCH_CHECK();
   return 0;
 }
@@ -674,9 +700,10 @@ __global__ void __launch_bounds__(256) emn_aggregate_bwd_recv_kernel(
     float* __restrict__ dEMx, float* __restrict__ dENx, float* __restrict__ st_mx, float* __restrict__ st_inv,
     float* __restrict__ st_dot, const float* __restrict__ dmsg, const float* __restrict__ EMx,
     const float* __restrict__ ENx, const float* __restrict__ EMm, const float* __restrict__ ENm, int ld,
-    const int* __restrict__ ent_dst, const int* __restrict__ ent_src, const int* __restrict__ dst_ptr, long long E) {
+    const int* __restrict__ ent_dst, const int* __restrict__ ent_src, const int* __restrict__ dst_ptr, long long E,
+    const int* __restrict__ live) {
   const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (idx >= E * ld) return;
+  if (idx >= live_rows(live, E) * ld) return;
   const long long r = idx / ld;
   const int c = (int)(idx % ld);
   const int si = __ldg(ent_dst + r), sj = __ldg(ent_src + r);
@@ -708,9 +735,11 @@ __global__ void __launch_bounds__(256) emn_aggregate_bwd_send_kernel(
     float* __restrict__ dEMm, float* __restrict__ dENm, const float* __restrict__ st_mx,
     const float* __restrict__ st_inv, const float* __restrict__ st_dot, const float* __restrict__ dmsg,
     const float* __restrict__ EMm, const float* __restrict__ ENm, int ld, const int* __restrict__ ent_dst,
-    const int* __restrict__ ent_src, const int* __restrict__ src_ptr, const int* __restrict__ src_ent, long long E) {
+    const int* __restrict__ ent_src, const int* __restrict__ src_ptr, const int* __restrict__ src_ent, long long E,
+    const int* __restrict__ live) {
   const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (idx >= E * ld) return;
+  const long long m = live_rows(live, E);
+  if (idx >= m * ld) return;
   const long long s = idx / ld;
   const int c = (int)(idx % ld);
   const int tail = __ldg(ent_dst + s);   // j: the atom bond s leaves from (its row)
@@ -720,6 +749,9 @@ __global__ void __launch_bounds__(256) emn_aggregate_bwd_send_kernel(
   float gm = 0.f, gn = 0.f;
   for (int q = q0; q < q1; ++q) {
     const int r = __ldg(src_ent + q);        // receiver r = (i, j): ent_src[r] == tail
+    // a receiver past the live count exists only in an overflowing batch (src_ent may name a bond the capacity cut
+    // off): it has no softmax state
+    if (r >= m) continue;
     if (__ldg(ent_dst + r) == head) continue;  // i == k: reverse bond excluded (edge_mpnn.py:158-160)
     const size_t o = (size_t)r * ld + c;
     const float a = expf(en - st_mx[o]) * st_inv[o];
@@ -732,29 +764,31 @@ __global__ void __launch_bounds__(256) emn_aggregate_bwd_send_kernel(
 }
 int emn_aggregate_bwd(float* dEMx, float* dENx, float* dEMm, float* dENm, float* st3, const float* dmsg,
                       const float* EMx, const float* ENx, const float* EMm, const float* ENm, int ld,
-                      const GraphArrays& ga, long long E, cudaStream_t st) {
+                      const GraphArrays& ga, long long E, const int* live, cudaStream_t st) {
   if (E <= 0) return 0;
   float* st_mx = st3;
   float* st_inv = st3 + (size_t)E * ld;
   float* st_dot = st3 + (size_t)2 * E * ld;
   emn_aggregate_bwd_recv_kernel<<<GIB_1D(E * ld, 256), 0, st>>>(dEMx, dENx, st_mx, st_inv, st_dot, dmsg, EMx, ENx, EMm,
-                                                               ENm, ld, ga.ent_dst, ga.ent_src, ga.dst_ptr, E);
+                                                               ENm, ld, ga.ent_dst, ga.ent_src, ga.dst_ptr, E, live);
   GIB_LAUNCH_CHECK();
   emn_aggregate_bwd_send_kernel<<<GIB_1D(E * ld, 256), 0, st>>>(dEMm, dENm, st_mx, st_inv, st_dot, dmsg, EMm, ENm, ld,
-                                                               ga.ent_dst, ga.ent_src, ga.src_ptr, ga.src_ent, E);
+                                                               ga.ent_dst, ga.ent_src, ga.src_ptr, ga.src_ent, E,
+                                                               live);
   GIB_LAUNCH_CHECK();
   return 0;
 }
 
 // elementwise helpers -------------------------------------------------------------------
+// G = d * selu'(y) over rows x ld
 __global__ void mul_dselu_kernel(float* __restrict__ G, const float* __restrict__ d, const float* __restrict__ y,
-                                 long long n) {
+                                 long long rows, int ld, const int* __restrict__ live) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n) G[i] = d[i] * dselu_from_out(y[i]);
+  if (i < live_rows(live, rows) * ld) G[i] = d[i] * dselu_from_out(y[i]);
 }
-int mul_dselu(float* G, const float* d, const float* y, long long n, cudaStream_t st) {
-  if (n <= 0) return 0;
-  mul_dselu_kernel<<<GIB_1D(n, 256), 0, st>>>(G, d, y, n);
+int mul_dselu(float* G, const float* d, const float* y, long long rows, int ld, const int* live, cudaStream_t st) {
+  if (rows <= 0) return 0;
+  mul_dselu_kernel<<<GIB_1D(rows * ld, 256), 0, st>>>(G, d, y, rows, ld, live);
   GIB_LAUNCH_CHECK();
   return 0;
 }

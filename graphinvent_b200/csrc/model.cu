@@ -212,7 +212,7 @@ int make_run(const gib_dims& d, const int* hdr, Run& r) {
   if (r.cap) {
     // capacity header (gib_graph_header_capacity): E / P are static capacities, the live counts stay in device memory;
     // every bond-type group is planned with the whole capacity and located through the device header at run time
-    if (d.model == GIB_EMN) { set_error("capacity mode is implemented for the node-state models (GGNN, MNN, AttentionGGNN)"); return -3; }
+    // (EMN: one untyped group, its bond rows [0, TYPE_COUNT[0]) of buffers of E rows)
     unsigned long long a = (unsigned)hdr[HDR_DEV_LO] | ((unsigned long long)(unsigned)hdr[HDR_DEV_HI] << 32);
     r.dev_hdr = reinterpret_cast<const int*>(a);
     if (!r.dev_hdr) { set_error("capacity header without a device header address"); return -1; }
@@ -401,7 +401,10 @@ static int mlp_forward_multi(const Run& r, const MlpJob* jobs, int n, int* flags
   for (int i = 1; i < n && same; ++i) same = jobs[i].m->n == jobs[0].m->n;
   if (!same) {
     for (int i = 0; i < n; ++i) {
-      if (jobs[i].m_dev) { set_error("mlp_forward_multi: device-side row counts need MLPs of equal depth"); return -2; }
+      if (jobs[i].m_dev) {   // device-side row counts need the grouped call pattern: one call per MLP
+        GIB_TRY(mlp_forward_multi(r, jobs + i, 1, flags));
+        continue;
+      }
       GIB_TRY(mlp_forward(r, *jobs[i].m, jobs[i].X0, *jobs[i].a, jobs[i].row0, jobs[i].rows, jobs[i].ext_out,
                           jobs[i].ext_ld, jobs[i].ext_valid));
     }
@@ -482,14 +485,23 @@ static int mlp_forward_multi(const Run& r, const MlpJob* jobs, int n, int* flags
 //       every G_l kept in its own buffer;
 //   (B) the weight gradients of ALL layers and members (dW_l = G_l^T X_{l-1}) as ONE grouped launch + ONE reduction;
 //   (C) the first layer's input gradient (if wanted).
-// plan_rows: expected total rows of the members of ONE layer (capacity mode: the entry capacity), 0 = their sum.
-static int mlp_backward_multi(const Run& r, const BwdBufs& bb, const MlpBwdJob* jobs, int n, long long plan_rows = 0) {
+// plan_rows: expected total rows of the members of ONE layer (capacity mode: the entry capacity the bond-type groups
+// share, or n x the capacity for the EMN's siblings, which each span it), 0 = their sum.
+// same_rows (capacity mode): the members run on the SAME device row range (the EMN's siblings) and keep one gradient
+// slice each; otherwise members with device row ranges are the disjoint bond-type groups of ONE buffer of `rows` rows
+// and share one slice.
+static int mlp_backward_multi(const Run& r, const BwdBufs& bb, const MlpBwdJob* jobs, int n, long long plan_rows = 0,
+                              bool same_rows = false) {
   bool same = n <= 4;
   for (int i = 1; i < n && same; ++i) same = jobs[i].m->n == jobs[0].m->n;
   const int depth = jobs[0].m->n;
   if (!same || depth > 8 || depth * n > kTc3MaxProblems) {
     for (int i = 0; i < n; ++i) {
-      if (jobs[i].m_dev) { set_error("mlp_backward_multi: device-side row counts need MLPs of equal depth"); return -2; }
+      if (jobs[i].m_dev) {
+        set_error("mlp_backward_multi: device-side row counts need <= 4 sibling MLPs of equal depth, at most 8 layers "
+                  "each and %d layers in all (got %d MLPs, depth of the first %d)", kTc3MaxProblems, n, depth);
+        return -2;
+      }
       GIB_TRY(mlp_backward(r, bb, *jobs[i].m, jobs[i].X0, *jobs[i].a, jobs[i].row0, jobs[i].rows, jobs[i].Gtop,
                            jobs[i].dX0, jobs[i].ld_dx, jobs[i].dx_aux));
     }
@@ -501,8 +513,8 @@ static int mlp_backward_multi(const Run& r, const BwdBufs& bb, const MlpBwdJob* 
   for (int i = 0; i < n; ++i) {
     G[depth][i] = jobs[i].Gtop;
     for (int l = 1; l < depth; ++l) G[l][i] = r.scratch + bb.Gl[l] + off;
-    // capacity mode: the members' live row ranges are disjoint parts of ONE buffer of `rows` rows -> shared slice
-    if (!jobs[i].m_dev) off += ((size_t)std::max(jobs[i].rows, 0) * mlp_max_ld(r.pl, *jobs[i].m) + 31) & ~(size_t)31;
+    if (!jobs[i].m_dev || same_rows)
+      off += ((size_t)std::max(jobs[i].rows, 0) * mlp_max_ld(r.pl, *jobs[i].m) + 31) & ~(size_t)31;
   }
   auto x_in = [&](const MlpBwdJob& j, int l, int* ld) -> const float* {   // input activations of layer l
     *ld = j.a->ld[l - 1];
@@ -719,7 +731,7 @@ static int node_model_forward(const Run& r, float* out) {
   for (int t = 0; t < d.T; ++t) {
     const float* h = r.ws + L.h[t];
     // mpnn.py:286-288 scales the neighbour state by the bond value for GGNN only
-    GIB_TRY(gather_rows(r.ws + L.x0[t], h, Hp, r.ga.ent_src, r.w(), d.model == GIB_GGNN, r.P, r.st));
+    GIB_TRY(gather_rows(r.ws + L.x0[t], h, Hp, r.ga.ent_src, r.w(), d.model == GIB_GGNN, r.P, nullptr, r.st));
     {   // one grouped launch per layer over the bond types (same input rows layout, per-type weights)
       MlpJob jobs[4];
       for (int g = 0; g < r.ngroups; ++g)
@@ -755,7 +767,7 @@ static int node_model_forward(const Run& r, float* out) {
       q2.work = 2.0 * S * (double)hh.R * hh.C;
       GIB_TRY(gemm_nt_group(ps, 2, r.st));
     }
-    GIB_TRY(gru_fwd(r.ws + L.h[t + 1], r.ws + L.gi[t], r.ws + L.gh[t], h, Hp, r.ga.dst_ptr, S, r.st));
+    GIB_TRY(gru_fwd(r.ws + L.h[t + 1], r.ws + L.gi[t], r.ws + L.gh[t], h, Hp, r.ga.dst_ptr, S, nullptr, r.st));
   }
   return readout_forward(r, out);
 }
@@ -780,7 +792,7 @@ static int node_model_backward(const Run& r, const BwdBufs& bb, const float* out
   for (int t = d.T - 1; t >= 0; --t) {
     const float* h = r.ws + L.h[t];
     GIB_TRY(gru_bwd(sc + bb.dgi, sc + bb.dgh, dh_dir, dh, r.ws + L.gi[t], r.ws + L.gh[t], h, Hp, r.ga.dst_ptr, S,
-                    r.st));
+                    nullptr, r.st));
     {   // weight gradients of the two GRU projections: one grouped launch
       GemmDW qs[2];
       GemmDW& q = qs[0];
@@ -854,6 +866,9 @@ static int node_model_backward(const Run& r, const BwdBufs& bb, const float* out
 // ------------------------------------------------------------------------------------
 // EMN
 // ------------------------------------------------------------------------------------
+// Capacity mode: E is the entry capacity; the live bond rows are [0, live) with live = TYPE_COUNT[0] in the device
+// header (the EMN's one untyped group starts at row 0).  Every MLP / GEMM runs on that device row range, every bond-row
+// kernel gets the count, and rows past it are neither written nor read by a live row.
 static int emn_forward(const Run& r, float* out) {
   const gib_dims& d = r.pl.d;
   const Plan& pl = r.pl;
@@ -861,39 +876,53 @@ static int emn_forward(const Run& r, float* out) {
   const int Hp = pl.Hp, E = r.E;
   const Lin& ih = pl.lins[pl.gru_ih];
   const Lin& hh = pl.lins[pl.gru_hh];
+  const int* live = type_count_dev(r, 0);
+  const int* base = type_base_dev(r, 0);
   GIB_TRY(emn_input(r.ws + L.xin, L.embnn.ld[0], r.nodes, r.edges, d.in_dtype, r.ga.ent_dst, r.ga.ent_src, d.N, d.F,
                     d.Ef, E, r.st));
   {   // the layers of an MLP run as one dependent-chain launch (mlp_forward_multi)
-    MlpJob j[1] = {{&pl.embnn, r.ws + L.xin, &L.embnn, 0, E, nullptr, 0, 0}};
+    MlpJob j[1] = {{&pl.embnn, r.ws + L.xin, &L.embnn, 0, E, nullptr, 0, 0, live, base}};
     GIB_TRY(mlp_forward_multi(r, j, 1, fwd_flags(r)));
   }
-  GIB_TRY(tanh_fwd(r.ws + L.xt, r.ws + L.embnn.y[pl.embnn.n], (long long)E * Hp, r.st));      // mpnn.py:469
+  GIB_TRY(tanh_fwd(r.ws + L.xt, r.ws + L.embnn.y[pl.embnn.n], E, Hp, live, r.st));      // mpnn.py:469
   {   // emb_msg_nn and att_msg_nn read the same rows: sibling chains in one launch
-    MlpJob j[2] = {{&pl.emsg, r.ws + L.xt, &L.emx, 0, E, nullptr, 0, 0}, {&pl.eatt, r.ws + L.xt, &L.enx, 0, E, nullptr, 0, 0}};
+    MlpJob j[2] = {{&pl.emsg, r.ws + L.xt, &L.emx, 0, E, nullptr, 0, 0, live, base},
+                   {&pl.eatt, r.ws + L.xt, &L.enx, 0, E, nullptr, 0, 0, live, base}};
     GIB_TRY(mlp_forward_multi(r, j, 2, fwd_flags(r)));
   }
   if (E > 0) GIB_CUDA_TRY(cudaMemsetAsync(r.ws + L.mem[0], 0, (size_t)E * Hp * sizeof(float), r.st));
   for (int t = 0; t < d.T; ++t) {
     {
-      MlpJob j[2] = {{&pl.emsg, r.ws + L.mem[t], &L.emm[t], 0, E, nullptr, 0, 0},
-                     {&pl.eatt, r.ws + L.mem[t], &L.enm[t], 0, E, nullptr, 0, 0}};
+      MlpJob j[2] = {{&pl.emsg, r.ws + L.mem[t], &L.emm[t], 0, E, nullptr, 0, 0, live, base},
+                     {&pl.eatt, r.ws + L.mem[t], &L.enm[t], 0, E, nullptr, 0, 0, live, base}};
       GIB_TRY(mlp_forward_multi(r, j, 2, fwd_flags(r)));
     }
     GIB_TRY(emn_aggregate_fwd(r.ws + L.emsg[t], r.ws + L.emx.y[pl.emsg.n], r.ws + L.enx.y[pl.eatt.n],
                               r.ws + L.emm[t].y[pl.emsg.n], r.ws + L.enm[t].y[pl.eatt.n], Hp, r.ga.ent_dst,
-                              r.ga.ent_src, r.ga.dst_ptr, E, r.st));
+                              r.ga.ent_src, r.ga.dst_ptr, E, live, r.st));
     GemmNT p;
     p.A = r.ws + L.emsg[t]; p.lda = Hp; p.B = r.packed + ih.ow; p.ldb = ih.Cp; p.C = r.ws + L.gi[t]; p.ldc = ih.Rp;
     p.B_hi = r.packed + ih.ow_hi; p.B_lo = r.packed + ih.ow_lo;
     p.M = E; p.N = ih.Rp; p.K = ih.Cp; p.bias = r.packed + ih.ob; p.act = ACT_NONE; p.mode = EPI_ACT;
     p.n_store = p.n_valid = ih.Rp;
+    p.m_dev = live; p.base_dev = base;
     GIB_TRY(gemm_nt(p, r.st));
     // GRUCell(message) with hx=None (mpnn.py:488): h = 0, so W_hh h + b_hh = b_hh
-    GIB_TRY(gru_fwd(r.ws + L.mem[t + 1], r.ws + L.gi[t], r.packed + hh.ob, nullptr, Hp, nullptr, E, r.st));
+    GIB_TRY(gru_fwd(r.ws + L.mem[t + 1], r.ws + L.gi[t], r.packed + hh.ob, nullptr, Hp, nullptr, E, live, r.st));
   }
   // edge_mpnn.py:178-189: node vector = sum of the memories of the bonds leaving it
   GIB_TRY(scatter_sum(r.ws + L.hfinal, r.ws + L.mem[d.T], Hp, r.ga.dst_ptr, r.ga.dst_ent, nullptr, 0, r.S, r.st));
   return readout_forward(r, out);
+}
+
+// backward of emb_msg_nn and att_msg_nn over the same bond rows: chained input gradients + one grouped weight-gradient
+// launch.  Capacity mode: the group is planned for both members' rows, and siblings of unequal depth (msg_depth !=
+// att_depth) run one after the other, each still on the device row range.
+static int emn_siblings_backward(const Run& r, const BwdBufs& bb, const MlpBwdJob* j) {
+  if (!r.cap) return mlp_backward_multi(r, bb, j, 2);
+  if (j[0].m->n == j[1].m->n) return mlp_backward_multi(r, bb, j, 2, 2LL * r.E, /*same_rows=*/true);
+  GIB_TRY(mlp_backward_multi(r, bb, j, 1, r.E));
+  return mlp_backward_multi(r, bb, j + 1, 1, r.E);
 }
 
 static int emn_backward(const Run& r, const BwdBufs& bb, const float* out, const float* dout, int part) {
@@ -903,6 +932,8 @@ static int emn_backward(const Run& r, const BwdBufs& bb, const float* out, const
   const int Hp = pl.Hp, E = r.E;
   const Lin& ih = pl.lins[pl.gru_ih];
   const Lin& hh = pl.lins[pl.gru_hh];
+  const int* live = type_count_dev(r, 0);
+  const int* base = type_base_dev(r, 0);
   float* sc = r.scratch;
   if (part != 2) GIB_TRY(readout_backward(r, bb, out, dout));
   if (part == 1 || E == 0) return 0;
@@ -911,47 +942,49 @@ static int emn_backward(const Run& r, const BwdBufs& bb, const float* out, const
   float* dmem2 = sc + bb.dmem2;
   float* T1 = sc + bb.T1;
   float* T2 = sc + bb.T2;
-  GIB_TRY(gather_rows(dmem, sc + bb.dh, Hp, r.ga.ent_dst, nullptr, 0, E, r.st));
+  GIB_TRY(gather_rows(dmem, sc + bb.dh, Hp, r.ga.ent_dst, nullptr, 0, E, live, r.st));
   GIB_CUDA_TRY(cudaMemsetAsync(sc + bb.dEMx, 0, EH * sizeof(float), r.st));
   GIB_CUDA_TRY(cudaMemsetAsync(sc + bb.dENx, 0, EH * sizeof(float), r.st));
   for (int t = d.T - 1; t >= 0; --t) {
     GIB_TRY(gru_bwd(sc + bb.dgi, sc + bb.dgh, nullptr, dmem, r.ws + L.gi[t], r.packed + hh.ob, nullptr, Hp, nullptr,
-                    E, r.st));
+                    E, live, r.st));
     GemmDW q;
     q.G = sc + bb.dgi; q.ldg = ih.Rp; q.Nn = ih.Rp; q.X = r.ws + L.emsg[t]; q.ldx = Hp; q.Kk = ih.Cp; q.M = E;
     q.dW = r.grads[ih.pw]; q.dbias = r.grads[ih.pb]; q.R = ih.R; q.C = ih.C; q.Rb = ih.Rb; q.Rbp = ih.Rbp;
     q.rs = ih.rs; q.cs = ih.cs; q.scratch = sc + bb.dw; q.half_floats = bb.dw_half;
+    q.m_dev = live; q.base_dev = base;
     GIB_TRY(gemm_dw(q, r.st));
-    GIB_TRY(colsum_add(r.grads[hh.pb], sc + bb.dgh, hh.Rp, E, hh.R, hh.Rb, hh.Rbp, r.st));  // d b_hh; d W_hh = 0
+    GIB_TRY(colsum_add(r.grads[hh.pb], sc + bb.dgh, hh.Rp, E, hh.R, hh.Rb, hh.Rbp, live, r.st));  // d b_hh; d W_hh = 0
     GemmNT p;
     p.A = sc + bb.dgi; p.lda = ih.Rp; p.B = r.packed + ih.owt; p.ldb = ih.Rp; p.C = sc + bb.dmsum; p.ldc = Hp;
     p.B_hi = r.packed + ih.owt_hi; p.B_lo = r.packed + ih.owt_lo;
     p.M = E; p.N = ih.Ctp; p.K = ih.Rp; p.mode = EPI_ACT; p.act = ACT_NONE; p.n_store = p.n_valid = ih.Ctp;
+    p.m_dev = live; p.base_dev = base;
     GIB_TRY(gemm_nt(p, r.st));
     const float* EMm = r.ws + L.emm[t].y[pl.emsg.n];
     const float* ENm = r.ws + L.enm[t].y[pl.eatt.n];
     GIB_TRY(emn_aggregate_bwd(sc + bb.dEMx, sc + bb.dENx, sc + bb.dEMm, sc + bb.dENm, sc + bb.st3, sc + bb.dmsum,
-                              r.ws + L.emx.y[pl.emsg.n], r.ws + L.enx.y[pl.eatt.n], EMm, ENm, Hp, r.ga, E, r.st));
-    GIB_TRY(mul_dselu(T1, sc + bb.dEMm, EMm, EH, r.st));
-    GIB_TRY(mul_dselu(T2, sc + bb.dENm, ENm, EH, r.st));
-    {   // sibling MLPs on the same rows: chained input gradients + one grouped weight-gradient launch
-      MlpBwdJob j[2] = {{&pl.emsg, r.ws + L.mem[t], &L.emm[t], 0, E, T1, dmem2, Hp, nullptr},
-                        {&pl.eatt, r.ws + L.mem[t], &L.enm[t], 0, E, T2, dmem, Hp, dmem2}};
-      GIB_TRY(mlp_backward_multi(r, bb, j, 2));
+                              r.ws + L.emx.y[pl.emsg.n], r.ws + L.enx.y[pl.eatt.n], EMm, ENm, Hp, r.ga, E, live, r.st));
+    GIB_TRY(mul_dselu(T1, sc + bb.dEMm, EMm, E, Hp, live, r.st));
+    GIB_TRY(mul_dselu(T2, sc + bb.dENm, ENm, E, Hp, live, r.st));
+    {
+      MlpBwdJob j[2] = {{&pl.emsg, r.ws + L.mem[t], &L.emm[t], 0, E, T1, dmem2, Hp, nullptr, live, base},
+                        {&pl.eatt, r.ws + L.mem[t], &L.enm[t], 0, E, T2, dmem, Hp, dmem2, live, base}};
+      GIB_TRY(emn_siblings_backward(r, bb, j));
     }
   }
   // pass-independent branch through x = tanh(embedding_nn(.))
-  GIB_TRY(mul_dselu(T1, sc + bb.dEMx, r.ws + L.emx.y[pl.emsg.n], EH, r.st));
-  GIB_TRY(mul_dselu(T2, sc + bb.dENx, r.ws + L.enx.y[pl.eatt.n], EH, r.st));
+  GIB_TRY(mul_dselu(T1, sc + bb.dEMx, r.ws + L.emx.y[pl.emsg.n], E, Hp, live, r.st));
+  GIB_TRY(mul_dselu(T2, sc + bb.dENx, r.ws + L.enx.y[pl.eatt.n], E, Hp, live, r.st));
   {
-    MlpBwdJob j[2] = {{&pl.emsg, r.ws + L.xt, &L.emx, 0, E, T1, dmem2, Hp, nullptr},
-                      {&pl.eatt, r.ws + L.xt, &L.enx, 0, E, T2, dmem, Hp, dmem2}};
-    GIB_TRY(mlp_backward_multi(r, bb, j, 2));
+    MlpBwdJob j[2] = {{&pl.emsg, r.ws + L.xt, &L.emx, 0, E, T1, dmem2, Hp, nullptr, live, base},
+                      {&pl.eatt, r.ws + L.xt, &L.enx, 0, E, T2, dmem, Hp, dmem2, live, base}};
+    GIB_TRY(emn_siblings_backward(r, bb, j));
   }
-  GIB_TRY(tanh_selu_bwd(T1, dmem, r.ws + L.xt, r.ws + L.embnn.y[pl.embnn.n], EH, r.st));
+  GIB_TRY(tanh_selu_bwd(T1, dmem, r.ws + L.xt, r.ws + L.embnn.y[pl.embnn.n], E, Hp, live, r.st));
   {
-    MlpBwdJob j[1] = {{&pl.embnn, r.ws + L.xin, &L.embnn, 0, E, T1, nullptr, 0, nullptr}};
-    GIB_TRY(mlp_backward_multi(r, bb, j, 1));
+    MlpBwdJob j[1] = {{&pl.embnn, r.ws + L.xin, &L.embnn, 0, E, T1, nullptr, 0, nullptr, live, base}};
+    GIB_TRY(mlp_backward_multi(r, bb, j, 1, r.cap ? r.E : 0));
   }
   return 0;
 }
@@ -1012,10 +1045,15 @@ void make_bwd(const Run& r, BwdBufs& bb) {
     mlp_extent(pl, pl.embnn, E, big, dw);
     mlp_extent(pl, pl.emsg, E, big, dw);
     mlp_extent(pl, pl.eatt, E, big, dw);
+    // the same plan rows as emn_backward / emn_siblings_backward (the split of a grouped weight gradient depends on them)
     const Mlp* one[1] = {&pl.embnn}; const size_t re[2] = {E, E};
-    group_extent(pl, one, re, 1, 0, dw);
+    group_extent(pl, one, re, 1, r.cap ? (long long)E : 0, dw);
     const Mlp* two[2] = {&pl.emsg, &pl.eatt};
-    group_extent(pl, two, re, 2, 0, dw);
+    group_extent(pl, two, re, 2, r.cap ? 2LL * (long long)E : 0, dw);
+    if (r.cap && pl.emsg.n != pl.eatt.n) {
+      group_extent(pl, two, re, 1, (long long)E, dw);
+      group_extent(pl, two + 1, re, 1, (long long)E, dw);
+    }
     big = std::max(big, E * (mlp_max_ld(pl, pl.emsg) + mlp_max_ld(pl, pl.eatt)) + 64);
   }
   const size_t gru_rows = d.model == GIB_EMN ? E : S;

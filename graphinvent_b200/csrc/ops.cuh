@@ -21,26 +21,28 @@ int concat_flat(float* dst, int ldd, const float* f1, int ldf, int N, int fa, co
 int unflatten_dact(float* G, int ldf, const float* dcat, int ldd, const float* f1, int N, int fa, long long S, cudaStream_t st);
 int dact_slice(float* G, int ldg, const float* dout, const float* out, int ldo, int off, int width, int act, int rows, cudaStream_t st);
 int sum3_cols(float* dst, int ldd, int W, const float* a, int lda, int offa, const float* b2, int ldb, int offb, const float* c3, int ldc, int rows, cudaStream_t st);
-int tanh_fwd(float* y, const float* x, long long n, cudaStream_t st);
-int tanh_selu_bwd(float* G, const float* dy, const float* y, const float* pre, long long n, cudaStream_t st);
-int gather_rows(float* dst, const float* h, int ld, const int* src, const float* w, int scale, long long P, cudaStream_t st);
+// live (may be null): device-side count of the live rows among the `rows` / P / S / E / M rows (EMN bond rows in
+// capacity mode, see graph_ops.cu: live_rows); the grid is sized from the capacity, rows past the count are untouched
+int tanh_fwd(float* y, const float* x, long long rows, int ld, const int* live, cudaStream_t st);
+int tanh_selu_bwd(float* G, const float* dy, const float* y, const float* pre, long long rows, int ld, const int* live, cudaStream_t st);
+int gather_rows(float* dst, const float* h, int ld, const int* src, const float* w, int scale, long long P, const int* live, cudaStream_t st);
 // bytes: algorithmic bytes of the launch for the profile hooks (0 = unknown)
 int scatter_sum(float* out, const float* msg, int ld, const int* ptr, const int* ent, const float* w, int accumulate, long long S, cudaStream_t st, double bytes = 0.0);
 extern int g_scatter_variant;
 int scatter_bwd(float* G, const float* dM, const float* Y, int ld, const int* dst, const float* w, int act, long long P, cudaStream_t st);
 int seg_softmax_fwd(float* out, const float* EM, const float* EN, int ld, const int* ptr, const int* ent, const float* w, long long S, cudaStream_t st);
 int seg_softmax_bwd(float* GM, float* GN, const float* dM, const float* EM, const float* EN, int ld, const int* ptr, const int* ent, const float* w, long long S, cudaStream_t st);
-int gru_fwd(float* hn, const float* gi, const float* gh, const float* h, int Hp, const int* ptr, long long S, cudaStream_t st);
-int gru_bwd(float* dgi, float* dgh, float* dh_direct, const float* dhn, const float* gi, const float* gh, const float* h, int Hp, const int* ptr, long long S, cudaStream_t st);
-int colsum_add(float* out, const float* G, int ldg, long long M, int R, int Rb, int Rbp, cudaStream_t st);
+int gru_fwd(float* hn, const float* gi, const float* gh, const float* h, int Hp, const int* ptr, long long S, const int* live, cudaStream_t st);
+int gru_bwd(float* dgi, float* dgh, float* dh_direct, const float* dhn, const float* gi, const float* gh, const float* h, int Hp, const int* ptr, long long S, const int* live, cudaStream_t st);
+int colsum_add(float* out, const float* G, int ldg, long long M, int R, int Rb, int Rbp, const int* live, cudaStream_t st);
 int graph_gather_fwd(float* g, float* att, const float* en, const float* em, int ld, const int* ptr, int N, int B, float big, cudaStream_t st);
 int graph_gather_bwd(float* Gen, float* Gem, const float* dg, const float* att, const float* en, const float* em, int ld, int N, int B, cudaStream_t st);
 int sum_nodes_fwd(float* g, const float* h, int ld, int N, int B, cudaStream_t st);
 int bcast_nodes_add(float* dh, const float* dg, int ld, int N, long long S, cudaStream_t st);
 int emn_input(float* X, int ld, const void* nodes, const void* edges, int i8, const int* ent_dst, const int* ent_src, int N, int F, int Ef, long long P, cudaStream_t st);
-int emn_aggregate_fwd(float* msg, const float* EMx, const float* ENx, const float* EMm, const float* ENm, int ld, const int* ent_dst, const int* ent_src, const int* dst_ptr, long long E, cudaStream_t st);
-int emn_aggregate_bwd(float* dEMx, float* dENx, float* dEMm, float* dENm, float* st3, const float* dmsg, const float* EMx, const float* ENx, const float* EMm, const float* ENm, int ld, const GraphArrays& ga, long long E, cudaStream_t st);
-int mul_dselu(float* G, const float* d, const float* y, long long n, cudaStream_t st);
+int emn_aggregate_fwd(float* msg, const float* EMx, const float* ENx, const float* EMm, const float* ENm, int ld, const int* ent_dst, const int* ent_src, const int* dst_ptr, long long E, const int* live, cudaStream_t st);
+int emn_aggregate_bwd(float* dEMx, float* dENx, float* dEMm, float* dENm, float* st3, const float* dmsg, const float* EMx, const float* ENx, const float* EMm, const float* ENm, int ld, const GraphArrays& ga, long long E, const int* live, cudaStream_t st);
+int mul_dselu(float* G, const float* d, const float* y, long long rows, int ld, const int* live, cudaStream_t st);
 int pack_weight(float* Wp, float* WTp, float* bp, const float* W, const float* bias, long long rs, long long cs, int nblk, int Rb, int Rbp, int C, int Cp, int Ct, int Ctp, cudaStream_t st);
 
 }  // namespace gib

@@ -110,7 +110,7 @@ class GraphBatch:
     two models of one family can share it (`build_graph`, SURVEY.md 8f rank 4: agent + prior of the RL rollout).
 
     `capacity=None` (exact mode): one 64-byte device->host read sizes every buffer exactly.
-    `capacity=n` (capacity mode, node-state models): buffers are sized for n bond entries, the live counts stay on the
+    `capacity=n` (capacity mode): buffers are sized for n bond entries, the live counts stay on the
     device and the kernels read them there -- no host synchronisation; `overflowed()` / `flags()` read the device
     header when the caller chooses to (a batch with more entries is truncated and flagged, never written out of
     bounds).  `buffers=(cws, buf)` re-uses the allocations of an earlier GraphBatch of equal dims and capacity (static

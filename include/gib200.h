@@ -63,9 +63,10 @@ typedef struct gib_dims {
  * Exact mode: the caller copies them to the host (the one D2H read of a forward) and passes them back as `hdr_host`;
  * buffers are then sized exactly.  Capacity mode: the caller never reads them -- gib_graph_header_capacity() builds a
  * host header that carries static capacities and the ADDRESS of the device header, every kernel whose extent depends
- * on the batch content (the per-bond-type GEMM row ranges, the split counts of the weight-gradient reductions) reads
- * the live counts from device memory, and no launch parameter depends on the batch: a step has no host
- * synchronisation and is capturable in a CUDA graph.  Index meaning: */
+ * on the batch content (the per-bond-type GEMM row ranges, the split counts of the weight-gradient reductions, and for
+ * the EMN every kernel over bond rows) reads the live counts from device memory, and no launch parameter depends on
+ * the batch: a step has no host synchronisation and is capturable in a CUDA graph.  All four models support it.
+ * Index meaning: */
 enum {
   GIB_HDR_E = 0,          /* bond entries (non-zero elements of `edges`) */
   GIB_HDR_P = 1,          /* rows of the type-grouped entry arrays (groups padded to 128) */
