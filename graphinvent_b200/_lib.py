@@ -25,11 +25,25 @@ class Dims(ctypes.Structure):
         "mlp1_hidden", "mlp1_depth", "mlp2_hidden", "mlp2_depth", "f_add", "f_conn")] + [("big", c_f), ("in_dtype", c_i)]
 
 
+class GemmProblem(ctypes.Structure):
+    """mirror of `gib_gemm_problem` (include/gib200.h, test hooks)"""
+    _fields_ = [("A", c_p), ("lda", c_i), ("W", c_p), ("ldw", c_i), ("W_hi", c_p), ("W_lo", c_p), ("C", c_p),
+                ("ldc", c_i), ("M", c_i), ("N", c_i), ("K", c_i), ("bias", c_p), ("act", c_i), ("mode", c_i),
+                ("aux", c_p), ("ldaux", c_i), ("n_store", c_i), ("n_valid", c_i), ("m_dev", c_p), ("base_dev", c_p)]
+
+
+class DwProblem(ctypes.Structure):
+    """mirror of `gib_dw_problem` (include/gib200.h, test hooks)"""
+    _fields_ = [("G", c_p), ("ldg", c_i), ("Nn", c_i), ("X", c_p), ("ldx", c_i), ("Kk", c_i), ("M", c_i),
+                ("dW", c_p), ("dbias", c_p), ("R", c_i), ("C", c_i), ("Rb", c_i), ("Rbp", c_i), ("rs", c_ll),
+                ("cs", c_ll), ("m_dev", c_p), ("base_dev", c_p)]
+
+
 MODEL_ID = {"GGNN": 0, "MNN": 1, "AttGGNN": 2, "EMN": 3}
 HDR_INTS = 16
 HDR_E, HDR_P, HDR_TYPE_COUNT, HDR_TYPE_BASE, HDR_FLAGS, HDR_CAPACITY = 0, 1, 2, 6, 11, 12
 FLAG_MULTITYPE, FLAG_NONBINARY, FLAG_OVERFLOW = 1, 2, 4
-ABI_VERSION = 201      # must equal gib_version() of the loaded library (include/gib200.h)
+ABI_VERSION = 202      # must equal gib_version() of the loaded library (include/gib200.h)
 
 _PROTOS = {
     "gib_last_error": (ctypes.c_char_p, []),
@@ -77,6 +91,17 @@ _PROTOS = {
     "gib_launch_count": (c_ll, []),
     "gib_profile_collect": (c_i, [c_p, c_p, c_p]),
     "gib_profile_records": (c_i, [c_p, c_p, c_p, c_i]),
+    "gib_test_chain_flag_bytes": (c_sz, [c_p, c_i]),
+    "gib_test_gemm_nt": (c_i, [c_p, c_i, c_p, c_p, c_p]),
+    "gib_test_dw_scratch_bytes": (c_sz, [c_p, c_p, c_i, c_ll]),
+    "gib_test_dw_groups": (c_i, [c_p, c_p, c_i, c_ll, c_p, c_p]),
+    "gib_test_scatter_bwd": (c_i, [c_p, c_p, c_p, c_i, c_p, c_p, c_i, c_ll, c_p]),
+    "gib_test_seg_softmax_bwd": (c_i, [c_p, c_p, c_p, c_p, c_p, c_i, c_p, c_p, c_p, c_ll, c_p]),
+    "gib_test_gru_bwd": (c_i, [c_p] * 7 + [c_i, c_p, c_ll, c_p, c_p]),
+    "gib_test_colsum_add": (c_i, [c_p, c_p, c_i, c_ll, c_i, c_i, c_i, c_p, c_p]),
+    "gib_test_graph_gather_bwd": (c_i, [c_p] * 6 + [c_i, c_i, c_i, c_p]),
+    "gib_test_emn_aggregate_fwd": (c_i, [c_p] * 5 + [c_i] + [c_p] * 3 + [c_ll, c_p, c_p]),
+    "gib_test_emn_aggregate_bwd": (c_i, [c_p] * 10 + [c_i] + [c_p] * 5 + [c_ll, c_p, c_p]),
 }
 
 

@@ -2,6 +2,8 @@
 #include <stdarg.h>
 #include <string.h>
 
+#include <algorithm>
+
 #include "../../include/gib200.h"
 #include "gemm.cuh"
 #include "model.cuh"
@@ -141,7 +143,8 @@ using namespace gib;
 extern "C" {
 
 const char* gib_last_error(void) { return g_err; }
-int gib_version(void) { return 201; }   // 200: capacity mode, int8 inputs, grouped dW; 201: 5 profile classes
+// 200: capacity mode, int8 inputs, grouped dW; 201: 5 profile classes; 202: test hooks
+int gib_version(void) { return 202; }
 void gib_set_tensor_cores(int on) { g_use_tc = on != 0; }
 int gib_get_tensor_cores(void) { return g_use_tc ? 1 : 0; }
 void gib_tc_debug(int mode) { g_tc_debug = mode; }
@@ -379,6 +382,112 @@ int gib_gru_gates(float* hn, const float* gi, const float* gh, const float* h, i
 int gib_graph_gather(float* g, float* att, const float* en, const float* em, int ld, const int* ptr, int N, int B,
                      float big, gib_stream stream) {
   return graph_gather_fwd(g, att, en, em, ld, ptr, N, B, big, ST(stream));
+}
+
+}  // extern "C"
+
+// ---- test hooks (include/gib200.h): C-ABI mirrors -> the internal structs, nothing else ----------------------------
+static GemmNT to_gemm_nt(const gib_gemm_problem& s) {
+  GemmNT p;
+  p.A = s.A; p.lda = s.lda; p.B = s.W; p.ldb = s.ldw; p.B_hi = s.W_hi; p.B_lo = s.W_lo;
+  p.C = s.C; p.ldc = s.ldc; p.M = s.M; p.N = s.N; p.K = s.K; p.bias = s.bias; p.act = s.act; p.mode = s.mode;
+  p.aux = s.aux; p.ldaux = s.ldaux; p.n_store = s.n_store; p.n_valid = s.n_valid;
+  p.m_dev = s.m_dev; p.base_dev = s.base_dev;
+  return p;
+}
+static GemmDW to_gemm_dw(const gib_dw_problem& s) {
+  GemmDW q;
+  q.G = s.G; q.ldg = s.ldg; q.Nn = s.Nn; q.X = s.X; q.ldx = s.ldx; q.Kk = s.Kk; q.M = s.M; q.dW = s.dW;
+  q.dbias = s.dbias; q.R = s.R; q.C = s.C; q.Rb = s.Rb; q.Rbp = s.Rbp; q.rs = s.rs; q.cs = s.cs;
+  q.m_dev = s.m_dev; q.base_dev = s.base_dev;
+  return q;
+}
+// both scratch halves, sized as make_bwd sizes them: the largest group (with the same plan rows) and member
+static size_t test_dw_scratch_floats(const gib_dw_problem* qs, const int* group_sizes, int n_groups,
+                                     long long plan_rows) {
+  size_t f = 0;
+  int k = 0;
+  for (int g = 0; g < n_groups; ++g) {
+    GemmDW grp[kTc3MaxProblems];
+    const int n = group_sizes[g];
+    if (n < 1 || n > kTc3MaxProblems) return 0;
+    for (int i = 0; i < n; ++i) grp[i] = to_gemm_dw(qs[k + i]);
+    f = std::max(f, 2 * gemm_dw_group_half_floats(grp, n, plan_rows));
+    k += n;
+  }
+  return f;
+}
+
+extern "C" {
+
+size_t gib_test_chain_flag_bytes(const gib_gemm_problem* ps, int n) {
+  if (n < 1 || n > kTc3MaxProblems) return 0;
+  GemmNT p[kTc3MaxProblems];
+  for (int i = 0; i < n; ++i) p[i] = to_gemm_nt(ps[i]);
+  return tc3_chain_flag_ints(p, n) * sizeof(int);
+}
+int gib_test_gemm_nt(const gib_gemm_problem* ps, int n, const int* dep, int* flags, gib_stream stream) {
+  if (n < 1 || n > kTc3MaxProblems) { set_error("gib_test_gemm_nt: %d problems (1..%d)", n, kTc3MaxProblems); return -2; }
+  GemmNT p[kTc3MaxProblems];
+  for (int i = 0; i < n; ++i) p[i] = to_gemm_nt(ps[i]);
+  if (!dep) return n == 1 ? gemm_nt(p[0], ST(stream)) : gemm_nt_group(p, n, ST(stream));
+  if (!gemm_nt_chain_ok(p, n)) { set_error("gib_test_gemm_nt: the problems do not qualify for a chain"); return -3; }
+  return gemm_nt_chain(p, dep, n, flags, ST(stream));
+}
+size_t gib_test_dw_scratch_bytes(const gib_dw_problem* qs, const int* group_sizes, int n_groups, long long plan_rows) {
+  return test_dw_scratch_floats(qs, group_sizes, n_groups, plan_rows) * sizeof(float);
+}
+int gib_test_dw_groups(const gib_dw_problem* qs, const int* group_sizes, int n_groups, long long plan_rows,
+                       void* scratch, gib_stream stream) {
+  const size_t floats = test_dw_scratch_floats(qs, group_sizes, n_groups, plan_rows);
+  if (n_groups < 1 || floats == 0) { set_error("gib_test_dw_groups: bad group sizes"); return -2; }
+  GIB_TRY(dw_begin());
+  int rc = 0;
+  for (int g = 0, k = 0; g < n_groups && rc == 0; k += group_sizes[g++]) {
+    GemmDW grp[kTc3MaxProblems];
+    for (int i = 0; i < group_sizes[g]; ++i) {
+      grp[i] = to_gemm_dw(qs[k + i]);
+      grp[i].scratch = reinterpret_cast<float*>(scratch);
+      grp[i].half_floats = floats / 2;
+    }
+    rc = group_sizes[g] == 1 ? gemm_dw(grp[0], ST(stream)) : gemm_dw_group(grp, group_sizes[g], plan_rows, ST(stream));
+  }
+  const int rj = dw_join(ST(stream));
+  return rc ? rc : rj;
+}
+int gib_test_scatter_bwd(float* G, const float* dM, const float* Y, int ld, const int* dst, const float* w, int act,
+                         long long P, gib_stream stream) {
+  return scatter_bwd(G, dM, Y, ld, dst, w, act, P, ST(stream));
+}
+int gib_test_seg_softmax_bwd(float* GM, float* GN, const float* dM, const float* EM, const float* EN, int ld,
+                             const int* ptr, const int* ent, const float* w, long long S, gib_stream stream) {
+  return seg_softmax_bwd(GM, GN, dM, EM, EN, ld, ptr, ent, w, S, ST(stream));
+}
+int gib_test_gru_bwd(float* dgi, float* dgh, float* dh, const float* dhn, const float* gi, const float* gh,
+                     const float* h, int Hp, const int* ptr, long long S, const int* live, gib_stream stream) {
+  return gru_bwd(dgi, dgh, dh, dhn, gi, gh, h, Hp, ptr, S, live, ST(stream));
+}
+int gib_test_colsum_add(float* out, const float* G, int ldg, long long M, int R, int Rb, int Rbp, const int* live,
+                        gib_stream stream) {
+  return colsum_add(out, G, ldg, M, R, Rb, Rbp, live, ST(stream));
+}
+int gib_test_graph_gather_bwd(float* Gen, float* Gem, const float* dg, const float* att, const float* en,
+                              const float* em, int ld, int N, int B, gib_stream stream) {
+  return graph_gather_bwd(Gen, Gem, dg, att, en, em, ld, N, B, ST(stream));
+}
+int gib_test_emn_aggregate_fwd(float* msg, const float* EMx, const float* ENx, const float* EMm, const float* ENm,
+                               int ld, const int* ent_dst, const int* ent_src, const int* dst_ptr, long long E,
+                               const int* live, gib_stream stream) {
+  return emn_aggregate_fwd(msg, EMx, ENx, EMm, ENm, ld, ent_dst, ent_src, dst_ptr, E, live, ST(stream));
+}
+int gib_test_emn_aggregate_bwd(float* dEMx, float* dENx, float* dEMm, float* dENm, float* st3, const float* dmsg,
+                               const float* EMx, const float* ENx, const float* EMm, const float* ENm, int ld,
+                               const int* ent_dst, const int* ent_src, const int* dst_ptr, const int* src_ptr,
+                               const int* src_ent, long long E, const int* live, gib_stream stream) {
+  GraphArrays ga{};
+  ga.ent_dst = const_cast<int*>(ent_dst); ga.ent_src = const_cast<int*>(ent_src); ga.dst_ptr = const_cast<int*>(dst_ptr);
+  ga.src_ptr = const_cast<int*>(src_ptr); ga.src_ent = const_cast<int*>(src_ent);
+  return emn_aggregate_bwd(dEMx, dENx, dEMm, dENm, st3, dmsg, EMx, ENx, EMm, ENm, ld, ga, E, live, ST(stream));
 }
 
 }  // extern "C"

@@ -238,16 +238,17 @@ int gemm_nt_simt(const GemmNT& p, cudaStream_t st) {
     return -2;
   }
   ProfScope prof(PROF_GEMM_NT_SIMT, p.work > 0 ? p.work : 2.0 * p.M * (double)p.N * p.K, st);
-  const long long ctas_big = (long long)ceil_div(p.M, 128) * ceil_div(p.N, 128);
+  const int ncols = std::max(p.N, p.n_store);     // columns [N, n_store) are stored too (zeros / epi(0))
+  const long long ctas_big = (long long)ceil_div(p.M, 128) * ceil_div(ncols, 128);
   const int num_sms = device_sm_count();
-  if (ctas_big >= num_sms && p.N > 64) {
-    dim3 grid(ceil_div(p.N, 128), ceil_div(p.M, 128));
+  if (ctas_big >= num_sms && ncols > 64) {
+    dim3 grid(ceil_div(ncols, 128), ceil_div(p.M, 128));
     sgemm_nt_kernel<128, 128, 2, 2><<<grid, 256, 0, st>>>(p);
-  } else if (p.N <= 64 && (long long)ceil_div(p.M, 128) >= num_sms) {
-    dim3 grid(ceil_div(p.N, 64), ceil_div(p.M, 128));
+  } else if (ncols <= 64 && (long long)ceil_div(p.M, 128) >= num_sms) {
+    dim3 grid(ceil_div(ncols, 64), ceil_div(p.M, 128));
     sgemm_nt_kernel<128, 64, 2, 1><<<grid, 256, 0, st>>>(p);
   } else {
-    dim3 grid(ceil_div(p.N, 64), ceil_div(p.M, 64));
+    dim3 grid(ceil_div(ncols, 64), ceil_div(p.M, 64));
     sgemm_nt_kernel<64, 64, 1, 1><<<grid, 256, 0, st>>>(p);
   }
   GIB_LAUNCH_CHECK();
@@ -643,13 +644,14 @@ int gemm_dw(const GemmDW& q, cudaStream_t st) {
   if (q.m_dev || (g_use_tc && use_tc3() && q.dW && q.M >= 2048 && q.Nn >= 32 && q.Kk >= 32 && tc3_dw_eligible(q) &&
                   q.half_floats > 0))
     return gemm_dw_group(&q, 1, 0, st);
-  ProfScope prof(g_use_tc && !use_tc3() ? PROF_GEMM_DW : PROF_GEMM_DW_SIMT, q.work > 0 ? q.work : 2.0 * q.M * (double)q.R * q.C, st);
+  const bool tc = g_use_tc && q.dW && tc_dw_eligible(q);
+  ProfScope prof(tc ? PROF_GEMM_DW : PROF_GEMM_DW_SIMT, q.work > 0 ? q.work : 2.0 * q.M * (double)q.R * q.C, st);
   DwSide* d;
   GIB_TRY(dw_side(&d));
   const int half = (int)(d->calls++ & 1);
   float* const scratch = q.scratch + (size_t)half * q.half_floats;
   if (d->done_valid[half]) GIB_CUDA_TRY(cudaStreamWaitEvent(st, d->ev_done[half], 0));   // job i-2 released this half
-  if (g_use_tc && q.dW && tc_dw_eligible(q)) {
+  if (tc) {
     // per-problem tensor-core partials (MN-major operands straight from the row-major activations) on the main
     // stream; bias column sums + the fixed-order split reduction on the side stream
     int tsplits = 0;

@@ -665,7 +665,7 @@ static int launch_nt(const GemmNT* ps, const int* dep, int n, int* flags, bool r
     if (planes) GIB_TRY(make_map(&maps.b_lo[np], p.B_lo, p.N, p.K, p.ldb, BN));
     P.bsplit[np] = planes ? 1 : 0;
     P.g[np] = p;
-    P.n_tiles[np] = ceil_div(p.N, BN);
+    P.n_tiles[np] = ceil_div(std::max(p.N, p.n_store), BN);   // columns [N, n_store) are stored too (zeros / epi(0))
     P.k_blocks[np] = ceil_div(p.K, BKF);
     P.dep[np] = -1;
     P.flag_off[np] = flag_ints;

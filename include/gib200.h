@@ -201,6 +201,77 @@ int gib_gru_gates(float* hn, const float* gi, const float* gh, const float* h, i
 int gib_graph_gather(float* g, float* att, const float* en, const float* em, int ld, const int* ptr, int N,
                      int B, float big, gib_stream stream);
 
+/* ---- test hooks: thin entries into the GEMM dispatchers and the backward / EMN kernels the model calls, so that each
+ *      can be checked on its own against a float64 reference (tests/test_gpu_gemm_patterns.py,
+ *      tests/test_gpu_graph_kernels.py).  Each entry calls the internal function the model calls and adds no path of its
+ *      own.  `ps`, `dep`, `qs` and `group_sizes` are HOST arrays; everything they point to lives on the device. ---- */
+/* one NT problem: C[M, :n_store] = epi(A[M,K] W[N,K]^T) with A, W row-major, K % 16 == 0, lda / ldb % 4 == 0;
+ * epi (mode): 0 act(acc + bias), 1 acc * act'(aux) (aux = the activation OUTPUT), 2 acc + aux (aux may alias C);
+ * act 0 none / 1 selu / 2 tanh.  Columns [n_valid, n_store) are stored as zeros, columns >= n_store are not touched.
+ * W_hi / W_lo (may be NULL): its TF32 planes (gib_split_planes).  m_dev / base_dev (may be NULL): the live row range
+ * [*base_dev, *base_dev + *m_dev) inside buffers of M rows. */
+typedef struct gib_gemm_problem {
+  const float* A; int lda;
+  const float* W; int ldw;
+  const float* W_hi; const float* W_lo;
+  float* C; int ldc;
+  int M, N, K;
+  const float* bias;
+  int act, mode;
+  const float* aux; int ldaux;
+  int n_store, n_valid;
+  const int* m_dev; const int* base_dev;
+} gib_gemm_problem;
+/* dep == NULL: the n problems as the model launches independent siblings (one problem: the single-GEMM dispatcher,
+ * n <= 4: one grouped tensor-core launch when they qualify, else problem by problem).  dep != NULL: ONE dependent-chain
+ * launch in which problem i reads as its A operand what problem dep[i] < i stores (-1: independent); returns < 0
+ * without launching when the problems do not qualify for a chain.  flags: >= gib_test_chain_flag_bytes(ps, n). */
+size_t gib_test_chain_flag_bytes(const gib_gemm_problem* ps, int n);
+int gib_test_gemm_nt(const gib_gemm_problem* ps, int n, const int* dep, int* flags, gib_stream stream);
+/* one weight-gradient problem: dW[r*rs + c*cs] += sum_m G[m, prow(r)] X[m, c], dbias[r] += sum_m G[m, prow(r)]
+ * (either may be NULL) for r < R, c < C, prow(r) = (r / Rb) * Rbp + r % Rb; G [M, Nn] (ldg), X [M, Kk] (ldx) */
+typedef struct gib_dw_problem {
+  const float* G; int ldg; int Nn;
+  const float* X; int ldx; int Kk;
+  int M;
+  float* dW; float* dbias;
+  int R, C, Rb, Rbp;
+  long long rs, cs;
+  const int* m_dev; const int* base_dev;
+} gib_dw_problem;
+/* n_groups consecutive groups of group_sizes[g] (<= 16) problems, each run as the model runs the weight gradients of one
+ * layer (one grouped tensor-core launch + one side-stream reduction when it qualifies), all on ONE scratch whose two
+ * halves alternate between groups; plan_rows: the expected reduction rows of a group (0: the sum of its M).  The
+ * members of one group write disjoint destinations; different groups may add into the same ones. */
+size_t gib_test_dw_scratch_bytes(const gib_dw_problem* qs, const int* group_sizes, int n_groups, long long plan_rows);
+int gib_test_dw_groups(const gib_dw_problem* qs, const int* group_sizes, int n_groups, long long plan_rows,
+                       void* scratch, gib_stream stream);
+/* G[p] = w[p] * dM[dst[p]] * act'(Y[p]) (rows with dst[p] < 0: zeros) */
+int gib_test_scatter_bwd(float* G, const float* dM, const float* Y, int ld, const int* dst, const float* w, int act,
+                         long long P, gib_stream stream);
+/* backward of gib_seg_softmax with SELU outputs EM / EN; GM / GN rows in no segment are not written */
+int gib_test_seg_softmax_bwd(float* GM, float* GN, const float* dM, const float* EM, const float* EN, int ld,
+                             const int* ptr, const int* ent, const float* w, long long S, gib_stream stream);
+/* backward of gib_gru_gates; h == NULL: h = 0 and gh is one bias row (the EMN form); live (may be NULL): device count
+ * of the rows to process, rows past it are not touched */
+int gib_test_gru_bwd(float* dgi, float* dgh, float* dh, const float* dhn, const float* gi, const float* gh,
+                     const float* h, int Hp, const int* ptr, long long S, const int* live, gib_stream stream);
+/* out[r] += sum over the first min(*live, M) rows m of G[m, prow(r)] (live may be NULL: all M rows) */
+int gib_test_colsum_add(float* out, const float* G, int ldg, long long M, int R, int Rb, int Rbp, const int* live,
+                        gib_stream stream);
+/* backward of gib_graph_gather at its stored attention `att`, SELU outputs en / em */
+int gib_test_graph_gather_bwd(float* Gen, float* Gem, const float* dg, const float* att, const float* en,
+                              const float* em, int ld, int N, int B, gib_stream stream);
+/* EMN line-graph aggregation over the bond entries (ordered by destination: ent_dst ascending) and its two-pass
+ * backward: dEMx / dENx are accumulated (+=), dEMm / dENm stored; st3 is a [3, E, ld] stash; rows >= *live untouched */
+int gib_test_emn_aggregate_fwd(float* msg, const float* EMx, const float* ENx, const float* EMm, const float* ENm,
+                               int ld, const int* ent_dst, const int* ent_src, const int* dst_ptr, long long E,
+                               const int* live, gib_stream stream);
+int gib_test_emn_aggregate_bwd(float* dEMx, float* dENx, float* dEMm, float* dENm, float* st3, const float* dmsg,
+                               const float* EMx, const float* ENx, const float* EMm, const float* ENm, int ld,
+                               const int* ent_dst, const int* ent_src, const int* dst_ptr, const int* src_ptr,
+                               const int* src_ent, long long E, const int* live, gib_stream stream);
+
 /* ---- generation round post-processing (SURVEY §8f #1): softmax + categorical sample of one
  *      action per molecule from the APD logits, inverse-CDF on a caller-provided uniform. ---- */
 int gib_sample_actions(const float* out, int B, int apd, const float* uniforms, int* action,

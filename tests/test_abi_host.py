@@ -26,6 +26,29 @@ def test_header_symbols_are_exported_and_bound():
     assert ctypes.sizeof(_lib.Dims) == 27 * 4      # 25 ints + big + in_dtype
 
 
+def test_test_hook_size_queries():
+    """host-only size queries of the GEMM test hooks: chain flags = one counter per 128-row block (+1) per problem;
+    the weight-gradient scratch covers its largest group and refuses a group of 0 or > 16 problems"""
+    from graphinvent_b200._lib import DwProblem, GemmProblem, lib
+    ps = (GemmProblem * 3)()
+    for p, m in zip(ps, (1, 128, 4097)):
+        p.M, p.N, p.K = m, 64, 32
+    assert lib.gib_test_chain_flag_bytes(ps, 3) == 4 * ((1 + 1) + (1 + 1) + (33 + 1))
+    assert lib.gib_test_chain_flag_bytes(ps, 0) == 0
+
+    def dw_bytes(ms, sizes):
+        qs = (DwProblem * len(ms))()
+        for q, m in zip(qs, ms):
+            q.M, q.Nn, q.Kk = m, 112, 144
+        return lib.gib_test_dw_scratch_bytes(qs, (ctypes.c_int * len(sizes))(*sizes), len(sizes), 0)
+
+    one = dw_bytes([4096], [1])
+    assert 0 < one < dw_bytes([40000], [1])
+    assert dw_bytes([4096, 40000], [1, 1]) == dw_bytes([40000], [1])
+    assert dw_bytes([4096] * 4, [4]) >= one
+    assert dw_bytes([4096] * 17, [17]) == 0 and dw_bytes([4096], [0]) == 0
+
+
 @pytest.mark.parametrize("model", MODELS)
 @pytest.mark.parametrize("big", [False, True])
 def test_plan_matches_reference_parameter_schema(model, big):

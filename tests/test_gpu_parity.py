@@ -379,7 +379,8 @@ def test_full_size_properties(cfg):
 #   gradients, per tensor:  ||g_cuda - g_fp64|| <= 2 ||g_ref32 - g_fp64|| + ||g_L(tau) - g_R(tau)|| + eps ||g_fp64||
 #                           eps = 1e-6 with fp32 SIMT GEMMs; 3e-5 with tensor cores: the arithmetic of the 3xTF32 GEMMs
 #                           themselves (dropped lo*lo term, the tensor core's truncation of the lo operands; checked
-#                           against fp64 on random operands by tests/test_gpu_kernels.py and tools/gemm_check.py)
+#                           against fp64 on random operands by tests/test_gpu_kernels.py and
+#                           tests/test_gpu_gemm_patterns.py)
 #   logits, per molecule:   max|o_cuda - o_fp64| <= 3 max|o_ref32 - o_fp64| + 1e-4
 #   APD argmax:             identical to the fp32 reference wherever the reference's own top-2 gap exceeds its own
 #                           fp32-vs-fp64 movement on that molecule (bond-less molecules included)
