@@ -10,13 +10,29 @@
 // is ~2^-22 relative).  The cross terms, 2^-11 of the main ones, get their own accumulator so that their roundings stay
 // away from the large running sum; the two are added in fp32 in the epilogue.
 //
-// Structure (one persistent CTA per SM, 288 threads, 6-stage shared-memory ring of 32 KB stages, 128 x 64 output tiles):
-//   warp 8      TMA producer   cp.async.bulk.tensor (128B swizzle) raw A tile [128 x 32 fp32] + W_hi / W_lo (or raw W)
-//                              tiles [64 x 32]; TN: G and X as [32 rows x 32 floats] boxes.  mbarrier expect_tx per stage
+// Both kernels are persistent (one CTA per SM, work items = output tiles of up to 16 problems, or (tile, reduction
+// chunk) pairs in TN mode) and fed by one TMA lane through a ring of shared-memory stages (cp.async.bulk.tensor with
+// the 128-byte swizzle, mbarrier expect_tx per stage).
+//
+// tc3_wgmma_kernel: NT with W as pre-split (hi, lo) planes, the model's call pattern.  384 threads, 4-stage ring of
+// 48 KB stages, 128 x 128 output tiles:
+//   warpgroup 2     TMA producer   raw A tile [128 x 32 fp32] + W_hi and W_lo tiles [128 x 32] per k-block
+//                                  (setmaxnreg.dec: one lane issues, the rest idle)
+//   warpgroups 0-1  consumers      64 x 128 outputs each (setmaxnreg.inc): per half k-block (2 k-steps) the A
+//                                  fragments are read from the swizzled tile and split into (hi, lo) in registers,
+//                                  then 6 wgmma.m64n128k8 TF32 (A from registers, W_hi / W_lo straight from shared
+//                                  memory through descriptors) into two fp32 register accumulators, one wgmma group.
+//                                  The A fragments of the next half are prepared while the group of this one runs; a
+//                                  stage is handed back to the producer once the last group that reads it has retired
+// tc3_gemm_kernel: TN (weight gradients) and NT with raw fp32 W.  288 threads, 6-stage ring of 32 KB stages,
+// 128 x 64 output tiles:
+//   warp 8      TMA producer   NT: raw A tile [128 x 32 fp32] + raw W tile [64 x 32]; TN: G and X as
+//                              [32 rows x 32 floats] boxes
 //   warps 0-7   consumers      4 (M) x 2 (N) warps, 32 x 32 outputs each: fragments straight from the swizzled tiles
 //                              (conflict-free for K-major operands), split into (hi, lo) in registers,
 //                              mma.sync.m16n8k8 TF32 into two fp32 register accumulators, one mbarrier arrival per warp
-//                              frees the stage; then bias / SELU / dSELU / residual and the stores from registers
+//                              frees the stage
+// Both end in the same epilogue from registers: bias / SELU / dSELU / residual and the stores.
 //
 // Dynamic row counts: a problem may name device ints (m_dev, base_dev) -- the bond-type group sizes written by K0 --
 // instead of host values; tile counts are then computed on the device, so the launch needs no device->host read
@@ -37,16 +53,17 @@ namespace tc3 {
 
 using namespace tcptx;
 
-// An SM sub-partition holds 16K registers and receives every fourth warp of the CTA: with 9 warps (3 on one
-// sub-partition) a thread may use at most 168, which two register accumulators of 32 x 32 outputs (64) leave room for.
-// Two consumer warps per sub-partition hide more of the latency of the fragment loads and of the dependent MMAs than
-// one warp of 64 x 32 outputs with 255 registers (measured: C2 step 14.5 instead of 15.4 ms on an H100 SXM, 400 W).
-constexpr int BM = 128, BN = 64, BKF = 32;
-constexpr int STAGES = 6;
+constexpr int BM = 128, BKF = 32;                 // output tile rows and k-block (one 128-byte swizzle row of fp32)
 constexpr int A_BYTES = BM * BKF * 4;             // 16 KB
+constexpr int CONS_WARPS = 8;                     // consumer warps of both kernels
+
+// tc3_gemm_kernel (mma.sync).  An SM sub-partition holds 16K registers and receives every fourth warp of the CTA:
+// with 9 warps (3 on one sub-partition) a thread may use at most 168, which two register accumulators of 32 x 32
+// outputs (64) leave room for.
+constexpr int BN = 64;
+constexpr int STAGES = 6;
 constexpr int B_BYTES = BN * BKF * 4;             // 8 KB
-constexpr int STAGE_BYTES = A_BYTES + 2 * B_BYTES;   // NT: A raw | W hi (or raw W) | W lo      TN: G raw | X raw
-constexpr int CONS_WARPS = 8;
+constexpr int STAGE_BYTES = A_BYTES + B_BYTES;   // NT: A raw | W raw      TN: G raw | X raw
 constexpr int NUM_THREADS = 32 * CONS_WARPS + 32;   // 288
 constexpr int WM = 32, WN = 32;                   // warp tile
 constexpr int MI = WM / 16, NI = WN / 8;          // m16n8k8 MMAs per warp tile and k-step
@@ -54,21 +71,34 @@ constexpr int OFF_BARS = STAGES * STAGE_BYTES;
 constexpr int OFF_SCHED = OFF_BARS + 256;
 constexpr int SMEM_BYTES = OFF_SCHED + 512 + 1024 /*align slack*/;
 
+// tc3_wgmma_kernel.  Register split by setmaxnreg: 256 consumer threads x 232 + 128 producer threads x 40 = 64512 of
+// the SM's 65536.  A consumer holds two accumulators of 64 outputs (128 registers) and two buffers of half a
+// k-block's A fragments in (hi, lo) (2 x 16).  Buffers of a whole k-block (2 x 32) do not fit beside the
+// accumulators: ptxas then serialises every wgmma.
+constexpr int WG_BN = 128;
+constexpr int WG_STAGES = 4;
+constexpr int WG_B_BYTES = WG_BN * BKF * 4;       // 16 KB
+constexpr int WG_STAGE_BYTES = A_BYTES + 2 * WG_B_BYTES;   // 48 KB: A raw | W hi | W lo
+constexpr int WG_THREADS = 32 * CONS_WARPS + 128;   // 384
+constexpr int WG_OFF_BARS = WG_STAGES * WG_STAGE_BYTES;
+constexpr int WG_OFF_SCHED = WG_OFF_BARS + 256;
+constexpr int WG_SMEM_BYTES = WG_OFF_SCHED + 512 + 1024 /*align slack*/;
+static_assert(WG_SMEM_BYTES <= 227 * 1024, "wgmma stages exceed the shared memory of an SM");
+
 constexpr int kMaxChunkRows = 4096;   // reduction rows per work item of the weight-gradient mode
 constexpr int MAXP = kTc3MaxProblems;   // 16: e.g. the 5 layers x 3 bond types of a message MLP as one dependent chain
 
 struct Maps {   // TMA descriptors in kernel-parameter space
   CUtensorMap a[MAXP];      // NT: activations A (box 128 x 32)    TN: G (box 32 x 32)
-  CUtensorMap b[MAXP];      // NT: W hi plane or raw W (box 64 x 32)    TN: X (box 32 x 32)
-  CUtensorMap b_lo[MAXP];   // NT: W lo plane (pre-split weights only)
+  CUtensorMap b[MAXP];      // NT: W hi plane (box 128 x 32) or raw W (box 64 x 32)    TN: X (box 32 x 32)
+  CUtensorMap b_lo[MAXP];   // NT: W lo plane (box 128 x 32; pre-split weights only)
 };
 
 struct Params {
   GemmNT g[MAXP];           // TN: A = G, B = X, M = rows (capacity when m_dev is set), C = partials of the problem,
                             //     ldc = Kk, N = n_store = n_valid = Kk
-  int n_tiles[MAXP];        // column tiles of the output (NT: ceil(N / BN), TN: ceil(Kk / BN))
+  int n_tiles[MAXP];        // column tiles of the output (NT: ceil(N / tile width), TN: ceil(Kk / BN))
   int k_blocks[MAXP];       // NT: ceil(K / 32)
-  int bsplit[MAXP];         // NT: 1 = W arrives as (hi, lo) planes, 0 = raw W, split in registers like A
   int tn_mt[MAXP];          // TN: ceil(Nn / 128)
   int tn_nn[MAXP];          // TN: Nn
   float* bias_part[MAXP];   // TN: [splits][Nn] partial column sums of G (nullptr: not wanted)
@@ -90,7 +120,8 @@ struct Sched {              // computed once per CTA from host values or the dev
 
 struct Item { int p, m0, n0, nkb, z, r0, rows; };
 
-template <bool TN>
+// TBN: output tile width of the kernel
+template <bool TN, int TBN>
 __device__ __forceinline__ Item decode_item(const Params& P, const Sched& S, int item) {
   Item it;
   int p = 0;
@@ -102,14 +133,14 @@ __device__ __forceinline__ Item decode_item(const Params& P, const Sched& S, int
     const int tile = local % tiles_mn;
     it.z = local / tiles_mn;
     it.m0 = (tile / P.n_tiles[p]) * BM;
-    it.n0 = (tile % P.n_tiles[p]) * BN;
+    it.n0 = (tile % P.n_tiles[p]) * TBN;
     it.r0 = it.z * P.chunk_rows;
     it.rows = min(S.M[p], it.r0 + P.chunk_rows) - it.r0;
     it.nkb = ceil_div(it.rows, BKF);
   } else {
     it.z = 0; it.r0 = 0; it.rows = 0;
     it.m0 = (local / P.n_tiles[p]) * BM;
-    it.n0 = (local % P.n_tiles[p]) * BN;
+    it.n0 = (local % P.n_tiles[p]) * TBN;
     it.nkb = P.k_blocks[p];
   }
   return it;
@@ -179,6 +210,114 @@ __device__ __forceinline__ float epi_one(float v, float b, float x, int mode, in
   }
 }
 
+// Schedule of the launch from host values or the device-side row counts (thread 0 only).
+template <bool TN>
+__device__ __forceinline__ void init_sched(const Params& P, Sched& S) {
+  int total = 0;
+  for (int p = 0; p < P.nprob; ++p) {
+    const GemmNT& g = P.g[p];
+    const int base = g.base_dev ? __ldg(g.base_dev) : 0;
+    int M = g.M;
+    if (g.m_dev) {                        // device-side row count inside a buffer of g.M rows
+      M = __ldg(g.m_dev);
+      if (M > g.M - base) M = g.M - base;
+      if (M < 0) M = 0;
+    }
+    S.M[p] = M; S.base[p] = base; S.begin[p] = total;
+    if constexpr (TN) {
+      const int s = ceil_div(M, P.chunk_rows);
+      S.splits[p] = s;
+      total += P.tn_mt[p] * P.n_tiles[p] * s;
+    } else {
+      S.splits[p] = 1;
+      total += ceil_div(M, BM) * P.n_tiles[p];
+    }
+  }
+  for (int p = P.nprob; p <= MAXP; ++p) S.begin[p] = total;
+}
+
+// dependent chain (NT producer): wait until the row block of the layer below that work item w reads is complete
+__device__ __forceinline__ void wait_rows(const Params& P, const Item& w) {
+  const int d = P.dep[w.p];
+  const int* f = P.flags + P.flag_off[d] + w.m0 / BM;
+  const int need = P.n_tiles[d];
+  const long long t0 = clock64();
+  int have;
+  do {
+    asm volatile("ld.acquire.gpu.global.s32 %0, [%1];" : "=r"(have) : "l"(f) : "memory");
+    if (have < need) {
+      __nanosleep(64);
+      if (clock64() - t0 > 20000000000LL) __trap();   // ~10 s: a dead-lock, not contention
+    }
+  } while (have < need);
+  fence_proxy_async_all();               // other SMs' generic-proxy stores -> this SM's async-proxy (TMA) reads
+}
+
+// one problem's epilogue operands, resolved once per tile
+struct EpiArgs {
+  float* C;                // row 0 of the output rows the tile indexes
+  const float* X;          // aux, same rows (nullptr: none)
+  const float* bias;       // EPI_ACT only
+  int ldc, ldaux, n_store, n_valid, Ncols, Mrows, mode, act;
+  bool vec_c, vec_x;
+};
+
+__device__ __forceinline__ EpiArgs epi_args(const GemmNT& g, float* C, size_t row_base, int Mrows) {
+  EpiArgs e;
+  e.C = C;
+  e.X = g.aux ? g.aux + row_base * g.ldaux : nullptr;
+  e.bias = (g.mode == EPI_ACT) ? g.bias : nullptr;
+  e.ldc = g.ldc; e.ldaux = g.ldaux; e.n_store = g.n_store; e.n_valid = g.n_valid; e.Ncols = g.N; e.Mrows = Mrows;
+  e.mode = g.mode; e.act = g.act;
+  e.vec_c = (g.ldc & 1) == 0 && (reinterpret_cast<uintptr_t>(g.C) & 7) == 0;
+  e.vec_x = e.X && (g.ldaux & 1) == 0 && (reinterpret_cast<uintptr_t>(g.aux) & 7) == 0;
+  return e;
+}
+
+// bias of this lane's column pair (n, n + 1), n < n_store
+template <int EPI>
+__device__ __forceinline__ void epi_bias(const EpiArgs& e, int n, float* b) {
+  b[0] = 0.f; b[1] = 0.f;
+  if (EPI == EPI_SPEC_SELU || EPI == EPI_SPEC_LINEAR || EPI == EPI_SPEC_GENERIC) {
+    if (e.bias) {
+      if (n < e.Ncols) b[0] = __ldg(e.bias + n);
+      if (n + 1 < e.Ncols) b[1] = __ldg(e.bias + n + 1);
+    }
+  }
+}
+
+// epilogue and store of the accumulated pair v at (row m < Mrows, columns n, n + 1), n < n_store
+template <int EPI>
+__device__ __forceinline__ void epi_store(const EpiArgs& e, int m, int n, float v0, float v1, const float* b) {
+  float v[2] = {v0, v1};
+  float x[2] = {0.f, 0.f};
+  const bool need_x = (EPI == EPI_SPEC_DSELU || EPI == EPI_SPEC_ADD) || (EPI == EPI_SPEC_GENERIC && e.mode != EPI_ACT);
+  if (need_x) {
+    const float* ax = e.X + (size_t)m * e.ldaux + n;
+    if ((EPI != EPI_SPEC_GENERIC || e.vec_x) && n + 1 < e.n_store) {
+      const float2 t2 = __ldg(reinterpret_cast<const float2*>(ax));
+      x[0] = t2.x; x[1] = t2.y;
+    } else {
+      x[0] = ax[0];
+      if (n + 1 < e.n_store) x[1] = ax[1];
+    }
+  }
+  v[0] = epi_one<EPI>(v[0], b[0], x[0], e.mode, e.act);
+  v[1] = epi_one<EPI>(v[1], b[1], x[1], e.mode, e.act);
+  if (EPI == EPI_SPEC_GENERIC) {
+    if (n >= e.n_valid) v[0] = 0.f;
+    if (n + 1 >= e.n_valid) v[1] = 0.f;
+  }
+  float* dst = e.C + (size_t)m * e.ldc + n;
+  if ((EPI != EPI_SPEC_GENERIC || e.vec_c) && n + 1 < e.n_store) {
+    *reinterpret_cast<float2*>(dst) = make_float2(v[0], v[1]);
+  } else {
+    dst[0] = v[0];
+    if (n + 1 < e.n_store) dst[1] = v[1];
+  }
+}
+
+// ---- mma.sync kernel: TN (weight gradients) and NT with raw fp32 W ----
 template <bool TN, int EPI>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 tc3_gemm_kernel(const __grid_constant__ Maps maps, const Params P) {
@@ -197,27 +336,7 @@ tc3_gemm_kernel(const __grid_constant__ Maps maps, const Params P) {
       mbar_init(&empty[s], CONS_WARPS);     // one arrival per consumer warp (after __syncwarp)
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    int total = 0;
-    for (int p = 0; p < P.nprob; ++p) {
-      const GemmNT& g = P.g[p];
-      const int base = g.base_dev ? __ldg(g.base_dev) : 0;
-      int M = g.M;
-      if (g.m_dev) {                        // device-side row count inside a buffer of g.M rows
-        M = __ldg(g.m_dev);
-        if (M > g.M - base) M = g.M - base;
-        if (M < 0) M = 0;
-      }
-      S.M[p] = M; S.base[p] = base; S.begin[p] = total;
-      if constexpr (TN) {
-        const int s = ceil_div(M, P.chunk_rows);
-        S.splits[p] = s;
-        total += P.tn_mt[p] * P.n_tiles[p] * s;
-      } else {
-        S.splits[p] = 1;
-        total += ceil_div(M, BM) * P.n_tiles[p];
-      }
-    }
-    for (int p = P.nprob; p <= MAXP; ++p) S.begin[p] = total;
+    init_sched<TN>(P, S);
   }
   __syncthreads();
   const int num_items = S.begin[MAXP];
@@ -228,38 +347,20 @@ tc3_gemm_kernel(const __grid_constant__ Maps maps, const Params P) {
       int stage = 0;
       uint32_t phase = 0;
       for (int item = blockIdx.x; item < num_items; item += gridDim.x) {
-        const Item w = decode_item<TN>(P, S, item);
+        const Item w = decode_item<TN, BN>(P, S, item);
         const CUtensorMap* map_a = &maps.a[w.p];
         const CUtensorMap* map_b = &maps.b[w.p];
         const int base = S.base[w.p];
-        if constexpr (!TN) {
-          if (P.flags && P.dep[w.p] >= 0) {       // chain: the row block of the layer below must be complete
-            const int d = P.dep[w.p];
-            const int* f = P.flags + P.flag_off[d] + w.m0 / BM;
-            const int need = P.n_tiles[d];
-            const long long t0 = clock64();
-            int have;
-            do {
-              asm volatile("ld.acquire.gpu.global.s32 %0, [%1];" : "=r"(have) : "l"(f) : "memory");
-              if (have < need) {
-                __nanosleep(64);
-                if (clock64() - t0 > 20000000000LL) __trap();   // ~10 s: a dead-lock, not contention
-              }
-            } while (have < need);
-            fence_proxy_async_all();               // other SMs' generic-proxy stores -> this SM's async-proxy (TMA) reads
-          }
-        }
+        if constexpr (!TN)
+          if (P.flags && P.dep[w.p] >= 0) wait_rows(P, w);
         for (int kb = 0; kb < w.nkb; ++kb) {
           mbar_wait(&empty[stage], phase ^ 1);
           uint8_t* st = smem + stage * STAGE_BYTES;
+          mbar_arrive_expect_tx(&full[stage], A_BYTES + B_BYTES);
           if constexpr (!TN) {
-            const bool blo = P.bsplit[w.p] != 0;
-            mbar_arrive_expect_tx(&full[stage], A_BYTES + (blo ? 2 : 1) * B_BYTES);
             tma_load_2d(map_a, &full[stage], st, kb * BKF, base + w.m0);
             tma_load_2d(map_b, &full[stage], st + A_BYTES, kb * BKF, w.n0);
-            if (blo) tma_load_2d(&maps.b_lo[w.p], &full[stage], st + A_BYTES + B_BYTES, kb * BKF, w.n0);
           } else {
-            mbar_arrive_expect_tx(&full[stage], A_BYTES + B_BYTES);
             const int row = base + w.r0 + kb * BKF;   // 32 reduction rows per stage
 #pragma unroll
             for (int j = 0; j < BM / 32; ++j)         // 32-float column groups of G
@@ -280,10 +381,9 @@ tc3_gemm_kernel(const __grid_constant__ Maps maps, const Params P) {
     uint32_t phase = 0;
     int it = 0;
     for (int item = blockIdx.x; item < num_items; item += gridDim.x, ++it) {
-      const Item w = decode_item<TN>(P, S, item);
+      const Item w = decode_item<TN, BN>(P, S, item);
       const bool tr = P.trace && blockIdx.x == 0 && it < P.trace_tiles && threadIdx.x == 0;
       if (tr) P.trace[it * 16 + 0] = clock64();
-      const bool raw_b = !TN && P.bsplit[w.p] == 0;
       float acc[MI][NI][4], accx[MI][NI][4];
 #pragma unroll
       for (int i = 0; i < MI; ++i)
@@ -299,7 +399,7 @@ tc3_gemm_kernel(const __grid_constant__ Maps maps, const Params P) {
       for (int kb = 0; kb < w.nkb; ++kb) {
         mbar_wait(&full[stage], phase);
         const uint32_t sa = smem_u32(smem + stage * STAGE_BYTES);
-        const uint32_t sb = sa + A_BYTES, sbl = sb + B_BYTES;
+        const uint32_t sb = sa + A_BYTES;
         const int valid = TN ? w.rows - kb * BKF : BKF;   // TN: reduction rows past the chunk / row count may hold anything
 #pragma unroll
         for (int ks = 0; ks < BKF / 8; ++ks) {
@@ -310,13 +410,8 @@ tc3_gemm_kernel(const __grid_constant__ Maps maps, const Params P) {
           for (int j = 0; j < NI; ++j) {
             const int n = wn * WN + j * 8 + g8;
             if constexpr (!TN) {
-              if (!raw_b) {
-                bh[j][0] = __float_as_uint(lds32(sb + swz(n, k0)));  bh[j][1] = __float_as_uint(lds32(sb + swz(n, k1)));
-                bl[j][0] = __float_as_uint(lds32(sbl + swz(n, k0))); bl[j][1] = __float_as_uint(lds32(sbl + swz(n, k1)));
-              } else {
-                split_tf32_rn(lds32(sb + swz(n, k0)), bh[j][0], bl[j][0]);
-                split_tf32_rn(lds32(sb + swz(n, k1)), bh[j][1], bl[j][1]);
-              }
+              split_tf32_rn(lds32(sb + swz(n, k0)), bh[j][0], bl[j][0]);
+              split_tf32_rn(lds32(sb + swz(n, k1)), bh[j][1], bl[j][1]);
             } else {                              // B = X: element (m, k) of the MN-major X boxes
               float b0 = lds32(sb + (n >> 5) * 4096 + swz(k0, n & 31));
               float b1 = lds32(sb + (n >> 5) * 4096 + swz(k1, n & 31));
@@ -374,60 +469,153 @@ tc3_gemm_kernel(const __grid_constant__ Maps maps, const Params P) {
       }
       const int Mrows = TN ? P.tn_nn[w.p] : S.M[w.p];
       const size_t row_base = TN ? (size_t)0 : (size_t)S.base[w.p];
-      float* const Cbase = g.C + (TN ? (size_t)w.z * P.tn_nn[w.p] * g.ldc : row_base * g.ldc);
-      const float* const Xbase = g.aux ? g.aux + row_base * g.ldaux : nullptr;
-      const int ldc = g.ldc, ldaux = g.ldaux, n_store = g.n_store, n_valid = g.n_valid, Ncols = g.N;
-      const int mode = g.mode, act = g.act;
-      const float* const bias = (mode == EPI_ACT) ? g.bias : nullptr;
-      const bool vec_c = (ldc & 1) == 0 && (reinterpret_cast<uintptr_t>(g.C) & 7) == 0;
-      const bool vec_x = Xbase && (ldaux & 1) == 0 && (reinterpret_cast<uintptr_t>(g.aux) & 7) == 0;
+      const EpiArgs e = epi_args(g, g.C + (TN ? (size_t)w.z * P.tn_nn[w.p] * g.ldc : row_base * g.ldc), row_base, Mrows);
 #pragma unroll
       for (int j = 0; j < NI; ++j) {
         const int n = w.n0 + wn * WN + j * 8 + 2 * t4;    // this lane's column pair
-        if (n >= n_store) continue;
-        float b[2] = {0.f, 0.f};
-        if (EPI == EPI_SPEC_SELU || EPI == EPI_SPEC_LINEAR || EPI == EPI_SPEC_GENERIC) {
-          if (bias) {
-            if (n < Ncols) b[0] = __ldg(bias + n);
-            if (n + 1 < Ncols) b[1] = __ldg(bias + n + 1);
-          }
-        }
+        if (n >= e.n_store) continue;
+        float b[2];
+        epi_bias<EPI>(e, n, b);
 #pragma unroll
         for (int i = 0; i < MI; ++i)
 #pragma unroll
           for (int h = 0; h < 2; ++h) {
             const int m = w.m0 + wm * WM + i * 16 + h * 8 + g8;
             if (m >= Mrows) continue;
-            float v[2] = {acc[i][j][2 * h] + accx[i][j][2 * h], acc[i][j][2 * h + 1] + accx[i][j][2 * h + 1]};
-            float x[2] = {0.f, 0.f};
-            const bool need_x = (EPI == EPI_SPEC_DSELU || EPI == EPI_SPEC_ADD) || (EPI == EPI_SPEC_GENERIC && mode != EPI_ACT);
-            if (need_x) {
-              const float* ax = Xbase + (size_t)m * ldaux + n;
-              if ((EPI != EPI_SPEC_GENERIC || vec_x) && n + 1 < n_store) {
-                const float2 t2 = __ldg(reinterpret_cast<const float2*>(ax));
-                x[0] = t2.x; x[1] = t2.y;
-              } else {
-                x[0] = ax[0];
-                if (n + 1 < n_store) x[1] = ax[1];
-              }
-            }
-            v[0] = epi_one<EPI>(v[0], b[0], x[0], mode, act);
-            v[1] = epi_one<EPI>(v[1], b[1], x[1], mode, act);
-            if (EPI == EPI_SPEC_GENERIC) {
-              if (n >= n_valid) v[0] = 0.f;
-              if (n + 1 >= n_valid) v[1] = 0.f;
-            }
-            float* dst = Cbase + (size_t)m * ldc + n;
-            if ((EPI != EPI_SPEC_GENERIC || vec_c) && n + 1 < n_store) {
-              *reinterpret_cast<float2*>(dst) = make_float2(v[0], v[1]);
-            } else {
-              dst[0] = v[0];
-              if (n + 1 < n_store) dst[1] = v[1];
-            }
+            epi_store<EPI>(e, m, n, acc[i][j][2 * h] + accx[i][j][2 * h], acc[i][j][2 * h + 1] + accx[i][j][2 * h + 1], b);
           }
       }
       if constexpr (!TN)
         if (P.flags) signal_tile(P.flags + P.flag_off[w.p] + w.m0 / BM);
+      if (tr) P.trace[it * 16 + 6] = clock64();
+    }
+  }
+}
+
+// ---- wgmma kernel: NT with pre-split W ----
+template <int EPI>
+__global__ void __launch_bounds__(WG_THREADS, 1)
+tc3_wgmma_kernel(const __grid_constant__ Maps maps, const Params P) {
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + WG_OFF_BARS);
+  uint64_t* full = bars;                    // [WG_STAGES] TMA -> consumers
+  uint64_t* empty = bars + WG_STAGES;       // [WG_STAGES] consumers -> TMA
+  Sched& S = *reinterpret_cast<Sched*>(smem + WG_OFF_SCHED);
+
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < WG_STAGES; ++s) {
+      mbar_init(&full[s], 1);
+      mbar_init(&empty[s], CONS_WARPS);     // one arrival per consumer warp, once its wgmma group has retired
+    }
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    init_sched<false>(P, S);
+  }
+  __syncthreads();
+  const int num_items = S.begin[MAXP];
+
+  if (warp >= CONS_WARPS) {
+    // ================= TMA producer (warpgroup 2) =================
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
+    if (warp == CONS_WARPS && lane == 0) {
+      int stage = 0;
+      uint32_t phase = 0;
+      for (int item = blockIdx.x; item < num_items; item += gridDim.x) {
+        const Item w = decode_item<false, WG_BN>(P, S, item);
+        const int base = S.base[w.p];
+        if (P.flags && P.dep[w.p] >= 0) wait_rows(P, w);
+        for (int kb = 0; kb < w.nkb; ++kb) {
+          mbar_wait(&empty[stage], phase ^ 1);
+          uint8_t* st = smem + stage * WG_STAGE_BYTES;
+          mbar_arrive_expect_tx(&full[stage], WG_STAGE_BYTES);
+          tma_load_2d(&maps.a[w.p], &full[stage], st, kb * BKF, base + w.m0);
+          tma_load_2d(&maps.b[w.p], &full[stage], st + A_BYTES, kb * BKF, w.n0);
+          tma_load_2d(&maps.b_lo[w.p], &full[stage], st + A_BYTES + WG_B_BYTES, kb * BKF, w.n0);
+          if (++stage == WG_STAGES) { stage = 0; phase ^= 1; }
+        }
+      }
+    }
+  } else {
+    // ================= consumers (warpgroups 0-1): A fragments -> (hi, lo) -> wgmma -> epilogue =================
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+    const int g8 = lane >> 2, t4 = lane & 3;     // fragment coordinates
+    const int r0 = (warp >> 2) * 64 + (warp & 3) * 16 + g8;   // this lane's A / output rows in the tile: r0, r0 + 8
+    int stage = 0;
+    uint32_t phase = 0;
+    int it = 0;
+    for (int item = blockIdx.x; item < num_items; item += gridDim.x, ++it) {
+      const Item w = decode_item<false, WG_BN>(P, S, item);
+      const bool tr = P.trace && blockIdx.x == 0 && it < P.trace_tiles && threadIdx.x == 0;
+      if (tr) P.trace[it * 16 + 0] = clock64();
+      float acc[64], accx[64];
+#pragma unroll
+      for (int e = 0; e < 64; ++e) { acc[e] = 0.f; accx[e] = 0.f; }
+
+      // A fragments are staged half a k-block (2 k-steps) at a time in two register buffers: half 0 of every k-block
+      // in (ah0, al0), half 1 in (ah1, al1), each followed by its 6 wgmma as one group.  wait_group 1 after each
+      // commit retires the group before it, so a buffer is rewritten only after the group that read it has retired,
+      // and the stage of k-block kb - 1 goes back to the producer once the group of its half 1 has retired (in
+      // half 0 of k-block kb) -- while the A fragments of the next half are prepared, a group is in flight.
+      uint32_t ah0[2][4], al0[2][4], ah1[2][4], al1[2][4];
+      int prev = -1;
+      auto half = [&](uint32_t sa, int hk, uint32_t (&ah)[2][4], uint32_t (&al)[2][4]) {
+#pragma unroll
+        for (int s = 0; s < 2; ++s) {
+          const int k0 = (2 * hk + s) * 8 + t4, k1 = k0 + 4;
+          split_tf32_rn(lds32(sa + swz(r0, k0)), ah[s][0], al[s][0]);
+          split_tf32_rn(lds32(sa + swz(r0 + 8, k0)), ah[s][1], al[s][1]);
+          split_tf32_rn(lds32(sa + swz(r0, k1)), ah[s][2], al[s][2]);
+          split_tf32_rn(lds32(sa + swz(r0 + 8, k1)), ah[s][3], al[s][3]);
+        }
+        wgmma_fence();
+#pragma unroll
+        for (int s = 0; s < 2; ++s) {
+          const uint32_t ko = (2 * hk + s) * 32;
+          const uint64_t dh = wgmma_desc_sw128(sa + A_BYTES + ko);
+          const uint64_t dl = wgmma_desc_sw128(sa + A_BYTES + WG_B_BYTES + ko);
+          wgmma_m64n128k8_tf32(acc, ah[s], dh);
+          wgmma_m64n128k8_tf32(accx, al[s], dh);
+          wgmma_m64n128k8_tf32(accx, ah[s], dl);
+        }
+        wgmma_commit();
+        wgmma_wait<1>();
+      };
+      for (int kb = 0; kb < w.nkb; ++kb) {
+        mbar_wait(&full[stage], phase);
+        const uint32_t sa = smem_u32(smem + stage * WG_STAGE_BYTES);
+        half(sa, 0, ah0, al0);
+        if (prev >= 0) {
+          __syncwarp();
+          if (lane == 0) mbar_arrive(&empty[prev]);
+        }
+        half(sa, 1, ah1, al1);
+        prev = stage;
+        if (++stage == WG_STAGES) { stage = 0; phase ^= 1; }
+      }
+      wgmma_wait<0>();
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&empty[prev]);
+
+      const GemmNT& g = P.g[w.p];
+      const int Mrows = S.M[w.p];
+      const size_t row_base = (size_t)S.base[w.p];
+      const EpiArgs e = epi_args(g, g.C + row_base * g.ldc, row_base, Mrows);
+#pragma unroll
+      for (int j = 0; j < WG_BN / 8; ++j) {
+        const int n = w.n0 + j * 8 + 2 * t4;      // this lane's column pair
+        if (n >= e.n_store) continue;
+        float b[2];
+        epi_bias<EPI>(e, n, b);
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int m = w.m0 + r0 + h * 8;
+          if (m >= Mrows) continue;
+          epi_store<EPI>(e, m, n, acc[4 * j + 2 * h] + accx[4 * j + 2 * h], acc[4 * j + 2 * h + 1] + accx[4 * j + 2 * h + 1], b);
+        }
+      }
+      if (P.flags) signal_tile(P.flags + P.flag_off[w.p] + w.m0 / BM);
       if (tr) P.trace[it * 16 + 6] = clock64();
     }
   }
@@ -582,6 +770,11 @@ static int prepare(int* num_sms_out) {
     GIB_CUDA_TRY(cudaFuncSetAttribute(tc3_gemm_kernel<false, EPI_SPEC_DSELU>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
     GIB_CUDA_TRY(cudaFuncSetAttribute(tc3_gemm_kernel<false, EPI_SPEC_ADD>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
     GIB_CUDA_TRY(cudaFuncSetAttribute(tc3_gemm_kernel<true, EPI_SPEC_LINEAR>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
+    GIB_CUDA_TRY(cudaFuncSetAttribute(tc3_wgmma_kernel<EPI_SPEC_GENERIC>, cudaFuncAttributeMaxDynamicSharedMemorySize, WG_SMEM_BYTES));
+    GIB_CUDA_TRY(cudaFuncSetAttribute(tc3_wgmma_kernel<EPI_SPEC_SELU>, cudaFuncAttributeMaxDynamicSharedMemorySize, WG_SMEM_BYTES));
+    GIB_CUDA_TRY(cudaFuncSetAttribute(tc3_wgmma_kernel<EPI_SPEC_LINEAR>, cudaFuncAttributeMaxDynamicSharedMemorySize, WG_SMEM_BYTES));
+    GIB_CUDA_TRY(cudaFuncSetAttribute(tc3_wgmma_kernel<EPI_SPEC_DSELU>, cudaFuncAttributeMaxDynamicSharedMemorySize, WG_SMEM_BYTES));
+    GIB_CUDA_TRY(cudaFuncSetAttribute(tc3_wgmma_kernel<EPI_SPEC_ADD>, cudaFuncAttributeMaxDynamicSharedMemorySize, WG_SMEM_BYTES));
     d.attr_done = true;
   }
   *num_sms_out = d.num_sms;
@@ -633,13 +826,14 @@ bool tc3_eligible(const GemmNT& p) {
          p.B_lo && al(p.A) && al(p.B_hi) && al(p.B_lo);
 }
 
-// up to MAXP NT problems in one persistent launch; dep == nullptr: independent.  raw_ok: W may be raw fp32 (split in
-// the kernel) when a problem carries no aligned planes
-static int launch_nt(const GemmNT* ps, const int* dep, int n, int* flags, bool raw_ok, cudaStream_t st) {
+// up to MAXP NT problems in one persistent launch; dep == nullptr: independent.  raw: every W is raw fp32 (split in
+// the kernel; mma.sync kernel), else every W comes as aligned (hi, lo) planes (wgmma kernel)
+static int launch_nt(const GemmNT* ps, const int* dep, int n, int* flags, bool raw, cudaStream_t st) {
   using namespace tc3;
   if (n < 1 || n > MAXP) { set_error("gemm_nt_tc3: %d problems (max %d)", n, MAXP); return -2; }
   int num_sms = 0;
   GIB_TRY(prepare(&num_sms));
+  const int tbn = raw ? BN : WG_BN;
   Maps maps;
   Params P;
   memset(&P, 0, sizeof(P));
@@ -653,19 +847,17 @@ static int launch_nt(const GemmNT* ps, const int* dep, int n, int* flags, bool r
     const GemmNT& p = ps[i];
     slot[i] = -1;
     if (p.M <= 0 || p.N <= 0) continue;
-    const bool planes = presplit(p);
-    if (!(planes ? tc3_eligible(p) : raw_ok && tc_eligible(p))) {
+    if (!(raw ? tc_eligible(p) : presplit(p) && tc3_eligible(p))) {
       set_error("gemm_nt_tc3: operands violate the TMA alignment / pre-split contract");
       return -2;
     }
     const int sp = epi_spec(p);
     spec = (spec < 0 || spec == sp) ? sp : EPI_SPEC_GENERIC;     // one epilogue specialisation per launch
     GIB_TRY(make_map(&maps.a[np], p.A, p.M, p.K, p.lda, BM));
-    GIB_TRY(make_map(&maps.b[np], planes ? p.B_hi : p.B, p.N, p.K, p.ldb, BN));
-    if (planes) GIB_TRY(make_map(&maps.b_lo[np], p.B_lo, p.N, p.K, p.ldb, BN));
-    P.bsplit[np] = planes ? 1 : 0;
+    GIB_TRY(make_map(&maps.b[np], raw ? p.B : p.B_hi, p.N, p.K, p.ldb, tbn));
+    if (!raw) GIB_TRY(make_map(&maps.b_lo[np], p.B_lo, p.N, p.K, p.ldb, tbn));
     P.g[np] = p;
-    P.n_tiles[np] = ceil_div(std::max(p.N, p.n_store), BN);   // columns [N, n_store) are stored too (zeros / epi(0))
+    P.n_tiles[np] = ceil_div(std::max(p.N, p.n_store), tbn);   // columns [N, n_store) are stored too (zeros / epi(0))
     P.k_blocks[np] = ceil_div(p.K, BKF);
     P.dep[np] = -1;
     P.flag_off[np] = flag_ints;
@@ -693,12 +885,22 @@ static int launch_nt(const GemmNT* ps, const int* dep, int n, int* flags, bool r
   }
   const int grid = (int)(tiles < num_sms ? tiles : num_sms);
   ProfScope prof(PROF_GEMM_NT, work, st);
-  switch (spec) {
-    case EPI_SPEC_SELU: tc3_gemm_kernel<false, EPI_SPEC_SELU><<<grid, NUM_THREADS, SMEM_BYTES, st>>>(maps, P); break;
-    case EPI_SPEC_LINEAR: tc3_gemm_kernel<false, EPI_SPEC_LINEAR><<<grid, NUM_THREADS, SMEM_BYTES, st>>>(maps, P); break;
-    case EPI_SPEC_DSELU: tc3_gemm_kernel<false, EPI_SPEC_DSELU><<<grid, NUM_THREADS, SMEM_BYTES, st>>>(maps, P); break;
-    case EPI_SPEC_ADD: tc3_gemm_kernel<false, EPI_SPEC_ADD><<<grid, NUM_THREADS, SMEM_BYTES, st>>>(maps, P); break;
-    default: tc3_gemm_kernel<false, EPI_SPEC_GENERIC><<<grid, NUM_THREADS, SMEM_BYTES, st>>>(maps, P); break;
+  if (raw) {
+    switch (spec) {
+      case EPI_SPEC_SELU: tc3_gemm_kernel<false, EPI_SPEC_SELU><<<grid, NUM_THREADS, SMEM_BYTES, st>>>(maps, P); break;
+      case EPI_SPEC_LINEAR: tc3_gemm_kernel<false, EPI_SPEC_LINEAR><<<grid, NUM_THREADS, SMEM_BYTES, st>>>(maps, P); break;
+      case EPI_SPEC_DSELU: tc3_gemm_kernel<false, EPI_SPEC_DSELU><<<grid, NUM_THREADS, SMEM_BYTES, st>>>(maps, P); break;
+      case EPI_SPEC_ADD: tc3_gemm_kernel<false, EPI_SPEC_ADD><<<grid, NUM_THREADS, SMEM_BYTES, st>>>(maps, P); break;
+      default: tc3_gemm_kernel<false, EPI_SPEC_GENERIC><<<grid, NUM_THREADS, SMEM_BYTES, st>>>(maps, P); break;
+    }
+  } else {
+    switch (spec) {
+      case EPI_SPEC_SELU: tc3_wgmma_kernel<EPI_SPEC_SELU><<<grid, WG_THREADS, WG_SMEM_BYTES, st>>>(maps, P); break;
+      case EPI_SPEC_LINEAR: tc3_wgmma_kernel<EPI_SPEC_LINEAR><<<grid, WG_THREADS, WG_SMEM_BYTES, st>>>(maps, P); break;
+      case EPI_SPEC_DSELU: tc3_wgmma_kernel<EPI_SPEC_DSELU><<<grid, WG_THREADS, WG_SMEM_BYTES, st>>>(maps, P); break;
+      case EPI_SPEC_ADD: tc3_wgmma_kernel<EPI_SPEC_ADD><<<grid, WG_THREADS, WG_SMEM_BYTES, st>>>(maps, P); break;
+      default: tc3_wgmma_kernel<EPI_SPEC_GENERIC><<<grid, WG_THREADS, WG_SMEM_BYTES, st>>>(maps, P); break;
+    }
   }
   GIB_LAUNCH_CHECK();
   return 0;
@@ -706,10 +908,19 @@ static int launch_nt(const GemmNT* ps, const int* dep, int n, int* flags, bool r
 
 int gemm_nt_tc3_group(const GemmNT* ps, int n, cudaStream_t st) { return launch_nt(ps, nullptr, n, nullptr, false, st); }
 
-// up to 4 independent problems whose weights may be raw fp32 (split in the kernel)
+// up to 4 independent problems whose weights may be raw fp32 (split in the kernel): members with aligned planes run
+// on the wgmma kernel, the others on the mma.sync kernel, one launch for each kind present
 int gemm_nt_tc_group(const GemmNT* ps, int n, cudaStream_t st) {
   if (n < 1 || n > 4) { set_error("gemm_nt_tc_group: %d problems (max 4)", n); return -2; }
-  return launch_nt(ps, nullptr, n, nullptr, true, st);
+  GemmNT planes[4], raw[4];
+  int np = 0, nr = 0;
+  for (int i = 0; i < n; ++i) {
+    if (tc3::presplit(ps[i])) planes[np++] = ps[i];
+    else raw[nr++] = ps[i];
+  }
+  if (np) GIB_TRY(launch_nt(planes, nullptr, np, nullptr, false, st));
+  if (nr) GIB_TRY(launch_nt(raw, nullptr, nr, nullptr, true, st));
+  return 0;
 }
 
 int gemm_nt_tc(const GemmNT& p, cudaStream_t st) { return gemm_nt_tc_group(&p, 1, st); }
