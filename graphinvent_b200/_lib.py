@@ -43,7 +43,7 @@ MODEL_ID = {"GGNN": 0, "MNN": 1, "AttGGNN": 2, "EMN": 3}
 HDR_INTS = 16
 HDR_E, HDR_P, HDR_TYPE_COUNT, HDR_TYPE_BASE, HDR_FLAGS, HDR_CAPACITY = 0, 1, 2, 6, 11, 12
 FLAG_MULTITYPE, FLAG_NONBINARY, FLAG_OVERFLOW = 1, 2, 4
-ABI_VERSION = 202      # must equal gib_version() of the loaded library (include/gib200.h)
+ABI_VERSION = 203     # must equal gib_version() of the loaded library (include/gib200.h)
 
 _PROTOS = {
     "gib_last_error": (ctypes.c_char_p, []),
@@ -102,7 +102,24 @@ _PROTOS = {
     "gib_test_graph_gather_bwd": (c_i, [c_p] * 6 + [c_i, c_i, c_i, c_p]),
     "gib_test_emn_aggregate_fwd": (c_i, [c_p] * 5 + [c_i] + [c_p] * 3 + [c_ll, c_p, c_p]),
     "gib_test_emn_aggregate_bwd": (c_i, [c_p] * 10 + [c_i] + [c_p] * 5 + [c_ll, c_p, c_p]),
+    "gib_test_scatter_sum": (c_i, [c_p, c_p, c_i, c_p, c_p, c_p, c_i, c_ll, c_p]),
+    "gib_test_gru_fwd": (c_i, [c_p, c_p, c_p, c_p, c_i, c_p, c_ll, c_p, c_p]),
+    "gib_test_gather_rows": (c_i, [c_p, c_p, c_i, c_p, c_p, c_i, c_ll, c_p, c_p]),
+    "gib_test_sum_nodes_fwd": (c_i, [c_p, c_p, c_i, c_i, c_i, c_p]),
+    "gib_test_bcast_nodes_add": (c_i, [c_p, c_p, c_i, c_i, c_ll, c_p]),
+    "gib_test_concat2_in": (c_i, [c_p, c_i, c_p, c_i, c_i, c_i, c_p, c_i, c_i, c_i, c_ll, c_p]),
+    "gib_test_concat_flat": (c_i, [c_p, c_i, c_p, c_i, c_i, c_i, c_p, c_i, c_i, c_i, c_p]),
+    "gib_test_unflatten_dact": (c_i, [c_p, c_i, c_p, c_i, c_p, c_i, c_i, c_ll, c_p]),
+    "gib_test_dact_slice": (c_i, [c_p, c_i, c_p, c_p, c_i, c_i, c_i, c_i, c_i, c_p]),
+    "gib_test_sum3_cols": (c_i, [c_p, c_i, c_i, c_p, c_i, c_i, c_p, c_i, c_i, c_p, c_i, c_i, c_p]),
+    "gib_test_tanh_fwd": (c_i, [c_p, c_p, c_ll, c_i, c_p, c_p]),
+    "gib_test_tanh_selu_bwd": (c_i, [c_p, c_p, c_p, c_p, c_ll, c_i, c_p, c_p]),
+    "gib_test_mul_dselu": (c_i, [c_p, c_p, c_p, c_ll, c_i, c_p, c_p]),
+    "gib_test_emn_input": (c_i, [c_p, c_i, c_p, c_p, c_i, c_p, c_p, c_i, c_i, c_i, c_ll, c_p]),
+    "gib_test_plan_linear": (c_i, [c_p, c_i, c_p]),
 }
+PLAN_LINEAR_FIELDS = ("pw", "pb", "src_off", "rs", "cs", "nblk", "Rb", "Rbp", "C", "Cp", "Ct", "Ctp",
+                      "ow", "owt", "ob", "ow_hi", "ow_lo", "owt_hi", "owt_lo")   # GIB_PLAN_LINEAR_FIELDS, in order
 
 
 def exported_symbols():

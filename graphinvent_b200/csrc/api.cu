@@ -109,22 +109,26 @@ __global__ void __launch_bounds__(256) sample_actions_kernel(const float* __rest
     for (int i = 1; i <= 256; ++i) pre[i] += pre[i - 1];   // fixed-order prefix: deterministic
   __syncthreads();
   const float total = pre[256];
-  const float target = uniforms[b] * total;
-  // the owner thread is the first chunk whose inclusive prefix exceeds the target
-  const bool owner = (pre[threadIdx.x] <= target && target < pre[threadIdx.x + 1]) ||
-                     (threadIdx.x == 255 && target >= pre[256]);
+  float target = uniforms[b] * total;
+  // u * total may round up to the total: keep the target inside [0, total) so that it always has an owner chunk
+  if (target >= total) target = nextafterf(total, 0.f);
+  // the owner thread is the chunk whose prefix bracket [pre[t], pre[t+1]) holds the target: its sum is > 0, so it holds
+  // an action of non-zero probability
+  const bool owner = pre[threadIdx.x] <= target && target < pre[threadIdx.x + 1];
   if (owner && hi > lo) {
     float run = pre[threadIdx.x];
-    int pick = hi - 1;
+    int pick = -1, last = lo;
     for (int k = lo; k < hi; ++k) {
-      run += expf(o[k] - mx);
+      const float e = expf(o[k] - mx);
+      run += e;
+      if (e > 0.f) last = k;
       if (target < run) { pick = k; break; }
     }
+    // the running sum can end a few ulps below pre[t+1] (other rounding order): the last action of the chunk with
+    // non-zero probability, never one of probability 0
+    if (pick < 0) pick = last;
     action[b] = pick;
     lik[b] = expf(o[pick] - mx) / total;
-  } else if (owner) {  // empty tail chunk: fall back to the last element
-    action[b] = apd - 1;
-    lik[b] = expf(o[apd - 1] - mx) / total;
   }
   // a row with NaN / Inf logits has no owner (every comparison with NaN is false): defined outputs instead of the
   // caller's uninitialised memory -- "terminate" with a NaN likelihood, which the caller can detect
@@ -143,8 +147,8 @@ using namespace gib;
 extern "C" {
 
 const char* gib_last_error(void) { return g_err; }
-// 200: capacity mode, int8 inputs, grouped dW; 201: 5 profile classes; 202: test hooks
-int gib_version(void) { return 202; }
+// 200: capacity mode, int8 inputs, grouped dW; 201: 5 profile classes; 202: test hooks; 203: forward / glue test hooks
+int gib_version(void) { return 203; }
 void gib_set_tensor_cores(int on) { g_use_tc = on != 0; }
 int gib_get_tensor_cores(void) { return g_use_tc ? 1 : 0; }
 void gib_tc_debug(int mode) { g_tc_debug = mode; }
@@ -488,6 +492,72 @@ int gib_test_emn_aggregate_bwd(float* dEMx, float* dENx, float* dEMm, float* dEN
   ga.ent_dst = const_cast<int*>(ent_dst); ga.ent_src = const_cast<int*>(ent_src); ga.dst_ptr = const_cast<int*>(dst_ptr);
   ga.src_ptr = const_cast<int*>(src_ptr); ga.src_ent = const_cast<int*>(src_ent);
   return emn_aggregate_bwd(dEMx, dENx, dEMm, dENm, st3, dmsg, EMx, ENx, EMm, ENm, ld, ga, E, live, ST(stream));
+}
+int gib_test_scatter_sum(float* out, const float* msg, int ld, const int* ptr, const int* ent, const float* w,
+                         int accumulate, long long S, gib_stream stream) {
+  return scatter_sum(out, msg, ld, ptr, ent, w, accumulate, S, ST(stream));
+}
+int gib_test_gru_fwd(float* hn, const float* gi, const float* gh, const float* h, int Hp, const int* ptr, long long S,
+                     const int* live, gib_stream stream) {
+  return gru_fwd(hn, gi, gh, h, Hp, ptr, S, live, ST(stream));
+}
+int gib_test_gather_rows(float* dst, const float* h, int ld, const int* src, const float* w, int scale, long long P,
+                         const int* live, gib_stream stream) {
+  return gather_rows(dst, h, ld, src, w, scale, P, live, ST(stream));
+}
+int gib_test_sum_nodes_fwd(float* g, const float* h, int ld, int N, int B, gib_stream stream) {
+  return sum_nodes_fwd(g, h, ld, N, B, ST(stream));
+}
+int gib_test_bcast_nodes_add(float* dh, const float* dg, int ld, int N, long long S, gib_stream stream) {
+  return bcast_nodes_add(dh, dg, ld, N, S, ST(stream));
+}
+int gib_test_concat2_in(float* dst, int ldd, const void* a, int lda, int wa, int a_i8, const void* b, int ldb, int wb,
+                        int b_i8, long long rows, gib_stream stream) {
+  return concat2_in(dst, ldd, a, lda, wa, a_i8, b, ldb, wb, b_i8, rows, ST(stream));
+}
+int gib_test_concat_flat(float* dst, int ldd, const float* f1, int ldf, int N, int fa, const float* g, int ldg, int W,
+                         int B, gib_stream stream) {
+  return concat_flat(dst, ldd, f1, ldf, N, fa, g, ldg, W, B, ST(stream));
+}
+int gib_test_unflatten_dact(float* G, int ldf, const float* dcat, int ldd, const float* f1, int N, int fa, long long S,
+                            gib_stream stream) {
+  return unflatten_dact(G, ldf, dcat, ldd, f1, N, fa, S, ST(stream));
+}
+int gib_test_dact_slice(float* G, int ldg, const float* dout, const float* out, int ldo, int off, int width, int act,
+                        int rows, gib_stream stream) {
+  return dact_slice(G, ldg, dout, out, ldo, off, width, act, rows, ST(stream));
+}
+int gib_test_sum3_cols(float* dst, int ldd, int W, const float* a, int lda, int offa, const float* b2, int ldb,
+                       int offb, const float* c3, int ldc, int rows, gib_stream stream) {
+  return sum3_cols(dst, ldd, W, a, lda, offa, b2, ldb, offb, c3, ldc, rows, ST(stream));
+}
+int gib_test_tanh_fwd(float* y, const float* x, long long rows, int ld, const int* live, gib_stream stream) {
+  return tanh_fwd(y, x, rows, ld, live, ST(stream));
+}
+int gib_test_tanh_selu_bwd(float* G, const float* dy, const float* y, const float* pre, long long rows, int ld,
+                           const int* live, gib_stream stream) {
+  return tanh_selu_bwd(G, dy, y, pre, rows, ld, live, ST(stream));
+}
+int gib_test_mul_dselu(float* G, const float* d, const float* y, long long rows, int ld, const int* live,
+                       gib_stream stream) {
+  return mul_dselu(G, d, y, rows, ld, live, ST(stream));
+}
+int gib_test_emn_input(float* X, int ld, const void* nodes, const void* edges, int i8, const int* ent_dst,
+                       const int* ent_src, int N, int F, int Ef, long long P, gib_stream stream) {
+  return emn_input(X, ld, nodes, edges, i8, ent_dst, ent_src, N, F, Ef, P, ST(stream));
+}
+int gib_test_plan_linear(const gib_dims* d, int i, long long* out) {
+  Plan pl;
+  GIB_TRY(build_plan(*d, pl));
+  const int n = (int)pl.lins.size();
+  if (i < 0 || i >= n) { set_error("gib_test_plan_linear: Linear %d of %d", i, n); return -2; }
+  const Lin& l = pl.lins[i];
+  const long long v[GIB_PLAN_LINEAR_FIELDS] = {l.pw, l.pb, l.src_off, l.rs, l.cs, l.nblk, l.Rb, l.Rbp, l.C, l.Cp, l.Ct,
+                                               l.Ctp, (long long)l.ow, (long long)l.owt, (long long)l.ob,
+                                               (long long)l.ow_hi, (long long)l.ow_lo, (long long)l.owt_hi,
+                                               (long long)l.owt_lo};
+  memcpy(out, v, sizeof(v));
+  return n;
 }
 
 }  // extern "C"

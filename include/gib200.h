@@ -203,7 +203,7 @@ int gib_graph_gather(float* g, float* att, const float* en, const float* em, int
 
 /* ---- test hooks: thin entries into the GEMM dispatchers and the backward / EMN kernels the model calls, so that each
  *      can be checked on its own against a float64 reference (tests/test_gpu_gemm_patterns.py,
- *      tests/test_gpu_graph_kernels.py).  Each entry calls the internal function the model calls and adds no path of its
+ *      tests/test_gpu_graph_kernels.py, tests/test_gpu_forward_kernels.py).  Each entry calls the internal function the model calls and adds no path of its
  *      own.  `ps`, `dep`, `qs` and `group_sizes` are HOST arrays; everything they point to lives on the device. ---- */
 /* one NT problem: C[M, :n_store] = epi(A[M,K] W[N,K]^T) with A, W row-major, K % 16 == 0, lda / ldb % 4 == 0;
  * epi (mode): 0 act(acc + bias), 1 acc * act'(aux) (aux = the activation OUTPUT), 2 acc + aux (aux may alias C);
@@ -271,6 +271,52 @@ int gib_test_emn_aggregate_bwd(float* dEMx, float* dENx, float* dEMm, float* dEN
                                const float* EMx, const float* ENx, const float* EMm, const float* ENm, int ld,
                                const int* ent_dst, const int* ent_src, const int* dst_ptr, const int* src_ptr,
                                const int* src_ent, long long E, const int* live, gib_stream stream);
+/* forward and glue kernels (tests/test_gpu_forward_kernels.py).  live (may be NULL): device count of the rows to
+ * process, clamped to the row count; rows past it are not touched.
+ * scatter_sum: out[s] (+= when accumulate) sum_{q in [ptr[s], ptr[s+1])} w[ent[q]] msg[ent[q]] (w may be NULL: 1),
+ * with the variant gib_scatter_variant selects; ld % 4 == 0 */
+int gib_test_scatter_sum(float* out, const float* msg, int ld, const int* ptr, const int* ent, const float* w,
+                         int accumulate, long long S, gib_stream stream);
+/* gib_gru_gates with a live count (h == NULL: h = 0 and gh is one bias row, the EMN form) */
+int gib_test_gru_fwd(float* hn, const float* gi, const float* gh, const float* h, int Hp, const int* ptr, long long S,
+                     const int* live, gib_stream stream);
+/* dst[p] = (scale && w ? w[p] : 1) * h[src[p]] (src[p] < 0: zeros); ld % 4 == 0 */
+int gib_test_gather_rows(float* dst, const float* h, int ld, const int* src, const float* w, int scale, long long P,
+                         const int* live, gib_stream stream);
+/* g[b] = sum_i h[b*N + i] (MNN readout) and its backward dh[s] += dg[s / N] */
+int gib_test_sum_nodes_fwd(float* g, const float* h, int ld, int N, int B, gib_stream stream);
+int gib_test_bcast_nodes_add(float* dh, const float* dg, int ld, int N, long long S, gib_stream stream);
+/* dst[r] = [a[r, :wa] | b[r, :wb] | 0] over ldd columns; a / b int8 when a_i8 / b_i8 */
+int gib_test_concat2_in(float* dst, int ldd, const void* a, int lda, int wa, int a_i8, const void* b, int ldb, int wb,
+                        int b_i8, long long rows, gib_stream stream);
+/* dst[b] = [f1[b*N + 0, :fa] | ... | f1[b*N + N-1, :fa] | g[b, :W] | 0] over ldd columns */
+int gib_test_concat_flat(float* dst, int ldd, const float* f1, int ldf, int N, int fa, const float* g, int ldg, int W,
+                         int B, gib_stream stream);
+/* G[s, a] = dcat[s / N, (s % N)*fa + a] * selu'(f1[s, a]) for a < fa, 0 up to ldf */
+int gib_test_unflatten_dact(float* G, int ldf, const float* dcat, int ldd, const float* f1, int N, int fa, long long S,
+                            gib_stream stream);
+/* G[m, n] = dout[m, off + n] * act'(out[m, off + n]) for n < width, 0 up to ldg (act: the activation OUTPUT) */
+int gib_test_dact_slice(float* G, int ldg, const float* dout, const float* out, int ldo, int off, int width, int act,
+                        int rows, gib_stream stream);
+/* dst[r, c] = a[r, offa + c] + b2[r, offb + c] + c3[r, c] for c < W, 0 up to ldd; any operand may be NULL, c3 may be dst */
+int gib_test_sum3_cols(float* dst, int ldd, int W, const float* a, int lda, int offa, const float* b2, int ldb,
+                       int offb, const float* c3, int ldc, int rows, gib_stream stream);
+/* EMN elementwise kernels over rows x ld: y = tanh(x);  G = dy (1 - y^2) selu'(pre);  G = d selu'(y) */
+int gib_test_tanh_fwd(float* y, const float* x, long long rows, int ld, const int* live, gib_stream stream);
+int gib_test_tanh_selu_bwd(float* G, const float* dy, const float* y, const float* pre, long long rows, int ld,
+                           const int* live, gib_stream stream);
+int gib_test_mul_dselu(float* G, const float* d, const float* y, long long rows, int ld, const int* live,
+                       gib_stream stream);
+/* EMN input rows X[r] = [nodes[i, :F] | nodes[j, :F] | edges[i, j % N, :Ef] | 0], i = ent_dst[r], j = ent_src[r]
+ * (i < 0: zeros); nodes / edges int8 when i8 */
+int gib_test_emn_input(float* X, int ld, const void* nodes, const void* edges, int i8, const int* ent_dst,
+                       const int* ent_src, int N, int F, int Ef, long long P, gib_stream stream);
+/* host only: the plan's descriptor of Linear i -- out[GIB_PLAN_LINEAR_FIELDS] = {pw, pb, src_off, rs, cs, nblk, Rb, Rbp,
+ * C, Cp, Ct, Ctp, ow, owt, ob, ow_hi, ow_lo, owt_hi, owt_lo}: parameter indices (pb = -1: no bias), source offset and
+ * strides, extents, and the float offsets of Wp, WTp, bp and the TF32 planes in gib_model_pack's output.  Returns the
+ * number of Linears of the plan, < 0 when i is out of range or the dims are unsupported. */
+#define GIB_PLAN_LINEAR_FIELDS 19
+int gib_test_plan_linear(const gib_dims* d, int i, long long* out);
 
 /* ---- generation round post-processing (SURVEY §8f #1): softmax + categorical sample of one
  *      action per molecule from the APD logits, inverse-CDF on a caller-provided uniform. ---- */

@@ -71,6 +71,43 @@ def test_plan_matches_reference_parameter_schema(model, big):
     assert lib.gib_model_packed_bytes(ctypes.byref(d)) >= 4 * sum(math.prod(s) for _, s in shapes)
 
 
+@pytest.mark.parametrize("model", MODELS)
+@pytest.mark.parametrize("big", [False, True])
+def test_plan_linear_offsets_are_disjoint_and_inside_the_packed_arena(model, big):
+    """gib_test_plan_linear: every copy of every Linear (Wp, WTp, bp and the four TF32 planes) is its own range of
+    gib_model_pack's output; the planes start on 128-byte boundaries"""
+    from graphinvent_b200 import functional as Fn
+    from graphinvent_b200._lib import PLAN_LINEAR_FIELDS, lib
+    from graphinvent_b200.gnn import mpnn
+    from oracle import mpnn_oracle as O
+    kw = dict(hidden_node_features=128, message_size=128, message_passes=4, edge_emb_size=128,
+              max_n_nodes=38, n_node_features=12, len_f_add_per_node=81) if big else {}
+    d = Fn.make_dims(mpnn.create(O.make_constants(model, **kw)), 64)
+    total = lib.gib_model_packed_bytes(ctypes.byref(d)) // 4
+    nparams = lib.gib_model_num_params(ctypes.byref(d))
+    out = (ctypes.c_longlong * len(PLAN_LINEAR_FIELDS))()
+    n = lib.gib_test_plan_linear(ctypes.byref(d), 0, out)
+    assert n > 0
+    assert lib.gib_test_plan_linear(ctypes.byref(d), n, out) < 0 and lib.gib_test_plan_linear(ctypes.byref(d), -1, out) < 0
+    ranges = []
+    for i in range(n):
+        assert lib.gib_test_plan_linear(ctypes.byref(d), i, out) == n
+        f = dict(zip(PLAN_LINEAR_FIELDS, out))
+        assert 0 <= f["pw"] < nparams and -1 <= f["pb"] < nparams and f["pb"] != f["pw"]
+        Rp = f["nblk"] * f["Rbp"]
+        assert f["Rbp"] == (f["Rb"] + 15) // 16 * 16 and f["Cp"] == (f["C"] + 15) // 16 * 16
+        assert f["Ctp"] == (f["Ct"] + 15) // 16 * 16 and 0 <= f["Ct"] <= f["C"]
+        for name, size in (("ow", Rp * f["Cp"]), ("owt", f["Ctp"] * Rp), ("ob", Rp), ("ow_hi", Rp * f["Cp"]),
+                           ("ow_lo", Rp * f["Cp"]), ("owt_hi", f["Ctp"] * Rp), ("owt_lo", f["Ctp"] * Rp)):
+            if name.endswith(("_hi", "_lo")):
+                assert f[name] % 32 == 0, (i, name)
+            ranges.append((f[name], f[name] + size, i, name))
+    ranges.sort()
+    assert ranges[0][0] >= 0 and ranges[-1][1] <= total
+    for a, b in zip(ranges, ranges[1:]):
+        assert a[1] <= b[0], f"{a[2:]} overlaps {b[2:]}"
+
+
 def test_workspace_queries_scale_with_the_graph_header():
     from graphinvent_b200 import functional as Fn
     from graphinvent_b200._lib import lib

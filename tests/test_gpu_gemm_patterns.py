@@ -276,12 +276,15 @@ def _epilogues(N):
             ("generic", dict(mode=EPI_ACT, act=1, n_store=N + 8, n_valid=N - 3, ldc=N + 21, lda_pad=16))]
 
 
-@pytest.mark.parametrize("M", [1, 127, 128, 129, 4097])
-@pytest.mark.parametrize("N", [48, 64, 65, 256, 608])
+@pytest.mark.parametrize("M", [1, 64, 65, 127, 128, 129, 4097])
+@pytest.mark.parametrize("N", [48, 64, 65, 128, 129, 200, 256, 608])
 def test_nt_shapes_and_epilogues(M, N):
     """every epilogue at every shape: the dispatcher's own choice, the tensor-core kernel forced through a device-side
-    row count (any M), and tensor cores off"""
-    for K in (16, 48, 144, 688):
+    row count (any M), and tensor cores off.  The wgmma tile is 128 x 128, split between two 64-row consumer
+    warpgroups: M = 64 / 65 fill one warpgroup / spill one row into the second, N = 129 / 200 leave one / 72 live
+    columns in a second column tile; K = 32 and 160 end on a full k-block (K = 160: five k-blocks, one more than the
+    ring has stages), the other K on a half-empty one"""
+    for K in (16, 32, 48, 144, 160, 688):
         for label, kw in _epilogues(N):
             kw = dict(kw)
             lda = K + kw.pop("lda_pad", 0)
@@ -390,7 +393,9 @@ def _chain(M, widths, members, mode, cap=None, base=0, seed=0, last_linear=False
                 kw.update(cap=cap, base=base)
             if ins[i] is not None:
                 kw["A"] = ins[i].C
-            t = NT(M, widths[l], widths[l - 1], **kw)
+            # widths that are not a multiple of 16 are stored with +0 pad columns up to the next one, which the
+            # layer above reads as its K (the model's padded layout)
+            t = NT(M, widths[l], pad16(widths[l - 1]), n_store=pad16(widths[l]), n_valid=widths[l], **kw)
             t.C.fill_(7.0)
             t.C0 = t.C.clone()
             t.m_dev, t.base_dev = rows
@@ -409,6 +414,7 @@ def _chain_cases():
         "4x2 dX chain": dict(M=2000, widths=[96, 128, 48, 64, 256], members=2, mode=EPI_MUL_DACT),
         "3x2 device rows": dict(M=2500, widths=[64, 128, 256, 48], members=2, mode=EPI_ACT, cap=4096, base=384),
         "2x3 device rows dX": dict(M=1111, widths=[48, 112, 64], members=3, mode=EPI_MUL_DACT, cap=2048, base=640),
+        "3x2 partial column tile": dict(M=3000, widths=[96, 200, 256, 200], members=2, mode=EPI_ACT),
         "3x1 device rows clamped": dict(M=1000, widths=[64, 64, 64, 64], members=1, mode=EPI_ACT, cap=4096,
                                         base=3968),
         "2x2 live count 0": dict(M=0, widths=[64, 96, 48], members=2, mode=EPI_ACT, cap=1024, base=0),
