@@ -33,3 +33,24 @@ def make_constants(model="GGNN", **overrides):
 
 def apd_length(C):
     return C.max_n_nodes * (C.len_f_add_per_node + C.len_f_conn_per_node) + 1
+
+
+def layout_dims(n_atom_types, n_formal_charge, n_edge_features=3, use_explicit_H=False, ignore_H=True,
+                use_chirality=False, n_imp_H_values=4, n_chirality_values=3):
+    """Derived node-feature and action dims of one of the reference's four action layouts, restated from
+    `parameters/constants.py:23-95, 169-184` (`n_imp_H_values` = len(imp_H), `n_chirality_values` = len(chirality)):
+    implicit-H counts form a node-feature segment only when H is neither explicit nor ignored, chirality when
+    `use_chirality` is set.  Pass the result to `make_constants` to build a model of the right shape."""
+    if use_explicit_H and ignore_H:
+        raise ValueError("use_explicit_H and ignore_H cannot both be set (the reference refuses the same flags)")
+    implicit_H = not use_explicit_H and not ignore_H
+    n_imp_H = int(implicit_H) * n_imp_H_values
+    n_chirality = int(use_chirality) * n_chirality_values
+    dim_f_add = [n_atom_types, n_formal_charge] + [n_imp_H] * implicit_H + [n_chirality] * use_chirality
+    len_f_add = n_edge_features
+    for n in dim_f_add:
+        len_f_add *= n
+    return dict(n_node_features=n_atom_types + n_formal_charge + n_imp_H + n_chirality,
+                n_edge_features=n_edge_features, len_f_add_per_node=len_f_add,
+                len_f_conn_per_node=n_edge_features,
+                n_atom_types=n_atom_types, n_formal_charge=n_formal_charge, n_imp_H=n_imp_H, n_chirality=n_chirality)

@@ -147,8 +147,9 @@ using namespace gib;
 extern "C" {
 
 const char* gib_last_error(void) { return g_err; }
-// 200: capacity mode, int8 inputs, grouped dW; 201: 5 profile classes; 202: test hooks; 203: forward / glue test hooks
-int gib_version(void) { return 203; }
+// 200: capacity mode, int8 inputs, grouped dW; 201: 5 profile classes; 202: test hooks; 203: forward / glue test hooks;
+// 204: gib_generation_round_layout (implicit-H / chirality action layouts)
+int gib_version(void) { return 204; }
 void gib_set_tensor_cores(int on) { g_use_tc = on != 0; }
 int gib_get_tensor_cores(void) { return g_use_tc ? 1 : 0; }
 void gib_tc_debug(int mode) { g_tc_debug = mode; }

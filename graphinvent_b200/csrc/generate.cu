@@ -6,10 +6,19 @@
 //   GraphGenerator.apply_actions                      (:211-338)
 //   GraphGenerator.reset_graphs                       (:425-465)
 // with three launches.  Semantics are the reference's, quirks included (they are observable in its outputs):
-//   * the flat APD index decodes row-major as f_add[bond_to, atom, charge, bond_type] | f_conn[bond_to, bond_type] | term
-//     (6-tuple layout only: no implicit-H / chirality segment -- the layout of every shipped configuration, and the only
-//     one for which the reference's own "max nodes" test `f_add_idc[5]` looks at bond_from);
+//   * the flat APD index decodes row-major as
+//       f_add[bond_to, atom, charge, (imp_h,) (chirality,) bond_type] | f_conn[bond_to, bond_type] | term
+//     where the implicit-H and chirality segments are present when their count (H, C) is > 0 (constants.py:23-95:
+//     L0 = neither, the layout of the shipped gdb13 data; L1 = implicit H; L2 = chirality; L3 = both).  An add sets one
+//     node feature per segment: atom, A + charge, A + CH + imp_h, A + CH + H + chirality;
 //   * bond_from = n_nodes for add, n_nodes - 1 for connect (-1 wraps to the last atom, as Python indexing does);
+//   * element 5 of the reference's add tuple (`f_add_idc[5]`, GraphGenerator.py:568, 618) is bond_from only in L0; it is
+//     bond_type in L1 / L2 and chirality in L3.  Its "max nodes" rule (element 5 >= max_n_nodes -> invalid) and its
+//     reset (element 5 = 0 for such adds and for every add into an empty graph) are applied to that element as the
+//     reference applies them: in L3 the chirality of every molecule's first atom is stored as index 0;
+//   * deliberate deviation: outside L0 the reference has no result for an add into a graph that already holds
+//     max_n_nodes atoms (it indexes nodes[b, N] and raises IndexError).  Here such a slot terminates as invalid, with
+//     bond_from = 0, in every layout -- which is the reference's own L0 outcome;
 //   * a slot terminates when it samples terminate or an invalid action; slot 0 (the dummy graph) never does, is never
 //     zeroed, and is re-stamped every round (so bonds it samples accumulate);
 //   * terminated graphs are copied out in their PRE-action state, terminate-sampled slots first (ascending), then
@@ -20,7 +29,8 @@
 
 namespace gib {
 
-struct GenDims { int B, N, F, Ef, A, CH, Lw; };   // Lw = likelihood columns (2 * max_n_nodes)
+// H / C = implicit-H / chirality index counts, 0 = segment absent; Lw = likelihood columns (2 * max_n_nodes)
+struct GenDims { int B, N, F, Ef, A, CH, H, C, Lw; };
 
 enum : int { ACT_ADD = 0, ACT_CONN = 1, ACT_TERM = 2 };
 
@@ -31,8 +41,8 @@ __global__ void gen_decode_kernel(GenDims d, const int* __restrict__ action, con
   if (b >= d.B) return;
   const int a = action[b];
   const int n = n_nodes[b];
-  const int len_add = d.N * d.A * d.CH * d.Ef, len_conn = d.N * d.Ef;
-  int kind, bond_to = 0, atom = 0, charge = 0, btype = 0, bond_from = 0, invalid = 0;
+  const int len_add = d.N * d.A * d.CH * max(d.H, 1) * max(d.C, 1) * d.Ef, len_conn = d.N * d.Ef;
+  int kind, bond_to = 0, atom = 0, charge = 0, imp_h = 0, chir = 0, btype = 0, bond_from = 0, invalid = 0;
   if (a < 0 || a > len_add + len_conn) {
     // not an APD index (a corrupted replay trace, or the sampler's NaN fallback): an invalid action that edits
     // nothing -- the slot terminates as "invalid" and is reset, no field of `rec` is out of range
@@ -40,16 +50,30 @@ __global__ void gen_decode_kernel(GenDims d, const int* __restrict__ action, con
     invalid = 1;
   } else if (a < len_add) {
     kind = ACT_ADD;
-    btype = a % d.Ef;
-    charge = (a / d.Ef) % d.CH;
-    atom = (a / (d.Ef * d.CH)) % d.A;
-    bond_to = a / (d.Ef * d.CH * d.A);
+    int r = a;
+    btype = r % d.Ef;
+    r /= d.Ef;
+    if (d.C) { chir = r % d.C; r /= d.C; }
+    if (d.H) { imp_h = r % d.H; r /= d.H; }
+    charge = r % d.CH;
+    r /= d.CH;
+    atom = r % d.A;
+    bond_to = r / d.A;
     bond_from = n;
     const bool empty = n == 0;
     if (!empty && bond_to >= n) invalid = 1;          // bond to a non-existing atom          (:600-604)
     if (empty && bond_to != 0) invalid = 1;           // first atom must use slot 0           (:606-610)
-    if (bond_from >= d.N) invalid = 1;                // graph already holds max_n_nodes atoms (:613)
-    if (bond_from >= d.N || empty) bond_from = 0;     // get_actions: f_add_idc[5][max_node_idc] = 0   (:568)
+    // f_add_idc[5]: bond_from (L0), bond_type (L1, L2) or chirality (L3)
+    const int e5_sel = (d.H == 0 && d.C == 0) ? 0 : (d.H && d.C) ? 2 : 1;
+    const int e5 = e5_sel == 0 ? bond_from : e5_sel == 2 ? chir : btype;
+    const bool madd = e5 >= d.N;
+    if (madd) invalid = 1;                            // "graph already holds max_n_nodes atoms" (:618)
+    if (madd || empty) {                              // get_actions: f_add_idc[5][max_node_idc] = 0   (:568)
+      if (e5_sel == 0) bond_from = 0;
+      else if (e5_sel == 2) chir = 0;
+      else btype = 0;
+    }
+    if (n >= d.N) { invalid = 1; bond_from = 0; }     // full graph: the L0 outcome in every layout (see above)
   } else if (a < len_add + len_conn) {
     kind = ACT_CONN;
     const int c = a - len_add;
@@ -68,7 +92,8 @@ __global__ void gen_decode_kernel(GenDims d, const int* __restrict__ action, con
   } else {
     kind = ACT_TERM;
   }
-  rec[b] = make_int4(kind | (invalid << 4), bond_to | (bond_from << 8), atom | (charge << 8), btype);
+  rec[b] = make_int4(kind | (invalid << 4), bond_to | (bond_from << 8), atom | (charge << 8),
+                     btype | (imp_h << 8) | (chir << 16));
   flags[b] = (kind == ACT_TERM ? 1 : 0) | (invalid ? 2 : 0);
 }
 
@@ -153,10 +178,12 @@ __global__ void __launch_bounds__(128) gen_apply_kernel(GenDims d, int round, co
     return;
   }
   if (threadIdx.x == 0) {
-    const int bond_to = r.y & 255, bond_from = r.y >> 8, atom = r.z & 255, charge = r.z >> 8, bt = r.w;
-    if (kind == ACT_ADD) {                                            // apply_actions._add_nodes :289-306
+    const int bond_to = r.y & 255, bond_from = r.y >> 8, atom = r.z & 255, charge = r.z >> 8, bt = r.w & 255;
+    if (kind == ACT_ADD) {                                            // apply_actions._add_nodes :257-306
       nb[bond_from * d.F + atom] = 1.f;
       nb[bond_from * d.F + d.A + charge] = 1.f;
+      if (d.H) nb[bond_from * d.F + d.A + d.CH + ((r.w >> 8) & 255)] = 1.f;
+      if (d.C) nb[bond_from * d.F + d.A + d.CH + d.H + (r.w >> 16)] = 1.f;
       if (n_nodes[b] != 0) {
         eb[(bond_to * d.N + bond_from) * d.Ef + bt] = 1.f;
         eb[(bond_from * d.N + bond_to) * d.Ef + bt] = 1.f;
@@ -180,19 +207,31 @@ __global__ void __launch_bounds__(128) gen_apply_kernel(GenDims d, int round, co
 
 using namespace gib;
 
-extern "C" int gib_generation_round(int B, int N, int F, int Ef, int n_atom_types, int n_charges, int round,
-                                    const int* action, const float* likelihood, float* nodes, float* edges,
-                                    int* n_nodes, float* likelihoods, float* gen_nodes, float* gen_edges,
-                                    signed char* gen_n_nodes, float* gen_likelihoods,
-                                    signed char* properly_terminated, int capacity, int* counters, void* scratch,
-                                    gib_stream stream) {
-  if (B <= 0 || N <= 0 || N > 127 || n_atom_types + n_charges != F || round < 0 || round >= 2 * N) {
-    set_error("gib_generation_round: unsupported arguments (B=%d N=%d F=%d round=%d; likelihood buffer holds 2N rounds)",
-              B, N, F, round);
+extern "C" int gib_generation_round_layout(int B, int N, int F, int Ef, int n_atom_types, int n_charges, int n_imp_H,
+                                           int n_chirality, int round, const int* action, const float* likelihood,
+                                           float* nodes, float* edges, int* n_nodes, float* likelihoods,
+                                           float* gen_nodes, float* gen_edges, signed char* gen_n_nodes,
+                                           float* gen_likelihoods, signed char* properly_terminated, int capacity,
+                                           int* counters, void* scratch, gib_stream stream) {
+  // every index travels in 8 bits of the int4 record; counts <= 255 keep each index <= 254
+  const bool counts_ok = n_atom_types > 0 && n_charges > 0 && Ef > 0 && n_imp_H >= 0 && n_chirality >= 0 &&
+                         n_atom_types <= 255 && n_charges <= 255 && Ef <= 255 && n_imp_H <= 255 && n_chirality <= 255;
+  if (!counts_ok) {
+    set_error("gib_generation_round: index counts must lie in 1..255 (0..255 for implicit H / chirality): "
+              "A=%d CH=%d H=%d C=%d Ef=%d", n_atom_types, n_charges, n_imp_H, n_chirality, Ef);
+    return -1;
+  }
+  const long long len_add = (long long)N * n_atom_types * n_charges * (n_imp_H ? n_imp_H : 1) *
+                            (n_chirality ? n_chirality : 1) * Ef;
+  if (B <= 0 || N <= 0 || N > 127 || n_atom_types + n_charges + n_imp_H + n_chirality != F || round < 0 ||
+      round >= 2 * N || len_add + (long long)N * Ef >= (1ll << 31)) {
+    set_error("gib_generation_round: unsupported arguments (B=%d N=%d F=%d A=%d CH=%d H=%d C=%d round=%d; F must be "
+              "A + CH + H + C, and the likelihood buffer holds 2N rounds)",
+              B, N, F, n_atom_types, n_charges, n_imp_H, n_chirality, round);
     return -1;
   }
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  GenDims d{B, N, F, Ef, n_atom_types, n_charges, 2 * N};
+  GenDims d{B, N, F, Ef, n_atom_types, n_charges, n_imp_H, n_chirality, 2 * N};
   int4* rec = reinterpret_cast<int4*>(scratch);
   int* flags = reinterpret_cast<int*>(rec + B);
   int* pos = flags + B;
@@ -204,6 +243,17 @@ extern "C" int gib_generation_round(int B, int N, int F, int Ef, int n_atom_type
                                       gen_edges, gen_n_nodes, gen_likelihoods);
   GIB_LAUNCH_CHECK();
   return 0;
+}
+
+extern "C" int gib_generation_round(int B, int N, int F, int Ef, int n_atom_types, int n_charges, int round,
+                                    const int* action, const float* likelihood, float* nodes, float* edges,
+                                    int* n_nodes, float* likelihoods, float* gen_nodes, float* gen_edges,
+                                    signed char* gen_n_nodes, float* gen_likelihoods,
+                                    signed char* properly_terminated, int capacity, int* counters, void* scratch,
+                                    gib_stream stream) {
+  return gib_generation_round_layout(B, N, F, Ef, n_atom_types, n_charges, 0, 0, round, action, likelihood, nodes,
+                                     edges, n_nodes, likelihoods, gen_nodes, gen_edges, gen_n_nodes, gen_likelihoods,
+                                     properly_terminated, capacity, counters, scratch, stream);
 }
 
 extern "C" size_t gib_generation_scratch_bytes(int B) { return (size_t)B * (sizeof(int4) + 2 * sizeof(int)) + 64; }

@@ -2,10 +2,18 @@
 Batched graph generation with the round post-processing on the device (SURVEY.md §8f rank 1).
 
 Mirror of the reference's `GraphGenerator` (GraphGenerator.py:25-161) for the part that is tensor work:
-`build_graphs()` runs model forward -> softmax/sample -> ONE `gib_generation_round` call per round (decode, validity
+`build_graphs()` runs model forward -> softmax/sample -> ONE `gib_generation_round(_layout)` call per round (decode, validity
 rules, copy-out, apply, reset; the reference issues ~800 ATen ops for the same) until `batch_size` molecules are
 finished; `sample()` returns the finished tensors and likelihood summaries.  Converting tensors to RDKit molecules
 (`graph_to_graph`, GraphGenerator.py:659-804) stays the reference's job -- feed it `generated_nodes/edges/n_nodes`.
+
+All four of the reference's action layouts are supported (parameters/constants.py:23-95): node features atom type +
+formal charge, plus an implicit-H segment (`n_imp_H` > 0) and / or a chirality segment (`n_chirality` > 0), with the
+add actions laid out as [bond_to, atom, charge, (imp_h,) (chirality,) bond_type].  `config.layout_dims` derives the
+dims of a layout from the reference's flags.  The reference's quirks are kept in every layout (graphinvent_b200/csrc/
+generate.cu lists them): with both segments present the first atom of every molecule gets chirality index 0.  An add
+into a graph that already holds max_n_nodes atoms terminates the molecule as invalid in every layout; outside the
+gdb13 layout the reference raises IndexError there instead.
 
 The sampler draws with inverse-CDF on `torch.rand` uniforms (same distribution as `Multinomial(1, probs)`, different
 RNG stream); `build_graphs(replay=...)` replays recorded draws instead, which is how the parity tests pin the state
@@ -29,15 +37,24 @@ def _ptr(t):
 
 
 class GraphGenerator:
-    def __init__(self, model, batch_size, constants=None, n_atom_types=None, n_formal_charge=None, device="cuda"):
+    def __init__(self, model, batch_size, constants=None, n_atom_types=None, n_formal_charge=None, n_imp_H=None,
+                 n_chirality=None, device="cuda"):
         C = constants if constants is not None else model.constants
         self.model, self.batch_size, self.device = model, int(batch_size), torch.device(device)
         self.N, self.F, self.Ef = C.max_n_nodes, C.n_node_features, C.n_edge_features
         self.A = n_atom_types if n_atom_types is not None else getattr(C, "n_atom_types")
         self.CH = n_formal_charge if n_formal_charge is not None else getattr(C, "n_formal_charge")
-        if self.A + self.CH != self.F or self.A * self.CH * self.Ef != C.len_f_add_per_node:
-            raise NotImplementedError("only the 6-tuple action layout (atom type + formal charge node features, no "
-                                      "implicit-H / chirality segment) is supported, as in every shipped configuration")
+        self.n_imp_H = n_imp_H if n_imp_H is not None else getattr(C, "n_imp_H", 0)
+        self.n_chirality = n_chirality if n_chirality is not None else getattr(C, "n_chirality", 0)
+        counts = (self.A, self.CH, self.n_imp_H, self.n_chirality)
+        len_f_add = self.A * self.CH * max(self.n_imp_H, 1) * max(self.n_chirality, 1) * self.Ef
+        if (min(self.A, self.CH) < 1 or min(self.n_imp_H, self.n_chirality) < 0 or max(counts) > 255
+                or sum(counts) != self.F or len_f_add != C.len_f_add_per_node):
+            raise ValueError(
+                f"inconsistent action layout: n_atom_types={self.A}, n_formal_charge={self.CH}, n_imp_H={self.n_imp_H}, "
+                f"n_chirality={self.n_chirality} (each <= 255; 0 = segment absent) need n_node_features = {sum(counts)} "
+                f"and len_f_add_per_node = {len_f_add}, the constants have {self.F} and {C.len_f_add_per_node} "
+                "(graphinvent_b200.config.layout_dims derives them from the reference's flags)")
         self.apd = self.N * (C.len_f_add_per_node + C.len_f_conn_per_node) + 1
         self.rounds = 0
         self._allocate()
@@ -60,6 +77,20 @@ class GraphGenerator:
         self.properly_terminated = z(cap, dt=torch.int8)
         self._counters = z(2, dt=torch.int32)
         self._scratch = torch.empty(lib.gib_generation_scratch_bytes(B), dtype=torch.uint8, device=dev)
+
+    def _round(self, rnd, action, lik, stream):
+        """one round of the device state machine; the gdb13 layout goes through `gib_generation_round`"""
+        state = (_ptr(action), _ptr(lik), _ptr(self.nodes), _ptr(self.edges), _ptr(self.n_nodes), _ptr(self.likelihoods),
+                 _ptr(self.generated_nodes), _ptr(self.generated_edges), _ptr(self.generated_n_nodes),
+                 _ptr(self.generated_likelihoods), _ptr(self.properly_terminated), self.capacity, _ptr(self._counters),
+                 _ptr(self._scratch), stream)
+        if self.n_imp_H == 0 and self.n_chirality == 0:
+            check(lib.gib_generation_round(self.batch_size, self.N, self.F, self.Ef, self.A, self.CH, rnd, *state),
+                  "gib_generation_round")
+        else:
+            check(lib.gib_generation_round_layout(self.batch_size, self.N, self.F, self.Ef, self.A, self.CH,
+                                                  self.n_imp_H, self.n_chirality, rnd, *state),
+                  "gib_generation_round_layout")
 
     def _model_inputs(self, model):
         """(nodes, edges) to evaluate `model` on.  The dummy graph in slot 0 is never reset (GraphGenerator.py:461-465
@@ -101,13 +132,7 @@ class GraphGenerator:
             else:
                 out = self.model(*self._model_inputs(self.model))    # GraphGenerator.py:121
                 action, lik = Fn.sample_actions(out, generator=generator)
-            check(lib.gib_generation_round(B, self.N, self.F, self.Ef, self.A, self.CH, rnd, _ptr(action), _ptr(lik),
-                                           _ptr(self.nodes), _ptr(self.edges), _ptr(self.n_nodes),
-                                           _ptr(self.likelihoods), _ptr(self.generated_nodes),
-                                           _ptr(self.generated_edges), _ptr(self.generated_n_nodes),
-                                           _ptr(self.generated_likelihoods), _ptr(self.properly_terminated),
-                                           self.capacity, _ptr(self._counters), _ptr(self._scratch), st),
-                  "gib_generation_round")
+            self._round(rnd, action, lik, st)
             n_generated = int(self._counters[0].item())           # the loop condition lives on the host (:118)
             rnd += 1
         self.rounds = rnd
@@ -181,13 +206,7 @@ class GraphGeneratorRL(GraphGenerator):
             idx = action.long().unsqueeze(1)
             lik_a.append(torch.softmax(out_a, dim=1).gather(1, idx).squeeze(1))       # `apds[apd_one_hot == 1]` :547-548
             lik_p.append(torch.softmax(out_p, dim=1).gather(1, idx).squeeze(1))
-            check(lib.gib_generation_round(B, N, self.F, self.Ef, self.A, self.CH, rnd, _ptr(action), _ptr(tags),
-                                           _ptr(self.nodes), _ptr(self.edges), _ptr(self.n_nodes),
-                                           _ptr(self.likelihoods), _ptr(self.generated_nodes),
-                                           _ptr(self.generated_edges), _ptr(self.generated_n_nodes),
-                                           _ptr(self.generated_likelihoods), _ptr(self.properly_terminated),
-                                           self.capacity, _ptr(self._counters), _ptr(self._scratch), st),
-                  "gib_generation_round")
+            self._round(rnd, action, tags, st)
             n_generated = int(self._counters[0].item())
             rnd += 1
         self.rounds = rnd

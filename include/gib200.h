@@ -327,7 +327,13 @@ int gib_sample_actions(const float* out, int B, int apd, const float* uniforms, 
  *      index per slot, validity rules, copy terminated graphs out (pre-action state; terminate-sampled first, then
  *      invalid, ascending), apply add / connect, reset, re-stamp the dummy graph in slot 0.  Replaces
  *      GraphGenerator.get_actions / get_invalid_actions / copy_terminated_graphs / apply_actions / reset_graphs
- *      (GraphGenerator.py:467-657, 340-385, 211-338, 425-465).  6-tuple action layout (no implicit-H / chirality).
+ *      (GraphGenerator.py:467-657, 340-385, 211-338, 425-465).
+ *      Action layout: f_add[bond_to, atom, charge, (imp_h,) (chirality,) bond_type] | f_conn[bond_to, bond_type] |
+ *      term, node features atom type + formal charge (+ implicit H) (+ chirality); n_imp_H / n_chirality = 0 means
+ *      the segment is absent, so F must equal n_atom_types + n_charges + n_imp_H + n_chirality.  Every index count is
+ *      <= 255.  The reference's `f_add_idc[5]` quirk is kept in every layout (its chirality reset makes the first
+ *      atom's chirality index 0 when both segments are present); an add into a full graph terminates as invalid.
+ *      gib_generation_round is this entry point with n_imp_H = n_chirality = 0 (the gdb13 layout).
  *      State: nodes [B,N,F] f32, edges [B,N,N,Ef] f32, n_nodes [B] i32, likelihoods [B,2N] f32; outputs
  *      gen_* with `capacity` rows; counters[0] = n_generated (in/out), counters[1] = graphs written this round. ---- */
 size_t gib_generation_scratch_bytes(int B);
@@ -336,6 +342,12 @@ int gib_generation_round(int B, int N, int F, int Ef, int n_atom_types, int n_ch
                          float* likelihoods, float* gen_nodes, float* gen_edges, signed char* gen_n_nodes,
                          float* gen_likelihoods, signed char* properly_terminated, int capacity, int* counters,
                          void* scratch, gib_stream stream);
+int gib_generation_round_layout(int B, int N, int F, int Ef, int n_atom_types, int n_charges, int n_imp_H,
+                                int n_chirality, int round, const int* action, const float* likelihood,
+                                float* nodes, float* edges, int* n_nodes, float* likelihoods, float* gen_nodes,
+                                float* gen_edges, signed char* gen_n_nodes, float* gen_likelihoods,
+                                signed char* properly_terminated, int capacity, int* counters, void* scratch,
+                                gib_stream stream);
 
 /* ---- measurement hooks: CUDA-event timing per kernel class on the launching stream.
  *      class 0 = forward/dX launches of the tensor-core kernel, 1 = its weight-gradient launches, 2 = scatter-aggregate (K2),
