@@ -10,7 +10,7 @@
 // is ~2^-22 relative).  The cross terms, 2^-11 of the main ones, get their own accumulator so that their roundings stay
 // away from the large running sum; the two are added in fp32 in the epilogue.
 //
-// Both kernels are persistent (one CTA per SM, work items = output tiles of up to 16 problems, or (tile, reduction
+// The kernels are persistent (one CTA per SM, work items = output tiles of up to 16 problems, or (tile, reduction
 // chunk) pairs in TN mode) and fed by one TMA lane through a ring of shared-memory stages (cp.async.bulk.tensor with
 // the 128-byte swizzle, mbarrier expect_tx per stage).
 //
@@ -24,15 +24,24 @@
 //                                  memory through descriptors) into two fp32 register accumulators, one wgmma group.
 //                                  The A fragments of the next half are prepared while the group of this one runs; a
 //                                  stage is handed back to the producer once the last group that reads it has retired
-// tc3_gemm_kernel: TN (weight gradients) and NT with raw fp32 W.  288 threads, 6-stage ring of 32 KB stages,
-// 128 x 64 output tiles:
-//   warp 8      TMA producer   NT: raw A tile [128 x 32 fp32] + raw W tile [64 x 32]; TN: G and X as
-//                              [32 rows x 32 floats] boxes
+// tc3_wgmma_dw_kernel: TN (weight gradients).  384 threads, 128 (Nn) x 128 (Kk) output tiles.  Both operands are
+// MN-major (row-major activations, reduced over rows) and TF32 wgmma reads shared-memory operands K-major only, so X
+// is transposed in shared memory:
+//   warpgroup 2     warp 8, one lane: TMA of G and X as [32 rows x 32 floats] boxes (4 + 4 per k-block of 32 rows)
+//                   into a 4-stage ring of 32 KB raw stages;
+//                   warps 9-11: transpose X into X_hi^T / X_lo^T [128 x 32] K-major tiles with the 128-byte swizzle
+//                   (the layout TMA gives the W planes above) in a 3-stage ring of 32 KB plane stages, split with the
+//                   same round-to-nearest, reduction rows past the chunk / row count written as 0
+//   warpgroups 0-1  consumers      64 x 128 outputs each: G^T fragments read in transposed order from the raw boxes and
+//                                  split in registers (the bias-gradient partials are summed from them), X planes
+//                                  through descriptors; the same half-k-block wgmma pipeline as tc3_wgmma_kernel
+// tc3_gemm_kernel: NT with raw fp32 W.  288 threads, 6-stage ring of 24 KB stages, 128 x 64 output tiles:
+//   warp 8      TMA producer   raw A tile [128 x 32 fp32] + raw W tile [64 x 32]
 //   warps 0-7   consumers      4 (M) x 2 (N) warps, 32 x 32 outputs each: fragments straight from the swizzled tiles
 //                              (conflict-free for K-major operands), split into (hi, lo) in registers,
 //                              mma.sync.m16n8k8 TF32 into two fp32 register accumulators, one mbarrier arrival per warp
 //                              frees the stage
-// Both end in the same epilogue from registers: bias / SELU / dSELU / residual and the stores.
+// All three end in the same epilogue from registers: bias / SELU / dSELU / residual and the stores.
 //
 // Dynamic row counts: a problem may name device ints (m_dev, base_dev) -- the bond-type group sizes written by K0 --
 // instead of host values; tile counts are then computed on the device, so the launch needs no device->host read
@@ -63,7 +72,7 @@ constexpr int CONS_WARPS = 8;                     // consumer warps of both kern
 constexpr int BN = 64;
 constexpr int STAGES = 6;
 constexpr int B_BYTES = BN * BKF * 4;             // 8 KB
-constexpr int STAGE_BYTES = A_BYTES + B_BYTES;   // NT: A raw | W raw      TN: G raw | X raw
+constexpr int STAGE_BYTES = A_BYTES + B_BYTES;   // A raw | W raw
 constexpr int NUM_THREADS = 32 * CONS_WARPS + 32;   // 288
 constexpr int WM = 32, WN = 32;                   // warp tile
 constexpr int MI = WM / 16, NI = WN / 8;          // m16n8k8 MMAs per warp tile and k-step
@@ -85,6 +94,22 @@ constexpr int WG_OFF_SCHED = WG_OFF_BARS + 256;
 constexpr int WG_SMEM_BYTES = WG_OFF_SCHED + 512 + 1024 /*align slack*/;
 static_assert(WG_SMEM_BYTES <= 227 * 1024, "wgmma stages exceed the shared memory of an SM");
 
+// tc3_wgmma_dw_kernel: 384 threads, registers 256 consumer threads x 224 + 128 producer / transpose threads x 56 =
+// 64512 (the transpose holds a 4 x 4 block and its split: ptxas spills it at 48).  Per k-block of 32 reduction rows the raw stage holds
+// G [32 x 128 columns] and X [32 x 128 columns] as 4 + 4 boxes of [32 rows x 32 floats]; the plane stage holds
+// X_hi^T | X_lo^T [128 x 32], K-major.
+constexpr int DW_BN = 128;
+constexpr int DW_RAW_STAGES = 4;
+constexpr int DW_RAW_BYTES = 2 * A_BYTES;                      // 32 KB: G boxes | X boxes
+constexpr int DW_PLANE_STAGES = 3;
+constexpr int DW_PLANE_BYTES = 2 * DW_BN * BKF * 4;           // 32 KB: X_hi^T | X_lo^T
+constexpr int DW_TR_WARPS = 3;                                 // warps 9-11
+constexpr int DW_OFF_PLANES = DW_RAW_STAGES * DW_RAW_BYTES;
+constexpr int DW_OFF_BARS = DW_OFF_PLANES + DW_PLANE_STAGES * DW_PLANE_BYTES;
+constexpr int DW_OFF_SCHED = DW_OFF_BARS + 256;
+constexpr int DW_SMEM_BYTES = DW_OFF_SCHED + 512 + 1024 /*align slack*/;
+static_assert(DW_SMEM_BYTES <= 227 * 1024, "weight-gradient stages exceed the shared memory of an SM");
+
 constexpr int kMaxChunkRows = 4096;   // reduction rows per work item of the weight-gradient mode
 constexpr int MAXP = kTc3MaxProblems;   // 16: e.g. the 5 layers x 3 bond types of a message MLP as one dependent chain
 
@@ -97,7 +122,7 @@ struct Maps {   // TMA descriptors in kernel-parameter space
 struct Params {
   GemmNT g[MAXP];           // TN: A = G, B = X, M = rows (capacity when m_dev is set), C = partials of the problem,
                             //     ldc = Kk, N = n_store = n_valid = Kk
-  int n_tiles[MAXP];        // column tiles of the output (NT: ceil(N / tile width), TN: ceil(Kk / BN))
+  int n_tiles[MAXP];        // column tiles of the output (NT: ceil(N / tile width), TN: ceil(Kk / DW_BN))
   int k_blocks[MAXP];       // NT: ceil(K / 32)
   int tn_mt[MAXP];          // TN: ceil(Nn / 128)
   int tn_nn[MAXP];          // TN: Nn
@@ -317,8 +342,8 @@ __device__ __forceinline__ void epi_store(const EpiArgs& e, int m, int n, float 
   }
 }
 
-// ---- mma.sync kernel: TN (weight gradients) and NT with raw fp32 W ----
-template <bool TN, int EPI>
+// ---- mma.sync kernel: NT with raw fp32 W ----
+template <int EPI>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 tc3_gemm_kernel(const __grid_constant__ Maps maps, const Params P) {
   extern __shared__ uint8_t smem_raw[];
@@ -336,7 +361,7 @@ tc3_gemm_kernel(const __grid_constant__ Maps maps, const Params P) {
       mbar_init(&empty[s], CONS_WARPS);     // one arrival per consumer warp (after __syncwarp)
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    init_sched<TN>(P, S);
+    init_sched<false>(P, S);
   }
   __syncthreads();
   const int num_items = S.begin[MAXP];
@@ -347,28 +372,15 @@ tc3_gemm_kernel(const __grid_constant__ Maps maps, const Params P) {
       int stage = 0;
       uint32_t phase = 0;
       for (int item = blockIdx.x; item < num_items; item += gridDim.x) {
-        const Item w = decode_item<TN, BN>(P, S, item);
-        const CUtensorMap* map_a = &maps.a[w.p];
-        const CUtensorMap* map_b = &maps.b[w.p];
+        const Item w = decode_item<false, BN>(P, S, item);
         const int base = S.base[w.p];
-        if constexpr (!TN)
-          if (P.flags && P.dep[w.p] >= 0) wait_rows(P, w);
+        if (P.flags && P.dep[w.p] >= 0) wait_rows(P, w);
         for (int kb = 0; kb < w.nkb; ++kb) {
           mbar_wait(&empty[stage], phase ^ 1);
           uint8_t* st = smem + stage * STAGE_BYTES;
           mbar_arrive_expect_tx(&full[stage], A_BYTES + B_BYTES);
-          if constexpr (!TN) {
-            tma_load_2d(map_a, &full[stage], st, kb * BKF, base + w.m0);
-            tma_load_2d(map_b, &full[stage], st + A_BYTES, kb * BKF, w.n0);
-          } else {
-            const int row = base + w.r0 + kb * BKF;   // 32 reduction rows per stage
-#pragma unroll
-            for (int j = 0; j < BM / 32; ++j)         // 32-float column groups of G
-              tma_load_2d(map_a, &full[stage], st + j * 4096, w.m0 + 32 * j, row);
-#pragma unroll
-            for (int j = 0; j < BN / 32; ++j)         // and of X
-              tma_load_2d(map_b, &full[stage], st + A_BYTES + j * 4096, w.n0 + 32 * j, row);
-          }
+          tma_load_2d(&maps.a[w.p], &full[stage], st, kb * BKF, base + w.m0);
+          tma_load_2d(&maps.b[w.p], &full[stage], st + A_BYTES, kb * BKF, w.n0);
           if (++stage == STAGES) { stage = 0; phase ^= 1; }
         }
       }
@@ -381,7 +393,7 @@ tc3_gemm_kernel(const __grid_constant__ Maps maps, const Params P) {
     uint32_t phase = 0;
     int it = 0;
     for (int item = blockIdx.x; item < num_items; item += gridDim.x, ++it) {
-      const Item w = decode_item<TN, BN>(P, S, item);
+      const Item w = decode_item<false, BN>(P, S, item);
       const bool tr = P.trace && blockIdx.x == 0 && it < P.trace_tiles && threadIdx.x == 0;
       if (tr) P.trace[it * 16 + 0] = clock64();
       float acc[MI][NI][4], accx[MI][NI][4];
@@ -391,16 +403,11 @@ tc3_gemm_kernel(const __grid_constant__ Maps maps, const Params P) {
         for (int j = 0; j < NI; ++j)
 #pragma unroll
           for (int e = 0; e < 4; ++e) { acc[i][j][e] = 0.f; accx[i][j][e] = 0.f; }
-      float colsum[MI][2];                       // TN: bias-gradient partials of this lane's G rows
-#pragma unroll
-      for (int i = 0; i < MI; ++i) { colsum[i][0] = 0.f; colsum[i][1] = 0.f; }
-      const bool want_cs = TN && P.bias_part[w.p] && w.n0 == 0 && wn == 0;
 
       for (int kb = 0; kb < w.nkb; ++kb) {
         mbar_wait(&full[stage], phase);
         const uint32_t sa = smem_u32(smem + stage * STAGE_BYTES);
         const uint32_t sb = sa + A_BYTES;
-        const int valid = TN ? w.rows - kb * BKF : BKF;   // TN: reduction rows past the chunk / row count may hold anything
 #pragma unroll
         for (int ks = 0; ks < BKF / 8; ++ks) {
           const int k0 = ks * 8 + t4, k1 = k0 + 4;
@@ -409,32 +416,15 @@ tc3_gemm_kernel(const __grid_constant__ Maps maps, const Params P) {
 #pragma unroll
           for (int j = 0; j < NI; ++j) {
             const int n = wn * WN + j * 8 + g8;
-            if constexpr (!TN) {
-              split_tf32_rn(lds32(sb + swz(n, k0)), bh[j][0], bl[j][0]);
-              split_tf32_rn(lds32(sb + swz(n, k1)), bh[j][1], bl[j][1]);
-            } else {                              // B = X: element (m, k) of the MN-major X boxes
-              float b0 = lds32(sb + (n >> 5) * 4096 + swz(k0, n & 31));
-              float b1 = lds32(sb + (n >> 5) * 4096 + swz(k1, n & 31));
-              if (k0 >= valid) b0 = 0.f;
-              if (k1 >= valid) b1 = 0.f;
-              split_tf32_rn(b0, bh[j][0], bl[j][0]);
-              split_tf32_rn(b1, bh[j][1], bl[j][1]);
-            }
+            split_tf32_rn(lds32(sb + swz(n, k0)), bh[j][0], bl[j][0]);
+            split_tf32_rn(lds32(sb + swz(n, k1)), bh[j][1], bl[j][1]);
           }
 #pragma unroll
           for (int i = 0; i < MI; ++i) {
             const int r0 = wm * WM + i * 16 + g8, r1 = r0 + 8;
             float a[4];
-            if constexpr (!TN) {
-              a[0] = lds32(sa + swz(r0, k0)); a[1] = lds32(sa + swz(r1, k0));
-              a[2] = lds32(sa + swz(r0, k1)); a[3] = lds32(sa + swz(r1, k1));
-            } else {                              // A = G^T: element (n, m) of the MN-major G boxes
-              a[0] = lds32(sa + (r0 >> 5) * 4096 + swz(k0, r0 & 31)); a[1] = lds32(sa + (r1 >> 5) * 4096 + swz(k0, r1 & 31));
-              a[2] = lds32(sa + (r0 >> 5) * 4096 + swz(k1, r0 & 31)); a[3] = lds32(sa + (r1 >> 5) * 4096 + swz(k1, r1 & 31));
-              if (k0 >= valid) { a[0] = 0.f; a[1] = 0.f; }
-              if (k1 >= valid) { a[2] = 0.f; a[3] = 0.f; }
-              if (want_cs) { colsum[i][0] += a[0] + a[2]; colsum[i][1] += a[1] + a[3]; }
-            }
+            a[0] = lds32(sa + swz(r0, k0)); a[1] = lds32(sa + swz(r1, k0));
+            a[2] = lds32(sa + swz(r0, k1)); a[3] = lds32(sa + swz(r1, k1));
             uint32_t ahi[4], alo[4];
 #pragma unroll
             for (int e = 0; e < 4; ++e) split_tf32_rn(a[e], ahi[e], alo[e]);
@@ -452,24 +442,9 @@ tc3_gemm_kernel(const __grid_constant__ Maps maps, const Params P) {
       }
 
       const GemmNT& g = P.g[w.p];
-      if constexpr (TN) {
-        if (want_cs) {
-          float* bp = P.bias_part[w.p] + (size_t)w.z * P.tn_nn[w.p];
-#pragma unroll
-          for (int i = 0; i < MI; ++i)
-#pragma unroll
-            for (int h = 0; h < 2; ++h) {
-              float s = colsum[i][h];
-              s += __shfl_xor_sync(0xffffffffu, s, 1);
-              s += __shfl_xor_sync(0xffffffffu, s, 2);
-              const int n = w.m0 + wm * WM + i * 16 + h * 8 + g8;
-              if (t4 == 0 && n < P.tn_nn[w.p]) bp[n] = s;
-            }
-        }
-      }
-      const int Mrows = TN ? P.tn_nn[w.p] : S.M[w.p];
-      const size_t row_base = TN ? (size_t)0 : (size_t)S.base[w.p];
-      const EpiArgs e = epi_args(g, g.C + (TN ? (size_t)w.z * P.tn_nn[w.p] * g.ldc : row_base * g.ldc), row_base, Mrows);
+      const int Mrows = S.M[w.p];
+      const size_t row_base = (size_t)S.base[w.p];
+      const EpiArgs e = epi_args(g, g.C + row_base * g.ldc, row_base, Mrows);
 #pragma unroll
       for (int j = 0; j < NI; ++j) {
         const int n = w.n0 + wn * WN + j * 8 + 2 * t4;    // this lane's column pair
@@ -485,8 +460,7 @@ tc3_gemm_kernel(const __grid_constant__ Maps maps, const Params P) {
             epi_store<EPI>(e, m, n, acc[i][j][2 * h] + accx[i][j][2 * h], acc[i][j][2 * h + 1] + accx[i][j][2 * h + 1], b);
           }
       }
-      if constexpr (!TN)
-        if (P.flags) signal_tile(P.flags + P.flag_off[w.p] + w.m0 / BM);
+      if (P.flags) signal_tile(P.flags + P.flag_off[w.p] + w.m0 / BM);
       if (tr) P.trace[it * 16 + 6] = clock64();
     }
   }
@@ -616,6 +590,230 @@ tc3_wgmma_kernel(const __grid_constant__ Maps maps, const Params P) {
         }
       }
       if (P.flags) signal_tile(P.flags + P.flag_off[w.p] + w.m0 / BM);
+      if (tr) P.trace[it * 16 + 6] = clock64();
+    }
+  }
+}
+
+__device__ __forceinline__ float4 lds128(uint32_t saddr) {
+  float4 v;
+  asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(saddr) : "memory");
+  return v;
+}
+
+__device__ __forceinline__ void sts128(uint32_t saddr, uint32_t x, uint32_t y, uint32_t z, uint32_t w) {
+  asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(saddr), "r"(x), "r"(y), "r"(z), "r"(w) : "memory");
+}
+
+// One 4 x 4 block of the X transpose: reduction rows k = 4a .. 4a + 3 of the raw X boxes at sx (valid: rows below it
+// are live; the others may hold anything, NaN included, and are written as 0) x columns n = 4b .. 4b + 3 of the tile,
+// into rows n, chunk a of the K-major (hi, lo) planes at sp.  Block t of the 256 of a k-block:
+//   t bits 0-2 = l, bits 3-4 = b >> 3 (the box), bit 5 = a >> 2, bits 6-7 = u;  b = 8 (b >> 3) + l,
+//   a = 4 (a >> 2) + 2 (l2 ^ u1) + (l1 ^ u0).
+// A 128-bit shared access is served 8 lanes at a time, and the 8 lanes of a group share everything but l: the raw
+// row k sits at 16-byte chunk l ^ (k & 7) with k & 7 = 4 (l1 ^ u0) + i, the plane row n = 4b + j at a ^ (n & 7) with
+// n & 7 = 4 l0 + j -- both take 8 distinct values over l, so reads and writes are free of bank conflicts.
+__device__ __forceinline__ void dw_transpose_block(uint32_t sx, uint32_t sp, int t, int valid) {
+  const int l = t & 7, u = t >> 6;
+  const int b = ((t >> 3) & 3) * 8 + l;
+  const int a = ((t >> 5) & 1) * 4 + ((((l >> 2) ^ (u >> 1)) & 1) << 1) + (((l >> 1) ^ u) & 1);
+  float4 v[4];
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    const int k = 4 * a + i;
+    v[i] = lds128(sx + (b >> 3) * 4096 + swz(k, 4 * (b & 7)));
+    if (k >= valid) v[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+  }
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    uint32_t hi[4], lo[4];
+#pragma unroll
+    for (int i = 0; i < 4; ++i) split_tf32_rn(j == 0 ? v[i].x : j == 1 ? v[i].y : j == 2 ? v[i].z : v[i].w, hi[i], lo[i]);
+    const uint32_t o = swz(4 * b + j, 4 * a);
+    sts128(sp + o, hi[0], hi[1], hi[2], hi[3]);
+    sts128(sp + DW_BN * BKF * 4 + o, lo[0], lo[1], lo[2], lo[3]);
+  }
+}
+
+// ---- wgmma kernel: TN (weight-gradient partials) ----
+__global__ void __launch_bounds__(WG_THREADS, 1)
+tc3_wgmma_dw_kernel(const __grid_constant__ Maps maps, const Params P) {
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + DW_OFF_BARS);
+  uint64_t* raw_full = bars;                            // [DW_RAW_STAGES] TMA -> consumers (G), transposers (X)
+  uint64_t* raw_empty = raw_full + DW_RAW_STAGES;       // [DW_RAW_STAGES] consumers + transposers -> TMA
+  uint64_t* pl_full = raw_empty + DW_RAW_STAGES;        // [DW_PLANE_STAGES] transposers -> consumers
+  uint64_t* pl_empty = pl_full + DW_PLANE_STAGES;       // [DW_PLANE_STAGES] consumers -> transposers
+  Sched& S = *reinterpret_cast<Sched*>(smem + DW_OFF_SCHED);
+
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < DW_RAW_STAGES; ++s) {
+      mbar_init(&raw_full[s], 1);
+      mbar_init(&raw_empty[s], CONS_WARPS + DW_TR_WARPS);
+    }
+    for (int s = 0; s < DW_PLANE_STAGES; ++s) {
+      mbar_init(&pl_full[s], DW_TR_WARPS);
+      mbar_init(&pl_empty[s], CONS_WARPS);   // once the last wgmma group reading the planes has retired
+    }
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    init_sched<true>(P, S);
+  }
+  __syncthreads();
+  const int num_items = S.begin[MAXP];
+
+  if (warp >= CONS_WARPS) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 56;");
+    if (warp == CONS_WARPS) {
+      // ================= TMA producer =================
+      if (lane == 0) {
+        int stage = 0;
+        uint32_t phase = 0;
+        for (int item = blockIdx.x; item < num_items; item += gridDim.x) {
+          const Item w = decode_item<true, DW_BN>(P, S, item);
+          const int row = S.base[w.p] + w.r0;
+          for (int kb = 0; kb < w.nkb; ++kb) {
+            mbar_wait(&raw_empty[stage], phase ^ 1);
+            uint8_t* st = smem + stage * DW_RAW_BYTES;
+            mbar_arrive_expect_tx(&raw_full[stage], DW_RAW_BYTES);
+#pragma unroll
+            for (int j = 0; j < BM / 32; ++j)          // 32-float column groups of G
+              tma_load_2d(&maps.a[w.p], &raw_full[stage], st + j * 4096, w.m0 + 32 * j, row + kb * BKF);
+#pragma unroll
+            for (int j = 0; j < DW_BN / 32; ++j)       // and of X
+              tma_load_2d(&maps.b[w.p], &raw_full[stage], st + A_BYTES + j * 4096, w.n0 + 32 * j, row + kb * BKF);
+            if (++stage == DW_RAW_STAGES) { stage = 0; phase ^= 1; }
+          }
+        }
+      }
+    } else {
+      // ================= transposers: raw X -> (X_hi^T, X_lo^T) planes =================
+      const int tt = threadIdx.x - 32 * (CONS_WARPS + 1);
+      int rs = 0, ps = 0;
+      uint32_t rph = 0, pph = 0;
+      for (int item = blockIdx.x; item < num_items; item += gridDim.x) {
+        const Item w = decode_item<true, DW_BN>(P, S, item);
+        for (int kb = 0; kb < w.nkb; ++kb) {
+          mbar_wait(&pl_empty[ps], pph ^ 1);
+          mbar_wait(&raw_full[rs], rph);
+          const uint32_t sx = smem_u32(smem + rs * DW_RAW_BYTES + A_BYTES);
+          const uint32_t sp = smem_u32(smem + DW_OFF_PLANES + ps * DW_PLANE_BYTES);
+          for (int t = tt; t < 256; t += 32 * DW_TR_WARPS) dw_transpose_block(sx, sp, t, w.rows - kb * BKF);
+          asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy stores -> wgmma reads
+          __syncwarp();
+          if (lane == 0) {
+            mbar_arrive(&raw_empty[rs]);
+            mbar_arrive(&pl_full[ps]);
+          }
+          if (++rs == DW_RAW_STAGES) { rs = 0; rph ^= 1; }
+          if (++ps == DW_PLANE_STAGES) { ps = 0; pph ^= 1; }
+        }
+      }
+    }
+  } else {
+    // ================= consumers (warpgroups 0-1): G^T fragments -> (hi, lo) -> wgmma -> partials =================
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 224;");
+    const int g8 = lane >> 2, t4 = lane & 3;     // fragment coordinates
+    const int r0 = (warp >> 2) * 64 + (warp & 3) * 16 + g8;   // this lane's G columns / output rows: r0, r0 + 8
+    // element (reduction row k, G column r) of the raw stage: box r / 32, swizzled row k
+    const uint32_t go0 = (r0 >> 5) * 4096, go1 = ((r0 + 8) >> 5) * 4096;
+    const int c0 = r0 & 31, c1 = (r0 + 8) & 31;
+    int rs = 0, ps = 0;
+    uint32_t rph = 0, pph = 0;
+    int it = 0;
+    for (int item = blockIdx.x; item < num_items; item += gridDim.x, ++it) {
+      const Item w = decode_item<true, DW_BN>(P, S, item);
+      const bool tr = P.trace && blockIdx.x == 0 && it < P.trace_tiles && threadIdx.x == 0;
+      if (tr) P.trace[it * 16 + 0] = clock64();
+      float acc[64], accx[64];
+#pragma unroll
+      for (int e = 0; e < 64; ++e) { acc[e] = 0.f; accx[e] = 0.f; }
+      float cs0 = 0.f, cs1 = 0.f;                // bias-gradient partials of this lane's G columns
+      const bool want_cs = P.bias_part[w.p] && w.n0 == 0;
+
+      // the pipeline of tc3_wgmma_kernel: half a k-block of fragments per buffer and wgmma group, wait_group 1; the
+      // raw stage (G only) is released as soon as the fragments of its half 1 are in registers, the plane stage once
+      // the group of its half 1 has retired
+      uint32_t ah0[2][4], al0[2][4], ah1[2][4], al1[2][4];
+      int prev = -1;
+      auto half = [&](uint32_t sg, uint32_t sp, int valid, int hk, uint32_t (&ah)[2][4], uint32_t (&al)[2][4]) {
+#pragma unroll
+        for (int s = 0; s < 2; ++s) {
+          const int k0 = (2 * hk + s) * 8 + t4, k1 = k0 + 4;
+          float a[4];
+          a[0] = lds32(sg + go0 + swz(k0, c0)); a[1] = lds32(sg + go1 + swz(k0, c1));
+          a[2] = lds32(sg + go0 + swz(k1, c0)); a[3] = lds32(sg + go1 + swz(k1, c1));
+          if (k0 >= valid) { a[0] = 0.f; a[1] = 0.f; }   // rows past the chunk / row count may hold anything
+          if (k1 >= valid) { a[2] = 0.f; a[3] = 0.f; }
+          if (want_cs) { cs0 += a[0] + a[2]; cs1 += a[1] + a[3]; }
+#pragma unroll
+          for (int e = 0; e < 4; ++e) split_tf32_rn(a[e], ah[s][e], al[s][e]);
+        }
+        wgmma_fence();
+#pragma unroll
+        for (int s = 0; s < 2; ++s) {
+          const uint32_t ko = (2 * hk + s) * 32;
+          const uint64_t dh = wgmma_desc_sw128(sp + ko);
+          const uint64_t dl = wgmma_desc_sw128(sp + DW_BN * BKF * 4 + ko);
+          wgmma_m64n128k8_tf32(acc, ah[s], dh);
+          wgmma_m64n128k8_tf32(accx, al[s], dh);
+          wgmma_m64n128k8_tf32(accx, ah[s], dl);
+        }
+        wgmma_commit();
+        wgmma_wait<1>();
+      };
+      for (int kb = 0; kb < w.nkb; ++kb) {
+        mbar_wait(&raw_full[rs], rph);
+        mbar_wait(&pl_full[ps], pph);
+        const uint32_t sg = smem_u32(smem + rs * DW_RAW_BYTES);
+        const uint32_t sp = smem_u32(smem + DW_OFF_PLANES + ps * DW_PLANE_BYTES);
+        const int valid = w.rows - kb * BKF;
+        half(sg, sp, valid, 0, ah0, al0);
+        if (prev >= 0) {
+          __syncwarp();
+          if (lane == 0) mbar_arrive(&pl_empty[prev]);
+        }
+        half(sg, sp, valid, 1, ah1, al1);
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&raw_empty[rs]);
+        prev = ps;
+        if (++rs == DW_RAW_STAGES) { rs = 0; rph ^= 1; }
+        if (++ps == DW_PLANE_STAGES) { ps = 0; pph ^= 1; }
+      }
+      wgmma_wait<0>();
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&pl_empty[prev]);
+
+      const int Nn = P.tn_nn[w.p];
+      if (want_cs) {
+        float* bp = P.bias_part[w.p] + (size_t)w.z * Nn;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          float s = h ? cs1 : cs0;
+          s += __shfl_xor_sync(0xffffffffu, s, 1);
+          s += __shfl_xor_sync(0xffffffffu, s, 2);
+          const int n = w.m0 + r0 + h * 8;
+          if (t4 == 0 && n < Nn) bp[n] = s;
+        }
+      }
+      const GemmNT& g = P.g[w.p];
+      const EpiArgs e = epi_args(g, g.C + (size_t)w.z * Nn * g.ldc, 0, Nn);
+#pragma unroll
+      for (int j = 0; j < DW_BN / 8; ++j) {
+        const int n = w.n0 + j * 8 + 2 * t4;      // this lane's column pair
+        if (n >= e.n_store) continue;
+        float b[2];
+        epi_bias<EPI_SPEC_LINEAR>(e, n, b);
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int m = w.m0 + r0 + h * 8;
+          if (m >= Nn) continue;
+          epi_store<EPI_SPEC_LINEAR>(e, m, n, acc[4 * j + 2 * h] + accx[4 * j + 2 * h],
+                                     acc[4 * j + 2 * h + 1] + accx[4 * j + 2 * h + 1], b);
+        }
+      }
       if (tr) P.trace[it * 16 + 6] = clock64();
     }
   }
@@ -764,17 +962,17 @@ static int prepare(int* num_sms_out) {
   DevInfo& d = g_dev[dev];
   if (!d.attr_done) {   // function attributes are per device
     GIB_CUDA_TRY(cudaDeviceGetAttribute(&d.num_sms, cudaDevAttrMultiProcessorCount, dev));
-    GIB_CUDA_TRY(cudaFuncSetAttribute(tc3_gemm_kernel<false, EPI_SPEC_GENERIC>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
-    GIB_CUDA_TRY(cudaFuncSetAttribute(tc3_gemm_kernel<false, EPI_SPEC_SELU>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
-    GIB_CUDA_TRY(cudaFuncSetAttribute(tc3_gemm_kernel<false, EPI_SPEC_LINEAR>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
-    GIB_CUDA_TRY(cudaFuncSetAttribute(tc3_gemm_kernel<false, EPI_SPEC_DSELU>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
-    GIB_CUDA_TRY(cudaFuncSetAttribute(tc3_gemm_kernel<false, EPI_SPEC_ADD>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
-    GIB_CUDA_TRY(cudaFuncSetAttribute(tc3_gemm_kernel<true, EPI_SPEC_LINEAR>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
+    GIB_CUDA_TRY(cudaFuncSetAttribute(tc3_gemm_kernel<EPI_SPEC_GENERIC>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
+    GIB_CUDA_TRY(cudaFuncSetAttribute(tc3_gemm_kernel<EPI_SPEC_SELU>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
+    GIB_CUDA_TRY(cudaFuncSetAttribute(tc3_gemm_kernel<EPI_SPEC_LINEAR>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
+    GIB_CUDA_TRY(cudaFuncSetAttribute(tc3_gemm_kernel<EPI_SPEC_DSELU>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
+    GIB_CUDA_TRY(cudaFuncSetAttribute(tc3_gemm_kernel<EPI_SPEC_ADD>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
     GIB_CUDA_TRY(cudaFuncSetAttribute(tc3_wgmma_kernel<EPI_SPEC_GENERIC>, cudaFuncAttributeMaxDynamicSharedMemorySize, WG_SMEM_BYTES));
     GIB_CUDA_TRY(cudaFuncSetAttribute(tc3_wgmma_kernel<EPI_SPEC_SELU>, cudaFuncAttributeMaxDynamicSharedMemorySize, WG_SMEM_BYTES));
     GIB_CUDA_TRY(cudaFuncSetAttribute(tc3_wgmma_kernel<EPI_SPEC_LINEAR>, cudaFuncAttributeMaxDynamicSharedMemorySize, WG_SMEM_BYTES));
     GIB_CUDA_TRY(cudaFuncSetAttribute(tc3_wgmma_kernel<EPI_SPEC_DSELU>, cudaFuncAttributeMaxDynamicSharedMemorySize, WG_SMEM_BYTES));
     GIB_CUDA_TRY(cudaFuncSetAttribute(tc3_wgmma_kernel<EPI_SPEC_ADD>, cudaFuncAttributeMaxDynamicSharedMemorySize, WG_SMEM_BYTES));
+    GIB_CUDA_TRY(cudaFuncSetAttribute(tc3_wgmma_dw_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, DW_SMEM_BYTES));
     d.attr_done = true;
   }
   *num_sms_out = d.num_sms;
@@ -887,11 +1085,11 @@ static int launch_nt(const GemmNT* ps, const int* dep, int n, int* flags, bool r
   ProfScope prof(PROF_GEMM_NT, work, st);
   if (raw) {
     switch (spec) {
-      case EPI_SPEC_SELU: tc3_gemm_kernel<false, EPI_SPEC_SELU><<<grid, NUM_THREADS, SMEM_BYTES, st>>>(maps, P); break;
-      case EPI_SPEC_LINEAR: tc3_gemm_kernel<false, EPI_SPEC_LINEAR><<<grid, NUM_THREADS, SMEM_BYTES, st>>>(maps, P); break;
-      case EPI_SPEC_DSELU: tc3_gemm_kernel<false, EPI_SPEC_DSELU><<<grid, NUM_THREADS, SMEM_BYTES, st>>>(maps, P); break;
-      case EPI_SPEC_ADD: tc3_gemm_kernel<false, EPI_SPEC_ADD><<<grid, NUM_THREADS, SMEM_BYTES, st>>>(maps, P); break;
-      default: tc3_gemm_kernel<false, EPI_SPEC_GENERIC><<<grid, NUM_THREADS, SMEM_BYTES, st>>>(maps, P); break;
+      case EPI_SPEC_SELU: tc3_gemm_kernel<EPI_SPEC_SELU><<<grid, NUM_THREADS, SMEM_BYTES, st>>>(maps, P); break;
+      case EPI_SPEC_LINEAR: tc3_gemm_kernel<EPI_SPEC_LINEAR><<<grid, NUM_THREADS, SMEM_BYTES, st>>>(maps, P); break;
+      case EPI_SPEC_DSELU: tc3_gemm_kernel<EPI_SPEC_DSELU><<<grid, NUM_THREADS, SMEM_BYTES, st>>>(maps, P); break;
+      case EPI_SPEC_ADD: tc3_gemm_kernel<EPI_SPEC_ADD><<<grid, NUM_THREADS, SMEM_BYTES, st>>>(maps, P); break;
+      default: tc3_gemm_kernel<EPI_SPEC_GENERIC><<<grid, NUM_THREADS, SMEM_BYTES, st>>>(maps, P); break;
     }
   } else {
     switch (spec) {
@@ -951,7 +1149,7 @@ int tc3_dw_chunk_rows(const GemmDW* qs, int n, long long plan_rows) {
   long long rows = 0;
   for (int i = 0; i < n; ++i) {
     if (qs[i].M <= 0) continue;
-    max_tiles = std::max(max_tiles, ceil_div(qs[i].Nn, BM) * ceil_div(qs[i].Kk, BN));
+    max_tiles = std::max(max_tiles, ceil_div(qs[i].Nn, BM) * ceil_div(qs[i].Kk, DW_BN));
     rows += qs[i].M;
   }
   if (plan_rows > 0) rows = plan_rows;
@@ -1009,7 +1207,7 @@ static int launch_tn(const GemmDW* qs, int n, int chunk_rows, float* const* part
     g.M = q.M; g.m_dev = q.m_dev; g.base_dev = q.base_dev;
     g.C = part[i]; g.ldc = q.Kk; g.N = q.Kk; g.n_store = q.Kk; g.n_valid = q.Kk;
     g.mode = EPI_ACT; g.act = ACT_NONE; g.bias = nullptr;
-    P.n_tiles[i] = ceil_div(q.Kk, BN);
+    P.n_tiles[i] = ceil_div(q.Kk, DW_BN);
     P.tn_mt[i] = ceil_div(q.Nn, BM);
     P.tn_nn[i] = q.Nn;
     P.bias_part[i] = bias_part[i];
@@ -1019,7 +1217,7 @@ static int launch_tn(const GemmDW* qs, int n, int chunk_rows, float* const* part
   P.chunk_rows = chunk_rows;
   P.trace = g_trace; P.trace_tiles = g_trace_tiles;
   const int grid = (int)(items < num_sms ? items : num_sms);
-  tc3_gemm_kernel<true, EPI_SPEC_LINEAR><<<grid, NUM_THREADS, SMEM_BYTES, st>>>(maps, P);
+  tc3_wgmma_dw_kernel<<<grid, WG_THREADS, DW_SMEM_BYTES, st>>>(maps, P);
   GIB_LAUNCH_CHECK();
   return 0;
 }
@@ -1037,7 +1235,7 @@ int gemm_dw_tc3_partials(const GemmDW* qs, int n, const Dw3Layout& L, float* scr
 
 // ---- single weight-gradient problem, partials only ([splits][Nn][Kk] into q.scratch; the caller reduces them) ----
 void tc_dw_plan(int M, int Nn, int Kk, int* splits, int* chunk) {
-  const int tiles = ceil_div(Nn, tc3::BM) * ceil_div(Kk, tc3::BN);
+  const int tiles = ceil_div(Nn, tc3::BM) * ceil_div(Kk, tc3::DW_BN);
   int s = ceil_div(device_sm_count(), tiles);         // about one work item per SM
   int c = ceil_div(ceil_div(M, s), tc3::BKF) * tc3::BKF;
   if (c < 8 * tc3::BKF) c = 8 * tc3::BKF;             // >= 256 reduction rows per item
