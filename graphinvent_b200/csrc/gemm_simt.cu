@@ -586,8 +586,9 @@ int gemm_dw_group(const GemmDW* qs, int n, long long plan_rows, cudaStream_t st)
   for (int i = 0; i < n; ++i) {
     const GemmDW& q = qs[i];
     if (q.M <= 0) continue;
-    const bool good = tc3 && tc3_dw_eligible(q) && q.Nn >= 32 && q.Kk >= 32 && q.scratch == qs[0].scratch &&
-                      q.half_floats == qs[0].half_floats;
+    // (16-wide operands are eligible; narrower than 32 is only worth the launch when the row count is on the device)
+    const bool good = tc3 && tc3_dw_eligible(q) && ((q.Nn >= 32 && q.Kk >= 32) || q.m_dev) &&
+                      q.scratch == qs[0].scratch && q.half_floats == qs[0].half_floats;
     if (q.m_dev) {
       dyn = true;
       if (!good) {

@@ -239,7 +239,7 @@ size_t graph_count_ws_ints(int B, int G) { return (size_t)2 * G * B + B + HDR_IN
 int graph_count(const void* edges, int in_dtype, int B, int N, int Ef, int by_type, int* ws, cudaStream_t st) {
   const int G = by_type ? Ef : 1;
   if (B <= 0 || N <= 0 || Ef <= 0 || Ef > 4 || (long long)N * N * G > 32768) {
-    set_error("graph_count: unsupported dims B=%d N=%d Ef=%d (need Ef<=4, N*N*groups<=32768)", B, N, Ef);
+    set_error("graph_count: unsupported dims B=%d N=%d Ef=%d (need 1 <= n_edge_features <= 4, N*N*groups<=32768)", B, N, Ef);
     return -1;
   }
   int* hdr = ws;

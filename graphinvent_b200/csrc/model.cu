@@ -81,12 +81,18 @@ int build_plan(const gib_dims& d, Plan& pl) {
   pl = Plan();
   pl.d = d;
   if (d.model < 0 || d.model > 3 || d.Ef < 1 || d.Ef > 4 || d.T < 1 || d.T > kMaxPasses || d.N < 1 || d.F < 1 ||
-      d.H < 1 || d.M < 1 || d.f_add < 1 || d.f_conn < 1 || d.mlp1_depth < 0 || d.mlp1_depth > 7 || d.mlp2_depth < 0 ||
-      d.mlp2_depth > 7 || d.msg_depth > 7 || d.att_depth > 7 || d.gatt_depth > 7 || d.gemb_depth > 7 ||
-      d.eemb_depth > 7) {
-    set_error("build_plan: unsupported dims (model=%d Ef=%d T=%d)", d.model, d.Ef, d.T);
+      d.H < 1 || d.M < 1 || d.f_add < 1 || d.f_conn < 1) {
+    set_error("build_plan: unsupported dims (model=%d Ef=%d T=%d; need 1 <= n_edge_features <= 4, "
+              "1 <= message_passes <= %d)", d.model, d.Ef, d.T, kMaxPasses);
     return -1;
   }
+  // an MLP of depth k has k + 1 Linears; the chained backward keeps one gradient buffer per layer (BwdBufs::Gl)
+  const int depths[7] = {d.mlp1_depth, d.mlp2_depth, d.msg_depth, d.att_depth, d.gatt_depth, d.gemb_depth, d.eemb_depth};
+  for (int k : depths)
+    if (k < 0 || k > 7) {
+      set_error("build_plan: MLP depth %d unsupported (need 0 <= depth <= 7)", k);
+      return -1;
+    }
   if (d.model != GIB_EMN && d.H < d.F) {
     set_error("build_plan: hidden_node_features (%d) < n_node_features (%d)", d.H, d.F);
     return -1;
@@ -130,15 +136,17 @@ int build_plan(const gib_dims& d, Plan& pl) {
   pl.fconn2 = add_mlp(pl, N * d.f_conn + pl.G, d.mlp2_hidden, d.mlp2_depth, N * d.f_conn);
   pl.fterm2 = add_mlp(pl, pl.G, d.mlp2_hidden, d.mlp2_depth, 1);
   pl.apd = N * d.f_add + N * d.f_conn + 1;
+  // checked here rather than at packing time, so that every size query refuses such a model with the same message
+  if ((int)pl.lins.size() > kMaxPackEntries) {
+    set_error("build_plan: %d Linears exceed the packing descriptor table (at most %d Linears)", (int)pl.lins.size(),
+              kMaxPackEntries);
+    return -1;
+  }
   return 0;
 }
 
 int pack_params(const Plan& pl, const float* const* params, float* packed, cudaStream_t st) {
-  if ((int)pl.lins.size() > kMaxPackEntries) {
-    set_error("pack_params: %d Linears exceed the descriptor table (%d)", (int)pl.lins.size(), kMaxPackEntries);
-    return -1;
-  }
-  {   // one launch for the whole model (52-67 Linears)
+  {   // one launch for the whole model (52-67 Linears at the reference's defaults, at most kMaxPackEntries)
     PackTable T;
     T.n = (int)pl.lins.size();
     unsigned blk = 0;
@@ -480,6 +488,16 @@ static int mlp_forward_multi(const Run& r, const MlpJob* jobs, int n, int* flags
   return 0;
 }
 
+// Sibling MLPs whose layers do not all fit one grouped launch (unequal depths, or more than kTc3MaxProblems layers in
+// all, e.g. 4 bond types x 5 Linears) run their backward in sub-groups: [i, i + k) is the longest run of members of
+// member i's depth that fits.
+static int sub_group(const Mlp* const* ms, int n, int i) {
+  const int per = std::max(1, kTc3MaxProblems / ms[i]->n);
+  int k = 1;
+  while (i + k < n && k < per && ms[i + k]->n == ms[i]->n) ++k;
+  return k;
+}
+
 // Backward of sibling MLPs of equal depth.  Three launches' worth of structure instead of three per layer:
 //   (A) the input-gradient GEMMs of layers n..2 (G_{l-1} = (G_l W_l) . selu'(X_{l-1})) as ONE dependent chain,
 //       every G_l kept in its own buffer;
@@ -495,16 +513,21 @@ static int mlp_backward_multi(const Run& r, const BwdBufs& bb, const MlpBwdJob* 
   bool same = n <= 4;
   for (int i = 1; i < n && same; ++i) same = jobs[i].m->n == jobs[0].m->n;
   const int depth = jobs[0].m->n;
-  if (!same || depth > 8 || depth * n > kTc3MaxProblems) {
-    for (int i = 0; i < n; ++i) {
-      if (jobs[i].m_dev) {
-        set_error("mlp_backward_multi: device-side row counts need <= 4 sibling MLPs of equal depth, at most 8 layers "
-                  "each and %d layers in all (got %d MLPs, depth of the first %d)", kTc3MaxProblems, n, depth);
-        return -2;
+  if (!same || depth * n > kTc3MaxProblems) {
+    if (jobs[0].m_dev) {
+      // device-side row counts need the grouped call pattern: sub-groups that fit one launch, each planned with the
+      // whole group's plan rows (make_bwd sizes the same split through group_extent)
+      const Mlp* ms[4];
+      for (int i = 0; i < n; ++i) ms[i] = jobs[i].m;
+      for (int i = 0, k; i < n; i += k) {
+        k = sub_group(ms, n, i);
+        GIB_TRY(mlp_backward_multi(r, bb, jobs + i, k, plan_rows, same_rows));
       }
+      return 0;
+    }
+    for (int i = 0; i < n; ++i)
       GIB_TRY(mlp_backward(r, bb, *jobs[i].m, jobs[i].X0, *jobs[i].a, jobs[i].row0, jobs[i].rows, jobs[i].Gtop,
                            jobs[i].dX0, jobs[i].ld_dx, jobs[i].dx_aux));
-    }
     return 0;
   }
   // G[l][i]: gradient w.r.t. the pre-activation of layer l of member i; G[depth] = the caller's Gtop
@@ -1000,12 +1023,21 @@ static void mlp_extent(const Plan& pl, const Mlp& m, size_t rows, size_t& big, s
     dw = std::max(dw, gemm_dw_scratch_floats((int)rows, L.Rp, L.Cp));
   }
 }
-// the same for sibling MLPs of equal depth whose weight gradients run as one grouped launch per layer
-static void group_extent(const Plan& pl, const Mlp* const* ms, const size_t* rows, int n, long long plan_rows, size_t& dw) {
-  for (int i = 1; i < n; ++i)
-    if (ms[i]->n != ms[0]->n) return;
+// the same for sibling MLPs of equal depth whose weight gradients run as one grouped launch per layer; split: siblings
+// that do not fit one launch run in the sub-groups of mlp_backward_multi (capacity mode), else one by one (mlp_extent)
+static void group_extent(const Plan& pl, const Mlp* const* ms, const size_t* rows, int n, long long plan_rows, size_t& dw,
+                         bool split = false) {
+  bool same = true;
+  for (int i = 1; i < n; ++i) same = same && ms[i]->n == ms[0]->n;
   const int depth = ms[0]->n;
-  if (depth * n > kTc3MaxProblems) return;
+  if (!same || depth * n > kTc3MaxProblems) {
+    if (split)
+      for (int i = 0, k; i < n; i += k) {
+        k = sub_group(ms, n, i);
+        group_extent(pl, ms + i, rows + i, k, plan_rows, dw);
+      }
+    return;
+  }
   GemmDW qs[kTc3MaxProblems];     // all layers of all members: one grouped launch (mlp_backward_multi)
   int nq = 0;
   for (int l = 0; l < depth; ++l)
@@ -1035,10 +1067,10 @@ void make_bwd(const Run& r, BwdBufs& bb) {
     {
       const Mlp* ms[4]; size_t rows[4];
       for (int g = 0; g < r.ngroups; ++g) { ms[g] = &pl.msg[g]; rows[g] = (size_t)r.tc[g]; }
-      group_extent(pl, ms, rows, r.ngroups, r.cap ? r.P : 0, dw);
+      group_extent(pl, ms, rows, r.ngroups, r.cap ? r.P : 0, dw, r.cap);
       if (d.model == GIB_ATTGGNN) {
         for (int g = 0; g < r.ngroups; ++g) ms[g] = &pl.att[g];
-        group_extent(pl, ms, rows, r.ngroups, r.cap ? r.P : 0, dw);
+        group_extent(pl, ms, rows, r.ngroups, r.cap ? r.P : 0, dw, r.cap);
       }
     }
   } else {

@@ -65,6 +65,8 @@ def _require_cuda(*tensors):
 
 def _check_params(model, d, params):
     n = lib.gib_model_num_params(ctypes.byref(d))
+    if n < 0:
+        check(n, "gib_model_num_params")     # dims the library does not support: its message names the limit
     if n != len(params):
         raise RuntimeError(f"parameter table mismatch: library expects {n} tensors, module has {len(params)}")
     for i, p in enumerate(params):

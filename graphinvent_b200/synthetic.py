@@ -10,11 +10,13 @@ atom list, formal charge fixed to the neutral slot (node rows sum to 2, as in th
 real gdb13 data); a random recursive tree (atom i bonds to a uniformly chosen
 earlier atom of degree < 4) plus floor(n/6) ring closures between non-adjacent
 atoms of degree < 4; bond type ~ Categorical(0.84, 0.14, 0.02) on tree bonds,
-single on closures.  Targets are uniform-random positive APD rows.
+single on closures.  With n_edge_features = 4 (the reference's `use_aromatic_bonds`)
+the fourth, aromatic type has weight 0.10 and the four are renormalised; fewer types
+take the leading weights, renormalised.  Targets are uniform-random positive APD rows.
 """
 import numpy as np
 
-BOND_P = (0.84, 0.14, 0.02)
+BOND_P = (0.84, 0.14, 0.02, 0.10)
 
 
 def random_graphs(batch, max_n_nodes, n_atom_types, n_charges, n_edge_features=3,
@@ -88,7 +90,7 @@ def corner_case_graphs(max_n_nodes, n_node_features, n_edge_features=3):
     nodes[2, 0, 0] = nodes[2, 0, F - 2] = 1
     k = min(6, N)
     for i in range(k):
-        nodes[3, i, i % (F - 3)] = nodes[3, i, F - 2] = 1
+        nodes[3, i, i % max(1, F - 3)] = nodes[3, i, F - 2] = 1
     for i in range(1, k):
         edges[3, 0, i, 0] = edges[3, i, 0, 0] = 1
     nodes[4, 0, 0] = nodes[4, 1, 1] = 1
