@@ -43,7 +43,7 @@ MODEL_ID = {"GGNN": 0, "MNN": 1, "AttGGNN": 2, "EMN": 3}
 HDR_INTS = 16
 HDR_E, HDR_P, HDR_TYPE_COUNT, HDR_TYPE_BASE, HDR_FLAGS, HDR_CAPACITY = 0, 1, 2, 6, 11, 12
 FLAG_MULTITYPE, FLAG_NONBINARY, FLAG_OVERFLOW = 1, 2, 4
-ABI_VERSION = 204     # must equal gib_version() of the loaded library (include/gib200.h)
+ABI_VERSION = 205     # must equal gib_version() of the loaded library (include/gib200.h)
 
 _PROTOS = {
     "gib_last_error": (ctypes.c_char_p, []),
@@ -88,6 +88,7 @@ _PROTOS = {
     "gib_generation_scratch_bytes": (c_sz, [c_i]),
     "gib_generation_round": (c_i, [c_i] * 7 + [c_p] * 11 + [c_i, c_p, c_p, c_p]),
     "gib_generation_round_layout": (c_i, [c_i] * 9 + [c_p] * 11 + [c_i, c_p, c_p, c_p]),
+    "gib_generation_sample_round": (c_i, [c_i] * 8 + [c_p, c_i] + [c_p] * 13 + [c_i, c_p, c_p, c_p]),
     "gib_profile_enable": (None, [c_i]),
     "gib_launch_count": (c_ll, []),
     "gib_profile_collect": (c_i, [c_p, c_p, c_p]),

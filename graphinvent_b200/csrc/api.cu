@@ -88,12 +88,27 @@ __global__ void __launch_bounds__(256) validation_nll_kernel(const float* __rest
 }
 
 // ---- categorical sampling of one action per molecule (GraphGenerator.py:121, 535-542) ----
+// g.state != null: the round-gated form of gib_generation_sample_round (ops.cuh: RoundGate)
 __global__ void __launch_bounds__(256) sample_actions_kernel(const float* __restrict__ out, int apd,
                                                              const float* __restrict__ uniforms,
-                                                             int* __restrict__ action, float* __restrict__ lik) {
+                                                             int* __restrict__ action, float* __restrict__ lik,
+                                                             RoundGate g) {
   __shared__ float sm[8];
   __shared__ float pre[257];
   const int b = blockIdx.x;
+  if (g.state) {
+    // every CTA reads the same words before any of them is written (state[0] / counters advance in gen_scan_kernel,
+    // which runs after this kernel); only CTA 0 writes, and a status it sets cannot change another CTA's decision
+    const int r = g.state[0], B = gridDim.x;
+    const bool live = g.counters[0] < B && g.state[1] == 0;
+    const bool go = live && r >= 0 && r < g.rounds;
+    if (b == 0 && threadIdx.x == 0) {
+      g.ctl[0] = go ? r : -1;
+      if (live && !go) g.state[1] = 1;
+    }
+    if (!go) return;
+    uniforms += (size_t)r * B;
+  }
   const float* o = out + (size_t)b * apd;
   float mx = -INFINITY;
   for (int k = threadIdx.x; k < apd; k += 256) mx = fmaxf(mx, o[k]);
@@ -138,6 +153,14 @@ __global__ void __launch_bounds__(256) sample_actions_kernel(const float* __rest
   }
 }
 
+int sample_actions_launch(const float* out, int B, int apd, const float* uniforms, int* action, float* lik,
+                          const RoundGate* gate, cudaStream_t st) {
+  if (B <= 0) return 0;
+  sample_actions_kernel<<<B, 256, 0, st>>>(out, apd, uniforms, action, lik, gate ? *gate : RoundGate{});
+  GIB_LAUNCH_CHECK();
+  return 0;
+}
+
 }  // namespace gib
 
 using namespace gib;
@@ -148,8 +171,8 @@ extern "C" {
 
 const char* gib_last_error(void) { return g_err; }
 // 200: capacity mode, int8 inputs, grouped dW; 201: 5 profile classes; 202: test hooks; 203: forward / glue test hooks;
-// 204: gib_generation_round_layout (implicit-H / chirality action layouts)
-int gib_version(void) { return 204; }
+// 204: gib_generation_round_layout (implicit-H / chirality action layouts); 205: gib_generation_sample_round
+int gib_version(void) { return 205; }
 void gib_set_tensor_cores(int on) { g_use_tc = on != 0; }
 int gib_get_tensor_cores(void) { return g_use_tc ? 1 : 0; }
 void gib_tc_debug(int mode) { g_tc_debug = mode; }
@@ -308,10 +331,7 @@ int gib_validation_nll(const float* out, const float* target, int B, int apd, fl
 
 int gib_sample_actions(const float* out, int B, int apd, const float* uniforms, int* action, float* likelihood,
                        gib_stream stream) {
-  if (B <= 0) return 0;
-  sample_actions_kernel<<<B, 256, 0, ST(stream)>>>(out, apd, uniforms, action, likelihood);
-  GIB_LAUNCH_CHECK();
-  return 0;
+  return sample_actions_launch(out, B, apd, uniforms, action, likelihood, nullptr, ST(stream));
 }
 
 int gib_linear_fwd(const float* X, int ldx, const float* W, int ldw, const float* bias, float* Y, int ldy, int M,

@@ -24,8 +24,14 @@
 //   * terminated graphs are copied out in their PRE-action state, terminate-sampled slots first (ascending), then
 //     invalid ones (ascending); `properly_terminated[k : k + #terminate-sampled]` counts slot 0 if it sampled terminate;
 //   * likelihoods are stored at the GLOBAL round index.
+//
+// gib_generation_sample_round runs the same kernels behind the sampler with the round index and the loop condition of
+// GraphGenerator.build_graphs in device memory (so a captured round can be replayed without reading anything back):
+// the sampler decides once per call whether the round runs and leaves the round index (or -1: inert) in `ctl`, which
+// the decode, scan and apply kernels read instead of their `round` argument.  The plain entry points pass ctl = null.
 #include "../../include/gib200.h"
 #include "common.cuh"
+#include "ops.cuh"
 
 namespace gib {
 
@@ -36,9 +42,10 @@ enum : int { ACT_ADD = 0, ACT_CONN = 1, ACT_TERM = 2 };
 
 // per slot: decoded action + validity  (one thread per slot)
 __global__ void gen_decode_kernel(GenDims d, const int* __restrict__ action, const float* __restrict__ edges,
-                                  const int* __restrict__ n_nodes, int4* __restrict__ rec, int* __restrict__ flags) {
+                                  const int* __restrict__ n_nodes, int4* __restrict__ rec, int* __restrict__ flags,
+                                  const int* __restrict__ ctl) {
   const int b = blockIdx.x * blockDim.x + threadIdx.x;
-  if (b >= d.B) return;
+  if (b >= d.B || (ctl && ctl[0] < 0)) return;
   const int a = action[b];
   const int n = n_nodes[b];
   const int len_add = d.N * d.A * d.CH * max(d.H, 1) * max(d.C, 1) * d.Ef, len_conn = d.N * d.Ef;
@@ -99,11 +106,15 @@ __global__ void gen_decode_kernel(GenDims d, const int* __restrict__ action, con
 
 // single CTA: output positions of the slots that terminate this round + counters
 // counters[0] = n_generated (in/out), counters[1] = written this round
+// ctl != null: the round index of this call (< 0: inert), and state = {next round, status} is advanced here
 __global__ void __launch_bounds__(1024) gen_scan_kernel(int B, const int* __restrict__ flags, int* __restrict__ pos,
                                                         int* __restrict__ counters,
-                                                        signed char* __restrict__ properly_terminated, int cap) {
+                                                        signed char* __restrict__ properly_terminated, int cap,
+                                                        const int* __restrict__ ctl, int* __restrict__ state,
+                                                        int rounds) {
   __shared__ int s_cnt[2][1024];
   __shared__ int s_tot[3];
+  if (ctl && ctl[0] < 0) return;
   const int L = ceil_div(B, 1024);
   const int lo = min(B, (int)threadIdx.x * L), hi = min(B, lo + L);
   int c_term = 0, c_inv = 0;
@@ -142,6 +153,11 @@ __global__ void __launch_bounds__(1024) gen_scan_kernel(int B, const int* __rest
   if (threadIdx.x == 0) {
     counters[1] = n_term + n_inv;
     counters[0] = k + n_term + n_inv;
+    if (ctl) {                        // build_graphs' loop rule: round 2N would be needed -> status 1 (round limit)
+      const int next = ctl[0] + 1;
+      state[0] = next;
+      if (k + n_term + n_inv < B && next >= rounds) state[1] = 1;
+    }
   }
 }
 
@@ -152,7 +168,11 @@ __global__ void __launch_bounds__(128) gen_apply_kernel(GenDims d, int round, co
                                                         int* __restrict__ n_nodes, float* __restrict__ likelihoods,
                                                         float* __restrict__ g_nodes, float* __restrict__ g_edges,
                                                         signed char* __restrict__ g_n_nodes,
-                                                        float* __restrict__ g_lik) {
+                                                        float* __restrict__ g_lik, const int* __restrict__ ctl) {
+  if (ctl) {
+    round = ctl[0];
+    if (round < 0) return;
+  }
   const int b = blockIdx.x;
   const int NF = d.N * d.F, NNE = d.N * d.N * d.Ef;
   float* nb = nodes + (size_t)b * NF;
@@ -207,12 +227,9 @@ __global__ void __launch_bounds__(128) gen_apply_kernel(GenDims d, int round, co
 
 using namespace gib;
 
-extern "C" int gib_generation_round_layout(int B, int N, int F, int Ef, int n_atom_types, int n_charges, int n_imp_H,
-                                           int n_chirality, int round, const int* action, const float* likelihood,
-                                           float* nodes, float* edges, int* n_nodes, float* likelihoods,
-                                           float* gen_nodes, float* gen_edges, signed char* gen_n_nodes,
-                                           float* gen_likelihoods, signed char* properly_terminated, int capacity,
-                                           int* counters, void* scratch, gib_stream stream) {
+// arguments shared by every round entry point; the messages name gib_generation_round
+static int check_round_args(int B, int N, int F, int Ef, int n_atom_types, int n_charges, int n_imp_H, int n_chirality,
+                            int round) {
   // every index travels in 8 bits of the int4 record; counts <= 255 keep each index <= 254
   const bool counts_ok = n_atom_types > 0 && n_charges > 0 && Ef > 0 && n_imp_H >= 0 && n_chirality >= 0 &&
                          n_atom_types <= 255 && n_charges <= 255 && Ef <= 255 && n_imp_H <= 255 && n_chirality <= 255;
@@ -230,19 +247,69 @@ extern "C" int gib_generation_round_layout(int B, int N, int F, int Ef, int n_at
               B, N, F, n_atom_types, n_charges, n_imp_H, n_chirality, round);
     return -1;
   }
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  GenDims d{B, N, F, Ef, n_atom_types, n_charges, n_imp_H, n_chirality, 2 * N};
+  return 0;
+}
+
+// decode -> scan -> apply on the scratch layout of gib_generation_scratch_bytes: rec int4[B], flags int[B], pos int[B],
+// then the control word of gib_generation_sample_round in the 64 spare bytes
+static int launch_round(const GenDims& d, int round, const int* ctl, int* state, const int* action,
+                        const float* likelihood, float* nodes, float* edges, int* n_nodes, float* likelihoods,
+                        float* gen_nodes, float* gen_edges, signed char* gen_n_nodes, float* gen_likelihoods,
+                        signed char* properly_terminated, int capacity, int* counters, void* scratch,
+                        cudaStream_t st) {
+  const int B = d.B;
   int4* rec = reinterpret_cast<int4*>(scratch);
   int* flags = reinterpret_cast<int*>(rec + B);
   int* pos = flags + B;
-  gen_decode_kernel<<<ceil_div(B, 128), 128, 0, st>>>(d, action, edges, n_nodes, rec, flags);
+  gen_decode_kernel<<<ceil_div(B, 128), 128, 0, st>>>(d, action, edges, n_nodes, rec, flags, ctl);
   GIB_LAUNCH_CHECK();
-  gen_scan_kernel<<<1, 1024, 0, st>>>(B, flags, pos, counters, properly_terminated, capacity);
+  gen_scan_kernel<<<1, 1024, 0, st>>>(B, flags, pos, counters, properly_terminated, capacity, ctl, state, d.Lw);
   GIB_LAUNCH_CHECK();
   gen_apply_kernel<<<B, 128, 0, st>>>(d, round, rec, pos, likelihood, nodes, edges, n_nodes, likelihoods, gen_nodes,
-                                      gen_edges, gen_n_nodes, gen_likelihoods);
+                                      gen_edges, gen_n_nodes, gen_likelihoods, ctl);
   GIB_LAUNCH_CHECK();
   return 0;
+}
+
+static int* round_ctl(void* scratch, int B) {
+  return reinterpret_cast<int*>(reinterpret_cast<int4*>(scratch) + B) + 2 * B;   // behind rec, flags and pos
+}
+
+extern "C" int gib_generation_round_layout(int B, int N, int F, int Ef, int n_atom_types, int n_charges, int n_imp_H,
+                                           int n_chirality, int round, const int* action, const float* likelihood,
+                                           float* nodes, float* edges, int* n_nodes, float* likelihoods,
+                                           float* gen_nodes, float* gen_edges, signed char* gen_n_nodes,
+                                           float* gen_likelihoods, signed char* properly_terminated, int capacity,
+                                           int* counters, void* scratch, gib_stream stream) {
+  GIB_TRY(check_round_args(B, N, F, Ef, n_atom_types, n_charges, n_imp_H, n_chirality, round));
+  GenDims d{B, N, F, Ef, n_atom_types, n_charges, n_imp_H, n_chirality, 2 * N};
+  return launch_round(d, round, nullptr, nullptr, action, likelihood, nodes, edges, n_nodes, likelihoods, gen_nodes,
+                      gen_edges, gen_n_nodes, gen_likelihoods, properly_terminated, capacity, counters, scratch,
+                      reinterpret_cast<cudaStream_t>(stream));
+}
+
+extern "C" int gib_generation_sample_round(int B, int N, int F, int Ef, int n_atom_types, int n_charges, int n_imp_H,
+                                           int n_chirality, const float* logits, int apd, const float* uniforms,
+                                           int* state, int* action, float* likelihood, float* nodes, float* edges,
+                                           int* n_nodes, float* likelihoods, float* gen_nodes, float* gen_edges,
+                                           signed char* gen_n_nodes, float* gen_likelihoods,
+                                           signed char* properly_terminated, int capacity, int* counters,
+                                           void* scratch, gib_stream stream) {
+  GIB_TRY(check_round_args(B, N, F, Ef, n_atom_types, n_charges, n_imp_H, n_chirality, 0));
+  const long long want = (long long)N * n_atom_types * n_charges * (n_imp_H ? n_imp_H : 1) *
+                         (n_chirality ? n_chirality : 1) * Ef + (long long)N * Ef + 1;
+  if (apd != want) {
+    set_error("gib_generation_round: apd=%d, the action layout (N=%d A=%d CH=%d H=%d C=%d Ef=%d) has %lld actions",
+              apd, N, n_atom_types, n_charges, n_imp_H, n_chirality, Ef, want);
+    return -1;
+  }
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  GenDims d{B, N, F, Ef, n_atom_types, n_charges, n_imp_H, n_chirality, 2 * N};
+  int* ctl = round_ctl(scratch, B);
+  const RoundGate gate{state, counters, ctl, 2 * N};
+  GIB_TRY(sample_actions_launch(logits, B, apd, uniforms, action, likelihood, &gate, st));
+  return launch_round(d, 0, ctl, state, action, likelihood, nodes, edges, n_nodes, likelihoods, gen_nodes, gen_edges,
+                      gen_n_nodes, gen_likelihoods, properly_terminated, capacity, counters, scratch, st);
 }
 
 extern "C" int gib_generation_round(int B, int N, int F, int Ef, int n_atom_types, int n_charges, int round,

@@ -45,4 +45,13 @@ int emn_aggregate_bwd(float* dEMx, float* dENx, float* dEMm, float* dENm, float*
 int mul_dselu(float* G, const float* d, const float* y, long long rows, int ld, const int* live, cudaStream_t st);
 int pack_weight(float* Wp, float* WTp, float* bp, const float* W, const float* bias, long long rs, long long cs, int nblk, int Rb, int Rbp, int C, int Cp, int Ct, int Ctp, cudaStream_t st);
 
+// The categorical sampler (api.cu).  gate != null (gib_generation_sample_round, generate.cu): the round index and the
+// loop condition are read from device memory.  state = {next round, status}; a call runs when counters[0] < B,
+// status == 0 and state[0] < rounds, samples row state[0] of uniforms [rounds, B] and leaves state[0] in ctl[0]
+// (-1 when it does not run: the round kernels then do nothing).  A call that finds state[0] >= rounds while
+// counters[0] < B sets status 1.
+struct RoundGate { int* state; const int* counters; int* ctl; int rounds; };
+int sample_actions_launch(const float* out, int B, int apd, const float* uniforms, int* action, float* lik,
+                          const RoundGate* gate, cudaStream_t st);
+
 }  // namespace gib

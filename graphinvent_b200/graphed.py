@@ -17,13 +17,23 @@ content; a batch with more bond entries than `entry_capacity` is truncated and f
 
 The optimizer is stepped eagerly after the graph (its step count / learning-rate schedule are host state); with
 `optim.FlatAdam` that is one more launch.  There is no CPU path.
+
+Generation rounds as replays of ONE captured round (`GraphedGenerator`, a drop-in for `generation.GraphGenerator`):
+
+    gen = graphinvent_b200.graphed.GraphedGenerator(model, batch_size=1000)
+    graphs, flat, final, proper = gen.sample(generator=g)     # what GraphGenerator.sample returns
+
+The captured round is K0 -> forward -> `gib_generation_sample_round`, whose round index, uniforms row and stop rule
+live in device memory, so the host replays the same graph until a status copied back asynchronously says the batch
+is done; it keeps two rounds in flight and never waits on the round it just launched.
 """
 import ctypes
 
 import torch
 
 from . import functional as F
-from ._lib import FLAG_MULTITYPE, FLAG_OVERFLOW, HDR_FLAGS, check, lib
+from ._lib import FLAG_MULTITYPE, FLAG_OVERFLOW, HDR_FLAGS, HDR_INTS, check, lib
+from .generation import GraphGenerator
 
 _u8 = torch.uint8
 
@@ -193,3 +203,195 @@ class TrainStep:
         if flags & FLAG_MULTITYPE and self.d.model == F.MODEL_ID["AttGGNN"]:
             raise RuntimeError("AttentionGGNN requires one bond type per bond (as the reference's AggregationMPNN does)")
         return flags
+
+
+# ---- generation -----------------------------------------------------------------------------------------------
+def entry_capacity(batch_size, max_n_nodes, n_edge_features):
+    """bond entries a generation batch can ever hand to the model: a round adds at most one bond (two `edges`
+    non-zeros) per slot -- an add into a non-empty graph or a connect; terminate, invalid and a first atom add none,
+    terminated slots are zeroed, the never-reset dummy slot 0 starts with one self-loop and gains at most two per
+    round as well -- and a batch runs at most 2N rounds: 1 + 2 * B * 2N.  Nor can there be more non-zeros than
+    `edges` has elements.  The AttentionGGNN slot-0 view only removes entries."""
+    B, N, Ef = int(batch_size), int(max_n_nodes), int(n_edge_features)
+    return min(1 + 4 * B * N, B * N * N * Ef)
+
+
+class GraphedGenerator(GraphGenerator):
+    """`GraphGenerator` with each round a replay of one captured CUDA graph:
+
+      1. the AttentionGGNN slot-0 view (`GraphGenerator._model_inputs`) into a static copy of `edges`,
+      2. K0 (`gib_graph_count` / `gib_graph_fill`) in capacity mode at `entry_capacity(B, N, Ef)` entries, which no
+         batch can exceed,
+      3. `gib_model_forward` on a static packed-weight arena,
+      4. `gib_generation_sample_round`: sample row state[0] of `uniforms` [2N, B] and run that round; a call after the
+         batch finished (or hit the 2N-round limit) changes nothing.
+
+    Every buffer is allocated once and reset in place between batches.  After each replay the counters and the round
+    state are copied into pinned host memory and an event is recorded; before launching round r + 2 the host waits
+    for round r only, and stops once a copy shows the batch finished, so one inert round per batch is launched past
+    the end (`inert_rounds`).  With the same uniforms the results equal, bit for bit, those of the eager
+    `GraphGenerator` with the model in capacity mode at the same capacity (`model.entry_capacity =
+    gen.entry_capacity`).  Exact mode can differ in the last bits of the logits: with few bond entries it runs some
+    message GEMMs on the fp32 SIMT kernel, capacity mode always on the 3xTF32 tensor-core kernel.
+
+    The weights are re-packed into the arena (one launch per batch, not per round) whenever a parameter's storage,
+    in-place version or `functional.invalidate_packed_weights` epoch changed; the graph reads only the arena, so no
+    recapture is needed for that.  Generation with recorded actions (`replay=`) and the RL rollout, which
+    back-propagates through every round, stay with the eager generators."""
+
+    def __init__(self, model, batch_size, constants=None, n_atom_types=None, n_formal_charge=None, n_imp_H=None,
+                 n_chirality=None, device="cuda"):
+        super().__init__(model, batch_size, constants=constants, n_atom_types=n_atom_types,
+                         n_formal_charge=n_formal_charge, n_imp_H=n_imp_H, n_chirality=n_chirality, device=device)
+        if not hasattr(model, "dims"):
+            raise TypeError("GraphedGenerator runs this package's models (graphinvent_b200.gnn.mpnn) only")
+        B, N, dev = self.batch_size, self.N, self.device
+        self.params = list(model.parameters())
+        F._require_cuda(*self.params)
+        self.d = F.make_dims(model, B, 0)
+        bd = ctypes.byref(self.d)
+        F._check_params(model, self.d, self.params)
+        self.entry_capacity = entry_capacity(B, N, self.Ef)
+        self._att_view = getattr(model, "MODEL", None) == "AttGGNN"
+        self._edges_in = torch.zeros_like(self.edges) if self._att_view else self.edges
+        probe = F.GraphBatch(self.d, self._edges_in, capacity=self.entry_capacity)
+        self.cws, self.gbuf, self.hdr_np, self.hdr = probe.cws, probe.buf, probe.hdr_np, probe.hdr
+        self.packed = torch.empty(lib.gib_model_packed_bytes(bd), dtype=torch.uint8, device=dev)
+        ws_bytes = lib.gib_model_workspace_bytes(bd, self.hdr)
+        if ws_bytes == 0:
+            check(-1, "gib_model_workspace_bytes")
+        self.workspace_bytes = ws_bytes
+        self.ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
+        self.logits = torch.empty(B, self.apd, dtype=torch.float32, device=dev)
+        self.action = torch.zeros(B, dtype=torch.int32, device=dev)
+        self.lik = torch.zeros(B, dtype=torch.float32, device=dev)
+        self.uniforms = torch.zeros(2 * N, B, dtype=torch.float32, device=dev)
+        # one row per replay: counters[0..1], state[0..1], K0 flags OR-ed over the batch.  A batch launches at most
+        # 2N + 1 rounds (the last one inert)
+        self._host = torch.zeros(2 * N + 1, 5, dtype=torch.int32, pin_memory=True)
+        self._host_np = self._host.numpy()
+        self._events = [torch.cuda.Event() for _ in range(2 * N + 1)]
+        self._hdr_flags = self.cws[: HDR_INTS * 4].view(torch.int32)[HDR_FLAGS:HDR_FLAGS + 1]
+        self._packed_key = None
+        self.graph = None
+        self.inert_rounds = 0
+
+    def _allocate(self):
+        super()._allocate()
+        # counters [2], round state [2] and the batch's K0 flags in one word group: one copy back per round
+        self._ctl = torch.zeros(5, dtype=torch.int32, device=self.device)
+        self._counters, self._state, self._flags = self._ctl[0:2], self._ctl[2:4], self._ctl[4:5]
+
+    def _reset(self):
+        """initialize_graph_batch's start state (GraphGenerator._allocate), in place: the graph keeps its addresses"""
+        for t in (self.nodes, self.edges, self.n_nodes, self.likelihoods, self.generated_nodes, self.generated_edges,
+                  self.generated_n_nodes, self.generated_likelihoods, self.properly_terminated, self._ctl):
+            t.zero_()
+        self.nodes[0].fill_(1.0)                    # fill_, not __setitem__: no host scalar is copied to the device
+        self.edges[0, 0, 0, 0].fill_(1.0)
+        self.n_nodes[0].fill_(1)
+
+    def _pack(self):
+        model = self.model
+        if model.training and any(p > 0.0 for p in model._dropout_ps()):
+            raise NotImplementedError("dropout_p > 0 in training mode is not supported by the fused sm_90a path")
+        params = list(model.parameters())
+        key = (F._weights_epoch[0],) + tuple((p.data_ptr(), p._version) for p in params)
+        if key == self._packed_key:
+            return
+        if len(params) != len(self.params) or any(p.shape != q.shape for p, q in zip(params, self.params)):
+            raise RuntimeError("the model's parameter table changed after the GraphedGenerator was built")
+        F._require_cuda(*params)
+        self.params = params
+        check(lib.gib_model_pack(ctypes.byref(self.d), F._ptr_table(params), F._ptr(self.packed),
+                                 F._stream(self.device)), "gib_model_pack")
+        self._packed_key = key
+
+    # ---- the captured round -------------------------------------------------------------------------------
+    def _enqueue_round(self):
+        d, st = self.d, F._stream(self.device)
+        bd = ctypes.byref(d)
+        if self._att_view:                          # GraphGenerator._model_inputs, into the static copy
+            self._edges_in.copy_(self.edges)
+            e0 = self.edges[0]
+            nz = e0 != 0
+            self._edges_in[0].copy_(e0 * (nz & (nz.to(torch.int32).cumsum(-1) == 1)).to(e0.dtype))
+        edges = self._edges_in
+        check(lib.gib_graph_count(bd, F._ptr(edges), F._ptr(self.cws), st), "gib_graph_count")
+        check(lib.gib_graph_fill(bd, F._ptr(edges), F._ptr(self.cws), self.hdr, F._ptr(self.gbuf), st),
+              "gib_graph_fill")
+        self._flags.bitwise_or_(self._hdr_flags)
+        check(lib.gib_model_forward(bd, self.hdr, F._ptr(self.nodes), F._ptr(edges), F._ptr(self.gbuf),
+                                    F._ptr(self.packed), F._ptr(self.ws), F._ptr(self.logits), st), "gib_model_forward")
+        check(lib.gib_generation_sample_round(
+            self.batch_size, self.N, self.F, self.Ef, self.A, self.CH, self.n_imp_H, self.n_chirality,
+            F._ptr(self.logits), self.apd, F._ptr(self.uniforms), F._ptr(self._state), F._ptr(self.action),
+            F._ptr(self.lik), F._ptr(self.nodes), F._ptr(self.edges), F._ptr(self.n_nodes), F._ptr(self.likelihoods),
+            F._ptr(self.generated_nodes), F._ptr(self.generated_edges), F._ptr(self.generated_n_nodes),
+            F._ptr(self.generated_likelihoods), F._ptr(self.properly_terminated), self.capacity,
+            F._ptr(self._counters), F._ptr(self._scratch), st), "gib_generation_sample_round")
+
+    def capture(self):
+        """warm up outside capture (lazy per-device init, function attributes), then capture one round"""
+        dev = self.device
+        side = torch.cuda.Stream(dev)
+        side.wait_stream(torch.cuda.current_stream(dev))
+        with torch.cuda.stream(side):
+            self._enqueue_round()
+        torch.cuda.current_stream(dev).wait_stream(side)
+        torch.cuda.synchronize(dev)
+        g = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(g):
+            self._enqueue_round()
+        self.graph = g
+
+    # ---- one batch ----------------------------------------------------------------------------------------
+    @torch.no_grad()
+    def build_graphs(self, generator=None, uniforms=None):
+        """uniforms: optional [2N, batch_size] draws, row r feeding round r (instead of torch.rand(2N, B,
+        generator=generator)); returns the number of finished molecules (may exceed batch_size, as in the reference)"""
+        B, N = self.batch_size, self.N
+        if uniforms is not None and tuple(uniforms.shape) != (2 * N, B):
+            raise ValueError(f"uniforms must have shape [2*max_n_nodes, batch_size] = [{2 * N}, {B}]")
+        self._pack()
+        if self.graph is None:
+            self.capture()
+        self._reset()
+        if uniforms is not None:
+            self.uniforms.copy_(uniforms)
+        else:
+            torch.rand(2 * N, B, generator=generator, device=self.device, out=self.uniforms)
+        rows, events, cur = self._host_np, self._events, torch.cuda.current_stream(self.device)
+        i = 0
+        while True:
+            if i >= 2:                              # round i - 2 has ended: is the batch done?
+                events[i - 2].synchronize()
+                if rows[i - 2, 0] >= B or rows[i - 2, 3] != 0:
+                    break
+            if i == len(events):
+                raise RuntimeError("GraphedGenerator: the round state did not stop the batch after 2N rounds")
+            self.graph.replay()
+            self._host[i].copy_(self._ctl, non_blocking=True)
+            events[i].record(cur)
+            i += 1
+        events[i - 1].synchronize()
+        n_generated, _, rounds, status, flags = (int(v) for v in rows[i - 1])
+        self.rounds, self.inert_rounds = rounds, i - rounds
+        if flags & FLAG_OVERFLOW:
+            raise RuntimeError(f"a generation round held more than {self.entry_capacity} bond entries: the static "
+                               "entry capacity is wrong, the batch is invalid")
+        if flags & FLAG_MULTITYPE and self._att_view:
+            raise RuntimeError("AttentionGGNN requires one bond type per bond (as the reference's AggregationMPNN does)")
+        if status != 0:
+            raise RuntimeError("generation needs more than 2*max_n_nodes rounds: the per-slot likelihood buffer "
+                               "(GraphGenerator.py:173, 'the 2 is arbitrary') would overflow, as in the reference")
+        return n_generated
+
+    def sample(self, generator=None, uniforms=None):
+        """what GraphGenerator.sample returns, as copies: the static buffers are overwritten by the next batch"""
+        self.build_graphs(generator=generator, uniforms=uniforms)
+        B = self.batch_size
+        final = torch.log(self.generated_likelihoods.sum(dim=1)[:B])
+        flat = self.generated_likelihoods[self.generated_likelihoods != 0]
+        graphs = (self.generated_nodes[:B].clone(), self.generated_edges[:B].clone(), self.generated_n_nodes[:B].clone())
+        return graphs, flat, final, self.properly_terminated[:B].clone()

@@ -348,6 +348,20 @@ int gib_generation_round_layout(int B, int N, int F, int Ef, int n_atom_types, i
                                 float* gen_edges, signed char* gen_n_nodes, float* gen_likelihoods,
                                 signed char* properly_terminated, int capacity, int* counters, void* scratch,
                                 gib_stream stream);
+/* One sample-and-round step with the round index, the stop rule and the uniforms read on the device (a CUDA-graph
+ * capturable round: the launch parameters never change between rounds).
+ * state (device, int[2]): [0] = index of the next round, [1] = status: 0 running, 1 round limit
+ * (a round 2N would be needed while counters[0] < B).  A call whose start finds counters[0] >= B or
+ * status != 0 changes nothing (an "inert" round); otherwise it samples row state[0] of `uniforms`
+ * ([2N, B], inverse CDF as gib_sample_actions) from `logits` [B, apd] into action / likelihood [B], runs the round at
+ * that index exactly as gib_generation_round_layout does, and increments state[0].  apd must be the layout's action
+ * count; the other arguments are validated as gib_generation_round_layout validates them. */
+int gib_generation_sample_round(int B, int N, int F, int Ef, int n_atom_types, int n_charges, int n_imp_H,
+                                int n_chirality, const float* logits, int apd, const float* uniforms, int* state,
+                                int* action, float* likelihood, float* nodes, float* edges, int* n_nodes,
+                                float* likelihoods, float* gen_nodes, float* gen_edges, signed char* gen_n_nodes,
+                                float* gen_likelihoods, signed char* properly_terminated, int capacity,
+                                int* counters, void* scratch, gib_stream stream);
 
 /* ---- measurement hooks: CUDA-event timing per kernel class on the launching stream.
  *      class 0 = forward/dX launches of the tensor-core kernel, 1 = its weight-gradient launches, 2 = scatter-aggregate (K2),

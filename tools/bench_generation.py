@@ -1,7 +1,7 @@
 """C5 (BASELINE.json configs[4]): `GraphGenerator.sample`, EMN model, 100 k molecules over 8 GPUs -- generation is
 embarrassingly parallel: N independent replicas with distinct seeds, no data-path collective.
 
-    python tools/bench_generation.py [--model EMN] [--molecules 12500] [--batch 1000]
+    python tools/bench_generation.py [--model EMN] [--molecules 12500] [--batch 1000] [--impl eager|graphed|both]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node 8 --master-addr 127.0.0.1 --master-port 29511 \
            tools/bench_generation.py --molecules 12500          # 8 x 12 500 = 100 000 molecules
 
@@ -10,13 +10,21 @@ seeded recipe: reference initialisers under torch.manual_seed(0), `--train-steps
 (lr 3e-4) on the 256 recorded real rows of gdb13_1K/train.h5 (tests/golden/gdb13_rows.npz), through this package's
 training step.  `--checkpoint` loads a reference .pth instead (e.g. the shipped GGNN one with --model GGNN).
 
-One JSON line (rank 0): molecules/s per GPU and in total (device-timed per replica, max over ranks), rounds, mean
-atoms, fraction properly terminated; `cpu_reference` = the unmodified reference `GraphGenerator.build_graphs` with the
-same weights on this host's cores for ONE batch (bounded sample), when oracle/_ref holds the reference modules.
+Implementations.  `--impl eager` is `generation.GraphGenerator` (two blocking reads per round), `graphed` is
+`graphed.GraphedGenerator` (each round a replay of one captured CUDA graph, the stop rule on the device); `both`
+alternates eager and graphed batches in one process with the same weights and batch size, so that clock and power
+drift hit both alike.  Each batch is timed with CUDA events around its `build_graphs` call.
+
+One JSON line (rank 0): per implementation molecules/s per GPU and in total (max over ranks), rounds and inert
+rounds (graphed rounds launched past the end of a batch) per batch, mean atoms, fraction properly terminated; the
+card name, power limit and SM clock read from nvidia-smi in the same call; `cpu_reference` = the unmodified reference
+`GraphGenerator.build_graphs` with the same weights on this host's cores for ONE batch (bounded sample), when
+oracle/_ref holds the reference modules.
 """
 import argparse
 import json
 import os
+import subprocess
 import sys
 import time
 import types
@@ -117,6 +125,17 @@ def cpu_reference_generation(C, state_dict, batch, model_name):
             "seed": seed, "failed_seeds": failed}
 
 
+def gpu_info(index):
+    """name, power limit and SM clock of the card, as nvidia-smi reports them now (None without nvidia-smi)"""
+    try:
+        out = subprocess.run(["nvidia-smi", "-i", str(index), "--query-gpu=name,power.limit,clocks.sm",
+                              "--format=csv,noheader"], capture_output=True, text=True, timeout=30).stdout.strip()
+    except (OSError, subprocess.SubprocessError):
+        return None
+    parts = [x.strip() for x in out.split(",")]
+    return dict(zip(("name", "power_limit", "sm_clock"), parts)) if len(parts) == 3 else {"raw": out}
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--model", default="EMN", choices=["EMN", "GGNN", "MNN", "AttGGNN"])
@@ -125,6 +144,7 @@ def main():
     ap.add_argument("--train-steps", type=int, default=300)
     ap.add_argument("--checkpoint", default=None)
     ap.add_argument("--no-cpu", action="store_true")
+    ap.add_argument("--impl", default="eager", choices=["eager", "graphed", "both"])
     args = ap.parse_args()
     world = int(os.environ.get("WORLD_SIZE", "1"))
     rank = int(os.environ.get("RANK", "0"))
@@ -136,6 +156,7 @@ def main():
         dist.init_process_group("nccl", device_id=dev)      # measurement plumbing only (barrier + max of the timings)
 
     from graphinvent_b200.generation import GraphGenerator
+    from graphinvent_b200.graphed import GraphedGenerator
     t_train0 = time.perf_counter()
     C, net, train_loss = train_weights(args.model, 0 if args.checkpoint else args.train_steps, dev)
     if args.checkpoint:
@@ -143,45 +164,68 @@ def main():
     torch.cuda.synchronize()
     t_train = time.perf_counter() - t_train0
 
-    g = torch.Generator(device=dev).manual_seed(1000 + rank)          # distinct sampling streams per replica
-    gen = GraphGenerator(net, batch_size=args.batch, n_atom_types=5, n_formal_charge=3, device=dev)
-    gen.build_graphs(generator=g)                                     # warm-up batch
+    impls = ["eager", "graphed"] if args.impl == "both" else [args.impl]
+    cls = {"eager": GraphGenerator, "graphed": GraphedGenerator}
+    gens, rngs = {}, {}
+    for k, name in enumerate(impls):
+        rngs[name] = torch.Generator(device=dev).manual_seed(1000 + 100 * k + rank)   # distinct streams per replica
+        gens[name] = cls[name](net, batch_size=args.batch, n_atom_types=5, n_formal_charge=3, device=dev)
+        gens[name].build_graphs(generator=rngs[name])                 # warm-up batch (graphed: the capture)
     torch.cuda.synchronize()
     if world > 1:
         dist.barrier()
-    done, rounds, atoms, proper = 0, 0, 0.0, 0.0
-    ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    ev0.record()
+    B = args.batch
+    events = {name: [] for name in impls}
+    # per implementation: batches, rounds, inert rounds, atoms, properly terminated
+    acc = {name: [0.0] * 5 for name in impls}
+    done = 0
     while done < args.molecules:
-        gen.build_graphs(generator=g)
-        B = args.batch
-        done += B                                                     # sample() hands out the first batch_size graphs
-        rounds += gen.rounds
-        atoms += float(gen.generated_n_nodes[:B].float().sum())
-        proper += float(gen.properly_terminated[:B].float().sum())
-    ev1.record()
+        for name in impls:
+            gen = gens[name]
+            ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            ev0.record()
+            gen.build_graphs(generator=rngs[name])
+            ev1.record()
+            events[name].append((ev0, ev1))
+            a = acc[name]
+            a[0] += 1
+            a[1] += gen.rounds
+            a[2] += getattr(gen, "inert_rounds", 0)
+            a[3] += float(gen.generated_n_nodes[:B].float().sum())   # sample() hands out the first batch_size graphs
+            a[4] += float(gen.properly_terminated[:B].float().sum())
+        done += B
     torch.cuda.synchronize()
-    ms = ev0.elapsed_time(ev1)
-    stats = torch.tensor([ms, done, rounds, atoms, proper], dtype=torch.float64, device=dev)
-    if world > 1:
-        mx = stats.clone()
-        dist.all_reduce(mx, op=dist.ReduceOp.MAX)
-        dist.all_reduce(stats, op=dist.ReduceOp.SUM)
-        ms_max = float(mx[0])
-    else:
+    results = {}
+    for name in impls:
+        ms = sum(e0.elapsed_time(e1) for e0, e1 in events[name])
+        batches, rounds, inert, atoms, proper = acc[name]
+        stats = torch.tensor([ms, batches * B, rounds, inert, atoms, proper], dtype=torch.float64, device=dev)
         ms_max = ms
-    if rank == 0:
+        if world > 1:
+            mx = stats.clone()
+            dist.all_reduce(mx, op=dist.ReduceOp.MAX)
+            dist.all_reduce(stats, op=dist.ReduceOp.SUM)
+            ms_max = float(mx[0])
         total = float(stats[1])
+        n_batches = total / B
+        results[name] = {"value": total / (ms_max / 1e3), "unit": "molecules/s",
+                         "per_gpu": total / world / (ms_max / 1e3), "molecules": int(total), "seconds": ms_max / 1e3,
+                         "rounds_per_batch": float(stats[2]) / n_batches,
+                         "inert_rounds_per_batch": float(stats[3]) / n_batches,
+                         "mean_atoms": float(stats[4]) / total, "properly_terminated": float(stats[5]) / total}
+    if rank == 0:
+        main_impl = impls[-1]
         line = {"metric": f"generated molecules/s ({args.model}, GraphGenerator.sample, device-side rounds)",
-                "value": total / (ms_max / 1e3), "unit": "molecules/s", "n_gpus": world,
-                "per_gpu": total / world / (ms_max / 1e3), "molecules": int(total), "batch": args.batch,
-                "seconds": ms_max / 1e3, "parallelism": f"{world} independent replicas, distinct seeds, no collective",
-                "rounds_per_batch": float(stats[2]) / (total / args.batch), "mean_atoms": float(stats[3]) / total,
-                "properly_terminated": float(stats[4]) / total, "data": "synthetic (sampled)",
+                "value": results[main_impl]["value"], "unit": "molecules/s", "impl": args.impl,
+                "n_gpus": world, "batch": args.batch, "impls": results, "gpu": gpu_info(local),
+                "parallelism": f"{world} independent replicas, distinct seeds, no collective",
+                "data": "synthetic (sampled)",
                 "weights": (f"checkpoint {args.checkpoint}" if args.checkpoint else
                             f"seeded recipe: {args.train_steps} Adam steps (lr 3e-4) on 256 real gdb13 rows, final loss {train_loss:.4f}, {t_train:.1f} s"),
                 "config": {"workload": "GraphGenerator.sample 100k-molecule batched generation, EMN model, 8xH100 embarrassingly parallel",
                            "name": "C5"}}
+        if "graphed" in results and "eager" in results:
+            line["graphed_over_eager"] = results["graphed"]["value"] / results["eager"]["value"]
         if getattr(train_weights, "trajectory", None):
             line["train_loss_trajectory"] = train_weights.trajectory
         if not args.no_cpu:
