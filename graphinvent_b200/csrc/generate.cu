@@ -101,7 +101,9 @@ __global__ void gen_decode_kernel(GenDims d, const int* __restrict__ action, con
   }
   rec[b] = make_int4(kind | (invalid << 4), bond_to | (bond_from << 8), atom | (charge << 8),
                      btype | (imp_h << 8) | (chir << 16));
-  flags[b] = (kind == ACT_TERM ? 1 : 0) | (invalid ? 2 : 0);
+  // one class per slot: an index outside the APD decodes as kind TERM but counts once, as invalid (the scan gives every
+  // flagged slot one output row; counting it in both classes left a row unwritten and over-counted n_generated)
+  flags[b] = invalid ? 2 : (kind == ACT_TERM ? 1 : 0);
 }
 
 // single CTA: output positions of the slots that terminate this round + counters

@@ -74,7 +74,7 @@ class GraphGenerator:
         self.generated_nodes, self.generated_edges = z(cap, N, F), z(cap, N, N, Ef)
         self.generated_n_nodes = z(cap, dt=torch.int8)
         self.likelihoods, self.generated_likelihoods = z(B, 2 * N), z(cap, 2 * N)
-        self.properly_terminated = z(cap, dt=torch.int8)
+        self.properly_terminated = z(cap, dt=torch.int8)     # must start zeroed: the rounds only set flags to 1
         self._counters = z(2, dt=torch.int32)
         self._scratch = torch.empty(lib.gib_generation_scratch_bytes(B), dtype=torch.uint8, device=dev)
 

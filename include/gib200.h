@@ -335,7 +335,10 @@ int gib_sample_actions(const float* out, int B, int apd, const float* uniforms, 
  *      atom's chirality index 0 when both segments are present); an add into a full graph terminates as invalid.
  *      gib_generation_round is this entry point with n_imp_H = n_chirality = 0 (the gdb13 layout).
  *      State: nodes [B,N,F] f32, edges [B,N,N,Ef] f32, n_nodes [B] i32, likelihoods [B,2N] f32; outputs
- *      gen_* with `capacity` rows; counters[0] = n_generated (in/out), counters[1] = graphs written this round. ---- */
+ *      gen_* with `capacity` rows; counters[0] = n_generated (in/out), counters[1] = graphs written this round.
+ *      An action index outside [0, apd) terminates its slot as invalid and edits nothing.  Output rows at or past
+ *      `capacity` are counted in n_generated but not written.  `scratch` and the gen_* rows may hold anything;
+ *      `properly_terminated` must be zeroed by the caller before the first round (the rounds only set flags to 1). ---- */
 size_t gib_generation_scratch_bytes(int B);
 int gib_generation_round(int B, int N, int F, int Ef, int n_atom_types, int n_charges, int round,
                          const int* action, const float* likelihood, float* nodes, float* edges, int* n_nodes,
