@@ -66,6 +66,7 @@ _PROTOS = {
     "gib_model_pack": (c_i, [c_p, c_p, c_p, c_p]),
     "gib_model_workspace_bytes": (c_sz, [c_p, c_p]),
     "gib_model_forward": (c_i, [c_p] * 9),
+    "gib_model_msg_rows": (c_p, [c_p, c_p, c_p, c_i]),
     "gib_model_bwd_scratch_bytes": (c_sz, [c_p, c_p]),
     "gib_model_backward": (c_i, [c_p] * 12),
     "gib_model_backward_part": (c_i, [c_p] * 11 + [c_i, c_p]),

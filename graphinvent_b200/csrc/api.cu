@@ -263,6 +263,14 @@ int gib_model_forward(const gib_dims* d, const int* hdr, const void* nodes, cons
   r.st = ST(stream);
   return model_forward(r, out);
 }
+void* gib_model_msg_rows(const gib_dims* d, const int* hdr, void* workspace, int which) {
+  Run r;
+  if (make_run(*d, hdr, r) || d->model == GIB_EMN || d->model == GIB_ATTGGNN) return nullptr;
+  const size_t offs[10] = {r.L.mr_src, r.L.mr_w, r.L.mr_ptr, r.L.mr_dst, r.L.mr_ent, r.L.mr_dst_u, r.L.mr_sptr,
+                           r.L.mr_su, r.L.mr_meta, r.L.mr_tmp};
+  if (which < 0 || which >= 10) return nullptr;
+  return reinterpret_cast<float*>(workspace) + offs[which];
+}
 size_t gib_model_bwd_scratch_bytes(const gib_dims* d, const int* hdr) {
   Run r;
   if (make_run(*d, hdr, r)) return 0;

@@ -580,6 +580,8 @@ int gemm_dw_group(const GemmDW* qs, int n, long long plan_rows, cudaStream_t st)
   bool dyn = false;
   long long rows = 0;
   double work = 0;
+  ProfRows dyn_rows[kTc3MaxProblems];
+  int ndyn = 0;
   GemmDW live[kTc3MaxProblems];      // members that run in the grouped tensor-core launch
   GemmDW rest[kTc3MaxProblems];      // too small / unaligned for it: one by one
   int nl = 0, nr = 0;
@@ -598,7 +600,9 @@ int gemm_dw_group(const GemmDW* qs, int n, long long plan_rows, cudaStream_t st)
     }
     if (good) {
       rows += q.M;
-      work += q.work > 0 ? q.work : 2.0 * q.M * (double)q.R * q.C;
+      const double qw = q.work > 0 ? q.work : 2.0 * q.M * (double)q.R * q.C;
+      if (q.m_dev) dyn_rows[ndyn++] = ProfRows{q.m_dev, q.base_dev, q.M, qw / q.M};   // the rows launched
+      else work += qw;
       live[nl++] = q;
     } else {
       rest[nr++] = q;
@@ -610,7 +614,7 @@ int gemm_dw_group(const GemmDW* qs, int n, long long plan_rows, cudaStream_t st)
   }
   for (int i = 0; i < nr; ++i) GIB_TRY(gemm_dw(rest[i], st));
   if (nl == 0) return 0;
-  ProfScope prof(PROF_GEMM_DW, work, st);
+  ProfScope prof(PROF_GEMM_DW, work, st, dyn_rows, ndyn);
   DwSide* d;
   GIB_TRY(dw_side(&d));
   const int half = (int)(d->calls++ & 1);

@@ -1036,6 +1036,8 @@ static int launch_nt(const GemmNT* ps, const int* dep, int n, int* flags, bool r
   Params P;
   memset(&P, 0, sizeof(P));
   double work = 0;
+  ProfRows dyn[MAXP];
+  int ndyn = 0;
   long long tiles = 0;
   int np = 0;
   int spec = -1;
@@ -1071,7 +1073,9 @@ static int launch_nt(const GemmNT* ps, const int* dep, int n, int* flags, bool r
     }
     slot[i] = np;
     tiles += (long long)ceil_div(p.M, BM) * P.n_tiles[np];      // upper bound when the row count lives on the device
-    work += p.work > 0 ? p.work : 2.0 * p.M * (double)p.N * p.K;
+    const double pw = p.work > 0 ? p.work : 2.0 * p.M * (double)p.N * p.K;
+    if (p.m_dev) dyn[ndyn++] = ProfRows{p.m_dev, p.base_dev, p.M, pw / p.M};   // the rows launched, not the capacity
+    else work += pw;
     ++np;
   }
   if (np == 0) return 0;
@@ -1082,7 +1086,7 @@ static int launch_nt(const GemmNT* ps, const int* dep, int n, int* flags, bool r
     GIB_CUDA_TRY(cudaMemsetAsync(flags, 0, (size_t)flag_ints * sizeof(int), st));
   }
   const int grid = (int)(tiles < num_sms ? tiles : num_sms);
-  ProfScope prof(PROF_GEMM_NT, work, st);
+  ProfScope prof(PROF_GEMM_NT, work, st, dyn, ndyn);
   if (raw) {
     switch (spec) {
       case EPI_SPEC_SELU: tc3_gemm_kernel<EPI_SPEC_SELU><<<grid, NUM_THREADS, SMEM_BYTES, st>>>(maps, P); break;

@@ -286,4 +286,209 @@ int graph_fill(const void* edges, int in_dtype, int B, int N, int Ef, int by_typ
   return 0;
 }
 
+// ---------------------------------------------------------------------------------
+// message-row table (graph.cuh: MsgRows): count / scan / fill / finish, like K0 -- one CTA per molecule counts and
+// fills, one CTA scans over molecules, no atomics.  Every index written is bounded by the array it goes to, so a
+// capacity-mode batch that overflowed (flagged by K0, results invalid) stays inside the buffers.
+// ---------------------------------------------------------------------------------
+struct TypeBases { int tb[5]; };
+
+__device__ __forceinline__ int type_of_row(int p, const int* tb, int G) {
+  int t = G - 1;
+  while (t > 0 && p < tb[t]) --t;
+  return t;
+}
+
+// a source-CSR position that lists a kept entry (capacity mode: K0 writes row 0 for an entry it dropped)
+__device__ __forceinline__ bool listed(const GraphArrays& ga, int e, int s) { return __ldg(ga.ent_src + e) == s; }
+
+// entries of source slot s per type: m1 with w == 1 (one shared row), nn with another value (one row each)
+__device__ __forceinline__ void slot_counts(int s, const GraphArrays& ga, const int* tb, int G, int* m1, int* nn) {
+  for (int t = 0; t < 4; ++t) m1[t] = nn[t] = 0;
+  const int q1 = __ldg(ga.src_ptr + s + 1);
+  for (int q = __ldg(ga.src_ptr + s); q < q1; ++q) {
+    const int e = __ldg(ga.src_ent + q);
+    if (!listed(ga, e, s)) continue;
+    const int t = type_of_row(e, tb, G);
+    if (__ldg(ga.ent_w + e) == 1.f) ++m1[t];
+    else ++nn[t];
+  }
+}
+
+__device__ __forceinline__ void load_bases(int* tb, const int* dev_hdr, const TypeBases& hb, int G) {
+  if (threadIdx.x <= (unsigned)G) tb[threadIdx.x] = dev_hdr ? dev_hdr[HDR_TYPE_BASE + threadIdx.x] : hb.tb[threadIdx.x];
+  __syncthreads();
+}
+
+// tmp layout: molU[(G+1) B] (g == G: all types), molE[G B], offU[(G+1) B], offE[G B]
+size_t msg_rows_tmp_ints(int B, int G) { return (size_t)(4 * G + 2) * B; }
+
+__global__ void __launch_bounds__(128) mr_count_kernel(GraphArrays ga, MsgRows mr, const int* __restrict__ dev_hdr,
+                                                       TypeBases hb, int N, int B, int G, int P) {
+  __shared__ int sm[8];
+  __shared__ int tb[5];
+  for (long long p = (long long)blockIdx.x * 128 + threadIdx.x; p < P; p += (long long)gridDim.x * 128) mr.ent_u[p] = -1;
+  load_bases(tb, dev_hdr, hb, G);
+  const int b = blockIdx.x;
+  int su[5] = {0, 0, 0, 0, 0}, se[4] = {0, 0, 0, 0};
+  for (int i = threadIdx.x; i < N; i += 128) {
+    int m1[4], nn[4];
+    slot_counts(b * N + i, ga, tb, G, m1, nn);
+    for (int t = 0; t < G; ++t) {
+      const int u = (m1[t] > 0) + nn[t];
+      su[t] += u; su[4] += u; se[t] += m1[t] + nn[t];
+    }
+  }
+  int* molU = mr.tmp;
+  int* molE = molU + (size_t)(G + 1) * B;
+  for (int g = 0; g <= G; ++g) {
+    int tot;
+    block_exscan<128>(g < G ? su[g] : su[4], sm, &tot);
+    if (threadIdx.x == 0) molU[(size_t)g * B + b] = tot;
+    if (g < G) {
+      block_exscan<128>(se[g], sm, &tot);
+      if (threadIdx.x == 0) molE[(size_t)g * B + b] = tot;
+    }
+  }
+}
+
+__global__ void __launch_bounds__(1024) mr_scan_kernel(MsgRows mr, const int* __restrict__ dev_hdr, TypeBases hb, int B,
+                                                       int G) {
+  __shared__ int sm[34];
+  __shared__ int tb[5];
+  if (threadIdx.x < MR_META_INTS) mr.meta[threadIdx.x] = 0;   // the words of absent types (ordered by the barrier)
+  load_bases(tb, dev_hdr, hb, G);
+  const int* molU = mr.tmp;
+  const int* molE = molU + (size_t)(G + 1) * B;
+  int* offU = mr.tmp + (size_t)(2 * G + 1) * B;
+  int* offE = offU + (size_t)(G + 1) * B;
+  const int L = ceil_div(B, 1024);
+  const int lo = min(B, (int)threadIdx.x * L), hi = min(B, lo + L);
+  int eoff = 0;
+  for (int k = 0; k <= 2 * G; ++k) {      // k < G: rows of type k; k == G: rows of all types; k > G: entries of type k-G-1
+    const bool rows = k <= G;
+    const int g = rows ? k : k - G - 1;
+    const int* cnt = (rows ? molU : molE) + (size_t)g * B;
+    int* off = (rows ? offU : offE) + (size_t)g * B;
+    int s = 0;
+    for (int b = lo; b < hi; ++b) s += cnt[b];
+    int tot;
+    int run = block_exscan<1024>(s, sm, &tot);
+    for (int b = lo; b < hi; ++b) { off[b] = run; run += cnt[b]; }
+    if (threadIdx.x == 0) {
+      if (k < G) mr.meta[MR_COUNT + g] = max(0, min(tot, tb[g + 1] - tb[g]));   // an overflowing batch: no group spills
+      else if (k == G) mr.meta[MR_TOTAL] = tot;
+      else { mr.meta[MR_EOFF + g] = eoff; eoff += tot; }
+    }
+  }
+  if (threadIdx.x <= (unsigned)G) mr.meta[MR_BASE + threadIdx.x] = tb[threadIdx.x];
+  if (threadIdx.x == 0) mr.meta[MR_EOFF + G] = eoff;
+}
+
+__global__ void __launch_bounds__(128) mr_fill_kernel(GraphArrays ga, MsgRows mr, int N, int B, int G, int E, int P) {
+  __shared__ int sm[8];
+  __shared__ int meta[MR_META_INTS];
+  if (threadIdx.x < MR_META_INTS) meta[threadIdx.x] = mr.meta[threadIdx.x];
+  __syncthreads();
+  const int* tb = meta + MR_BASE;
+  const int b = blockIdx.x;
+  const int* offU = mr.tmp + (size_t)(2 * G + 1) * B;
+  const int* offE = offU + (size_t)(G + 1) * B;
+  // each thread owns a contiguous run of the molecule's slots (N <= 181: at most two)
+  const int L = ceil_div(N, 128);
+  const int lo = min(N, (int)threadIdx.x * L), hi = min(N, lo + L);
+  int runU[5], runE[4];
+  for (int g = 0; g <= G; ++g) {
+    int su = 0, se = 0;
+    for (int i = lo; i < hi; ++i) {
+      int m1[4], nn[4];
+      slot_counts(b * N + i, ga, tb, G, m1, nn);
+      if (g < G) { su += (m1[g] > 0) + nn[g]; se += m1[g] + nn[g]; }
+      else for (int t = 0; t < G; ++t) su += (m1[t] > 0) + nn[t];
+    }
+    int tot;
+    runU[g] = offU[(size_t)g * B + b] + block_exscan<128>(su, sm, &tot);
+    if (g < G) runE[g] = meta[MR_EOFF + g] + offE[(size_t)g * B + b] + block_exscan<128>(se, sm, &tot);
+  }
+  for (int i = lo; i < hi; ++i) {
+    const int s = b * N + i;
+    int m1[4], nn[4];
+    slot_counts(s, ga, tb, G, m1, nn);
+    mr.s_ptr[s] = min(E, runU[G]);
+    const int q0 = __ldg(ga.src_ptr + s), q1 = __ldg(ga.src_ptr + s + 1);
+    for (int t = 0; t < G; ++t) {
+      const int has1 = m1[t] > 0, r0 = runU[t], p0 = runE[t];
+      auto row_of = [&](int local) { return local < meta[MR_COUNT + t] ? tb[t] + local : -1; };
+      // rows of (s, t): the shared row first, then one per other entry; s_u lists them in the same order
+      for (int k = 0; k < has1 + nn[t]; ++k) {
+        const int row = row_of(r0 + k);
+        if (row >= 0 && row < P) mr.u_ptr[row] = min(E, p0 + (k == 0 || !has1 ? k : m1[t] + k - 1));
+        if (runU[G] + k < E) mr.s_u[runU[G] + k] = row < P ? row : -1;
+      }
+      int k1 = 0, kn = 0;
+      for (int q = q0; q < q1; ++q) {
+        const int e = __ldg(ga.src_ent + q);
+        if (!listed(ga, e, s) || type_of_row(e, tb, G) != t) continue;
+        const float w = __ldg(ga.ent_w + e);
+        const bool shared = w == 1.f;
+        const int local = shared ? r0 : r0 + has1 + kn;
+        const int pos = shared ? p0 + k1 : p0 + m1[t] + kn;
+        k1 += shared; kn += !shared;
+        const int row = row_of(local);
+        if (row >= 0 && row < P) {
+          mr.u_src[row] = s;
+          mr.u_w[row] = w;
+          mr.ent_u[e] = row;
+        }
+        if (pos < E) mr.u_dst[pos] = __ldg(ga.ent_dst + e);
+      }
+      runU[t] += has1 + nn[t];
+      runE[t] += m1[t] + nn[t];
+      runU[G] += has1 + nn[t];
+    }
+  }
+}
+
+// pad rows, the closing CSR pointers, dst_u, and the unused tails of the E-sized arrays
+__global__ void mr_finish_kernel(GraphArrays ga, MsgRows mr, long long S, int G, int E, int P) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  const int* meta = mr.meta;
+  const int* tb = meta + MR_BASE;
+  if (i < P) {
+    const int p = (int)i, t = type_of_row(p, tb, G);
+    if (p >= tb[t] + meta[MR_COUNT + t] || p >= tb[G]) {   // (type_of_row: p >= tb[t])
+      mr.u_src[p] = -1;
+      mr.u_w[p] = 0.f;
+      mr.u_ptr[p] = min(E, meta[MR_EOFF + t + 1]);
+    }
+  }
+  if (i < E) {
+    const int q = (int)i;
+    mr.dst_u[q] = q < __ldg(ga.dst_ptr + S) ? mr.ent_u[__ldg(ga.dst_ent + q)] : -1;
+    if (q >= meta[MR_EOFF + G]) mr.u_dst[q] = -1;
+    if (q >= meta[MR_TOTAL]) mr.s_u[q] = -1;
+  }
+  if (i == 0) {
+    mr.u_ptr[P] = min(E, meta[MR_EOFF + G]);
+    mr.s_ptr[S] = min(E, meta[MR_TOTAL]);
+  }
+}
+
+int msg_rows_build(const GraphArrays& ga, const MsgRows& mr, const int* dev_hdr, const int* tb, int B, int N, int G,
+                   int E, int P, cudaStream_t st) {
+  if (G < 1 || G > 4 || B < 1) { set_error("msg_rows_build: %d bond-type groups, %d molecules", G, B); return -1; }
+  TypeBases hb{};
+  for (int g = 0; g <= G; ++g) hb.tb[g] = dev_hdr ? 0 : tb[g];
+  mr_count_kernel<<<B, 128, 0, st>>>(ga, mr, dev_hdr, hb, N, B, G, P);
+  GIB_LAUNCH_CHECK();
+  mr_scan_kernel<<<1, 1024, 0, st>>>(mr, dev_hdr, hb, B, G);
+  GIB_LAUNCH_CHECK();
+  mr_fill_kernel<<<B, 128, 0, st>>>(ga, mr, N, B, G, E, P);
+  GIB_LAUNCH_CHECK();
+  const long long n = (P > E ? P : E) + 1;
+  mr_finish_kernel<<<(unsigned)ceil_div_ll(n, 256), 256, 0, st>>>(ga, mr, (long long)B * N, G, E, P);
+  GIB_LAUNCH_CHECK();
+  return 0;
+}
+
 }  // namespace gib

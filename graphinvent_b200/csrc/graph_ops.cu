@@ -214,11 +214,15 @@ template <int HINT> __device__ __forceinline__ void st_row(float4* p, const floa
 // SLOTS slots per thread, interleaved level by level (row pointers of all slots, then their entry indices, then their
 // message rows) so that a thread has SLOTS x 4 row reads in flight instead of 4: the kernel is latency-bound (ncu:
 // 77 % of the warps resident, DRAM 51 % busy), each extra independent load chain hides one more round trip.
+// Y != null: the backward of the message rows (seg_reduce_dact) instead of an aggregate -- out[s] = row_w[s] * acc *
+// act'(Y[s]), and an empty segment (a pad row) is written as exact 0 without reading Y.
 template <int SLOTS, int HINT>
 __global__ void __launch_bounds__(256) scatter_sum_kernel(float4* __restrict__ out, const float4* __restrict__ msg,
                                                           int ld4, const int* __restrict__ ptr,
                                                           const int* __restrict__ ent, const float* __restrict__ w,
-                                                          int accumulate, long long S, long long slots_per_pass) {
+                                                          int accumulate, long long S, long long slots_per_pass,
+                                                          const float* __restrict__ row_w,
+                                                          const float4* __restrict__ Y, int act) {
   const long long idx0 = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (idx0 >= slots_per_pass * ld4) return;
   const long long s0 = idx0 / ld4;
@@ -271,30 +275,54 @@ __global__ void __launch_bounds__(256) scatter_sum_kernel(float4* __restrict__ o
   }
 #pragma unroll
   for (int k = 0; k < SLOTS; ++k)
-    if (s[k] < S) st_row<HINT>(out + s[k] * ld4 + c, acc[k]);
+    if (s[k] < S) {
+      if (Y) {
+        float4 g = make_float4(0.f, 0.f, 0.f, 0.f);
+        if (q1[k] > q0[k]) {
+          const float ww = row_w ? __ldg(row_w + s[k]) : 1.f;
+          const float4 y = __ldg(Y + s[k] * ld4 + c);
+          g.x = ww * acc[k].x * dact_from_out(y.x, act); g.y = ww * acc[k].y * dact_from_out(y.y, act);
+          g.z = ww * acc[k].z * dact_from_out(y.z, act); g.w = ww * acc[k].w * dact_from_out(y.w, act);
+        }
+        acc[k] = g;
+      }
+      st_row<HINT>(out + s[k] * ld4 + c, acc[k]);
+    }
 }
 
 // tools/k2_variants.py times the variants at the C4 shape
 int g_scatter_variant = 2;     // 0: 1 slot / thread, default caching   1: 2 slots   2: 1 slot + streaming hints   3: 2 slots + hints
 
-int scatter_sum(float* out, const float* msg, int ld, const int* ptr, const int* ent, const float* w, int accumulate,
-                long long S, cudaStream_t st, double bytes) {
-  if (S <= 0) return 0;
-  ProfScope prof(PROF_SCATTER, bytes, st);   // algorithmic bytes (SURVEY.md 8d) when the caller knows the entry count
+static int scatter_launch(float* out, const float* msg, int ld, const int* ptr, const int* ent, const float* w,
+                          int accumulate, long long S, const float* row_w, const float* Y, int act, cudaStream_t st) {
   float4* o = reinterpret_cast<float4*>(out);
   const float4* m = reinterpret_cast<const float4*>(msg);
+  const float4* y = reinterpret_cast<const float4*>(Y);
   const int ld4 = ld / 4;
   const int slots = (g_scatter_variant & 1) ? 2 : 1;
   const long long per_pass = ceil_div_ll(S, slots);
   const unsigned grid = (unsigned)ceil_div_ll(per_pass * ld4, 256);
   switch (g_scatter_variant & 3) {
-    case 0: scatter_sum_kernel<1, 0><<<grid, 256, 0, st>>>(o, m, ld4, ptr, ent, w, accumulate, S, per_pass); break;
-    case 1: scatter_sum_kernel<2, 0><<<grid, 256, 0, st>>>(o, m, ld4, ptr, ent, w, accumulate, S, per_pass); break;
-    case 2: scatter_sum_kernel<1, 1><<<grid, 256, 0, st>>>(o, m, ld4, ptr, ent, w, accumulate, S, per_pass); break;
-    default: scatter_sum_kernel<2, 1><<<grid, 256, 0, st>>>(o, m, ld4, ptr, ent, w, accumulate, S, per_pass); break;
+    case 0: scatter_sum_kernel<1, 0><<<grid, 256, 0, st>>>(o, m, ld4, ptr, ent, w, accumulate, S, per_pass, row_w, y, act); break;
+    case 1: scatter_sum_kernel<2, 0><<<grid, 256, 0, st>>>(o, m, ld4, ptr, ent, w, accumulate, S, per_pass, row_w, y, act); break;
+    case 2: scatter_sum_kernel<1, 1><<<grid, 256, 0, st>>>(o, m, ld4, ptr, ent, w, accumulate, S, per_pass, row_w, y, act); break;
+    default: scatter_sum_kernel<2, 1><<<grid, 256, 0, st>>>(o, m, ld4, ptr, ent, w, accumulate, S, per_pass, row_w, y, act); break;
   }
   GIB_LAUNCH_CHECK();
   return 0;
+}
+
+int scatter_sum(float* out, const float* msg, int ld, const int* ptr, const int* ent, const float* w, int accumulate,
+                long long S, cudaStream_t st, double bytes) {
+  if (S <= 0) return 0;
+  ProfScope prof(PROF_SCATTER, bytes, st);   // algorithmic bytes (SURVEY.md 8d) when the caller knows the entry count
+  return scatter_launch(out, msg, ld, ptr, ent, w, accumulate, S, nullptr, nullptr, ACT_NONE, st);
+}
+
+int seg_reduce_dact(float* G, const float* dM, const float* Y, int ld, const int* ptr, const int* ent,
+                    const float* row_w, int act, long long rows, cudaStream_t st) {
+  if (rows <= 0) return 0;
+  return scatter_launch(G, dM, ld, ptr, ent, nullptr, 0, rows, row_w, Y, act, st);
 }
 
 // backward of K2 (gather-broadcast) fused with the activation derivative of the message MLP's

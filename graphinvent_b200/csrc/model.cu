@@ -210,6 +210,34 @@ GraphArrays graph_arrays(void* buf, long long S, int E, int P) {
   return ga;
 }
 
+// Exact mode: would the message MLPs on the entry groups' host row counts run on the tensor-core kernels (a chain of all
+// layers, or one grouped launch per layer; mlp_forward_multi / gemm_nt_group)?  Only then do the message rows run on
+// their device-side counts -- the same kernels, so the logits stay those of the per-entry path to the bit; otherwise
+// (tensor cores off, small batches on the fp32 SIMT kernel) they run on the entry groups' host ranges, pad rows included.
+static bool msg_mlp_on_tc3(const Run& r) {
+  if (!g_use_tc || (g_tc_debug & 1)) return false;
+  const Plan& pl = r.pl;
+  const int depth = pl.msg[0].n, n = r.ngroups;
+  const bool chain = depth >= 2 && depth * n <= kTc3MaxProblems && (g_tc_debug & 2) == 0;
+  long long chain_tiles = 0;
+  for (int l = 0; l < depth; ++l) {
+    long long tiles = 0;
+    int live = 0, big = 0;
+    for (int g = 0; g < n; ++g) {
+      const Lin& L = pl.lins[pl.msg[g].first + l];
+      const int M = r.tc[g];
+      if (M <= 0) continue;
+      if (L.Rp < 48 || L.Cp < 32) return false;
+      tiles += (long long)ceil_div(M, 128) * ceil_div(L.Rp, 128);
+      ++live;
+      big += M >= 256;
+    }
+    chain_tiles += tiles;
+    if (!chain && !(live > 1 ? tiles >= 4 || big == live : big == live)) return false;
+  }
+  return !chain || chain_tiles >= 16;
+}
+
 int make_run(const gib_dims& d, const int* hdr, Run& r) {
   GIB_TRY(build_plan(d, r.pl));
   r.E = hdr[HDR_E];
@@ -265,6 +293,14 @@ int make_run(const gib_dims& d, const int* hdr, Run& r) {
       L.gh[t] = bp.take(S * 3 * Hp);
     }
     L.hfinal = L.h[d.T];
+    if (d.model != GIB_ATTGGNN) {   // reserved whatever gib_tc_debug says: the workspace size does not depend on it
+      const size_t E = (size_t)r.E;
+      L.mr_src = bp.take(P); L.mr_w = bp.take(P); L.mr_ptr = bp.take(P + 1); L.mr_ent = bp.take(P);
+      L.mr_dst = bp.take(E); L.mr_dst_u = bp.take(E); L.mr_su = bp.take(E); L.mr_sptr = bp.take(S + 1);
+      L.mr_meta = bp.take(MR_META_INTS); L.mr_tmp = bp.take(msg_rows_tmp_ints(d.B, G));
+      r.msg_rows = (g_tc_debug & 8) == 0;
+      r.msg_dev_rows = r.msg_rows && (r.cap || msg_mlp_on_tc3(r));
+    }
   } else {
     const size_t E = (size_t)r.E;
     L.xin = bp.take(E * pl.lins[pl.embnn.first].Cp);
@@ -397,6 +433,26 @@ struct MlpBwdJob {
 static int* fwd_flags(const Run& r) { return reinterpret_cast<int*>(r.ws + r.L.flags); }
 static const int* type_count_dev(const Run& r, int g) { return r.cap ? r.dev_hdr + HDR_TYPE_COUNT + g : nullptr; }
 static const int* type_base_dev(const Run& r, int g) { return r.cap ? r.dev_hdr + HDR_TYPE_BASE + g : nullptr; }
+
+static MsgRows msg_rows_of(const Run& r) {
+  const Layout& L = r.L;
+  auto ip = [&](size_t off) { return reinterpret_cast<int*>(r.ws + off); };
+  MsgRows mr;
+  mr.u_src = ip(L.mr_src); mr.u_w = r.ws + L.mr_w; mr.u_ptr = ip(L.mr_ptr); mr.u_dst = ip(L.mr_dst);
+  mr.ent_u = ip(L.mr_ent); mr.dst_u = ip(L.mr_dst_u); mr.s_ptr = ip(L.mr_sptr); mr.s_u = ip(L.mr_su);
+  mr.meta = ip(L.mr_meta); mr.tmp = ip(L.mr_tmp);
+  return mr;
+}
+// rows the message MLP of bond type g runs on: [row0, row0 + rows), or on the device-side range inside them
+struct MsgRange { long long row0; int rows; const int* m_dev; const int* base_dev; };
+static bool msg_dev(const Run& r) { return r.cap || r.msg_dev_rows; }
+static MsgRange msg_range(const Run& r, int g) {
+  if (r.msg_dev_rows) {
+    const int* meta = reinterpret_cast<const int*>(r.ws + r.L.mr_meta);
+    return {0, r.P, meta + MR_COUNT + g, meta + MR_BASE + g};
+  }
+  return {r.tb[g], r.tc[g], type_count_dev(r, g), type_base_dev(r, g)};
+}
 
 static size_t mlp_max_ld(const Plan& pl, const Mlp& m) {
   size_t w = 16;
@@ -751,15 +807,24 @@ static int node_model_forward(const Run& r, float* out) {
   const Lin& hh = pl.lins[pl.gru_hh];
   // summation_mpnn.py:121-125: zero-padded node features
   GIB_TRY(concat2_in(r.ws + L.h[0], Hp, r.nodes, d.F, d.F, d.in_dtype, nullptr, 0, 0, 0, S, r.st));
+  // rows of the message MLPs: message rows (mpnn.py:60-65, 284-294 read only the source atom's state, the bond type
+  // and the bond value), or one per bond entry
+  const MsgRows mr = r.msg_rows ? msg_rows_of(r) : MsgRows{};
+  if (r.msg_rows)
+    GIB_TRY(msg_rows_build(r.ga, mr, r.cap ? r.dev_hdr : nullptr, r.tb, d.B, d.N, r.ngroups, r.E, r.P, r.st));
+  const int* row_src = r.msg_rows ? mr.u_src : r.ga.ent_src;
+  const int* dst_rows = r.msg_rows ? mr.dst_u : r.ga.dst_ent;
+  const float* row_w = r.msg_rows ? (r.unit_bonds ? nullptr : mr.u_w) : r.w();
   for (int t = 0; t < d.T; ++t) {
     const float* h = r.ws + L.h[t];
     // mpnn.py:286-288 scales the neighbour state by the bond value for GGNN only
-    GIB_TRY(gather_rows(r.ws + L.x0[t], h, Hp, r.ga.ent_src, r.w(), d.model == GIB_GGNN, r.P, nullptr, r.st));
+    GIB_TRY(gather_rows(r.ws + L.x0[t], h, Hp, row_src, row_w, d.model == GIB_GGNN, r.P, nullptr, r.st));
     {   // one grouped launch per layer over the bond types (same input rows layout, per-type weights)
       MlpJob jobs[4];
-      for (int g = 0; g < r.ngroups; ++g)
-        jobs[g] = MlpJob{&pl.msg[g], r.ws + L.x0[t], &L.msg[t], r.tb[g], r.tc[g], nullptr, 0, 0,
-                         type_count_dev(r, g), type_base_dev(r, g)};
+      for (int g = 0; g < r.ngroups; ++g) {
+        const MsgRange rr = msg_range(r, g);
+        jobs[g] = MlpJob{&pl.msg[g], r.ws + L.x0[t], &L.msg[t], rr.row0, rr.rows, nullptr, 0, 0, rr.m_dev, rr.base_dev};
+      }
       GIB_TRY(mlp_forward_multi(r, jobs, r.ngroups, fwd_flags(r)));
       if (d.model == GIB_ATTGGNN) {
         for (int g = 0; g < r.ngroups; ++g)
@@ -773,7 +838,7 @@ static int node_model_forward(const Run& r, float* out) {
       GIB_TRY(seg_softmax_fwd(r.ws + L.msum[t], msgs, r.ws + L.att[t].y[pl.att[0].n], Mp, r.ga.dst_ptr, r.ga.dst_ent,
                               r.w(), S, r.st));
     else
-      GIB_TRY(scatter_sum(r.ws + L.msum[t], msgs, Mp, r.ga.dst_ptr, r.ga.dst_ent, r.w(), 0, S, r.st,
+      GIB_TRY(scatter_sum(r.ws + L.msum[t], msgs, Mp, r.ga.dst_ptr, dst_rows, row_w, 0, S, r.st,
                           r.cap ? 0.0 : 4.0 * ((double)r.E * d.M + (double)S * d.M + (double)(S + 1))));   // SURVEY.md 8d bytes
     {   // the two GRU input projections are independent: one grouped launch
       GemmNT ps[2];
@@ -812,6 +877,8 @@ static int node_model_backward(const Run& r, const BwdBufs& bb, const float* out
   if (part == 1) return 0;
   float* dh = sc + bb.dh;        // d h[t+1]
   float* dh_dir = sc + bb.dh2;   // direct path through the GRU
+  const MsgRows mr = r.msg_rows ? msg_rows_of(r) : MsgRows{};   // built by the forward
+  const float* row_w = r.unit_bonds ? nullptr : mr.u_w;
   for (int t = d.T - 1; t >= 0; --t) {
     const float* h = r.ws + L.h[t];
     GIB_TRY(gru_bwd(sc + bb.dgi, sc + bb.dgh, dh_dir, dh, r.ws + L.gi[t], r.ws + L.gh[t], h, Hp, r.ga.dst_ptr, S,
@@ -856,6 +923,10 @@ static int node_model_backward(const Run& r, const BwdBufs& bb, const float* out
       GIB_CUDA_TRY(cudaMemsetAsync(T2, 0, (size_t)r.P * Mp * sizeof(float), r.st));
       GIB_TRY(seg_softmax_bwd(T1, T2, sc + bb.dmsum, r.ws + L.msg[t].y[nm], r.ws + L.att[t].y[pl.att[0].n], Mp,
                               r.ga.dst_ptr, r.ga.dst_ent, r.w(), S, r.st));
+    } else if (r.msg_rows) {
+      // every entry of a message row adds its destination's gradient: duplicates are summed before the GEMMs
+      GIB_TRY(seg_reduce_dact(T1, sc + bb.dmsum, r.ws + L.msg[t].y[nm], Mp, mr.u_ptr, mr.u_dst, row_w, pl.msg[0].act,
+                              r.P, r.st));
     } else {
       GIB_TRY(scatter_bwd(T1, sc + bb.dmsum, r.ws + L.msg[t].y[nm], Mp, r.ga.ent_dst, r.w(), pl.msg[0].act, r.P,
                           r.st));
@@ -863,11 +934,12 @@ static int node_model_backward(const Run& r, const BwdBufs& bb, const float* out
     {
       MlpBwdJob jobs[4];
       for (int g = 0; g < r.ngroups; ++g) {
-        const size_t ro = (size_t)r.tb[g];
-        jobs[g] = MlpBwdJob{&pl.msg[g], r.ws + L.x0[t], &L.msg[t], r.tb[g], r.tc[g], T1 + ro * Mp,
-                            t == 0 ? nullptr : dx0 + ro * Hp, Hp, nullptr, type_count_dev(r, g), type_base_dev(r, g)};
+        const MsgRange rr = msg_range(r, g);
+        const size_t ro = (size_t)rr.row0;
+        jobs[g] = MlpBwdJob{&pl.msg[g], r.ws + L.x0[t], &L.msg[t], rr.row0, rr.rows, T1 + ro * Mp,
+                            t == 0 ? nullptr : dx0 + ro * Hp, Hp, nullptr, rr.m_dev, rr.base_dev};
       }
-      GIB_TRY(mlp_backward_multi(r, bb, jobs, r.ngroups, r.cap ? r.P : 0));
+      GIB_TRY(mlp_backward_multi(r, bb, jobs, r.ngroups, msg_dev(r) ? r.P : 0));
       if (d.model == GIB_ATTGGNN) {
         for (int g = 0; g < r.ngroups; ++g) {
           const size_t ro = (size_t)r.tb[g];
@@ -878,10 +950,15 @@ static int node_model_backward(const Run& r, const BwdBufs& bb, const float* out
         GIB_TRY(mlp_backward_multi(r, bb, jobs, r.ngroups, r.cap ? r.P : 0));
       }
     }
-    // dh[t][src] += (w) dX0   -- deterministic gather-reduce over the by-source CSR
-    if (t > 0)
-      GIB_TRY(scatter_sum(dh, dx0, Hp, r.ga.src_ptr, r.ga.src_ent, d.model == GIB_GGNN ? r.w() : nullptr, 1, S,
-                          r.st, r.cap ? 0.0 : 4.0 * ((double)r.E * d.H + 2.0 * S * d.H + (double)(S + 1))));
+    // dh[t][src] += (w) dX0   -- deterministic gather-reduce over the by-source CSR (of message rows or of entries; the
+    // host knows the row count of the latter only)
+    if (t > 0) {
+      if (r.msg_rows)
+        GIB_TRY(scatter_sum(dh, dx0, Hp, mr.s_ptr, mr.s_u, d.model == GIB_GGNN ? row_w : nullptr, 1, S, r.st));
+      else
+        GIB_TRY(scatter_sum(dh, dx0, Hp, r.ga.src_ptr, r.ga.src_ent, d.model == GIB_GGNN ? r.w() : nullptr, 1, S,
+                            r.st, r.cap ? 0.0 : 4.0 * ((double)r.E * d.H + 2.0 * S * d.H + (double)(S + 1))));
+    }
   }
   return 0;
 }
@@ -1058,19 +1135,23 @@ void make_bwd(const Run& r, BwdBufs& bb) {
   size_t big = 32, dw = 32;
   size_t maxtc = 0;
   for (int g = 0; g < r.ngroups; ++g) maxtc = std::max(maxtc, (size_t)r.tc[g]);
+  // planned rows of the message MLPs (msg_range): the whole buffer per type on device-side row counts
+  const bool dev = msg_dev(r);
+  size_t mrows[4] = {0, 0, 0, 0};
+  for (int g = 0; g < r.ngroups; ++g) mrows[g] = dev ? P : (size_t)r.tc[g];
   if (d.model != GIB_EMN) {
     for (int g = 0; g < r.ngroups; ++g) {
-      mlp_extent(pl, pl.msg[g], (size_t)r.tc[g], big, dw);
-      if (d.model == GIB_ATTGGNN) mlp_extent(pl, pl.att[g], (size_t)r.tc[g], big, dw);
+      mlp_extent(pl, pl.msg[g], mrows[g], big, dw);
+      if (d.model == GIB_ATTGGNN) mlp_extent(pl, pl.att[g], mrows[g], big, dw);
     }
     big = std::max(big, P * (size_t)std::max(Mp, Hp));
     {
-      const Mlp* ms[4]; size_t rows[4];
-      for (int g = 0; g < r.ngroups; ++g) { ms[g] = &pl.msg[g]; rows[g] = (size_t)r.tc[g]; }
-      group_extent(pl, ms, rows, r.ngroups, r.cap ? r.P : 0, dw, r.cap);
+      const Mlp* ms[4];
+      for (int g = 0; g < r.ngroups; ++g) ms[g] = &pl.msg[g];
+      group_extent(pl, ms, mrows, r.ngroups, dev ? r.P : 0, dw, dev);
       if (d.model == GIB_ATTGGNN) {
         for (int g = 0; g < r.ngroups; ++g) ms[g] = &pl.att[g];
-        group_extent(pl, ms, rows, r.ngroups, r.cap ? r.P : 0, dw, r.cap);
+        group_extent(pl, ms, mrows, r.ngroups, dev ? r.P : 0, dw, dev);
       }
     }
   } else {
@@ -1118,7 +1199,7 @@ void make_bwd(const Run& r, BwdBufs& bb) {
     for (int g = 0; g < r.ngroups && d.model != GIB_EMN; ++g) {
       size_t w = mlp_max_ld(pl, pl.msg[g]);
       if (d.model == GIB_ATTGGNN) w = std::max(w, mlp_max_ld(pl, pl.att[g]));
-      if (r.cap) types = std::max(types, (size_t)r.P * w + 64);   // capacity mode: the groups share one slice
+      if (dev) types = std::max(types, (size_t)r.P * w + 64);   // device-side row counts: the groups share one slice
       else types += (size_t)r.tc[g] * w + 32;
     }
     big = std::max(big, types);

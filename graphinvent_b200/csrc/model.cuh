@@ -51,6 +51,8 @@ struct Layout {
   size_t x0[kMaxPasses];
   MlpAct msg[kMaxPasses], att[kMaxPasses];
   size_t msum[kMaxPasses], gi[kMaxPasses], gh[kMaxPasses];
+  // GGNN / MNN: the message-row table (graph.cuh: MsgRows), int / float arrays
+  size_t mr_src, mr_w, mr_ptr, mr_dst, mr_ent, mr_dst_u, mr_sptr, mr_su, mr_meta, mr_tmp;
   // EMN
   size_t xin, xt, mem[kMaxPasses + 1], emsg[kMaxPasses];
   MlpAct embnn, emx, enx, emm[kMaxPasses], enm[kMaxPasses];
@@ -75,7 +77,11 @@ struct Run {
   Layout L;
   int E = 0, P = 0, ngroups = 0;
   bool unit_bonds = false;
-  bool cap = false;                 // capacity header: E / P / tc are capacities, live counts are read from dev_hdr
+  // GGNN / MNN: the message MLPs run on message rows (one per source atom and bond type, graph.cuh: MsgRows) unless
+  // gib_tc_debug bit 3 asks for one row per bond entry; msg_dev_rows: on the device-side row counts of the table (the
+  // grouped tensor-core call pattern), else on the entry groups' host row ranges, pad rows included
+  bool msg_rows = false, msg_dev_rows = false;
+  bool cap = false;                // capacity header: E / P / tc are capacities, live counts are read from dev_hdr
   const int* dev_hdr = nullptr;     // device copy of the graph header (written by K0)
   const float* w() const { return unit_bonds ? nullptr : ga.ent_w; }
   int tc[4], tb[5];

@@ -30,6 +30,9 @@ int gather_rows(float* dst, const float* h, int ld, const int* src, const float*
 int scatter_sum(float* out, const float* msg, int ld, const int* ptr, const int* ent, const float* w, int accumulate, long long S, cudaStream_t st, double bytes = 0.0);
 extern int g_scatter_variant;
 int scatter_bwd(float* G, const float* dM, const float* Y, int ld, const int* dst, const float* w, int act, long long P, cudaStream_t st);
+// backward of the message rows (K2 with a fused epilogue): G[u] = row_w[u] * act'(Y[u]) * sum_{q in [ptr[u], ptr[u+1])}
+// dM[ent[q]] for rows u < rows (row_w may be null: 1); an empty segment gives exact 0 and Y is not read there
+int seg_reduce_dact(float* G, const float* dM, const float* Y, int ld, const int* ptr, const int* ent, const float* row_w, int act, long long rows, cudaStream_t st);
 int seg_softmax_fwd(float* out, const float* EM, const float* EN, int ld, const int* ptr, const int* ent, const float* w, long long S, cudaStream_t st);
 int seg_softmax_bwd(float* GM, float* GN, const float* dM, const float* EM, const float* EN, int ld, const int* ptr, const int* ent, const float* w, long long S, cudaStream_t st);
 int gru_fwd(float* hn, const float* gi, const float* gh, const float* h, int Hp, const int* ptr, long long S, const int* live, cudaStream_t st);

@@ -12,14 +12,19 @@ enum ProfClass : int { PROF_GEMM_NT = 0, PROF_GEMM_DW = 1, PROF_SCATTER = 2, PRO
                        PROF_NCLASS = 5 };
 
 extern bool g_prof_on;
-void prof_begin(int cls, double work, cudaStream_t st);
+// Work of a problem whose row count lives on the device (GemmNT::m_dev): per_row x min(*m_dev, cap - *base_dev) rows.
+// The two ints are copied to pinned host memory ahead of the launch's first event and resolved when the records are read
+// (after the caller's stream sync), so that the record holds the rows actually launched without a host synchronisation.
+struct ProfRows { const int* m_dev; const int* base_dev; int cap; double per_row; };
+void prof_begin(int cls, double work, cudaStream_t st, const ProfRows* rows = nullptr, int nrows = 0);
 void prof_end(cudaStream_t st);
 
 struct ProfScope {
   cudaStream_t st;
   bool on;
-  ProfScope(int cls, double work, cudaStream_t s) : st(s), on(g_prof_on) {
-    if (on) prof_begin(cls, work, st);
+  ProfScope(int cls, double work, cudaStream_t s, const ProfRows* rows = nullptr, int nrows = 0)
+      : st(s), on(g_prof_on) {
+    if (on) prof_begin(cls, work, st, rows, nrows);
   }
   ~ProfScope() {
     if (on) prof_end(st);

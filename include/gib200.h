@@ -85,7 +85,8 @@ int gib_version(void);
 /* tensor-core 3xTF32 GEMM path on (default) / off (fp32 SIMT GEMMs only); process-wide switch */
 void gib_set_tensor_cores(int on);
 int gib_get_tensor_cores(void);
-/* bit 2: narrow outputs (N < 48, the APD heads) on the tensor-core kernel too (default: fp32 SIMT, see gemm_simt.cu).
+/* bit 3: GGNN / MNN message MLPs on one row per bond entry (the AttentionGGNN's layout) instead of one per message row.
+ * bit 2: narrow outputs (N < 48, the APD heads) on the tensor-core kernel too (default: fp32 SIMT, see gemm_simt.cu).
  * bit 1: no dependent-chain launches (every MLP layer its own launch).
  * bit 0: per-problem call pattern: no grouped or chained tensor-core launches, raw weights split inside the kernel,
  * single-problem weight gradients with the bias column sums on the side stream; process-wide, A/B measurements only.
@@ -128,6 +129,12 @@ size_t gib_model_workspace_bytes(const gib_dims* d, const int* hdr_host);
 int gib_model_forward(const gib_dims* d, const int* hdr_host, const void* nodes, const void* edges,
                       const void* graph_buf, const void* packed, void* workspace, float* out,
                       gib_stream stream);
+/* GGNN / MNN: device addresses of the message-row table the forward builds in `workspace` (one message row per
+ * (molecule, source atom, bond type) for the bond entries of value 1, one per other entry; layout in
+ * graphinvent_b200/csrc/graph.cuh, MsgRows), for tests: which = 0 u_src [P], 1 u_w [P] (float), 2 u_ptr [P+1],
+ * 3 u_dst [E], 4 ent_u [P], 5 dst_u [E], 6 s_ptr [S+1], 7 s_u [E], 8 meta [16], 9 build scratch.  NULL for the other
+ * models or a bad `which`. */
+void* gib_model_msg_rows(const gib_dims* d, const int* hdr_host, void* workspace, int which);
 size_t gib_model_bwd_scratch_bytes(const gib_dims* d, const int* hdr_host);
 /* The backward in two parts on the same scratch: part 1 = readout only -- afterwards the gradients of the gather.* and
  * APDReadout.* parameters (the tail of the parameter order, 79 % of the bytes) are final and a data-parallel caller
