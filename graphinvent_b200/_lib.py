@@ -99,6 +99,7 @@ _PROTOS = {
     "gib_test_dw_scratch_bytes": (c_sz, [c_p, c_p, c_i, c_ll]),
     "gib_test_dw_groups": (c_i, [c_p, c_p, c_i, c_ll, c_p, c_p]),
     "gib_test_scatter_bwd": (c_i, [c_p, c_p, c_p, c_i, c_p, c_p, c_i, c_ll, c_p]),
+    "gib_test_seg_reduce_dact": (c_i, [c_p, c_p, c_p, c_i, c_p, c_p, c_p, c_i, c_ll, c_p]),
     "gib_test_seg_softmax_bwd": (c_i, [c_p, c_p, c_p, c_p, c_p, c_i, c_p, c_p, c_p, c_ll, c_p]),
     "gib_test_gru_bwd": (c_i, [c_p] * 7 + [c_i, c_p, c_ll, c_p, c_p]),
     "gib_test_colsum_add": (c_i, [c_p, c_p, c_i, c_ll, c_i, c_i, c_i, c_p, c_p]),

@@ -492,6 +492,10 @@ int gib_test_scatter_bwd(float* G, const float* dM, const float* Y, int ld, cons
                          long long P, gib_stream stream) {
   return scatter_bwd(G, dM, Y, ld, dst, w, act, P, ST(stream));
 }
+int gib_test_seg_reduce_dact(float* G, const float* dM, const float* Y, int ld, const int* ptr, const int* ent,
+                             const float* row_w, int act, long long rows, gib_stream stream) {
+  return seg_reduce_dact(G, dM, Y, ld, ptr, ent, row_w, act, rows, ST(stream));
+}
 int gib_test_seg_softmax_bwd(float* GM, float* GN, const float* dM, const float* EM, const float* EN, int ld,
                              const int* ptr, const int* ent, const float* w, long long S, gib_stream stream) {
   return seg_softmax_bwd(GM, GN, dM, EM, EN, ld, ptr, ent, w, S, ST(stream));

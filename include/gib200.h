@@ -256,6 +256,10 @@ int gib_test_dw_groups(const gib_dw_problem* qs, const int* group_sizes, int n_g
 /* G[p] = w[p] * dM[dst[p]] * act'(Y[p]) (rows with dst[p] < 0: zeros) */
 int gib_test_scatter_bwd(float* G, const float* dM, const float* Y, int ld, const int* dst, const float* w, int act,
                          long long P, gib_stream stream);
+/* backward of the message rows: G[u] = row_w[u] * act'(Y[u]) * sum_{q in [ptr[u], ptr[u+1])} dM[ent[q]] (row_w may be
+ * NULL: 1; rows with an empty segment: zeros, Y not read), with the variant gib_scatter_variant selects; ld % 4 == 0 */
+int gib_test_seg_reduce_dact(float* G, const float* dM, const float* Y, int ld, const int* ptr, const int* ent,
+                             const float* row_w, int act, long long rows, gib_stream stream);
 /* backward of gib_seg_softmax with SELU outputs EM / EN; GM / GN rows in no segment are not written */
 int gib_test_seg_softmax_bwd(float* GM, float* GN, const float* dM, const float* EM, const float* EN, int ld,
                              const int* ptr, const int* ent, const float* w, long long S, gib_stream stream);

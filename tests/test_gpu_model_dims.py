@@ -67,8 +67,10 @@ def test_fp64_anchored(cid, tensor_cores):
 
 # Rows whose capacity-mode step runs the same kernels with the same reduction split as exact mode, up to the plan rows of
 # the grouped weight gradients.  The others are held to fp64 instead (test_capacity_mode_is_fp64_anchored):
-#   A, G  capacity mode runs the message-MLP backward in sub-groups of <= 16 layers, exact mode one MLP at a time with
-#         fp32 SIMT weight gradients (bond-type groups of < 2048 rows);
+#   A, G  both modes run the message MLPs on the message-row table's device-side counts (the profiling records of
+#         tests/test_gpu_message_rows_fp64.py show exact mode taking that branch for these rows) and their backward in
+#         sub-groups of <= 16 layers, but the grouped weight gradients are planned with each mode's own entry-row count
+#         (exact P, or the capacity's), so their split points differ;
 #   I     exact mode sends GEMMs narrower than 48 columns to the fp32 SIMT kernel, capacity mode runs every bond-row
 #         GEMM on the tensor-core kernel;
 #   J     the re-split 640-wide grouped weight gradients differ by 2.03e-6 x max|g| (one element of msg_nns.2.seq.0),
