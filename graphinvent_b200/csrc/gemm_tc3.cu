@@ -41,7 +41,9 @@
 //                              (conflict-free for K-major operands), split into (hi, lo) in registers,
 //                              mma.sync.m16n8k8 TF32 into two fp32 register accumulators, one mbarrier arrival per warp
 //                              frees the stage
-// All three end in the same epilogue from registers: bias / SELU / dSELU / residual and the stores.
+// All three end in the same epilogue from registers (bias / SELU / dSELU / residual and the stores), except
+// tc3_wgmma_kernel with a specialised epilogue: a 3-stage ring, and the epilogue through a shared-memory tile buffer
+// that warpgroup 2 fills (aux or bias) and drains to C (see the kernel).
 //
 // Dynamic row counts: a problem may name device ints (m_dev, base_dev) -- the bond-type group sizes written by K0 --
 // instead of host values; tile counts are then computed on the device, so the launch needs no device->host read
@@ -93,6 +95,18 @@ constexpr int WG_OFF_BARS = WG_STAGES * WG_STAGE_BYTES;
 constexpr int WG_OFF_SCHED = WG_OFF_BARS + 256;
 constexpr int WG_SMEM_BYTES = WG_OFF_SCHED + 512 + 1024 /*align slack*/;
 static_assert(WG_SMEM_BYTES <= 227 * 1024, "wgmma stages exceed the shared memory of an SM");
+// The same kernel with a specialised epilogue (EPI != EPI_SPEC_GENERIC) drains its tiles through shared memory: a
+// 3-stage ring, then one 64 KB tile buffer (4 TMA boxes [128 x 32] with the 128-byte swizzle) that receives the aux
+// block and is overwritten in place by the results, and the bias slice of the tile.
+constexpr int WG_EPI_STAGES = 3;
+constexpr int WG_EPI_BUF_BYTES = BM * WG_BN * 4;                    // 64 KB
+constexpr int WG_EPI_OFF_BUF = WG_EPI_STAGES * WG_STAGE_BYTES;
+constexpr int WG_EPI_OFF_BARS = WG_EPI_OFF_BUF + WG_EPI_BUF_BYTES;
+constexpr int WG_EPI_OFF_SCHED = WG_EPI_OFF_BARS + 256;
+constexpr int WG_EPI_OFF_BIAS = WG_EPI_OFF_SCHED + 512;
+constexpr int WG_EPI_SMEM_BYTES = WG_EPI_OFF_BIAS + WG_BN * 4 + 1024 /*align slack*/;
+static_assert(WG_EPI_SMEM_BYTES <= 227 * 1024, "wgmma stages and tile buffer exceed the shared memory of an SM");
+constexpr int WG_STORE_WARPS = 2;                                    // warps 10-11
 
 // tc3_wgmma_dw_kernel: 384 threads, registers 256 consumer threads x 224 + 128 producer / transpose threads x 56 =
 // 64512 (the transpose holds a 4 x 4 block and its split: ptxas spills it at 48).  Per k-block of 32 reduction rows the raw stage holds
@@ -117,6 +131,7 @@ struct Maps {   // TMA descriptors in kernel-parameter space
   CUtensorMap a[MAXP];      // NT: activations A (box 128 x 32)    TN: G (box 32 x 32)
   CUtensorMap b[MAXP];      // NT: W hi plane (box 128 x 32) or raw W (box 64 x 32)    TN: X (box 32 x 32)
   CUtensorMap b_lo[MAXP];   // NT: W lo plane (box 128 x 32; pre-split weights only)
+  CUtensorMap aux[MAXP];    // NT, EPI_SPEC_DSELU / EPI_SPEC_ADD: aux [M x n_store] (box 128 x 32)
 };
 
 struct Params {
@@ -202,13 +217,14 @@ __device__ __forceinline__ void mma_tf32(float* d, const uint32_t* a, uint32_t b
       : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
 }
 
-// chain hand-off: all consumer warps have stored their part of the tile -> one release increment of the row block's
-// counter (named barrier 1 = the consumer threads)
+// chain hand-off: all THREADS threads that store the tile (named barrier BAR, led by thread LEAD) have stored their
+// part -> one release increment of the row block's counter
+template <int BAR, int THREADS, int LEAD>
 __device__ __forceinline__ void signal_tile(int* flag) {
   fence_proxy_async_all();
   __threadfence();
-  asm volatile("bar.sync 1, %0;" ::"n"(32 * CONS_WARPS) : "memory");
-  if (threadIdx.x == 0) {
+  asm volatile("bar.sync %0, %1;" ::"n"(BAR), "n"(THREADS) : "memory");
+  if (threadIdx.x == LEAD) {
     __threadfence();
     atomicAdd(flag, 1);
   }
@@ -460,29 +476,66 @@ tc3_gemm_kernel(const __grid_constant__ Maps maps, const Params P) {
             epi_store<EPI>(e, m, n, acc[i][j][2 * h] + accx[i][j][2 * h], acc[i][j][2 * h + 1] + accx[i][j][2 * h + 1], b);
           }
       }
-      if (P.flags) signal_tile(P.flags + P.flag_off[w.p] + w.m0 / BM);
+      if (P.flags) signal_tile<1, 32 * CONS_WARPS, 0>(P.flags + P.flag_off[w.p] + w.m0 / BM);
       if (tr) P.trace[it * 16 + 6] = clock64();
     }
   }
 }
 
+__device__ __forceinline__ void lds64(uint32_t saddr, float& x, float& y) {
+  asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(x), "=f"(y) : "r"(saddr) : "memory");
+}
+__device__ __forceinline__ void sts64(uint32_t saddr, float x, float y) {
+  asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(saddr), "f"(x), "f"(y) : "memory");
+}
+__device__ __forceinline__ float4 lds128(uint32_t saddr) {
+  float4 v;
+  asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(saddr) : "memory");
+  return v;
+}
+
+// byte offset of output element (row r, column c < 128) in the tile buffer: box c / 32, swizzled as TMA writes it
+__device__ __forceinline__ uint32_t epi_off(int r, int c) { return (uint32_t)(c >> 5) * (BM * BKF * 4) + swz(r, c & 31); }
+
 // ---- wgmma kernel: NT with pre-split W ----
+//
+// With a specialised epilogue (SE) the consumers only touch registers and shared memory between a tile's last wgmma
+// and the next tile's first; warpgroup 2 does the global-memory side of the epilogue:
+//   warp 8, lane 0    k-block TMA (as in the generic kernel)
+//   warp 9            epilogue operands of tile t into the tile buffer once the stores of tile t - 1 have drained it:
+//                     the aux block by TMA (DSELU / ADD; rows past the map and columns >= n_store zero-filled), or the
+//                     bias slice by plain loads (SELU / LINEAR) -> epi_full
+//   warps 0-7         epi(acc + accx) in place over the tile buffer -> epi_done
+//   warps 10-11       tile buffer -> C with 16-byte stores (rows < the live row count, columns < n_store) -> epi_empty,
+//                     then the chain hand-off of the tile.  They wait on nothing but epi_done, so a chain cannot
+//                     dead-lock on them.
 template <int EPI>
 __global__ void __launch_bounds__(WG_THREADS, 1)
 tc3_wgmma_kernel(const __grid_constant__ Maps maps, const Params P) {
+  constexpr bool SE = EPI != EPI_SPEC_GENERIC;
+  constexpr bool AUX = EPI == EPI_SPEC_DSELU || EPI == EPI_SPEC_ADD;
+  constexpr int NST = SE ? WG_EPI_STAGES : WG_STAGES;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + WG_OFF_BARS);
-  uint64_t* full = bars;                    // [WG_STAGES] TMA -> consumers
-  uint64_t* empty = bars + WG_STAGES;       // [WG_STAGES] consumers -> TMA
-  Sched& S = *reinterpret_cast<Sched*>(smem + WG_OFF_SCHED);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + (SE ? WG_EPI_OFF_BARS : WG_OFF_BARS));
+  uint64_t* full = bars;                    // [NST] TMA -> consumers
+  uint64_t* empty = bars + NST;             // [NST] consumers -> TMA
+  uint64_t* epi_full = bars + 2 * NST;      // SE: epilogue operands of the tile are in the buffer
+  uint64_t* epi_done = epi_full + 1;        // SE: results of the tile are in the buffer
+  uint64_t* epi_empty = epi_full + 2;       // SE: the buffer is drained
+  Sched& S = *reinterpret_cast<Sched*>(smem + (SE ? WG_EPI_OFF_SCHED : WG_OFF_SCHED));
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < WG_STAGES; ++s) {
+    for (int s = 0; s < NST; ++s) {
       mbar_init(&full[s], 1);
       mbar_init(&empty[s], CONS_WARPS);     // one arrival per consumer warp, once its wgmma group has retired
+    }
+    if (SE) {
+      mbar_init(epi_full, 1);
+      mbar_init(epi_done, CONS_WARPS);
+      mbar_init(epi_empty, WG_STORE_WARPS);
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     init_sched<false>(P, S);
@@ -491,7 +544,7 @@ tc3_wgmma_kernel(const __grid_constant__ Maps maps, const Params P) {
   const int num_items = S.begin[MAXP];
 
   if (warp >= CONS_WARPS) {
-    // ================= TMA producer (warpgroup 2) =================
+    // ================= warpgroup 2: TMA producer, epilogue operands, stores =================
     asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
     if (warp == CONS_WARPS && lane == 0) {
       int stage = 0;
@@ -507,8 +560,60 @@ tc3_wgmma_kernel(const __grid_constant__ Maps maps, const Params P) {
           tma_load_2d(&maps.a[w.p], &full[stage], st, kb * BKF, base + w.m0);
           tma_load_2d(&maps.b[w.p], &full[stage], st + A_BYTES, kb * BKF, w.n0);
           tma_load_2d(&maps.b_lo[w.p], &full[stage], st + A_BYTES + WG_B_BYTES, kb * BKF, w.n0);
-          if (++stage == WG_STAGES) { stage = 0; phase ^= 1; }
+          if (++stage == NST) { stage = 0; phase ^= 1; }
         }
+      }
+    } else if (SE && warp == CONS_WARPS + 1) {
+      uint32_t phase = 0;
+      for (int item = blockIdx.x; item < num_items; item += gridDim.x, phase ^= 1) {
+        const Item w = decode_item<false, WG_BN>(P, S, item);
+        const GemmNT& g = P.g[w.p];
+        mbar_wait(epi_empty, phase ^ 1);
+        if constexpr (AUX) {
+          if (lane == 0) {
+            if (P.flags && P.dep[w.p] >= 0) wait_rows(P, w);   // aux is read no earlier than the A operand
+            const int boxes = min(WG_BN / BKF, ceil_div(g.n_store - w.n0, BKF));
+            mbar_arrive_expect_tx(epi_full, boxes * A_BYTES);
+            for (int b = 0; b < boxes; ++b)
+              tma_load_2d(&maps.aux[w.p], epi_full, smem + WG_EPI_OFF_BUF + b * A_BYTES, w.n0 + b * BKF,
+                          S.base[w.p] + w.m0);
+          }
+        } else {
+          const float* bias = g.bias;
+          float* sb = reinterpret_cast<float*>(smem + WG_EPI_OFF_BIAS);
+          for (int c = lane; c < WG_BN; c += 32) {
+            const int n = w.n0 + c;
+            sb[c] = (bias && n < g.N) ? __ldg(bias + n) : 0.f;
+          }
+          __syncwarp();
+          if (lane == 0) mbar_arrive(epi_full);
+        }
+      }
+    } else if (SE && warp >= CONS_WARPS + 2) {
+      const int sw = warp - (CONS_WARPS + 2);   // store warp 0 / 1: rows sw, sw + 2, ...
+      uint32_t phase = 0;
+      int it = 0;
+      for (int item = blockIdx.x; item < num_items; item += gridDim.x, phase ^= 1, ++it) {
+        const Item w = decode_item<false, WG_BN>(P, S, item);
+        const GemmNT& g = P.g[w.p];
+        const int rows = min(BM, S.M[w.p] - w.m0);
+        const int chunks = min(WG_BN, g.n_store - w.n0) >> 2;    // 16-byte chunks per row (n_store % 4 == 0)
+        float* C = g.C + ((size_t)S.base[w.p] + w.m0) * g.ldc + w.n0 + 4 * lane;
+        const uint32_t src = smem_u32(smem + WG_EPI_OFF_BUF) + (uint32_t)(lane >> 3) * (BM * BKF * 4);
+        mbar_wait(epi_done, phase);
+        if (lane < chunks) {
+#pragma unroll 2
+          for (int r = sw; r < rows; r += WG_STORE_WARPS) {
+            const float4 v = lds128(src + swz(r, 4 * (lane & 7)));
+            *reinterpret_cast<float4*>(C + (size_t)r * g.ldc) = v;
+          }
+        }
+        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic reads of the buffer -> next TMA write
+        __syncwarp();
+        if (lane == 0) mbar_arrive(epi_empty);
+        if (P.flags) signal_tile<2, 32 * WG_STORE_WARPS, 32 * (CONS_WARPS + 2)>(P.flags + P.flag_off[w.p] + w.m0 / BM);
+        if (P.trace && blockIdx.x == 0 && it < P.trace_tiles && threadIdx.x == 32 * (CONS_WARPS + 2))
+          P.trace[it * 16 + 3] = clock64();
       }
     }
   } else {
@@ -566,11 +671,36 @@ tc3_wgmma_kernel(const __grid_constant__ Maps maps, const Params P) {
         }
         half(sa, 1, ah1, al1);
         prev = stage;
-        if (++stage == WG_STAGES) { stage = 0; phase ^= 1; }
+        if (++stage == NST) { stage = 0; phase ^= 1; }
       }
       wgmma_wait<0>();
       __syncwarp();
       if (lane == 0) mbar_arrive(&empty[prev]);
+      if (tr) P.trace[it * 16 + 1] = clock64();
+
+      if constexpr (SE) {
+        // epi(acc + accx) in place over the tile buffer: each lane reads (aux) and writes its own column pairs
+        mbar_wait(epi_full, it & 1);
+        const uint32_t ebuf = smem_u32(smem + WG_EPI_OFF_BUF), ebias = smem_u32(smem + WG_EPI_OFF_BIAS);
+#pragma unroll
+        for (int j = 0; j < WG_BN / 8; ++j) {
+          const int c = j * 8 + 2 * t4;
+          float b[2] = {0.f, 0.f};
+          if (!AUX) lds64(ebias + c * 4, b[0], b[1]);
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const uint32_t a = ebuf + epi_off(r0 + h * 8, c);
+            float x[2] = {0.f, 0.f};
+            if (AUX) lds64(a, x[0], x[1]);
+            sts64(a, epi_one<EPI>(acc[4 * j + 2 * h] + accx[4 * j + 2 * h], b[0], x[0], 0, 0),
+                  epi_one<EPI>(acc[4 * j + 2 * h + 1] + accx[4 * j + 2 * h + 1], b[1], x[1], 0, 0));
+          }
+        }
+        __syncwarp();
+        if (lane == 0) mbar_arrive(epi_done);
+        if (tr) P.trace[it * 16 + 2] = clock64();
+        continue;
+      }
 
       const GemmNT& g = P.g[w.p];
       const int Mrows = S.M[w.p];
@@ -589,16 +719,10 @@ tc3_wgmma_kernel(const __grid_constant__ Maps maps, const Params P) {
           epi_store<EPI>(e, m, n, acc[4 * j + 2 * h] + accx[4 * j + 2 * h], acc[4 * j + 2 * h + 1] + accx[4 * j + 2 * h + 1], b);
         }
       }
-      if (P.flags) signal_tile(P.flags + P.flag_off[w.p] + w.m0 / BM);
+      if (P.flags) signal_tile<1, 32 * CONS_WARPS, 0>(P.flags + P.flag_off[w.p] + w.m0 / BM);
       if (tr) P.trace[it * 16 + 6] = clock64();
     }
   }
-}
-
-__device__ __forceinline__ float4 lds128(uint32_t saddr) {
-  float4 v;
-  asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(saddr) : "memory");
-  return v;
 }
 
 __device__ __forceinline__ void sts128(uint32_t saddr, uint32_t x, uint32_t y, uint32_t z, uint32_t w) {
@@ -968,10 +1092,10 @@ static int prepare(int* num_sms_out) {
     GIB_CUDA_TRY(cudaFuncSetAttribute(tc3_gemm_kernel<EPI_SPEC_DSELU>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
     GIB_CUDA_TRY(cudaFuncSetAttribute(tc3_gemm_kernel<EPI_SPEC_ADD>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
     GIB_CUDA_TRY(cudaFuncSetAttribute(tc3_wgmma_kernel<EPI_SPEC_GENERIC>, cudaFuncAttributeMaxDynamicSharedMemorySize, WG_SMEM_BYTES));
-    GIB_CUDA_TRY(cudaFuncSetAttribute(tc3_wgmma_kernel<EPI_SPEC_SELU>, cudaFuncAttributeMaxDynamicSharedMemorySize, WG_SMEM_BYTES));
-    GIB_CUDA_TRY(cudaFuncSetAttribute(tc3_wgmma_kernel<EPI_SPEC_LINEAR>, cudaFuncAttributeMaxDynamicSharedMemorySize, WG_SMEM_BYTES));
-    GIB_CUDA_TRY(cudaFuncSetAttribute(tc3_wgmma_kernel<EPI_SPEC_DSELU>, cudaFuncAttributeMaxDynamicSharedMemorySize, WG_SMEM_BYTES));
-    GIB_CUDA_TRY(cudaFuncSetAttribute(tc3_wgmma_kernel<EPI_SPEC_ADD>, cudaFuncAttributeMaxDynamicSharedMemorySize, WG_SMEM_BYTES));
+    GIB_CUDA_TRY(cudaFuncSetAttribute(tc3_wgmma_kernel<EPI_SPEC_SELU>, cudaFuncAttributeMaxDynamicSharedMemorySize, WG_EPI_SMEM_BYTES));
+    GIB_CUDA_TRY(cudaFuncSetAttribute(tc3_wgmma_kernel<EPI_SPEC_LINEAR>, cudaFuncAttributeMaxDynamicSharedMemorySize, WG_EPI_SMEM_BYTES));
+    GIB_CUDA_TRY(cudaFuncSetAttribute(tc3_wgmma_kernel<EPI_SPEC_DSELU>, cudaFuncAttributeMaxDynamicSharedMemorySize, WG_EPI_SMEM_BYTES));
+    GIB_CUDA_TRY(cudaFuncSetAttribute(tc3_wgmma_kernel<EPI_SPEC_ADD>, cudaFuncAttributeMaxDynamicSharedMemorySize, WG_EPI_SMEM_BYTES));
     GIB_CUDA_TRY(cudaFuncSetAttribute(tc3_wgmma_dw_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, DW_SMEM_BYTES));
     d.attr_done = true;
   }
@@ -1056,6 +1180,7 @@ static int launch_nt(const GemmNT* ps, const int* dep, int n, int* flags, bool r
     GIB_TRY(make_map(&maps.a[np], p.A, p.M, p.K, p.lda, BM));
     GIB_TRY(make_map(&maps.b[np], raw ? p.B : p.B_hi, p.N, p.K, p.ldb, tbn));
     if (!raw) GIB_TRY(make_map(&maps.b_lo[np], p.B_lo, p.N, p.K, p.ldb, tbn));
+    if (!raw && (sp == EPI_SPEC_DSELU || sp == EPI_SPEC_ADD)) GIB_TRY(make_map(&maps.aux[np], p.aux, p.M, p.n_store, p.ldaux, BM));
     P.g[np] = p;
     P.n_tiles[np] = ceil_div(std::max(p.N, p.n_store), tbn);   // columns [N, n_store) are stored too (zeros / epi(0))
     P.k_blocks[np] = ceil_div(p.K, BKF);
@@ -1097,10 +1222,10 @@ static int launch_nt(const GemmNT* ps, const int* dep, int n, int* flags, bool r
     }
   } else {
     switch (spec) {
-      case EPI_SPEC_SELU: tc3_wgmma_kernel<EPI_SPEC_SELU><<<grid, WG_THREADS, WG_SMEM_BYTES, st>>>(maps, P); break;
-      case EPI_SPEC_LINEAR: tc3_wgmma_kernel<EPI_SPEC_LINEAR><<<grid, WG_THREADS, WG_SMEM_BYTES, st>>>(maps, P); break;
-      case EPI_SPEC_DSELU: tc3_wgmma_kernel<EPI_SPEC_DSELU><<<grid, WG_THREADS, WG_SMEM_BYTES, st>>>(maps, P); break;
-      case EPI_SPEC_ADD: tc3_wgmma_kernel<EPI_SPEC_ADD><<<grid, WG_THREADS, WG_SMEM_BYTES, st>>>(maps, P); break;
+      case EPI_SPEC_SELU: tc3_wgmma_kernel<EPI_SPEC_SELU><<<grid, WG_THREADS, WG_EPI_SMEM_BYTES, st>>>(maps, P); break;
+      case EPI_SPEC_LINEAR: tc3_wgmma_kernel<EPI_SPEC_LINEAR><<<grid, WG_THREADS, WG_EPI_SMEM_BYTES, st>>>(maps, P); break;
+      case EPI_SPEC_DSELU: tc3_wgmma_kernel<EPI_SPEC_DSELU><<<grid, WG_THREADS, WG_EPI_SMEM_BYTES, st>>>(maps, P); break;
+      case EPI_SPEC_ADD: tc3_wgmma_kernel<EPI_SPEC_ADD><<<grid, WG_THREADS, WG_EPI_SMEM_BYTES, st>>>(maps, P); break;
       default: tc3_wgmma_kernel<EPI_SPEC_GENERIC><<<grid, WG_THREADS, WG_SMEM_BYTES, st>>>(maps, P); break;
     }
   }
