@@ -235,11 +235,11 @@ def _model_case(name):
 def run_step(net, nodes, edges, target, capacity, fill, parts=False, grad_fill="zero", ws_delta=0):
     """K0 -> header -> fill -> pack -> forward -> KL loss -> backward (whole, or part 1 then 2) -> Adam, every buffer
     guarded.  fill: "poison" or "zero" for the buffers the contract lets hold garbage; the gradient bucket (accumulated
-    into) and the Adam moments are zeroed unless grad_fill says otherwise."""
+    into) and the Adam moments are zeroed unless grad_fill says otherwise.  int8 nodes / edges run as an int8 batch."""
     from graphinvent_b200 import functional as Fn
     lib, check = _lib()
     B = nodes.shape[0]
-    d = Fn.make_dims(net, B, 0)
+    d = Fn.make_dims(net, B, Fn.input_dtype_code(nodes, edges))
     bd, st = ctypes.byref(d), _st()
     params = [p.detach() for p in net.parameters()]
     total = sum(p.numel() for p in params)

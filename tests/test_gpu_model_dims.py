@@ -154,14 +154,19 @@ def test_graphed_train_step_matches_eager_steps(cid):
         opt.zero_grad(set_to_none=True)
         loss.backward()
         opt.step()
-        losses.append(float(loss.detach()))
+        losses.append(loss.detach().clone())
     step = TrainStep(net2, opt2, batch_size=nodes.shape[0], entry_capacity=capacity)
-    got = [float(step(nodes, edges, target)) for _ in range(2)]
+    got = [step(nodes, edges, target).clone() for _ in range(2)]
     assert step.check() & 4 == 0
-    # the captured step replays the eager step's launches (K0, packing, forward, loss, backward) with the same capacity
-    assert np.allclose(got, losses, rtol=0, atol=1e-5), (got, losses)
+    # the captured step replays the eager step's launches (K0, packing, forward, loss, backward) with the same capacity:
+    # the parameters agree bit for bit.  The losses are float32 sums of the same non-negative loss rows in two orders
+    # (torch's for the eager step, gib_sum_scaled's for the captured one): they agree to twice the rounding bound of
+    # such a sum (tests/test_gpu_batch_stream.py compares the rows themselves)
+    B = nodes.shape[0]
+    for a, b in zip(got, losses):
+        assert abs(float(a) - float(b)) <= 2 * B * 2.0 ** -24 * abs(float(b)), (got, losses)
     for a, b in zip(net.parameters(), net2.parameters()):
-        assert (a - b).abs().max().item() <= 1e-4
+        assert torch.equal(a, b)
 
 
 @pytest.mark.parametrize("cid", ["A", "M"])
