@@ -90,6 +90,13 @@ _PROTOS = {
     "gib_generation_round": (c_i, [c_i] * 7 + [c_p] * 11 + [c_i, c_p, c_p, c_p]),
     "gib_generation_round_layout": (c_i, [c_i] * 9 + [c_p] * 11 + [c_i, c_p, c_p, c_p]),
     "gib_generation_sample_round": (c_i, [c_i] * 8 + [c_p, c_i] + [c_p] * 13 + [c_i, c_p, c_p, c_p]),
+    "gib_rl_sample_round": (c_i, [c_i] * 8 + [c_p, c_p, c_i] + [c_p] * 17 + [c_i, c_p, c_p, c_p]),
+    "gib_rl_snapshot": (c_i, [c_i] * 5 + [c_p] * 9),
+    "gib_rl_restore": (c_i, [c_i] * 4 + [c_p] * 6),
+    "gib_rl_gather": (c_i, [c_i] * 3 + [c_p] * 6),
+    "gib_rl_scatter_grad": (c_i, [c_i] * 3 + [c_p] * 6),
+    "gib_rl_dlogits": (c_i, [c_i, c_i] + [c_p] * 7),
+    "gib_rl_next_round": (c_i, [c_p, c_p]),
     "gib_profile_enable": (None, [c_i]),
     "gib_launch_count": (c_ll, []),
     "gib_profile_collect": (c_i, [c_p, c_p, c_p]),

@@ -20,22 +20,6 @@ void set_error(const char* fmt, ...) {
 }
 
 // ---- KL-divergence loss + gradient (Workflow.py:833-860), one CTA per molecule ---------
-template <int NT>
-__device__ __forceinline__ float block_reduce(float v, float* sm, bool is_max) {
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    float t = __shfl_xor_sync(0xffffffffu, v, o);
-    v = is_max ? fmaxf(v, t) : v + t;
-  }
-  __syncthreads();
-  if (lane == 0) sm[wid] = v;
-  __syncthreads();
-  float r = sm[0];
-  for (int i = 1; i < NT / 32; ++i) r = is_max ? fmaxf(r, sm[i]) : r + sm[i];
-  return r;
-}
-
 __global__ void __launch_bounds__(256) kl_loss_kernel(const float* __restrict__ out, const float* __restrict__ target,
                                                       int apd, float grad_scale, float* __restrict__ loss_rows,
                                                       float* __restrict__ dout) {
@@ -107,6 +91,10 @@ __global__ void __launch_bounds__(256) sample_actions_kernel(const float* __rest
       if (live && !go) g.state[1] = 1;
     }
     if (!go) return;
+    if (g.actions) {                  // recorded actions: row r is the draw, the caller computes the likelihoods
+      if (threadIdx.x == 0) action[b] = g.actions[(size_t)r * B + b];
+      return;
+    }
     uniforms += (size_t)r * B;
   }
   const float* o = out + (size_t)b * apd;

@@ -37,6 +37,24 @@ __device__ __forceinline__ float dact_from_out(float y, int act) {
 }
 __device__ __forceinline__ float sigmoid_f(float x) { return 1.f / (1.f + expf(-x)); }
 
+// CTA-wide max / sum of one float per thread (NT threads, sm >= NT / 32 floats of shared memory); every thread
+// gets the result.  Fixed order: deterministic.
+template <int NT>
+__device__ __forceinline__ float block_reduce(float v, float* sm, bool is_max) {
+  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    float t = __shfl_xor_sync(0xffffffffu, v, o);
+    v = is_max ? fmaxf(v, t) : v + t;
+  }
+  __syncthreads();
+  if (lane == 0) sm[wid] = v;
+  __syncthreads();
+  float r = sm[0];
+  for (int i = 1; i < NT / 32; ++i) r = is_max ? fmaxf(r, sm[i]) : r + sm[i];
+  return r;
+}
+
 // error plumbing: kernels are launched through GIB_LAUNCH_CHECK so that a bad launch
 // configuration is reported at the C-ABI boundary as a cudaError_t (>0).
 #define GIB_CUDA_TRY(expr)                                   \

@@ -314,6 +314,33 @@ extern "C" int gib_generation_sample_round(int B, int N, int F, int Ef, int n_at
                       gen_n_nodes, gen_likelihoods, properly_terminated, capacity, counters, scratch, st);
 }
 
+extern "C" int gib_rl_sample_round(int B, int N, int F, int Ef, int n_atom_types, int n_charges, int n_imp_H,
+                                   int n_chirality, const float* logits_a, const float* logits_b, int apd,
+                                   const float* uniforms, const int* actions, int* state, int* act_rec, float* p_a,
+                                   float* p_b, int* action, float* tags, float* nodes, float* edges, int* n_nodes,
+                                   float* likelihoods, float* gen_nodes, float* gen_edges, signed char* gen_n_nodes,
+                                   float* gen_likelihoods, signed char* properly_terminated, int capacity,
+                                   int* counters, void* scratch, gib_stream stream) {
+  GIB_TRY(check_round_args(B, N, F, Ef, n_atom_types, n_charges, n_imp_H, n_chirality, 0));
+  const long long want = (long long)N * n_atom_types * n_charges * (n_imp_H ? n_imp_H : 1) *
+                         (n_chirality ? n_chirality : 1) * Ef + (long long)N * Ef + 1;
+  if (apd != want || B + 1 >= (1 << 24) || !logits_a || !logits_b || (!uniforms && !actions) || !act_rec || !p_a ||
+      !p_b) {
+    set_error("gib_rl_sample_round: apd=%d (the action layout N=%d A=%d CH=%d H=%d C=%d Ef=%d has %lld actions), "
+              "B=%d (slot tags travel as fp32: B < 2^24 - 1), and logits, draws and record tables must be given",
+              apd, N, n_atom_types, n_charges, n_imp_H, n_chirality, Ef, want, B);
+    return -1;
+  }
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  GenDims d{B, N, F, Ef, n_atom_types, n_charges, n_imp_H, n_chirality, 2 * N};
+  int* ctl = round_ctl(scratch, B);
+  const RoundGate gate{state, counters, ctl, 2 * N, actions};
+  GIB_TRY(sample_actions_launch(logits_a, B, apd, uniforms, action, tags, &gate, st));
+  GIB_TRY(rl_probs_launch(logits_a, logits_b, B, apd, action, ctl, act_rec, p_a, p_b, tags, st));
+  return launch_round(d, 0, ctl, state, action, tags, nodes, edges, n_nodes, likelihoods, gen_nodes, gen_edges,
+                      gen_n_nodes, gen_likelihoods, properly_terminated, capacity, counters, scratch, st);
+}
+
 extern "C" int gib_generation_round(int B, int N, int F, int Ef, int n_atom_types, int n_charges, int round,
                                     const int* action, const float* likelihood, float* nodes, float* edges,
                                     int* n_nodes, float* likelihoods, float* gen_nodes, float* gen_edges,

@@ -52,9 +52,16 @@ int pack_weight(float* Wp, float* WTp, float* bp, const float* W, const float* b
 // loop condition are read from device memory.  state = {next round, status}; a call runs when counters[0] < B,
 // status == 0 and state[0] < rounds, samples row state[0] of uniforms [rounds, B] and leaves state[0] in ctl[0]
 // (-1 when it does not run: the round kernels then do nothing).  A call that finds state[0] >= rounds while
-// counters[0] < B sets status 1.
-struct RoundGate { int* state; const int* counters; int* ctl; int rounds; };
+// counters[0] < B sets status 1.  actions != null ([rounds, B]): a running call takes row state[0] of it as the
+// draw instead of sampling, and leaves `lik` untouched.
+struct RoundGate { int* state; const int* counters; int* ctl; int rounds; const int* actions; };
 int sample_actions_launch(const float* out, int B, int apd, const float* uniforms, int* action, float* lik,
                           const RoundGate* gate, cudaStream_t st);
+
+// RL rollout (rl.cu): for every slot b of a running round r = ctl[0] (ctl[0] < 0: nothing), the softmax
+// probability of action[b] under logits_a / logits_b [B, apd] into p_a / p_b[r, b], action[b] into act_rec[r, b], and
+// the slot tag b + 1 into tags[b] (the "likelihood" the round kernels store: the (molecule, round) -> slot map)
+int rl_probs_launch(const float* logits_a, const float* logits_b, int B, int apd, const int* action, const int* ctl,
+                    int* act_rec, float* p_a, float* p_b, float* tags, cudaStream_t st);
 
 }  // namespace gib

@@ -26,8 +26,18 @@ Generation rounds as replays of ONE captured round (`GraphedGenerator`, a drop-i
 The captured round is K0 -> forward -> `gib_generation_sample_round`, whose round index, uniforms row and stop rule
 live in device memory, so the host replays the same graph until a status copied back asynchronously says the batch
 is done; it keeps two rounds in flight and never waits on the round it just launched.
+
+The RL rollout of `Workflow.learning_step` as replays of captured rounds (`GraphedGeneratorRL`, a drop-in for
+`generation.GraphGeneratorRL`):
+
+    gen = graphinvent_b200.graphed.GraphedGeneratorRL(agent, batch_size=1000)      # once
+    graphs, agent_ll, prior_ll, proper = gen.sample(agent, prior)                # per rollout; autograd tensors
+
+Each rollout keeps only the int8 input of every round; `loss.backward()` recomputes each round's forward before its
+backward, one captured backward round per model that needs gradients.
 """
 import ctypes
+import types
 
 import torch
 
@@ -236,8 +246,8 @@ class GraphedGenerator(GraphGenerator):
 
     The weights are re-packed into the arena (one launch per batch, not per round) whenever a parameter's storage,
     in-place version or `functional.invalidate_packed_weights` epoch changed; the graph reads only the arena, so no
-    recapture is needed for that.  Generation with recorded actions (`replay=`) and the RL rollout, which
-    back-propagates through every round, stay with the eager generators."""
+    recapture is needed for that.  Generation with recorded actions (`replay=`) stays with the eager generator; the
+    RL rollout has its own captured form, `GraphedGeneratorRL`."""
 
     def __init__(self, model, batch_size, constants=None, n_atom_types=None, n_formal_charge=None, n_imp_H=None,
                  n_chirality=None, device="cuda"):
@@ -395,3 +405,311 @@ class GraphedGenerator(GraphGenerator):
         flat = self.generated_likelihoods[self.generated_likelihoods != 0]
         graphs = (self.generated_nodes[:B].clone(), self.generated_edges[:B].clone(), self.generated_n_nodes[:B].clone())
         return graphs, flat, final, self.properly_terminated[:B].clone()
+
+
+# ---- the RL rollout -------------------------------------------------------------------------------------------
+def rl_record_bytes(batch_size, max_n_nodes, n_node_features, n_edge_features):
+    """device bytes one `GraphedGeneratorRL.sample()` keeps for its backward at the 2N-round limit (a rollout of R
+    rounds keeps R / 2N of the per-round part): the int8 model input of every round, the action and both models'
+    probabilities per (round, slot), and the (molecule, round) -> slot map [2B, 2N] in fp32"""
+    B, N, F_, Ef = int(batch_size), int(max_n_nodes), int(n_node_features), int(n_edge_features)
+    per_round = B * (N * F_ + N * N * Ef) + B * (4 + 4 + 4)
+    return 2 * N * per_round + 2 * B * 2 * N * 4
+
+
+class _RolloutLikelihoods(torch.autograd.Function):
+    """generated_{agent,prior}_likelihoods [2B, 2N] of one rollout as a function of both models' parameters; the
+    backward recomputes every round's forward (GraphedGeneratorRL._backward)"""
+
+    @staticmethod
+    def forward(ctx, gen, rec, n_a, *params):
+        ctx.gen, ctx.rec, ctx.n_a = gen, rec, n_a
+        ctx.ptrs = [p.data_ptr() for p in params]
+        ctx.save_for_backward(*params)
+        return gen._gather(rec)
+
+    @staticmethod
+    def backward(ctx, d_a, d_b):
+        params = ctx.saved_tensors          # autograd raises here if a parameter was modified in place since the rollout
+        if [p.data_ptr() for p in params] != ctx.ptrs:
+            raise RuntimeError("one of the variables needed for gradient computation has been modified by an inplace "
+                               "operation: a parameter's storage changed between the RL rollout and its backward")
+        n_a, need = ctx.n_a, ctx.needs_input_grad[3:]
+        pa, pb = params[:n_a], params[n_a:]
+        ga, gb = ctx.gen._backward(ctx.rec, d_a, d_b, pa if any(need[:n_a]) else None, pb if any(need[n_a:]) else None)
+        return (None, None, None, *(ga if ga is not None else [None] * len(pa)),
+                *(gb if gb is not None else [None] * len(pb)))
+
+
+class GraphedGeneratorRL(GraphedGenerator):
+    """`generation.GraphGeneratorRL` with each rollout round a replay of one captured CUDA graph, and a backward that
+    recomputes each round's forward instead of keeping its activations.
+
+    Rollout round (two rounds in flight, round state in device memory, as `GraphedGenerator`):
+      1. `gib_rl_snapshot`: the live `nodes` / `edges` as int8 into a static model input (the AttentionGGNN view of
+         slot 0 applied) and into row r of the rollout record,
+      2. K0 in capacity mode at `entry_capacity(B, N, Ef)`, shared by both models,
+      3. the agent's and the prior's forward on one workspace,
+      4. `gib_rl_sample_round`: sample from the agent (row r of `uniforms`, or row r of recorded `actions`), keep the
+         action and its probability under both models per (round, slot), run the round with slot tags.
+
+    `sample()` returns what the eager class returns, as copies; the two log-likelihood vectors are autograd tensors.
+    Each call owns its rollout record (`rl_record_bytes`: int8 inputs, actions, both probability tables, the owner
+    map), so several rollouts can wait for one `loss.backward()` as in `Workflow.learning_step`.  The backward inverts
+    the owner map (`gib_rl_scatter_grad`), then, for each model whose parameters require grad, repacks the weights and
+    replays a captured backward round R times in ascending order: restore round r's input, K0, forward,
+    `gib_rl_dlogits`, `gib_model_backward` into one flat gradient bucket.  The kernels are deterministic and int8
+    inputs give the float inputs' logits bit for bit, so the recomputed probabilities equal the rollout's
+    (`recomputed_p`).  A frozen model costs no backward at all.
+
+    The agent and the prior must be this package's models of the generator's family with equal dims (in
+    `learning_step` they are deep copies of one model); other pairs raise ValueError.  A parameter modified in place,
+    or moved, between a rollout and its backward makes the backward raise, as autograd does."""
+
+    def __init__(self, model, batch_size, constants=None, n_atom_types=None, n_formal_charge=None, n_imp_H=None,
+                 n_chirality=None, device="cuda"):
+        GraphGenerator.__init__(self, model, batch_size, constants=constants, n_atom_types=n_atom_types,
+                                n_formal_charge=n_formal_charge, n_imp_H=n_imp_H, n_chirality=n_chirality,
+                                device=device)
+        if not hasattr(model, "dims"):
+            raise TypeError("GraphedGeneratorRL runs this package's models (graphinvent_b200.gnn.mpnn) only")
+        B, N, dev = self.batch_size, self.N, self.device
+        if B + 1 >= 1 << 24:
+            raise ValueError("batch_size must stay below 2**24 (slot ids travel as fp32)")
+        self.params = list(model.parameters())
+        F._require_cuda(*self.params)
+        self.d = F.make_dims(model, B, 1)                 # int8 model inputs: the 0/1 state, bit-exact logits
+        self._key = F.dims_key(model, B, 1)
+        bd = ctypes.byref(self.d)
+        F._check_params(model, self.d, self.params)
+        self.entry_capacity = entry_capacity(B, N, self.Ef)
+        self._att_view = getattr(model, "MODEL", None) == "AttGGNN"
+        i8, f32, i32 = torch.int8, torch.float32, torch.int32
+        self.in_nodes = torch.zeros(B, N, self.F, dtype=i8, device=dev)
+        self.in_edges = torch.zeros(B, N, N, self.Ef, dtype=i8, device=dev)
+        probe = F.GraphBatch(self.d, self.in_edges, capacity=self.entry_capacity)
+        self.cws, self.gbuf, self.hdr_np, self.hdr = probe.cws, probe.buf, probe.hdr_np, probe.hdr
+        pbytes = lib.gib_model_packed_bytes(bd)
+        self.packed = [torch.empty(pbytes, dtype=torch.uint8, device=dev) for _ in range(2)]   # agent, prior
+        ws_bytes = lib.gib_model_workspace_bytes(bd, self.hdr)
+        if ws_bytes == 0:
+            check(-1, "gib_model_workspace_bytes")
+        self.workspace_bytes = ws_bytes
+        self.ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
+        self.logits = [torch.empty(B, self.apd, dtype=f32, device=dev) for _ in range(2)]
+        self.action = torch.zeros(B, dtype=i32, device=dev)
+        self.lik = torch.zeros(B, dtype=f32, device=dev)             # the slot tags b + 1
+        self.uniforms = torch.zeros(2 * N, B, dtype=f32, device=dev)
+        self.actions = torch.full((2 * N, B), -1, dtype=i32, device=dev)
+        # the static rollout record: every round's int8 input, its actions and both models' probabilities
+        self.rec_nodes = torch.zeros(2 * N, B, N, self.F, dtype=i8, device=dev)
+        self.rec_edges = torch.zeros(2 * N, B, N, N, self.Ef, dtype=i8, device=dev)
+        self.act_rec = torch.zeros(2 * N, B, dtype=i32, device=dev)
+        self.p_a = torch.zeros(2 * N, B, dtype=f32, device=dev)
+        self.p_b = torch.zeros(2 * N, B, dtype=f32, device=dev)
+        self._host = torch.zeros(2 * N + 1, 5, dtype=torch.int32, pin_memory=True)
+        self._host_np = self._host.numpy()
+        self._events = [torch.cuda.Event() for _ in range(2 * N + 1)]
+        self._hdr_flags = self.cws[: HDR_INTS * 4].view(torch.int32)[HDR_FLAGS:HDR_FLAGS + 1]
+        self._packed_key = None
+        self.graph = None
+        self._graphs = {}                               # sampling / replaying recorded actions
+        self._replay = False
+        self._pair = (model, model)
+        self._bwd = None
+        self.inert_rounds = 0
+        self.backward_rounds = [0, 0]
+
+    def _check_pair(self, agent, prior):
+        for m in (agent, prior):
+            if not hasattr(m, "dims") or type(m) is not type(self.model) or F.dims_key(m, self.batch_size, 1) != self._key:
+                raise ValueError("GraphedGeneratorRL needs the agent and the prior to be this package's models of the "
+                                 "generator's family with equal dims (Workflow.learning_step's deep copies); use "
+                                 "generation.GraphGeneratorRL for other pairs")
+
+    def _pack(self):
+        models = self._pair
+        for m in models:
+            if m.training and any(p > 0.0 for p in m._dropout_ps()):
+                raise NotImplementedError("dropout_p > 0 in training mode is not supported by the fused sm_90a path")
+        tables = [list(m.parameters()) for m in models]
+        key = (F._weights_epoch[0],) + tuple((p.data_ptr(), p._version) for ps in tables for p in ps)
+        if key == self._packed_key:
+            return
+        for slot, ps in enumerate(tables):
+            self._pack_slot(slot, ps)
+        self._packed_key = key
+
+    def _pack_slot(self, slot, params):
+        if len(params) != len(self.params) or any(p.shape != q.shape for p, q in zip(params, self.params)):
+            raise RuntimeError("the model's parameter table changed after the GraphedGeneratorRL was built")
+        F._require_cuda(*params)
+        check(lib.gib_model_pack(ctypes.byref(self.d), F._ptr_table(params), F._ptr(self.packed[slot]),
+                                 F._stream(self.device)), "gib_model_pack")
+
+    # ---- the captured rollout round -----------------------------------------------------------------------
+    def _k0_forward(self, slots):
+        """K0 on the static int8 input, then the forward of model slot s into logits[i] for the i-th slot given"""
+        bd, st = ctypes.byref(self.d), F._stream(self.device)
+        check(lib.gib_graph_count(bd, F._ptr(self.in_edges), F._ptr(self.cws), st), "gib_graph_count")
+        check(lib.gib_graph_fill(bd, F._ptr(self.in_edges), F._ptr(self.cws), self.hdr, F._ptr(self.gbuf), st),
+              "gib_graph_fill")
+        for i, slot in enumerate(slots):
+            check(lib.gib_model_forward(bd, self.hdr, F._ptr(self.in_nodes), F._ptr(self.in_edges), F._ptr(self.gbuf),
+                                        F._ptr(self.packed[slot]), F._ptr(self.ws), F._ptr(self.logits[i]), st),
+                  "gib_model_forward")
+
+    def _enqueue_round(self):
+        B, N, st = self.batch_size, self.N, F._stream(self.device)
+        check(lib.gib_rl_snapshot(B, N, self.F, self.Ef, int(self._att_view), F._ptr(self.nodes), F._ptr(self.edges),
+                                  F._ptr(self._state), F._ptr(self._counters), F._ptr(self.rec_nodes),
+                                  F._ptr(self.rec_edges), F._ptr(self.in_nodes), F._ptr(self.in_edges), st),
+              "gib_rl_snapshot")
+        self._k0_forward((0, 1))
+        self._flags.bitwise_or_(self._hdr_flags)
+        check(lib.gib_rl_sample_round(
+            B, N, self.F, self.Ef, self.A, self.CH, self.n_imp_H, self.n_chirality, F._ptr(self.logits[0]),
+            F._ptr(self.logits[1]), self.apd, F._ptr(self.uniforms), F._ptr(self.actions if self._replay else None),
+            F._ptr(self._state), F._ptr(self.act_rec), F._ptr(self.p_a), F._ptr(self.p_b), F._ptr(self.action),
+            F._ptr(self.lik), F._ptr(self.nodes), F._ptr(self.edges), F._ptr(self.n_nodes), F._ptr(self.likelihoods),
+            F._ptr(self.generated_nodes), F._ptr(self.generated_edges), F._ptr(self.generated_n_nodes),
+            F._ptr(self.generated_likelihoods), F._ptr(self.properly_terminated), self.capacity,
+            F._ptr(self._counters), F._ptr(self._scratch), st), "gib_rl_sample_round")
+
+    # ---- the captured backward round ----------------------------------------------------------------------
+    def _enqueue_backward_round(self, slot):
+        """round bctl[0] of model `slot`: restore its input, recompute the forward, dlogits, accumulate the gradient"""
+        b, B, st = self._bwd, self.batch_size, F._stream(self.device)
+        check(lib.gib_rl_restore(B, self.N, self.F, self.Ef, F._ptr(self.rec_nodes), F._ptr(self.rec_edges),
+                                 F._ptr(b.ctl), F._ptr(self.in_nodes), F._ptr(self.in_edges), st), "gib_rl_restore")
+        self._k0_forward((slot,))
+        check(lib.gib_rl_dlogits(B, self.apd, F._ptr(self.logits[0]), F._ptr(self.act_rec), F._ptr(b.dp[slot]),
+                                 F._ptr(b.ctl), F._ptr(b.dlogits), F._ptr(self.recomputed_p[slot]), st), "gib_rl_dlogits")
+        check(lib.gib_model_backward(ctypes.byref(self.d), self.hdr, F._ptr(self.in_nodes), F._ptr(self.in_edges),
+                                     F._ptr(self.gbuf), F._ptr(self.packed[slot]), F._ptr(self.ws),
+                                     F._ptr(self.logits[0]), F._ptr(b.dlogits), F._ptr_table(b.views[slot]),
+                                     F._ptr(b.scratch), st), "gib_model_backward")
+        check(lib.gib_rl_next_round(F._ptr(b.ctl), st), "gib_rl_next_round")
+
+    def _ensure_backward(self):
+        """backward buffers and the two captured backward rounds, built by the first rollout that needs gradients"""
+        if self._bwd is not None:
+            return
+        B, N, dev = self.batch_size, self.N, self.device
+        bd = ctypes.byref(self.d)
+        total = sum(p.numel() for p in self.params)
+        b = types.SimpleNamespace()
+        b.scratch = torch.empty(lib.gib_model_bwd_scratch_bytes(bd, self.hdr), dtype=torch.uint8, device=dev)
+        b.dlogits = torch.empty(B, self.apd, dtype=torch.float32, device=dev)
+        b.dp = torch.zeros(2, 2 * N, B, dtype=torch.float32, device=dev)
+        b.gflat = torch.zeros(2, total, dtype=torch.float32, device=dev)
+        b.views = []
+        for slot in range(2):
+            views, o = [], 0
+            for p in self.params:
+                views.append(b.gflat[slot, o:o + p.numel()])
+                o += p.numel()
+            b.views.append(views)
+        b.ctl = torch.zeros(1, dtype=torch.int32, device=dev)
+        self.recomputed_p = torch.zeros(2, 2 * N, B, dtype=torch.float32, device=dev)
+        self._bwd = b
+        side = torch.cuda.Stream(dev)
+        side.wait_stream(torch.cuda.current_stream(dev))
+        with torch.cuda.stream(side):              # warm-up outside capture (lazy per-device init, function attributes)
+            for slot in range(2):
+                self._enqueue_backward_round(slot)
+        torch.cuda.current_stream(dev).wait_stream(side)
+        torch.cuda.synchronize(dev)
+        b.graphs = []
+        for slot in range(2):
+            g = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(g):
+                self._enqueue_backward_round(slot)
+            b.graphs.append(g)
+
+    def _gather(self, rec):
+        """both [2B, 2N] generated-likelihood tables of a rollout record"""
+        out = [torch.zeros_like(rec.owner) for _ in range(2)]
+        check(lib.gib_rl_gather(self.batch_size, rec.owner.shape[0], rec.owner.shape[1], F._ptr(rec.owner),
+                                F._ptr(rec.p_a), F._ptr(rec.p_b), F._ptr(out[0]), F._ptr(out[1]),
+                                F._stream(self.device)), "gib_rl_gather")
+        return tuple(out)
+
+    @torch.no_grad()
+    def _backward(self, rec, d_a, d_b, params_a, params_b):
+        """gradients of sum(d_a * agent table + d_b * prior table) w.r.t. the models given (None: frozen, skipped)"""
+        B, N, R, st = self.batch_size, self.N, rec.rounds, F._stream(self.device)
+        b = self._bwd
+        self.backward_rounds = [0, 0]
+        self.rec_nodes[:R].copy_(rec.nodes)
+        self.rec_edges[:R].copy_(rec.edges)
+        self.act_rec[:R].copy_(rec.act)
+        grads = [d.contiguous().float() if ps is not None else None
+                 for d, ps in ((d_a, params_a), (d_b, params_b))]
+        check(lib.gib_rl_scatter_grad(B, 2 * B, 2 * N, F._ptr(rec.owner), F._ptr(grads[0]), F._ptr(grads[1]),
+                                      F._ptr(b.dp[0]), F._ptr(b.dp[1]), st), "gib_rl_scatter_grad")
+        out = []
+        for slot, params in enumerate((params_a, params_b)):
+            if params is None:
+                out.append(None)
+                continue
+            self._pack_slot(slot, params)               # the arenas may hold another rollout's models by now
+            b.gflat[slot].zero_()
+            b.ctl.zero_()
+            for _ in range(R):
+                b.graphs[slot].replay()
+            self.backward_rounds[slot] = R
+            flat = b.gflat[slot].clone()                # a fresh bucket: autograd may keep it as .grad
+            views, o = [], 0
+            for p in params:
+                views.append(flat[o:o + p.numel()].view(p.shape))
+                o += p.numel()
+            out.append(views)
+        self._packed_key = None
+        return out
+
+    # ---- one rollout --------------------------------------------------------------------------------------
+    @torch.no_grad()
+    def build_graphs(self, agent_model=None, prior_model=None, generator=None, uniforms=None, actions=None):
+        """uniforms: optional [2N, B] draws (instead of torch.rand); actions: optional [R, B] recorded flat APD indices
+        replayed instead of sampling (both models are still evaluated).  Returns the number of finished molecules."""
+        agent = agent_model if agent_model is not None else self.model
+        prior = prior_model if prior_model is not None else self.model
+        self._check_pair(agent, prior)
+        B, N = self.batch_size, self.N
+        replay = actions is not None
+        if replay:
+            actions = torch.as_tensor(actions)
+            if actions.dim() != 2 or actions.shape[1] != B or not 1 <= actions.shape[0] <= 2 * N:
+                raise ValueError(f"actions must have shape [rounds, batch_size] with 1 <= rounds <= 2*max_n_nodes = {2 * N}")
+            self.actions.fill_(-1)                      # past the trace: an invalid action that ends every slot
+            self.actions[:actions.shape[0]].copy_(actions)
+        self._pair = (agent, prior)
+        self._replay = replay
+        self.graph = self._graphs.get(replay)
+        n = GraphedGenerator.build_graphs(self, generator=generator, uniforms=uniforms)
+        self._graphs[replay] = self.graph
+        if replay and self.rounds > actions.shape[0]:
+            raise RuntimeError("replay trace ended before batch_size molecules were finished")
+        return n
+
+    def sample(self, agent_model, prior_model, generator=None, uniforms=None, actions=None):
+        """what GraphGeneratorRL.sample returns, as copies: (nodes, edges, n_nodes), agent_ll, prior_ll,
+        properly_terminated; agent_ll / prior_ll are differentiable w.r.t. every model parameter that requires grad"""
+        self.build_graphs(agent_model, prior_model, generator=generator, uniforms=uniforms, actions=actions)
+        agent, prior = self._pair
+        B, R = self.batch_size, self.rounds
+        pa, pb = list(agent.parameters()), list(prior.parameters())
+        rec = types.SimpleNamespace(owner=self.generated_likelihoods.clone(), p_a=self.p_a[:R].clone(),
+                                    p_b=self.p_b[:R].clone(), rounds=R)
+        if torch.is_grad_enabled() and any(p.requires_grad for p in pa + pb):
+            self._ensure_backward()
+            rec.nodes, rec.edges, rec.act = self.rec_nodes[:R].clone(), self.rec_edges[:R].clone(), self.act_rec[:R].clone()
+            lik_a, lik_b = _RolloutLikelihoods.apply(self, rec, len(pa), *pa, *pb)
+        else:
+            lik_a, lik_b = self._gather(rec)
+        self.generated_agent_likelihoods, self.generated_prior_likelihoods = lik_a, lik_b
+        agent_ll = torch.log(torch.sum(lik_a, dim=1)[:B])          # GraphGeneratorRL.py:92-97
+        prior_ll = torch.log(torch.sum(lik_b, dim=1)[:B])
+        graphs = (self.generated_nodes[:B].clone(), self.generated_edges[:B].clone(), self.generated_n_nodes[:B].clone())
+        return graphs, agent_ll, prior_ll, self.properly_terminated[:B].clone()

@@ -377,6 +377,46 @@ int gib_generation_sample_round(int B, int N, int F, int Ef, int n_atom_types, i
                                 float* gen_likelihoods, signed char* properly_terminated, int capacity,
                                 int* counters, void* scratch, gib_stream stream);
 
+/* ---- the RL rollout (GraphGeneratorRL.py:109-172) as captured rounds, and its backward by recomputation
+ *      (graphinvent_b200.graphed.GraphedGeneratorRL).  Tables indexed [round, slot] have 2N rows of B. ----
+ * gib_rl_sample_round: gib_generation_sample_round with two models.  The draw comes from logits_a (row state[0] of
+ * `uniforms`), or, when `actions` is given, is row state[0] of `actions` [2N, B].  A running round stores the draw in
+ * act_rec[r, b] and its softmax probability under logits_a / logits_b [B, apd] in p_a / p_b[r, b], then runs the round
+ * with the slot tag b + 1 as every slot's likelihood (written to `tags` [B]): gen_likelihoods becomes the map from
+ * (finished molecule, round) to slot + 1.  B < 2^24 - 1; the other arguments are validated as for
+ * gib_generation_sample_round. */
+int gib_rl_sample_round(int B, int N, int F, int Ef, int n_atom_types, int n_charges, int n_imp_H, int n_chirality,
+                        const float* logits_a, const float* logits_b, int apd, const float* uniforms,
+                        const int* actions, int* state, int* act_rec, float* p_a, float* p_b, int* action,
+                        float* tags, float* nodes, float* edges, int* n_nodes, float* likelihoods, float* gen_nodes,
+                        float* gen_edges, signed char* gen_n_nodes, float* gen_likelihoods,
+                        signed char* properly_terminated, int capacity, int* counters, void* scratch,
+                        gib_stream stream);
+/* the model input of a round: nodes [B,N,F] / edges [B,N,N,Ef] (float 0/1) as int8 into in_nodes / in_edges and, when
+ * the round runs (gib_generation_sample_round's state / counters: 0 <= state[0] < 2N, state[1] == 0,
+ * counters[0] < B), into row state[0] of rec_nodes [2N,B,N,F] / rec_edges [2N,B,N,N,Ef].  att_view != 0: slot 0's
+ * bonds keep their first non-zero type only (the AttentionGGNN view of the dummy graph, GraphGenerator._model_inputs) */
+int gib_rl_snapshot(int B, int N, int F, int Ef, int att_view, const float* nodes, const float* edges,
+                    const int* state, const int* counters, signed char* rec_nodes, signed char* rec_edges,
+                    signed char* in_nodes, signed char* in_edges, gib_stream stream);
+/* row ctl[0] (device int) of rec_nodes / rec_edges into in_nodes / in_edges */
+int gib_rl_restore(int B, int N, int F, int Ef, const signed char* rec_nodes, const signed char* rec_edges,
+                   const int* ctl, signed char* in_nodes, signed char* in_edges, gib_stream stream);
+/* out[g, t] = p[t, owner[g, t] - 1] for owner[g, t] in 1..B, else 0; owner / out [rows, Lw], p [Lw, B] */
+int gib_rl_gather(int B, int rows, int Lw, const float* owner, const float* p_a, const float* p_b, float* out_a,
+                  float* out_b, gib_stream stream);
+/* the gradient of gib_rl_gather: dp [Lw, B] = 0, then dp[t, owner[g, t] - 1] = d[g, t].  d_a or d_b may be null
+ * (that table is then not written).  Each (round, slot) belongs to at most one molecule. */
+int gib_rl_scatter_grad(int B, int rows, int Lw, const float* owner, const float* d_a, const float* d_b, float* dp_a,
+                        float* dp_b, gib_stream stream);
+/* dlogits[b, :] = dp[r, b] * p * (onehot(a) - softmax(logits[b])) with a = act[r, b], p = softmax(logits[b])[a] (0 for
+ * an a outside [0, apd)), and p into p_out[r, b] when p_out is given; r = ctl[0] (device int), or 0 when ctl is null.
+ * The softmax is computed exactly as gib_rl_sample_round computes p_a / p_b. */
+int gib_rl_dlogits(int B, int apd, const float* logits, const int* act, const float* dp, const int* ctl,
+                   float* dlogits, float* p_out, gib_stream stream);
+/* ctl[0] += 1 on the device (the round counter of a captured backward round) */
+int gib_rl_next_round(int* ctl, gib_stream stream);
+
 /* ---- measurement hooks: CUDA-event timing per kernel class on the launching stream.
  *      class 0 = forward/dX launches of the tensor-core kernel, 1 = its weight-gradient launches, 2 = scatter-aggregate (K2),
  *      3 / 4 = forward/dX and weight-gradient GEMMs on the fp32 SIMT kernels.  GIB_PROFILE_CLASSES entries per array.
