@@ -39,6 +39,17 @@ class DwProblem(ctypes.Structure):
                 ("cs", c_ll), ("m_dev", c_p), ("base_dev", c_p)]
 
 
+class BatchCtl(ctypes.Structure):
+    """mirror of `gib_batch_ctl` (include/gib200.h): the live molecule count and loss scale of a captured batch"""
+    _fields_ = [("live", c_i), ("scale", c_f)]
+
+
+class EvalPass(ctypes.Structure):
+    """mirror of `gib_eval_pass` (include/gib200.h): the device-resident state of one validation pass"""
+    _fields_ = [("batch_loss", c_p), ("lik", c_p), ("lik_len", c_ll), ("n_slots", c_i), ("idx", c_i),
+                ("n_structures", c_f), ("flags", c_i), ("clipped", c_i), ("reserved", c_i)]
+
+
 MODEL_ID = {"GGNN": 0, "MNN": 1, "AttGGNN": 2, "EMN": 3}
 HDR_INTS = 16
 HDR_E, HDR_P, HDR_TYPE_COUNT, HDR_TYPE_BASE, HDR_FLAGS, HDR_CAPACITY = 0, 1, 2, 6, 11, 12
@@ -84,6 +95,10 @@ _PROTOS = {
     "gib_validation_nll": (c_i, [c_p, c_p, c_i, c_i, c_p, c_p]),
     "gib_sum_scaled": (c_i, [c_p, c_i, c_f, c_p, c_p]),
     "gib_fill_zero": (c_i, [c_p, c_sz, c_p]),
+    "gib_kl_loss_fwd_bwd_ctl": (c_i, [c_p, c_p, c_i, c_i, c_p, c_p, c_p, c_p]),
+    "gib_sum_scaled_ctl": (c_i, [c_p, c_i, c_p, c_p, c_p]),
+    "gib_validation_nll_ctl": (c_i, [c_p, c_p, c_i, c_i, c_p, c_p, c_p]),
+    "gib_eval_collect": (c_i, [c_p, c_p, c_p, c_i, c_i, c_p, c_p, c_p, c_p]),
     "gib_adam_step": (c_i, [c_p, c_p, c_p, c_p, c_ll, c_ll, c_d, c_d, c_d, c_d, c_d, c_d, c_p]),
     "gib_sample_actions": (c_i, [c_p, c_i, c_i, c_p, c_p, c_p, c_p]),
     "gib_generation_scratch_bytes": (c_sz, [c_i]),

@@ -21,10 +21,19 @@ void set_error(const char* fmt, ...) {
 
 // ---- KL-divergence loss + gradient (Workflow.py:833-860), one CTA per molecule ---------
 __global__ void __launch_bounds__(256) kl_loss_kernel(const float* __restrict__ out, const float* __restrict__ target,
-                                                      int apd, float grad_scale, float* __restrict__ loss_rows,
-                                                      float* __restrict__ dout) {
+                                                      int apd, float grad_scale, const gib_batch_ctl* ctl,
+                                                      float* __restrict__ loss_rows, float* __restrict__ dout) {
   __shared__ float sm[8];
   const int b = blockIdx.x;
+  if (ctl) {                                    // a partial batch: rows past the live count are padding
+    if (b >= ctl->live) {
+      if (dout)
+        for (int k = threadIdx.x; k < apd; k += 256) dout[(size_t)b * apd + k] = 0.f;
+      if (threadIdx.x == 0 && loss_rows) loss_rows[b] = 0.f;
+      return;
+    }
+    grad_scale = ctl->scale;
+  }
   const float* o = out + (size_t)b * apd;
   const float* t = target + (size_t)b * apd;
   float mx = -INFINITY, ts = 0.f;
@@ -51,9 +60,13 @@ __global__ void __launch_bounds__(256) kl_loss_kernel(const float* __restrict__ 
 //      which the reference filters out afterwards (Analyzer.py:756) -----------------------------------------------
 __global__ void __launch_bounds__(256) validation_nll_kernel(const float* __restrict__ out,
                                                              const float* __restrict__ target, int apd,
-                                                             float* __restrict__ nll) {
+                                                             const gib_batch_ctl* ctl, float* __restrict__ nll) {
   __shared__ float sm[8];
   const int b = blockIdx.x;
+  if (ctl && b >= ctl->live) {
+    if (threadIdx.x == 0) nll[b] = 0.f;
+    return;
+  }
   const float* o = out + (size_t)b * apd;
   const float* t = target + (size_t)b * apd;
   float mx = -INFINITY, ts = 0.f;
@@ -147,6 +160,63 @@ int sample_actions_launch(const float* out, int B, int apd, const float* uniform
   sample_actions_kernel<<<B, 256, 0, st>>>(out, apd, uniforms, action, lik, gate ? *gate : RoundGate{});
   GIB_LAUNCH_CHECK();
   return 0;
+}
+
+// ---- the per-batch tail of a validation pass (include/gib200.h: gib_eval_collect), one CTA --------------------------
+constexpr int kEvalThreads = 1024;
+__global__ void __launch_bounds__(kEvalThreads) eval_collect_kernel(const float* __restrict__ kl_rows,
+                                                                    const float* __restrict__ nll_rows,
+                                                                    const float* __restrict__ target, int B, int apd,
+                                                                    const gib_batch_ctl* __restrict__ ctl,
+                                                                    const int* __restrict__ count_ws,
+                                                                    gib_eval_pass* pass) {
+  __shared__ float sm[kEvalThreads / 32];
+  __shared__ int warp_kept[kEvalThreads / 32];
+  const int live = max(0, min(B, ctl->live));
+  const int idx = pass->idx;     // read by every thread before the first barrier; thread 0 advances it at the end
+  float kl = 0.f, ns = 0.f;
+  for (int b = threadIdx.x; b < live; b += kEvalThreads) {
+    kl += kl_rows[b];
+    ns += target[(size_t)b * apd + apd - 1];      // the unnormalised target: its last column counts the sub-graphs
+  }
+  kl = block_reduce<kEvalThreads>(kl, sm, false);
+  ns = block_reduce<kEvalThreads>(ns, sm, false);
+  // likelihood[~isnan(likelihood)] written from idx * B: an order-preserving compaction, one CTA-wide scan per chunk
+  float* lik = pass->lik;
+  const long long base = (long long)idx * B;
+  int kept = 0;                  // uniform across the CTA
+  if (lik) {
+    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+    const long long len = pass->lik_len;
+    for (int c = 0; c < live; c += kEvalThreads) {
+      const int b = c + threadIdx.x;
+      const float v = b < live ? nll_rows[b] : NAN;
+      const bool keep = !isnan(v);
+      const unsigned m = __ballot_sync(0xffffffffu, keep);
+      if (lane == 0) warp_kept[wid] = __popc(m);
+      __syncthreads();
+      int before = __popc(m & ((1u << lane) - 1u)), total = 0;
+      for (int w = 0; w < kEvalThreads / 32; ++w) {
+        const int x = warp_kept[w];
+        before += w < wid ? x : 0;
+        total += x;
+      }
+      const long long pos = base + kept + before;
+      if (keep && pos < len) lik[pos] = v;
+      kept += total;
+      __syncthreads();           // warp_kept is rewritten by the next chunk
+    }
+  }
+  if (threadIdx.x == 0) {
+    if (pass->batch_loss && idx >= 0 && idx < pass->n_slots) pass->batch_loss[idx] = kl / (float)live;
+    if (lik) {
+      const long long past = base + kept - pass->lik_len;     // kept rows at positions >= lik_len
+      pass->clipped += (int)(past <= 0 ? 0 : past < kept ? past : kept);
+    }
+    pass->n_structures += ns;
+    pass->flags |= count_ws[HDR_FLAGS];
+    pass->idx = idx + 1;
+  }
 }
 
 }  // namespace gib
@@ -292,23 +362,42 @@ int gib_model_backward_part(const gib_dims* d, const int* hdr, const void* nodes
 int gib_kl_loss_fwd_bwd(const float* out, const float* target, int B, int apd, float grad_scale, float* loss_rows,
                         float* dout, gib_stream stream) {
   if (B <= 0) return 0;
-  kl_loss_kernel<<<B, 256, 0, ST(stream)>>>(out, target, apd, grad_scale, loss_rows, dout);
+  kl_loss_kernel<<<B, 256, 0, ST(stream)>>>(out, target, apd, grad_scale, nullptr, loss_rows, dout);
+  GIB_LAUNCH_CHECK();
+  return 0;
+}
+int gib_kl_loss_fwd_bwd_ctl(const float* out, const float* target, int B, int apd, const gib_batch_ctl* ctl,
+                            float* loss_rows, float* dout, gib_stream stream) {
+  if (!ctl) { set_error("gib_kl_loss_fwd_bwd_ctl: ctl is null"); return -1; }
+  if (B <= 0) return 0;
+  kl_loss_kernel<<<B, 256, 0, ST(stream)>>>(out, target, apd, 0.f, ctl, loss_rows, dout);
   GIB_LAUNCH_CHECK();
   return 0;
 }
 
 // out[0] = scale * sum_b rows[b], fixed order (one CTA): the batch-mean of the per-molecule losses without an ATen
 // reduction inside a captured step
+// ctl != null: the first min(n, ctl->live) rows, scaled by ctl->scale
 __global__ void __launch_bounds__(256) sum_scaled_kernel(const float* __restrict__ rows, int n, float scale,
-                                                         float* __restrict__ out) {
+                                                         const gib_batch_ctl* ctl, float* __restrict__ out) {
   __shared__ float sm[8];
+  if (ctl) {
+    n = min(n, ctl->live);
+    scale = ctl->scale;
+  }
   float s = 0.f;
   for (int i = threadIdx.x; i < n; i += 256) s += rows[i];
   s = block_reduce<256>(s, sm, false);
   if (threadIdx.x == 0) out[0] = s * scale;
 }
 int gib_sum_scaled(const float* rows, int n, float scale, float* out, gib_stream stream) {
-  sum_scaled_kernel<<<1, 256, 0, ST(stream)>>>(rows, n, scale, out);
+  sum_scaled_kernel<<<1, 256, 0, ST(stream)>>>(rows, n, scale, nullptr, out);
+  GIB_LAUNCH_CHECK();
+  return 0;
+}
+int gib_sum_scaled_ctl(const float* rows, int n, const gib_batch_ctl* ctl, float* out, gib_stream stream) {
+  if (!ctl) { set_error("gib_sum_scaled_ctl: ctl is null"); return -1; }
+  sum_scaled_kernel<<<1, 256, 0, ST(stream)>>>(rows, n, 0.f, ctl, out);
   GIB_LAUNCH_CHECK();
   return 0;
 }
@@ -320,7 +409,27 @@ int gib_fill_zero(void* ptr, size_t bytes, gib_stream stream) {
 
 int gib_validation_nll(const float* out, const float* target, int B, int apd, float* nll, gib_stream stream) {
   if (B <= 0) return 0;
-  validation_nll_kernel<<<B, 256, 0, ST(stream)>>>(out, target, apd, nll);
+  validation_nll_kernel<<<B, 256, 0, ST(stream)>>>(out, target, apd, nullptr, nll);
+  GIB_LAUNCH_CHECK();
+  return 0;
+}
+int gib_validation_nll_ctl(const float* out, const float* target, int B, int apd, const gib_batch_ctl* ctl, float* nll,
+                           gib_stream stream) {
+  if (!ctl) { set_error("gib_validation_nll_ctl: ctl is null"); return -1; }
+  if (B <= 0) return 0;
+  validation_nll_kernel<<<B, 256, 0, ST(stream)>>>(out, target, apd, ctl, nll);
+  GIB_LAUNCH_CHECK();
+  return 0;
+}
+
+int gib_eval_collect(const float* kl_rows, const float* nll_rows, const float* target, int B, int apd,
+                     const gib_batch_ctl* ctl, const void* count_ws, gib_eval_pass* pass, gib_stream stream) {
+  if (B <= 0 || apd <= 0 || !kl_rows || !nll_rows || !target || !ctl || !count_ws || !pass) {
+    set_error("gib_eval_collect: B = %d, apd = %d (both > 0) and every pointer non-null", B, apd);
+    return -1;
+  }
+  eval_collect_kernel<<<1, kEvalThreads, 0, ST(stream)>>>(kl_rows, nll_rows, target, B, apd, ctl,
+                                                          reinterpret_cast<const int*>(count_ws), pass);
   GIB_LAUNCH_CHECK();
   return 0;
 }

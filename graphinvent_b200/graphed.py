@@ -16,7 +16,16 @@ keeps every data-dependent extent in device memory, so the captured launch param
 content; a batch with more bond entries than `entry_capacity` is truncated and flagged, `check()` reports it.
 
 The optimizer is stepped eagerly after the graph (its step count / learning-rate schedule are host state); with
-`optim.FlatAdam` that is one more launch.  There is no CPU path.
+`optim.FlatAdam` that is one more launch.  There is no CPU path.  A batch may hold fewer than `batch_size` molecules
+(the tail batch of each block of the reference's loader): the live count and the loss scale are device memory
+(`gib_batch_ctl`), so the same graph serves it.
+
+The validation pass (`Workflow.validation_epoch`, `Analyzer.get_validation_likelihood`) as replays of one captured
+graph per batch (`EvalStep`), optionally on a TrainStep's buffers:
+
+    ev = graphinvent_b200.graphed.EvalStep(model, batch_size=B, entry_capacity=E_cap, share=step)
+    val_loss = ev.validation_epoch(valid_loader)
+    lik, avg = ev.validation_likelihood(loader, n_samples)
 
 Generation rounds as replays of ONE captured round (`GraphedGenerator`, a drop-in for `generation.GraphGenerator`):
 
@@ -42,10 +51,35 @@ import types
 import torch
 
 from . import functional as F
-from ._lib import FLAG_MULTITYPE, FLAG_OVERFLOW, HDR_FLAGS, HDR_INTS, check, lib
+from ._lib import FLAG_MULTITYPE, FLAG_OVERFLOW, HDR_FLAGS, HDR_INTS, Dims, EvalPass, check, lib
 from .generation import GraphGenerator
 
 _u8 = torch.uint8
+
+
+def _set_ctl(ctl, live, denominator):
+    """gib_batch_ctl {live, 1 / denominator} by device-side fills: no host buffer that a queued copy could still read,
+    no synchronisation"""
+    ctl[0:1].fill_(live)
+    ctl[1:2].view(torch.float32).fill_(1.0 / denominator if denominator > 0 else 0.0)
+
+
+def _batch_rows(step, name, nodes, edges, target):
+    b = nodes.shape[0]
+    if not 0 <= b <= step.B:
+        raise ValueError(f"{name} was built for batches of up to {step.B} molecules, got {b}")
+    if edges.shape[0] != b or target.shape[0] != b:
+        raise ValueError(f"nodes, edges and target hold {b}, {edges.shape[0]} and {target.shape[0]} molecules")
+    return b
+
+
+def _load_rows(step, b, nodes, edges, target):
+    """rows [0, b) of the static inputs from the batch (pinned host tensors: asynchronous H2D), rows [b, B) zeroed:
+    empty molecules, which every model maps to finite logits"""
+    for dst, src in ((step.nodes, nodes), (step.edges, edges), (step.target, target)):
+        dst[:b].copy_(src, non_blocking=True)
+        if b < step.B:
+            dst[b:].zero_()
 
 
 class TrainStep:
@@ -87,6 +121,9 @@ class TrainStep:
         self.dout = torch.empty_like(self.out)
         self.rows = torch.empty(self.B, dtype=torch.float32, device=dev)
         self.loss = torch.zeros((), dtype=torch.float32, device=dev)
+        # gib_batch_ctl {live, scale}: the captured loss kernels read the live molecule count and the loss scale here
+        self.ctl = torch.zeros(2, dtype=torch.int32, device=dev)
+        _set_ctl(self.ctl, self.B, self.global_batch)
         total = sum(p.numel() for p in params)
         self.gflat = torch.zeros(total, dtype=torch.float32, device=dev)   # ONE bucket: grads are views of it
         self.views, o = [], 0
@@ -128,12 +165,12 @@ class TrainStep:
         check(lib.gib_model_pack(bd, F._ptr_table(self.params), F._ptr(self.packed), st), "gib_model_pack")
         check(lib.gib_model_forward(bd, self.hdr, F._ptr(self.nodes), F._ptr(self.edges), F._ptr(self.gbuf),
                                     F._ptr(self.packed), F._ptr(self.ws), F._ptr(self.out), st), "gib_model_forward")
-        # Workflow.loss (Workflow.py:833-860) with the batch-mean taken over the GLOBAL batch (data-parallel shards)
-        check(lib.gib_kl_loss_fwd_bwd(F._ptr(self.out), F._ptr(self.target), self.B, self.apd,
-                                      1.0 / self.global_batch, F._ptr(self.rows), F._ptr(self.dout), st),
-              "gib_kl_loss_fwd_bwd")
-        check(lib.gib_sum_scaled(F._ptr(self.rows), self.B, 1.0 / self.global_batch, F._ptr(self.loss), st),
-              "gib_sum_scaled")
+        # Workflow.loss (Workflow.py:833-860) over the live rows, the batch-mean taken over ctl's denominator (the
+        # GLOBAL batch of data-parallel shards); padding rows get dout = 0 and add exact zeros to every gradient
+        check(lib.gib_kl_loss_fwd_bwd_ctl(F._ptr(self.out), F._ptr(self.target), self.B, self.apd, F._ptr(self.ctl),
+                                          F._ptr(self.rows), F._ptr(self.dout), st), "gib_kl_loss_fwd_bwd_ctl")
+        check(lib.gib_sum_scaled_ctl(F._ptr(self.rows), self.B, F._ptr(self.ctl), F._ptr(self.loss), st),
+              "gib_sum_scaled_ctl")
         check(lib.gib_fill_zero(F._ptr(self.gflat), self.gflat.numel() * 4, st), "gib_fill_zero")
         self._backward(1 if self.world > 1 else 0)
 
@@ -170,17 +207,25 @@ class TrainStep:
         self._param_ptrs = [p.data_ptr() for p in self.params]
 
     # ---- one step -----------------------------------------------------------------------------------------
-    def load(self, nodes, edges, target):
-        """copy one batch into the static input buffers (pinned host tensors: asynchronous H2D)"""
-        if nodes.shape[0] != self.B:
-            raise ValueError(f"TrainStep was built for batches of {self.B} molecules, got {nodes.shape[0]}")
-        self.nodes.copy_(nodes, non_blocking=True)
-        self.edges.copy_(edges, non_blocking=True)
-        self.target.copy_(target, non_blocking=True)
+    def load(self, nodes, edges, target, global_batch=None):
+        """copy one batch of 0 <= b <= batch_size molecules into the static input buffers (pinned host tensors:
+        asynchronous H2D).  A short batch -- the tail batch of every block of the reference's BlockDataLoader -- fills
+        rows [0, b); rows [b, batch_size) become empty molecules whose loss rows and gradients are exact zeros.  The
+        loss is the batch mean over `global_batch` molecules: by default batch_size's `global_batch` for a full batch
+        and b for a short one (KLDivLoss(batchmean) on a b-row batch).  A data-parallel rank passes the global size
+        of a short global batch; a rank whose shard is empty runs with b = 0 and still joins the all-reduce."""
+        b = _batch_rows(self, "TrainStep", nodes, edges, target)
+        if global_batch is None:
+            if b < self.B and self.world > 1:
+                raise ValueError("a short batch on a data-parallel rank needs the global batch size: "
+                                 "load(..., global_batch=<molecules over all ranks>)")
+            global_batch = self.global_batch if b == self.B else b
+        _load_rows(self, b, nodes, edges, target)
+        _set_ctl(self.ctl, b, int(global_batch))
 
-    def __call__(self, nodes=None, edges=None, target=None):
+    def __call__(self, nodes=None, edges=None, target=None, global_batch=None):
         if nodes is not None:
-            self.load(nodes, edges, target)
+            self.load(nodes, edges, target, global_batch=global_batch)
         if [p.data_ptr() for p in self.params] != self._param_ptrs:
             self.capture()                        # the parameters moved (optimizer re-flattened them)
         for p, v in zip(self.params, self.views):
@@ -213,6 +258,180 @@ class TrainStep:
         if flags & FLAG_MULTITYPE and self.d.model == F.MODEL_ID["AttGGNN"]:
             raise RuntimeError("AttentionGGNN requires one bond type per bond (as the reference's AggregationMPNN does)")
         return flags
+
+
+# ---- the validation pass --------------------------------------------------------------------------------------
+class EvalStep:
+    """The validation pass as replays of ONE captured graph: K0 (capacity mode) -> forward -> KL loss rows
+    (`gib_kl_loss_fwd_bwd_ctl`, no dout) -> NLL rows (`gib_validation_nll_ctl`) -> `gib_eval_collect`, which writes the
+    batch's slot of the pass, compacts its non-NaN NLL rows into the likelihood buffer and counts its sub-graphs, all
+    on the device.  No backward, scratch or gradient bucket.
+
+        ev = graphinvent_b200.graphed.EvalStep(model, batch_size=B, entry_capacity=cap, share=step)
+        val_loss = ev.validation_epoch(valid_loader)              # Workflow.validation_epoch's value
+        lik, avg = ev.validation_likelihood(loader, n_samples)    # Analyzer.get_validation_likelihood's values
+        ev.check()                                                # raises if a batch of the last pass overflowed
+
+    The weights are packed once per pass, outside the graph, and a pass reads the device once, at its end.  Batches
+    of 0 <= b <= batch_size molecules are taken as `TrainStep` takes them; a loader of another batch size would move
+    the reference's write offsets (idx * batch_size), so it must yield at most `batch_size` molecules per batch.
+
+    `share=` a TrainStep of equal dims, capacity and input dtype: the pass runs on the step's static inputs, K0 buffers,
+    packed arena, forward workspace and logits, and allocates only its slots and its likelihood buffer.  The step's
+    graph rewrites everything it reads from its inputs (the weights repacked included), so training results do not
+    change; load the next batch into the step before its next replay.  The forward has no dropout: the model is
+    evaluated as in eval mode, whatever its dropout_p."""
+
+    def __init__(self, model, batch_size, entry_capacity, input_dtype=torch.float32, share=None, device=None):
+        params = list(model.parameters())
+        F._require_cuda(*params)
+        self.model = model
+        self.dev = device or params[0].device
+        self.B = int(batch_size)
+        self.capacity = int(entry_capacity)
+        self.code = 1 if input_dtype == torch.int8 else 0
+        C = model.constants
+        self.N = C.max_n_nodes
+        self.apd = self.N * (C.len_f_add_per_node + C.len_f_conn_per_node) + 1
+        self.d = F.make_dims(model, self.B, self.code)
+        F._check_params(model, self.d, params)
+        dev, bd = self.dev, ctypes.byref(self.d)
+        if share is not None:
+            key = tuple(getattr(self.d, n) for n, _ in Dims._fields_)
+            if (not isinstance(share, TrainStep) or tuple(getattr(share.d, n) for n, _ in Dims._fields_) != key
+                    or share.capacity != self.capacity or share.dev != torch.device(dev)):
+                raise ValueError("EvalStep(share=) needs a TrainStep of equal model dims, batch size, entry capacity, "
+                                 "input dtype and device")
+            self._share = share               # keeps the step's host header alive
+            for name in ("nodes", "edges", "target", "cws", "gbuf", "hdr_np", "hdr", "packed", "ws", "out",
+                         "workspace_bytes"):
+                setattr(self, name, getattr(share, name))
+        else:
+            in_dt = torch.int8 if self.code else torch.float32
+            self.nodes = torch.zeros(self.B, self.N, C.n_node_features, dtype=in_dt, device=dev)
+            self.edges = torch.zeros(self.B, self.N, self.N, C.n_edge_features, dtype=in_dt, device=dev)
+            self.target = torch.zeros(self.B, self.apd, dtype=torch.float32, device=dev)
+            probe = F.GraphBatch(self.d, self.edges, capacity=self.capacity)
+            self.cws, self.gbuf, self.hdr_np, self.hdr = probe.cws, probe.buf, probe.hdr_np, probe.hdr
+            self.packed = torch.empty(lib.gib_model_packed_bytes(bd), dtype=_u8, device=dev)
+            ws_bytes = lib.gib_model_workspace_bytes(bd, self.hdr)
+            if ws_bytes == 0:
+                check(-1, "gib_model_workspace_bytes")
+            self.workspace_bytes = ws_bytes
+            self.ws = torch.empty(ws_bytes, dtype=_u8, device=dev)
+            self.out = torch.empty(self.B, self.apd, dtype=torch.float32, device=dev)
+        self.rows = torch.zeros(self.B, dtype=torch.float32, device=dev)
+        self.nll = torch.zeros(self.B, dtype=torch.float32, device=dev)
+        self.ctl = torch.zeros(2, dtype=torch.int32, device=dev)
+        _set_ctl(self.ctl, self.B, self.B)
+        # gib_eval_pass: written from pinned memory at the start of a pass, read back once at its end
+        self._pass = torch.zeros(ctypes.sizeof(EvalPass), dtype=_u8, device=dev)
+        self._pass_host = torch.zeros(ctypes.sizeof(EvalPass), dtype=_u8, pin_memory=True)
+        self._pass_copied = torch.cuda.Event()
+        self.flags, self.clipped, self.batches = 0, 0, 0
+        self.graph = None
+        self.capture()
+
+    def _enqueue(self):
+        bd, st = ctypes.byref(self.d), F._stream(self.dev)
+        check(lib.gib_graph_count(bd, F._ptr(self.edges), F._ptr(self.cws), st), "gib_graph_count")
+        check(lib.gib_graph_fill(bd, F._ptr(self.edges), F._ptr(self.cws), self.hdr, F._ptr(self.gbuf), st),
+              "gib_graph_fill")
+        check(lib.gib_model_forward(bd, self.hdr, F._ptr(self.nodes), F._ptr(self.edges), F._ptr(self.gbuf),
+                                    F._ptr(self.packed), F._ptr(self.ws), F._ptr(self.out), st), "gib_model_forward")
+        check(lib.gib_kl_loss_fwd_bwd_ctl(F._ptr(self.out), F._ptr(self.target), self.B, self.apd, F._ptr(self.ctl),
+                                          F._ptr(self.rows), None, st), "gib_kl_loss_fwd_bwd_ctl")
+        check(lib.gib_validation_nll_ctl(F._ptr(self.out), F._ptr(self.target), self.B, self.apd, F._ptr(self.ctl),
+                                         F._ptr(self.nll), st), "gib_validation_nll_ctl")
+        check(lib.gib_eval_collect(F._ptr(self.rows), F._ptr(self.nll), F._ptr(self.target), self.B, self.apd,
+                                   F._ptr(self.ctl), F._ptr(self.cws), F._ptr(self._pass), st), "gib_eval_collect")
+
+    def capture(self):
+        """warm up outside capture (lazy per-device init, function attributes), then capture; the warm-up's pass
+        state is overwritten by the next pass's start"""
+        side = torch.cuda.Stream(self.dev)
+        side.wait_stream(torch.cuda.current_stream(self.dev))
+        with torch.cuda.stream(side):
+            self._enqueue()
+        torch.cuda.current_stream(self.dev).wait_stream(side)
+        torch.cuda.synchronize(self.dev)
+        g = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(g):
+            self._enqueue()
+        self.graph = g
+
+    # ---- one pass -----------------------------------------------------------------------------------------
+    def _begin(self, slots, lik):
+        params = list(self.model.parameters())
+        F._require_cuda(*params)
+        F._check_params(self.model, self.d, params)
+        st = F._stream(self.dev)
+        check(lib.gib_model_pack(ctypes.byref(self.d), F._ptr_table(params), F._ptr(self.packed), st),
+              "gib_model_pack")
+        desc = EvalPass(batch_loss=slots.data_ptr() if slots.numel() else None,
+                        lik=lik.data_ptr() if lik is not None and lik.numel() else None,
+                        lik_len=lik.numel() if lik is not None else 0, n_slots=slots.numel())
+        self._pass_copied.synchronize()            # the previous pass's copy has read the pinned buffer
+        self._pass_host.copy_(torch.frombuffer(bytearray(desc), dtype=_u8))
+        self._pass.copy_(self._pass_host, non_blocking=True)
+        self._pass_copied.record(torch.cuda.current_stream(self.dev))
+
+    def _replay(self, batch):
+        nodes, edges, target = batch
+        b = _batch_rows(self, "EvalStep", nodes, edges, target)
+        _load_rows(self, b, nodes, edges, target)
+        _set_ctl(self.ctl, b, b)
+        self.graph.replay()
+
+    def _end(self):
+        """the pass's one synchronising read: batch count, K0 flags OR-ed over its batches, clipped likelihood rows"""
+        desc = EvalPass.from_buffer_copy(bytes(self._pass.cpu().numpy()))
+        self.batches, self.flags, self.clipped = desc.idx, desc.flags, desc.clipped
+        return desc
+
+    @torch.no_grad()
+    def validation_epoch(self, loader):
+        """Workflow.validation_epoch (Workflow.py:813-831): the KLDivLoss(batchmean) of every batch into one of
+        len(loader) zero-initialised slots, their mean as a 0-d device tensor (NaN if a target row is all zero)"""
+        slots = torch.zeros(len(loader), dtype=torch.float32, device=self.dev)
+        self._begin(slots, None)
+        for idx, batch in enumerate(loader):
+            if idx >= slots.numel():
+                raise IndexError(f"the loader yielded more than len(loader) = {slots.numel()} batches")
+            self._replay(batch)
+        self._end()
+        return torch.mean(slots)
+
+    @torch.no_grad()
+    def validation_likelihood(self, loader, n_samples):
+        """Analyzer.get_validation_likelihood (Analyzer.py:734-778): the NLL of the "correct" actions of the first
+        batches (until idx * batch_size > min(100000, n_samples)), each batch's non-NaN rows written from
+        idx * batch_size into n * (max_n_nodes + 5) zeros; returns (likelihoods, sum(likelihoods) / n_structures)"""
+        n = min(100000, int(n_samples))
+        lik = torch.zeros(n * (self.N + 5), dtype=torch.float32, device=self.dev)
+        self._begin(lik[:0], lik)
+        for idx, batch in enumerate(loader):
+            if idx * self.B > n:
+                break
+            self._replay(batch)
+        desc = self._end()
+        if desc.clipped:
+            raise RuntimeError(f"{desc.clipped} likelihood rows fall past the end of the {lik.numel()}-element buffer "
+                               f"(n_samples = {n}, max_n_nodes + 5 = {self.N + 5}): the reference's slice assignment "
+                               "raises there too")
+        off = EvalPass.n_structures.offset
+        n_structures = self._pass[off:off + 4].view(torch.float32).clone()
+        return lik, torch.sum(lik, dim=0) / n_structures[0]
+
+    def check(self):
+        """raises if a batch of the last pass exceeded the entry capacity (or an AttentionGGNN batch had a bond of
+        several types); the read already happened at the end of the pass"""
+        if self.flags & FLAG_OVERFLOW:
+            raise RuntimeError(f"a batch held more bond entries than entry_capacity={self.capacity}; the results of "
+                               "that pass are invalid -- rebuild EvalStep with a larger capacity")
+        if self.flags & FLAG_MULTITYPE and self.d.model == F.MODEL_ID["AttGGNN"]:
+            raise RuntimeError("AttentionGGNN requires one bond type per bond (as the reference's AggregationMPNN does)")
+        return self.flags
 
 
 # ---- generation -----------------------------------------------------------------------------------------------

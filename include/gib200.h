@@ -165,6 +165,45 @@ int gib_fill_zero(void* ptr, size_t bytes, gib_stream stream);
  *      give NaN (the reference drops them afterwards, Analyzer.py:756). -------------------------------------- */
 int gib_validation_nll(const float* out, const float* target, int B, int apd, float* nll, gib_stream stream);
 
+/* ---- partial batches of a captured step: the live molecule count and the loss scale of the batch in the static
+ *      buffers, in DEVICE memory, written by the host before each replay.  The _ctl forms below take `ctl` instead of
+ *      a host scale; rows b >= ctl->live are padding: their loss / NLL row is +0 and their dout row is zero.  On a
+ *      batch with live == B they compute exactly what the host-argument forms compute with scale == ctl->scale. */
+typedef struct gib_batch_ctl {
+  int live;       /* molecules [0, live) of the B rows are real */
+  float scale;    /* gradient and sum scale (1 / the batch-mean's denominator) */
+} gib_batch_ctl;
+int gib_kl_loss_fwd_bwd_ctl(const float* out, const float* target, int B, int apd, const gib_batch_ctl* ctl,
+                            float* loss_rows, float* dout, gib_stream stream);   /* dout may be NULL */
+/* out[0] = ctl->scale * sum(rows[0..min(n, ctl->live))), the order gib_sum_scaled uses for those rows */
+int gib_sum_scaled_ctl(const float* rows, int n, const gib_batch_ctl* ctl, float* out, gib_stream stream);
+int gib_validation_nll_ctl(const float* out, const float* target, int B, int apd, const gib_batch_ctl* ctl,
+                           float* nll, gib_stream stream);
+
+/* ---- the per-batch tail of a validation pass (Workflow.validation_epoch, Workflow.py:813-831, and
+ *      Analyzer.get_validation_likelihood, Analyzer.py:734-778), one CTA.  `pass` is DEVICE memory; with
+ *      i = pass->idx (the batch cursor) and L = ctl->live:
+ *        batch_loss[i] = sum_{b<L} kl_rows[b] / L      when batch_loss != NULL and 0 <= i < n_slots (KLDivLoss batchmean)
+ *        lik[i*B + j] = j-th non-NaN nll_rows[b], b < L, in order   when lik != NULL; positions >= lik_len are not
+ *                       written and counted in `clipped` (the reference's slice assignment raises there)
+ *        n_structures += sum_{b<L} target[b, apd-1]
+ *        flags |= count_ws[GIB_HDR_FLAGS]              (the batch's K0 header)
+ *        idx += 1
+ *      Every sum runs in a fixed order. */
+typedef struct gib_eval_pass {
+  float* batch_loss;
+  float* lik;
+  long long lik_len;
+  int n_slots;
+  int idx;
+  float n_structures;
+  int flags;
+  int clipped;
+  int reserved;
+} gib_eval_pass;
+int gib_eval_collect(const float* kl_rows, const float* nll_rows, const float* target, int B, int apd,
+                     const gib_batch_ctl* ctl, const void* count_ws, gib_eval_pass* pass, gib_stream stream);
+
 /* ---- flat-bucket Adam step: replaces torch.optim.Adam.step() on the model parameters (constructed at
  *      Workflow.py:191,221,245, stepped at Workflow.py:795-796; same update rule, L2 weight decay, no amsgrad)
  *      with ONE launch over contiguous params / grads / exp_avg / exp_avg_sq of n floats.  `step` is the
