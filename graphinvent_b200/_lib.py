@@ -18,25 +18,29 @@ c_sz = ctypes.c_size_t
 
 
 class Dims(ctypes.Structure):
-    """mirror of `gib_dims` (include/gib200.h)"""
+    """mirror of `gib_dims` (include/gib200.h).  `tf32` is host-side only: the matmul precision the model entry
+    points run in for these dims (0 = 3xTF32, 1 = single-pass TF32), applied per call through gib_set_matmul_tf32
+    (functional.matmul_precision); it is not part of the C struct."""
     _fields_ = [(n, c_i) for n in (
         "model", "B", "N", "F", "Ef", "H", "M", "T", "msg_hidden", "msg_depth", "att_hidden", "att_depth",
         "eemb_hidden", "eemb_depth", "gather_width", "gatt_hidden", "gatt_depth", "gemb_hidden", "gemb_depth",
         "mlp1_hidden", "mlp1_depth", "mlp2_hidden", "mlp2_depth", "f_add", "f_conn")] + [("big", c_f), ("in_dtype", c_i)]
+    tf32 = 0
 
 
 class GemmProblem(ctypes.Structure):
     """mirror of `gib_gemm_problem` (include/gib200.h, test hooks)"""
     _fields_ = [("A", c_p), ("lda", c_i), ("W", c_p), ("ldw", c_i), ("W_hi", c_p), ("W_lo", c_p), ("C", c_p),
                 ("ldc", c_i), ("M", c_i), ("N", c_i), ("K", c_i), ("bias", c_p), ("act", c_i), ("mode", c_i),
-                ("aux", c_p), ("ldaux", c_i), ("n_store", c_i), ("n_valid", c_i), ("m_dev", c_p), ("base_dev", c_p)]
+                ("aux", c_p), ("ldaux", c_i), ("n_store", c_i), ("n_valid", c_i), ("m_dev", c_p), ("base_dev", c_p),
+                ("tf32", c_i)]
 
 
 class DwProblem(ctypes.Structure):
     """mirror of `gib_dw_problem` (include/gib200.h, test hooks)"""
     _fields_ = [("G", c_p), ("ldg", c_i), ("Nn", c_i), ("X", c_p), ("ldx", c_i), ("Kk", c_i), ("M", c_i),
                 ("dW", c_p), ("dbias", c_p), ("R", c_i), ("C", c_i), ("Rb", c_i), ("Rbp", c_i), ("rs", c_ll),
-                ("cs", c_ll), ("m_dev", c_p), ("base_dev", c_p)]
+                ("cs", c_ll), ("m_dev", c_p), ("base_dev", c_p), ("tf32", c_i)]
 
 
 class BatchCtl(ctypes.Structure):
@@ -61,6 +65,8 @@ _PROTOS = {
     "gib_version": (c_i, []),
     "gib_set_tensor_cores": (None, [c_i]),
     "gib_get_tensor_cores": (c_i, []),
+    "gib_set_matmul_tf32": (None, [c_i]),
+    "gib_get_matmul_tf32": (c_i, []),
     "gib_tc_debug": (None, [c_i]),
     "gib_device_sm_count": (c_i, []),
     "gib_scatter_variant": (None, [c_i]),

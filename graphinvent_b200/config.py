@@ -23,6 +23,20 @@ DEFAULTS = dict(
 )
 
 
+def tf32_enabled():
+    """True when torch would run a CUDA float32 matmul on single-pass TF32 tensor cores, which is then the precision of
+    this package's tensor-core GEMMs too (else 3xTF32, fp32-accurate).  torch's rule: the matmul backend's
+    `torch.backends.cuda.matmul.fp32_precision`, or the global `torch.backends.fp32_precision` when the backend's is
+    "none"; "tf32" means TF32.  `torch.set_float32_matmul_precision("high")` and `("medium")` show up as "tf32" there.
+    Only these two values are read: the legacy getters (`allow_tf32`, `get_float32_matmul_precision`) raise after a
+    mix of the legacy and the new setters."""
+    import torch
+    p = getattr(torch.backends.cuda.matmul, "fp32_precision", "none")
+    if p == "none":
+        p = getattr(torch.backends, "fp32_precision", "none")
+    return p == "tf32"
+
+
 def make_constants(model="GGNN", **overrides):
     d = dict(DEFAULTS, model=model)
     d.update(overrides)

@@ -233,6 +233,8 @@ const char* gib_last_error(void) { return g_err; }
 int gib_version(void) { return 205; }
 void gib_set_tensor_cores(int on) { g_use_tc = on != 0; }
 int gib_get_tensor_cores(void) { return g_use_tc ? 1 : 0; }
+void gib_set_matmul_tf32(int on) { g_matmul_tf32 = on != 0; }
+int gib_get_matmul_tf32(void) { return g_matmul_tf32; }
 void gib_tc_debug(int mode) { g_tc_debug = mode; }
 int gib_device_sm_count(void) { return device_sm_count(); }
 void gib_scatter_variant(int v) { g_scatter_variant = v; }
@@ -522,14 +524,14 @@ static GemmNT to_gemm_nt(const gib_gemm_problem& s) {
   p.A = s.A; p.lda = s.lda; p.B = s.W; p.ldb = s.ldw; p.B_hi = s.W_hi; p.B_lo = s.W_lo;
   p.C = s.C; p.ldc = s.ldc; p.M = s.M; p.N = s.N; p.K = s.K; p.bias = s.bias; p.act = s.act; p.mode = s.mode;
   p.aux = s.aux; p.ldaux = s.ldaux; p.n_store = s.n_store; p.n_valid = s.n_valid;
-  p.m_dev = s.m_dev; p.base_dev = s.base_dev;
+  p.m_dev = s.m_dev; p.base_dev = s.base_dev; p.tf32 = s.tf32;
   return p;
 }
 static GemmDW to_gemm_dw(const gib_dw_problem& s) {
   GemmDW q;
   q.G = s.G; q.ldg = s.ldg; q.Nn = s.Nn; q.X = s.X; q.ldx = s.ldx; q.Kk = s.Kk; q.M = s.M; q.dW = s.dW;
   q.dbias = s.dbias; q.R = s.R; q.C = s.C; q.Rb = s.Rb; q.Rbp = s.Rbp; q.rs = s.rs; q.cs = s.cs;
-  q.m_dev = s.m_dev; q.base_dev = s.base_dev;
+  q.m_dev = s.m_dev; q.base_dev = s.base_dev; q.tf32 = s.tf32;
   return q;
 }
 // both scratch halves, sized as make_bwd sizes them: the largest group (with the same plan rows) and member

@@ -33,6 +33,9 @@ struct GemmNT {
   // group sizes K0 leaves in device memory, so no launch parameter depends on the batch content.
   const int* m_dev = nullptr;
   const int* base_dev = nullptr;
+  // Precision of the tensor-core kernels: 0 = 3xTF32 (fp32-accurate), 1 = single-pass TF32 (the hi*hi term only).
+  // The fp32 SIMT kernel ignores it.
+  int tf32 = 0;
 };
 
 struct GemmTN {  // kernel-level args of the split-K dW kernel
@@ -57,6 +60,7 @@ struct GemmDW {
   double work = 0;                                    // algorithmic FLOPs (0: derive)
   const int* m_dev = nullptr;                         // device-side row range inside buffers of M rows (see GemmNT)
   const int* base_dev = nullptr;
+  int tf32 = 0;                                       // tensor-core precision (see GemmNT)
 };
 
 constexpr int kTc3MaxProblems = 16;   // problems per launch of the tensor-core kernel
@@ -96,6 +100,8 @@ int device_sm_count();     // SMs of the current device (cached per device)
 void tc3_set_trace(long long* buf, int tiles);   // diagnosis: per-tile clock64 stamps of CTA 0
 extern bool g_use_tc;
 extern int g_tc_debug;
+// precision of the model entry points' tensor-core GEMMs on this host thread (gib_set_matmul_tf32; GemmNT::tf32)
+extern thread_local int g_matmul_tf32;
 
 int gemm_dw(const GemmDW& q, cudaStream_t st);
 // n <= 16 weight-gradient problems that may run as ONE grouped tensor-core launch + ONE reduction launch (siblings of a

@@ -10,6 +10,12 @@
 // is ~2^-22 relative).  The cross terms, 2^-11 of the main ones, get their own accumulator so that their roundings stay
 // away from the large running sum; the two are added in fp32 in the epilogue.
 //
+// Single-pass TF32 (template parameter TF1; GemmNT::tf32 / GemmDW::tf32, set when the caller accepts TF32 matmuls):
+// the product is the hi*hi term alone -- W from its hi plane only (raw W rounded in the kernel as gib_model_pack
+// rounds it), the activations rounded in registers or in the X transpose with the same round-to-nearest, one
+// accumulator, no lo loads and no cross-term MMAs.  Schedules, stage rings, epilogues, chains and the split-K
+// reduction are those of the 3xTF32 kernels.
+//
 // The kernels are persistent (one CTA per SM, work items = output tiles of up to 16 problems, or (tile, reduction
 // chunk) pairs in TN mode) and fed by one TMA lane through a ring of shared-memory stages (cp.async.bulk.tensor with
 // the 128-byte swizzle, mbarrier expect_tx per stage).
@@ -204,9 +210,22 @@ __device__ __forceinline__ void fence_proxy_async_all() { asm volatile("fence.pr
 // of the 10-bit mantissa, clear 13 bits; inf stays inf), lo = x - hi exact in fp32 (the tensor core reads its top
 // 19 bits).  With hi = trunc(x), lo would always carry the sign of x and its truncation would be a systematic bias
 // towards zero that adds up linearly over K; with hi rounded to nearest the sign of lo is random.
+__device__ __forceinline__ uint32_t tf32_rn(float x) { return (__float_as_uint(x) + 0x1000u) & 0xffffe000u; }
 __device__ __forceinline__ void split_tf32_rn(float x, uint32_t& hi, uint32_t& lo) {
-  hi = (__float_as_uint(x) + 0x1000u) & 0xffffe000u;
+  hi = tf32_rn(x);
   lo = __float_as_uint(x - __uint_as_float(hi));
+}
+// TF1: hi only (single-pass TF32); lo is left untouched and never read
+template <bool TF1>
+__device__ __forceinline__ void round_or_split(float x, uint32_t& hi, uint32_t& lo) {
+  if constexpr (TF1) hi = tf32_rn(x);
+  else split_tf32_rn(x, hi, lo);
+}
+// the accumulated product: main + cross-term accumulator, or (TF1) the main one alone
+template <bool TF1>
+__device__ __forceinline__ float acc_total(float acc, float accx) {
+  if constexpr (TF1) return acc;
+  else return acc + accx;
 }
 
 __device__ __forceinline__ void mma_tf32(float* d, const uint32_t* a, uint32_t b0, uint32_t b1) {
@@ -359,7 +378,7 @@ __device__ __forceinline__ void epi_store(const EpiArgs& e, int m, int n, float 
 }
 
 // ---- mma.sync kernel: NT with raw fp32 W ----
-template <int EPI>
+template <int EPI, bool TF1>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 tc3_gemm_kernel(const __grid_constant__ Maps maps, const Params P) {
   extern __shared__ uint8_t smem_raw[];
@@ -432,8 +451,8 @@ tc3_gemm_kernel(const __grid_constant__ Maps maps, const Params P) {
 #pragma unroll
           for (int j = 0; j < NI; ++j) {
             const int n = wn * WN + j * 8 + g8;
-            split_tf32_rn(lds32(sb + swz(n, k0)), bh[j][0], bl[j][0]);
-            split_tf32_rn(lds32(sb + swz(n, k1)), bh[j][1], bl[j][1]);
+            round_or_split<TF1>(lds32(sb + swz(n, k0)), bh[j][0], bl[j][0]);
+            round_or_split<TF1>(lds32(sb + swz(n, k1)), bh[j][1], bl[j][1]);
           }
 #pragma unroll
           for (int i = 0; i < MI; ++i) {
@@ -443,12 +462,14 @@ tc3_gemm_kernel(const __grid_constant__ Maps maps, const Params P) {
             a[2] = lds32(sa + swz(r0, k1)); a[3] = lds32(sa + swz(r1, k1));
             uint32_t ahi[4], alo[4];
 #pragma unroll
-            for (int e = 0; e < 4; ++e) split_tf32_rn(a[e], ahi[e], alo[e]);
+            for (int e = 0; e < 4; ++e) round_or_split<TF1>(a[e], ahi[e], alo[e]);
 #pragma unroll
             for (int j = 0; j < NI; ++j) {
               mma_tf32(acc[i][j], ahi, bh[j][0], bh[j][1]);
-              mma_tf32(accx[i][j], alo, bh[j][0], bh[j][1]);
-              mma_tf32(accx[i][j], ahi, bl[j][0], bl[j][1]);
+              if constexpr (!TF1) {
+                mma_tf32(accx[i][j], alo, bh[j][0], bh[j][1]);
+                mma_tf32(accx[i][j], ahi, bl[j][0], bl[j][1]);
+              }
             }
           }
         }
@@ -473,7 +494,8 @@ tc3_gemm_kernel(const __grid_constant__ Maps maps, const Params P) {
           for (int h = 0; h < 2; ++h) {
             const int m = w.m0 + wm * WM + i * 16 + h * 8 + g8;
             if (m >= Mrows) continue;
-            epi_store<EPI>(e, m, n, acc[i][j][2 * h] + accx[i][j][2 * h], acc[i][j][2 * h + 1] + accx[i][j][2 * h + 1], b);
+            epi_store<EPI>(e, m, n, acc_total<TF1>(acc[i][j][2 * h], accx[i][j][2 * h]),
+                           acc_total<TF1>(acc[i][j][2 * h + 1], accx[i][j][2 * h + 1]), b);
           }
       }
       if (P.flags) signal_tile<1, 32 * CONS_WARPS, 0>(P.flags + P.flag_off[w.p] + w.m0 / BM);
@@ -509,7 +531,7 @@ __device__ __forceinline__ uint32_t epi_off(int r, int c) { return (uint32_t)(c 
 //   warps 10-11       tile buffer -> C with 16-byte stores (rows < the live row count, columns < n_store) -> epi_empty,
 //                     then the chain hand-off of the tile.  They wait on nothing but epi_done, so a chain cannot
 //                     dead-lock on them.
-template <int EPI>
+template <int EPI, bool TF1>
 __global__ void __launch_bounds__(WG_THREADS, 1)
 tc3_wgmma_kernel(const __grid_constant__ Maps maps, const Params P) {
   constexpr bool SE = EPI != EPI_SPEC_GENERIC;
@@ -556,10 +578,10 @@ tc3_wgmma_kernel(const __grid_constant__ Maps maps, const Params P) {
         for (int kb = 0; kb < w.nkb; ++kb) {
           mbar_wait(&empty[stage], phase ^ 1);
           uint8_t* st = smem + stage * WG_STAGE_BYTES;
-          mbar_arrive_expect_tx(&full[stage], WG_STAGE_BYTES);
+          mbar_arrive_expect_tx(&full[stage], TF1 ? A_BYTES + WG_B_BYTES : WG_STAGE_BYTES);
           tma_load_2d(&maps.a[w.p], &full[stage], st, kb * BKF, base + w.m0);
           tma_load_2d(&maps.b[w.p], &full[stage], st + A_BYTES, kb * BKF, w.n0);
-          tma_load_2d(&maps.b_lo[w.p], &full[stage], st + A_BYTES + WG_B_BYTES, kb * BKF, w.n0);
+          if (!TF1) tma_load_2d(&maps.b_lo[w.p], &full[stage], st + A_BYTES + WG_B_BYTES, kb * BKF, w.n0);
           if (++stage == NST) { stage = 0; phase ^= 1; }
         }
       }
@@ -643,20 +665,22 @@ tc3_wgmma_kernel(const __grid_constant__ Maps maps, const Params P) {
 #pragma unroll
         for (int s = 0; s < 2; ++s) {
           const int k0 = (2 * hk + s) * 8 + t4, k1 = k0 + 4;
-          split_tf32_rn(lds32(sa + swz(r0, k0)), ah[s][0], al[s][0]);
-          split_tf32_rn(lds32(sa + swz(r0 + 8, k0)), ah[s][1], al[s][1]);
-          split_tf32_rn(lds32(sa + swz(r0, k1)), ah[s][2], al[s][2]);
-          split_tf32_rn(lds32(sa + swz(r0 + 8, k1)), ah[s][3], al[s][3]);
+          round_or_split<TF1>(lds32(sa + swz(r0, k0)), ah[s][0], al[s][0]);
+          round_or_split<TF1>(lds32(sa + swz(r0 + 8, k0)), ah[s][1], al[s][1]);
+          round_or_split<TF1>(lds32(sa + swz(r0, k1)), ah[s][2], al[s][2]);
+          round_or_split<TF1>(lds32(sa + swz(r0 + 8, k1)), ah[s][3], al[s][3]);
         }
         wgmma_fence();
 #pragma unroll
         for (int s = 0; s < 2; ++s) {
           const uint32_t ko = (2 * hk + s) * 32;
           const uint64_t dh = wgmma_desc_sw128(sa + A_BYTES + ko);
-          const uint64_t dl = wgmma_desc_sw128(sa + A_BYTES + WG_B_BYTES + ko);
           wgmma_m64n128k8_tf32(acc, ah[s], dh);
-          wgmma_m64n128k8_tf32(accx, al[s], dh);
-          wgmma_m64n128k8_tf32(accx, ah[s], dl);
+          if constexpr (!TF1) {
+            const uint64_t dl = wgmma_desc_sw128(sa + A_BYTES + WG_B_BYTES + ko);
+            wgmma_m64n128k8_tf32(accx, al[s], dh);
+            wgmma_m64n128k8_tf32(accx, ah[s], dl);
+          }
         }
         wgmma_commit();
         wgmma_wait<1>();
@@ -692,8 +716,8 @@ tc3_wgmma_kernel(const __grid_constant__ Maps maps, const Params P) {
             const uint32_t a = ebuf + epi_off(r0 + h * 8, c);
             float x[2] = {0.f, 0.f};
             if (AUX) lds64(a, x[0], x[1]);
-            sts64(a, epi_one<EPI>(acc[4 * j + 2 * h] + accx[4 * j + 2 * h], b[0], x[0], 0, 0),
-                  epi_one<EPI>(acc[4 * j + 2 * h + 1] + accx[4 * j + 2 * h + 1], b[1], x[1], 0, 0));
+            sts64(a, epi_one<EPI>(acc_total<TF1>(acc[4 * j + 2 * h], accx[4 * j + 2 * h]), b[0], x[0], 0, 0),
+                  epi_one<EPI>(acc_total<TF1>(acc[4 * j + 2 * h + 1], accx[4 * j + 2 * h + 1]), b[1], x[1], 0, 0));
           }
         }
         __syncwarp();
@@ -716,7 +740,8 @@ tc3_wgmma_kernel(const __grid_constant__ Maps maps, const Params P) {
         for (int h = 0; h < 2; ++h) {
           const int m = w.m0 + r0 + h * 8;
           if (m >= Mrows) continue;
-          epi_store<EPI>(e, m, n, acc[4 * j + 2 * h] + accx[4 * j + 2 * h], acc[4 * j + 2 * h + 1] + accx[4 * j + 2 * h + 1], b);
+          epi_store<EPI>(e, m, n, acc_total<TF1>(acc[4 * j + 2 * h], accx[4 * j + 2 * h]),
+                         acc_total<TF1>(acc[4 * j + 2 * h + 1], accx[4 * j + 2 * h + 1]), b);
         }
       }
       if (P.flags) signal_tile<1, 32 * CONS_WARPS, 0>(P.flags + P.flag_off[w.p] + w.m0 / BM);
@@ -737,6 +762,8 @@ __device__ __forceinline__ void sts128(uint32_t saddr, uint32_t x, uint32_t y, u
 // A 128-bit shared access is served 8 lanes at a time, and the 8 lanes of a group share everything but l: the raw
 // row k sits at 16-byte chunk l ^ (k & 7) with k & 7 = 4 (l1 ^ u0) + i, the plane row n = 4b + j at a ^ (n & 7) with
 // n & 7 = 4 l0 + j -- both take 8 distinct values over l, so reads and writes are free of bank conflicts.
+// TF1: the X_hi^T plane only.
+template <bool TF1>
 __device__ __forceinline__ void dw_transpose_block(uint32_t sx, uint32_t sp, int t, int valid) {
   const int l = t & 7, u = t >> 6;
   const int b = ((t >> 3) & 3) * 8 + l;
@@ -752,14 +779,16 @@ __device__ __forceinline__ void dw_transpose_block(uint32_t sx, uint32_t sp, int
   for (int j = 0; j < 4; ++j) {
     uint32_t hi[4], lo[4];
 #pragma unroll
-    for (int i = 0; i < 4; ++i) split_tf32_rn(j == 0 ? v[i].x : j == 1 ? v[i].y : j == 2 ? v[i].z : v[i].w, hi[i], lo[i]);
+    for (int i = 0; i < 4; ++i)
+      round_or_split<TF1>(j == 0 ? v[i].x : j == 1 ? v[i].y : j == 2 ? v[i].z : v[i].w, hi[i], lo[i]);
     const uint32_t o = swz(4 * b + j, 4 * a);
     sts128(sp + o, hi[0], hi[1], hi[2], hi[3]);
-    sts128(sp + DW_BN * BKF * 4 + o, lo[0], lo[1], lo[2], lo[3]);
+    if (!TF1) sts128(sp + DW_BN * BKF * 4 + o, lo[0], lo[1], lo[2], lo[3]);
   }
 }
 
 // ---- wgmma kernel: TN (weight-gradient partials) ----
+template <bool TF1>
 __global__ void __launch_bounds__(WG_THREADS, 1)
 tc3_wgmma_dw_kernel(const __grid_constant__ Maps maps, const Params P) {
   extern __shared__ uint8_t smem_raw[];
@@ -824,7 +853,7 @@ tc3_wgmma_dw_kernel(const __grid_constant__ Maps maps, const Params P) {
           mbar_wait(&raw_full[rs], rph);
           const uint32_t sx = smem_u32(smem + rs * DW_RAW_BYTES + A_BYTES);
           const uint32_t sp = smem_u32(smem + DW_OFF_PLANES + ps * DW_PLANE_BYTES);
-          for (int t = tt; t < 256; t += 32 * DW_TR_WARPS) dw_transpose_block(sx, sp, t, w.rows - kb * BKF);
+          for (int t = tt; t < 256; t += 32 * DW_TR_WARPS) dw_transpose_block<TF1>(sx, sp, t, w.rows - kb * BKF);
           asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy stores -> wgmma reads
           __syncwarp();
           if (lane == 0) {
@@ -873,17 +902,19 @@ tc3_wgmma_dw_kernel(const __grid_constant__ Maps maps, const Params P) {
           if (k1 >= valid) { a[2] = 0.f; a[3] = 0.f; }
           if (want_cs) { cs0 += a[0] + a[2]; cs1 += a[1] + a[3]; }
 #pragma unroll
-          for (int e = 0; e < 4; ++e) split_tf32_rn(a[e], ah[s][e], al[s][e]);
+          for (int e = 0; e < 4; ++e) round_or_split<TF1>(a[e], ah[s][e], al[s][e]);
         }
         wgmma_fence();
 #pragma unroll
         for (int s = 0; s < 2; ++s) {
           const uint32_t ko = (2 * hk + s) * 32;
           const uint64_t dh = wgmma_desc_sw128(sp + ko);
-          const uint64_t dl = wgmma_desc_sw128(sp + DW_BN * BKF * 4 + ko);
           wgmma_m64n128k8_tf32(acc, ah[s], dh);
-          wgmma_m64n128k8_tf32(accx, al[s], dh);
-          wgmma_m64n128k8_tf32(accx, ah[s], dl);
+          if constexpr (!TF1) {
+            const uint64_t dl = wgmma_desc_sw128(sp + DW_BN * BKF * 4 + ko);
+            wgmma_m64n128k8_tf32(accx, al[s], dh);
+            wgmma_m64n128k8_tf32(accx, ah[s], dl);
+          }
         }
         wgmma_commit();
         wgmma_wait<1>();
@@ -934,8 +965,8 @@ tc3_wgmma_dw_kernel(const __grid_constant__ Maps maps, const Params P) {
         for (int h = 0; h < 2; ++h) {
           const int m = w.m0 + r0 + h * 8;
           if (m >= Nn) continue;
-          epi_store<EPI_SPEC_LINEAR>(e, m, n, acc[4 * j + 2 * h] + accx[4 * j + 2 * h],
-                                     acc[4 * j + 2 * h + 1] + accx[4 * j + 2 * h + 1], b);
+          epi_store<EPI_SPEC_LINEAR>(e, m, n, acc_total<TF1>(acc[4 * j + 2 * h], accx[4 * j + 2 * h]),
+                                     acc_total<TF1>(acc[4 * j + 2 * h + 1], accx[4 * j + 2 * h + 1]), b);
         }
       }
       if (tr) P.trace[it * 16 + 6] = clock64();
@@ -1078,6 +1109,23 @@ struct DevInfo { int num_sms = 0; bool attr_done = false; };
 static std::mutex g_dev_mu;
 static DevInfo g_dev[64];
 
+// shared-memory attributes of one precision's kernels
+template <bool TF1>
+static int set_attributes() {
+  GIB_CUDA_TRY(cudaFuncSetAttribute(tc3_gemm_kernel<EPI_SPEC_GENERIC, TF1>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
+  GIB_CUDA_TRY(cudaFuncSetAttribute(tc3_gemm_kernel<EPI_SPEC_SELU, TF1>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
+  GIB_CUDA_TRY(cudaFuncSetAttribute(tc3_gemm_kernel<EPI_SPEC_LINEAR, TF1>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
+  GIB_CUDA_TRY(cudaFuncSetAttribute(tc3_gemm_kernel<EPI_SPEC_DSELU, TF1>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
+  GIB_CUDA_TRY(cudaFuncSetAttribute(tc3_gemm_kernel<EPI_SPEC_ADD, TF1>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
+  GIB_CUDA_TRY(cudaFuncSetAttribute(tc3_wgmma_kernel<EPI_SPEC_GENERIC, TF1>, cudaFuncAttributeMaxDynamicSharedMemorySize, WG_SMEM_BYTES));
+  GIB_CUDA_TRY(cudaFuncSetAttribute(tc3_wgmma_kernel<EPI_SPEC_SELU, TF1>, cudaFuncAttributeMaxDynamicSharedMemorySize, WG_EPI_SMEM_BYTES));
+  GIB_CUDA_TRY(cudaFuncSetAttribute(tc3_wgmma_kernel<EPI_SPEC_LINEAR, TF1>, cudaFuncAttributeMaxDynamicSharedMemorySize, WG_EPI_SMEM_BYTES));
+  GIB_CUDA_TRY(cudaFuncSetAttribute(tc3_wgmma_kernel<EPI_SPEC_DSELU, TF1>, cudaFuncAttributeMaxDynamicSharedMemorySize, WG_EPI_SMEM_BYTES));
+  GIB_CUDA_TRY(cudaFuncSetAttribute(tc3_wgmma_kernel<EPI_SPEC_ADD, TF1>, cudaFuncAttributeMaxDynamicSharedMemorySize, WG_EPI_SMEM_BYTES));
+  GIB_CUDA_TRY(cudaFuncSetAttribute(tc3_wgmma_dw_kernel<TF1>, cudaFuncAttributeMaxDynamicSharedMemorySize, DW_SMEM_BYTES));
+  return 0;
+}
+
 static int prepare(int* num_sms_out) {
   int dev = 0;
   GIB_CUDA_TRY(cudaGetDevice(&dev));
@@ -1086,17 +1134,8 @@ static int prepare(int* num_sms_out) {
   DevInfo& d = g_dev[dev];
   if (!d.attr_done) {   // function attributes are per device
     GIB_CUDA_TRY(cudaDeviceGetAttribute(&d.num_sms, cudaDevAttrMultiProcessorCount, dev));
-    GIB_CUDA_TRY(cudaFuncSetAttribute(tc3_gemm_kernel<EPI_SPEC_GENERIC>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
-    GIB_CUDA_TRY(cudaFuncSetAttribute(tc3_gemm_kernel<EPI_SPEC_SELU>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
-    GIB_CUDA_TRY(cudaFuncSetAttribute(tc3_gemm_kernel<EPI_SPEC_LINEAR>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
-    GIB_CUDA_TRY(cudaFuncSetAttribute(tc3_gemm_kernel<EPI_SPEC_DSELU>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
-    GIB_CUDA_TRY(cudaFuncSetAttribute(tc3_gemm_kernel<EPI_SPEC_ADD>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
-    GIB_CUDA_TRY(cudaFuncSetAttribute(tc3_wgmma_kernel<EPI_SPEC_GENERIC>, cudaFuncAttributeMaxDynamicSharedMemorySize, WG_SMEM_BYTES));
-    GIB_CUDA_TRY(cudaFuncSetAttribute(tc3_wgmma_kernel<EPI_SPEC_SELU>, cudaFuncAttributeMaxDynamicSharedMemorySize, WG_EPI_SMEM_BYTES));
-    GIB_CUDA_TRY(cudaFuncSetAttribute(tc3_wgmma_kernel<EPI_SPEC_LINEAR>, cudaFuncAttributeMaxDynamicSharedMemorySize, WG_EPI_SMEM_BYTES));
-    GIB_CUDA_TRY(cudaFuncSetAttribute(tc3_wgmma_kernel<EPI_SPEC_DSELU>, cudaFuncAttributeMaxDynamicSharedMemorySize, WG_EPI_SMEM_BYTES));
-    GIB_CUDA_TRY(cudaFuncSetAttribute(tc3_wgmma_kernel<EPI_SPEC_ADD>, cudaFuncAttributeMaxDynamicSharedMemorySize, WG_EPI_SMEM_BYTES));
-    GIB_CUDA_TRY(cudaFuncSetAttribute(tc3_wgmma_dw_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, DW_SMEM_BYTES));
+    GIB_TRY(set_attributes<false>());
+    GIB_TRY(set_attributes<true>());
     d.attr_done = true;
   }
   *num_sms_out = d.num_sms;
@@ -1126,6 +1165,7 @@ static bool presplit(const GemmNT& p) {
 
 bool g_use_tc = true;
 int g_tc_debug = 0;
+thread_local int g_matmul_tf32 = 0;
 
 void tc3_set_trace(long long* buf, int tiles) { tc3::g_trace = buf; tc3::g_trace_tiles = tiles; }
 
@@ -1148,8 +1188,32 @@ bool tc3_eligible(const GemmNT& p) {
          p.B_lo && al(p.A) && al(p.B_hi) && al(p.B_lo);
 }
 
+template <bool TF1>
+static void launch_nt_kernel(const tc3::Maps& maps, const tc3::Params& P, bool raw, int spec, int grid,
+                             cudaStream_t st) {
+  using namespace tc3;
+  if (raw) {
+    switch (spec) {
+      case EPI_SPEC_SELU: tc3_gemm_kernel<EPI_SPEC_SELU, TF1><<<grid, NUM_THREADS, SMEM_BYTES, st>>>(maps, P); break;
+      case EPI_SPEC_LINEAR: tc3_gemm_kernel<EPI_SPEC_LINEAR, TF1><<<grid, NUM_THREADS, SMEM_BYTES, st>>>(maps, P); break;
+      case EPI_SPEC_DSELU: tc3_gemm_kernel<EPI_SPEC_DSELU, TF1><<<grid, NUM_THREADS, SMEM_BYTES, st>>>(maps, P); break;
+      case EPI_SPEC_ADD: tc3_gemm_kernel<EPI_SPEC_ADD, TF1><<<grid, NUM_THREADS, SMEM_BYTES, st>>>(maps, P); break;
+      default: tc3_gemm_kernel<EPI_SPEC_GENERIC, TF1><<<grid, NUM_THREADS, SMEM_BYTES, st>>>(maps, P); break;
+    }
+  } else {
+    switch (spec) {
+      case EPI_SPEC_SELU: tc3_wgmma_kernel<EPI_SPEC_SELU, TF1><<<grid, WG_THREADS, WG_EPI_SMEM_BYTES, st>>>(maps, P); break;
+      case EPI_SPEC_LINEAR: tc3_wgmma_kernel<EPI_SPEC_LINEAR, TF1><<<grid, WG_THREADS, WG_EPI_SMEM_BYTES, st>>>(maps, P); break;
+      case EPI_SPEC_DSELU: tc3_wgmma_kernel<EPI_SPEC_DSELU, TF1><<<grid, WG_THREADS, WG_EPI_SMEM_BYTES, st>>>(maps, P); break;
+      case EPI_SPEC_ADD: tc3_wgmma_kernel<EPI_SPEC_ADD, TF1><<<grid, WG_THREADS, WG_EPI_SMEM_BYTES, st>>>(maps, P); break;
+      default: tc3_wgmma_kernel<EPI_SPEC_GENERIC, TF1><<<grid, WG_THREADS, WG_SMEM_BYTES, st>>>(maps, P); break;
+    }
+  }
+}
+
 // up to MAXP NT problems in one persistent launch; dep == nullptr: independent.  raw: every W is raw fp32 (split in
-// the kernel; mma.sync kernel), else every W comes as aligned (hi, lo) planes (wgmma kernel)
+// the kernel; mma.sync kernel), else every W comes as aligned (hi, lo) planes (wgmma kernel).  Every problem of a
+// launch has the same precision (GemmNT::tf32).
 static int launch_nt(const GemmNT* ps, const int* dep, int n, int* flags, bool raw, cudaStream_t st) {
   using namespace tc3;
   if (n < 1 || n > MAXP) { set_error("gemm_nt_tc3: %d problems (max %d)", n, MAXP); return -2; }
@@ -1167,9 +1231,11 @@ static int launch_nt(const GemmNT* ps, const int* dep, int n, int* flags, bool r
   int spec = -1;
   int slot[MAXP];                 // input index -> launch slot (-1: skipped, no rows)
   int flag_ints = 0;
+  const bool tf32 = ps[0].tf32 != 0;
   for (int i = 0; i < n; ++i) {
     const GemmNT& p = ps[i];
     slot[i] = -1;
+    if ((p.tf32 != 0) != tf32) { set_error("gemm_nt_tc3: problems of one launch with different precisions"); return -2; }
     if (p.M <= 0 || p.N <= 0) continue;
     if (!(raw ? tc_eligible(p) : presplit(p) && tc3_eligible(p))) {
       set_error("gemm_nt_tc3: operands violate the TMA alignment / pre-split contract");
@@ -1179,7 +1245,7 @@ static int launch_nt(const GemmNT* ps, const int* dep, int n, int* flags, bool r
     spec = (spec < 0 || spec == sp) ? sp : EPI_SPEC_GENERIC;     // one epilogue specialisation per launch
     GIB_TRY(make_map(&maps.a[np], p.A, p.M, p.K, p.lda, BM));
     GIB_TRY(make_map(&maps.b[np], raw ? p.B : p.B_hi, p.N, p.K, p.ldb, tbn));
-    if (!raw) GIB_TRY(make_map(&maps.b_lo[np], p.B_lo, p.N, p.K, p.ldb, tbn));
+    if (!raw && !tf32) GIB_TRY(make_map(&maps.b_lo[np], p.B_lo, p.N, p.K, p.ldb, tbn));
     if (!raw && (sp == EPI_SPEC_DSELU || sp == EPI_SPEC_ADD)) GIB_TRY(make_map(&maps.aux[np], p.aux, p.M, p.n_store, p.ldaux, BM));
     P.g[np] = p;
     P.n_tiles[np] = ceil_div(std::max(p.N, p.n_store), tbn);   // columns [N, n_store) are stored too (zeros / epi(0))
@@ -1212,23 +1278,8 @@ static int launch_nt(const GemmNT* ps, const int* dep, int n, int* flags, bool r
   }
   const int grid = (int)(tiles < num_sms ? tiles : num_sms);
   ProfScope prof(PROF_GEMM_NT, work, st, dyn, ndyn);
-  if (raw) {
-    switch (spec) {
-      case EPI_SPEC_SELU: tc3_gemm_kernel<EPI_SPEC_SELU><<<grid, NUM_THREADS, SMEM_BYTES, st>>>(maps, P); break;
-      case EPI_SPEC_LINEAR: tc3_gemm_kernel<EPI_SPEC_LINEAR><<<grid, NUM_THREADS, SMEM_BYTES, st>>>(maps, P); break;
-      case EPI_SPEC_DSELU: tc3_gemm_kernel<EPI_SPEC_DSELU><<<grid, NUM_THREADS, SMEM_BYTES, st>>>(maps, P); break;
-      case EPI_SPEC_ADD: tc3_gemm_kernel<EPI_SPEC_ADD><<<grid, NUM_THREADS, SMEM_BYTES, st>>>(maps, P); break;
-      default: tc3_gemm_kernel<EPI_SPEC_GENERIC><<<grid, NUM_THREADS, SMEM_BYTES, st>>>(maps, P); break;
-    }
-  } else {
-    switch (spec) {
-      case EPI_SPEC_SELU: tc3_wgmma_kernel<EPI_SPEC_SELU><<<grid, WG_THREADS, WG_EPI_SMEM_BYTES, st>>>(maps, P); break;
-      case EPI_SPEC_LINEAR: tc3_wgmma_kernel<EPI_SPEC_LINEAR><<<grid, WG_THREADS, WG_EPI_SMEM_BYTES, st>>>(maps, P); break;
-      case EPI_SPEC_DSELU: tc3_wgmma_kernel<EPI_SPEC_DSELU><<<grid, WG_THREADS, WG_EPI_SMEM_BYTES, st>>>(maps, P); break;
-      case EPI_SPEC_ADD: tc3_wgmma_kernel<EPI_SPEC_ADD><<<grid, WG_THREADS, WG_EPI_SMEM_BYTES, st>>>(maps, P); break;
-      default: tc3_wgmma_kernel<EPI_SPEC_GENERIC><<<grid, WG_THREADS, WG_SMEM_BYTES, st>>>(maps, P); break;
-    }
-  }
+  if (tf32) launch_nt_kernel<true>(maps, P, raw, spec, grid, st);
+  else launch_nt_kernel<false>(maps, P, raw, spec, grid, st);
   GIB_LAUNCH_CHECK();
   return 0;
 }
@@ -1325,9 +1376,11 @@ static int launch_tn(const GemmDW* qs, int n, int chunk_rows, float* const* part
   Params P;
   memset(&P, 0, sizeof(P));
   long long items = 0;
+  const bool tf32 = qs[0].tf32 != 0;
   for (int i = 0; i < n; ++i) {
     const GemmDW& q = qs[i];
     if (!tc3_dw_eligible(q)) { set_error("gemm_dw_tc3: operands violate the TMA alignment contract"); return -2; }
+    if ((q.tf32 != 0) != tf32) { set_error("gemm_dw_tc3: problems of one launch with different precisions"); return -2; }
     GIB_TRY(make_map(&maps.a[i], q.G, q.M, q.Nn, q.ldg, BKF));          // 32 x 32 boxes
     GIB_TRY(make_map(&maps.b[i], q.X, q.M, q.Kk, q.ldx, BKF));
     GemmNT& g = P.g[i];
@@ -1346,7 +1399,8 @@ static int launch_tn(const GemmDW* qs, int n, int chunk_rows, float* const* part
   P.chunk_rows = chunk_rows;
   P.trace = g_trace; P.trace_tiles = g_trace_tiles;
   const int grid = (int)(items < num_sms ? items : num_sms);
-  tc3_wgmma_dw_kernel<<<grid, WG_THREADS, DW_SMEM_BYTES, st>>>(maps, P);
+  if (tf32) tc3_wgmma_dw_kernel<true><<<grid, WG_THREADS, DW_SMEM_BYTES, st>>>(maps, P);
+  else tc3_wgmma_dw_kernel<false><<<grid, WG_THREADS, DW_SMEM_BYTES, st>>>(maps, P);
   GIB_LAUNCH_CHECK();
   return 0;
 }

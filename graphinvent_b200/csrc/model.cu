@@ -240,6 +240,7 @@ static bool msg_mlp_on_tc3(const Run& r) {
 
 int make_run(const gib_dims& d, const int* hdr, Run& r) {
   GIB_TRY(build_plan(d, r.pl));
+  r.tf32 = g_matmul_tf32;
   r.E = hdr[HDR_E];
   r.P = hdr[HDR_P];
   const int G = d.model == GIB_EMN ? 1 : d.Ef;
@@ -358,7 +359,7 @@ static int mlp_forward(const Run& r, const Mlp& m, const float* X0, const MlpAct
     p.B = r.packed + L.ow; p.ldb = L.Cp; p.B_hi = r.packed + L.ow_hi; p.B_lo = r.packed + L.ow_lo;
     p.M = rows; p.N = L.Rp; p.K = L.Cp;
     p.bias = L.pb >= 0 ? r.packed + L.ob : nullptr;
-    p.act = m.act; p.mode = EPI_ACT;
+    p.act = m.act; p.mode = EPI_ACT; p.tf32 = r.tf32;
     p.work = 2.0 * rows * (double)L.R * L.C;
     if (l == m.n && ext_out) {
       p.C = ext_out + (size_t)row0 * ext_ld; p.ldc = ext_ld; p.n_store = ext_valid; p.n_valid = ext_valid;
@@ -393,13 +394,14 @@ static int mlp_backward(const Run& r, const BwdBufs& bb, const Mlp& m, const flo
     q.R = L.R; q.C = L.C; q.Rb = L.Rb; q.Rbp = L.Rbp; q.rs = L.rs; q.cs = L.cs;
     q.scratch = r.scratch + bb.dw; q.half_floats = bb.dw_half;
     q.work = 2.0 * rows * (double)L.R * L.C;
+    q.tf32 = r.tf32;
     GIB_TRY(gemm_dw(q, r.st));
     if (l > 1 || dX0) {
       GemmNT p;
       p.A = G; p.lda = L.Rp;
       p.B = r.packed + L.owt; p.ldb = L.Rp; p.B_hi = r.packed + L.owt_hi; p.B_lo = r.packed + L.owt_lo;
       p.M = rows; p.N = L.Ctp; p.K = L.Rp;
-      p.n_store = L.Ctp; p.n_valid = L.Ctp;
+      p.n_store = L.Ctp; p.n_valid = L.Ctp; p.tf32 = r.tf32;
       p.work = 2.0 * rows * (double)L.R * L.Ct;
       if (l > 1) {
         p.C = (G == ping) ? pong : ping; p.ldc = L.Ctp;
@@ -493,7 +495,7 @@ static int mlp_forward_multi(const Run& r, const MlpJob* jobs, int n, int* flags
       p.B = r.packed + L.ow; p.ldb = L.Cp; p.B_hi = r.packed + L.ow_hi; p.B_lo = r.packed + L.ow_lo;
       p.M = j.rows; p.N = L.Rp; p.K = L.Cp;
       p.bias = L.pb >= 0 ? r.packed + L.ob : nullptr;
-      p.act = j.m->act; p.mode = EPI_ACT;
+      p.act = j.m->act; p.mode = EPI_ACT; p.tf32 = r.tf32;
       p.work = 2.0 * j.rows * (double)L.R * L.C;
       p.m_dev = j.m_dev; p.base_dev = j.base_dev;
       if (l == j.m->n && j.ext_out) {
@@ -617,7 +619,7 @@ static int mlp_backward_multi(const Run& r, const BwdBufs& bb, const MlpBwdJob* 
       p.work = 2.0 * j.rows * (double)L.R * L.Ct;
       p.C = const_cast<float*>(G[l - 1][i]); p.ldc = L.Ctp;
       p.mode = EPI_MUL_DACT; p.act = j.m->act; p.aux = Xin; p.ldaux = ldxin;
-      p.m_dev = j.m_dev; p.base_dev = j.base_dev;
+      p.m_dev = j.m_dev; p.base_dev = j.base_dev; p.tf32 = r.tf32;
       dep[nall] = last[i];
       layer_of[nall] = l;
       last[i] = nall++;
@@ -650,7 +652,7 @@ static int mlp_backward_multi(const Run& r, const BwdBufs& bb, const MlpBwdJob* 
     p1.M = j.rows; p1.N = L.Ctp; p1.K = L.Rp; p1.n_store = L.Ctp; p1.n_valid = L.Ctp;
     p1.work = 2.0 * j.rows * (double)L.R * L.Ct;
     p1.C = j.dX0; p1.ldc = j.ld_dx;
-    p1.m_dev = j.m_dev; p1.base_dev = j.base_dev;
+    p1.m_dev = j.m_dev; p1.base_dev = j.base_dev; p1.tf32 = r.tf32;
     if (j.dx_aux) { p1.mode = EPI_ADD; p1.aux = j.dx_aux; p1.ldaux = j.ld_dx; }
     else { p1.mode = EPI_ACT; p1.act = ACT_NONE; p1.bias = nullptr; }
     GIB_TRY(gemm_nt(p1, r.st));
@@ -673,7 +675,7 @@ static int mlp_backward_multi(const Run& r, const BwdBufs& bb, const MlpBwdJob* 
       q.R = L.R; q.C = L.C; q.Rb = L.Rb; q.Rbp = L.Rbp; q.rs = L.rs; q.cs = L.cs;
       q.scratch = r.scratch + bb.dw; q.half_floats = bb.dw_half;
       q.work = 2.0 * j.rows * (double)L.R * L.C;
-      q.m_dev = j.m_dev; q.base_dev = j.base_dev;
+      q.m_dev = j.m_dev; q.base_dev = j.base_dev; q.tf32 = r.tf32;
     }
   GIB_TRY(gemm_dw_group(qs, nq, plan_rows * depth, r.st));
   // the side-stream reduction reads only its scratch half; a first-generation / SIMT fallback job may still read
@@ -846,7 +848,7 @@ static int node_model_forward(const Run& r, float* out) {
       p.A = r.ws + L.msum[t]; p.lda = Mp; p.B = r.packed + ih.ow; p.ldb = ih.Cp; p.C = r.ws + L.gi[t]; p.ldc = ih.Rp;
       p.B_hi = r.packed + ih.ow_hi; p.B_lo = r.packed + ih.ow_lo;
       p.M = (int)S; p.N = ih.Rp; p.K = ih.Cp; p.bias = r.packed + ih.ob; p.act = ACT_NONE; p.mode = EPI_ACT;
-      p.n_store = p.n_valid = ih.Rp; p.work = 2.0 * S * (double)ih.R * ih.C;
+      p.n_store = p.n_valid = ih.Rp; p.work = 2.0 * S * (double)ih.R * ih.C; p.tf32 = r.tf32;
       GemmNT& q2 = ps[1];
       q2 = p;
       q2.A = h; q2.lda = Hp; q2.B = r.packed + hh.ow; q2.ldb = hh.Cp; q2.C = r.ws + L.gh[t]; q2.ldc = hh.Rp;
@@ -889,7 +891,7 @@ static int node_model_backward(const Run& r, const BwdBufs& bb, const float* out
       q.G = sc + bb.dgi; q.ldg = ih.Rp; q.Nn = ih.Rp; q.X = r.ws + L.msum[t]; q.ldx = Mp; q.Kk = ih.Cp; q.M = (int)S;
       q.dW = r.grads[ih.pw]; q.dbias = r.grads[ih.pb]; q.R = ih.R; q.C = ih.C; q.Rb = ih.Rb; q.Rbp = ih.Rbp;
       q.rs = ih.rs; q.cs = ih.cs; q.scratch = sc + bb.dw; q.half_floats = bb.dw_half;
-      q.work = 2.0 * S * (double)ih.R * ih.C;
+      q.work = 2.0 * S * (double)ih.R * ih.C; q.tf32 = r.tf32;
       qs[1] = q;
       GemmDW& q2 = qs[1];
       q2.G = sc + bb.dgh; q2.ldg = hh.Rp; q2.Nn = hh.Rp; q2.X = h; q2.ldx = Hp; q2.Kk = hh.Cp;
@@ -903,8 +905,9 @@ static int node_model_backward(const Run& r, const BwdBufs& bb, const float* out
       p.A = sc + bb.dgi; p.lda = ih.Rp; p.B = r.packed + ih.owt; p.ldb = ih.Rp; p.C = sc + bb.dmsum; p.ldc = Mp;
       p.B_hi = r.packed + ih.owt_hi; p.B_lo = r.packed + ih.owt_lo;
       p.M = (int)S; p.N = ih.Ctp; p.K = ih.Rp; p.mode = EPI_ACT; p.act = ACT_NONE; p.n_store = p.n_valid = ih.Ctp;
-      p.work = 2.0 * S * (double)ih.R * ih.C;
+      p.work = 2.0 * S * (double)ih.R * ih.C; p.tf32 = r.tf32;
       GemmNT& q2 = ps[1];
+      q2.tf32 = r.tf32;
       q2.A = sc + bb.dgh; q2.lda = hh.Rp; q2.B = r.packed + hh.owt; q2.ldb = hh.Rp; q2.C = dh; q2.ldc = Hp;
       q2.B_hi = r.packed + hh.owt_hi; q2.B_lo = r.packed + hh.owt_lo;
       q2.M = (int)S; q2.N = hh.Ctp; q2.K = hh.Rp; q2.mode = EPI_ADD; q2.aux = dh_dir; q2.ldaux = Hp;
@@ -1005,7 +1008,7 @@ static int emn_forward(const Run& r, float* out) {
     p.B_hi = r.packed + ih.ow_hi; p.B_lo = r.packed + ih.ow_lo;
     p.M = E; p.N = ih.Rp; p.K = ih.Cp; p.bias = r.packed + ih.ob; p.act = ACT_NONE; p.mode = EPI_ACT;
     p.n_store = p.n_valid = ih.Rp;
-    p.m_dev = live; p.base_dev = base;
+    p.m_dev = live; p.base_dev = base; p.tf32 = r.tf32;
     GIB_TRY(gemm_nt(p, r.st));
     // GRUCell(message) with hx=None (mpnn.py:488): h = 0, so W_hh h + b_hh = b_hh
     GIB_TRY(gru_fwd(r.ws + L.mem[t + 1], r.ws + L.gi[t], r.packed + hh.ob, nullptr, Hp, nullptr, E, live, r.st));
@@ -1052,14 +1055,14 @@ static int emn_backward(const Run& r, const BwdBufs& bb, const float* out, const
     q.G = sc + bb.dgi; q.ldg = ih.Rp; q.Nn = ih.Rp; q.X = r.ws + L.emsg[t]; q.ldx = Hp; q.Kk = ih.Cp; q.M = E;
     q.dW = r.grads[ih.pw]; q.dbias = r.grads[ih.pb]; q.R = ih.R; q.C = ih.C; q.Rb = ih.Rb; q.Rbp = ih.Rbp;
     q.rs = ih.rs; q.cs = ih.cs; q.scratch = sc + bb.dw; q.half_floats = bb.dw_half;
-    q.m_dev = live; q.base_dev = base;
+    q.m_dev = live; q.base_dev = base; q.tf32 = r.tf32;
     GIB_TRY(gemm_dw(q, r.st));
     GIB_TRY(colsum_add(r.grads[hh.pb], sc + bb.dgh, hh.Rp, E, hh.R, hh.Rb, hh.Rbp, live, r.st));  // d b_hh; d W_hh = 0
     GemmNT p;
     p.A = sc + bb.dgi; p.lda = ih.Rp; p.B = r.packed + ih.owt; p.ldb = ih.Rp; p.C = sc + bb.dmsum; p.ldc = Hp;
     p.B_hi = r.packed + ih.owt_hi; p.B_lo = r.packed + ih.owt_lo;
     p.M = E; p.N = ih.Ctp; p.K = ih.Rp; p.mode = EPI_ACT; p.act = ACT_NONE; p.n_store = p.n_valid = ih.Ctp;
-    p.m_dev = live; p.base_dev = base;
+    p.m_dev = live; p.base_dev = base; p.tf32 = r.tf32;
     GIB_TRY(gemm_nt(p, r.st));
     const float* EMm = r.ws + L.emm[t].y[pl.emsg.n];
     const float* ENm = r.ws + L.enm[t].y[pl.eatt.n];

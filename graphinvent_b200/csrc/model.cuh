@@ -94,6 +94,7 @@ struct Run {
   float* scratch = nullptr;     // backward scratch
   float* const* grads = nullptr;
   cudaStream_t st = nullptr;
+  int tf32 = 0;                 // precision of every tensor-core GEMM of the call (GemmNT::tf32), from gib_set_matmul_tf32
 };
 
 int build_plan(const gib_dims& d, Plan& pl);

@@ -5,12 +5,14 @@ forward/backward are `gib_model_forward` / `gib_model_backward`, plus the fused 
 PyTorch is used for device memory (caching allocator), streams and autograd plumbing only.
 No computation of the hot path happens in ATen, and there is no CPU path: CPU tensors raise.
 """
+import contextlib
 import ctypes
 
 import numpy as np
 import torch
 
 from ._lib import (Dims, FLAG_MULTITYPE, FLAG_OVERFLOW, HDR_E, HDR_FLAGS, HDR_INTS, HDR_P, MODEL_ID, check, lib)
+from .config import tf32_enabled
 
 _u8 = torch.uint8
 
@@ -23,10 +25,13 @@ def _stream(device):
     return ctypes.c_void_p(torch.cuda.current_stream(device).cuda_stream)
 
 
-def make_dims(model, batch, in_dtype=0):
+def make_dims(model, batch, in_dtype=0, tf32=None):
     """`in_dtype`: 0 = float32 batches (BlockDatasetLoader layout), 1 = int8 batches (the on-disk HDF5 type, read
-    directly by K0 and the first-layer kernels)"""
+    directly by K0 and the first-layer kernels).  `tf32`: precision of the tensor-core GEMMs of the model calls made
+    with these dims (`matmul_precision`), 1 = single-pass TF32, 0 = 3xTF32; None = torch's current setting
+    (`config.tf32_enabled`)."""
     d = Dims()
+    d.tf32 = int(tf32_enabled() if tf32 is None else bool(tf32))
     kw = model.dims()
     for name, _ in Dims._fields_:
         if name in ("model", "B", "big", "in_dtype"):
@@ -39,10 +44,27 @@ def make_dims(model, batch, in_dtype=0):
     return d
 
 
-def dims_key(model, batch, in_dtype=0):
-    """hashable copy of the `gib_dims` a model would be run with (two models with equal keys can share K0's output)"""
-    d = make_dims(model, batch, in_dtype)
-    return tuple(getattr(d, name) for name, _ in Dims._fields_)
+def dims_key(model, batch, in_dtype=0, tf32=None):
+    """hashable copy of the `gib_dims` a model would be run with, and its matmul precision (two models with equal keys
+    can share K0's output)"""
+    return key_of(make_dims(model, batch, in_dtype, tf32))
+
+
+def key_of(d):
+    """the fields of a `Dims` and its matmul precision, as a tuple"""
+    return tuple(getattr(d, name) for name, _ in Dims._fields_) + (d.tf32,)
+
+
+@contextlib.contextmanager
+def matmul_precision(d):
+    """run the model entry points called inside in the precision of `d` (gib_set_matmul_tf32 is per host thread and
+    read when a call launches its kernels; the previous setting is restored afterwards)"""
+    prev = lib.gib_get_matmul_tf32()
+    lib.gib_set_matmul_tf32(int(d.tf32))
+    try:
+        yield
+    finally:
+        lib.gib_set_matmul_tf32(prev)
 
 
 def input_dtype_code(nodes, edges):
@@ -191,8 +213,9 @@ class _MPNNFunction(torch.autograd.Function):
         ws = torch.empty(ws_bytes, dtype=_u8, device=dev)
         apd = d.N * d.f_add + d.N * d.f_conn + 1
         out = torch.empty(B, apd, dtype=torch.float32, device=dev)
-        check(lib.gib_model_forward(ctypes.byref(d), graph.hdr, _ptr(nodes), _ptr(edges), _ptr(graph.buf),
-                                    _ptr(packed), _ptr(ws), _ptr(out), st), "gib_model_forward")
+        with matmul_precision(d):
+            check(lib.gib_model_forward(ctypes.byref(d), graph.hdr, _ptr(nodes), _ptr(edges), _ptr(graph.buf),
+                                        _ptr(packed), _ptr(ws), _ptr(out), st), "gib_model_forward")
         model.last_stats = {"entries": graph.n_entries, "rows": graph.n_rows, "workspace_bytes": ws_bytes,
                             "flags": graph._flags, "capacity": graph.capacity}
         ctx.model, ctx.d, ctx.graph = model, d, graph
@@ -213,9 +236,10 @@ class _MPNNFunction(torch.autograd.Function):
             views.append(flat[o:o + n].view(shape))
             o += n
         scratch = torch.empty(lib.gib_model_bwd_scratch_bytes(ctypes.byref(d), graph.hdr), dtype=_u8, device=dev)
-        check(lib.gib_model_backward(ctypes.byref(d), graph.hdr, _ptr(nodes), _ptr(edges), _ptr(graph.buf),
-                                     _ptr(packed), _ptr(ws), _ptr(out), _ptr(dout), _ptr_table(views),
-                                     _ptr(scratch), _stream(dev)), "gib_model_backward")
+        with matmul_precision(d):             # the forward's precision, whatever torch's setting is by now
+            check(lib.gib_model_backward(ctypes.byref(d), graph.hdr, _ptr(nodes), _ptr(edges), _ptr(graph.buf),
+                                         _ptr(packed), _ptr(ws), _ptr(out), _ptr(dout), _ptr_table(views),
+                                         _ptr(scratch), _stream(dev)), "gib_model_backward")
         if model._grad_hook is not None:
             model._grad_hook(flat)      # e.g. the single NCCL all-reduce of data-parallel training
         return (None, None, None, *views)

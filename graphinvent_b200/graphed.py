@@ -44,6 +44,12 @@ The RL rollout of `Workflow.learning_step` as replays of captured rounds (`Graph
 
 Each rollout keeps only the int8 input of every round; `loss.backward()` recomputes each round's forward before its
 backward, one captured backward round per model that needs gradients.
+
+Matmul precision: each of these objects reads torch's float32 matmul precision once, at construction
+(`config.tf32_enabled`, exposed as its `tf32` attribute), and bakes it into its graphs -- single-pass TF32 GEMMs when
+the user allowed TF32, 3xTF32 otherwise -- as torch's own captured cuBLAS calls keep the math mode of their capture.
+Changing the setting afterwards does not change what a replay computes (the RL backward rounds included); build a new
+object to switch.
 """
 import ctypes
 import types
@@ -51,7 +57,7 @@ import types
 import torch
 
 from . import functional as F
-from ._lib import FLAG_MULTITYPE, FLAG_OVERFLOW, HDR_FLAGS, HDR_INTS, Dims, EvalPass, check, lib
+from ._lib import FLAG_MULTITYPE, FLAG_OVERFLOW, HDR_FLAGS, HDR_INTS, EvalPass, check, lib
 from .generation import GraphGenerator
 
 _u8 = torch.uint8
@@ -102,6 +108,7 @@ class TrainStep:
         self.edges = torch.zeros(self.B, N, N, Ef, dtype=in_dt, device=dev)
         self.target = torch.zeros(self.B, self.apd, dtype=torch.float32, device=dev)
         self.d = F.make_dims(model, self.B, self.code)
+        self.tf32 = bool(self.d.tf32)             # torch's matmul precision at construction, baked into the graphs
         d = self.d
         self.capacity = int(entry_capacity)
         # static buffers (addresses are baked into the graph)
@@ -163,8 +170,9 @@ class TrainStep:
         check(lib.gib_graph_fill(bd, F._ptr(self.edges), F._ptr(self.cws), self.hdr, F._ptr(self.gbuf), st),
               "gib_graph_fill")
         check(lib.gib_model_pack(bd, F._ptr_table(self.params), F._ptr(self.packed), st), "gib_model_pack")
-        check(lib.gib_model_forward(bd, self.hdr, F._ptr(self.nodes), F._ptr(self.edges), F._ptr(self.gbuf),
-                                    F._ptr(self.packed), F._ptr(self.ws), F._ptr(self.out), st), "gib_model_forward")
+        with F.matmul_precision(d):
+            check(lib.gib_model_forward(bd, self.hdr, F._ptr(self.nodes), F._ptr(self.edges), F._ptr(self.gbuf),
+                                        F._ptr(self.packed), F._ptr(self.ws), F._ptr(self.out), st), "gib_model_forward")
         # Workflow.loss (Workflow.py:833-860) over the live rows, the batch-mean taken over ctl's denominator (the
         # GLOBAL batch of data-parallel shards); padding rows get dout = 0 and add exact zeros to every gradient
         check(lib.gib_kl_loss_fwd_bwd_ctl(F._ptr(self.out), F._ptr(self.target), self.B, self.apd, F._ptr(self.ctl),
@@ -176,10 +184,11 @@ class TrainStep:
 
     def _backward(self, part):
         st = F._stream(self.dev)
-        check(lib.gib_model_backward_part(ctypes.byref(self.d), self.hdr, F._ptr(self.nodes), F._ptr(self.edges),
-                                          F._ptr(self.gbuf), F._ptr(self.packed), F._ptr(self.ws), F._ptr(self.out),
-                                          F._ptr(self.dout), F._ptr_table(self.views), F._ptr(self.scratch), part, st),
-              "gib_model_backward_part")
+        with F.matmul_precision(self.d):
+            check(lib.gib_model_backward_part(ctypes.byref(self.d), self.hdr, F._ptr(self.nodes), F._ptr(self.edges),
+                                              F._ptr(self.gbuf), F._ptr(self.packed), F._ptr(self.ws),
+                                              F._ptr(self.out), F._ptr(self.dout), F._ptr_table(self.views),
+                                              F._ptr(self.scratch), part, st), "gib_model_backward_part")
 
     def _enqueue_all(self):
         """the whole step's launch sequence, eagerly (warm-up, kernel-class timing)"""
@@ -294,14 +303,14 @@ class EvalStep:
         self.N = C.max_n_nodes
         self.apd = self.N * (C.len_f_add_per_node + C.len_f_conn_per_node) + 1
         self.d = F.make_dims(model, self.B, self.code)
+        self.tf32 = bool(self.d.tf32)             # torch's matmul precision at construction, baked into the graph
         F._check_params(model, self.d, params)
         dev, bd = self.dev, ctypes.byref(self.d)
         if share is not None:
-            key = tuple(getattr(self.d, n) for n, _ in Dims._fields_)
-            if (not isinstance(share, TrainStep) or tuple(getattr(share.d, n) for n, _ in Dims._fields_) != key
+            if (not isinstance(share, TrainStep) or F.key_of(share.d) != F.key_of(self.d)
                     or share.capacity != self.capacity or share.dev != torch.device(dev)):
                 raise ValueError("EvalStep(share=) needs a TrainStep of equal model dims, batch size, entry capacity, "
-                                 "input dtype and device")
+                                 "input dtype, matmul precision and device")
             self._share = share               # keeps the step's host header alive
             for name in ("nodes", "edges", "target", "cws", "gbuf", "hdr_np", "hdr", "packed", "ws", "out",
                          "workspace_bytes"):
@@ -337,8 +346,9 @@ class EvalStep:
         check(lib.gib_graph_count(bd, F._ptr(self.edges), F._ptr(self.cws), st), "gib_graph_count")
         check(lib.gib_graph_fill(bd, F._ptr(self.edges), F._ptr(self.cws), self.hdr, F._ptr(self.gbuf), st),
               "gib_graph_fill")
-        check(lib.gib_model_forward(bd, self.hdr, F._ptr(self.nodes), F._ptr(self.edges), F._ptr(self.gbuf),
-                                    F._ptr(self.packed), F._ptr(self.ws), F._ptr(self.out), st), "gib_model_forward")
+        with F.matmul_precision(self.d):
+            check(lib.gib_model_forward(bd, self.hdr, F._ptr(self.nodes), F._ptr(self.edges), F._ptr(self.gbuf),
+                                        F._ptr(self.packed), F._ptr(self.ws), F._ptr(self.out), st), "gib_model_forward")
         check(lib.gib_kl_loss_fwd_bwd_ctl(F._ptr(self.out), F._ptr(self.target), self.B, self.apd, F._ptr(self.ctl),
                                           F._ptr(self.rows), None, st), "gib_kl_loss_fwd_bwd_ctl")
         check(lib.gib_validation_nll_ctl(F._ptr(self.out), F._ptr(self.target), self.B, self.apd, F._ptr(self.ctl),
@@ -478,6 +488,7 @@ class GraphedGenerator(GraphGenerator):
         self.params = list(model.parameters())
         F._require_cuda(*self.params)
         self.d = F.make_dims(model, B, 0)
+        self.tf32 = bool(self.d.tf32)             # torch's matmul precision at construction, baked into the graph
         bd = ctypes.byref(self.d)
         F._check_params(model, self.d, self.params)
         self.entry_capacity = entry_capacity(B, N, self.Ef)
@@ -550,8 +561,10 @@ class GraphedGenerator(GraphGenerator):
         check(lib.gib_graph_fill(bd, F._ptr(edges), F._ptr(self.cws), self.hdr, F._ptr(self.gbuf), st),
               "gib_graph_fill")
         self._flags.bitwise_or_(self._hdr_flags)
-        check(lib.gib_model_forward(bd, self.hdr, F._ptr(self.nodes), F._ptr(edges), F._ptr(self.gbuf),
-                                    F._ptr(self.packed), F._ptr(self.ws), F._ptr(self.logits), st), "gib_model_forward")
+        with F.matmul_precision(d):
+            check(lib.gib_model_forward(bd, self.hdr, F._ptr(self.nodes), F._ptr(edges), F._ptr(self.gbuf),
+                                        F._ptr(self.packed), F._ptr(self.ws), F._ptr(self.logits), st),
+                  "gib_model_forward")
         check(lib.gib_generation_sample_round(
             self.batch_size, self.N, self.F, self.Ef, self.A, self.CH, self.n_imp_H, self.n_chirality,
             F._ptr(self.logits), self.apd, F._ptr(self.uniforms), F._ptr(self._state), F._ptr(self.action),
@@ -698,7 +711,8 @@ class GraphedGeneratorRL(GraphedGenerator):
         self.params = list(model.parameters())
         F._require_cuda(*self.params)
         self.d = F.make_dims(model, B, 1)                 # int8 model inputs: the 0/1 state, bit-exact logits
-        self._key = F.dims_key(model, B, 1)
+        self.tf32 = bool(self.d.tf32)   # torch's matmul precision at construction: rollouts and their backward rounds
+        self._key = F.key_of(self.d)
         bd = ctypes.byref(self.d)
         F._check_params(model, self.d, self.params)
         self.entry_capacity = entry_capacity(B, N, self.Ef)
@@ -741,7 +755,8 @@ class GraphedGeneratorRL(GraphedGenerator):
 
     def _check_pair(self, agent, prior):
         for m in (agent, prior):
-            if not hasattr(m, "dims") or type(m) is not type(self.model) or F.dims_key(m, self.batch_size, 1) != self._key:
+            if (not hasattr(m, "dims") or type(m) is not type(self.model)
+                    or F.dims_key(m, self.batch_size, 1, self.d.tf32) != self._key):
                 raise ValueError("GraphedGeneratorRL needs the agent and the prior to be this package's models of the "
                                  "generator's family with equal dims (Workflow.learning_step's deep copies); use "
                                  "generation.GraphGeneratorRL for other pairs")
@@ -773,10 +788,11 @@ class GraphedGeneratorRL(GraphedGenerator):
         check(lib.gib_graph_count(bd, F._ptr(self.in_edges), F._ptr(self.cws), st), "gib_graph_count")
         check(lib.gib_graph_fill(bd, F._ptr(self.in_edges), F._ptr(self.cws), self.hdr, F._ptr(self.gbuf), st),
               "gib_graph_fill")
-        for i, slot in enumerate(slots):
-            check(lib.gib_model_forward(bd, self.hdr, F._ptr(self.in_nodes), F._ptr(self.in_edges), F._ptr(self.gbuf),
-                                        F._ptr(self.packed[slot]), F._ptr(self.ws), F._ptr(self.logits[i]), st),
-                  "gib_model_forward")
+        with F.matmul_precision(self.d):
+            for i, slot in enumerate(slots):
+                check(lib.gib_model_forward(bd, self.hdr, F._ptr(self.in_nodes), F._ptr(self.in_edges),
+                                            F._ptr(self.gbuf), F._ptr(self.packed[slot]), F._ptr(self.ws),
+                                            F._ptr(self.logits[i]), st), "gib_model_forward")
 
     def _enqueue_round(self):
         B, N, st = self.batch_size, self.N, F._stream(self.device)
@@ -804,10 +820,11 @@ class GraphedGeneratorRL(GraphedGenerator):
         self._k0_forward((slot,))
         check(lib.gib_rl_dlogits(B, self.apd, F._ptr(self.logits[0]), F._ptr(self.act_rec), F._ptr(b.dp[slot]),
                                  F._ptr(b.ctl), F._ptr(b.dlogits), F._ptr(self.recomputed_p[slot]), st), "gib_rl_dlogits")
-        check(lib.gib_model_backward(ctypes.byref(self.d), self.hdr, F._ptr(self.in_nodes), F._ptr(self.in_edges),
-                                     F._ptr(self.gbuf), F._ptr(self.packed[slot]), F._ptr(self.ws),
-                                     F._ptr(self.logits[0]), F._ptr(b.dlogits), F._ptr_table(b.views[slot]),
-                                     F._ptr(b.scratch), st), "gib_model_backward")
+        with F.matmul_precision(self.d):
+            check(lib.gib_model_backward(ctypes.byref(self.d), self.hdr, F._ptr(self.in_nodes), F._ptr(self.in_edges),
+                                         F._ptr(self.gbuf), F._ptr(self.packed[slot]), F._ptr(self.ws),
+                                         F._ptr(self.logits[0]), F._ptr(b.dlogits), F._ptr_table(b.views[slot]),
+                                         F._ptr(b.scratch), st), "gib_model_backward")
         check(lib.gib_rl_next_round(F._ptr(b.ctl), st), "gib_rl_next_round")
 
     def _ensure_backward(self):

@@ -85,6 +85,15 @@ int gib_version(void);
 /* tensor-core 3xTF32 GEMM path on (default) / off (fp32 SIMT GEMMs only); process-wide switch */
 void gib_set_tensor_cores(int on);
 int gib_get_tensor_cores(void);
+/* Precision of the tensor-core GEMMs that the model entry points (gib_model_forward, gib_model_backward,
+ * gib_model_backward_part) launch from the calling host thread: 0 = 3xTF32, fp32-accurate (default); 1 = single-pass
+ * TF32, the hi*hi term of the 3xTF32 split alone (both operands rounded to TF32 to nearest, fp32 accumulation): the
+ * precision torch gives a CUDA fp32 matmul when its fp32_precision is "tf32".  The fp32 SIMT GEMMs (narrow APD output
+ * layers, small exact-mode problems) and every non-GEMM kernel are fp32 in both modes.  The setting is read when a
+ * call launches its kernels, so a CUDA graph captured around a call keeps the mode it was captured with.  No size
+ * query, workspace or packed-weight layout depends on it.  Thread-local; the other entry points ignore it. */
+void gib_set_matmul_tf32(int on);
+int gib_get_matmul_tf32(void);
 /* bit 3: GGNN / MNN message MLPs on one row per bond entry (the AttentionGGNN's layout) instead of one per message row.
  * bit 2: narrow outputs (N < 48, the APD heads) on the tensor-core kernel too (default: fp32 SIMT, see gemm_simt.cu).
  * bit 1: no dependent-chain launches (every MLP layer its own launch).
@@ -255,7 +264,9 @@ int gib_graph_gather(float* g, float* att, const float* en, const float* em, int
  * epi (mode): 0 act(acc + bias), 1 acc * act'(aux) (aux = the activation OUTPUT), 2 acc + aux (aux may alias C);
  * act 0 none / 1 selu / 2 tanh.  Columns [n_valid, n_store) are stored as zeros, columns >= n_store are not touched.
  * W_hi / W_lo (may be NULL): its TF32 planes (gib_split_planes).  m_dev / base_dev (may be NULL): the live row range
- * [*base_dev, *base_dev + *m_dev) inside buffers of M rows. */
+ * [*base_dev, *base_dev + *m_dev) inside buffers of M rows.  tf32: precision of the tensor-core kernels (0 = 3xTF32,
+ * 1 = single-pass TF32, as gib_set_matmul_tf32; W then read from W_hi only, or raw W rounded in the kernel); the
+ * problems of one call must agree. */
 typedef struct gib_gemm_problem {
   const float* A; int lda;
   const float* W; int ldw;
@@ -267,6 +278,7 @@ typedef struct gib_gemm_problem {
   const float* aux; int ldaux;
   int n_store, n_valid;
   const int* m_dev; const int* base_dev;
+  int tf32;
 } gib_gemm_problem;
 /* dep == NULL: the n problems as the model launches independent siblings (one problem: the single-GEMM dispatcher,
  * n <= 4: one grouped tensor-core launch when they qualify, else problem by problem).  dep != NULL: ONE dependent-chain
@@ -275,7 +287,8 @@ typedef struct gib_gemm_problem {
 size_t gib_test_chain_flag_bytes(const gib_gemm_problem* ps, int n);
 int gib_test_gemm_nt(const gib_gemm_problem* ps, int n, const int* dep, int* flags, gib_stream stream);
 /* one weight-gradient problem: dW[r*rs + c*cs] += sum_m G[m, prow(r)] X[m, c], dbias[r] += sum_m G[m, prow(r)]
- * (either may be NULL) for r < R, c < C, prow(r) = (r / Rb) * Rbp + r % Rb; G [M, Nn] (ldg), X [M, Kk] (ldx) */
+ * (either may be NULL) for r < R, c < C, prow(r) = (r / Rb) * Rbp + r % Rb; G [M, Nn] (ldg), X [M, Kk] (ldx); tf32 as in
+ * gib_gemm_problem (the bias sums stay fp32 sums of G); the members of one group must agree */
 typedef struct gib_dw_problem {
   const float* G; int ldg; int Nn;
   const float* X; int ldx; int Kk;
@@ -284,6 +297,7 @@ typedef struct gib_dw_problem {
   int R, C, Rb, Rbp;
   long long rs, cs;
   const int* m_dev; const int* base_dev;
+  int tf32;
 } gib_dw_problem;
 /* n_groups consecutive groups of group_sizes[g] (<= 16) problems, each run as the model runs the weight gradients of one
  * layer (one grouped tensor-core launch + one side-stream reduction when it qualifies), all on ONE scratch whose two
