@@ -54,6 +54,16 @@ class EvalPass(ctypes.Structure):
                 ("n_structures", c_f), ("flags", c_i), ("clipped", c_i), ("reserved", c_i)]
 
 
+class MolLayout(ctypes.Structure):
+    """mirror of `gib_mol_layout` (include/gib200.h): how `_features_to_atom` reads a node feature row"""
+    _fields_ = [(n, c_i) for n in ("n_atom_types", "n_formal_charge", "n_imp_H", "use_imp_H", "use_chirality",
+                                   "len_atom_types", "len_formal_charge", "len_imp_H", "len_chirality")]
+
+
+MOL_HDR_WORDS, MOL_WORDS, MOL_ATOM_WORDS = 8, 6, 3                  # GIB_MOL_* (include/gib200.h)
+MOL_DECODES, MOL_KEY_ERROR, MOL_DUPLICATE_BOND = 1, 2, 4
+MOL_ERR_VALUE, MOL_ERR_OVERFLOW, MOL_ERR_INDEX = 1, 2, 3
+
 MODEL_ID = {"GGNN": 0, "MNN": 1, "AttGGNN": 2, "EMN": 3}
 HDR_INTS = 16
 HDR_E, HDR_P, HDR_TYPE_COUNT, HDR_TYPE_BASE, HDR_FLAGS, HDR_CAPACITY = 0, 1, 2, 6, 11, 12
@@ -118,6 +128,11 @@ _PROTOS = {
     "gib_rl_scatter_grad": (c_i, [c_i] * 3 + [c_p] * 6),
     "gib_rl_dlogits": (c_i, [c_i, c_i] + [c_p] * 7),
     "gib_rl_next_round": (c_i, [c_p, c_p]),
+    "gib_molecule_table_bytes": (c_sz, [c_i] * 4),
+    "gib_molecule_table": (c_i, [c_i] * 4 + [c_p] * 6),
+    "gib_graph_statistics_bytes": (c_sz, [c_i] * 3),
+    "gib_graph_statistics_ws_bytes": (c_sz, [c_i] * 4),
+    "gib_graph_statistics": (c_i, [c_i] * 4 + [c_p] * 6),
     "gib_profile_enable": (None, [c_i]),
     "gib_launch_count": (c_ll, []),
     "gib_profile_collect": (c_i, [c_p, c_p, c_p]),

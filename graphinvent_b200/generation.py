@@ -40,6 +40,7 @@ class GraphGenerator:
     def __init__(self, model, batch_size, constants=None, n_atom_types=None, n_formal_charge=None, n_imp_H=None,
                  n_chirality=None, device="cuda"):
         C = constants if constants is not None else model.constants
+        self.constants = C
         self.model, self.batch_size, self.device = model, int(batch_size), torch.device(device)
         self.N, self.F, self.Ef = C.max_n_nodes, C.n_node_features, C.n_edge_features
         self.A = n_atom_types if n_atom_types is not None else getattr(C, "n_atom_types")
@@ -148,6 +149,18 @@ class GraphGenerator:
         flat = self.generated_likelihoods[self.generated_likelihoods != 0]        # :86-88
         graphs = (self.generated_nodes[:B], self.generated_edges[:B], self.generated_n_nodes[:B])
         return graphs, flat, final, self.properly_terminated[:B]
+
+    def sample_molecules(self, *args, constants=None, **kw):
+        """what the reference's `sample()` returns (GraphGenerator.py:48-96, GraphGeneratorRL.py:53-107): `sample(*args,
+        **kw)` of this generator with its tensors turned into the reference's `GenerationGraph` list by one
+        `molecules.MoleculeBatch`, which stays at `self.molecules` for `self.molecules.properties(...)` (the Analyzer's
+        statistics of the same batch).  `constants`: the reference constants the molecules are read with (atom_types,
+        formal_charge, int_to_bondtype, ...), by default those the generator was built with.  The likelihood tensors
+        are those of `sample()`, autograd history included."""
+        from .molecules import MoleculeBatch
+        (nodes, edges, n_nodes), likelihoods_a, likelihoods_b, terminated = self.sample(*args, **kw)
+        self.molecules = MoleculeBatch(nodes, edges, n_nodes, constants if constants is not None else self.constants)
+        return self.molecules.generation_graphs(), likelihoods_a, likelihoods_b, terminated
 
 
 class GraphGeneratorRL(GraphGenerator):

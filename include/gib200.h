@@ -470,6 +470,47 @@ int gib_rl_dlogits(int B, int apd, const float* logits, const int* act, const fl
 /* ctl[0] += 1 on the device (the round counter of a captured backward round) */
 int gib_rl_next_round(int* ctl, gib_stream stream);
 
+/* ---- generated molecules: the host table of graph_to_graph (GraphGenerator.py:659-804) and the histograms of
+ *      Analyzer.get_molecular_properties (Analyzer.py:311-599), from generated_nodes [B,N,F] f32, generated_edges
+ *      [B,N,N,Ef] f32 and generated_n_nodes [B] int8 (graphinvent_b200.molecules).  1 <= N <= 255, 1 <= F <= 32767,
+ *      1 <= Ef <= 16.
+ * Table (int32 words, gib_molecule_table_bytes from the dims; only the first GIB_MOL_HDR_WORDS + GIB_MOL_WORDS * B
+ * words plus the used records are written):
+ *   [0] atom records, [1] bonds, [2] first molecule whose statistics raise in the reference (-1: none; written by
+ *   gib_graph_statistics), [3] its GIB_MOL_ERR_*, [4] its atom, [5] OR of the molecules' key-error / duplicate flags.
+ *   Molecule m at GIB_MOL_HDR_WORDS + GIB_MOL_WORDS * m: n_nodes, atom records (min(max(n_nodes, 0), N)), bonds,
+ *   atom offset, bond offset, GIB_MOL_* flags.
+ *   Atom records from word GIB_MOL_HDR_WORDS + GIB_MOL_WORDS * B, GIB_MOL_ATOM_WORDS words = int16 [nnz, first,
+ *   second, third, last non-zero feature index, 0] (-1 where absent); non-zero as torch.nonzero (NaN counts).
+ *   Bonds right after the atom records, one word each = uint8 [i, j, type, 0], in the order of
+ *   torch.nonzero(edges * triu(ones(N, N), 1)) over the padded N x N x Ef (NaN / inf on or below the diagonal is listed).
+ * GIB_MOL_DECODES: every row _features_to_atom reads decodes (enough non-zeros, every list index inside [-len, len))
+ * and n_nodes <= N; GIB_MOL_KEY_ERROR: a bond to an atom >= n_nodes; GIB_MOL_DUPLICATE_BOND: an unordered pair listed
+ * twice, or a self bond (RDKit's AddBond raises). */
+#define GIB_MOL_HDR_WORDS 8
+#define GIB_MOL_WORDS 6
+#define GIB_MOL_ATOM_WORDS 3
+enum { GIB_MOL_DECODES = 1, GIB_MOL_KEY_ERROR = 2, GIB_MOL_DUPLICATE_BOND = 4 };
+enum { GIB_MOL_ERR_VALUE = 1, GIB_MOL_ERR_OVERFLOW = 2, GIB_MOL_ERR_INDEX = 3 };
+typedef struct gib_mol_layout {
+  int n_atom_types, n_formal_charge, n_imp_H;  /* constants.n_* (feature segment widths) */
+  int use_imp_H;                               /* not use_explicit_H and not ignore_H */
+  int use_chirality;
+  int len_atom_types, len_formal_charge, len_imp_H, len_chirality;  /* len() of the constants' lists */
+} gib_mol_layout;
+size_t gib_molecule_table_bytes(int B, int N, int F, int Ef);
+int gib_molecule_table(int B, int N, int F, int Ef, const gib_mol_layout* layout, const float* nodes,
+                       const float* edges, const signed char* n_nodes, int* table, gib_stream stream);
+/* Statistics of the molecules of a table built from the same tensors, with n_nodes = 0 for a molecule that does not
+ * decode.  out (f32): n_nodes_hist [N+1] | column sums of the nodes [F] | n_edges_hist [10] | edge_feature_hist [Ef] |
+ * sum_k k * n_nodes_hist[k] | sum_k (k+1) * n_edges_hist[k].  Sums run in molecule order, as the reference's loops do
+ * (exact for integer-valued features); a per-(atom, type) row sum beyond +-1e12 is clamped before it is summed.
+ * Writes words [2..4] of the table.  ws: gib_graph_statistics_ws_bytes, may hold anything. */
+size_t gib_graph_statistics_bytes(int N, int F, int Ef);
+size_t gib_graph_statistics_ws_bytes(int B, int N, int F, int Ef);
+int gib_graph_statistics(int B, int N, int F, int Ef, const float* nodes, const float* edges, int* table, float* out,
+                         void* ws, gib_stream stream);
+
 /* ---- measurement hooks: CUDA-event timing per kernel class on the launching stream.
  *      class 0 = forward/dX launches of the tensor-core kernel, 1 = its weight-gradient launches, 2 = scatter-aggregate (K2),
  *      3 / 4 = forward/dX and weight-gradient GEMMs on the fp32 SIMT kernels.  GIB_PROFILE_CLASSES entries per array.
