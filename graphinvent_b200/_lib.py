@@ -19,8 +19,8 @@ c_sz = ctypes.c_size_t
 
 class Dims(ctypes.Structure):
     """mirror of `gib_dims` (include/gib200.h).  `tf32` is host-side only: the matmul precision the model entry
-    points run in for these dims (0 = 3xTF32, 1 = single-pass TF32), applied per call through gib_set_matmul_tf32
-    (functional.matmul_precision); it is not part of the C struct."""
+    points run in for these dims (0 = 3xTF32, 1 = single-pass TF32, 2 = bf16, 3 = fp16 operands), applied per call
+    through gib_set_matmul_tf32 (functional.matmul_precision); it is not part of the C struct."""
     _fields_ = [(n, c_i) for n in (
         "model", "B", "N", "F", "Ef", "H", "M", "T", "msg_hidden", "msg_depth", "att_hidden", "att_depth",
         "eemb_hidden", "eemb_depth", "gather_width", "gatt_hidden", "gatt_depth", "gemb_hidden", "gemb_depth",
@@ -102,6 +102,7 @@ _PROTOS = {
     "gib_linear_fwd_tc": (c_i, [c_p, c_i, c_p, c_i, c_p, c_p, c_i, c_i, c_i, c_i, c_i, c_p]),
     "gib_linear_fwd_tc_planes": (c_i, [c_p, c_i, c_p, c_p, c_i, c_p, c_p, c_i, c_i, c_i, c_i, c_i, c_p, c_p, c_p]),
     "gib_split_planes": (c_i, [c_p, c_p, c_p, c_ll, c_p]),
+    "gib_round_plane16": (c_i, [c_p, c_p, c_ll, c_i, c_p]),
     "gib_dw_scratch_bytes": (c_sz, [c_i, c_i, c_i]),
     "gib_linear_bwd_dw": (c_i, [c_p, c_i, c_i, c_p, c_i, c_i, c_i, c_p, c_p, c_i, c_i, c_p, c_p, c_p, c_p]),
     "gib_scatter_sum": (c_i, [c_p, c_p, c_i, c_p, c_p, c_p, c_ll, c_p]),

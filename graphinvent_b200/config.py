@@ -37,6 +37,41 @@ def tf32_enabled():
     return p == "tf32"
 
 
+def autocast_dtype():
+    """`torch.bfloat16` / `torch.float16` when torch's CUDA autocast is on with one of these dtypes -- the reference's
+    `Linear`s and `GRUCell`s then run on 16-bit tensor cores, and so do this package's tensor-core GEMMs -- else None
+    (autocast off, or another autocast dtype)."""
+    import torch
+    if not torch.is_autocast_enabled("cuda"):
+        return None
+    dt = torch.get_autocast_dtype("cuda")
+    return dt if dt in (torch.bfloat16, torch.float16) else None
+
+
+# precision codes of the tensor-core GEMMs (gib_set_matmul_tf32, `Dims.tf32`)
+PREC_3XTF32, PREC_TF32, PREC_BF16, PREC_FP16 = 0, 1, 2, 3
+
+
+def matmul_code(fp16=True):
+    """The precision code the tensor-core GEMMs follow, by torch's own precedence: a 16-bit autocast dtype
+    (`autocast_dtype`: 2 = bf16, 3 = fp16), else the TF32 setting (`tf32_enabled`: 1), else 3xTF32 (0).  Under autocast
+    the TF32 setting does not matter, as for torch's autocast matmuls.  `fp16=False`: fp16 autocast is not honoured and
+    the rule continues with the TF32 setting (the captured training step, whose fused loss has no gradient scaling)."""
+    import torch
+    dt = autocast_dtype()
+    if dt is torch.bfloat16:
+        return PREC_BF16
+    if dt is torch.float16 and fp16:
+        return PREC_FP16
+    return PREC_TF32 if tf32_enabled() else PREC_3XTF32
+
+
+def dtype_of_code(code):
+    """the autocast dtype a precision code stands for (None for the fp32-input codes 0 / 1)"""
+    import torch
+    return {PREC_BF16: torch.bfloat16, PREC_FP16: torch.float16}.get(int(code))
+
+
 def make_constants(model="GGNN", **overrides):
     d = dict(DEFAULTS, model=model)
     d.update(overrides)

@@ -233,7 +233,8 @@ const char* gib_last_error(void) { return g_err; }
 int gib_version(void) { return 205; }
 void gib_set_tensor_cores(int on) { g_use_tc = on != 0; }
 int gib_get_tensor_cores(void) { return g_use_tc ? 1 : 0; }
-void gib_set_matmul_tf32(int on) { g_matmul_tf32 = on != 0; }
+// 0 3xTF32, 1 TF32 (any other nonzero value too), 2 bf16, 3 fp16
+void gib_set_matmul_tf32(int on) { g_matmul_tf32 = (on == 2 || on == 3) ? on : on != 0; }
 int gib_get_matmul_tf32(void) { return g_matmul_tf32; }
 void gib_tc_debug(int mode) { g_tc_debug = mode; }
 int gib_device_sm_count(void) { return device_sm_count(); }
@@ -304,7 +305,7 @@ size_t gib_model_packed_bytes(const gib_dims* d) {
 int gib_model_pack(const gib_dims* d, const float* const* params, void* packed, gib_stream stream) {
   Plan pl;
   GIB_TRY(build_plan(*d, pl));
-  return pack_params(pl, params, reinterpret_cast<float*>(packed), ST(stream));
+  return pack_params(pl, params, reinterpret_cast<float*>(packed), g_matmul_tf32, ST(stream));
 }
 
 size_t gib_model_workspace_bytes(const gib_dims* d, const int* hdr) {
@@ -316,6 +317,7 @@ int gib_model_forward(const gib_dims* d, const int* hdr, const void* nodes, cons
                       const void* packed, void* workspace, float* out, gib_stream stream) {
   Run r;
   GIB_TRY(make_run(*d, hdr, r));
+  GIB_TRY(check_precision(r.tf32, "gib_model_forward"));
   r.nodes = nodes; r.edges = edges;
   r.ga = graph_arrays(const_cast<void*>(graph_buf), r.S, r.E, r.P);
   r.packed = reinterpret_cast<const float*>(packed);
@@ -349,6 +351,7 @@ int gib_model_backward_part(const gib_dims* d, const int* hdr, const void* nodes
                             const float* dout, float* const* grads, void* scratch, int part, gib_stream stream) {
   Run r;
   GIB_TRY(make_run(*d, hdr, r));
+  GIB_TRY(check_precision(r.tf32, "gib_model_backward"));
   r.nodes = nodes; r.edges = edges;
   r.ga = graph_arrays(const_cast<void*>(graph_buf), r.S, r.E, r.P);
   r.packed = reinterpret_cast<const float*>(packed);
@@ -485,6 +488,21 @@ int gib_split_planes(const float* W, float* W_hi, float* W_lo, long long n, gib_
   GIB_LAUNCH_CHECK();
   return 0;
 }
+__global__ void round_plane16_kernel(const float* __restrict__ W, uint16_t* __restrict__ out, long long n, int kind) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  uint16_t u;
+  if (kind == 2) asm("cvt.rn.bf16.f32 %0, %1;" : "=h"(u) : "f"(W[i]));
+  else asm("cvt.rn.f16.f32 %0, %1;" : "=h"(u) : "f"(W[i]));
+  out[i] = u;
+}
+int gib_round_plane16(const float* W, void* out, long long n, int kind, gib_stream stream) {
+  if (kind != 2 && kind != 3) { set_error("gib_round_plane16: kind %d (2 = bf16, 3 = fp16)", kind); return -2; }
+  if (n <= 0) return 0;
+  round_plane16_kernel<<<(unsigned)ceil_div_ll(n, 256), 256, 0, ST(stream)>>>(W, reinterpret_cast<uint16_t*>(out), n, kind);
+  GIB_LAUNCH_CHECK();
+  return 0;
+}
 size_t gib_dw_scratch_bytes(int M, int Nn, int Kk) { return gemm_dw_scratch_floats(M, Nn, Kk) * sizeof(float); }
 int gib_linear_bwd_dw(const float* G, int ldg, int Nn, const float* X, int ldx, int Kk, int M, float* dW, float* dbias,
                       int R, int C, void* scratch, const int* m_dev, const int* base_dev, gib_stream stream) {
@@ -525,6 +543,7 @@ static GemmNT to_gemm_nt(const gib_gemm_problem& s) {
   p.C = s.C; p.ldc = s.ldc; p.M = s.M; p.N = s.N; p.K = s.K; p.bias = s.bias; p.act = s.act; p.mode = s.mode;
   p.aux = s.aux; p.ldaux = s.ldaux; p.n_store = s.n_store; p.n_valid = s.n_valid;
   p.m_dev = s.m_dev; p.base_dev = s.base_dev; p.tf32 = s.tf32;
+  if (s.tf32 >= 2) p.B_lo = nullptr;        // W_hi: the 16-bit plane; W_lo is not read
   return p;
 }
 static GemmDW to_gemm_dw(const gib_dw_problem& s) {
@@ -561,7 +580,13 @@ size_t gib_test_chain_flag_bytes(const gib_gemm_problem* ps, int n) {
 int gib_test_gemm_nt(const gib_gemm_problem* ps, int n, const int* dep, int* flags, gib_stream stream) {
   if (n < 1 || n > kTc3MaxProblems) { set_error("gib_test_gemm_nt: %d problems (1..%d)", n, kTc3MaxProblems); return -2; }
   GemmNT p[kTc3MaxProblems];
-  for (int i = 0; i < n; ++i) p[i] = to_gemm_nt(ps[i]);
+  for (int i = 0; i < n; ++i) {
+    if (ps[i].tf32 >= 2 && !ps[i].W_hi) {
+      set_error("gib_test_gemm_nt: problem %d is bf16 / fp16 but has no 16-bit plane (W_hi, gib_round_plane16)", i);
+      return -2;
+    }
+    p[i] = to_gemm_nt(ps[i]);
+  }
   if (!dep) return n == 1 ? gemm_nt(p[0], ST(stream)) : gemm_nt_group(p, n, ST(stream));
   if (!gemm_nt_chain_ok(p, n)) { set_error("gib_test_gemm_nt: the problems do not qualify for a chain"); return -3; }
   return gemm_nt_chain(p, dep, n, flags, ST(stream));

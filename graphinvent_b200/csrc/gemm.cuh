@@ -33,8 +33,9 @@ struct GemmNT {
   // group sizes K0 leaves in device memory, so no launch parameter depends on the batch content.
   const int* m_dev = nullptr;
   const int* base_dev = nullptr;
-  // Precision of the tensor-core kernels: 0 = 3xTF32 (fp32-accurate), 1 = single-pass TF32 (the hi*hi term only).
-  // The fp32 SIMT kernel ignores it.
+  // Precision of the tensor-core kernels: 0 = 3xTF32 (fp32-accurate), 1 = single-pass TF32 (the hi*hi term only),
+  // 2 = bf16, 3 = fp16 operands (fp32 accumulation; B_hi then points at the 16-bit plane of B, ldb in elements, and
+  // B_lo is not read).  The fp32 SIMT kernel ignores it.
   int tf32 = 0;
 };
 
@@ -102,6 +103,9 @@ extern bool g_use_tc;
 extern int g_tc_debug;
 // precision of the model entry points' tensor-core GEMMs on this host thread (gib_set_matmul_tf32; GemmNT::tf32)
 extern thread_local int g_matmul_tf32;
+// 0 when a GEMM of precision `prec` can run as asked (a known code; 16-bit codes need the tensor-core path), else the
+// error code with the message set
+int check_precision(int prec, const char* who);
 
 int gemm_dw(const GemmDW& q, cudaStream_t st);
 // n <= 16 weight-gradient problems that may run as ONE grouped tensor-core launch + ONE reduction launch (siblings of a

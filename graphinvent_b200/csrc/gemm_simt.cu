@@ -170,7 +170,19 @@ __global__ void __launch_bounds__(256, 2) sgemm_nt_kernel(const GemmNT p) {
 // gib_tc_debug bit 0: the per-problem call pattern (no grouped / chained launches, W split in the kernel)
 static inline bool use_tc3() { return (g_tc_debug & 1) == 0; }
 
+// bf16 / fp16 operands (precision 2 / 3) exist on the wgmma kernels only: with tensor cores off or debug bit 0 a
+// 16-bit call is refused rather than run in another precision
+int check_precision(int prec, const char* who) {
+  if (prec < 0 || prec > 3) { set_error("%s: unknown matmul precision %d", who, prec); return -2; }
+  if (prec >= 2 && (!g_use_tc || !use_tc3())) {
+    set_error("%s: bf16 / fp16 GEMMs need the tensor-core path (tensor cores on, gib_tc_debug bit 0 clear)", who);
+    return -2;
+  }
+  return 0;
+}
+
 int gemm_nt(const GemmNT& p, cudaStream_t st) {
+  GIB_TRY(check_precision(p.tf32, "gemm_nt"));
   // tensor-core path for all but the tiny / skinny GEMMs (those stay on the SIMT kernel); a problem whose row count
   // lives on the device (capacity mode) needs the grouped call pattern
   if (p.m_dev) {
@@ -197,6 +209,7 @@ int gemm_nt(const GemmNT& p, cudaStream_t st) {
 // together they fill the machine reasonably, else problem by problem.
 int gemm_nt_group(const GemmNT* ps, int n, cudaStream_t st) {
   if (n == 1) return gemm_nt(ps[0], st);
+  for (int i = 0; i < n; ++i) GIB_TRY(check_precision(ps[i].tf32, "gemm_nt_group"));
   bool ok = g_use_tc && n <= 4, ok3 = ok && use_tc3(), dyn = false;
   long long tiles = 0;
   for (int i = 0; i < n && ok; ++i) {
@@ -576,6 +589,7 @@ void gemm_dw_plan(int M, int Nn, int Kk, int* splits, int* chunk) {
 int gemm_dw_group(const GemmDW* qs, int n, long long plan_rows, cudaStream_t st) {
   if (n < 1) return 0;
   if (n > kTc3MaxProblems) { set_error("gemm_dw_group: %d problems (max %d)", n, kTc3MaxProblems); return -2; }
+  for (int i = 0; i < n; ++i) GIB_TRY(check_precision(qs[i].tf32, "gemm_dw_group"));
   const bool tc3 = g_use_tc && use_tc3();
   bool dyn = false;
   long long rows = 0;
@@ -642,6 +656,7 @@ int gemm_dw_group(const GemmDW* qs, int n, long long plan_rows, cudaStream_t st)
 
 int gemm_dw(const GemmDW& q, cudaStream_t st) {
   if (q.M <= 0) return 0;  // nothing to add
+  GIB_TRY(check_precision(q.tf32, "gemm_dw"));
   if ((q.ldg & 3) || (q.ldx & 3) || (q.Nn & 3) || (q.Kk & 3)) {
     set_error("gemm_dw: ldg=%d ldx=%d Nn=%d Kk=%d violate the padded-layout contract", q.ldg, q.ldx, q.Nn, q.Kk);
     return -2;

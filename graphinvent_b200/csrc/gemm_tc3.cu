@@ -16,6 +16,15 @@
 // accumulator, no lo loads and no cross-term MMAs.  Schedules, stage rings, epilogues, chains and the split-K
 // reduction are those of the 3xTF32 kernels.
 //
+// 16-bit operands (template parameter H16 = 1 bf16 / 2 fp16 of the two wgmma kernels; GemmNT::tf32 / GemmDW::tf32 =
+// 2 / 3, set when the caller runs under torch.autocast): every operand rounded to nearest-even to 16 bits, as
+// tensor.to(dtype) rounds, fp32 accumulation.  W is one K-major 16-bit plane (gib_model_pack writes it over the bytes
+// of the lo plane; the problem's W_hi points at it), read by TMA as [128 x 32] boxes of 64-byte rows with the 64-byte
+// swizzle, so the k-block stays 32 and the stage rings, schedules, epilogues, chains and the split-K reduction are
+// shared.  The A / G fragments are rounded in registers from the fp32 tiles (cvt.rn.{bf16,f16}x2.f32), the X
+// transpose writes a 16-bit K-major plane; per k-block one group of 2 wgmma.m64n128k16 (A from registers).  No run-time
+// branch in the inner loop; the raw-W mma.sync kernel has no 16-bit instantiation.
+//
 // The kernels are persistent (one CTA per SM, work items = output tiles of up to 16 problems, or (tile, reduction
 // chunk) pairs in TN mode) and fed by one TMA lane through a ring of shared-memory stages (cp.async.bulk.tensor with
 // the 128-byte swizzle, mbarrier expect_tx per stage).
@@ -95,6 +104,7 @@ constexpr int SMEM_BYTES = OFF_SCHED + 512 + 1024 /*align slack*/;
 constexpr int WG_BN = 128;
 constexpr int WG_STAGES = 4;
 constexpr int WG_B_BYTES = WG_BN * BKF * 4;       // 16 KB
+constexpr int WG_B16_BYTES = WG_BN * BKF * 2;     // 8 KB: the 16-bit W tile (at the W hi offset of a stage)
 constexpr int WG_STAGE_BYTES = A_BYTES + 2 * WG_B_BYTES;   // 48 KB: A raw | W hi | W lo
 constexpr int WG_THREADS = 32 * CONS_WARPS + 128;   // 384
 constexpr int WG_OFF_BARS = WG_STAGES * WG_STAGE_BYTES;
@@ -202,6 +212,12 @@ __device__ __forceinline__ float lds32(uint32_t saddr) {
 // 16-byte chunk j of row r sits at chunk j ^ (r & 7) (tile bases are 1024-byte aligned)
 __device__ __forceinline__ uint32_t swz(int r, int c) {
   return (uint32_t)r * 128u + ((((uint32_t)c >> 2) ^ (uint32_t)r) & 7u) * 16u + ((uint32_t)c & 3u) * 4u;
+}
+
+// byte offset of 16-bit element (row r, value c < 32) in a tile of 64-byte rows written with CU_TENSOR_MAP_SWIZZLE_64B:
+// 16-byte chunk j of row r sits at chunk j ^ ((r >> 1) & 3) (tile bases are 512-byte aligned)
+__device__ __forceinline__ uint32_t swz64(int r, int c) {
+  return (uint32_t)r * 64u + ((((uint32_t)c >> 3) ^ ((uint32_t)r >> 1)) & 3u) * 16u + ((uint32_t)c & 7u) * 2u;
 }
 
 __device__ __forceinline__ void fence_proxy_async_all() { asm volatile("fence.proxy.async;" ::: "memory"); }
@@ -519,6 +535,34 @@ __device__ __forceinline__ float4 lds128(uint32_t saddr) {
 // byte offset of output element (row r, column c < 128) in the tile buffer: box c / 32, swizzled as TMA writes it
 __device__ __forceinline__ uint32_t epi_off(int r, int c) { return (uint32_t)(c >> 5) * (BM * BKF * 4) + swz(r, c & 31); }
 
+// 16-bit A fragments of one k-block (two k16 steps) for rows r0, r0 + 8 (r0 & 7 = g) from the fp32 activation tile at
+// sa: f[s] = the m16n8k16 fragment of k16 step s.  A lane reads its four column pairs (step s, half h: columns
+// 16 s + 8 h + 2t, +1) of a row as 8-byte loads, in a lane-dependent order -- load i takes (s, h) = (i1 ^ g1, i0 ^ g0)
+// -- so that the 16 lanes of each half-warp phase (g < 4 or g >= 4, t < 4) hit 16 distinct 8-byte slots: with the
+// 128-byte swizzle the chunk index is (4 s + 2 h + t1) ^ g, whose bits are (i1 ^ g1 ^ g2, i0 ^ g0 ^ g1, t1 ^ g0), a
+// bijection of (g1, g0, t1); in natural order lanes g and g ^ 1 would share chunks (2-way conflicts).  Two selects per
+// register then undo the permutation.
+template <int H16>
+__device__ __forceinline__ void a_frags16(uint32_t sa, int r0, int g, int t4, uint32_t (&f)[2][4]) {
+  const bool g0 = g & 1, g1 = (g >> 1) & 1;
+#pragma unroll
+  for (int h8 = 0; h8 < 2; ++h8) {
+    uint32_t q[4];
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      const int s = (i >> 1) ^ (int)g1, hh = (i & 1) ^ (int)g0;
+      float x, y;
+      lds64(sa + swz(r0 + 8 * h8, 16 * s + 8 * hh + 2 * t4), x, y);
+      q[i] = pack16<H16>(x, y);
+    }
+    const uint32_t p0 = g0 ? q[1] : q[0], p1 = g0 ? q[0] : q[1], p2 = g0 ? q[3] : q[2], p3 = g0 ? q[2] : q[3];
+    f[0][h8] = g1 ? p2 : p0;          // (s 0, h 0)
+    f[0][2 + h8] = g1 ? p3 : p1;      // (s 0, h 1)
+    f[1][h8] = g1 ? p0 : p2;          // (s 1, h 0)
+    f[1][2 + h8] = g1 ? p1 : p3;      // (s 1, h 1)
+  }
+}
+
 // ---- wgmma kernel: NT with pre-split W ----
 //
 // With a specialised epilogue (SE) the consumers only touch registers and shared memory between a tile's last wgmma
@@ -531,9 +575,12 @@ __device__ __forceinline__ uint32_t epi_off(int r, int c) { return (uint32_t)(c 
 //   warps 10-11       tile buffer -> C with 16-byte stores (rows < the live row count, columns < n_store) -> epi_empty,
 //                     then the chain hand-off of the tile.  They wait on nothing but epi_done, so a chain cannot
 //                     dead-lock on them.
-template <int EPI, bool TF1>
+// H16 (bf16 / fp16 operands, instantiated with TF1 = true: one accumulator): W is the 16-bit plane, one 8 KB box per
+// k-block at the W hi offset of the stage, and the consumers issue one group of 2 k16 wgmma per k-block.
+template <int EPI, bool TF1, int H16 = 0>
 __global__ void __launch_bounds__(WG_THREADS, 1)
 tc3_wgmma_kernel(const __grid_constant__ Maps maps, const Params P) {
+  static_assert(H16 == 0 || TF1, "16-bit operands use the single accumulator");
   constexpr bool SE = EPI != EPI_SPEC_GENERIC;
   constexpr bool AUX = EPI == EPI_SPEC_DSELU || EPI == EPI_SPEC_ADD;
   constexpr int NST = SE ? WG_EPI_STAGES : WG_STAGES;
@@ -578,7 +625,7 @@ tc3_wgmma_kernel(const __grid_constant__ Maps maps, const Params P) {
         for (int kb = 0; kb < w.nkb; ++kb) {
           mbar_wait(&empty[stage], phase ^ 1);
           uint8_t* st = smem + stage * WG_STAGE_BYTES;
-          mbar_arrive_expect_tx(&full[stage], TF1 ? A_BYTES + WG_B_BYTES : WG_STAGE_BYTES);
+          mbar_arrive_expect_tx(&full[stage], H16 ? A_BYTES + WG_B16_BYTES : TF1 ? A_BYTES + WG_B_BYTES : WG_STAGE_BYTES);
           tma_load_2d(&maps.a[w.p], &full[stage], st, kb * BKF, base + w.m0);
           tma_load_2d(&maps.b[w.p], &full[stage], st + A_BYTES, kb * BKF, w.n0);
           if (!TF1) tma_load_2d(&maps.b_lo[w.p], &full[stage], st + A_BYTES + WG_B_BYTES, kb * BKF, w.n0);
@@ -685,15 +732,31 @@ tc3_wgmma_kernel(const __grid_constant__ Maps maps, const Params P) {
         wgmma_commit();
         wgmma_wait<1>();
       };
+      // H16: a whole k-block's fragments per buffer and group (even k-blocks in f0, odd in f1), the same wait_group 1
+      // discipline: the group of k-block kb - 1 has retired once that of kb is committed, and its stage goes back
+      uint32_t f0[2][4], f1[2][4];
+      auto kblock16 = [&](uint32_t sa, uint32_t (&f)[2][4]) {
+        a_frags16<H16 ? H16 : 1>(sa, r0, g8, t4, f);
+        wgmma_fence();
+#pragma unroll
+        for (int s = 0; s < 2; ++s) wgmma_m64n128k16_h16<H16 ? H16 : 1>(acc, f[s], wgmma_desc_sw64(sa + A_BYTES + s * 32));
+        wgmma_commit();
+        wgmma_wait<1>();
+      };
       for (int kb = 0; kb < w.nkb; ++kb) {
         mbar_wait(&full[stage], phase);
         const uint32_t sa = smem_u32(smem + stage * WG_STAGE_BYTES);
-        half(sa, 0, ah0, al0);
+        if constexpr (H16) {
+          if (kb & 1) kblock16(sa, f1);
+          else kblock16(sa, f0);
+        } else {
+          half(sa, 0, ah0, al0);
+        }
         if (prev >= 0) {
           __syncwarp();
           if (lane == 0) mbar_arrive(&empty[prev]);
         }
-        half(sa, 1, ah1, al1);
+        if constexpr (!H16) half(sa, 1, ah1, al1);
         prev = stage;
         if (++stage == NST) { stage = 0; phase ^= 1; }
       }
@@ -787,10 +850,37 @@ __device__ __forceinline__ void dw_transpose_block(uint32_t sx, uint32_t sp, int
   }
 }
 
+// The same 4 x 4 block into the 16-bit K-major X^T plane (64-byte rows, 64-byte swizzle, swz64): the four reduction
+// rows of plane row n = 4b + j are one 8-byte store.  The raw reads are those above; the stores of a group of 8 lanes
+// take 8 distinct 8-byte slots of one 64-byte bank range (the chunk (a >> 1) ^ (n >> 1) and the half a & 1 take 8
+// values over l), and the two groups of a half-warp phase share it: 2-way, on half the bytes the TF32 planes store.
+template <int H16>
+__device__ __forceinline__ void dw_transpose_block16(uint32_t sx, uint32_t sp, int t, int valid) {
+  const int l = t & 7, u = t >> 6;
+  const int b = ((t >> 3) & 3) * 8 + l;
+  const int a = ((t >> 5) & 1) * 4 + ((((l >> 2) ^ (u >> 1)) & 1) << 1) + (((l >> 1) ^ u) & 1);
+  float4 v[4];
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    const int k = 4 * a + i;
+    v[i] = lds128(sx + (b >> 3) * 4096 + swz(k, 4 * (b & 7)));
+    if (k >= valid) v[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+  }
+  auto c = [](const float4& x, int j) { return j == 0 ? x.x : j == 1 ? x.y : j == 2 ? x.z : x.w; };
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    const uint32_t lo = pack16<H16>(c(v[0], j), c(v[1], j)), hi = pack16<H16>(c(v[2], j), c(v[3], j));
+    asm volatile("st.shared.v2.b32 [%0], {%1, %2};" ::"r"(sp + swz64(4 * b + j, 4 * a)), "r"(lo), "r"(hi) : "memory");
+  }
+}
+
 // ---- wgmma kernel: TN (weight-gradient partials) ----
-template <bool TF1>
+// H16 (instantiated with TF1 = true): G fragments rounded in registers, X transposed into one 16-bit plane, one group
+// of 2 k16 wgmma per k-block.
+template <bool TF1, int H16 = 0>
 __global__ void __launch_bounds__(WG_THREADS, 1)
 tc3_wgmma_dw_kernel(const __grid_constant__ Maps maps, const Params P) {
+  static_assert(H16 == 0 || TF1, "16-bit operands use the single accumulator");
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + DW_OFF_BARS);
@@ -853,7 +943,10 @@ tc3_wgmma_dw_kernel(const __grid_constant__ Maps maps, const Params P) {
           mbar_wait(&raw_full[rs], rph);
           const uint32_t sx = smem_u32(smem + rs * DW_RAW_BYTES + A_BYTES);
           const uint32_t sp = smem_u32(smem + DW_OFF_PLANES + ps * DW_PLANE_BYTES);
-          for (int t = tt; t < 256; t += 32 * DW_TR_WARPS) dw_transpose_block<TF1>(sx, sp, t, w.rows - kb * BKF);
+          for (int t = tt; t < 256; t += 32 * DW_TR_WARPS) {
+            if constexpr (H16) dw_transpose_block16<H16>(sx, sp, t, w.rows - kb * BKF);
+            else dw_transpose_block<TF1>(sx, sp, t, w.rows - kb * BKF);
+          }
           asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy stores -> wgmma reads
           __syncwarp();
           if (lane == 0) {
@@ -919,18 +1012,48 @@ tc3_wgmma_dw_kernel(const __grid_constant__ Maps maps, const Params P) {
         wgmma_commit();
         wgmma_wait<1>();
       };
+      // H16: a whole k-block per buffer and group (even k-blocks in f0, odd in f1).  Fragment register 2h + e of k16
+      // step s holds G column r0 + 8e at reduction rows k = 16 s + 8 h + 2t, +1; these 4-byte reads are free of bank
+      // conflicts (chunk (c >> 2) ^ (k & 7) with k & 7 = 2t + const: 8 distinct chunks over (g >> 2, t)).
+      uint32_t f0[2][4], f1[2][4];
+      auto kblock16 = [&](uint32_t sg, uint32_t sp, int valid, uint32_t (&f)[2][4]) {
+#pragma unroll
+        for (int s = 0; s < 2; ++s)
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int k = 16 * s + 8 * h + 2 * t4;
+            float a[4];
+            a[0] = lds32(sg + go0 + swz(k, c0)); a[1] = lds32(sg + go0 + swz(k + 1, c0));
+            a[2] = lds32(sg + go1 + swz(k, c1)); a[3] = lds32(sg + go1 + swz(k + 1, c1));
+            if (k >= valid) { a[0] = 0.f; a[2] = 0.f; }     // rows past the chunk / row count may hold anything
+            if (k + 1 >= valid) { a[1] = 0.f; a[3] = 0.f; }
+            if (want_cs) { cs0 += a[0] + a[1]; cs1 += a[2] + a[3]; }
+            f[s][2 * h] = pack16<H16 ? H16 : 1>(a[0], a[1]);
+            f[s][2 * h + 1] = pack16<H16 ? H16 : 1>(a[2], a[3]);
+          }
+        wgmma_fence();
+#pragma unroll
+        for (int s = 0; s < 2; ++s) wgmma_m64n128k16_h16<H16 ? H16 : 1>(acc, f[s], wgmma_desc_sw64(sp + s * 32));
+        wgmma_commit();
+        wgmma_wait<1>();
+      };
       for (int kb = 0; kb < w.nkb; ++kb) {
         mbar_wait(&raw_full[rs], rph);
         mbar_wait(&pl_full[ps], pph);
         const uint32_t sg = smem_u32(smem + rs * DW_RAW_BYTES);
         const uint32_t sp = smem_u32(smem + DW_OFF_PLANES + ps * DW_PLANE_BYTES);
         const int valid = w.rows - kb * BKF;
-        half(sg, sp, valid, 0, ah0, al0);
+        if constexpr (H16) {
+          if (kb & 1) kblock16(sg, sp, valid, f1);
+          else kblock16(sg, sp, valid, f0);
+        } else {
+          half(sg, sp, valid, 0, ah0, al0);
+        }
         if (prev >= 0) {
           __syncwarp();
           if (lane == 0) mbar_arrive(&pl_empty[prev]);
         }
-        half(sg, sp, valid, 1, ah1, al1);
+        if constexpr (!H16) half(sg, sp, valid, 1, ah1, al1);
         __syncwarp();
         if (lane == 0) mbar_arrive(&raw_empty[rs]);
         prev = ps;
@@ -1056,11 +1179,12 @@ static EncodeTiledFn encode_fn() {
 
 // Encoded descriptors are pure functions of (base, rows, cols, ld, box): the training step presents the same few
 // hundred operands every iteration, so they are memoised (an encode costs ~1 us of host time, 3-12 per launch).
-// Every tile is a [box_rows x 32 fp32] box with the 128-byte swizzle the consumers decode (swz()).
+// Every tile is a [box_rows x 32 fp32] box with the 128-byte swizzle the consumers decode (swz()), or (kind 1 / 2: a
+// bf16 / fp16 plane, ld in 16-bit elements) a [box_rows x 32] box of 16-bit values with the 64-byte swizzle (swz64()).
 struct MapKey {
-  const void* base; int rows, cols, ld, box_rows;
+  const void* base; int rows, cols, ld, box_rows, kind;
   bool operator==(const MapKey& o) const {
-    return base == o.base && rows == o.rows && cols == o.cols && ld == o.ld && box_rows == o.box_rows;
+    return base == o.base && rows == o.rows && cols == o.cols && ld == o.ld && box_rows == o.box_rows && kind == o.kind;
   }
 };
 struct MapKeyHash {
@@ -1070,14 +1194,15 @@ struct MapKeyHash {
     h = h * 1000003u ^ (size_t)k.cols;
     h = h * 1000003u ^ (size_t)k.ld;
     h = h * 1000003u ^ (size_t)k.box_rows;
+    h = h * 1000003u ^ (size_t)k.kind;
     return h;
   }
 };
 static std::mutex g_map_mu;
 static std::unordered_map<MapKey, CUtensorMap, MapKeyHash> g_map_cache;
 
-static int make_map(CUtensorMap* map, const float* base, int rows, int cols, int ld, int box_rows) {
-  const MapKey key{base, rows, cols, ld, box_rows};
+static int make_map(CUtensorMap* map, const float* base, int rows, int cols, int ld, int box_rows, int kind = 0) {
+  const MapKey key{base, rows, cols, ld, box_rows, kind};
   {
     std::lock_guard<std::mutex> lk(g_map_mu);
     auto it = g_map_cache.find(key);
@@ -1086,14 +1211,18 @@ static int make_map(CUtensorMap* map, const float* base, int rows, int cols, int
   EncodeTiledFn fn = encode_fn();
   if (!fn) { set_error("cuTensorMapEncodeTiled entry point unavailable"); return -4; }
   cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
-  cuuint64_t strides[1] = {(cuuint64_t)ld * 4};
+  cuuint64_t strides[1] = {(cuuint64_t)ld * (kind ? 2 : 4)};
   cuuint32_t box[2] = {(cuuint32_t)BKF, (cuuint32_t)box_rows};
   cuuint32_t estr[2] = {1, 1};
-  CUresult r = fn(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(base), dims, strides, box, estr,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+  const CUtensorMapDataType dt = kind == 1   ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16
+                                 : kind == 2 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16
+                                             : CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
+  CUresult r = fn(map, dt, 2, const_cast<float*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                  kind ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
-    set_error("cuTensorMapEncodeTiled failed (%d) rows=%d cols=%d ld=%d box_rows=%d", (int)r, rows, cols, ld, box_rows);
+    set_error("cuTensorMapEncodeTiled failed (%d) rows=%d cols=%d ld=%d box_rows=%d kind=%d", (int)r, rows, cols, ld,
+              box_rows, kind);
     return -4;
   }
   std::lock_guard<std::mutex> lk(g_map_mu);
@@ -1125,6 +1254,17 @@ static int set_attributes() {
   GIB_CUDA_TRY(cudaFuncSetAttribute(tc3_wgmma_dw_kernel<TF1>, cudaFuncAttributeMaxDynamicSharedMemorySize, DW_SMEM_BYTES));
   return 0;
 }
+// and of one 16-bit type's (wgmma kernels only)
+template <int H16>
+static int set_attributes16() {
+  GIB_CUDA_TRY(cudaFuncSetAttribute(tc3_wgmma_kernel<EPI_SPEC_GENERIC, true, H16>, cudaFuncAttributeMaxDynamicSharedMemorySize, WG_SMEM_BYTES));
+  GIB_CUDA_TRY(cudaFuncSetAttribute(tc3_wgmma_kernel<EPI_SPEC_SELU, true, H16>, cudaFuncAttributeMaxDynamicSharedMemorySize, WG_EPI_SMEM_BYTES));
+  GIB_CUDA_TRY(cudaFuncSetAttribute(tc3_wgmma_kernel<EPI_SPEC_LINEAR, true, H16>, cudaFuncAttributeMaxDynamicSharedMemorySize, WG_EPI_SMEM_BYTES));
+  GIB_CUDA_TRY(cudaFuncSetAttribute(tc3_wgmma_kernel<EPI_SPEC_DSELU, true, H16>, cudaFuncAttributeMaxDynamicSharedMemorySize, WG_EPI_SMEM_BYTES));
+  GIB_CUDA_TRY(cudaFuncSetAttribute(tc3_wgmma_kernel<EPI_SPEC_ADD, true, H16>, cudaFuncAttributeMaxDynamicSharedMemorySize, WG_EPI_SMEM_BYTES));
+  GIB_CUDA_TRY(cudaFuncSetAttribute(tc3_wgmma_dw_kernel<true, H16>, cudaFuncAttributeMaxDynamicSharedMemorySize, DW_SMEM_BYTES));
+  return 0;
+}
 
 static int prepare(int* num_sms_out) {
   int dev = 0;
@@ -1136,6 +1276,8 @@ static int prepare(int* num_sms_out) {
     GIB_CUDA_TRY(cudaDeviceGetAttribute(&d.num_sms, cudaDevAttrMultiProcessorCount, dev));
     GIB_TRY(set_attributes<false>());
     GIB_TRY(set_attributes<true>());
+    GIB_TRY(set_attributes16<1>());
+    GIB_TRY(set_attributes16<2>());
     d.attr_done = true;
   }
   *num_sms_out = d.num_sms;
@@ -1157,7 +1299,10 @@ static int epi_spec(const GemmNT& p) {
   return EPI_SPEC_ADD;
 }
 
+// W given as the planes of the problem's precision: aligned (hi, lo) TF32 planes, or (16-bit modes) one aligned
+// 16-bit plane at B_hi whose rows are whole 16-byte units (the TMA stride rule)
 static bool presplit(const GemmNT& p) {
+  if (p.tf32 >= 2) return p.B_hi && (reinterpret_cast<uintptr_t>(p.B_hi) & 15) == 0 && (p.ldb % 8) == 0;
   return p.B_hi && p.B_lo && (reinterpret_cast<uintptr_t>(p.B_hi) & 15) == 0 && (reinterpret_cast<uintptr_t>(p.B_lo) & 15) == 0;
 }
 
@@ -1184,8 +1329,8 @@ bool tc_eligible(const GemmNT& p) {
 // the model's call pattern: W as pre-split planes
 bool tc3_eligible(const GemmNT& p) {
   auto al = [](const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15) == 0; };
-  return p.M >= 1 && p.N >= 1 && p.K >= 16 && (p.K % 16) == 0 && (p.lda % 4) == 0 && (p.ldb % 4) == 0 && p.B_hi &&
-         p.B_lo && al(p.A) && al(p.B_hi) && al(p.B_lo);
+  return p.M >= 1 && p.N >= 1 && p.K >= 16 && (p.K % 16) == 0 && (p.lda % 4) == 0 && (p.ldb % 4) == 0 && al(p.A) &&
+         tc3::presplit(p);
 }
 
 template <bool TF1>
@@ -1210,6 +1355,17 @@ static void launch_nt_kernel(const tc3::Maps& maps, const tc3::Params& P, bool r
     }
   }
 }
+template <int H16>
+static void launch_nt_kernel16(const tc3::Maps& maps, const tc3::Params& P, int spec, int grid, cudaStream_t st) {
+  using namespace tc3;
+  switch (spec) {
+    case EPI_SPEC_SELU: tc3_wgmma_kernel<EPI_SPEC_SELU, true, H16><<<grid, WG_THREADS, WG_EPI_SMEM_BYTES, st>>>(maps, P); break;
+    case EPI_SPEC_LINEAR: tc3_wgmma_kernel<EPI_SPEC_LINEAR, true, H16><<<grid, WG_THREADS, WG_EPI_SMEM_BYTES, st>>>(maps, P); break;
+    case EPI_SPEC_DSELU: tc3_wgmma_kernel<EPI_SPEC_DSELU, true, H16><<<grid, WG_THREADS, WG_EPI_SMEM_BYTES, st>>>(maps, P); break;
+    case EPI_SPEC_ADD: tc3_wgmma_kernel<EPI_SPEC_ADD, true, H16><<<grid, WG_THREADS, WG_EPI_SMEM_BYTES, st>>>(maps, P); break;
+    default: tc3_wgmma_kernel<EPI_SPEC_GENERIC, true, H16><<<grid, WG_THREADS, WG_SMEM_BYTES, st>>>(maps, P); break;
+  }
+}
 
 // up to MAXP NT problems in one persistent launch; dep == nullptr: independent.  raw: every W is raw fp32 (split in
 // the kernel; mma.sync kernel), else every W comes as aligned (hi, lo) planes (wgmma kernel).  Every problem of a
@@ -1231,11 +1387,18 @@ static int launch_nt(const GemmNT* ps, const int* dep, int n, int* flags, bool r
   int spec = -1;
   int slot[MAXP];                 // input index -> launch slot (-1: skipped, no rows)
   int flag_ints = 0;
-  const bool tf32 = ps[0].tf32 != 0;
+  const int prec = ps[0].tf32;
+  const bool tf32 = prec != 0;
+  const int h16 = prec >= 2 ? prec - 1 : 0;      // 16-bit operand kind: 1 bf16, 2 fp16
+  if (prec < 0 || prec > 3) { set_error("gemm_nt_tc3: unknown precision %d", prec); return -2; }
+  if (h16 && raw) {
+    set_error("gemm_nt_tc3: 16-bit operands need W as a 16-bit plane (W_hi); raw fp32 W runs in the TF32 modes only");
+    return -2;
+  }
   for (int i = 0; i < n; ++i) {
     const GemmNT& p = ps[i];
     slot[i] = -1;
-    if ((p.tf32 != 0) != tf32) { set_error("gemm_nt_tc3: problems of one launch with different precisions"); return -2; }
+    if (p.tf32 != prec) { set_error("gemm_nt_tc3: problems of one launch with different precisions"); return -2; }
     if (p.M <= 0 || p.N <= 0) continue;
     if (!(raw ? tc_eligible(p) : presplit(p) && tc3_eligible(p))) {
       set_error("gemm_nt_tc3: operands violate the TMA alignment / pre-split contract");
@@ -1244,7 +1407,7 @@ static int launch_nt(const GemmNT* ps, const int* dep, int n, int* flags, bool r
     const int sp = epi_spec(p);
     spec = (spec < 0 || spec == sp) ? sp : EPI_SPEC_GENERIC;     // one epilogue specialisation per launch
     GIB_TRY(make_map(&maps.a[np], p.A, p.M, p.K, p.lda, BM));
-    GIB_TRY(make_map(&maps.b[np], raw ? p.B : p.B_hi, p.N, p.K, p.ldb, tbn));
+    GIB_TRY(make_map(&maps.b[np], raw ? p.B : p.B_hi, p.N, p.K, p.ldb, tbn, h16));
     if (!raw && !tf32) GIB_TRY(make_map(&maps.b_lo[np], p.B_lo, p.N, p.K, p.ldb, tbn));
     if (!raw && (sp == EPI_SPEC_DSELU || sp == EPI_SPEC_ADD)) GIB_TRY(make_map(&maps.aux[np], p.aux, p.M, p.n_store, p.ldaux, BM));
     P.g[np] = p;
@@ -1278,7 +1441,9 @@ static int launch_nt(const GemmNT* ps, const int* dep, int n, int* flags, bool r
   }
   const int grid = (int)(tiles < num_sms ? tiles : num_sms);
   ProfScope prof(PROF_GEMM_NT, work, st, dyn, ndyn);
-  if (tf32) launch_nt_kernel<true>(maps, P, raw, spec, grid, st);
+  if (h16 == 1) launch_nt_kernel16<1>(maps, P, spec, grid, st);
+  else if (h16 == 2) launch_nt_kernel16<2>(maps, P, spec, grid, st);
+  else if (tf32) launch_nt_kernel<true>(maps, P, raw, spec, grid, st);
   else launch_nt_kernel<false>(maps, P, raw, spec, grid, st);
   GIB_LAUNCH_CHECK();
   return 0;
@@ -1376,11 +1541,13 @@ static int launch_tn(const GemmDW* qs, int n, int chunk_rows, float* const* part
   Params P;
   memset(&P, 0, sizeof(P));
   long long items = 0;
-  const bool tf32 = qs[0].tf32 != 0;
+  const int prec = qs[0].tf32;
+  const bool tf32 = prec != 0;
+  if (prec < 0 || prec > 3) { set_error("gemm_dw_tc3: unknown precision %d", prec); return -2; }
   for (int i = 0; i < n; ++i) {
     const GemmDW& q = qs[i];
     if (!tc3_dw_eligible(q)) { set_error("gemm_dw_tc3: operands violate the TMA alignment contract"); return -2; }
-    if ((q.tf32 != 0) != tf32) { set_error("gemm_dw_tc3: problems of one launch with different precisions"); return -2; }
+    if (q.tf32 != prec) { set_error("gemm_dw_tc3: problems of one launch with different precisions"); return -2; }
     GIB_TRY(make_map(&maps.a[i], q.G, q.M, q.Nn, q.ldg, BKF));          // 32 x 32 boxes
     GIB_TRY(make_map(&maps.b[i], q.X, q.M, q.Kk, q.ldx, BKF));
     GemmNT& g = P.g[i];
@@ -1399,7 +1566,9 @@ static int launch_tn(const GemmDW* qs, int n, int chunk_rows, float* const* part
   P.chunk_rows = chunk_rows;
   P.trace = g_trace; P.trace_tiles = g_trace_tiles;
   const int grid = (int)(items < num_sms ? items : num_sms);
-  if (tf32) tc3_wgmma_dw_kernel<true><<<grid, WG_THREADS, DW_SMEM_BYTES, st>>>(maps, P);
+  if (prec == 2) tc3_wgmma_dw_kernel<true, 1><<<grid, WG_THREADS, DW_SMEM_BYTES, st>>>(maps, P);
+  else if (prec == 3) tc3_wgmma_dw_kernel<true, 2><<<grid, WG_THREADS, DW_SMEM_BYTES, st>>>(maps, P);
+  else if (tf32) tc3_wgmma_dw_kernel<true><<<grid, WG_THREADS, DW_SMEM_BYTES, st>>>(maps, P);
   else tc3_wgmma_dw_kernel<false><<<grid, WG_THREADS, DW_SMEM_BYTES, st>>>(maps, P);
   GIB_LAUNCH_CHECK();
   return 0;

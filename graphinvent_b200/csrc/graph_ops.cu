@@ -866,6 +866,14 @@ __device__ __forceinline__ float tf32_rna(float x) {
   return __uint_as_float(r);
 }
 
+// element i of a 16-bit plane (h16 1: bf16, 2: fp16) at `plane`: v rounded to nearest-even, as tensor.to(dtype)
+__device__ __forceinline__ void store16(float* plane, long long i, float v, int h16) {
+  uint16_t u;
+  if (h16 == 1) asm("cvt.rn.bf16.f32 %0, %1;" : "=h"(u) : "f"(v));
+  else asm("cvt.rn.f16.f32 %0, %1;" : "=h"(u) : "f"(v));
+  reinterpret_cast<uint16_t*>(plane)[i] = u;
+}
+
 // all Linears of a model in ONE launch: the per-Linear descriptors travel as a kernel parameter (__grid_constant__)
 __global__ void __launch_bounds__(256) pack_all_kernel(const __grid_constant__ PackTable T, float* __restrict__ packed) {
   __shared__ int s_idx;
@@ -890,7 +898,8 @@ __global__ void __launch_bounds__(256) pack_all_kernel(const __grid_constant__ P
       packed[E.ow + idx] = v;
       const float h = tf32_rna(v);
       packed[E.ow_hi + idx] = h;
-      packed[E.ow_lo + idx] = tf32_rna(v - h);
+      if (T.h16) store16(packed + E.ow_lo, idx, v, T.h16);
+      else packed[E.ow_lo + idx] = tf32_rna(v - h);
     } else if (idx < n1 + n2) {
       const long long k = idx - n1;
       const int c = (int)(k / Rp), pr = (int)(k % Rp);
@@ -900,7 +909,8 @@ __global__ void __launch_bounds__(256) pack_all_kernel(const __grid_constant__ P
       packed[E.owt + k] = v;
       const float h = tf32_rna(v);
       packed[E.owt_hi + k] = h;
-      packed[E.owt_lo + k] = tf32_rna(v - h);
+      if (T.h16) store16(packed + E.owt_lo, k, v, T.h16);
+      else packed[E.owt_lo + k] = tf32_rna(v - h);
     } else if (idx < n1 + n2 + Rp) {
       const int pr = (int)(idx - n1 - n2);
       const int g = pr / E.Rbp, rr = pr % E.Rbp;

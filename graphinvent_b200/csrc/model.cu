@@ -145,10 +145,12 @@ int build_plan(const gib_dims& d, Plan& pl) {
   return 0;
 }
 
-int pack_params(const Plan& pl, const float* const* params, float* packed, cudaStream_t st) {
+int pack_params(const Plan& pl, const float* const* params, float* packed, int prec, cudaStream_t st) {
+  GIB_TRY(check_precision(prec, "gib_model_pack"));
   {   // one launch for the whole model (52-67 Linears at the reference's defaults, at most kMaxPackEntries)
     PackTable T;
     T.n = (int)pl.lins.size();
+    T.h16 = prec >= 2 ? prec - 1 : 0;
     unsigned blk = 0;
     for (int i = 0; i < T.n; ++i) {
       const Lin& l = pl.lins[i];
@@ -356,7 +358,7 @@ static int mlp_forward(const Run& r, const Mlp& m, const float* X0, const MlpAct
     const Lin& L = r.pl.lins[m.first + l - 1];
     GemmNT p;
     p.A = x; p.lda = ldx;
-    p.B = r.packed + L.ow; p.ldb = L.Cp; p.B_hi = r.packed + L.ow_hi; p.B_lo = r.packed + L.ow_lo;
+    p.B = r.packed + L.ow; p.ldb = L.Cp; r.planes(p, L.ow_hi, L.ow_lo);
     p.M = rows; p.N = L.Rp; p.K = L.Cp;
     p.bias = L.pb >= 0 ? r.packed + L.ob : nullptr;
     p.act = m.act; p.mode = EPI_ACT; p.tf32 = r.tf32;
@@ -399,7 +401,7 @@ static int mlp_backward(const Run& r, const BwdBufs& bb, const Mlp& m, const flo
     if (l > 1 || dX0) {
       GemmNT p;
       p.A = G; p.lda = L.Rp;
-      p.B = r.packed + L.owt; p.ldb = L.Rp; p.B_hi = r.packed + L.owt_hi; p.B_lo = r.packed + L.owt_lo;
+      p.B = r.packed + L.owt; p.ldb = L.Rp; r.planes(p, L.owt_hi, L.owt_lo);
       p.M = rows; p.N = L.Ctp; p.K = L.Rp;
       p.n_store = L.Ctp; p.n_valid = L.Ctp; p.tf32 = r.tf32;
       p.work = 2.0 * rows * (double)L.R * L.Ct;
@@ -492,7 +494,7 @@ static int mlp_forward_multi(const Run& r, const MlpJob* jobs, int n, int* flags
       GemmNT& p = ps[np];
       p = GemmNT();
       p.A = x[i]; p.lda = ldx[i];
-      p.B = r.packed + L.ow; p.ldb = L.Cp; p.B_hi = r.packed + L.ow_hi; p.B_lo = r.packed + L.ow_lo;
+      p.B = r.packed + L.ow; p.ldb = L.Cp; r.planes(p, L.ow_hi, L.ow_lo);
       p.M = j.rows; p.N = L.Rp; p.K = L.Cp;
       p.bias = L.pb >= 0 ? r.packed + L.ob : nullptr;
       p.act = j.m->act; p.mode = EPI_ACT; p.tf32 = r.tf32;
@@ -614,7 +616,7 @@ static int mlp_backward_multi(const Run& r, const BwdBufs& bb, const MlpBwdJob* 
       GemmNT& p = all[nall];
       p = GemmNT();
       p.A = G[l][i]; p.lda = L.Rp; p.B = r.packed + L.owt; p.ldb = L.Rp;
-      p.B_hi = r.packed + L.owt_hi; p.B_lo = r.packed + L.owt_lo;
+      r.planes(p, L.owt_hi, L.owt_lo);
       p.M = j.rows; p.N = L.Ctp; p.K = L.Rp; p.n_store = L.Ctp; p.n_valid = L.Ctp;
       p.work = 2.0 * j.rows * (double)L.R * L.Ct;
       p.C = const_cast<float*>(G[l - 1][i]); p.ldc = L.Ctp;
@@ -648,7 +650,7 @@ static int mlp_backward_multi(const Run& r, const BwdBufs& bb, const MlpBwdJob* 
     const Lin& L = r.pl.lins[j.m->first];
     GemmNT p1;
     p1.A = G[1][i]; p1.lda = L.Rp; p1.B = r.packed + L.owt; p1.ldb = L.Rp;
-    p1.B_hi = r.packed + L.owt_hi; p1.B_lo = r.packed + L.owt_lo;
+    r.planes(p1, L.owt_hi, L.owt_lo);
     p1.M = j.rows; p1.N = L.Ctp; p1.K = L.Rp; p1.n_store = L.Ctp; p1.n_valid = L.Ctp;
     p1.work = 2.0 * j.rows * (double)L.R * L.Ct;
     p1.C = j.dX0; p1.ldc = j.ld_dx;
@@ -846,13 +848,13 @@ static int node_model_forward(const Run& r, float* out) {
       GemmNT ps[2];
       GemmNT& p = ps[0];
       p.A = r.ws + L.msum[t]; p.lda = Mp; p.B = r.packed + ih.ow; p.ldb = ih.Cp; p.C = r.ws + L.gi[t]; p.ldc = ih.Rp;
-      p.B_hi = r.packed + ih.ow_hi; p.B_lo = r.packed + ih.ow_lo;
+      r.planes(p, ih.ow_hi, ih.ow_lo);
       p.M = (int)S; p.N = ih.Rp; p.K = ih.Cp; p.bias = r.packed + ih.ob; p.act = ACT_NONE; p.mode = EPI_ACT;
       p.n_store = p.n_valid = ih.Rp; p.work = 2.0 * S * (double)ih.R * ih.C; p.tf32 = r.tf32;
       GemmNT& q2 = ps[1];
       q2 = p;
       q2.A = h; q2.lda = Hp; q2.B = r.packed + hh.ow; q2.ldb = hh.Cp; q2.C = r.ws + L.gh[t]; q2.ldc = hh.Rp;
-      q2.B_hi = r.packed + hh.ow_hi; q2.B_lo = r.packed + hh.ow_lo;
+      r.planes(q2, hh.ow_hi, hh.ow_lo);
       q2.N = hh.Rp; q2.K = hh.Cp; q2.bias = r.packed + hh.ob; q2.n_store = q2.n_valid = hh.Rp;
       q2.work = 2.0 * S * (double)hh.R * hh.C;
       GIB_TRY(gemm_nt_group(ps, 2, r.st));
@@ -903,13 +905,13 @@ static int node_model_backward(const Run& r, const BwdBufs& bb, const float* out
       GemmNT ps[2];
       GemmNT& p = ps[0];
       p.A = sc + bb.dgi; p.lda = ih.Rp; p.B = r.packed + ih.owt; p.ldb = ih.Rp; p.C = sc + bb.dmsum; p.ldc = Mp;
-      p.B_hi = r.packed + ih.owt_hi; p.B_lo = r.packed + ih.owt_lo;
+      r.planes(p, ih.owt_hi, ih.owt_lo);
       p.M = (int)S; p.N = ih.Ctp; p.K = ih.Rp; p.mode = EPI_ACT; p.act = ACT_NONE; p.n_store = p.n_valid = ih.Ctp;
       p.work = 2.0 * S * (double)ih.R * ih.C; p.tf32 = r.tf32;
       GemmNT& q2 = ps[1];
       q2.tf32 = r.tf32;
       q2.A = sc + bb.dgh; q2.lda = hh.Rp; q2.B = r.packed + hh.owt; q2.ldb = hh.Rp; q2.C = dh; q2.ldc = Hp;
-      q2.B_hi = r.packed + hh.owt_hi; q2.B_lo = r.packed + hh.owt_lo;
+      r.planes(q2, hh.owt_hi, hh.owt_lo);
       q2.M = (int)S; q2.N = hh.Ctp; q2.K = hh.Rp; q2.mode = EPI_ADD; q2.aux = dh_dir; q2.ldaux = Hp;
       q2.n_store = q2.n_valid = hh.Ctp; q2.work = 2.0 * S * (double)hh.R * hh.C;
       // h[0] is the zero-padded input (summation_mpnn.py:121-125): nothing consumes d h[0], so at t == 0 the dh GEMM,
@@ -1005,7 +1007,7 @@ static int emn_forward(const Run& r, float* out) {
                               r.ga.ent_src, r.ga.dst_ptr, E, live, r.st));
     GemmNT p;
     p.A = r.ws + L.emsg[t]; p.lda = Hp; p.B = r.packed + ih.ow; p.ldb = ih.Cp; p.C = r.ws + L.gi[t]; p.ldc = ih.Rp;
-    p.B_hi = r.packed + ih.ow_hi; p.B_lo = r.packed + ih.ow_lo;
+    r.planes(p, ih.ow_hi, ih.ow_lo);
     p.M = E; p.N = ih.Rp; p.K = ih.Cp; p.bias = r.packed + ih.ob; p.act = ACT_NONE; p.mode = EPI_ACT;
     p.n_store = p.n_valid = ih.Rp;
     p.m_dev = live; p.base_dev = base; p.tf32 = r.tf32;
@@ -1060,7 +1062,7 @@ static int emn_backward(const Run& r, const BwdBufs& bb, const float* out, const
     GIB_TRY(colsum_add(r.grads[hh.pb], sc + bb.dgh, hh.Rp, E, hh.R, hh.Rb, hh.Rbp, live, r.st));  // d b_hh; d W_hh = 0
     GemmNT p;
     p.A = sc + bb.dgi; p.lda = ih.Rp; p.B = r.packed + ih.owt; p.ldb = ih.Rp; p.C = sc + bb.dmsum; p.ldc = Hp;
-    p.B_hi = r.packed + ih.owt_hi; p.B_lo = r.packed + ih.owt_lo;
+    r.planes(p, ih.owt_hi, ih.owt_lo);
     p.M = E; p.N = ih.Ctp; p.K = ih.Rp; p.mode = EPI_ACT; p.act = ACT_NONE; p.n_store = p.n_valid = ih.Ctp;
     p.m_dev = live; p.base_dev = base; p.tf32 = r.tf32;
     GIB_TRY(gemm_nt(p, r.st));

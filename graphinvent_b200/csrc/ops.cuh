@@ -12,7 +12,9 @@ struct PackEntry {   // one reference weight (+bias) -> its padded / transposed 
   int nblk, Rb, Rbp, C, Cp, Ct, Ctp;
   unsigned blk_begin;
 };
-struct PackTable { int n; unsigned total_blocks; PackEntry e[kMaxPackEntries]; };
+// h16: 0 = the TF32 (hi, lo) planes of Wp / WTp; 1 / 2 = their hi planes and, over the bytes of each lo plane, the
+// bf16 / fp16 plane (Wp / WTp rounded to nearest-even, same shape, ld in 16-bit elements) of the 16-bit matmul modes
+struct PackTable { int n; unsigned total_blocks; int h16; PackEntry e[kMaxPackEntries]; };
 int pack_all(const PackTable& T, float* packed, cudaStream_t st);
 
 int concat2(float* dst, int ldd, const float* a, int lda, int wa, const float* b, int ldb, int wb, long long rows, cudaStream_t st);

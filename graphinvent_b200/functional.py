@@ -12,7 +12,7 @@ import numpy as np
 import torch
 
 from ._lib import (Dims, FLAG_MULTITYPE, FLAG_OVERFLOW, HDR_E, HDR_FLAGS, HDR_INTS, HDR_P, MODEL_ID, check, lib)
-from .config import tf32_enabled
+from .config import dtype_of_code, matmul_code
 
 _u8 = torch.uint8
 
@@ -28,10 +28,10 @@ def _stream(device):
 def make_dims(model, batch, in_dtype=0, tf32=None):
     """`in_dtype`: 0 = float32 batches (BlockDatasetLoader layout), 1 = int8 batches (the on-disk HDF5 type, read
     directly by K0 and the first-layer kernels).  `tf32`: precision of the tensor-core GEMMs of the model calls made
-    with these dims (`matmul_precision`), 1 = single-pass TF32, 0 = 3xTF32; None = torch's current setting
-    (`config.tf32_enabled`)."""
+    with these dims (`matmul_precision`), 0 = 3xTF32, 1 (or True) = single-pass TF32, 2 = bf16, 3 = fp16 operands;
+    None = torch's current autocast / TF32 state (`config.matmul_code`)."""
     d = Dims()
-    d.tf32 = int(tf32_enabled() if tf32 is None else bool(tf32))
+    d.tf32 = matmul_code() if tf32 is None else precision_code(tf32)
     kw = model.dims()
     for name, _ in Dims._fields_:
         if name in ("model", "B", "big", "in_dtype"):
@@ -42,6 +42,16 @@ def make_dims(model, batch, in_dtype=0, tf32=None):
     d.big = float(kw.get("big", 1e6))
     d.in_dtype = int(in_dtype)
     return d
+
+
+def precision_code(tf32):
+    """a precision code from a code or a bool: 2 / 3 stay, any other value counts as a TF32 flag"""
+    return int(tf32) if tf32 in (2, 3) and not isinstance(tf32, bool) else int(bool(tf32))
+
+
+def autocast_dtype_of(d):
+    """the autocast dtype whose precision dims `d` run in (None: the fp32-input modes)"""
+    return dtype_of_code(d.tf32)
 
 
 def dims_key(model, batch, in_dtype=0, tf32=None):
@@ -115,7 +125,9 @@ def invalidate_packed_weights():
 def packed_weights(model, d, params):
     """Zero-padded / transposed weight arena, rebuilt only when a parameter changed
     (keyed on data_ptr + in-place version counter, so generation re-uses it every round)."""
-    key = (_weights_epoch[0],) + tuple((p.data_ptr(), p._version) for p in params)
+    # the arena of a 16-bit mode holds that mode's weight planes (gib_model_pack): it serves that mode only
+    kind = d.tf32 if d.tf32 >= 2 else 0
+    key = (_weights_epoch[0], kind) + tuple((p.data_ptr(), p._version) for p in params)
     if model._packed is not None and model._packed_key == key:
         return model._packed
     if model._packed_key is None or len(model._packed_key) != len(key):
@@ -123,7 +135,8 @@ def packed_weights(model, d, params):
     dev = params[0].device
     nbytes = lib.gib_model_packed_bytes(ctypes.byref(d))
     packed = torch.empty(nbytes, dtype=_u8, device=dev)
-    check(lib.gib_model_pack(ctypes.byref(d), _ptr_table(params), _ptr(packed), _stream(dev)), "gib_model_pack")
+    with matmul_precision(d):
+        check(lib.gib_model_pack(ctypes.byref(d), _ptr_table(params), _ptr(packed), _stream(dev)), "gib_model_pack")
     model._packed, model._packed_key = packed, key
     return packed
 

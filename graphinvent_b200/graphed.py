@@ -49,7 +49,11 @@ Matmul precision: each of these objects reads torch's float32 matmul precision o
 (`config.tf32_enabled`, exposed as its `tf32` attribute), and bakes it into its graphs -- single-pass TF32 GEMMs when
 the user allowed TF32, 3xTF32 otherwise -- as torch's own captured cuBLAS calls keep the math mode of their capture.
 Changing the setting afterwards does not change what a replay computes (the RL backward rounds included); build a new
-object to switch.
+object to switch.  The same holds for `torch.autocast("cuda", dtype=torch.bfloat16 | torch.float16)`: built inside
+such a context, an object runs its tensor-core GEMMs on bf16 / fp16 operands (`config.matmul_code`; exposed as its
+`autocast_dtype`, None otherwise) whether or not later replays run inside one.  `TrainStep` honours bf16 only: built
+under fp16 autocast it keeps the fp32-input precision (`autocast_dtype` None), because its fused loss has no gradient
+scaling and unscaled fp16 gradients underflow.
 """
 import ctypes
 import types
@@ -57,6 +61,7 @@ import types
 import torch
 
 from . import functional as F
+from .config import matmul_code
 from ._lib import FLAG_MULTITYPE, FLAG_OVERFLOW, HDR_FLAGS, HDR_INTS, EvalPass, check, lib
 from .generation import GraphGenerator
 
@@ -107,8 +112,10 @@ class TrainStep:
         self.nodes = torch.zeros(self.B, N, Fn, dtype=in_dt, device=dev)
         self.edges = torch.zeros(self.B, N, N, Ef, dtype=in_dt, device=dev)
         self.target = torch.zeros(self.B, self.apd, dtype=torch.float32, device=dev)
-        self.d = F.make_dims(model, self.B, self.code)
-        self.tf32 = bool(self.d.tf32)             # torch's matmul precision at construction, baked into the graphs
+        # torch's matmul precision at construction, baked into the graphs (fp16 autocast is not honoured: no loss scaling)
+        self.d = F.make_dims(model, self.B, self.code, tf32=matmul_code(fp16=False))
+        self.tf32 = self.d.tf32 == 1
+        self.autocast_dtype = F.autocast_dtype_of(self.d)
         d = self.d
         self.capacity = int(entry_capacity)
         # static buffers (addresses are baked into the graph)
@@ -169,8 +176,8 @@ class TrainStep:
         check(lib.gib_graph_count(bd, F._ptr(self.edges), F._ptr(self.cws), st), "gib_graph_count")
         check(lib.gib_graph_fill(bd, F._ptr(self.edges), F._ptr(self.cws), self.hdr, F._ptr(self.gbuf), st),
               "gib_graph_fill")
-        check(lib.gib_model_pack(bd, F._ptr_table(self.params), F._ptr(self.packed), st), "gib_model_pack")
         with F.matmul_precision(d):
+            check(lib.gib_model_pack(bd, F._ptr_table(self.params), F._ptr(self.packed), st), "gib_model_pack")
             check(lib.gib_model_forward(bd, self.hdr, F._ptr(self.nodes), F._ptr(self.edges), F._ptr(self.gbuf),
                                         F._ptr(self.packed), F._ptr(self.ws), F._ptr(self.out), st), "gib_model_forward")
         # Workflow.loss (Workflow.py:833-860) over the live rows, the batch-mean taken over ctl's denominator (the
@@ -303,7 +310,8 @@ class EvalStep:
         self.N = C.max_n_nodes
         self.apd = self.N * (C.len_f_add_per_node + C.len_f_conn_per_node) + 1
         self.d = F.make_dims(model, self.B, self.code)
-        self.tf32 = bool(self.d.tf32)             # torch's matmul precision at construction, baked into the graph
+        self.tf32 = self.d.tf32 == 1              # torch's matmul precision at construction, baked into the graph
+        self.autocast_dtype = F.autocast_dtype_of(self.d)
         F._check_params(model, self.d, params)
         dev, bd = self.dev, ctypes.byref(self.d)
         if share is not None:
@@ -376,8 +384,9 @@ class EvalStep:
         F._require_cuda(*params)
         F._check_params(self.model, self.d, params)
         st = F._stream(self.dev)
-        check(lib.gib_model_pack(ctypes.byref(self.d), F._ptr_table(params), F._ptr(self.packed), st),
-              "gib_model_pack")
+        with F.matmul_precision(self.d):
+            check(lib.gib_model_pack(ctypes.byref(self.d), F._ptr_table(params), F._ptr(self.packed), st),
+                  "gib_model_pack")
         desc = EvalPass(batch_loss=slots.data_ptr() if slots.numel() else None,
                         lik=lik.data_ptr() if lik is not None and lik.numel() else None,
                         lik_len=lik.numel() if lik is not None else 0, n_slots=slots.numel())
@@ -488,7 +497,8 @@ class GraphedGenerator(GraphGenerator):
         self.params = list(model.parameters())
         F._require_cuda(*self.params)
         self.d = F.make_dims(model, B, 0)
-        self.tf32 = bool(self.d.tf32)             # torch's matmul precision at construction, baked into the graph
+        self.tf32 = self.d.tf32 == 1              # torch's matmul precision at construction, baked into the graph
+        self.autocast_dtype = F.autocast_dtype_of(self.d)
         bd = ctypes.byref(self.d)
         F._check_params(model, self.d, self.params)
         self.entry_capacity = entry_capacity(B, N, self.Ef)
@@ -536,15 +546,16 @@ class GraphedGenerator(GraphGenerator):
         if model.training and any(p > 0.0 for p in model._dropout_ps()):
             raise NotImplementedError("dropout_p > 0 in training mode is not supported by the fused sm_90a path")
         params = list(model.parameters())
-        key = (F._weights_epoch[0],) + tuple((p.data_ptr(), p._version) for p in params)
+        key = (F._weights_epoch[0], self.d.tf32) + tuple((p.data_ptr(), p._version) for p in params)
         if key == self._packed_key:
             return
         if len(params) != len(self.params) or any(p.shape != q.shape for p, q in zip(params, self.params)):
             raise RuntimeError("the model's parameter table changed after the GraphedGenerator was built")
         F._require_cuda(*params)
         self.params = params
-        check(lib.gib_model_pack(ctypes.byref(self.d), F._ptr_table(params), F._ptr(self.packed),
-                                 F._stream(self.device)), "gib_model_pack")
+        with F.matmul_precision(self.d):     # the arena of a 16-bit mode holds that mode's planes
+            check(lib.gib_model_pack(ctypes.byref(self.d), F._ptr_table(params), F._ptr(self.packed),
+                                     F._stream(self.device)), "gib_model_pack")
         self._packed_key = key
 
     # ---- the captured round -------------------------------------------------------------------------------
@@ -711,7 +722,8 @@ class GraphedGeneratorRL(GraphedGenerator):
         self.params = list(model.parameters())
         F._require_cuda(*self.params)
         self.d = F.make_dims(model, B, 1)                 # int8 model inputs: the 0/1 state, bit-exact logits
-        self.tf32 = bool(self.d.tf32)   # torch's matmul precision at construction: rollouts and their backward rounds
+        self.tf32 = self.d.tf32 == 1    # torch's matmul precision at construction: rollouts and their backward rounds
+        self.autocast_dtype = F.autocast_dtype_of(self.d)
         self._key = F.key_of(self.d)
         bd = ctypes.byref(self.d)
         F._check_params(model, self.d, self.params)
@@ -767,7 +779,7 @@ class GraphedGeneratorRL(GraphedGenerator):
             if m.training and any(p > 0.0 for p in m._dropout_ps()):
                 raise NotImplementedError("dropout_p > 0 in training mode is not supported by the fused sm_90a path")
         tables = [list(m.parameters()) for m in models]
-        key = (F._weights_epoch[0],) + tuple((p.data_ptr(), p._version) for ps in tables for p in ps)
+        key = (F._weights_epoch[0], self.d.tf32) + tuple((p.data_ptr(), p._version) for ps in tables for p in ps)
         if key == self._packed_key:
             return
         for slot, ps in enumerate(tables):
@@ -778,8 +790,9 @@ class GraphedGeneratorRL(GraphedGenerator):
         if len(params) != len(self.params) or any(p.shape != q.shape for p, q in zip(params, self.params)):
             raise RuntimeError("the model's parameter table changed after the GraphedGeneratorRL was built")
         F._require_cuda(*params)
-        check(lib.gib_model_pack(ctypes.byref(self.d), F._ptr_table(params), F._ptr(self.packed[slot]),
-                                 F._stream(self.device)), "gib_model_pack")
+        with F.matmul_precision(self.d):
+            check(lib.gib_model_pack(ctypes.byref(self.d), F._ptr_table(params), F._ptr(self.packed[slot]),
+                                     F._stream(self.device)), "gib_model_pack")
 
     # ---- the captured rollout round -----------------------------------------------------------------------
     def _k0_forward(self, slots):

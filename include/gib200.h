@@ -91,7 +91,14 @@ int gib_get_tensor_cores(void);
  * precision torch gives a CUDA fp32 matmul when its fp32_precision is "tf32".  The fp32 SIMT GEMMs (narrow APD output
  * layers, small exact-mode problems) and every non-GEMM kernel are fp32 in both modes.  The setting is read when a
  * call launches its kernels, so a CUDA graph captured around a call keeps the mode it was captured with.  No size
- * query, workspace or packed-weight layout depends on it.  Thread-local; the other entry points ignore it. */
+ * query, workspace or packed-weight layout depends on it.  Thread-local; the other entry points ignore it.
+ * 2 = bf16, 3 = fp16 (torch.autocast): every tensor-core GEMM operand (activations, output gradients, inputs, weights)
+ * rounded to nearest-even to 16 bits, as tensor.to(torch.bfloat16 / torch.float16) rounds, fp32 accumulation; an fp16
+ * operand beyond +-65504 becomes +-inf as torch's cast makes it.  The SIMT GEMMs, the bias-gradient sums, every other
+ * kernel and every buffer stay fp32.  gib_model_pack also reads the setting: in the 16-bit modes it writes the 16-bit
+ * planes of the weights over the bytes of their TF32 lo planes (the arena size is the same), so an arena packed in a
+ * 16-bit mode serves that mode only.  A 16-bit call is refused when the tensor cores are off (gib_set_tensor_cores) or
+ * gib_tc_debug bit 0 is set.  Other values: nonzero = 1. */
 void gib_set_matmul_tf32(int on);
 int gib_get_matmul_tf32(void);
 /* bit 3: GGNN / MNN message MLPs on one row per bond entry (the AttentionGGNN's layout) instead of one per message row.
@@ -238,6 +245,9 @@ int gib_linear_fwd_tc_planes(const float* X, int ldx, const float* W_hi, const f
                              const int* m_dev, const int* base_dev, gib_stream stream);
 /* TF32 hi / lo planes of a row-major matrix (round-to-nearest split), for callers of the entry above */
 int gib_split_planes(const float* W, float* W_hi, float* W_lo, long long n, gib_stream stream);
+/* the 16-bit plane of n fp32 values (kind 2 = bf16, 3 = fp16: the gib_set_matmul_tf32 codes), rounded to nearest-even
+ * as gib_model_pack rounds them, into n 16-bit values at out -- the W_hi of a 16-bit test-hook problem */
+int gib_round_plane16(const float* W, void* out, long long n, int kind, gib_stream stream);
 /* dW[R,C] += G^T X, dbias[R] += colsum(G); G [M, ldg], X [M, ldx]; scratch from gib_dw_scratch_bytes */
 size_t gib_dw_scratch_bytes(int M, int Nn, int Kk);
 int gib_linear_bwd_dw(const float* G, int ldg, int Nn, const float* X, int ldx, int Kk, int M, float* dW,
@@ -265,8 +275,10 @@ int gib_graph_gather(float* g, float* att, const float* en, const float* em, int
  * act 0 none / 1 selu / 2 tanh.  Columns [n_valid, n_store) are stored as zeros, columns >= n_store are not touched.
  * W_hi / W_lo (may be NULL): its TF32 planes (gib_split_planes).  m_dev / base_dev (may be NULL): the live row range
  * [*base_dev, *base_dev + *m_dev) inside buffers of M rows.  tf32: precision of the tensor-core kernels (0 = 3xTF32,
- * 1 = single-pass TF32, as gib_set_matmul_tf32; W then read from W_hi only, or raw W rounded in the kernel); the
- * problems of one call must agree. */
+ * 1 = single-pass TF32, as gib_set_matmul_tf32; W then read from W_hi only, or raw W rounded in the kernel; 2 / 3 =
+ * bf16 / fp16: W_hi then points at the 16-bit plane (gib_round_plane16, ldw in its elements, a multiple of 8 for the
+ * tensor-core path) and W_lo is ignored; a 16-bit problem without W_hi is refused); the problems of one call must
+ * agree. */
 typedef struct gib_gemm_problem {
   const float* A; int lda;
   const float* W; int ldw;
