@@ -113,10 +113,14 @@ _PROTOS = {
     "gib_sum_scaled": (c_i, [c_p, c_i, c_f, c_p, c_p]),
     "gib_fill_zero": (c_i, [c_p, c_sz, c_p]),
     "gib_kl_loss_fwd_bwd_ctl": (c_i, [c_p, c_p, c_i, c_i, c_p, c_p, c_p, c_p]),
+    "gib_kl_loss_fwd_bwd_ctl_scaled": (c_i, [c_p, c_p, c_i, c_i, c_p, c_p, c_p, c_p, c_p]),
     "gib_sum_scaled_ctl": (c_i, [c_p, c_i, c_p, c_p, c_p]),
     "gib_validation_nll_ctl": (c_i, [c_p, c_p, c_i, c_i, c_p, c_p, c_p]),
     "gib_eval_collect": (c_i, [c_p, c_p, c_p, c_i, c_i, c_p, c_p, c_p, c_p]),
     "gib_adam_step": (c_i, [c_p, c_p, c_p, c_p, c_ll, c_ll, c_d, c_d, c_d, c_d, c_d, c_d, c_p]),
+    "gib_nonfinite_check": (c_i, [c_p, c_ll, c_p, c_p]),
+    "gib_adam_step_scaled": (c_i, [c_p, c_p, c_p, c_p, c_ll, c_p, c_p, c_p, c_d, c_d, c_d, c_d, c_d, c_d, c_p]),
+    "gib_amp_update_scale": (c_i, [c_p, c_p, c_p, c_d, c_d, c_i, c_p, c_i, c_p]),
     "gib_sample_actions": (c_i, [c_p, c_i, c_i, c_p, c_p, c_p, c_p]),
     "gib_generation_scratch_bytes": (c_sz, [c_i]),
     "gib_generation_round": (c_i, [c_i] * 7 + [c_p] * 11 + [c_i, c_p, c_p, c_p]),

@@ -22,6 +22,7 @@ void set_error(const char* fmt, ...) {
 // ---- KL-divergence loss + gradient (Workflow.py:833-860), one CTA per molecule ---------
 __global__ void __launch_bounds__(256) kl_loss_kernel(const float* __restrict__ out, const float* __restrict__ target,
                                                       int apd, float grad_scale, const gib_batch_ctl* ctl,
+                                                      const float* __restrict__ loss_scale,
                                                       float* __restrict__ loss_rows, float* __restrict__ dout) {
   __shared__ float sm[8];
   const int b = blockIdx.x;
@@ -49,7 +50,11 @@ __global__ void __launch_bounds__(256) kl_loss_kernel(const float* __restrict__ 
     const float th = t[k] / ts;                 // Workflow.py:854 (NaN for an all-zero target row, as in the reference)
     const float logp = o[k] - lse;
     acc += (th > 0.f ? th * logf(th) : (th == 0.f ? 0.f : th)) - th * logp;   // xlogy(t,t) - t*logp
-    if (dout) dout[(size_t)b * apd + k] = (expf(logp) - th) * grad_scale;
+    if (dout) {
+      float d = (expf(logp) - th) * grad_scale;
+      if (loss_scale) d *= *loss_scale;         // autograd's dout * g for g = the GradScaler's scale
+      dout[(size_t)b * apd + k] = d;
+    }
   }
   acc = block_reduce<256>(acc, sm, false);
   if (threadIdx.x == 0 && loss_rows) loss_rows[b] = acc;
@@ -367,7 +372,7 @@ int gib_model_backward_part(const gib_dims* d, const int* hdr, const void* nodes
 int gib_kl_loss_fwd_bwd(const float* out, const float* target, int B, int apd, float grad_scale, float* loss_rows,
                         float* dout, gib_stream stream) {
   if (B <= 0) return 0;
-  kl_loss_kernel<<<B, 256, 0, ST(stream)>>>(out, target, apd, grad_scale, nullptr, loss_rows, dout);
+  kl_loss_kernel<<<B, 256, 0, ST(stream)>>>(out, target, apd, grad_scale, nullptr, nullptr, loss_rows, dout);
   GIB_LAUNCH_CHECK();
   return 0;
 }
@@ -375,7 +380,15 @@ int gib_kl_loss_fwd_bwd_ctl(const float* out, const float* target, int B, int ap
                             float* loss_rows, float* dout, gib_stream stream) {
   if (!ctl) { set_error("gib_kl_loss_fwd_bwd_ctl: ctl is null"); return -1; }
   if (B <= 0) return 0;
-  kl_loss_kernel<<<B, 256, 0, ST(stream)>>>(out, target, apd, 0.f, ctl, loss_rows, dout);
+  kl_loss_kernel<<<B, 256, 0, ST(stream)>>>(out, target, apd, 0.f, ctl, nullptr, loss_rows, dout);
+  GIB_LAUNCH_CHECK();
+  return 0;
+}
+int gib_kl_loss_fwd_bwd_ctl_scaled(const float* out, const float* target, int B, int apd, const gib_batch_ctl* ctl,
+                                   const float* loss_scale, float* loss_rows, float* dout, gib_stream stream) {
+  if (!ctl || !loss_scale) { set_error("gib_kl_loss_fwd_bwd_ctl_scaled: ctl and loss_scale must be non-null"); return -1; }
+  if (B <= 0) return 0;
+  kl_loss_kernel<<<B, 256, 0, ST(stream)>>>(out, target, apd, 0.f, ctl, loss_scale, loss_rows, dout);
   GIB_LAUNCH_CHECK();
   return 0;
 }

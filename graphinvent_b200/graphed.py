@@ -15,8 +15,8 @@ data-parallel all-reduce when a process group is given, and the optimizer step. 
 keeps every data-dependent extent in device memory, so the captured launch parameters never depend on the batch
 content; a batch with more bond entries than `entry_capacity` is truncated and flagged, `check()` reports it.
 
-The optimizer is stepped eagerly after the graph (its step count / learning-rate schedule are host state); with
-`optim.FlatAdam` that is one more launch.  There is no CPU path.  A batch may hold fewer than `batch_size` molecules
+The optimizer is stepped eagerly after the graph (its learning-rate schedule is host state, and so is its step count
+unless a gradient scaler is given); with `optim.FlatAdam` that is one more launch.  There is no CPU path.  A batch may hold fewer than `batch_size` molecules
 (the tail batch of each block of the reference's loader): the live count and the loss scale are device memory
 (`gib_batch_ctl`), so the same graph serves it.
 
@@ -51,9 +51,19 @@ the user allowed TF32, 3xTF32 otherwise -- as torch's own captured cuBLAS calls 
 Changing the setting afterwards does not change what a replay computes (the RL backward rounds included); build a new
 object to switch.  The same holds for `torch.autocast("cuda", dtype=torch.bfloat16 | torch.float16)`: built inside
 such a context, an object runs its tensor-core GEMMs on bf16 / fp16 operands (`config.matmul_code`; exposed as its
-`autocast_dtype`, None otherwise) whether or not later replays run inside one.  `TrainStep` honours bf16 only: built
-under fp16 autocast it keeps the fp32-input precision (`autocast_dtype` None), because its fused loss has no gradient
-scaling and unscaled fp16 gradients underflow.
+`autocast_dtype`, None otherwise) whether or not later replays run inside one.  `TrainStep` without a gradient scaler
+honours bf16 only: built under fp16 autocast it keeps the fp32-input precision (`autocast_dtype` None), because
+unscaled fp16 gradients underflow.  With `grad_scaler=` an enabled `torch.amp.GradScaler("cuda")` and a `FlatAdam`, it
+takes every mode, fp16 included, and runs torch's dynamic loss scaling on the device:
+
+    scaler = torch.amp.GradScaler("cuda")
+    with torch.autocast("cuda", dtype=torch.float16):
+        step = graphinvent_b200.graphed.TrainStep(model, FlatAdam(model.parameters()), B, E_cap, grad_scaler=scaler)
+
+Each step then equals, bit for bit, the eager `scaler.scale(loss).backward(); scaler.step(opt); scaler.update()`: the
+loss gradient is multiplied by the scaler's scale inside the fused loss, a check over the gradient bucket sets
+`step.found_inf`, and `FlatAdam.scaled_step` skips or takes the Adam step and updates the scaler's own `_scale` /
+`_growth_tracker` tensors, all in stream order without a host read.
 """
 import ctypes
 import types
@@ -93,10 +103,44 @@ def _load_rows(step, b, nodes, edges, target):
             dst[b:].zero_()
 
 
+_SCALER_STATE = ("_scale", "_growth_tracker", "_growth_factor", "_backoff_factor", "_growth_interval",
+                 "_lazy_init_scale_growth_tracker")
+
+
+def _grad_scaler(scaler, optimizer):
+    """the scaler TrainStep runs with: None without one or for a disabled one; refuses what it cannot run"""
+    if scaler is None:
+        return None
+    if not isinstance(scaler, torch.amp.GradScaler):
+        raise TypeError(f"grad_scaler must be a torch.amp.GradScaler, got {type(scaler).__name__}")
+    if not scaler.is_enabled():
+        return None
+    if getattr(scaler, "_device", "cuda") != "cuda":
+        raise ValueError("grad_scaler must be a CUDA GradScaler: torch.amp.GradScaler(\"cuda\")")
+    from .optim import FlatAdam
+    if not isinstance(optimizer, FlatAdam):
+        raise ValueError("TrainStep(grad_scaler=) needs a graphinvent_b200.optim.FlatAdam optimizer (its step is gated "
+                         f"and unscaled on the device), got {type(optimizer).__name__}")
+    missing = [a for a in _SCALER_STATE if not hasattr(scaler, a)]
+    if missing:
+        raise RuntimeError(f"this torch's GradScaler lacks {missing}: TrainStep(grad_scaler=) updates the scaler's "
+                           "scale and growth-tracker tensors in place and cannot run with it")
+    return scaler
+
+
 class TrainStep:
+    @staticmethod
+    def precision_code(grad_scaler=None):
+        """the matmul precision code a TrainStep built now bakes in: torch's autocast / TF32 state, except that fp16
+        autocast counts only with an enabled gradient scaler"""
+        if grad_scaler is not None and grad_scaler.is_enabled():
+            return matmul_code()
+        return matmul_code(fp16=False)
+
     def __init__(self, model, optimizer, batch_size, entry_capacity, input_dtype=torch.float32, global_batch=None,
-                 group=None, device=None, warmup=True):
+                 group=None, device=None, warmup=True, grad_scaler=None):
         params = list(model.parameters())
+        self.grad_scaler = _grad_scaler(grad_scaler, optimizer)
         F._require_cuda(*params)
         self.model, self.optimizer = model, optimizer
         self.dev = device or params[0].device
@@ -112,8 +156,9 @@ class TrainStep:
         self.nodes = torch.zeros(self.B, N, Fn, dtype=in_dt, device=dev)
         self.edges = torch.zeros(self.B, N, N, Ef, dtype=in_dt, device=dev)
         self.target = torch.zeros(self.B, self.apd, dtype=torch.float32, device=dev)
-        # torch's matmul precision at construction, baked into the graphs (fp16 autocast is not honoured: no loss scaling)
-        self.d = F.make_dims(model, self.B, self.code, tf32=matmul_code(fp16=False))
+        # torch's matmul precision at construction, baked into the graphs (fp16 autocast only with a gradient scaler:
+        # unscaled fp16 gradients underflow)
+        self.d = F.make_dims(model, self.B, self.code, tf32=self.precision_code(self.grad_scaler))
         self.tf32 = self.d.tf32 == 1
         self.autocast_dtype = F.autocast_dtype_of(self.d)
         d = self.d
@@ -147,6 +192,12 @@ class TrainStep:
             p.grad = v
             o += p.numel()
         self.workspace_bytes = ws_bytes
+        # dynamic loss scaling: 1.0 when the last step's gradient bucket held an inf or NaN (that step was skipped)
+        self.found_inf = torch.zeros((), dtype=torch.float32, device=dev)
+        if self.grad_scaler is not None:
+            if self.grad_scaler._scale is None:
+                self.grad_scaler._lazy_init_scale_growth_tracker(dev)
+            optimizer.device_step_counts()
         # data parallel: the gradients of the readout parameters (gather.*, APDReadout.*: the tail of the parameter
         # order, 79 % of the bucket) are final after the first part of the backward; their all-reduce runs on a side
         # stream while the message-passing backward (second captured graph) still executes (SURVEY.md 8e)
@@ -182,12 +233,30 @@ class TrainStep:
                                         F._ptr(self.packed), F._ptr(self.ws), F._ptr(self.out), st), "gib_model_forward")
         # Workflow.loss (Workflow.py:833-860) over the live rows, the batch-mean taken over ctl's denominator (the
         # GLOBAL batch of data-parallel shards); padding rows get dout = 0 and add exact zeros to every gradient
-        check(lib.gib_kl_loss_fwd_bwd_ctl(F._ptr(self.out), F._ptr(self.target), self.B, self.apd, F._ptr(self.ctl),
-                                          F._ptr(self.rows), F._ptr(self.dout), st), "gib_kl_loss_fwd_bwd_ctl")
+        if self.grad_scaler is None:
+            check(lib.gib_kl_loss_fwd_bwd_ctl(F._ptr(self.out), F._ptr(self.target), self.B, self.apd,
+                                              F._ptr(self.ctl), F._ptr(self.rows), F._ptr(self.dout), st),
+                  "gib_kl_loss_fwd_bwd_ctl")
+        else:
+            # scaler.scale(loss).backward(): the loss gradient times the scaler's current scale, read on the device
+            check(lib.gib_fill_zero(F._ptr(self.found_inf), 4, st), "gib_fill_zero")
+            check(lib.gib_kl_loss_fwd_bwd_ctl_scaled(F._ptr(self.out), F._ptr(self.target), self.B, self.apd,
+                                                     F._ptr(self.ctl), F._ptr(self.grad_scaler._scale),
+                                                     F._ptr(self.rows), F._ptr(self.dout), st),
+                  "gib_kl_loss_fwd_bwd_ctl_scaled")
         check(lib.gib_sum_scaled_ctl(F._ptr(self.rows), self.B, F._ptr(self.ctl), F._ptr(self.loss), st),
               "gib_sum_scaled_ctl")
         check(lib.gib_fill_zero(F._ptr(self.gflat), self.gflat.numel() * 4, st), "gib_fill_zero")
         self._backward(1 if self.world > 1 else 0)
+        if self.grad_scaler is not None and self.world == 1:
+            self._check_grads()
+
+    def _check_grads(self):
+        """found_inf = 1 if the (all-reduced) gradient bucket holds an inf or NaN: the last node of the captured graph on
+        one GPU; after both all-reduces, outside the graphs, with a process group, so that every rank sees the same
+        bucket and skips the same steps"""
+        check(lib.gib_nonfinite_check(F._ptr(self.gflat), self.gflat.numel(), F._ptr(self.found_inf),
+                                      F._stream(self.dev)), "gib_nonfinite_check")
 
     def _backward(self, part):
         st = F._stream(self.dev)
@@ -220,7 +289,16 @@ class TrainStep:
             with torch.cuda.graph(g2):
                 self._backward(2)
             self.graph2 = g2
-        self._param_ptrs = [p.data_ptr() for p in self.params]
+        self._param_ptrs = self._captured_ptrs()
+
+    def _captured_ptrs(self):
+        """the addresses the graphs read that live outside this object: the parameters and the scaler's scale"""
+        ptrs = [p.data_ptr() for p in self.params]
+        if self.grad_scaler is not None:
+            if self.grad_scaler._scale is None:
+                self.grad_scaler._lazy_init_scale_growth_tracker(self.dev)
+            ptrs.append(self.grad_scaler._scale.data_ptr())
+        return ptrs
 
     # ---- one step -----------------------------------------------------------------------------------------
     def load(self, nodes, edges, target, global_batch=None):
@@ -242,7 +320,7 @@ class TrainStep:
     def __call__(self, nodes=None, edges=None, target=None, global_batch=None):
         if nodes is not None:
             self.load(nodes, edges, target, global_batch=global_batch)
-        if [p.data_ptr() for p in self.params] != self._param_ptrs:
+        if self._captured_ptrs() != self._param_ptrs:
             self.capture()                        # the parameters moved (optimizer re-flattened them)
         for p, v in zip(self.params, self.views):
             if p.grad is not v:
@@ -260,7 +338,12 @@ class TrainStep:
             if self.tail_off > 0:
                 dist.all_reduce(self.gflat[:self.tail_off], op=dist.ReduceOp.SUM, group=grp)
             cur.wait_stream(self.comm_stream)
-        self.optimizer.step()
+            if self.grad_scaler is not None:
+                self._check_grads()
+        if self.grad_scaler is not None:
+            self.optimizer.scaled_step(self.found_inf, self.grad_scaler)     # scaler.step(opt); scaler.update()
+        else:
+            self.optimizer.step()
         F.invalidate_packed_weights()
         self.steps += 1
         return self.loss

@@ -191,6 +191,11 @@ typedef struct gib_batch_ctl {
 } gib_batch_ctl;
 int gib_kl_loss_fwd_bwd_ctl(const float* out, const float* target, int B, int apd, const gib_batch_ctl* ctl,
                             float* loss_rows, float* dout, gib_stream stream);   /* dout may be NULL */
+/* gib_kl_loss_fwd_bwd_ctl with dynamic loss scaling: every dout value it writes is multiplied once more, by the
+ * DEVICE float *loss_scale (a torch.amp.GradScaler's scale; autograd's `dout * scale` of scaler.scale(loss)).  The
+ * loss rows are not scaled.  ctl and loss_scale must be non-NULL. */
+int gib_kl_loss_fwd_bwd_ctl_scaled(const float* out, const float* target, int B, int apd, const gib_batch_ctl* ctl,
+                                   const float* loss_scale, float* loss_rows, float* dout, gib_stream stream);
 /* out[0] = ctl->scale * sum(rows[0..min(n, ctl->live))), the order gib_sum_scaled uses for those rows */
 int gib_sum_scaled_ctl(const float* rows, int n, const gib_batch_ctl* ctl, float* out, gib_stream stream);
 int gib_validation_nll_ctl(const float* out, const float* target, int B, int apd, const gib_batch_ctl* ctl,
@@ -229,6 +234,24 @@ int gib_eval_collect(const float* kl_rows, const float* nll_rows, const float* t
 int gib_adam_step(float* params, const float* grads, float* exp_avg, float* exp_avg_sq, long long n,
                   long long step, double lr, double beta1, double beta2, double eps, double weight_decay,
                   double grad_scale, gib_stream stream);
+
+/* ---- dynamic loss scaling on the device: torch.amp.GradScaler's `step(optimizer); update()` without a host read.
+ *      All scalars are DEVICE memory.
+ *      gib_nonfinite_check: *found_inf = 1.0f if any of x[0, n) is inf or NaN (the check of
+ *        torch._amp_foreach_non_finite_check_and_unscale_); it never clears *found_inf.
+ *      gib_adam_step_scaled: gib_adam_step gated on *found_inf -- nothing is written when it is non-zero -- with the
+ *        gradients multiplied by (float)(1 / (double)*scale) before grad_scale (GradScaler.unscale_) and the step
+ *        taken as *step_count + 1 (bias corrections in double on the device).  It does not advance *step_count.
+ *      gib_amp_update_scale: torch._amp_update_scale_ on (*scale, *growth_tracker) from *found_inf, and, when
+ *        *found_inf is zero, step_counts[0, n_counts) += 1 (the counts of the optimizer gated on it). */
+int gib_nonfinite_check(const float* x, long long n, float* found_inf, gib_stream stream);
+int gib_adam_step_scaled(float* params, const float* grads, float* exp_avg, float* exp_avg_sq, long long n,
+                         const long long* step_count, const float* found_inf, const float* scale, double lr,
+                         double beta1, double beta2, double eps, double weight_decay, double grad_scale,
+                         gib_stream stream);
+int gib_amp_update_scale(float* scale, int* growth_tracker, const float* found_inf, double growth_factor,
+                         double backoff_factor, int growth_interval, long long* step_counts, int n_counts,
+                         gib_stream stream);
 
 /* ---- single kernels (unit tests, ncu evidence, reuse) --------------------------------- */
 /* Y = act(X W^T + b); X [M, ldx], W packed [Np, Kp] (ldw), Y [M, ldy]; act 0 none / 1 selu / 2 tanh */

@@ -3,9 +3,11 @@
     python tools/bench_autocast.py [--steps 50] [--warmup 10] [--repeats 3] [--gen-batches 3]
 
 Per mode (default, bf16, fp16), alternating, `--repeats` times; each object is built inside the mode's autocast
-context and keeps its mode for its replays.  The training step honours bf16 only, so fp16 has no training rows:
+context and keeps its mode for its replays.  The fp16 training step runs with a `torch.amp.GradScaler` (dynamic loss
+scaling on the device, `TrainStep(grad_scaler=)`); default and bf16 run without one:
   - the C2 and C5T training steps of bench.py (graphed.TrainStep, int8 batches, FlatAdam): ms/step and graphs/s from
-    CUDA events around `--steps` replays after `--warmup`;
+    CUDA events around `--steps` replays after `--warmup`; for fp16 also the time of the loss-scaling launches of one
+    step (the non-finite check, the gated Adam and the scale update) against the plain Adam step of the same bucket;
   - the tensor-core GEMM classes of one profiled step (gib_profile_records, classes 0 forward/dX and 1 weight
     gradients): ms per step and achieved TFLOP/s (algorithmic FLOPs over kernel time);
   - C5 generation (graphed.GraphedGenerator, EMN gdb13 dims, batch 1000): ms per batch over `--gen-batches` batches
@@ -53,8 +55,10 @@ def train_step(cfg, mode):
     net = mpnn.create(C).cuda()
     opt = FlatAdam(net.parameters(), lr=1e-4)
     cap = int(torch.count_nonzero(edges).item()) + 1024
+    scaler = torch.amp.GradScaler("cuda") if mode == "fp16" else None
     with mode_ctx(mode):
-        step = TrainStep(net, opt, batch_size=nodes.shape[0], entry_capacity=cap, input_dtype=torch.int8)
+        step = TrainStep(net, opt, batch_size=nodes.shape[0], entry_capacity=cap, input_dtype=torch.int8,
+                         grad_scaler=scaler)
     assert step.autocast_dtype is DTYPE[mode]
     batch = (nodes.to(torch.int8).cuda(), edges.to(torch.int8).cuda(), target.float().cuda())
     return step, batch, net
@@ -71,6 +75,35 @@ def time_steps(step, batch, steps, warmup):
     e1.record()
     torch.cuda.synchronize()
     return e0.elapsed_time(e1) / steps
+
+
+def scaling_launches(step, reps=20):
+    """ms of (non-finite check + gated Adam + scale update) and of the plain Adam step alone, on the step's bucket
+    (CUDA events around `reps` repetitions of each)"""
+    from graphinvent_b200 import functional as Fn
+    from graphinvent_b200._lib import check, lib
+    flat, found, opt = step.gflat, step.found_inf, step.optimizer
+    saved = [t.clone() for t in (opt._flat, opt._m, opt._v)]
+    def scaled():
+        check(lib.gib_nonfinite_check(Fn._ptr(flat), flat.numel(), Fn._ptr(found), Fn._stream(step.dev)), "check")
+        opt.scaled_step(found, step.grad_scaler)
+    def plain():
+        check(lib.gib_adam_step(Fn._ptr(opt._flat), Fn._ptr(flat), Fn._ptr(opt._m), Fn._ptr(opt._v), flat.numel(), 1,
+                                1e-4, 0.9, 0.999, 1e-8, 0.0, 1.0, Fn._stream(step.dev)), "gib_adam_step")
+    out = []
+    for fn in (scaled, plain):
+        fn()
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        torch.cuda.synchronize()
+        e0.record()
+        for _ in range(reps):
+            fn()
+        e1.record()
+        torch.cuda.synchronize()
+        out.append(round(e0.elapsed_time(e1) / reps, 4))
+    for t, v in zip((opt._flat, opt._m, opt._v), saved):
+        t.copy_(v)
+    return {"check_gated_adam_update_ms": out[0], "plain_adam_ms": out[1], "bucket_floats": flat.numel()}
 
 
 def gemm_classes(step):
@@ -133,13 +166,15 @@ def main():
         for mode in ("default", "bf16", "fp16"):
             row = {"repeat": r, "mode": mode}
             for cfg in ("C2", "C5T"):
-                if mode != "fp16":
-                    step, batch, net = train_step(cfg, mode)
-                    ms = time_steps(step, batch, args.steps, args.warmup)
-                    B = batch[0].shape[0]
-                    row[cfg] = {"ms_per_step": round(ms, 3), "graphs_per_s": round(B / ms * 1e3, 1),
-                                "gemm_classes": gemm_classes(step)}
-                    del step, net
+                step, batch, net = train_step(cfg, mode)
+                ms = time_steps(step, batch, args.steps, args.warmup)
+                B = batch[0].shape[0]
+                row[cfg] = {"ms_per_step": round(ms, 3), "graphs_per_s": round(B / ms * 1e3, 1),
+                            "gemm_classes": gemm_classes(step)}
+                if step.grad_scaler is not None:
+                    row[cfg]["loss_scale"] = step.grad_scaler.get_scale()
+                    row[cfg]["scaling"] = scaling_launches(step)
+                del step, net
                 if cfg == "C2" and r == 0:
                     C, nodes, edges, _, _ = bench.make_batch(cfg, seed=1002)
                     torch.manual_seed(0)
