@@ -91,6 +91,59 @@ KINK = None
 _SELU_SCALE, _SELU_ALPHA = 1.0507009873554804934193349852946, 1.6732632423543772848170429916717
 
 
+# Operand-rounding probe (tests only).  OPERANDS = "tf32" | "bf16" | "fp16": every product the package runs on its GEMM
+# kernels -- each Linear of `mlp`, both Linears of `gru_cell` and the MNN message product -- takes its operands rounded
+# the way the package rounds them, in the backward too (dX = r(G) r(W), dW = r(G)^T r(X), db = sum G unrounded), while
+# the arithmetic stays in the oracle's dtype.  The summation-matrix product and the attention softmax stay unrounded: the
+# package computes them in fp32 kernels.  |o_mode - o64| is then what a correct implementation of that precision loses
+# against exact arithmetic.  None: the plain ops, unchanged.
+OPERANDS = None
+_DTYPE16 = {"bf16": torch.bfloat16, "fp16": torch.float16}
+
+
+def round_operand(x, mode):
+    """x rounded as the package rounds a GEMM operand, returned in x's dtype.  The package's operands are fp32 values,
+    so x goes through fp32 first.  tf32: round to nearest, ties away from zero (cvt.rna); bf16 / fp16: torch's
+    `.to(dtype)` (round to nearest even; fp16 overflows to +-inf)."""
+    x32 = x.float()
+    if mode == "tf32":
+        b = x32.contiguous().view(torch.int32)
+        return ((b + 0x1000) & -0x2000).view(torch.float32).to(x.dtype)
+    return x32.to(_DTYPE16[mode]).to(x.dtype)
+
+
+class _RoundedMatmul(torch.autograd.Function):
+    """r(a) @ r(b); the backward rounds the incoming gradient and reuses the rounded operands"""
+
+    @staticmethod
+    def forward(ctx, a, b, mode):
+        ra, rb = round_operand(a, mode), round_operand(b, mode)
+        ctx.save_for_backward(ra, rb)
+        ctx.mode = mode
+        return ra @ rb
+
+    @staticmethod
+    def backward(ctx, g):
+        ra, rb = ctx.saved_tensors
+        rg = round_operand(g, ctx.mode)
+        return rg @ rb.transpose(-1, -2), ra.transpose(-1, -2) @ rg, None
+
+
+def linear(x, w, b):
+    """F.linear, or under OPERANDS its product on rounded operands (the bias added unrounded)"""
+    if OPERANDS is None:
+        return F.linear(x, w, b)
+    y = _RoundedMatmul.apply(x.reshape(-1, x.shape[-1]), w.t(), OPERANDS)
+    return y.reshape(*x.shape[:-1], w.shape[0]) + b
+
+
+def matmul(a, b):
+    """torch.matmul, or under OPERANDS its product on rounded operands (same batch shape on both sides)"""
+    if OPERANDS is None:
+        return torch.matmul(a, b)
+    return _RoundedMatmul.apply(a, b, OPERANDS)
+
+
 class _SeluKink(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x, tau, side):
@@ -112,7 +165,7 @@ def mlp(sd, prefix, x):
     for every layer INCLUDING the last; Linear layers sit at seq.0, seq.3, ..."""
     i = 0
     while f"{prefix}.seq.{i}.weight" in sd:
-        pre = F.linear(x, sd[f"{prefix}.seq.{i}.weight"], sd[f"{prefix}.seq.{i}.bias"])
+        pre = linear(x, sd[f"{prefix}.seq.{i}.weight"], sd[f"{prefix}.seq.{i}.bias"])
         if MARGINS is not None and pre.numel():
             MARGINS.append(float(pre.detach().abs().min()))
         x = F.selu(pre) if KINK is None else _SeluKink.apply(pre, KINK[0], KINK[1])
@@ -123,8 +176,8 @@ def mlp(sd, prefix, x):
 def gru_cell(sd, x, h):
     """torch.nn.GRUCell as used at gnn/mpnn.py:67,296,391,488 (gate order r,z,n;
     SURVEY Appendix D).  Written out so the gate arithmetic is explicit."""
-    gi = F.linear(x, sd["gru.weight_ih"], sd["gru.bias_ih"])
-    gh = F.linear(h, sd["gru.weight_hh"], sd["gru.bias_hh"])
+    gi = linear(x, sd["gru.weight_ih"], sd["gru.bias_ih"])
+    gh = linear(h, sd["gru.weight_hh"], sd["gru.bias_hh"])
     i_r, i_z, i_n = gi.chunk(3, 1)
     h_r, h_z, h_n = gh.chunk(3, 1)
     r = torch.sigmoid(i_r + h_r)
@@ -211,7 +264,9 @@ def mnn_forward(sd, C, nodes, edges):
 
     def message_terms(nghb_rows, edge_feats):                          # mpnn.py:60-65
         per_edge = (edge_feats.view(-1, 1, 1, C.n_edge_features) * W.unsqueeze(0)).sum(3)
-        return torch.matmul(per_edge, nghb_rows.unsqueeze(-1)).squeeze()
+        # the package's message product (one Linear per bond type on the strided slice W[:, :, t]); with unit bond
+        # values the rounded per_edge is the rounded slice
+        return matmul(per_edge, nghb_rows.unsqueeze(-1)).squeeze()
 
     def readout(hidden, inputs, mask):                                 # mpnn.py:70-74
         return global_readout(sd, hidden, hidden.sum(dim=1))

@@ -120,14 +120,18 @@ def test_nt_shapes_and_epilogues_16bit(dt, M, N):
 @pytest.mark.parametrize("dt", list(DTYPES))
 @pytest.mark.parametrize("case", list(P._group_cases()))
 def test_nt_groups_16bit(dt, case):
+    """a group that does not qualify for one grouped launch (k16 member) runs member by member: each member is checked
+    against the path the dispatch rule gives it, the fp32 SIMT kernel or the 16-bit tensor-core kernel"""
     nts = P._group_cases()[case]()
     rc, cls = _run_nt16(nts, dt)
     assert rc == 0, P._lib().lib.gib_last_error().decode()
-    if P.SIMT_NT in cls:
-        pytest.skip("a member runs on the fp32 SIMT kernel in this group (k16 member)")
-    assert cls and set(cls) == {P.TC_NT}, f"{case}: kernel classes {cls}"
+    assert cls == P._expect_group(nts, 1, 0) and P.TC_NT in cls, f"{case}: kernel classes {cls}"
+    assert (cls == [P.TC_NT]) == (case != "k16 member"), f"{case}: kernel classes {cls}"
     for i, t in enumerate(nts):
-        _check_nt16(t, dt, f"{case} member {i}")
+        if cls == [P.TC_NT] or P._expect_single(t, 1, 0) == [P.TC_NT]:
+            _check_nt16(t, dt, f"{case} member {i}")
+        else:
+            t.check("simt", f"{case} member {i} [simt]")
 
 
 @pytest.mark.parametrize("dt", list(DTYPES))

@@ -136,14 +136,18 @@ def test_nt_shapes_and_epilogues_tf32(M, N):
 
 @pytest.mark.parametrize("case", list(P._group_cases()))
 def test_nt_groups_tf32(case):
+    """a group that does not qualify for one grouped launch (k16 member) runs member by member: each member is checked
+    against the path the dispatch rule gives it, the fp32 SIMT kernel or the TF32 tensor-core kernel"""
     nts = P._group_cases()[case]()
     rc, cls = _run_nt1(nts)
     assert rc == 0, P._lib().lib.gib_last_error().decode()
-    assert cls and set(cls) == {P.TC_NT} or case == "k16 member", f"{case}: kernel classes {cls}"
-    if P.SIMT_NT in cls:
-        pytest.skip("a member runs on the fp32 SIMT kernel in this group (k16 member): covered by the 3xTF32 sweep")
+    assert cls == P._expect_group(nts, 1, 0) and P.TC_NT in cls, f"{case}: kernel classes {cls}"
+    assert (cls == [P.TC_NT]) == (case != "k16 member"), f"{case}: kernel classes {cls}"
     for i, t in enumerate(nts):
-        _check_nt1(t, f"{case} member {i}")
+        if cls == [P.TC_NT] or P._expect_single(t, 1, 0) == [P.TC_NT]:
+            _check_nt1(t, f"{case} member {i}")
+        else:
+            t.check("simt", f"{case} member {i} [simt]")
 
 
 def test_nt_raw_weights_grouped_tf32():
