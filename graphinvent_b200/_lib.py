@@ -60,7 +60,16 @@ class MolLayout(ctypes.Structure):
                                    "len_atom_types", "len_formal_charge", "len_imp_H", "len_chirality")]
 
 
-MOL_HDR_WORDS, MOL_WORDS, MOL_ATOM_WORDS = 8, 6, 3                  # GIB_MOL_* (include/gib200.h)
+class PPDims(ctypes.Structure):
+    """mirror of `gib_pp_dims` (include/gib200.h): dims and action layout of the training-set construction"""
+    _fields_ = [(n, c_i) for n in ("N", "F", "Ef", "n_atom_types", "n_formal_charge", "n_imp_H", "n_chirality",
+                                   "batch_size")]
+
+
+PP_STATUS_INTS = 8                                                  # GIB_PP_* (include/gib200.h)
+PP_BAD_NODES, PP_BAD_EDGES, PP_EMPTY, PP_DISCONNECTED = 1, 2, 4, 8
+
+MOL_HDR_WORDS, MOL_WORDS, MOL_ATOM_WORDS = 8, 6, 3                 # GIB_MOL_* (include/gib200.h)
 MOL_DECODES, MOL_KEY_ERROR, MOL_DUPLICATE_BOND = 1, 2, 4
 MOL_ERR_VALUE, MOL_ERR_OVERFLOW, MOL_ERR_INDEX = 1, 2, 3
 
@@ -138,6 +147,9 @@ _PROTOS = {
     "gib_graph_statistics_bytes": (c_sz, [c_i] * 3),
     "gib_graph_statistics_ws_bytes": (c_sz, [c_i] * 4),
     "gib_graph_statistics": (c_i, [c_i] * 4 + [c_p] * 6),
+    "gib_preprocess_apd_length": (c_i, [c_p]),
+    "gib_preprocess_ws_bytes": (c_sz, [c_p, c_i, c_i]),
+    "gib_preprocess_chunk": (c_i, [c_p, c_p, c_p, c_i, c_i, c_i, c_i] + [c_p] * 7),
     "gib_profile_enable": (None, [c_i]),
     "gib_launch_count": (c_ll, []),
     "gib_profile_collect": (c_i, [c_p, c_p, c_p]),

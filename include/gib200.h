@@ -546,6 +546,40 @@ size_t gib_graph_statistics_ws_bytes(int B, int N, int F, int Ef);
 int gib_graph_statistics(int B, int N, int F, int Ef, const float* nodes, const float* edges, int* table, float* out,
                          void* ws, gib_stream stream);
 
+/* ---- training-set construction: DataProcesser.get_subgraphs (DataProcesser.py:167-271) over the decoding routes of
+ *      PreprocessingGraph (MolecularGraph.py:463-555, 635-732), for one chunk of molecules (graphinvent_b200.preprocess).
+ * Input: `nodes` int8 [n, N, F] and `edges` int8 [n, N, N, Ef], padded one-hot graphs in decoding order: node rows
+ * [0, n_atoms) one-hot per segment with 0 / 1 entries, zero rows after; edges symmetric, 0 / 1, one bond type per
+ * atom pair, no self bond; every route connected.  A chunk holding any other molecule produces no group; status[3]
+ * then holds GIB_PP_* bits and status[4] the first such molecule (a route that disconnects only flags that molecule
+ * when it is reached, see status[3]).
+ * Groups start at molecule 0 of the chunk and follow each other as the reference's do: a group reads at most
+ * batch_size molecules, appends rows by the reference's rule (a state matching no row, or whose first match is the
+ * last row) and ends when it reaches batch_size rows (the rest of that molecule's route is dropped) or runs out of
+ * its molecules.  A group that runs out of the chunk's molecules before either, when last_chunk == 0, is not
+ * written: the caller starts the next chunk at its first molecule (status[1]).  No group starts once fewer than
+ * batch_size rows of max_rows are left.
+ * Output: rows [0, status[2]) of out_nodes [max_rows, N, F] int8, out_edges [max_rows, N, N, Ef] int8 and out_apds
+ * [max_rows, apd] int32 (APD counts, apd = gib_preprocess_apd_length); groups [max_molecules, 4] int32 per group:
+ * first molecule, molecule after the last one it visited, first row, rows.  status int32 [GIB_PP_STATUS_INTS]:
+ * [0] groups, [1] first molecule not yet in a group, [2] rows, [3] GIB_PP_* flags, [4] first bad molecule
+ * (INT_MAX: none), [5] route states of the chunk.  The workspace may hold anything; results are deterministic.
+ * Limits: N*N*Ef <= 32768, N*F <= 8192, n_atom_types and n_formal_charge >= 1, n_imp_H and n_chirality >= 0 (0: the
+ * segment is absent: the four action layouts), F their sum, batch_size >= 1, max_rows >= batch_size,
+ * max_molecules * (N*(N-1)/2 + 2) < 2^30. */
+#define GIB_PP_STATUS_INTS 8
+enum { GIB_PP_BAD_NODES = 1, GIB_PP_BAD_EDGES = 2, GIB_PP_EMPTY = 4, GIB_PP_DISCONNECTED = 8 };
+typedef struct gib_pp_dims {
+  int N, F, Ef;                                             /* max_n_nodes, n_node_features, n_edge_features */
+  int n_atom_types, n_formal_charge, n_imp_H, n_chirality;  /* node-feature segment widths, in order */
+  int batch_size;                                           /* rows per group (constants.batch_size) */
+} gib_pp_dims;
+int gib_preprocess_apd_length(const gib_pp_dims* d);        /* N * (f_add + Ef) + 1, < 0 for unsupported dims */
+size_t gib_preprocess_ws_bytes(const gib_pp_dims* d, int max_molecules, int max_rows);
+int gib_preprocess_chunk(const gib_pp_dims* d, const signed char* nodes, const signed char* edges, int n_molecules,
+                         int last_chunk, int max_molecules, int max_rows, void* ws, signed char* out_nodes,
+                         signed char* out_edges, int* out_apds, int* groups, int* status, gib_stream stream);
+
 /* ---- measurement hooks: CUDA-event timing per kernel class on the launching stream.
  *      class 0 = forward/dX launches of the tensor-core kernel, 1 = its weight-gradient launches, 2 = scatter-aggregate (K2),
  *      3 / 4 = forward/dX and weight-gradient GEMMs on the fp32 SIMT kernels.  GIB_PROFILE_CLASSES entries per array.
