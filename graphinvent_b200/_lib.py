@@ -18,14 +18,13 @@ c_sz = ctypes.c_size_t
 
 
 class Dims(ctypes.Structure):
-    """mirror of `gib_dims` (include/gib200.h).  `tf32` is host-side only: the matmul precision the model entry
-    points run in for these dims (0 = 3xTF32, 1 = single-pass TF32, 2 = bf16, 3 = fp16 operands), applied per call
-    through gib_set_matmul_tf32 (functional.matmul_precision); it is not part of the C struct."""
+    """mirror of `gib_dims` (include/gib200.h).  `tf32`: the matmul precision the model entry points run in for these
+    dims (0 = 3xTF32, 1 = single-pass TF32, 2 = bf16, 3 = fp16 operands)."""
     _fields_ = [(n, c_i) for n in (
         "model", "B", "N", "F", "Ef", "H", "M", "T", "msg_hidden", "msg_depth", "att_hidden", "att_depth",
         "eemb_hidden", "eemb_depth", "gather_width", "gatt_hidden", "gatt_depth", "gemb_hidden", "gemb_depth",
-        "mlp1_hidden", "mlp1_depth", "mlp2_hidden", "mlp2_depth", "f_add", "f_conn")] + [("big", c_f), ("in_dtype", c_i)]
-    tf32 = 0
+        "mlp1_hidden", "mlp1_depth", "mlp2_hidden", "mlp2_depth", "f_add", "f_conn")] + [
+        ("big", c_f), ("in_dtype", c_i), ("tf32", c_i)]
 
 
 class GemmProblem(ctypes.Structure):
@@ -77,15 +76,13 @@ MODEL_ID = {"GGNN": 0, "MNN": 1, "AttGGNN": 2, "EMN": 3}
 HDR_INTS = 16
 HDR_E, HDR_P, HDR_TYPE_COUNT, HDR_TYPE_BASE, HDR_FLAGS, HDR_CAPACITY = 0, 1, 2, 6, 11, 12
 FLAG_MULTITYPE, FLAG_NONBINARY, FLAG_OVERFLOW = 1, 2, 4
-ABI_VERSION = 205     # must equal gib_version() of the loaded library (include/gib200.h)
+ABI_VERSION = 206     # must equal gib_version() of the loaded library (include/gib200.h)
 
 _PROTOS = {
     "gib_last_error": (ctypes.c_char_p, []),
     "gib_version": (c_i, []),
     "gib_set_tensor_cores": (None, [c_i]),
     "gib_get_tensor_cores": (c_i, []),
-    "gib_set_matmul_tf32": (None, [c_i]),
-    "gib_get_matmul_tf32": (c_i, []),
     "gib_tc_debug": (None, [c_i]),
     "gib_device_sm_count": (c_i, []),
     "gib_scatter_variant": (None, [c_i]),

@@ -48,7 +48,7 @@ def autocast_dtype():
     return dt if dt in (torch.bfloat16, torch.float16) else None
 
 
-# precision codes of the tensor-core GEMMs (gib_set_matmul_tf32, `Dims.tf32`)
+# precision codes of the tensor-core GEMMs (`gib_dims.tf32`, `Dims.tf32`)
 PREC_3XTF32, PREC_TF32, PREC_BF16, PREC_FP16 = 0, 1, 2, 3
 
 

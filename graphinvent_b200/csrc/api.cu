@@ -234,13 +234,11 @@ extern "C" {
 
 const char* gib_last_error(void) { return g_err; }
 // 200: capacity mode, int8 inputs, grouped dW; 201: 5 profile classes; 202: test hooks; 203: forward / glue test hooks;
-// 204: gib_generation_round_layout (implicit-H / chirality action layouts); 205: gib_generation_sample_round
-int gib_version(void) { return 205; }
+// 204: gib_generation_round_layout (implicit-H / chirality action layouts); 205: gib_generation_sample_round;
+// 206: the matmul precision is gib_dims.tf32, no longer a thread-local setting
+int gib_version(void) { return 206; }
 void gib_set_tensor_cores(int on) { g_use_tc = on != 0; }
 int gib_get_tensor_cores(void) { return g_use_tc ? 1 : 0; }
-// 0 3xTF32, 1 TF32 (any other nonzero value too), 2 bf16, 3 fp16
-void gib_set_matmul_tf32(int on) { g_matmul_tf32 = (on == 2 || on == 3) ? on : on != 0; }
-int gib_get_matmul_tf32(void) { return g_matmul_tf32; }
 void gib_tc_debug(int mode) { g_tc_debug = mode; }
 int gib_device_sm_count(void) { return device_sm_count(); }
 void gib_scatter_variant(int v) { g_scatter_variant = v; }
@@ -310,7 +308,7 @@ size_t gib_model_packed_bytes(const gib_dims* d) {
 int gib_model_pack(const gib_dims* d, const float* const* params, void* packed, gib_stream stream) {
   Plan pl;
   GIB_TRY(build_plan(*d, pl));
-  return pack_params(pl, params, reinterpret_cast<float*>(packed), g_matmul_tf32, ST(stream));
+  return pack_params(pl, params, reinterpret_cast<float*>(packed), d->tf32, ST(stream));
 }
 
 size_t gib_model_workspace_bytes(const gib_dims* d, const int* hdr) {

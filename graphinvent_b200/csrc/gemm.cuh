@@ -101,8 +101,6 @@ int device_sm_count();     // SMs of the current device (cached per device)
 void tc3_set_trace(long long* buf, int tiles);   // diagnosis: per-tile clock64 stamps of CTA 0
 extern bool g_use_tc;
 extern int g_tc_debug;
-// precision of the model entry points' tensor-core GEMMs on this host thread (gib_set_matmul_tf32; GemmNT::tf32)
-extern thread_local int g_matmul_tf32;
 // 0 when a GEMM of precision `prec` can run as asked (a known code; 16-bit codes need the tensor-core path), else the
 // error code with the message set
 int check_precision(int prec, const char* who);

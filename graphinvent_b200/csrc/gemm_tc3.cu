@@ -1310,7 +1310,6 @@ static bool presplit(const GemmNT& p) {
 
 bool g_use_tc = true;
 int g_tc_debug = 0;
-thread_local int g_matmul_tf32 = 0;
 
 void tc3_set_trace(long long* buf, int tiles) { tc3::g_trace = buf; tc3::g_trace_tiles = tiles; }
 

@@ -242,7 +242,7 @@ static bool msg_mlp_on_tc3(const Run& r) {
 
 int make_run(const gib_dims& d, const int* hdr, Run& r) {
   GIB_TRY(build_plan(d, r.pl));
-  r.tf32 = g_matmul_tf32;
+  r.tf32 = d.tf32;
   r.E = hdr[HDR_E];
   r.P = hdr[HDR_P];
   const int G = d.model == GIB_EMN ? 1 : d.Ef;

@@ -94,7 +94,7 @@ struct Run {
   float* scratch = nullptr;     // backward scratch
   float* const* grads = nullptr;
   cudaStream_t st = nullptr;
-  int tf32 = 0;                 // precision of every tensor-core GEMM of the call (GemmNT::tf32), from gib_set_matmul_tf32
+  int tf32 = 0;                 // precision of every tensor-core GEMM of the call (GemmNT::tf32), from gib_dims.tf32
   // the B operand planes of a tensor-core problem on packed weight `hi` / `lo`: the TF32 (hi, lo) planes, or in the
   // 16-bit modes the 16-bit plane that gib_model_pack writes over the bytes of the lo plane (as B_hi; B_lo unused)
   template <class P>
@@ -105,7 +105,7 @@ struct Run {
 };
 
 int build_plan(const gib_dims& d, Plan& pl);
-// prec: the matmul precision code (gib_set_matmul_tf32) whose planes to write (0 / 1: TF32 hi / lo, 2 / 3: bf16 / fp16)
+// prec: the matmul precision code (gib_dims.tf32) whose planes to write (0 / 1: TF32 hi / lo, 2 / 3: bf16 / fp16)
 int pack_params(const Plan& pl, const float* const* params, float* packed, int prec, cudaStream_t st);
 size_t graph_buf_ints(long long S, int E, int P);
 GraphArrays graph_arrays(void* buf, long long S, int E, int P);

@@ -5,7 +5,6 @@ forward/backward are `gib_model_forward` / `gib_model_backward`, plus the fused 
 PyTorch is used for device memory (caching allocator), streams and autograd plumbing only.
 No computation of the hot path happens in ATen, and there is no CPU path: CPU tensors raise.
 """
-import contextlib
 import ctypes
 
 import numpy as np
@@ -28,19 +27,19 @@ def _stream(device):
 def make_dims(model, batch, in_dtype=0, tf32=None):
     """`in_dtype`: 0 = float32 batches (BlockDatasetLoader layout), 1 = int8 batches (the on-disk HDF5 type, read
     directly by K0 and the first-layer kernels).  `tf32`: precision of the tensor-core GEMMs of the model calls made
-    with these dims (`matmul_precision`), 0 = 3xTF32, 1 (or True) = single-pass TF32, 2 = bf16, 3 = fp16 operands;
+    with these dims (`gib_dims.tf32`), 0 = 3xTF32, 1 (or True) = single-pass TF32, 2 = bf16, 3 = fp16 operands;
     None = torch's current autocast / TF32 state (`config.matmul_code`)."""
     d = Dims()
-    d.tf32 = matmul_code() if tf32 is None else precision_code(tf32)
     kw = model.dims()
     for name, _ in Dims._fields_:
-        if name in ("model", "B", "big", "in_dtype"):
+        if name in ("model", "B", "big", "in_dtype", "tf32"):
             continue
         setattr(d, name, int(kw.get(name, 0)))
     d.model = MODEL_ID[kw["model"]]
     d.B = int(batch)
     d.big = float(kw.get("big", 1e6))
     d.in_dtype = int(in_dtype)
+    d.tf32 = matmul_code() if tf32 is None else precision_code(tf32)
     return d
 
 
@@ -55,26 +54,14 @@ def autocast_dtype_of(d):
 
 
 def dims_key(model, batch, in_dtype=0, tf32=None):
-    """hashable copy of the `gib_dims` a model would be run with, and its matmul precision (two models with equal keys
-    can share K0's output)"""
+    """hashable copy of the `gib_dims` a model would be run with, its matmul precision included (two models with equal
+    keys can share K0's output)"""
     return key_of(make_dims(model, batch, in_dtype, tf32))
 
 
 def key_of(d):
-    """the fields of a `Dims` and its matmul precision, as a tuple"""
-    return tuple(getattr(d, name) for name, _ in Dims._fields_) + (d.tf32,)
-
-
-@contextlib.contextmanager
-def matmul_precision(d):
-    """run the model entry points called inside in the precision of `d` (gib_set_matmul_tf32 is per host thread and
-    read when a call launches its kernels; the previous setting is restored afterwards)"""
-    prev = lib.gib_get_matmul_tf32()
-    lib.gib_set_matmul_tf32(int(d.tf32))
-    try:
-        yield
-    finally:
-        lib.gib_set_matmul_tf32(prev)
+    """the fields of a `Dims`, as a tuple"""
+    return tuple(getattr(d, name) for name, _ in Dims._fields_)
 
 
 def input_dtype_code(nodes, edges):
@@ -135,8 +122,7 @@ def packed_weights(model, d, params):
     dev = params[0].device
     nbytes = lib.gib_model_packed_bytes(ctypes.byref(d))
     packed = torch.empty(nbytes, dtype=_u8, device=dev)
-    with matmul_precision(d):
-        check(lib.gib_model_pack(ctypes.byref(d), _ptr_table(params), _ptr(packed), _stream(dev)), "gib_model_pack")
+    check(lib.gib_model_pack(ctypes.byref(d), _ptr_table(params), _ptr(packed), _stream(dev)), "gib_model_pack")
     model._packed, model._packed_key = packed, key
     return packed
 
@@ -226,9 +212,8 @@ class _MPNNFunction(torch.autograd.Function):
         ws = torch.empty(ws_bytes, dtype=_u8, device=dev)
         apd = d.N * d.f_add + d.N * d.f_conn + 1
         out = torch.empty(B, apd, dtype=torch.float32, device=dev)
-        with matmul_precision(d):
-            check(lib.gib_model_forward(ctypes.byref(d), graph.hdr, _ptr(nodes), _ptr(edges), _ptr(graph.buf),
-                                        _ptr(packed), _ptr(ws), _ptr(out), st), "gib_model_forward")
+        check(lib.gib_model_forward(ctypes.byref(d), graph.hdr, _ptr(nodes), _ptr(edges), _ptr(graph.buf),
+                                    _ptr(packed), _ptr(ws), _ptr(out), st), "gib_model_forward")
         model.last_stats = {"entries": graph.n_entries, "rows": graph.n_rows, "workspace_bytes": ws_bytes,
                             "flags": graph._flags, "capacity": graph.capacity}
         ctx.model, ctx.d, ctx.graph = model, d, graph
@@ -249,10 +234,10 @@ class _MPNNFunction(torch.autograd.Function):
             views.append(flat[o:o + n].view(shape))
             o += n
         scratch = torch.empty(lib.gib_model_bwd_scratch_bytes(ctypes.byref(d), graph.hdr), dtype=_u8, device=dev)
-        with matmul_precision(d):             # the forward's precision, whatever torch's setting is by now
-            check(lib.gib_model_backward(ctypes.byref(d), graph.hdr, _ptr(nodes), _ptr(edges), _ptr(graph.buf),
-                                         _ptr(packed), _ptr(ws), _ptr(out), _ptr(dout), _ptr_table(views),
-                                         _ptr(scratch), _stream(dev)), "gib_model_backward")
+        # ctx.d carries the forward's precision, whatever torch's setting is by now
+        check(lib.gib_model_backward(ctypes.byref(d), graph.hdr, _ptr(nodes), _ptr(edges), _ptr(graph.buf),
+                                     _ptr(packed), _ptr(ws), _ptr(out), _ptr(dout), _ptr_table(views),
+                                     _ptr(scratch), _stream(dev)), "gib_model_backward")
         if model._grad_hook is not None:
             model._grad_hook(flat)      # e.g. the single NCCL all-reduce of data-parallel training
         return (None, None, None, *views)

@@ -227,10 +227,9 @@ class TrainStep:
         check(lib.gib_graph_count(bd, F._ptr(self.edges), F._ptr(self.cws), st), "gib_graph_count")
         check(lib.gib_graph_fill(bd, F._ptr(self.edges), F._ptr(self.cws), self.hdr, F._ptr(self.gbuf), st),
               "gib_graph_fill")
-        with F.matmul_precision(d):
-            check(lib.gib_model_pack(bd, F._ptr_table(self.params), F._ptr(self.packed), st), "gib_model_pack")
-            check(lib.gib_model_forward(bd, self.hdr, F._ptr(self.nodes), F._ptr(self.edges), F._ptr(self.gbuf),
-                                        F._ptr(self.packed), F._ptr(self.ws), F._ptr(self.out), st), "gib_model_forward")
+        check(lib.gib_model_pack(bd, F._ptr_table(self.params), F._ptr(self.packed), st), "gib_model_pack")
+        check(lib.gib_model_forward(bd, self.hdr, F._ptr(self.nodes), F._ptr(self.edges), F._ptr(self.gbuf),
+                                    F._ptr(self.packed), F._ptr(self.ws), F._ptr(self.out), st), "gib_model_forward")
         # Workflow.loss (Workflow.py:833-860) over the live rows, the batch-mean taken over ctl's denominator (the
         # GLOBAL batch of data-parallel shards); padding rows get dout = 0 and add exact zeros to every gradient
         if self.grad_scaler is None:
@@ -260,11 +259,10 @@ class TrainStep:
 
     def _backward(self, part):
         st = F._stream(self.dev)
-        with F.matmul_precision(self.d):
-            check(lib.gib_model_backward_part(ctypes.byref(self.d), self.hdr, F._ptr(self.nodes), F._ptr(self.edges),
-                                              F._ptr(self.gbuf), F._ptr(self.packed), F._ptr(self.ws),
-                                              F._ptr(self.out), F._ptr(self.dout), F._ptr_table(self.views),
-                                              F._ptr(self.scratch), part, st), "gib_model_backward_part")
+        check(lib.gib_model_backward_part(ctypes.byref(self.d), self.hdr, F._ptr(self.nodes), F._ptr(self.edges),
+                                          F._ptr(self.gbuf), F._ptr(self.packed), F._ptr(self.ws),
+                                          F._ptr(self.out), F._ptr(self.dout), F._ptr_table(self.views),
+                                          F._ptr(self.scratch), part, st), "gib_model_backward_part")
 
     def _enqueue_all(self):
         """the whole step's launch sequence, eagerly (warm-up, kernel-class timing)"""
@@ -437,9 +435,8 @@ class EvalStep:
         check(lib.gib_graph_count(bd, F._ptr(self.edges), F._ptr(self.cws), st), "gib_graph_count")
         check(lib.gib_graph_fill(bd, F._ptr(self.edges), F._ptr(self.cws), self.hdr, F._ptr(self.gbuf), st),
               "gib_graph_fill")
-        with F.matmul_precision(self.d):
-            check(lib.gib_model_forward(bd, self.hdr, F._ptr(self.nodes), F._ptr(self.edges), F._ptr(self.gbuf),
-                                        F._ptr(self.packed), F._ptr(self.ws), F._ptr(self.out), st), "gib_model_forward")
+        check(lib.gib_model_forward(bd, self.hdr, F._ptr(self.nodes), F._ptr(self.edges), F._ptr(self.gbuf),
+                                    F._ptr(self.packed), F._ptr(self.ws), F._ptr(self.out), st), "gib_model_forward")
         check(lib.gib_kl_loss_fwd_bwd_ctl(F._ptr(self.out), F._ptr(self.target), self.B, self.apd, F._ptr(self.ctl),
                                           F._ptr(self.rows), None, st), "gib_kl_loss_fwd_bwd_ctl")
         check(lib.gib_validation_nll_ctl(F._ptr(self.out), F._ptr(self.target), self.B, self.apd, F._ptr(self.ctl),
@@ -467,9 +464,8 @@ class EvalStep:
         F._require_cuda(*params)
         F._check_params(self.model, self.d, params)
         st = F._stream(self.dev)
-        with F.matmul_precision(self.d):
-            check(lib.gib_model_pack(ctypes.byref(self.d), F._ptr_table(params), F._ptr(self.packed), st),
-                  "gib_model_pack")
+        check(lib.gib_model_pack(ctypes.byref(self.d), F._ptr_table(params), F._ptr(self.packed), st),
+              "gib_model_pack")
         desc = EvalPass(batch_loss=slots.data_ptr() if slots.numel() else None,
                         lik=lik.data_ptr() if lik is not None and lik.numel() else None,
                         lik_len=lik.numel() if lik is not None else 0, n_slots=slots.numel())
@@ -636,9 +632,8 @@ class GraphedGenerator(GraphGenerator):
             raise RuntimeError("the model's parameter table changed after the GraphedGenerator was built")
         F._require_cuda(*params)
         self.params = params
-        with F.matmul_precision(self.d):     # the arena of a 16-bit mode holds that mode's planes
-            check(lib.gib_model_pack(ctypes.byref(self.d), F._ptr_table(params), F._ptr(self.packed),
-                                     F._stream(self.device)), "gib_model_pack")
+        check(lib.gib_model_pack(ctypes.byref(self.d), F._ptr_table(params), F._ptr(self.packed),
+                                 F._stream(self.device)), "gib_model_pack")
         self._packed_key = key
 
     # ---- the captured round -------------------------------------------------------------------------------
@@ -655,10 +650,9 @@ class GraphedGenerator(GraphGenerator):
         check(lib.gib_graph_fill(bd, F._ptr(edges), F._ptr(self.cws), self.hdr, F._ptr(self.gbuf), st),
               "gib_graph_fill")
         self._flags.bitwise_or_(self._hdr_flags)
-        with F.matmul_precision(d):
-            check(lib.gib_model_forward(bd, self.hdr, F._ptr(self.nodes), F._ptr(edges), F._ptr(self.gbuf),
-                                        F._ptr(self.packed), F._ptr(self.ws), F._ptr(self.logits), st),
-                  "gib_model_forward")
+        check(lib.gib_model_forward(bd, self.hdr, F._ptr(self.nodes), F._ptr(edges), F._ptr(self.gbuf),
+                                    F._ptr(self.packed), F._ptr(self.ws), F._ptr(self.logits), st),
+              "gib_model_forward")
         check(lib.gib_generation_sample_round(
             self.batch_size, self.N, self.F, self.Ef, self.A, self.CH, self.n_imp_H, self.n_chirality,
             F._ptr(self.logits), self.apd, F._ptr(self.uniforms), F._ptr(self._state), F._ptr(self.action),
@@ -873,9 +867,8 @@ class GraphedGeneratorRL(GraphedGenerator):
         if len(params) != len(self.params) or any(p.shape != q.shape for p, q in zip(params, self.params)):
             raise RuntimeError("the model's parameter table changed after the GraphedGeneratorRL was built")
         F._require_cuda(*params)
-        with F.matmul_precision(self.d):
-            check(lib.gib_model_pack(ctypes.byref(self.d), F._ptr_table(params), F._ptr(self.packed[slot]),
-                                     F._stream(self.device)), "gib_model_pack")
+        check(lib.gib_model_pack(ctypes.byref(self.d), F._ptr_table(params), F._ptr(self.packed[slot]),
+                                 F._stream(self.device)), "gib_model_pack")
 
     # ---- the captured rollout round -----------------------------------------------------------------------
     def _k0_forward(self, slots):
@@ -884,11 +877,10 @@ class GraphedGeneratorRL(GraphedGenerator):
         check(lib.gib_graph_count(bd, F._ptr(self.in_edges), F._ptr(self.cws), st), "gib_graph_count")
         check(lib.gib_graph_fill(bd, F._ptr(self.in_edges), F._ptr(self.cws), self.hdr, F._ptr(self.gbuf), st),
               "gib_graph_fill")
-        with F.matmul_precision(self.d):
-            for i, slot in enumerate(slots):
-                check(lib.gib_model_forward(bd, self.hdr, F._ptr(self.in_nodes), F._ptr(self.in_edges),
-                                            F._ptr(self.gbuf), F._ptr(self.packed[slot]), F._ptr(self.ws),
-                                            F._ptr(self.logits[i]), st), "gib_model_forward")
+        for i, slot in enumerate(slots):
+            check(lib.gib_model_forward(bd, self.hdr, F._ptr(self.in_nodes), F._ptr(self.in_edges),
+                                        F._ptr(self.gbuf), F._ptr(self.packed[slot]), F._ptr(self.ws),
+                                        F._ptr(self.logits[i]), st), "gib_model_forward")
 
     def _enqueue_round(self):
         B, N, st = self.batch_size, self.N, F._stream(self.device)
@@ -916,11 +908,10 @@ class GraphedGeneratorRL(GraphedGenerator):
         self._k0_forward((slot,))
         check(lib.gib_rl_dlogits(B, self.apd, F._ptr(self.logits[0]), F._ptr(self.act_rec), F._ptr(b.dp[slot]),
                                  F._ptr(b.ctl), F._ptr(b.dlogits), F._ptr(self.recomputed_p[slot]), st), "gib_rl_dlogits")
-        with F.matmul_precision(self.d):
-            check(lib.gib_model_backward(ctypes.byref(self.d), self.hdr, F._ptr(self.in_nodes), F._ptr(self.in_edges),
-                                         F._ptr(self.gbuf), F._ptr(self.packed[slot]), F._ptr(self.ws),
-                                         F._ptr(self.logits[0]), F._ptr(b.dlogits), F._ptr_table(b.views[slot]),
-                                         F._ptr(b.scratch), st), "gib_model_backward")
+        check(lib.gib_model_backward(ctypes.byref(self.d), self.hdr, F._ptr(self.in_nodes), F._ptr(self.in_edges),
+                                     F._ptr(self.gbuf), F._ptr(self.packed[slot]), F._ptr(self.ws),
+                                     F._ptr(self.logits[0]), F._ptr(b.dlogits), F._ptr_table(b.views[slot]),
+                                     F._ptr(b.scratch), st), "gib_model_backward")
         check(lib.gib_rl_next_round(F._ptr(b.ctl), st), "gib_rl_next_round")
 
     def _ensure_backward(self):

@@ -57,6 +57,19 @@ typedef struct gib_dims {
   int in_dtype;                    /* element type of `nodes` / `edges`: 0 = float32 (BlockDatasetLoader.py:139-143),
                                       1 = int8, the reference's on-disk type (DataProcesser.py:157-161), read
                                       directly by K0 and the first-layer kernels */
+  /* tf32: precision of the tensor-core GEMMs that gib_model_forward, gib_model_backward and gib_model_backward_part
+   * launch: 0 = 3xTF32, fp32-accurate; 1 = single-pass TF32, the hi*hi term of the 3xTF32 split alone (both operands
+   * rounded to TF32 to nearest, fp32 accumulation): the precision torch gives a CUDA fp32 matmul when its fp32_precision
+   * is "tf32".  The fp32 SIMT GEMMs (narrow APD output layers, small exact-mode problems) and every non-GEMM kernel are
+   * fp32 in both modes.  2 = bf16, 3 = fp16 (torch.autocast): every tensor-core GEMM operand (activations, output
+   * gradients, inputs, weights) rounded to nearest-even to 16 bits, as tensor.to(torch.bfloat16 / torch.float16)
+   * rounds, fp32 accumulation; an fp16 operand beyond +-65504 becomes +-inf as torch's cast makes it.  The SIMT GEMMs,
+   * the bias-gradient sums, every other kernel and every buffer stay fp32.  gib_model_pack also reads it: in the 16-bit
+   * modes it writes the 16-bit planes of the weights over the bytes of their TF32 lo planes (the arena size is the
+   * same), so an arena packed in a 16-bit mode serves that mode only.  Other codes are refused, and so is a 16-bit code
+   * when the tensor cores are off (gib_set_tensor_cores) or gib_tc_debug bit 0 is set.  K0 and every size query ignore
+   * it: no size, workspace or packed-weight layout depends on it. */
+  int tf32;
 } gib_dims;
 
 /* Graph header: 16 ints written on the device by gib_graph_count() at the start of its workspace.
@@ -85,22 +98,6 @@ int gib_version(void);
 /* tensor-core 3xTF32 GEMM path on (default) / off (fp32 SIMT GEMMs only); process-wide switch */
 void gib_set_tensor_cores(int on);
 int gib_get_tensor_cores(void);
-/* Precision of the tensor-core GEMMs that the model entry points (gib_model_forward, gib_model_backward,
- * gib_model_backward_part) launch from the calling host thread: 0 = 3xTF32, fp32-accurate (default); 1 = single-pass
- * TF32, the hi*hi term of the 3xTF32 split alone (both operands rounded to TF32 to nearest, fp32 accumulation): the
- * precision torch gives a CUDA fp32 matmul when its fp32_precision is "tf32".  The fp32 SIMT GEMMs (narrow APD output
- * layers, small exact-mode problems) and every non-GEMM kernel are fp32 in both modes.  The setting is read when a
- * call launches its kernels, so a CUDA graph captured around a call keeps the mode it was captured with.  No size
- * query, workspace or packed-weight layout depends on it.  Thread-local; the other entry points ignore it.
- * 2 = bf16, 3 = fp16 (torch.autocast): every tensor-core GEMM operand (activations, output gradients, inputs, weights)
- * rounded to nearest-even to 16 bits, as tensor.to(torch.bfloat16 / torch.float16) rounds, fp32 accumulation; an fp16
- * operand beyond +-65504 becomes +-inf as torch's cast makes it.  The SIMT GEMMs, the bias-gradient sums, every other
- * kernel and every buffer stay fp32.  gib_model_pack also reads the setting: in the 16-bit modes it writes the 16-bit
- * planes of the weights over the bytes of their TF32 lo planes (the arena size is the same), so an arena packed in a
- * 16-bit mode serves that mode only.  A 16-bit call is refused when the tensor cores are off (gib_set_tensor_cores) or
- * gib_tc_debug bit 0 is set.  Other values: nonzero = 1. */
-void gib_set_matmul_tf32(int on);
-int gib_get_matmul_tf32(void);
 /* bit 3: GGNN / MNN message MLPs on one row per bond entry (the AttentionGGNN's layout) instead of one per message row.
  * bit 2: narrow outputs (N < 48, the APD heads) on the tensor-core kernel too (default: fp32 SIMT, see gemm_simt.cu).
  * bit 1: no dependent-chain launches (every MLP layer its own launch).
@@ -268,7 +265,7 @@ int gib_linear_fwd_tc_planes(const float* X, int ldx, const float* W_hi, const f
                              const int* m_dev, const int* base_dev, gib_stream stream);
 /* TF32 hi / lo planes of a row-major matrix (round-to-nearest split), for callers of the entry above */
 int gib_split_planes(const float* W, float* W_hi, float* W_lo, long long n, gib_stream stream);
-/* the 16-bit plane of n fp32 values (kind 2 = bf16, 3 = fp16: the gib_set_matmul_tf32 codes), rounded to nearest-even
+/* the 16-bit plane of n fp32 values (kind 2 = bf16, 3 = fp16: the gib_dims.tf32 codes), rounded to nearest-even
  * as gib_model_pack rounds them, into n 16-bit values at out -- the W_hi of a 16-bit test-hook problem */
 int gib_round_plane16(const float* W, void* out, long long n, int kind, gib_stream stream);
 /* dW[R,C] += G^T X, dbias[R] += colsum(G); G [M, ldg], X [M, ldx]; scratch from gib_dw_scratch_bytes */
@@ -298,7 +295,7 @@ int gib_graph_gather(float* g, float* att, const float* en, const float* em, int
  * act 0 none / 1 selu / 2 tanh.  Columns [n_valid, n_store) are stored as zeros, columns >= n_store are not touched.
  * W_hi / W_lo (may be NULL): its TF32 planes (gib_split_planes).  m_dev / base_dev (may be NULL): the live row range
  * [*base_dev, *base_dev + *m_dev) inside buffers of M rows.  tf32: precision of the tensor-core kernels (0 = 3xTF32,
- * 1 = single-pass TF32, as gib_set_matmul_tf32; W then read from W_hi only, or raw W rounded in the kernel; 2 / 3 =
+ * 1 = single-pass TF32, as gib_dims.tf32; W then read from W_hi only, or raw W rounded in the kernel; 2 / 3 =
  * bf16 / fp16: W_hi then points at the 16-bit plane (gib_round_plane16, ldw in its elements, a multiple of 8 for the
  * tensor-core path) and W_lo is ignored; a 16-bit problem without W_hi is refused); the problems of one call must
  * agree. */

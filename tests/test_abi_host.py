@@ -23,7 +23,7 @@ def test_header_symbols_are_exported_and_bound():
         assert hasattr(raw, name), f"{name} declared in gib200.h but not exported by libgib200.so"
     assert declared == _lib.exported_symbols()
     assert _lib.lib.gib_version() == _lib.ABI_VERSION
-    assert ctypes.sizeof(_lib.Dims) == 27 * 4      # 25 ints + big + in_dtype
+    assert ctypes.sizeof(_lib.Dims) == 28 * 4      # 25 ints + big + in_dtype + tf32
 
 
 def test_test_hook_size_queries():

@@ -1,6 +1,6 @@
 """CPU: the autocast precision rule -- `config.autocast_dtype` / `config.matmul_code` over torch's autocast and TF32
-state, the codes 2 / 3 carried by `make_dims` / `dims_key` and the thread-local switch -- and the C-ABI pieces of the
-16-bit modes that need no GPU.  A real `torch.autocast("cuda")` context turns itself off without a CUDA device, so the
+state, the codes 2 / 3 carried by `make_dims` / `dims_key` in `gib_dims.tf32` -- and the C-ABI pieces of the 16-bit
+modes that need no GPU.  A real `torch.autocast("cuda")` context turns itself off without a CUDA device, so the
 state is set with torch's setters and restored afterwards."""
 import contextlib
 import ctypes
@@ -61,7 +61,7 @@ def test_make_dims_and_keys_carry_the_16bit_codes():
             d, k = Fn.make_dims(net, 64), Fn.dims_key(net, 64)
         assert d.tf32 == code and k[-1] == code and k[:-1] == k0[:-1] and Fn.key_of(d) == k
         assert Fn.autocast_dtype_of(d) is dt
-        assert bytes(d) == bytes(Fn.make_dims(net, 64, tf32=0))    # the mode is not part of the C struct
+        assert bytes(d) != bytes(Fn.make_dims(net, 64, tf32=0))    # the mode is part of the C struct
         got[code] = k
     assert len({k0, got[2], got[3], Fn.dims_key(net, 64, tf32=1)}) == 4
     assert Fn.make_dims(net, 64, tf32=2).tf32 == 2 and Fn.make_dims(net, 64, tf32=3).tf32 == 3
@@ -69,19 +69,23 @@ def test_make_dims_and_keys_carry_the_16bit_codes():
     assert Fn.autocast_dtype_of(Fn.make_dims(net, 64, tf32=1)) is None
 
 
-def test_thread_local_switch_takes_the_16bit_codes():
+def test_model_calls_refuse_16bit_codes_without_tensor_cores():
+    """the 16-bit codes travel with the dims to each call that reads them, which refuses them on the fp32 SIMT path"""
     from graphinvent_b200 import functional as Fn
     from graphinvent_b200._lib import lib
-    for code in (2, 3):
-        with Fn.matmul_precision(Fn.make_dims(_net(), 8, tf32=code)):
-            assert lib.gib_get_matmul_tf32() == code
-        assert lib.gib_get_matmul_tf32() == 0
+    from tests.test_tf32_host import _model_calls
+    d = Fn.make_dims(_net(), 256)
+    prev = lib.gib_get_tensor_cores()
+    lib.gib_set_tensor_cores(0)
     try:
-        for v, want in ((2, 2), (3, 3), (1, 1), (5, 1), (-1, 1), (0, 0)):
-            lib.gib_set_matmul_tf32(v)
-            assert lib.gib_get_matmul_tf32() == want, v
+        for code in (2, 3):
+            d.tf32 = code
+            for name, call in _model_calls(d).items():
+                assert call() == -2, (name, code)
+                err = lib.gib_last_error().decode()
+                assert err.startswith(name) and "tensor-core path" in err, (name, err)
     finally:
-        lib.gib_set_matmul_tf32(0)
+        lib.gib_set_tensor_cores(prev)
 
 
 def test_size_queries_do_not_depend_on_any_mode():
@@ -95,12 +99,9 @@ def test_size_queries_do_not_depend_on_any_mode():
         h = hdr.ctypes.data_as(ctypes.c_void_p)
         sizes = []
         for on in (0, 1, 2, 3):
-            lib.gib_set_matmul_tf32(on)
-            try:
-                sizes.append((lib.gib_model_packed_bytes(ctypes.byref(d)), lib.gib_model_workspace_bytes(ctypes.byref(d), h),
-                              lib.gib_model_bwd_scratch_bytes(ctypes.byref(d), h)))
-            finally:
-                lib.gib_set_matmul_tf32(0)
+            d.tf32 = on
+            sizes.append((lib.gib_model_packed_bytes(ctypes.byref(d)), lib.gib_model_workspace_bytes(ctypes.byref(d), h),
+                          lib.gib_model_bwd_scratch_bytes(ctypes.byref(d), h)))
         assert len(set(sizes)) == 1 and all(s > 0 for s in sizes[0]), (model, sizes)
     qs = (DwProblem * 2)()
     ps = (GemmProblem * 2)()
@@ -118,8 +119,8 @@ def test_size_queries_do_not_depend_on_any_mode():
 def test_abi_layout_unchanged_and_the_plane_helper_is_exported():
     from graphinvent_b200 import _lib
     hdr = open(os.path.join(ROOT, "include", "gib200.h")).read()
-    assert ctypes.sizeof(_lib.Dims) == 27 * 4 and _lib.ABI_VERSION == 205 == _lib.lib.gib_version()
-    for struct in ("gib_gemm_problem", "gib_dw_problem"):
+    assert ctypes.sizeof(_lib.Dims) == 28 * 4 and _lib.ABI_VERSION == 206 == _lib.lib.gib_version()
+    for struct in ("gib_dims", "gib_gemm_problem", "gib_dw_problem"):
         body = re.search(r"typedef struct %s \{(.*?)\} %s;" % (struct, struct), hdr, re.S).group(1)
         assert body.strip().endswith("int tf32;"), struct
     assert "gib_round_plane16" in _lib.exported_symbols()

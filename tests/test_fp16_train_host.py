@@ -29,7 +29,7 @@ def test_new_symbols_are_declared_and_bound():
     for name in NEW:
         assert name in _lib.exported_symbols()
         assert callable(getattr(_lib.lib, name))
-    assert _lib.lib.gib_version() == 205
+    assert _lib.lib.gib_version() == 206
 
 
 def test_argument_refusals():

@@ -60,7 +60,7 @@ def test_bond_entries_stay_within_the_static_capacity(stream, seed, N, Ef, B):
 def test_sample_round_symbol_is_exported_bound_and_versioned():
     from graphinvent_b200 import _lib
     assert "gib_generation_sample_round" in _lib.exported_symbols()
-    assert _lib.ABI_VERSION == 205 == _lib.lib.gib_version()
+    assert _lib.ABI_VERSION == 206 == _lib.lib.gib_version()
     assert _lib.lib.gib_generation_sample_round.restype is not None
 
 

@@ -281,8 +281,7 @@ def test_packed_16bit_planes_are_torch_casts(dt, model):
     params = [(p.detach() * 40.0).contiguous() for p in net.parameters()]   # fp16 overflow of the largest weights
     d = Fn.make_dims(net, 64, tf32=code)
     packed = torch.zeros(lib.gib_model_packed_bytes(ctypes.byref(d)), dtype=torch.uint8, device="cuda")
-    with Fn.matmul_precision(d):
-        assert lib.gib_model_pack(ctypes.byref(d), Fn._ptr_table(params), Fn._ptr(packed), P._st()) == 0
+    assert lib.gib_model_pack(ctypes.byref(d), Fn._ptr_table(params), Fn._ptr(packed), P._st()) == 0
     torch.cuda.synchronize()
     out = (ctypes.c_longlong * len(PLAN_LINEAR_FIELDS))()
     n = lib.gib_test_plan_linear(ctypes.byref(d), 0, out)

@@ -216,9 +216,8 @@ def test_packed_16bit_planes_are_torch_casts(cid, mode):
     params = [(p.detach() * scales[i % 3]).contiguous() for i, p in enumerate(net.parameters())]
     d = Fn.make_dims(net, 64, tf32=code)
     packed = torch.full((lib.gib_model_packed_bytes(ctypes.byref(d)),), 0x7F, dtype=torch.uint8, device="cuda")
-    with Fn.matmul_precision(d):
-        assert lib.gib_model_pack(ctypes.byref(d), Fn._ptr_table(params), Fn._ptr(packed),
-                                  ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)) == 0
+    assert lib.gib_model_pack(ctypes.byref(d), Fn._ptr_table(params), Fn._ptr(packed),
+                              ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)) == 0
     torch.cuda.synchronize()
     out = (ctypes.c_longlong * len(PLAN_LINEAR_FIELDS))()
     n = lib.gib_test_plan_linear(ctypes.byref(d), 0, out)

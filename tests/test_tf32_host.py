@@ -1,9 +1,8 @@
-"""CPU: the matmul-precision switch -- torch's setting read by `config.tf32_enabled`, carried by `make_dims` /
-`dims_key`, applied per call through gib_set_matmul_tf32 -- and the C-ABI pieces that do not need a GPU."""
+"""CPU: the matmul precision -- torch's setting read by `config.tf32_enabled`, carried by `make_dims` / `dims_key` in
+`gib_dims.tf32` to every call -- and the C-ABI pieces that do not need a GPU."""
 import ctypes
 import os
 import re
-import threading
 
 import pytest
 import torch
@@ -64,6 +63,7 @@ def _net():
 
 def test_make_dims_and_dims_key_carry_the_mode():
     from graphinvent_b200 import functional as Fn
+    from graphinvent_b200._lib import Dims
     net = _net()
     torch.backends.cuda.matmul.fp32_precision = "ieee"
     d0, k0 = Fn.make_dims(net, 64), Fn.dims_key(net, 64)
@@ -72,41 +72,48 @@ def test_make_dims_and_dims_key_carry_the_mode():
     assert (d0.tf32, d1.tf32) == (0, 1)
     assert k0 != k1 and k0[:-1] == k1[:-1] and (k0[-1], k1[-1]) == (0, 1)
     assert Fn.make_dims(net, 64, tf32=False).tf32 == 0 and Fn.dims_key(net, 64, tf32=0) == k0
-    assert Fn.key_of(d1) == k1
-    assert bytes(d0) == bytes(d1)                # the mode is not part of the C struct
+    assert Fn.key_of(d1) == k1 == tuple(getattr(d1, name) for name, _ in Dims._fields_)
+    assert bytes(d0) != bytes(d1)                # the mode is part of the C struct
+    d1.tf32 = 0
+    assert bytes(d0) == bytes(d1)
 
 
 def test_abi_struct_layouts_match_the_header():
-    """gib_dims keeps its 27 fields; the test-hook problems end in `int tf32`; the switch is declared and bound"""
+    """gib_dims has 28 fields; it and the test-hook problems end in `int tf32`"""
     from graphinvent_b200 import _lib
     hdr = open(os.path.join(ROOT, "include", "gib200.h")).read()
-    assert ctypes.sizeof(_lib.Dims) == 27 * 4
-    for struct, cls in (("gib_gemm_problem", _lib.GemmProblem), ("gib_dw_problem", _lib.DwProblem)):
+    assert ctypes.sizeof(_lib.Dims) == 28 * 4 and len(_lib.Dims._fields_) == 28
+    for struct, cls in (("gib_dims", _lib.Dims), ("gib_gemm_problem", _lib.GemmProblem),
+                        ("gib_dw_problem", _lib.DwProblem)):
         body = re.search(r"typedef struct %s \{(.*?)\} %s;" % (struct, struct), hdr, re.S).group(1)
         assert body.strip().endswith("int tf32;"), struct
         assert cls._fields_[-1] == ("tf32", ctypes.c_int)
         assert cls.tf32.offset + 4 <= ctypes.sizeof(cls)
     assert _lib.ABI_VERSION == _lib.lib.gib_version()
-    for name in ("gib_set_matmul_tf32", "gib_get_matmul_tf32"):
-        assert name in _lib.exported_symbols() and re.search(r"\b%s\s*\(" % name, hdr)
 
 
-def test_setter_is_thread_local_and_restored():
+def _model_calls(d):
+    """gib_model_pack, gib_model_forward and gib_model_backward on dims `d` with null device pointers (an exact-mode
+    host header): each one that refuses the dims returns before it touches the device"""
+    from graphinvent_b200._lib import lib
+    h = (ctypes.c_int * 16)(1000, 1024, 1000, 0, 0, 0, 0, 1024)      # E, P, one type group of 1000 entries
+    bd = ctypes.byref(d)
+    return {"gib_model_pack": lambda: lib.gib_model_pack(bd, None, None, None),
+            "gib_model_forward": lambda: lib.gib_model_forward(bd, h, *[None] * 7),
+            "gib_model_backward": lambda: lib.gib_model_backward(bd, h, *[None] * 10)}
+
+
+def test_model_calls_refuse_an_unknown_precision():
+    """the precision travels with the dims: an unknown code is refused by each call that reads it"""
     from graphinvent_b200 import functional as Fn
     from graphinvent_b200._lib import lib
-    d = Fn.make_dims(_net(), 8, tf32=1)
-    assert lib.gib_get_matmul_tf32() == 0
-    seen = []
-    with Fn.matmul_precision(d):
-        assert lib.gib_get_matmul_tf32() == 1
-        t = threading.Thread(target=lambda: seen.append(lib.gib_get_matmul_tf32()))
-        t.start()
-        t.join()
-    assert seen == [0] and lib.gib_get_matmul_tf32() == 0
-    with pytest.raises(KeyError):
-        with Fn.matmul_precision(d):
-            raise KeyError
-    assert lib.gib_get_matmul_tf32() == 0
+    d = Fn.make_dims(_net(), 256)
+    for code in (5, -1):
+        d.tf32 = code
+        for name, call in _model_calls(d).items():
+            assert call() == -2, (name, code)
+            err = lib.gib_last_error().decode()
+            assert err.startswith(name) and "precision %d" % code in err, (name, err)
 
 
 def test_size_queries_do_not_depend_on_the_mode():
@@ -123,12 +130,9 @@ def test_size_queries_do_not_depend_on_the_mode():
         h = hdr.ctypes.data_as(ctypes.c_void_p)
         sizes = []
         for on in (0, 1):
-            lib.gib_set_matmul_tf32(on)
-            try:
-                sizes.append((lib.gib_model_packed_bytes(ctypes.byref(d)), lib.gib_model_workspace_bytes(ctypes.byref(d), h),
-                              lib.gib_model_bwd_scratch_bytes(ctypes.byref(d), h)))
-            finally:
-                lib.gib_set_matmul_tf32(0)
+            d.tf32 = on
+            sizes.append((lib.gib_model_packed_bytes(ctypes.byref(d)), lib.gib_model_workspace_bytes(ctypes.byref(d), h),
+                          lib.gib_model_bwd_scratch_bytes(ctypes.byref(d), h)))
         assert sizes[0] == sizes[1] and all(s > 0 for s in sizes[0]), (model, sizes)
     qs = (DwProblem * 2)()
     ps = (GemmProblem * 2)()
