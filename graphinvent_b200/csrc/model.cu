@@ -346,35 +346,71 @@ int make_run(const gib_dims& d, const int* hdr, Run& r) {
 }
 
 // ------------------------------------------------------------------------------------
-// MLP forward / backward over a row range
+// the GEMM problems of one Linear: the only code that reads a Lin's packed-arena offsets
 // ------------------------------------------------------------------------------------
-// rows [row0, row0+rows) of the activation buffers; X0 points at row 0 of the input buffer.
-static int mlp_forward(const Run& r, const Mlp& m, const float* X0, const MlpAct& a, long long row0, int rows,
-                       float* ext_out = nullptr, int ext_ld = 0, int ext_valid = 0) {
-  if (rows <= 0) return 0;
-  const float* x = X0 + (size_t)row0 * a.ld[0];
-  int ldx = a.ld[0];
-  for (int l = 1; l <= m.n; ++l) {
-    const Lin& L = r.pl.lins[m.first + l - 1];
-    GemmNT p;
-    p.A = x; p.lda = ldx;
-    p.B = r.packed + L.ow; p.ldb = L.Cp; r.planes(p, L.ow_hi, L.ow_lo);
-    p.M = rows; p.N = L.Rp; p.K = L.Cp;
-    p.bias = L.pb >= 0 ? r.packed + L.ob : nullptr;
-    p.act = m.act; p.mode = EPI_ACT; p.tf32 = r.tf32;
-    p.work = 2.0 * rows * (double)L.R * L.C;
-    if (l == m.n && ext_out) {
-      p.C = ext_out + (size_t)row0 * ext_ld; p.ldc = ext_ld; p.n_store = ext_valid; p.n_valid = ext_valid;
-    } else {
-      p.C = r.ws + a.y[l] + (size_t)row0 * a.ld[l]; p.ldc = a.ld[l]; p.n_store = L.Rp; p.n_valid = L.Rp;
-    }
-    if (ldx < L.Cp) { set_error("mlp_forward: input ld %d < padded K %d", ldx, L.Cp); return -2; }
-    GIB_TRY(gemm_nt(p, r.st));
-    x = p.C; ldx = p.ldc;
-  }
-  return 0;
+// Each problem covers rows [0, rows) of its operands, or with m_dev set (capacity mode, device-side row counts) the
+// rows [*base_dev, *base_dev + *m_dev) of buffers of `rows` rows.  work counts the real extents: 2 rows R C (Ct for dX).
+
+// B = the packed copy at `w`, plus the planes the tensor-core kernels read: the TF32 (hi, lo) planes, or in the 16-bit
+// modes the 16-bit plane that gib_model_pack writes over the bytes of the lo plane (as B_hi; B_lo unused)
+static void set_b(const Run& r, GemmNT& p, size_t w, size_t hi, size_t lo, int ldb) {
+  p.B = r.packed + w; p.ldb = ldb;
+  p.B_hi = r.packed + (r.tf32 >= 2 ? lo : hi);
+  p.B_lo = r.tf32 >= 2 ? nullptr : r.packed + lo;
 }
 
+// forward: C = act(X W^T + b), X [rows, Cp] at ld ldx, C [rows, Rp] at ld ldc
+static GemmNT lin_fwd(const Run& r, const Lin& L, const float* X, int ldx, int rows, int act, float* C, int ldc,
+                      const int* m_dev = nullptr, const int* base_dev = nullptr) {
+  GemmNT p;
+  p.A = X; p.lda = ldx;
+  set_b(r, p, L.ow, L.ow_hi, L.ow_lo, L.Cp);
+  p.C = C; p.ldc = ldc;
+  p.M = rows; p.N = L.Rp; p.K = L.Cp;
+  p.bias = L.pb >= 0 ? r.packed + L.ob : nullptr;
+  p.act = act; p.mode = EPI_ACT;
+  p.n_store = p.n_valid = L.Rp;
+  p.work = 2.0 * rows * (double)L.R * L.C;
+  p.m_dev = m_dev; p.base_dev = base_dev; p.tf32 = r.tf32;
+  return p;
+}
+
+// input gradient: C = G W over the leading Ct input columns, G [rows, Rp], C [rows, Ctp] at ld ldc, stored as is;
+// callers switch the epilogue to EPI_MUL_DACT (through the previous layer's activation) or EPI_ADD
+static GemmNT lin_dx(const Run& r, const Lin& L, const float* G, int rows, float* C, int ldc,
+                     const int* m_dev = nullptr, const int* base_dev = nullptr) {
+  GemmNT p;
+  p.A = G; p.lda = L.Rp;
+  set_b(r, p, L.owt, L.owt_hi, L.owt_lo, L.Rp);
+  p.C = C; p.ldc = ldc;
+  p.M = rows; p.N = L.Ctp; p.K = L.Rp;
+  p.act = ACT_NONE; p.mode = EPI_ACT;
+  p.n_store = p.n_valid = L.Ctp;
+  p.work = 2.0 * rows * (double)L.R * L.Ct;
+  p.m_dev = m_dev; p.base_dev = base_dev; p.tf32 = r.tf32;
+  return p;
+}
+
+// weight gradient: grads[pw] += G^T X at the Linear's source strides (and grads[pb] += column sums of G), G [rows, Rp],
+// X [rows, Cp] at ld ldx, through the dW scratch of bb
+static GemmDW lin_dw(const Run& r, const BwdBufs& bb, const Lin& L, const float* G, const float* X, int ldx, int rows,
+                     const int* m_dev = nullptr, const int* base_dev = nullptr) {
+  GemmDW q;
+  q.G = G; q.ldg = L.Rp; q.Nn = L.Rp;
+  q.X = X; q.ldx = ldx; q.Kk = L.Cp;
+  q.M = rows;
+  q.dW = r.grads[L.pw] + L.src_off;
+  q.dbias = L.pb >= 0 ? r.grads[L.pb] : nullptr;
+  q.R = L.R; q.C = L.C; q.Rb = L.Rb; q.Rbp = L.Rbp; q.rs = L.rs; q.cs = L.cs;
+  q.scratch = r.scratch + bb.dw; q.half_floats = bb.dw_half;
+  q.work = 2.0 * rows * (double)L.R * L.C;
+  q.m_dev = m_dev; q.base_dev = base_dev; q.tf32 = r.tf32;
+  return q;
+}
+
+// ------------------------------------------------------------------------------------
+// MLP forward / backward over a row range
+// ------------------------------------------------------------------------------------
 // Gtop: gradient w.r.t. the PRE-activation of the last layer, [rows, Rp_last] at Gtop (row 0 = row0).
 // dX0 (optional): [rows, ld_dx] ; dx_aux (optional) is added (may alias dX0).
 static int mlp_backward(const Run& r, const BwdBufs& bb, const Mlp& m, const float* X0, const MlpAct& a,
@@ -387,35 +423,16 @@ static int mlp_backward(const Run& r, const BwdBufs& bb, const Mlp& m, const flo
     const Lin& L = r.pl.lins[m.first + l - 1];
     const float* Xin = (l == 1) ? X0 + (size_t)row0 * a.ld[0] : r.ws + a.y[l - 1] + (size_t)row0 * a.ld[l - 1];
     const int ldxin = a.ld[l - 1];
-    GemmDW q;
-    q.G = G; q.ldg = L.Rp; q.Nn = L.Rp;
-    q.X = Xin; q.ldx = ldxin; q.Kk = L.Cp;
-    q.M = rows;
-    q.dW = r.grads[L.pw] + L.src_off;
-    q.dbias = L.pb >= 0 ? r.grads[L.pb] : nullptr;
-    q.R = L.R; q.C = L.C; q.Rb = L.Rb; q.Rbp = L.Rbp; q.rs = L.rs; q.cs = L.cs;
-    q.scratch = r.scratch + bb.dw; q.half_floats = bb.dw_half;
-    q.work = 2.0 * rows * (double)L.R * L.C;
-    q.tf32 = r.tf32;
-    GIB_TRY(gemm_dw(q, r.st));
-    if (l > 1 || dX0) {
-      GemmNT p;
-      p.A = G; p.lda = L.Rp;
-      p.B = r.packed + L.owt; p.ldb = L.Rp; r.planes(p, L.owt_hi, L.owt_lo);
-      p.M = rows; p.N = L.Ctp; p.K = L.Rp;
-      p.n_store = L.Ctp; p.n_valid = L.Ctp; p.tf32 = r.tf32;
-      p.work = 2.0 * rows * (double)L.R * L.Ct;
-      if (l > 1) {
-        p.C = (G == ping) ? pong : ping; p.ldc = L.Ctp;
-        p.mode = EPI_MUL_DACT; p.act = m.act;
-        p.aux = Xin; p.ldaux = ldxin;
-      } else {
-        p.C = dX0; p.ldc = ld_dx;
-        if (dx_aux) { p.mode = EPI_ADD; p.aux = dx_aux; p.ldaux = ld_dx; }
-        else { p.mode = EPI_ACT; p.act = ACT_NONE; p.bias = nullptr; }
-      }
+    GIB_TRY(gemm_dw(lin_dw(r, bb, L, G, Xin, ldxin, rows), r.st));
+    if (l > 1) {
+      GemmNT p = lin_dx(r, L, G, rows, (G == ping) ? pong : ping, L.Ctp);
+      p.mode = EPI_MUL_DACT; p.act = m.act; p.aux = Xin; p.ldaux = ldxin;
       GIB_TRY(gemm_nt(p, r.st));
       G = p.C;
+    } else if (dX0) {
+      GemmNT p = lin_dx(r, L, G, rows, dX0, ld_dx);
+      if (dx_aux) { p.mode = EPI_ADD; p.aux = dx_aux; p.ldaux = ld_dx; }
+      GIB_TRY(gemm_nt(p, r.st));
     }
   }
   // single-layer MLP: the pending side-stream job reads the caller's Gtop buffer -- finish it before returning
@@ -424,6 +441,7 @@ static int mlp_backward(const Run& r, const BwdBufs& bb, const Mlp& m, const flo
 }
 
 // ---- several MLPs of equal depth advanced layer by layer, each layer as ONE grouped GEMM launch --------------
+// A job covers rows [row0, row0 + rows) of the activation buffers; X0 points at row 0 of the input buffer.
 struct MlpJob {
   const Mlp* m; const float* X0; const MlpAct* a; long long row0; int rows;
   float* ext_out; int ext_ld, ext_valid;
@@ -468,14 +486,8 @@ static int mlp_forward_multi(const Run& r, const MlpJob* jobs, int n, int* flags
   bool same = n <= 4;
   for (int i = 1; i < n && same; ++i) same = jobs[i].m->n == jobs[0].m->n;
   if (!same) {
-    for (int i = 0; i < n; ++i) {
-      if (jobs[i].m_dev) {   // device-side row counts need the grouped call pattern: one call per MLP
-        GIB_TRY(mlp_forward_multi(r, jobs + i, 1, flags));
-        continue;
-      }
-      GIB_TRY(mlp_forward(r, *jobs[i].m, jobs[i].X0, *jobs[i].a, jobs[i].row0, jobs[i].rows, jobs[i].ext_out,
-                          jobs[i].ext_ld, jobs[i].ext_valid));
-    }
+    // one call per MLP: on host rows layer by layer, on device-side row counts (grouped call pattern) still as a chain
+    for (int i = 0; i < n; ++i) GIB_TRY(mlp_forward_multi(r, jobs + i, 1, jobs[i].m_dev ? flags : nullptr));
     return 0;
   }
   const float* x[4]; int ldx[4];
@@ -492,18 +504,13 @@ static int mlp_forward_multi(const Run& r, const MlpJob* jobs, int n, int* flags
       if (j.rows <= 0) continue;
       const Lin& L = r.pl.lins[j.m->first + l - 1];
       GemmNT& p = ps[np];
-      p = GemmNT();
-      p.A = x[i]; p.lda = ldx[i];
-      p.B = r.packed + L.ow; p.ldb = L.Cp; r.planes(p, L.ow_hi, L.ow_lo);
-      p.M = j.rows; p.N = L.Rp; p.K = L.Cp;
-      p.bias = L.pb >= 0 ? r.packed + L.ob : nullptr;
-      p.act = j.m->act; p.mode = EPI_ACT; p.tf32 = r.tf32;
-      p.work = 2.0 * j.rows * (double)L.R * L.C;
-      p.m_dev = j.m_dev; p.base_dev = j.base_dev;
       if (l == j.m->n && j.ext_out) {
-        p.C = j.ext_out + (size_t)j.row0 * j.ext_ld; p.ldc = j.ext_ld; p.n_store = j.ext_valid; p.n_valid = j.ext_valid;
+        p = lin_fwd(r, L, x[i], ldx[i], j.rows, j.m->act, j.ext_out + (size_t)j.row0 * j.ext_ld, j.ext_ld, j.m_dev,
+                    j.base_dev);
+        p.n_store = p.n_valid = j.ext_valid;
       } else {
-        p.C = r.ws + j.a->y[l] + (size_t)j.row0 * j.a->ld[l]; p.ldc = j.a->ld[l]; p.n_store = L.Rp; p.n_valid = L.Rp;
+        p = lin_fwd(r, L, x[i], ldx[i], j.rows, j.m->act, r.ws + j.a->y[l] + (size_t)j.row0 * j.a->ld[l], j.a->ld[l],
+                    j.m_dev, j.base_dev);
       }
       if (ldx[i] < L.Cp) { set_error("mlp_forward_multi: input ld %d < padded K %d", ldx[i], L.Cp); return -2; }
       idx[np++] = i;
@@ -614,14 +621,8 @@ static int mlp_backward_multi(const Run& r, const BwdBufs& bb, const MlpBwdJob* 
       int ldxin;
       const float* Xin = x_in(j, l, &ldxin);
       GemmNT& p = all[nall];
-      p = GemmNT();
-      p.A = G[l][i]; p.lda = L.Rp; p.B = r.packed + L.owt; p.ldb = L.Rp;
-      r.planes(p, L.owt_hi, L.owt_lo);
-      p.M = j.rows; p.N = L.Ctp; p.K = L.Rp; p.n_store = L.Ctp; p.n_valid = L.Ctp;
-      p.work = 2.0 * j.rows * (double)L.R * L.Ct;
-      p.C = const_cast<float*>(G[l - 1][i]); p.ldc = L.Ctp;
+      p = lin_dx(r, L, G[l][i], j.rows, const_cast<float*>(G[l - 1][i]), L.Ctp, j.m_dev, j.base_dev);
       p.mode = EPI_MUL_DACT; p.act = j.m->act; p.aux = Xin; p.ldaux = ldxin;
-      p.m_dev = j.m_dev; p.base_dev = j.base_dev; p.tf32 = r.tf32;
       dep[nall] = last[i];
       layer_of[nall] = l;
       last[i] = nall++;
@@ -647,16 +648,8 @@ static int mlp_backward_multi(const Run& r, const BwdBufs& bb, const MlpBwdJob* 
   for (int i = 0; i < n; ++i) {
     const MlpBwdJob& j = jobs[i];
     if (j.rows <= 0 || !j.dX0) continue;
-    const Lin& L = r.pl.lins[j.m->first];
-    GemmNT p1;
-    p1.A = G[1][i]; p1.lda = L.Rp; p1.B = r.packed + L.owt; p1.ldb = L.Rp;
-    r.planes(p1, L.owt_hi, L.owt_lo);
-    p1.M = j.rows; p1.N = L.Ctp; p1.K = L.Rp; p1.n_store = L.Ctp; p1.n_valid = L.Ctp;
-    p1.work = 2.0 * j.rows * (double)L.R * L.Ct;
-    p1.C = j.dX0; p1.ldc = j.ld_dx;
-    p1.m_dev = j.m_dev; p1.base_dev = j.base_dev; p1.tf32 = r.tf32;
+    GemmNT p1 = lin_dx(r, r.pl.lins[j.m->first], G[1][i], j.rows, j.dX0, j.ld_dx, j.m_dev, j.base_dev);
     if (j.dx_aux) { p1.mode = EPI_ADD; p1.aux = j.dx_aux; p1.ldaux = j.ld_dx; }
-    else { p1.mode = EPI_ACT; p1.act = ACT_NONE; p1.bias = nullptr; }
     GIB_TRY(gemm_nt(p1, r.st));
   }
   // ---- (B) weight gradients of every layer and member: one grouped launch + one reduction -----------------------
@@ -669,15 +662,7 @@ static int mlp_backward_multi(const Run& r, const BwdBufs& bb, const MlpBwdJob* 
       const Lin& L = r.pl.lins[j.m->first + l - 1];
       int ldxin;
       const float* Xin = x_in(j, l, &ldxin);
-      GemmDW& q = qs[nq++];
-      q = GemmDW();
-      q.G = G[l][i]; q.ldg = L.Rp; q.Nn = L.Rp; q.X = Xin; q.ldx = ldxin; q.Kk = L.Cp; q.M = j.rows;
-      q.dW = r.grads[L.pw] + L.src_off;
-      q.dbias = L.pb >= 0 ? r.grads[L.pb] : nullptr;
-      q.R = L.R; q.C = L.C; q.Rb = L.Rb; q.Rbp = L.Rbp; q.rs = L.rs; q.cs = L.cs;
-      q.scratch = r.scratch + bb.dw; q.half_floats = bb.dw_half;
-      q.work = 2.0 * j.rows * (double)L.R * L.C;
-      q.m_dev = j.m_dev; q.base_dev = j.base_dev; q.tf32 = r.tf32;
+      qs[nq++] = lin_dw(r, bb, L, G[l][i], Xin, ldxin, j.rows, j.m_dev, j.base_dev);
     }
   GIB_TRY(gemm_dw_group(qs, nq, plan_rows * depth, r.st));
   // the side-stream reduction reads only its scratch half; a first-generation / SIMT fallback job may still read
@@ -845,18 +830,8 @@ static int node_model_forward(const Run& r, float* out) {
       GIB_TRY(scatter_sum(r.ws + L.msum[t], msgs, Mp, r.ga.dst_ptr, dst_rows, row_w, 0, S, r.st,
                           r.cap ? 0.0 : 4.0 * ((double)r.E * d.M + (double)S * d.M + (double)(S + 1))));   // SURVEY.md 8d bytes
     {   // the two GRU input projections are independent: one grouped launch
-      GemmNT ps[2];
-      GemmNT& p = ps[0];
-      p.A = r.ws + L.msum[t]; p.lda = Mp; p.B = r.packed + ih.ow; p.ldb = ih.Cp; p.C = r.ws + L.gi[t]; p.ldc = ih.Rp;
-      r.planes(p, ih.ow_hi, ih.ow_lo);
-      p.M = (int)S; p.N = ih.Rp; p.K = ih.Cp; p.bias = r.packed + ih.ob; p.act = ACT_NONE; p.mode = EPI_ACT;
-      p.n_store = p.n_valid = ih.Rp; p.work = 2.0 * S * (double)ih.R * ih.C; p.tf32 = r.tf32;
-      GemmNT& q2 = ps[1];
-      q2 = p;
-      q2.A = h; q2.lda = Hp; q2.B = r.packed + hh.ow; q2.ldb = hh.Cp; q2.C = r.ws + L.gh[t]; q2.ldc = hh.Rp;
-      r.planes(q2, hh.ow_hi, hh.ow_lo);
-      q2.N = hh.Rp; q2.K = hh.Cp; q2.bias = r.packed + hh.ob; q2.n_store = q2.n_valid = hh.Rp;
-      q2.work = 2.0 * S * (double)hh.R * hh.C;
+      const GemmNT ps[2] = {lin_fwd(r, ih, r.ws + L.msum[t], Mp, (int)S, ACT_NONE, r.ws + L.gi[t], ih.Rp),
+                            lin_fwd(r, hh, h, Hp, (int)S, ACT_NONE, r.ws + L.gh[t], hh.Rp)};
       GIB_TRY(gemm_nt_group(ps, 2, r.st));
     }
     GIB_TRY(gru_fwd(r.ws + L.h[t + 1], r.ws + L.gi[t], r.ws + L.gh[t], h, Hp, r.ga.dst_ptr, S, nullptr, r.st));
@@ -888,32 +863,13 @@ static int node_model_backward(const Run& r, const BwdBufs& bb, const float* out
     GIB_TRY(gru_bwd(sc + bb.dgi, sc + bb.dgh, dh_dir, dh, r.ws + L.gi[t], r.ws + L.gh[t], h, Hp, r.ga.dst_ptr, S,
                     nullptr, r.st));
     {   // weight gradients of the two GRU projections: one grouped launch
-      GemmDW qs[2];
-      GemmDW& q = qs[0];
-      q.G = sc + bb.dgi; q.ldg = ih.Rp; q.Nn = ih.Rp; q.X = r.ws + L.msum[t]; q.ldx = Mp; q.Kk = ih.Cp; q.M = (int)S;
-      q.dW = r.grads[ih.pw]; q.dbias = r.grads[ih.pb]; q.R = ih.R; q.C = ih.C; q.Rb = ih.Rb; q.Rbp = ih.Rbp;
-      q.rs = ih.rs; q.cs = ih.cs; q.scratch = sc + bb.dw; q.half_floats = bb.dw_half;
-      q.work = 2.0 * S * (double)ih.R * ih.C; q.tf32 = r.tf32;
-      qs[1] = q;
-      GemmDW& q2 = qs[1];
-      q2.G = sc + bb.dgh; q2.ldg = hh.Rp; q2.Nn = hh.Rp; q2.X = h; q2.ldx = Hp; q2.Kk = hh.Cp;
-      q2.dW = r.grads[hh.pw]; q2.dbias = r.grads[hh.pb]; q2.R = hh.R; q2.C = hh.C; q2.Rb = hh.Rb; q2.Rbp = hh.Rbp;
-      q2.rs = hh.rs; q2.cs = hh.cs; q2.work = 2.0 * S * (double)hh.R * hh.C;
+      const GemmDW qs[2] = {lin_dw(r, bb, ih, sc + bb.dgi, r.ws + L.msum[t], Mp, (int)S),
+                            lin_dw(r, bb, hh, sc + bb.dgh, h, Hp, (int)S)};
       GIB_TRY(gemm_dw_group(qs, 2, 0, r.st));
     }
     {   // dMsum = dgi W_ih  and  dh[t] = dgh W_hh + direct  (dh[t+1] is dead after gru_bwd): one grouped launch
-      GemmNT ps[2];
-      GemmNT& p = ps[0];
-      p.A = sc + bb.dgi; p.lda = ih.Rp; p.B = r.packed + ih.owt; p.ldb = ih.Rp; p.C = sc + bb.dmsum; p.ldc = Mp;
-      r.planes(p, ih.owt_hi, ih.owt_lo);
-      p.M = (int)S; p.N = ih.Ctp; p.K = ih.Rp; p.mode = EPI_ACT; p.act = ACT_NONE; p.n_store = p.n_valid = ih.Ctp;
-      p.work = 2.0 * S * (double)ih.R * ih.C; p.tf32 = r.tf32;
-      GemmNT& q2 = ps[1];
-      q2.tf32 = r.tf32;
-      q2.A = sc + bb.dgh; q2.lda = hh.Rp; q2.B = r.packed + hh.owt; q2.ldb = hh.Rp; q2.C = dh; q2.ldc = Hp;
-      r.planes(q2, hh.owt_hi, hh.owt_lo);
-      q2.M = (int)S; q2.N = hh.Ctp; q2.K = hh.Rp; q2.mode = EPI_ADD; q2.aux = dh_dir; q2.ldaux = Hp;
-      q2.n_store = q2.n_valid = hh.Ctp; q2.work = 2.0 * S * (double)hh.R * hh.C;
+      GemmNT ps[2] = {lin_dx(r, ih, sc + bb.dgi, (int)S, sc + bb.dmsum, Mp), lin_dx(r, hh, sc + bb.dgh, (int)S, dh, Hp)};
+      ps[1].mode = EPI_ADD; ps[1].aux = dh_dir; ps[1].ldaux = Hp;
       // h[0] is the zero-padded input (summation_mpnn.py:121-125): nothing consumes d h[0], so at t == 0 the dh GEMM,
       // the first-layer input gradients of the message MLPs and their scatter are skipped
       GIB_TRY(gemm_nt_group(ps, t == 0 ? 1 : 2, r.st));
@@ -1005,13 +961,7 @@ static int emn_forward(const Run& r, float* out) {
     GIB_TRY(emn_aggregate_fwd(r.ws + L.emsg[t], r.ws + L.emx.y[pl.emsg.n], r.ws + L.enx.y[pl.eatt.n],
                               r.ws + L.emm[t].y[pl.emsg.n], r.ws + L.enm[t].y[pl.eatt.n], Hp, r.ga.ent_dst,
                               r.ga.ent_src, r.ga.dst_ptr, E, live, r.st));
-    GemmNT p;
-    p.A = r.ws + L.emsg[t]; p.lda = Hp; p.B = r.packed + ih.ow; p.ldb = ih.Cp; p.C = r.ws + L.gi[t]; p.ldc = ih.Rp;
-    r.planes(p, ih.ow_hi, ih.ow_lo);
-    p.M = E; p.N = ih.Rp; p.K = ih.Cp; p.bias = r.packed + ih.ob; p.act = ACT_NONE; p.mode = EPI_ACT;
-    p.n_store = p.n_valid = ih.Rp;
-    p.m_dev = live; p.base_dev = base; p.tf32 = r.tf32;
-    GIB_TRY(gemm_nt(p, r.st));
+    GIB_TRY(gemm_nt(lin_fwd(r, ih, r.ws + L.emsg[t], Hp, E, ACT_NONE, r.ws + L.gi[t], ih.Rp, live, base), r.st));
     // GRUCell(message) with hx=None (mpnn.py:488): h = 0, so W_hh h + b_hh = b_hh
     GIB_TRY(gru_fwd(r.ws + L.mem[t + 1], r.ws + L.gi[t], r.packed + hh.ob, nullptr, Hp, nullptr, E, live, r.st));
   }
@@ -1053,19 +1003,9 @@ static int emn_backward(const Run& r, const BwdBufs& bb, const float* out, const
   for (int t = d.T - 1; t >= 0; --t) {
     GIB_TRY(gru_bwd(sc + bb.dgi, sc + bb.dgh, nullptr, dmem, r.ws + L.gi[t], r.packed + hh.ob, nullptr, Hp, nullptr,
                     E, live, r.st));
-    GemmDW q;
-    q.G = sc + bb.dgi; q.ldg = ih.Rp; q.Nn = ih.Rp; q.X = r.ws + L.emsg[t]; q.ldx = Hp; q.Kk = ih.Cp; q.M = E;
-    q.dW = r.grads[ih.pw]; q.dbias = r.grads[ih.pb]; q.R = ih.R; q.C = ih.C; q.Rb = ih.Rb; q.Rbp = ih.Rbp;
-    q.rs = ih.rs; q.cs = ih.cs; q.scratch = sc + bb.dw; q.half_floats = bb.dw_half;
-    q.m_dev = live; q.base_dev = base; q.tf32 = r.tf32;
-    GIB_TRY(gemm_dw(q, r.st));
+    GIB_TRY(gemm_dw(lin_dw(r, bb, ih, sc + bb.dgi, r.ws + L.emsg[t], Hp, E, live, base), r.st));
     GIB_TRY(colsum_add(r.grads[hh.pb], sc + bb.dgh, hh.Rp, E, hh.R, hh.Rb, hh.Rbp, live, r.st));  // d b_hh; d W_hh = 0
-    GemmNT p;
-    p.A = sc + bb.dgi; p.lda = ih.Rp; p.B = r.packed + ih.owt; p.ldb = ih.Rp; p.C = sc + bb.dmsum; p.ldc = Hp;
-    r.planes(p, ih.owt_hi, ih.owt_lo);
-    p.M = E; p.N = ih.Ctp; p.K = ih.Rp; p.mode = EPI_ACT; p.act = ACT_NONE; p.n_store = p.n_valid = ih.Ctp;
-    p.m_dev = live; p.base_dev = base; p.tf32 = r.tf32;
-    GIB_TRY(gemm_nt(p, r.st));
+    GIB_TRY(gemm_nt(lin_dx(r, ih, sc + bb.dgi, E, sc + bb.dmsum, Hp, live, base), r.st));
     const float* EMm = r.ws + L.emm[t].y[pl.emsg.n];
     const float* ENm = r.ws + L.enm[t].y[pl.eatt.n];
     GIB_TRY(emn_aggregate_bwd(sc + bb.dEMx, sc + bb.dENx, sc + bb.dEMm, sc + bb.dENm, sc + bb.st3, sc + bb.dmsum,

@@ -95,13 +95,6 @@ struct Run {
   float* const* grads = nullptr;
   cudaStream_t st = nullptr;
   int tf32 = 0;                 // precision of every tensor-core GEMM of the call (GemmNT::tf32), from gib_dims.tf32
-  // the B operand planes of a tensor-core problem on packed weight `hi` / `lo`: the TF32 (hi, lo) planes, or in the
-  // 16-bit modes the 16-bit plane that gib_model_pack writes over the bytes of the lo plane (as B_hi; B_lo unused)
-  template <class P>
-  void planes(P& p, size_t hi, size_t lo) const {
-    if (tf32 >= 2) { p.B_hi = packed + lo; p.B_lo = nullptr; }
-    else { p.B_hi = packed + hi; p.B_lo = packed + lo; }
-  }
 };
 
 int build_plan(const gib_dims& d, Plan& pl);
