@@ -6,6 +6,7 @@ PyTorch is used for device memory (caching allocator), streams and autograd plum
 No computation of the hot path happens in ATen, and there is no CPU path: CPU tensors raise.
 """
 import ctypes
+import math
 
 import numpy as np
 import torch
@@ -101,6 +102,17 @@ def _ptr_table(tensors):
     return arr
 
 
+def _bucket_views(flat, shapes):
+    """views of the flat gradient bucket `flat`, back to back in order, one per parameter or shape"""
+    views, o = [], 0
+    for s in shapes:
+        s = getattr(s, "shape", s)
+        n = math.prod(s)
+        views.append(flat[o:o + n].view(s))
+        o += n
+    return views
+
+
 _weights_epoch = [0]
 
 
@@ -109,12 +121,17 @@ def invalidate_packed_weights():
     _weights_epoch[0] += 1
 
 
+def _weights_key(kind, *tables):
+    """cache key of a packed arena: the invalidation epoch, the arena's kind, and the storage and in-place version of
+    every parameter of the tables"""
+    return (_weights_epoch[0], kind) + tuple((p.data_ptr(), p._version) for ps in tables for p in ps)
+
+
 def packed_weights(model, d, params):
     """Zero-padded / transposed weight arena, rebuilt only when a parameter changed
     (keyed on data_ptr + in-place version counter, so generation re-uses it every round)."""
     # the arena of a 16-bit mode holds that mode's weight planes (gib_model_pack): it serves that mode only
-    kind = d.tf32 if d.tf32 >= 2 else 0
-    key = (_weights_epoch[0], kind) + tuple((p.data_ptr(), p._version) for p in params)
+    key = _weights_key(d.tf32 if d.tf32 >= 2 else 0, params)
     if model._packed is not None and model._packed_key == key:
         return model._packed
     if model._packed_key is None or len(model._packed_key) != len(key):
@@ -193,6 +210,14 @@ class GraphBatch:
         return self.buf[off: off + count * 4].view(dtype)
 
 
+def _workspace(d, hdr, dev):
+    """the forward workspace of a model call with dims d on the graph of host header `hdr`"""
+    nbytes = lib.gib_model_workspace_bytes(ctypes.byref(d), hdr)
+    if nbytes == 0:
+        check(-1, "gib_model_workspace_bytes")
+    return torch.empty(nbytes, dtype=_u8, device=dev)
+
+
 class _MPNNFunction(torch.autograd.Function):
     @staticmethod
     def forward(ctx, model, nodes, edges, *params):
@@ -206,19 +231,16 @@ class _MPNNFunction(torch.autograd.Function):
         elif not graph.matches(d, edges):
             raise ValueError("the shared GraphBatch was built for another batch, model family or edges tensor")
         packed = packed_weights(model, d, params)
-        ws_bytes = lib.gib_model_workspace_bytes(ctypes.byref(d), graph.hdr)
-        if ws_bytes == 0:
-            check(-1, "gib_model_workspace_bytes")
-        ws = torch.empty(ws_bytes, dtype=_u8, device=dev)
+        ws = _workspace(d, graph.hdr, dev)
         apd = d.N * d.f_add + d.N * d.f_conn + 1
         out = torch.empty(B, apd, dtype=torch.float32, device=dev)
         check(lib.gib_model_forward(ctypes.byref(d), graph.hdr, _ptr(nodes), _ptr(edges), _ptr(graph.buf),
                                     _ptr(packed), _ptr(ws), _ptr(out), st), "gib_model_forward")
-        model.last_stats = {"entries": graph.n_entries, "rows": graph.n_rows, "workspace_bytes": ws_bytes,
+        model.last_stats = {"entries": graph.n_entries, "rows": graph.n_rows, "workspace_bytes": ws.numel(),
                             "flags": graph._flags, "capacity": graph.capacity}
         ctx.model, ctx.d, ctx.graph = model, d, graph
         ctx.save_for_backward(nodes, edges, packed, ws, out)
-        ctx.param_meta = [(p.shape, p.numel()) for p in params]
+        ctx.shapes = [p.shape for p in params]
         return out
 
     @staticmethod
@@ -227,12 +249,8 @@ class _MPNNFunction(torch.autograd.Function):
         d, graph, model = ctx.d, ctx.graph, ctx.model
         dev = nodes.device
         dout = dout.contiguous().float()
-        total = sum(n for _, n in ctx.param_meta)
-        flat = torch.zeros(total, dtype=torch.float32, device=dev)   # one bucket: grads are views of it
-        views, o = [], 0
-        for shape, n in ctx.param_meta:
-            views.append(flat[o:o + n].view(shape))
-            o += n
+        flat = torch.zeros(sum(math.prod(s) for s in ctx.shapes), dtype=torch.float32, device=dev)
+        views = _bucket_views(flat, ctx.shapes)        # one bucket: grads are views of it
         scratch = torch.empty(lib.gib_model_bwd_scratch_bytes(ctypes.byref(d), graph.hdr), dtype=_u8, device=dev)
         # ctx.d carries the forward's precision, whatever torch's setting is by now
         check(lib.gib_model_backward(ctypes.byref(d), graph.hdr, _ptr(nodes), _ptr(edges), _ptr(graph.buf),

@@ -49,13 +49,17 @@ class _FusedMPNN(torch.nn.Module):
     def _dropout_ps(self):
         return [m.dropout_p for m in self.modules() if isinstance(m, MLP)]
 
-    def forward(self, nodes: torch.Tensor, edges: torch.Tensor, graph=None) -> torch.Tensor:
-        """`graph`: optional `functional.build_graph(model, edges)` shared between several models of one family
-        evaluated on the same batch (not part of the reference's signature)"""
+    def _check_dropout(self):
+        """refuses training mode with dropout: every fused path (forward, the captured generators) runs without it"""
         if self.training and any(p > 0.0 for p in self._dropout_ps()):
             # AlphaDropout draws from torch's RNG stream inside the reference's ATen graph; the
             # fused path cannot reproduce that stream (all reference defaults use p = 0).
             raise NotImplementedError("dropout_p > 0 in training mode is not supported by the fused sm_90a path")
+
+    def forward(self, nodes: torch.Tensor, edges: torch.Tensor, graph=None) -> torch.Tensor:
+        """`graph`: optional `functional.build_graph(model, edges)` shared between several models of one family
+        evaluated on the same batch (not part of the reference's signature)"""
+        self._check_dropout()
         return _F.mpnn_forward(self, nodes, edges, graph)
 
     def _gather_kwargs(self, node_features, hidden):

@@ -128,6 +128,78 @@ def _grad_scaler(scaler, optimizer):
     return scaler
 
 
+# ---- the static model call of the captured objects ------------------------------------------------------------
+def _static_dims(obj, model, batch, in_dtype, tf32=None):
+    """obj.d for a static call of `model` on its CUDA parameters, checked against the parameter table, and the
+    precision attributes obj.tf32 / obj.autocast_dtype: torch's matmul precision at construction unless `tf32` is
+    given, baked into the object's graphs; returns the parameter table"""
+    params = list(model.parameters())
+    F._require_cuda(*params)
+    obj.d = F.make_dims(model, batch, in_dtype, tf32=tf32)
+    obj.tf32 = obj.d.tf32 == 1
+    obj.autocast_dtype = F.autocast_dtype_of(obj.d)
+    F._check_params(model, obj.d, params)
+    return params
+
+
+def _static_inputs(d, dev):
+    """zeroed static nodes / edges (int8 for int8 batches, float32 otherwise) and target of dims d"""
+    dt = torch.int8 if d.in_dtype else torch.float32
+    return (torch.zeros(d.B, d.N, d.F, dtype=dt, device=dev), torch.zeros(d.B, d.N, d.N, d.Ef, dtype=dt, device=dev),
+            torch.zeros(d.B, d.N * (d.f_add + d.f_conn) + 1, dtype=torch.float32, device=dev))
+
+
+def _model_buffers(d, edges, capacity):
+    """the static buffers of a capacity-mode model call on `edges`, sized by a probe GraphBatch: (cws, gbuf, hdr_np,
+    hdr, ws, workspace_bytes) -- K0's count workspace, graph buffer and host header, and the forward workspace.  The
+    caller allocates the packed arena(s)."""
+    probe = F.GraphBatch(d, edges, capacity=capacity)
+    ws = F._workspace(d, probe.hdr, edges.device)
+    return probe.cws, probe.buf, probe.hdr_np, probe.hdr, ws, ws.numel()
+
+
+def _k0_forward(s, nodes, edges, runs, st, params=None):
+    """K0 on `edges` into s.cws / s.gbuf, then one forward on s.ws per (packed arena, logits) pair of `runs`;
+    `params`: a parameter table packed into the first arena between the two (the training step repacks every step)"""
+    bd = ctypes.byref(s.d)
+    check(lib.gib_graph_count(bd, F._ptr(edges), F._ptr(s.cws), st), "gib_graph_count")
+    check(lib.gib_graph_fill(bd, F._ptr(edges), F._ptr(s.cws), s.hdr, F._ptr(s.gbuf), st), "gib_graph_fill")
+    if params is not None:
+        check(lib.gib_model_pack(bd, F._ptr_table(params), F._ptr(runs[0][0]), st), "gib_model_pack")
+    for packed, out in runs:
+        check(lib.gib_model_forward(bd, s.hdr, F._ptr(nodes), F._ptr(edges), F._ptr(s.gbuf), F._ptr(packed),
+                                    F._ptr(s.ws), F._ptr(out), st), "gib_model_forward")
+
+
+def _capture(dev, enqueues):
+    """one CUDA graph per enqueue function, in order.  All of them run once first, in order, on a side stream and
+    outside capture (lazy per-device init, function attributes)."""
+    side = torch.cuda.Stream(dev)
+    side.wait_stream(torch.cuda.current_stream(dev))
+    with torch.cuda.stream(side):
+        for enqueue in enqueues:
+            enqueue()
+    torch.cuda.current_stream(dev).wait_stream(side)
+    torch.cuda.synchronize(dev)
+    graphs = []
+    for enqueue in enqueues:
+        g = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(g):
+            enqueue()
+        graphs.append(g)
+    return graphs
+
+
+def _check_flags(flags, d, overflow):
+    """raises the error of the K0 `flags` of a model call with dims d (`overflow`: the caller's message for a batch
+    over the entry capacity); returns the flags"""
+    if flags & FLAG_OVERFLOW:
+        raise RuntimeError(overflow)
+    if flags & FLAG_MULTITYPE and d.model == F.MODEL_ID["AttGGNN"]:
+        raise RuntimeError("AttentionGGNN requires one bond type per bond (as the reference's AggregationMPNN does)")
+    return flags
+
+
 class TrainStep:
     @staticmethod
     def precision_code(grad_scaler=None):
@@ -139,43 +211,24 @@ class TrainStep:
 
     def __init__(self, model, optimizer, batch_size, entry_capacity, input_dtype=torch.float32, global_batch=None,
                  group=None, device=None, warmup=True, grad_scaler=None):
-        params = list(model.parameters())
         self.grad_scaler = _grad_scaler(grad_scaler, optimizer)
-        F._require_cuda(*params)
-        self.model, self.optimizer = model, optimizer
-        self.dev = device or params[0].device
         self.B = int(batch_size)
+        self.code = 1 if input_dtype == torch.int8 else 0
+        # fp16 autocast only with a gradient scaler: unscaled fp16 gradients underflow
+        self.params = params = _static_dims(self, model, self.B, self.code, tf32=self.precision_code(self.grad_scaler))
+        self.model, self.optimizer = model, optimizer
+        self.dev = dev = device or params[0].device
         self.global_batch = int(global_batch) if global_batch else self.B
         self.group = group
-        self.code = 1 if input_dtype == torch.int8 else 0
-        C = model.constants
-        N, Fn, Ef = C.max_n_nodes, C.n_node_features, C.n_edge_features
-        self.apd = N * (C.len_f_add_per_node + C.len_f_conn_per_node) + 1
-        in_dt = torch.int8 if self.code else torch.float32
-        dev = self.dev
-        self.nodes = torch.zeros(self.B, N, Fn, dtype=in_dt, device=dev)
-        self.edges = torch.zeros(self.B, N, N, Ef, dtype=in_dt, device=dev)
-        self.target = torch.zeros(self.B, self.apd, dtype=torch.float32, device=dev)
-        # torch's matmul precision at construction, baked into the graphs (fp16 autocast only with a gradient scaler:
-        # unscaled fp16 gradients underflow)
-        self.d = F.make_dims(model, self.B, self.code, tf32=self.precision_code(self.grad_scaler))
-        self.tf32 = self.d.tf32 == 1
-        self.autocast_dtype = F.autocast_dtype_of(self.d)
-        d = self.d
         self.capacity = int(entry_capacity)
         # static buffers (addresses are baked into the graph)
-        self.cws = torch.zeros(lib.gib_graph_count_ws_bytes(ctypes.byref(d)), dtype=_u8, device=dev)
-        probe = F.GraphBatch(d, self.edges, capacity=self.capacity, buffers=None)
-        self.cws, self.gbuf = probe.cws, probe.buf
-        self.hdr_np, self.hdr = probe.hdr_np, probe.hdr
-        F._check_params(model, d, params)
-        self.params = params
-        self.packed = torch.empty(lib.gib_model_packed_bytes(ctypes.byref(d)), dtype=_u8, device=dev)
-        ws_bytes = lib.gib_model_workspace_bytes(ctypes.byref(d), self.hdr)
-        if ws_bytes == 0:
-            check(-1, "gib_model_workspace_bytes")
-        self.ws = torch.empty(ws_bytes, dtype=_u8, device=dev)
-        self.scratch = torch.empty(lib.gib_model_bwd_scratch_bytes(ctypes.byref(d), self.hdr), dtype=_u8, device=dev)
+        self.nodes, self.edges, self.target = _static_inputs(self.d, dev)
+        self.apd = self.target.shape[1]
+        self.cws, self.gbuf, self.hdr_np, self.hdr, self.ws, self.workspace_bytes = _model_buffers(
+            self.d, self.edges, self.capacity)
+        self.packed = torch.empty(lib.gib_model_packed_bytes(ctypes.byref(self.d)), dtype=_u8, device=dev)
+        self.scratch = torch.empty(lib.gib_model_bwd_scratch_bytes(ctypes.byref(self.d), self.hdr), dtype=_u8,
+                                   device=dev)
         self.out = torch.empty(self.B, self.apd, dtype=torch.float32, device=dev)
         self.dout = torch.empty_like(self.out)
         self.rows = torch.empty(self.B, dtype=torch.float32, device=dev)
@@ -185,13 +238,9 @@ class TrainStep:
         _set_ctl(self.ctl, self.B, self.global_batch)
         total = sum(p.numel() for p in params)
         self.gflat = torch.zeros(total, dtype=torch.float32, device=dev)   # ONE bucket: grads are views of it
-        self.views, o = [], 0
-        for p in params:
-            v = self.gflat[o:o + p.numel()].view(p.shape)
-            self.views.append(v)
+        self.views = F._bucket_views(self.gflat, params)
+        for p, v in zip(params, self.views):
             p.grad = v
-            o += p.numel()
-        self.workspace_bytes = ws_bytes
         # dynamic loss scaling: 1.0 when the last step's gradient bucket held an inf or NaN (that step was skipped)
         self.found_inf = torch.zeros((), dtype=torch.float32, device=dev)
         if self.grad_scaler is not None:
@@ -221,15 +270,8 @@ class TrainStep:
 
     # ---- the captured region ------------------------------------------------------------------------------
     def _enqueue(self):
-        d, dev = self.d, self.dev
-        st = F._stream(dev)
-        bd = ctypes.byref(d)
-        check(lib.gib_graph_count(bd, F._ptr(self.edges), F._ptr(self.cws), st), "gib_graph_count")
-        check(lib.gib_graph_fill(bd, F._ptr(self.edges), F._ptr(self.cws), self.hdr, F._ptr(self.gbuf), st),
-              "gib_graph_fill")
-        check(lib.gib_model_pack(bd, F._ptr_table(self.params), F._ptr(self.packed), st), "gib_model_pack")
-        check(lib.gib_model_forward(bd, self.hdr, F._ptr(self.nodes), F._ptr(self.edges), F._ptr(self.gbuf),
-                                    F._ptr(self.packed), F._ptr(self.ws), F._ptr(self.out), st), "gib_model_forward")
+        st = F._stream(self.dev)
+        _k0_forward(self, self.nodes, self.edges, [(self.packed, self.out)], st, params=self.params)
         # Workflow.loss (Workflow.py:833-860) over the live rows, the batch-mean taken over ctl's denominator (the
         # GLOBAL batch of data-parallel shards); padding rows get dout = 0 and add exact zeros to every gradient
         if self.grad_scaler is None:
@@ -271,22 +313,12 @@ class TrainStep:
             self._backward(2)
 
     def capture(self):
-        """(re)capture; called by the constructor and again if the parameters were moved (e.g. by FlatAdam)"""
-        side = torch.cuda.Stream(self.dev)
-        side.wait_stream(torch.cuda.current_stream(self.dev))
-        with torch.cuda.stream(side):            # warm-up outside capture: lazy per-device init, function attributes
-            self._enqueue_all()
-        torch.cuda.current_stream(self.dev).wait_stream(side)
-        torch.cuda.synchronize(self.dev)
-        g = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(g):
-            self._enqueue()
-        self.graph = g
+        """(re)capture; called by the constructor and again if the parameters were moved (e.g. by FlatAdam).  The
+        warm-up runs `_enqueue_all`'s sequence."""
         if self.world > 1:
-            g2 = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(g2):
-                self._backward(2)
-            self.graph2 = g2
+            self.graph, self.graph2 = _capture(self.dev, [self._enqueue, lambda: self._backward(2)])
+        else:
+            self.graph, = _capture(self.dev, [self._enqueue])
         self._param_ptrs = self._captured_ptrs()
 
     def _captured_ptrs(self):
@@ -349,12 +381,8 @@ class TrainStep:
     def check(self):
         """synchronising read of the K0 flags of the LAST step; raises if it did not fit the capacity"""
         flags = int(self.cws[: 64].view(torch.int32).cpu()[HDR_FLAGS])
-        if flags & FLAG_OVERFLOW:
-            raise RuntimeError(f"a batch held more bond entries than entry_capacity={self.capacity}; "
-                               "the results of that step are invalid -- rebuild TrainStep with a larger capacity")
-        if flags & FLAG_MULTITYPE and self.d.model == F.MODEL_ID["AttGGNN"]:
-            raise RuntimeError("AttentionGGNN requires one bond type per bond (as the reference's AggregationMPNN does)")
-        return flags
+        return _check_flags(flags, self.d, f"a batch held more bond entries than entry_capacity={self.capacity}; "
+                            "the results of that step are invalid -- rebuild TrainStep with a larger capacity")
 
 
 # ---- the validation pass --------------------------------------------------------------------------------------
@@ -380,21 +408,15 @@ class EvalStep:
     evaluated as in eval mode, whatever its dropout_p."""
 
     def __init__(self, model, batch_size, entry_capacity, input_dtype=torch.float32, share=None, device=None):
-        params = list(model.parameters())
-        F._require_cuda(*params)
-        self.model = model
-        self.dev = device or params[0].device
         self.B = int(batch_size)
-        self.capacity = int(entry_capacity)
         self.code = 1 if input_dtype == torch.int8 else 0
+        params = _static_dims(self, model, self.B, self.code)
+        self.model = model
+        self.dev = dev = device or params[0].device
+        self.capacity = int(entry_capacity)
         C = model.constants
         self.N = C.max_n_nodes
         self.apd = self.N * (C.len_f_add_per_node + C.len_f_conn_per_node) + 1
-        self.d = F.make_dims(model, self.B, self.code)
-        self.tf32 = self.d.tf32 == 1              # torch's matmul precision at construction, baked into the graph
-        self.autocast_dtype = F.autocast_dtype_of(self.d)
-        F._check_params(model, self.d, params)
-        dev, bd = self.dev, ctypes.byref(self.d)
         if share is not None:
             if (not isinstance(share, TrainStep) or F.key_of(share.d) != F.key_of(self.d)
                     or share.capacity != self.capacity or share.dev != torch.device(dev)):
@@ -405,18 +427,10 @@ class EvalStep:
                          "workspace_bytes"):
                 setattr(self, name, getattr(share, name))
         else:
-            in_dt = torch.int8 if self.code else torch.float32
-            self.nodes = torch.zeros(self.B, self.N, C.n_node_features, dtype=in_dt, device=dev)
-            self.edges = torch.zeros(self.B, self.N, self.N, C.n_edge_features, dtype=in_dt, device=dev)
-            self.target = torch.zeros(self.B, self.apd, dtype=torch.float32, device=dev)
-            probe = F.GraphBatch(self.d, self.edges, capacity=self.capacity)
-            self.cws, self.gbuf, self.hdr_np, self.hdr = probe.cws, probe.buf, probe.hdr_np, probe.hdr
-            self.packed = torch.empty(lib.gib_model_packed_bytes(bd), dtype=_u8, device=dev)
-            ws_bytes = lib.gib_model_workspace_bytes(bd, self.hdr)
-            if ws_bytes == 0:
-                check(-1, "gib_model_workspace_bytes")
-            self.workspace_bytes = ws_bytes
-            self.ws = torch.empty(ws_bytes, dtype=_u8, device=dev)
+            self.nodes, self.edges, self.target = _static_inputs(self.d, dev)
+            self.cws, self.gbuf, self.hdr_np, self.hdr, self.ws, self.workspace_bytes = _model_buffers(
+                self.d, self.edges, self.capacity)
+            self.packed = torch.empty(lib.gib_model_packed_bytes(ctypes.byref(self.d)), dtype=_u8, device=dev)
             self.out = torch.empty(self.B, self.apd, dtype=torch.float32, device=dev)
         self.rows = torch.zeros(self.B, dtype=torch.float32, device=dev)
         self.nll = torch.zeros(self.B, dtype=torch.float32, device=dev)
@@ -431,12 +445,8 @@ class EvalStep:
         self.capture()
 
     def _enqueue(self):
-        bd, st = ctypes.byref(self.d), F._stream(self.dev)
-        check(lib.gib_graph_count(bd, F._ptr(self.edges), F._ptr(self.cws), st), "gib_graph_count")
-        check(lib.gib_graph_fill(bd, F._ptr(self.edges), F._ptr(self.cws), self.hdr, F._ptr(self.gbuf), st),
-              "gib_graph_fill")
-        check(lib.gib_model_forward(bd, self.hdr, F._ptr(self.nodes), F._ptr(self.edges), F._ptr(self.gbuf),
-                                    F._ptr(self.packed), F._ptr(self.ws), F._ptr(self.out), st), "gib_model_forward")
+        st = F._stream(self.dev)
+        _k0_forward(self, self.nodes, self.edges, [(self.packed, self.out)], st)
         check(lib.gib_kl_loss_fwd_bwd_ctl(F._ptr(self.out), F._ptr(self.target), self.B, self.apd, F._ptr(self.ctl),
                                           F._ptr(self.rows), None, st), "gib_kl_loss_fwd_bwd_ctl")
         check(lib.gib_validation_nll_ctl(F._ptr(self.out), F._ptr(self.target), self.B, self.apd, F._ptr(self.ctl),
@@ -445,18 +455,8 @@ class EvalStep:
                                    F._ptr(self.ctl), F._ptr(self.cws), F._ptr(self._pass), st), "gib_eval_collect")
 
     def capture(self):
-        """warm up outside capture (lazy per-device init, function attributes), then capture; the warm-up's pass
-        state is overwritten by the next pass's start"""
-        side = torch.cuda.Stream(self.dev)
-        side.wait_stream(torch.cuda.current_stream(self.dev))
-        with torch.cuda.stream(side):
-            self._enqueue()
-        torch.cuda.current_stream(self.dev).wait_stream(side)
-        torch.cuda.synchronize(self.dev)
-        g = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(g):
-            self._enqueue()
-        self.graph = g
+        """the warm-up's pass state is overwritten by the next pass's start"""
+        self.graph, = _capture(self.dev, [self._enqueue])
 
     # ---- one pass -----------------------------------------------------------------------------------------
     def _begin(self, slots, lik):
@@ -524,12 +524,8 @@ class EvalStep:
     def check(self):
         """raises if a batch of the last pass exceeded the entry capacity (or an AttentionGGNN batch had a bond of
         several types); the read already happened at the end of the pass"""
-        if self.flags & FLAG_OVERFLOW:
-            raise RuntimeError(f"a batch held more bond entries than entry_capacity={self.capacity}; the results of "
-                               "that pass are invalid -- rebuild EvalStep with a larger capacity")
-        if self.flags & FLAG_MULTITYPE and self.d.model == F.MODEL_ID["AttGGNN"]:
-            raise RuntimeError("AttentionGGNN requires one bond type per bond (as the reference's AggregationMPNN does)")
-        return self.flags
+        return _check_flags(self.flags, self.d, f"a batch held more bond entries than entry_capacity={self.capacity}; "
+                            "the results of that pass are invalid -- rebuild EvalStep with a larger capacity")
 
 
 # ---- generation -----------------------------------------------------------------------------------------------
@@ -573,24 +569,13 @@ class GraphedGenerator(GraphGenerator):
         if not hasattr(model, "dims"):
             raise TypeError("GraphedGenerator runs this package's models (graphinvent_b200.gnn.mpnn) only")
         B, N, dev = self.batch_size, self.N, self.device
-        self.params = list(model.parameters())
-        F._require_cuda(*self.params)
-        self.d = F.make_dims(model, B, 0)
-        self.tf32 = self.d.tf32 == 1              # torch's matmul precision at construction, baked into the graph
-        self.autocast_dtype = F.autocast_dtype_of(self.d)
-        bd = ctypes.byref(self.d)
-        F._check_params(model, self.d, self.params)
+        self.params = _static_dims(self, model, B, 0)
         self.entry_capacity = entry_capacity(B, N, self.Ef)
         self._att_view = getattr(model, "MODEL", None) == "AttGGNN"
         self._edges_in = torch.zeros_like(self.edges) if self._att_view else self.edges
-        probe = F.GraphBatch(self.d, self._edges_in, capacity=self.entry_capacity)
-        self.cws, self.gbuf, self.hdr_np, self.hdr = probe.cws, probe.buf, probe.hdr_np, probe.hdr
-        self.packed = torch.empty(lib.gib_model_packed_bytes(bd), dtype=torch.uint8, device=dev)
-        ws_bytes = lib.gib_model_workspace_bytes(bd, self.hdr)
-        if ws_bytes == 0:
-            check(-1, "gib_model_workspace_bytes")
-        self.workspace_bytes = ws_bytes
-        self.ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
+        self.cws, self.gbuf, self.hdr_np, self.hdr, self.ws, self.workspace_bytes = _model_buffers(
+            self.d, self._edges_in, self.entry_capacity)
+        self.packed = torch.empty(lib.gib_model_packed_bytes(ctypes.byref(self.d)), dtype=_u8, device=dev)
         self.logits = torch.empty(B, self.apd, dtype=torch.float32, device=dev)
         self.action = torch.zeros(B, dtype=torch.int32, device=dev)
         self.lik = torch.zeros(B, dtype=torch.float32, device=dev)
@@ -621,38 +606,33 @@ class GraphedGenerator(GraphGenerator):
         self.n_nodes[0].fill_(1)
 
     def _pack(self):
-        model = self.model
-        if model.training and any(p > 0.0 for p in model._dropout_ps()):
-            raise NotImplementedError("dropout_p > 0 in training mode is not supported by the fused sm_90a path")
-        params = list(model.parameters())
-        key = (F._weights_epoch[0], self.d.tf32) + tuple((p.data_ptr(), p._version) for p in params)
+        self.model._check_dropout()
+        params = list(self.model.parameters())
+        key = F._weights_key(self.d.tf32, params)
         if key == self._packed_key:
             return
-        if len(params) != len(self.params) or any(p.shape != q.shape for p, q in zip(params, self.params)):
-            raise RuntimeError("the model's parameter table changed after the GraphedGenerator was built")
-        F._require_cuda(*params)
+        self._pack_arena(self.packed, params)
         self.params = params
-        check(lib.gib_model_pack(ctypes.byref(self.d), F._ptr_table(params), F._ptr(self.packed),
-                                 F._stream(self.device)), "gib_model_pack")
         self._packed_key = key
+
+    def _pack_arena(self, packed, params):
+        """`params` into the arena `packed`; they must have the shapes of the table the generator was built for"""
+        if len(params) != len(self.params) or any(p.shape != q.shape for p, q in zip(params, self.params)):
+            raise RuntimeError(f"the model's parameter table changed after the {type(self).__name__} was built")
+        F._require_cuda(*params)
+        check(lib.gib_model_pack(ctypes.byref(self.d), F._ptr_table(params), F._ptr(packed),
+                                 F._stream(self.device)), "gib_model_pack")
 
     # ---- the captured round -------------------------------------------------------------------------------
     def _enqueue_round(self):
-        d, st = self.d, F._stream(self.device)
-        bd = ctypes.byref(d)
+        st = F._stream(self.device)
         if self._att_view:                          # GraphGenerator._model_inputs, into the static copy
             self._edges_in.copy_(self.edges)
             e0 = self.edges[0]
             nz = e0 != 0
             self._edges_in[0].copy_(e0 * (nz & (nz.to(torch.int32).cumsum(-1) == 1)).to(e0.dtype))
-        edges = self._edges_in
-        check(lib.gib_graph_count(bd, F._ptr(edges), F._ptr(self.cws), st), "gib_graph_count")
-        check(lib.gib_graph_fill(bd, F._ptr(edges), F._ptr(self.cws), self.hdr, F._ptr(self.gbuf), st),
-              "gib_graph_fill")
+        _k0_forward(self, self.nodes, self._edges_in, [(self.packed, self.logits)], st)
         self._flags.bitwise_or_(self._hdr_flags)
-        check(lib.gib_model_forward(bd, self.hdr, F._ptr(self.nodes), F._ptr(edges), F._ptr(self.gbuf),
-                                    F._ptr(self.packed), F._ptr(self.ws), F._ptr(self.logits), st),
-              "gib_model_forward")
         check(lib.gib_generation_sample_round(
             self.batch_size, self.N, self.F, self.Ef, self.A, self.CH, self.n_imp_H, self.n_chirality,
             F._ptr(self.logits), self.apd, F._ptr(self.uniforms), F._ptr(self._state), F._ptr(self.action),
@@ -662,18 +642,7 @@ class GraphedGenerator(GraphGenerator):
             F._ptr(self._counters), F._ptr(self._scratch), st), "gib_generation_sample_round")
 
     def capture(self):
-        """warm up outside capture (lazy per-device init, function attributes), then capture one round"""
-        dev = self.device
-        side = torch.cuda.Stream(dev)
-        side.wait_stream(torch.cuda.current_stream(dev))
-        with torch.cuda.stream(side):
-            self._enqueue_round()
-        torch.cuda.current_stream(dev).wait_stream(side)
-        torch.cuda.synchronize(dev)
-        g = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(g):
-            self._enqueue_round()
-        self.graph = g
+        self.graph, = _capture(self.device, [self._enqueue_round])
 
     # ---- one batch ----------------------------------------------------------------------------------------
     @torch.no_grad()
@@ -707,11 +676,8 @@ class GraphedGenerator(GraphGenerator):
         events[i - 1].synchronize()
         n_generated, _, rounds, status, flags = (int(v) for v in rows[i - 1])
         self.rounds, self.inert_rounds = rounds, i - rounds
-        if flags & FLAG_OVERFLOW:
-            raise RuntimeError(f"a generation round held more than {self.entry_capacity} bond entries: the static "
-                               "entry capacity is wrong, the batch is invalid")
-        if flags & FLAG_MULTITYPE and self._att_view:
-            raise RuntimeError("AttentionGGNN requires one bond type per bond (as the reference's AggregationMPNN does)")
+        _check_flags(flags, self.d, f"a generation round held more than {self.entry_capacity} bond entries: the static "
+                     "entry capacity is wrong, the batch is invalid")
         if status != 0:
             raise RuntimeError("generation needs more than 2*max_n_nodes rounds: the per-slot likelihood buffer "
                                "(GraphGenerator.py:173, 'the 2 is arbitrary') would overflow, as in the reference")
@@ -796,28 +762,18 @@ class GraphedGeneratorRL(GraphedGenerator):
         B, N, dev = self.batch_size, self.N, self.device
         if B + 1 >= 1 << 24:
             raise ValueError("batch_size must stay below 2**24 (slot ids travel as fp32)")
-        self.params = list(model.parameters())
-        F._require_cuda(*self.params)
-        self.d = F.make_dims(model, B, 1)                 # int8 model inputs: the 0/1 state, bit-exact logits
-        self.tf32 = self.d.tf32 == 1    # torch's matmul precision at construction: rollouts and their backward rounds
-        self.autocast_dtype = F.autocast_dtype_of(self.d)
+        # int8 model inputs: the 0/1 state, bit-exact logits; the precision holds for rollouts and backward rounds
+        self.params = _static_dims(self, model, B, 1)
         self._key = F.key_of(self.d)
-        bd = ctypes.byref(self.d)
-        F._check_params(model, self.d, self.params)
         self.entry_capacity = entry_capacity(B, N, self.Ef)
         self._att_view = getattr(model, "MODEL", None) == "AttGGNN"
         i8, f32, i32 = torch.int8, torch.float32, torch.int32
         self.in_nodes = torch.zeros(B, N, self.F, dtype=i8, device=dev)
         self.in_edges = torch.zeros(B, N, N, self.Ef, dtype=i8, device=dev)
-        probe = F.GraphBatch(self.d, self.in_edges, capacity=self.entry_capacity)
-        self.cws, self.gbuf, self.hdr_np, self.hdr = probe.cws, probe.buf, probe.hdr_np, probe.hdr
-        pbytes = lib.gib_model_packed_bytes(bd)
-        self.packed = [torch.empty(pbytes, dtype=torch.uint8, device=dev) for _ in range(2)]   # agent, prior
-        ws_bytes = lib.gib_model_workspace_bytes(bd, self.hdr)
-        if ws_bytes == 0:
-            check(-1, "gib_model_workspace_bytes")
-        self.workspace_bytes = ws_bytes
-        self.ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
+        self.cws, self.gbuf, self.hdr_np, self.hdr, self.ws, self.workspace_bytes = _model_buffers(
+            self.d, self.in_edges, self.entry_capacity)
+        pbytes = lib.gib_model_packed_bytes(ctypes.byref(self.d))
+        self.packed = [torch.empty(pbytes, dtype=_u8, device=dev) for _ in range(2)]   # agent, prior
         self.logits = [torch.empty(B, self.apd, dtype=f32, device=dev) for _ in range(2)]
         self.action = torch.zeros(B, dtype=i32, device=dev)
         self.lik = torch.zeros(B, dtype=f32, device=dev)             # the slot tags b + 1
@@ -851,44 +807,24 @@ class GraphedGeneratorRL(GraphedGenerator):
                                  "generation.GraphGeneratorRL for other pairs")
 
     def _pack(self):
-        models = self._pair
-        for m in models:
-            if m.training and any(p > 0.0 for p in m._dropout_ps()):
-                raise NotImplementedError("dropout_p > 0 in training mode is not supported by the fused sm_90a path")
-        tables = [list(m.parameters()) for m in models]
-        key = (F._weights_epoch[0], self.d.tf32) + tuple((p.data_ptr(), p._version) for ps in tables for p in ps)
+        for m in self._pair:
+            m._check_dropout()
+        tables = [list(m.parameters()) for m in self._pair]
+        key = F._weights_key(self.d.tf32, *tables)
         if key == self._packed_key:
             return
-        for slot, ps in enumerate(tables):
-            self._pack_slot(slot, ps)
+        for packed, ps in zip(self.packed, tables):
+            self._pack_arena(packed, ps)
         self._packed_key = key
 
-    def _pack_slot(self, slot, params):
-        if len(params) != len(self.params) or any(p.shape != q.shape for p, q in zip(params, self.params)):
-            raise RuntimeError("the model's parameter table changed after the GraphedGeneratorRL was built")
-        F._require_cuda(*params)
-        check(lib.gib_model_pack(ctypes.byref(self.d), F._ptr_table(params), F._ptr(self.packed[slot]),
-                                 F._stream(self.device)), "gib_model_pack")
-
     # ---- the captured rollout round -----------------------------------------------------------------------
-    def _k0_forward(self, slots):
-        """K0 on the static int8 input, then the forward of model slot s into logits[i] for the i-th slot given"""
-        bd, st = ctypes.byref(self.d), F._stream(self.device)
-        check(lib.gib_graph_count(bd, F._ptr(self.in_edges), F._ptr(self.cws), st), "gib_graph_count")
-        check(lib.gib_graph_fill(bd, F._ptr(self.in_edges), F._ptr(self.cws), self.hdr, F._ptr(self.gbuf), st),
-              "gib_graph_fill")
-        for i, slot in enumerate(slots):
-            check(lib.gib_model_forward(bd, self.hdr, F._ptr(self.in_nodes), F._ptr(self.in_edges),
-                                        F._ptr(self.gbuf), F._ptr(self.packed[slot]), F._ptr(self.ws),
-                                        F._ptr(self.logits[i]), st), "gib_model_forward")
-
     def _enqueue_round(self):
         B, N, st = self.batch_size, self.N, F._stream(self.device)
         check(lib.gib_rl_snapshot(B, N, self.F, self.Ef, int(self._att_view), F._ptr(self.nodes), F._ptr(self.edges),
                                   F._ptr(self._state), F._ptr(self._counters), F._ptr(self.rec_nodes),
                                   F._ptr(self.rec_edges), F._ptr(self.in_nodes), F._ptr(self.in_edges), st),
               "gib_rl_snapshot")
-        self._k0_forward((0, 1))
+        _k0_forward(self, self.in_nodes, self.in_edges, list(zip(self.packed, self.logits)), st)
         self._flags.bitwise_or_(self._hdr_flags)
         check(lib.gib_rl_sample_round(
             B, N, self.F, self.Ef, self.A, self.CH, self.n_imp_H, self.n_chirality, F._ptr(self.logits[0]),
@@ -905,7 +841,7 @@ class GraphedGeneratorRL(GraphedGenerator):
         b, B, st = self._bwd, self.batch_size, F._stream(self.device)
         check(lib.gib_rl_restore(B, self.N, self.F, self.Ef, F._ptr(self.rec_nodes), F._ptr(self.rec_edges),
                                  F._ptr(b.ctl), F._ptr(self.in_nodes), F._ptr(self.in_edges), st), "gib_rl_restore")
-        self._k0_forward((slot,))
+        _k0_forward(self, self.in_nodes, self.in_edges, [(self.packed[slot], self.logits[0])], st)
         check(lib.gib_rl_dlogits(B, self.apd, F._ptr(self.logits[0]), F._ptr(self.act_rec), F._ptr(b.dp[slot]),
                                  F._ptr(b.ctl), F._ptr(b.dlogits), F._ptr(self.recomputed_p[slot]), st), "gib_rl_dlogits")
         check(lib.gib_model_backward(ctypes.byref(self.d), self.hdr, F._ptr(self.in_nodes), F._ptr(self.in_edges),
@@ -919,36 +855,17 @@ class GraphedGeneratorRL(GraphedGenerator):
         if self._bwd is not None:
             return
         B, N, dev = self.batch_size, self.N, self.device
-        bd = ctypes.byref(self.d)
         total = sum(p.numel() for p in self.params)
         b = types.SimpleNamespace()
-        b.scratch = torch.empty(lib.gib_model_bwd_scratch_bytes(bd, self.hdr), dtype=torch.uint8, device=dev)
+        b.scratch = torch.empty(lib.gib_model_bwd_scratch_bytes(ctypes.byref(self.d), self.hdr), dtype=_u8, device=dev)
         b.dlogits = torch.empty(B, self.apd, dtype=torch.float32, device=dev)
         b.dp = torch.zeros(2, 2 * N, B, dtype=torch.float32, device=dev)
         b.gflat = torch.zeros(2, total, dtype=torch.float32, device=dev)
-        b.views = []
-        for slot in range(2):
-            views, o = [], 0
-            for p in self.params:
-                views.append(b.gflat[slot, o:o + p.numel()])
-                o += p.numel()
-            b.views.append(views)
+        b.views = [F._bucket_views(b.gflat[slot], self.params) for slot in range(2)]
         b.ctl = torch.zeros(1, dtype=torch.int32, device=dev)
         self.recomputed_p = torch.zeros(2, 2 * N, B, dtype=torch.float32, device=dev)
         self._bwd = b
-        side = torch.cuda.Stream(dev)
-        side.wait_stream(torch.cuda.current_stream(dev))
-        with torch.cuda.stream(side):              # warm-up outside capture (lazy per-device init, function attributes)
-            for slot in range(2):
-                self._enqueue_backward_round(slot)
-        torch.cuda.current_stream(dev).wait_stream(side)
-        torch.cuda.synchronize(dev)
-        b.graphs = []
-        for slot in range(2):
-            g = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(g):
-                self._enqueue_backward_round(slot)
-            b.graphs.append(g)
+        b.graphs = _capture(dev, [lambda: self._enqueue_backward_round(0), lambda: self._enqueue_backward_round(1)])
 
     def _gather(self, rec):
         """both [2B, 2N] generated-likelihood tables of a rollout record"""
@@ -976,18 +893,14 @@ class GraphedGeneratorRL(GraphedGenerator):
             if params is None:
                 out.append(None)
                 continue
-            self._pack_slot(slot, params)               # the arenas may hold another rollout's models by now
+            self._pack_arena(self.packed[slot], params)     # the arenas may hold another rollout's models by now
             b.gflat[slot].zero_()
             b.ctl.zero_()
             for _ in range(R):
                 b.graphs[slot].replay()
             self.backward_rounds[slot] = R
-            flat = b.gflat[slot].clone()                # a fresh bucket: autograd may keep it as .grad
-            views, o = [], 0
-            for p in params:
-                views.append(flat[o:o + p.numel()].view(p.shape))
-                o += p.numel()
-            out.append(views)
+            # a fresh bucket: autograd may keep it as .grad
+            out.append(F._bucket_views(b.gflat[slot].clone(), params))
         self._packed_key = None
         return out
 
