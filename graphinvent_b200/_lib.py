@@ -123,6 +123,7 @@ _PROTOS = {
     "gib_sum_scaled_ctl": (c_i, [c_p, c_i, c_p, c_p, c_p]),
     "gib_validation_nll_ctl": (c_i, [c_p, c_p, c_i, c_i, c_p, c_p, c_p]),
     "gib_eval_collect": (c_i, [c_p, c_p, c_p, c_i, c_i, c_p, c_p, c_p, c_p]),
+    "gib_gather_rows": (c_i, [c_p, c_p, c_p, c_p, c_i, c_i, c_i, c_i, c_i, c_p, c_p, c_i, c_p, c_p, c_p]),
     "gib_adam_step": (c_i, [c_p, c_p, c_p, c_p, c_ll, c_ll, c_d, c_d, c_d, c_d, c_d, c_d, c_p]),
     "gib_nonfinite_check": (c_i, [c_p, c_ll, c_p, c_p]),
     "gib_adam_step_scaled": (c_i, [c_p, c_p, c_p, c_p, c_ll, c_p, c_p, c_p, c_d, c_d, c_d, c_d, c_d, c_d, c_p]),

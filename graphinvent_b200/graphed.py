@@ -8,6 +8,10 @@ CUDA-graph capturable").
         ...
     step.check()                                     # raises if a batch exceeded the capacity (one 64-byte read)
 
+or, over a `loader.DeviceBlockLoader`, a whole epoch with one gather launch per batch and no host copies:
+
+    loss = step.train_epoch(loader, scheduler)       # Workflow.train_epoch's return value
+
 replaces the body of `Workflow.train_epoch` (Workflow.py:781-796: batch -> device, `model(nodes, edges)`, `loss`,
 `zero_grad`, `backward`, `optimizer.step`) by: three copies into static input buffers, one graph launch
 (K0 -> weight packing -> forward -> fused KL loss -> explicit backward into ONE flat gradient bucket), the
@@ -200,6 +204,20 @@ def _check_flags(flags, d, overflow):
     return flags
 
 
+def _device_loader(obj, loader, name):
+    """True for a DeviceBlockLoader whose batches fit `obj`'s static inputs; raises for one that does not"""
+    from .loader import DeviceBlockLoader
+    if not isinstance(loader, DeviceBlockLoader):
+        return False
+    d = obj.d
+    if (loader.batch_size != obj.B or (loader.N, loader.F, loader.Ef, loader.apd) != (d.N, d.F, d.Ef, obj.apd)
+            or loader.device != torch.device(obj.dev)):
+        raise ValueError(f"{name} needs a DeviceBlockLoader of the step's batch size {obj.B}, dims (N, F, Ef, apd) = "
+                         f"{(d.N, d.F, d.Ef, obj.apd)} and device {obj.dev}; got batch size {loader.batch_size}, dims "
+                         f"{(loader.N, loader.F, loader.Ef, loader.apd)} on {loader.device}")
+    return True
+
+
 class TrainStep:
     @staticmethod
     def precision_code(grad_scaler=None):
@@ -378,6 +396,37 @@ class TrainStep:
         self.steps += 1
         return self.loss
 
+    def train_epoch(self, loader, scheduler=None):
+        """Workflow.train_epoch (Workflow.py:774-798) over a `loader.DeviceBlockLoader`: per batch one gather launch
+        into the static inputs (and `ctl`), the replay and the optimizer step as `__call__` runs them, then
+        `scheduler.step()` if a scheduler is given, and the batch loss into slot idx of len(loader) zero-initialised
+        device slots.  Returns their mean as a 0-d device tensor.  The K0 flags of every batch are OR-ed on the device
+        and read once, at the end: a batch over the entry capacity (or a multi-type AttentionGGNN batch) anywhere in
+        the epoch raises then, with check()'s message."""
+        if not _device_loader(self, loader, "TrainStep.train_epoch"):
+            raise TypeError(f"TrainStep.train_epoch takes a graphinvent_b200.loader.DeviceBlockLoader, got "
+                            f"{type(loader).__name__}; feed other loaders batch by batch through step(nodes, edges, "
+                            "target)")
+        if self.world > 1 or self.global_batch != self.B:
+            raise ValueError("TrainStep.train_epoch runs one process's whole batches: build the step without a "
+                             "data-parallel group or global_batch")
+        slots = torch.zeros(len(loader), dtype=torch.float32, device=self.dev)
+        flags = torch.zeros(1, dtype=torch.int32, device=self.dev)
+        hdr_flags = self.cws[: HDR_INTS * 4].view(torch.int32)[HDR_FLAGS:HDR_FLAGS + 1]
+        for idx, item in enumerate(loader.batches()):
+            if idx >= slots.numel():
+                raise IndexError(f"the loader yielded more than len(loader) = {slots.numel()} batches")
+            loader.gather(item, self.nodes, self.edges, self.target, self.ctl)
+            loss = self()
+            flags.bitwise_or_(hdr_flags)
+            slots[idx:idx + 1].copy_(loss.view(1))
+            if scheduler is not None:
+                scheduler.step()
+        _check_flags(int(flags.item()), self.d, f"a batch of the epoch held more bond entries than entry_capacity="
+                     f"{self.capacity}; the results of that step are invalid -- rebuild TrainStep with a larger "
+                     "capacity")
+        return torch.mean(slots)
+
     def check(self):
         """synchronising read of the K0 flags of the LAST step; raises if it did not fit the capacity"""
         flags = int(self.cws[: 64].view(torch.int32).cpu()[HDR_FLAGS])
@@ -474,12 +523,22 @@ class EvalStep:
         self._pass.copy_(self._pass_host, non_blocking=True)
         self._pass_copied.record(torch.cuda.current_stream(self.dev))
 
-    def _replay(self, batch):
-        nodes, edges, target = batch
-        b = _batch_rows(self, "EvalStep", nodes, edges, target)
-        _load_rows(self, b, nodes, edges, target)
-        _set_ctl(self.ctl, b, b)
+    def _replay(self, batch, loader=None):
+        """one batch: a host or device (nodes, edges, target), or with `loader` a DeviceBlockLoader batch item"""
+        if loader is not None:
+            loader.gather(batch, self.nodes, self.edges, self.target, self.ctl)
+        else:
+            nodes, edges, target = batch
+            b = _batch_rows(self, "EvalStep", nodes, edges, target)
+            _load_rows(self, b, nodes, edges, target)
+            _set_ctl(self.ctl, b, b)
         self.graph.replay()
+
+    def _batches(self, loader, name):
+        """(batches, the loader for _replay): a DeviceBlockLoader's batch items, or any other loader's batches"""
+        if _device_loader(self, loader, name):
+            return loader.batches(), loader
+        return loader, None
 
     def _end(self):
         """the pass's one synchronising read: batch count, K0 flags OR-ed over its batches, clipped likelihood rows"""
@@ -492,11 +551,12 @@ class EvalStep:
         """Workflow.validation_epoch (Workflow.py:813-831): the KLDivLoss(batchmean) of every batch into one of
         len(loader) zero-initialised slots, their mean as a 0-d device tensor (NaN if a target row is all zero)"""
         slots = torch.zeros(len(loader), dtype=torch.float32, device=self.dev)
+        batches, dev_loader = self._batches(loader, "EvalStep.validation_epoch")
         self._begin(slots, None)
-        for idx, batch in enumerate(loader):
+        for idx, batch in enumerate(batches):
             if idx >= slots.numel():
                 raise IndexError(f"the loader yielded more than len(loader) = {slots.numel()} batches")
-            self._replay(batch)
+            self._replay(batch, dev_loader)
         self._end()
         return torch.mean(slots)
 
@@ -507,11 +567,12 @@ class EvalStep:
         idx * batch_size into n * (max_n_nodes + 5) zeros; returns (likelihoods, sum(likelihoods) / n_structures)"""
         n = min(100000, int(n_samples))
         lik = torch.zeros(n * (self.N + 5), dtype=torch.float32, device=self.dev)
+        batches, dev_loader = self._batches(loader, "EvalStep.validation_likelihood")
         self._begin(lik[:0], lik)
-        for idx, batch in enumerate(loader):
+        for idx, batch in enumerate(batches):
             if idx * self.B > n:
                 break
-            self._replay(batch)
+            self._replay(batch, dev_loader)
         desc = self._end()
         if desc.clipped:
             raise RuntimeError(f"{desc.clipped} likelihood rows fall past the end of the {lik.numel()}-element buffer "

@@ -222,6 +222,19 @@ typedef struct gib_eval_pass {
 int gib_eval_collect(const float* kl_rows, const float* nll_rows, const float* target, int B, int apd,
                      const gib_batch_ctl* ctl, const void* count_ws, gib_eval_pass* pass, gib_stream stream);
 
+/* ---- one batch from a device-resident block of int8 rows (graphinvent_b200/loader.py, DeviceBlockLoader; replaces
+ *      BlockDatasetLoader.py's ShuffleBlockWrapper indexing, default collate and the three host-to-device copies of
+ *      Workflow.train_epoch, Workflow.py:781-783).  nodes [*, row_nodes], edges [*, row_edges], apds [*, apd]: the
+ *      block, row-major int8.  For r < b, output row r is block row rows[r]: out_nodes / out_edges as int8
+ *      (out_dtype 1) or widened to float32 (out_dtype 0), out_target always float32 widened from signed int8 (as
+ *      HDFDataset.__getitem__'s .type(torch.float32)).  Rows b <= r < B are zero (empty molecules).  ctl, when not
+ *      NULL, is set to {b, b > 0 ? float32(1.0 / b) : 0}.  One launch; rows[] must index the block (the loader makes
+ *      them).  Block and output pointers must be 16-byte aligned; b > B, non-positive dims, null pointers and an
+ *      unknown out_dtype are refused. */
+int gib_gather_rows(const signed char* nodes, const signed char* edges, const signed char* apds, const int* rows,
+                    int b, int B, int row_nodes, int row_edges, int apd, void* out_nodes, void* out_edges,
+                    int out_dtype, float* out_target, gib_batch_ctl* ctl, gib_stream stream);   /* ctl may be NULL */
+
 /* ---- flat-bucket Adam step: replaces torch.optim.Adam.step() on the model parameters (constructed at
  *      Workflow.py:191,221,245, stepped at Workflow.py:795-796; same update rule, L2 weight decay, no amsgrad)
  *      with ONE launch over contiguous params / grads / exp_avg / exp_avg_sq of n floats.  `step` is the
