@@ -148,6 +148,9 @@ _PROTOS = {
     "gib_preprocess_apd_length": (c_i, [c_p]),
     "gib_preprocess_ws_bytes": (c_sz, [c_p, c_i, c_i]),
     "gib_preprocess_chunk": (c_i, [c_p, c_p, c_p, c_i, c_i, c_i, c_i] + [c_p] * 7),
+    "gib_preprocess_group_statistics_bytes": (c_sz, [c_p, c_i]),
+    "gib_preprocess_group_statistics_ws_bytes": (c_sz, [c_p, c_i]),
+    "gib_preprocess_group_statistics": (c_i, [c_p, c_p, c_p, c_i, c_i] + [c_p] * 5),
     "gib_profile_enable": (None, [c_i]),
     "gib_launch_count": (c_ll, []),
     "gib_profile_collect": (c_i, [c_p, c_p, c_p]),

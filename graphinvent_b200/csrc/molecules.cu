@@ -5,7 +5,8 @@
 // single-CTA scan over molecules, then every record at its final offset.  No atomics; bonds come out in the order of
 // `torch.nonzero(edge_features * triu(ones(N, N), 1))` (row-major (i, j, type) over the padded N x N x Ef).
 // The statistics are a per-molecule pass into a workspace and one single-CTA pass that sums it over molecules in
-// molecule order, as the reference's Python loops do.
+// molecule order, as the reference's Python loops do.  The same per-molecule pass, on the int8 chunk of
+// gib_preprocess_chunk, gives the training-set properties of each group it completed (one CTA per group, integer sums).
 #include "common.cuh"
 #include "../../include/gib200.h"
 
@@ -217,28 +218,22 @@ __global__ void __launch_bounds__(kNT) mol_fill_kernel(int B, int N, int F, int 
 // workspace per molecule: F column sums, Ef bond-type sums (f32), 10 n_edges bins, n_nodes, error (i32)
 __host__ __device__ inline size_t stat_ws_words(int F, int Ef) { return (size_t)F + Ef + 10 + 2; }
 
-__global__ void __launch_bounds__(kStatNT) mol_stats_kernel(int N, int F, int Ef, const float* __restrict__ nodes,
-                                                            const float* __restrict__ edges,
-                                                            const int* __restrict__ table, float* __restrict__ ws) {
-  __shared__ float s_row[kMaxN * kMaxEf];
-  __shared__ int s_bin[kMaxN];
-  const int b = blockIdx.x;
-  const int* m = table + kHdr + (size_t)b * kMolWords;
-  // GenerationGraph.n_nodes: molecule.GetNumAtoms(), 0 when graph_to_graph gave mol = None
-  const int n_eff = (m[5] & GIB_MOL_DECODES) ? max(m[0], 0) : 0;
-  const float* nd = nodes + (size_t)b * N * F;
-  const float* e = edges + (size_t)b * N * N * Ef;
-  float* w = ws + (size_t)b * stat_ws_words(F, Ef);
+// One molecule's partials, shared by the generated batches (float32 input) and the preprocessed chunks (int8 input):
+// n_eff atoms are binned; s_row / s_bin are shared scratch of the calling CTA (kStatNT threads).
+template <typename T>
+__device__ __forceinline__ void mol_stats_one(int N, int F, int Ef, int n_eff, const T* __restrict__ nd,
+                                              const T* __restrict__ e, float* __restrict__ w, float* s_row,
+                                              int* s_bin) {
   int* wi = reinterpret_cast<int*>(w + F + Ef);
   for (int f = threadIdx.x; f < F; f += kStatNT) {  // torch.sum(node_features, dim=0) over all N padded rows
     float acc = 0.f;
-    for (int r = 0; r < N; ++r) acc += nd[(size_t)r * F + f];
+    for (int r = 0; r < N; ++r) acc += (float)nd[(size_t)r * F + f];
     w[f] = acc;
   }
   for (int i = threadIdx.x; i < N; i += kStatNT) {  // torch.sum(edges[i, :, t])
     for (int t = 0; t < Ef; ++t) {
       float acc = 0.f;
-      for (int j = 0; j < N; ++j) acc += e[((size_t)i * N + j) * Ef + t];
+      for (int j = 0; j < N; ++j) acc += (float)e[((size_t)i * N + j) * Ef + t];
       s_row[i * Ef + t] = acc;
     }
   }
@@ -279,6 +274,19 @@ __global__ void __launch_bounds__(kStatNT) mol_stats_kernel(int N, int F, int Ef
     for (int i = 0; i < N; ++i) acc += s_row[i * Ef + t];
     w[F + t] = acc;
   }
+}
+
+__global__ void __launch_bounds__(kStatNT) mol_stats_kernel(int N, int F, int Ef, const float* __restrict__ nodes,
+                                                            const float* __restrict__ edges,
+                                                            const int* __restrict__ table, float* __restrict__ ws) {
+  __shared__ float s_row[kMaxN * kMaxEf];
+  __shared__ int s_bin[kMaxN];
+  const int b = blockIdx.x;
+  const int* m = table + kHdr + (size_t)b * kMolWords;
+  // GenerationGraph.n_nodes: molecule.GetNumAtoms(), 0 when graph_to_graph gave mol = None
+  const int n_eff = (m[5] & GIB_MOL_DECODES) ? max(m[0], 0) : 0;
+  mol_stats_one(N, F, Ef, n_eff, nodes + (size_t)b * N * F, edges + (size_t)b * N * N * Ef,
+                ws + (size_t)b * stat_ws_words(F, Ef), s_row, s_bin);
 }
 
 // ---- statistics: over molecules, in molecule order (single CTA) -------------------------------------------------
@@ -328,6 +336,65 @@ __global__ void __launch_bounds__(kStatNT) mol_stats_sum_kernel(int B, int N, in
     table[2] = mol;
     table[3] = mol < 0 ? 0 : err & 3;
     table[4] = mol < 0 ? 0 : err >> 2;
+  }
+}
+
+// ---- training-set properties of the groups of one gib_preprocess_chunk call ----------------------------------------
+// per molecule of the chunk that ended up in a group: the partials above from the int8 graph, with
+// n_nodes = the rows up to the last non-zero one (PreprocessingGraph.n_nodes = GetNumAtoms(): the chunk pass refuses a
+// zero row between atoms)
+__global__ void __launch_bounds__(kStatNT) pp_mol_stats_kernel(int N, int F, int Ef,
+                                                               const signed char* __restrict__ nodes,
+                                                               const signed char* __restrict__ edges,
+                                                               const int* __restrict__ status, float* __restrict__ ws) {
+  __shared__ float s_row[kMaxN * kMaxEf];
+  __shared__ int s_bin[kMaxN];
+  __shared__ int s_last;
+  const int b = blockIdx.x;
+  if (b >= status[1]) return;  // not in a completed group (status[1] is 0 when the chunk was refused)
+  const signed char* nd = nodes + (size_t)b * N * F;
+  if (threadIdx.x == 0) s_last = -1;
+  __syncthreads();
+  int last = -1;
+  for (int r = threadIdx.x; r < N; r += kStatNT) {
+    bool any = false;
+    for (int f = 0; f < F; ++f) any |= nd[(size_t)r * F + f] != 0;
+    if (any) last = r;
+  }
+  atomicMax(&s_last, last);
+  __syncthreads();
+  mol_stats_one(N, F, Ef, s_last + 1, nd, edges + (size_t)b * N * N * Ef, ws + (size_t)b * stat_ws_words(F, Ef),
+                s_row, s_bin);
+}
+
+// one CTA per group, each output word summed over the group's molecules in molecule order, in integers
+__host__ __device__ inline int pp_stat_words(int N, int F, int Ef) { return 4 + N + 1 + F + 10 + Ef; }
+
+__global__ void __launch_bounds__(kStatNT) pp_group_stats_kernel(int N, int F, int Ef, const float* __restrict__ ws,
+                                                                 const int* __restrict__ groups,
+                                                                 const int* __restrict__ status, int* __restrict__ out) {
+  const size_t W = stat_ws_words(F, Ef);
+  const int S = pp_stat_words(N, F, Ef);
+  const int o_nf = 4 + N + 1, o_ne = o_nf + F, o_ef = o_ne + 10;
+  const int ng = status[0];
+  for (int g = blockIdx.x; g < ng; g += gridDim.x) {
+    const int s = groups[4 * g], e = groups[4 * g + 1];
+    int* o = out + (size_t)g * S;
+    for (int k = threadIdx.x; k < S; k += kStatNT) {
+      int acc = 0;
+      if (k < 4) {
+        acc = groups[4 * g + k];
+      } else if (k < o_nf) {                           // n_nodes_hist[k - 4]
+        for (int m = s; m < e; ++m) acc += reinterpret_cast<const int*>(ws + m * W + F + Ef)[10] == k - 4;
+      } else if (k < o_ne) {                           // node-feature column sums
+        for (int m = s; m < e; ++m) acc += (int)ws[m * W + (k - o_nf)];
+      } else if (k < o_ef) {                           // n_edges_hist
+        for (int m = s; m < e; ++m) acc += reinterpret_cast<const int*>(ws + m * W + F + Ef)[k - o_ne];
+      } else {                                         // bonds per type: the symmetric entry sum / 2
+        for (int m = s; m < e; ++m) acc += (int)ws[m * W + F + (k - o_ef)] / 2;
+      }
+      o[k] = acc;
+    }
   }
 }
 
@@ -396,6 +463,40 @@ int gib_graph_statistics(int B, int N, int F, int Ef, const float* nodes, const 
   mol_stats_kernel<<<B, kStatNT, 0, s>>>(N, F, Ef, nodes, edges, table, (float*)ws);
   GIB_LAUNCH_CHECK();
   mol_stats_sum_kernel<<<1, kStatNT, 0, s>>>(B, N, F, Ef, (const float*)ws, table, out);
+  GIB_LAUNCH_CHECK();
+  return 0;
+}
+
+size_t gib_preprocess_group_statistics_bytes(const gib_pp_dims* d, int max_groups) {
+  if (gib_preprocess_apd_length(d) < 0) return 0;
+  if (check_mol_dims("gib_preprocess_group_statistics_bytes", max_groups, d->N, d->F, d->Ef)) return 0;
+  return 4 * (size_t)max_groups * pp_stat_words(d->N, d->F, d->Ef);
+}
+
+size_t gib_preprocess_group_statistics_ws_bytes(const gib_pp_dims* d, int max_molecules) {
+  if (gib_preprocess_apd_length(d) < 0) return 0;
+  if (check_mol_dims("gib_preprocess_group_statistics_ws_bytes", max_molecules, d->N, d->F, d->Ef)) return 0;
+  return 4 * (size_t)max_molecules * stat_ws_words(d->F, d->Ef);
+}
+
+int gib_preprocess_group_statistics(const gib_pp_dims* d, const signed char* nodes, const signed char* edges,
+                                    int n_molecules, int max_molecules, const int* groups, const int* status,
+                                    void* ws, int* out, gib_stream stream) {
+  if (!gib_preprocess_group_statistics_ws_bytes(d, max_molecules)) return -1;
+  if (n_molecules < 1 || n_molecules > max_molecules) {
+    set_error("gib_preprocess_group_statistics: n_molecules %d outside [1, max_molecules = %d]", n_molecules,
+              max_molecules);
+    return -1;
+  }
+  if (!nodes || !edges || !groups || !status || !ws || !out) {
+    set_error("gib_preprocess_group_statistics: null argument");
+    return -1;
+  }
+  cudaStream_t s = (cudaStream_t)stream;
+  pp_mol_stats_kernel<<<n_molecules, kStatNT, 0, s>>>(d->N, d->F, d->Ef, nodes, edges, status, (float*)ws);
+  GIB_LAUNCH_CHECK();
+  pp_group_stats_kernel<<<min(n_molecules, 1024), kStatNT, 0, s>>>(d->N, d->F, d->Ef, (const float*)ws, groups,
+                                                                    status, out);
   GIB_LAUNCH_CHECK();
   return 0;
 }

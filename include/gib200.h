@@ -589,6 +589,24 @@ size_t gib_preprocess_ws_bytes(const gib_pp_dims* d, int max_molecules, int max_
 int gib_preprocess_chunk(const gib_pp_dims* d, const signed char* nodes, const signed char* edges, int n_molecules,
                          int last_chunk, int max_molecules, int max_rows, void* ws, signed char* out_nodes,
                          signed char* out_edges, int* out_apds, int* groups, int* status, gib_stream stream);
+/* The training-set properties of the groups a gib_preprocess_chunk call completed (Analyzer.get_molecular_properties,
+ * Analyzer.py:311-599, as DataProcesser.get_ts_properties runs it per group), on the same stream after that call, from
+ * the same `nodes` / `edges`, `n_molecules`, `max_molecules`, `groups` and `status` (the group count is read on the
+ * device).  Row g of `out` (int32, gib_preprocess_group_statistics_bytes(d, max_molecules) bytes; rows past status[0]
+ * are not written) is group g's 4 words of `groups` followed by integer sums over its molecules [first, after last):
+ *   n_nodes_hist [N+1]     molecules per atom count (the rows up to the last non-zero one)
+ *   node sums [F]          column sums of the node features
+ *   n_edges_hist [10]      atoms per bond count, as _get_n_edges_distribution bins them: a count above 10 goes to bin
+ *                          9, and so does an atom without bonds (bin n_edges - 1 = -1)
+ *   bonds [Ef]             bonds per type (half the sum of the symmetric edge entries)
+ * Each molecule's partials come from the per-molecule pass of gib_graph_statistics; each group is summed by one CTA
+ * in molecule order: the results are deterministic.  Besides gib_preprocess_chunk's limits: N <= 255, Ef <= 16.
+ * ws: gib_preprocess_group_statistics_ws_bytes(d, max_molecules), may hold anything. */
+size_t gib_preprocess_group_statistics_bytes(const gib_pp_dims* d, int max_groups);
+size_t gib_preprocess_group_statistics_ws_bytes(const gib_pp_dims* d, int max_molecules);
+int gib_preprocess_group_statistics(const gib_pp_dims* d, const signed char* nodes, const signed char* edges,
+                                    int n_molecules, int max_molecules, const int* groups, const int* status,
+                                    void* ws, int* out, gib_stream stream);
 
 /* ---- measurement hooks: CUDA-event timing per kernel class on the launching stream.
  *      class 0 = forward/dX launches of the tensor-core kernel, 1 = its weight-gradient launches, 2 = scatter-aggregate (K2),
