@@ -151,6 +151,12 @@ _PROTOS = {
     "gib_preprocess_group_statistics_bytes": (c_sz, [c_p, c_i]),
     "gib_preprocess_group_statistics_ws_bytes": (c_sz, [c_p, c_i]),
     "gib_preprocess_group_statistics": (c_i, [c_p, c_p, c_p, c_i, c_i] + [c_p] * 5),
+    "gib_route_plan_ws_bytes": (c_sz, [c_p, c_i]),
+    "gib_route_max_states": (c_ll, [c_p, c_i]),
+    "gib_route_plan": (c_i, [c_p, c_p, c_p, c_i, c_i] + [c_p] * 4),
+    "gib_route_fill": (c_i, [c_p, c_p, c_p, c_i] + [c_p] * 8),
+    "gib_route_probs": (c_i, [c_i, c_i, c_p, c_p, c_p, c_p]),
+    "gib_route_reduce": (c_i, [c_i] + [c_p] * 5),
     "gib_profile_enable": (None, [c_i]),
     "gib_launch_count": (c_ll, []),
     "gib_profile_collect": (c_i, [c_p, c_p, c_p]),

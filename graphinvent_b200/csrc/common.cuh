@@ -55,6 +55,29 @@ __device__ __forceinline__ float block_reduce(float v, float* sm, bool is_max) {
   return r;
 }
 
+// Unaligned int8 rows through aligned 16-byte loads (the loader's gather and the route fill): every aligned word
+// load_span reads holds at least one byte of the span, so no load leaves a 16-byte aligned allocation.
+typedef unsigned __int128 u128;
+
+__device__ __forceinline__ u128 ld16(const uint8_t* p) {
+  const uint4 w = __ldg(reinterpret_cast<const uint4*>(p));
+  return (u128)w.x | ((u128)w.y << 32) | ((u128)w.z << 64) | ((u128)w.w << 96);
+}
+
+// bytes p[0, len) in the low bytes of the result, 1 <= len <= 16; the bytes above len are unspecified
+__device__ __forceinline__ u128 load_span(const uint8_t* p, int len) {
+  const int off = (int)(reinterpret_cast<uintptr_t>(p) & 15);
+  const uint8_t* a = p - off;
+  const u128 lo = ld16(a);
+  if (off == 0) return lo;
+  const u128 hi = off + len > 16 ? ld16(a + 16) : (u128)0;
+  return (lo >> (8 * off)) | (hi << (128 - 8 * off));
+}
+
+__device__ __forceinline__ void st16(void* p, u128 v) {
+  *reinterpret_cast<uint4*>(p) = make_uint4((unsigned)v, (unsigned)(v >> 32), (unsigned)(v >> 64), (unsigned)(v >> 96));
+}
+
 // error plumbing: kernels are launched through GIB_LAUNCH_CHECK so that a bad launch
 // configuration is reported at the C-ABI boundary as a cudaError_t (>0).
 #define GIB_CUDA_TRY(expr)                                   \

@@ -16,8 +16,6 @@ namespace gib {
 
 namespace {
 
-typedef unsigned __int128 u128;
-
 constexpr int kGatherNT = 256;
 constexpr int kGatherMaxBlocks = 4096;
 
@@ -28,21 +26,6 @@ struct GatherArray {
   int widen;              // 1: float32 output
   long long chunks;       // ceil(B * rb / 16)
 };
-
-__device__ __forceinline__ u128 ld16(const uint8_t* p) {
-  const uint4 w = __ldg(reinterpret_cast<const uint4*>(p));
-  return (u128)w.x | ((u128)w.y << 32) | ((u128)w.z << 64) | ((u128)w.w << 96);
-}
-
-// bytes p[0, len) in the low bytes of the result, 1 <= len <= 16; the bytes above len are unspecified
-__device__ __forceinline__ u128 load_span(const uint8_t* p, int len) {
-  const int off = (int)(reinterpret_cast<uintptr_t>(p) & 15);
-  const uint8_t* a = p - off;
-  const u128 lo = ld16(a);
-  if (off == 0) return lo;
-  const u128 hi = off + len > 16 ? ld16(a + 16) : (u128)0;
-  return (lo >> (8 * off)) | (hi << (128 - 8 * off));
-}
 
 __device__ __forceinline__ void gather_chunk(const GatherArray& g, long long c, const int* __restrict__ rows, int b,
                                              int B) {
@@ -66,8 +49,7 @@ __device__ __forceinline__ void gather_chunk(const GatherArray& g, long long c, 
   if (!g.widen) {
     int8_t* out = static_cast<int8_t*>(g.dst) + e0;
     if (n == 16) {
-      *reinterpret_cast<uint4*>(out) = make_uint4((unsigned)v, (unsigned)(v >> 32), (unsigned)(v >> 64),
-                                                  (unsigned)(v >> 96));
+      st16(out, v);
     } else {
       for (int j = 0; j < n; ++j) out[j] = (int8_t)(uint8_t)(v >> (8 * j));
     }

@@ -18,6 +18,7 @@
 // and appends the state when no row matched OR the match was the last row.  Rows are appended in state order and a
 // first occurrence is always appended, so with pf(i) = the latest first occurrence at or before state i, a repeated
 // state i is appended iff first(i) == pf(i) and no state in (pf(i), i) was appended the same way.
+#include <algorithm>
 #include <climits>
 
 #include "common.cuh"
@@ -597,6 +598,165 @@ __global__ void pp_scatter_kernel(PP p, const int* off, const int* apd, const in
   }
 }
 
+// ---- count -> scan -> route: the decoding routes of n molecules, shared by the training-set construction and the
+// route scorer ----------------------------------------------------------------------------------------------------
+struct RouteBufs {
+  int* len;
+  int* n0;
+  int* off;
+  short* rs;
+  unsigned long long* hash;
+  int* apd;
+  int* nn;
+  int* mol;
+};
+
+int launch_route(const PP& p, const signed char* nodes, const signed char* edges, int n, const RouteBufs& r,
+                 int* status, cudaStream_t s) {
+  pp_count_kernel<<<n, 32, 0, s>>>(p, nodes, edges, r.len, r.n0, status);
+  GIB_LAUNCH_CHECK();
+  pp_scan_kernel<<<1, 1024, 0, s>>>(n, r.len, r.off, status);
+  GIB_LAUNCH_CHECK();
+  const size_t smem = 4 * (size_t)p.N + (size_t)p.N * p.F + (size_t)p.N * p.N * p.Ef;
+  pp_route_kernel<<<n, 32, smem, s>>>(p, nodes, edges, r.off, r.n0, r.hash, r.apd, r.nn, r.mol, r.rs, status);
+  GIB_LAUNCH_CHECK();
+  return 0;
+}
+
+// ---- the route scorer (graphinvent_b200.graphed.RouteScorer): its plan workspace, the fill of one batch of route
+// states into the model's static int8 inputs, the per-molecule reduction ----------------------------------------
+constexpr int kFillNT = 256;
+constexpr int kFillMaxBlocks = 4096;
+constexpr int kCursor = 6;      // status word: replays of the chunk done so far (the fill's batch index)
+
+struct RouteWs {
+  size_t len, n0, rs, hash, apd, nn, mol, total;
+};
+
+RouteWs route_ws_layout(const PP& p, int max_mols) {
+  RouteWs w{};
+  const long long states = (long long)max_mols * p.s_max;
+  size_t o = 0;
+  auto take = [&](size_t bytes) { size_t r = o; o = align256(o + bytes); return r; };
+  w.len = take(4ull * max_mols);
+  w.n0 = take(4ull * max_mols);
+  w.rs = take(2ull * max_mols * p.N * p.N);
+  w.hash = take(8ull * states);
+  w.apd = take(4ull * states);
+  w.nn = take(4ull * states);
+  w.mol = take(4ull * states);
+  w.total = o;
+  return w;
+}
+
+struct FillSrc {
+  const signed char* nodes;
+  const signed char* edges;
+  const int* off;
+  const int* nn;
+  const int* mol;
+  const int* apd;
+  const short* rs;
+};
+
+// one 16-byte chunk of the flat [B, rb] output (edges_part: the edges array, else the nodes array): each row segment
+// it covers comes from its state's molecule through the aligned-word funnel, then the bytes the state does not hold
+// (node rows >= nn, bonds with rs <= k) are cleared.  Rows past the chunk's last state are zero.
+__device__ __forceinline__ void fill_chunk(const PP& p, const FillSrc& f, bool edges_part, long long c, int s0,
+                                           int S, signed char* dst) {
+  const int rb = edges_part ? p.N * p.N * p.Ef : p.N * p.F;
+  const long long total = (long long)p.B * rb;
+  const long long e0 = c * 16;
+  const int n = (int)min(16LL, total - e0);
+  long long r = e0 / rb;
+  int col = (int)(e0 - r * rb);
+  u128 v = 0;
+  for (int k = 0; k < n;) {
+    const int seg = min(n - k, rb - col);
+    const int i = s0 + (int)r;
+    if (i < S) {
+      const int m = f.mol[i];
+      const uint8_t* src = reinterpret_cast<const uint8_t*>(edges_part ? f.edges : f.nodes) + (size_t)m * rb + col;
+      u128 s = load_span(src, seg);
+      if (edges_part) {
+        const int step = i - f.off[m];
+        const short* rs = f.rs + (size_t)m * p.N * p.N;
+        for (int j = 0; j < seg; ++j)
+          if (rs[(col + j) / p.Ef] <= step) s &= ~((u128)0xff << (8 * j));
+      } else {
+        const int nn = f.nn[i];
+        for (int j = 0; j < seg; ++j)
+          if ((col + j) / p.F >= nn) s &= ~((u128)0xff << (8 * j));
+      }
+      if (seg < 16) s &= ((u128)1 << (8 * seg)) - 1;
+      v |= s << (8 * k);
+    }
+    k += seg;
+    ++r;
+    col = 0;
+  }
+  signed char* out = dst + e0;
+  if (n == 16) {
+    st16(out, v);
+  } else {
+    for (int j = 0; j < n; ++j) out[j] = (signed char)(uint8_t)(v >> (8 * j));
+  }
+}
+
+// states [s0, s0 + B) of the chunk, s0 = status[kCursor] * B, into the model's int8 inputs; per slot b its action and
+// its place in the likelihood buffer (build order: the molecule's empty graph first), -1 / -1 past the last state
+__global__ void __launch_bounds__(kFillNT) route_fill_kernel(PP p, FillSrc f, const int* __restrict__ status,
+                                                             gib_batch_ctl* ctl, int* __restrict__ slots,
+                                                             signed char* __restrict__ out_nodes,
+                                                             signed char* __restrict__ out_edges,
+                                                             long long node_chunks, long long edge_chunks) {
+  const int B = p.B, S = status[5], s0 = status[kCursor] * B;
+  const long long tid = (long long)blockIdx.x * kFillNT + threadIdx.x, stride = (long long)gridDim.x * kFillNT;
+  if (tid == 0) ctl->live = max(0, min(B, S - s0));
+  for (long long b = tid; b < B; b += stride) {
+    const int i = s0 + (int)b;
+    int a = -1, d = -1;
+    if (i < S) {
+      const int m = f.mol[i];
+      a = f.apd[i];
+      d = f.off[m] + f.off[m + 1] - 1 - i;
+    }
+    slots[b] = a;
+    slots[B + b] = d;
+  }
+  for (long long c = tid; c < node_chunks + edge_chunks; c += stride) {
+    if (c < node_chunks) fill_chunk(p, f, false, c, s0, S, out_nodes);
+    else fill_chunk(p, f, true, c - node_chunks, s0, S, out_edges);
+  }
+}
+
+// per molecule, in build order: nll = -sum log p and final = log(sum p), both accumulated in fp64 and rounded once
+__global__ void route_reduce_kernel(int n, const int* __restrict__ off, const float* __restrict__ lik,
+                                    float* __restrict__ nll, float* __restrict__ fin) {
+  const int m = blockIdx.x * blockDim.x + threadIdx.x;
+  if (m >= n) return;
+  double l = 0.0, s = 0.0;
+  for (int i = off[m]; i < off[m + 1]; ++i) {
+    const double q = (double)lik[i];
+    l -= log(q);
+    s += q;
+  }
+  nll[m] = (float)l;
+  fin[m] = (float)log(s);
+}
+
+bool aligned16(const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15) == 0; }
+
+int route_limits(const char* who, const gib_pp_dims* d, int max_molecules, PP* p) {
+  GIB_TRY(make_pp(who, d, p));
+  if (max_molecules < 1 || (long long)max_molecules * p->s_max >= INT_MAX / 2) {
+    set_error("%s: need max_molecules >= 1 and max_molecules * (N*(N-1)/2 + 2) < %d states, got %d", who,
+              INT_MAX / 2, max_molecules);
+    return -1;
+  }
+  return 0;
+}
+
 }  // namespace
 }  // namespace gib
 
@@ -656,13 +816,7 @@ int gib_preprocess_chunk(const gib_pp_dims* d, const signed char* nodes, const s
   const int init_blocks = (int)(w.table / 256 < 1024 ? w.table / 256 : 1024);
   pp_init_kernel<<<init_blocks, 256, 0, s>>>(status, keys, vals, w.table);
   GIB_LAUNCH_CHECK();
-  pp_count_kernel<<<n_molecules, 32, 0, s>>>(p, nodes, edges, len, n0, status);
-  GIB_LAUNCH_CHECK();
-  pp_scan_kernel<<<1, 1024, 0, s>>>(n_molecules, len, off, status);
-  GIB_LAUNCH_CHECK();
-  const size_t smem = 4 * (size_t)p.N + (size_t)p.N * p.F + (size_t)p.N * p.N * p.Ef;
-  pp_route_kernel<<<n_molecules, 32, smem, s>>>(p, nodes, edges, off, n0, hash, apd, nn, mol, rs, status);
-  GIB_LAUNCH_CHECK();
+  GIB_TRY(launch_route(p, nodes, edges, n_molecules, RouteBufs{len, n0, off, rs, hash, apd, nn, mol}, status, s));
   const StateRef S{off, nn, mol, rs, nodes, edges};
   pp_group_kernel<<<1, kGroupNT, 0, s>>>(p, S, n_molecules, last_chunk, max_rows, hash, keys, vals, w.table - 1,
                                          (int*)(b + w.slot), (int*)(b + w.row_of), (int*)(b + w.dst),
@@ -673,6 +827,81 @@ int gib_preprocess_chunk(const gib_pp_dims* d, const signed char* nodes, const s
   GIB_LAUNCH_CHECK();
   pp_scatter_kernel<<<1024, 256, 0, s>>>(p, off, apd, (const int*)(b + w.dst), (const int*)(b + w.own), status,
                                          out_apds);
+  GIB_LAUNCH_CHECK();
+  return 0;
+}
+
+size_t gib_route_plan_ws_bytes(const gib_pp_dims* d, int max_molecules) {
+  PP p;
+  if (route_limits("gib_route_plan_ws_bytes", d, max_molecules, &p)) return 0;
+  return route_ws_layout(p, max_molecules).total;
+}
+
+long long gib_route_max_states(const gib_pp_dims* d, int max_molecules) {
+  PP p;
+  GIB_TRY(route_limits("gib_route_max_states", d, max_molecules, &p));
+  return (long long)max_molecules * p.s_max;
+}
+
+int gib_route_plan(const gib_pp_dims* d, const signed char* nodes, const signed char* edges, int n_molecules,
+                   int max_molecules, void* ws, int* offsets, int* status, gib_stream stream) {
+  PP p;
+  GIB_TRY(route_limits("gib_route_plan", d, max_molecules, &p));
+  if (n_molecules < 1 || n_molecules > max_molecules) {
+    set_error("gib_route_plan: n_molecules %d outside [1, max_molecules = %d]", n_molecules, max_molecules);
+    return -1;
+  }
+  if (!nodes || !edges || !ws || !offsets || !status) {
+    set_error("gib_route_plan: null argument");
+    return -1;
+  }
+  const RouteWs w = route_ws_layout(p, max_molecules);
+  char* b = static_cast<char*>(ws);
+  cudaStream_t s = (cudaStream_t)stream;
+  pp_init_kernel<<<1, 32, 0, s>>>(status, nullptr, nullptr, 0);
+  GIB_LAUNCH_CHECK();
+  return launch_route(p, nodes, edges, n_molecules,
+                      RouteBufs{(int*)(b + w.len), (int*)(b + w.n0), offsets, (short*)(b + w.rs),
+                                (unsigned long long*)(b + w.hash), (int*)(b + w.apd), (int*)(b + w.nn),
+                                (int*)(b + w.mol)},
+                      status, s);
+}
+
+int gib_route_fill(const gib_pp_dims* d, const signed char* nodes, const signed char* edges, int max_molecules,
+                   const void* ws, const int* offsets, const int* status, gib_batch_ctl* ctl, int* slots,
+                   signed char* out_nodes, signed char* out_edges, gib_stream stream) {
+  PP p;
+  GIB_TRY(route_limits("gib_route_fill", d, max_molecules, &p));
+  if (!nodes || !edges || !ws || !offsets || !status || !ctl || !slots || !out_nodes || !out_edges) {
+    set_error("gib_route_fill: null argument");
+    return -1;
+  }
+  if (!aligned16(nodes) || !aligned16(edges) || !aligned16(out_nodes) || !aligned16(out_edges)) {
+    set_error("gib_route_fill: nodes, edges, out_nodes and out_edges must be 16-byte aligned");
+    return -1;
+  }
+  const RouteWs w = route_ws_layout(p, max_molecules);
+  const char* b = static_cast<const char*>(ws);
+  const FillSrc f{nodes, edges, offsets, (const int*)(b + w.nn), (const int*)(b + w.mol), (const int*)(b + w.apd),
+                  (const short*)(b + w.rs)};
+  const long long nc = ceil_div_ll((long long)p.B * p.N * p.F, 16);
+  const long long ec = ceil_div_ll((long long)p.B * p.N * p.N * p.Ef, 16);
+  const long long need = std::max<long long>(ceil_div_ll(nc + ec, kFillNT), ceil_div_ll(p.B, kFillNT));
+  const int blocks = (int)std::min<long long>(need, kFillMaxBlocks);
+  route_fill_kernel<<<blocks, kFillNT, 0, (cudaStream_t)stream>>>(p, f, status, ctl, slots, out_nodes, out_edges, nc,
+                                                                  ec);
+  GIB_LAUNCH_CHECK();
+  return 0;
+}
+
+int gib_route_reduce(int n_molecules, const int* offsets, const float* likelihoods, float* nll, float* final_,
+                     gib_stream stream) {
+  if (n_molecules < 1 || !offsets || !likelihoods || !nll || !final_) {
+    set_error("gib_route_reduce: need n_molecules >= 1 and every pointer, got n_molecules = %d", n_molecules);
+    return -1;
+  }
+  route_reduce_kernel<<<ceil_div(n_molecules, 128), 128, 0, (cudaStream_t)stream>>>(n_molecules, offsets,
+                                                                                    likelihoods, nll, final_);
   GIB_LAUNCH_CHECK();
   return 0;
 }

@@ -70,6 +70,22 @@ int rl_probs_launch(const float* logits_a, const float* logits_b, int B, int apd
   return 0;
 }
 
+// the route scorer's probability of each slot's route action (graphed.RouteScorer): p = softmax(logits[b])[a] by
+// rl_probs_kernel's reduction, written at the state's place dst; slots [2B] = {action[B], dst[B]}, dst < 0: padding
+__global__ void __launch_bounds__(kRowThreads) route_probs_kernel(const float* __restrict__ logits, int apd,
+                                                                  const int* __restrict__ slots,
+                                                                  float* __restrict__ lik) {
+  __shared__ float sm[kRowThreads / 32];
+  const int b = blockIdx.x, B = gridDim.x;
+  const int dst = slots[B + b];
+  if (dst < 0) return;
+  const float* o = logits + (size_t)b * apd;
+  float mx, se;
+  row_softmax(o, apd, sm, mx, se);
+  const float p = row_prob(o, apd, slots[b], mx, se);
+  if (threadIdx.x == 0) lik[dst] = p;
+}
+
 // one CTA per slot: float 0/1 state -> int8 model input and, for a running round, the record row state[0]
 __global__ void __launch_bounds__(128) rl_snapshot_kernel(int N, int F, int Ef, int att_view,
                                                           const float* __restrict__ nodes,
@@ -246,6 +262,16 @@ int gib_rl_dlogits(int B, int apd, const float* logits, const int* act, const fl
     return -1;
   }
   rl_dlogits_kernel<<<B, kRowThreads, 0, ST(stream)>>>(apd, logits, act, dp, ctl, dlogits, p);
+  GIB_LAUNCH_CHECK();
+  return 0;
+}
+
+int gib_route_probs(int B, int apd, const float* logits, const int* slots, float* likelihoods, gib_stream stream) {
+  if (B <= 0 || apd <= 0 || !logits || !slots || !likelihoods) {
+    set_error("gib_route_probs: bad arguments (B=%d apd=%d; logits, slots and likelihoods must be given)", B, apd);
+    return -1;
+  }
+  route_probs_kernel<<<B, kRowThreads, 0, ST(stream)>>>(logits, apd, slots, likelihoods);
   GIB_LAUNCH_CHECK();
   return 0;
 }

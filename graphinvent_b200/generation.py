@@ -36,26 +36,35 @@ def _ptr(t):
     return ctypes.c_void_p(t.data_ptr())
 
 
+def action_layout(model, constants=None, n_atom_types=None, n_formal_charge=None, n_imp_H=None, n_chirality=None):
+    """(constants, n_atom_types, n_formal_charge, n_imp_H, n_chirality) of a generator's layout arguments: each one
+    not given comes from the constants (the model's by default); raises ValueError for a layout the constants'
+    n_node_features and len_f_add_per_node do not fit"""
+    C = constants if constants is not None else model.constants
+    A = n_atom_types if n_atom_types is not None else getattr(C, "n_atom_types")
+    CH = n_formal_charge if n_formal_charge is not None else getattr(C, "n_formal_charge")
+    H = n_imp_H if n_imp_H is not None else getattr(C, "n_imp_H", 0)
+    X = n_chirality if n_chirality is not None else getattr(C, "n_chirality", 0)
+    counts = (A, CH, H, X)
+    len_f_add = A * CH * max(H, 1) * max(X, 1) * C.n_edge_features
+    if (min(A, CH) < 1 or min(H, X) < 0 or max(counts) > 255
+            or sum(counts) != C.n_node_features or len_f_add != C.len_f_add_per_node):
+        raise ValueError(
+            f"inconsistent action layout: n_atom_types={A}, n_formal_charge={CH}, n_imp_H={H}, "
+            f"n_chirality={X} (each <= 255; 0 = segment absent) need n_node_features = {sum(counts)} "
+            f"and len_f_add_per_node = {len_f_add}, the constants have {C.n_node_features} and {C.len_f_add_per_node} "
+            "(graphinvent_b200.config.layout_dims derives them from the reference's flags)")
+    return C, A, CH, H, X
+
+
 class GraphGenerator:
     def __init__(self, model, batch_size, constants=None, n_atom_types=None, n_formal_charge=None, n_imp_H=None,
                  n_chirality=None, device="cuda"):
-        C = constants if constants is not None else model.constants
+        C, self.A, self.CH, self.n_imp_H, self.n_chirality = action_layout(
+            model, constants, n_atom_types, n_formal_charge, n_imp_H, n_chirality)
         self.constants = C
         self.model, self.batch_size, self.device = model, int(batch_size), torch.device(device)
         self.N, self.F, self.Ef = C.max_n_nodes, C.n_node_features, C.n_edge_features
-        self.A = n_atom_types if n_atom_types is not None else getattr(C, "n_atom_types")
-        self.CH = n_formal_charge if n_formal_charge is not None else getattr(C, "n_formal_charge")
-        self.n_imp_H = n_imp_H if n_imp_H is not None else getattr(C, "n_imp_H", 0)
-        self.n_chirality = n_chirality if n_chirality is not None else getattr(C, "n_chirality", 0)
-        counts = (self.A, self.CH, self.n_imp_H, self.n_chirality)
-        len_f_add = self.A * self.CH * max(self.n_imp_H, 1) * max(self.n_chirality, 1) * self.Ef
-        if (min(self.A, self.CH) < 1 or min(self.n_imp_H, self.n_chirality) < 0 or max(counts) > 255
-                or sum(counts) != self.F or len_f_add != C.len_f_add_per_node):
-            raise ValueError(
-                f"inconsistent action layout: n_atom_types={self.A}, n_formal_charge={self.CH}, n_imp_H={self.n_imp_H}, "
-                f"n_chirality={self.n_chirality} (each <= 255; 0 = segment absent) need n_node_features = {sum(counts)} "
-                f"and len_f_add_per_node = {len_f_add}, the constants have {self.F} and {C.len_f_add_per_node} "
-                "(graphinvent_b200.config.layout_dims derives them from the reference's flags)")
         self.apd = self.N * (C.len_f_add_per_node + C.len_f_conn_per_node) + 1
         self.rounds = 0
         self._allocate()

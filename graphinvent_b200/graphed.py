@@ -49,6 +49,11 @@ The RL rollout of `Workflow.learning_step` as replays of captured rounds (`Graph
 Each rollout keeps only the int8 input of every round; `loss.backward()` recomputes each round's forward before its
 backward, one captured backward round per model that needs gradients.
 
+The likelihood of molecules under a model, p(action | state) over each molecule's decoding route, as replays of one
+captured fill -> K0 -> forward -> probability graph per batch of route states (`RouteScorer`):
+
+    lik, offsets, nll, final = graphinvent_b200.graphed.RouteScorer(model, batch_size=1000).score(nodes, edges)
+
 Matmul precision: each of these objects reads torch's float32 matmul precision once, at construction
 (`config.tf32_enabled`, exposed as its `tf32` attribute), and bakes it into its graphs -- single-pass TF32 GEMMs when
 the user allowed TF32, 3xTF32 otherwise -- as torch's own captured cuBLAS calls keep the math mode of their capture.
@@ -71,7 +76,9 @@ loss gradient is multiplied by the scaler's scale inside the fused loss, a check
 """
 import ctypes
 import types
+from collections import namedtuple
 
+import numpy as np
 import torch
 
 from . import functional as F
@@ -1010,3 +1017,178 @@ class GraphedGeneratorRL(GraphedGenerator):
         prior_ll = torch.log(torch.sum(lik_b, dim=1)[:B])
         graphs = (self.generated_nodes[:B].clone(), self.generated_edges[:B].clone(), self.generated_n_nodes[:B].clone())
         return graphs, agent_ll, prior_ll, self.properly_terminated[:B].clone()
+
+
+# ---- the likelihood of a molecule's decoding route -------------------------------------------------------------
+RouteScores = namedtuple("RouteScores", "likelihoods offsets nll final")
+RouteScores.__doc__ = """What `RouteScorer.score` returns, all device tensors:
+likelihoods float32 [S]: p(action | state) of every route state; molecule m's are likelihoods[offsets[m]:offsets[m+1]],
+    n_edges + 2 of them, in build order (the empty graph with its first "add" action first, the full graph with the
+    terminate action last), the order the generator records its rounds in
+offsets int64 [M + 1]
+nll float32 [M]: -sum(log p) over the molecule's states, accumulated in fp64 in build order and rounded once
+final float32 [M]: log(sum p), GraphGenerator.sample's `final` convention (GraphGenerator.py:81-83), in fp64 likewise"""
+
+
+ROUTE_MIN_BATCH = 256        # rows from which the forward GEMMs take the tensor-core kernel (csrc/gemm_simt.cu)
+
+
+def route_entry_capacity(batch_size, max_n_nodes, n_edge_features):
+    """bond entries a batch of route states can hand to the model: a state holds a subset of a valid molecule's bonds,
+    at most N (N - 1) / 2 of them with one type each, two `edges` non-zeros per bond"""
+    B, N, Ef = int(batch_size), int(max_n_nodes), int(n_edge_features)
+    return max(1, min(B * N * (N - 1), B * N * N * Ef))
+
+
+def _int8_stack(x, name, ndim):
+    t = torch.from_numpy(np.ascontiguousarray(x)) if isinstance(x, np.ndarray) else x
+    if not isinstance(t, torch.Tensor) or t.dtype != torch.int8 or t.dim() != ndim:
+        raise ValueError(f"{name} must be an int8 numpy array or torch tensor of {ndim} dims (nodes [M, N, F], edges "
+                         f"[M, N, N, Ef]), got {getattr(t, 'dtype', type(t).__name__)} "
+                         f"{tuple(getattr(t, 'shape', ()))}")
+    return t.contiguous()
+
+
+class RouteScorer:
+    """The likelihood of molecules under a model: for every state of each molecule's decoding route (the states
+    `PreprocessingGraph.get_decoding_route_state` walks, MolecularGraph.py:676-732), p(action | state) =
+    softmax(model(state))[action], the probability the generator gives the action that rebuilds the molecule.
+
+        scorer = graphinvent_b200.graphed.RouteScorer(model, batch_size=1000)
+        lik, offsets, nll, final = scorer.score(nodes, edges)      # int8 [M, N, F] / [M, N, N, Ef], host or device
+
+    Per chunk of `chunk_molecules` molecules: one upload, `gib_route_plan` (the training-set construction's route
+    kernels: each state's action, node count and the step at which each bond goes; one status read), then
+    ceil(S / batch_size) replays of ONE captured graph -- `gib_route_fill` (the next batch_size states into the int8
+    static inputs, the batch index in device memory), K0 in capacity mode at `route_entry_capacity`, the forward,
+    `gib_route_probs` (the RL sampler's softmax reduction), the batch index advanced -- and `gib_route_reduce`.  The
+    K0 flags are OR-ed on the device and read once per chunk.
+
+    The graph holds max(batch_size, ROUTE_MIN_BATCH) states (`B`): below 256 rows the graph-level GEMMs would run on
+    the fp32 SIMT kernel instead of the tensor-core kernel, and the results would depend on the batch size in the last
+    bits.  With it, every output is bit-identical for any batch_size and chunk_molecules, from host or device input.
+
+    The layout arguments are `GraphedGenerator`'s and are checked the same way.  Molecules the route cannot take raise
+    `preprocess.groups`' ValueError, naming the first.  The model is scored as in eval mode (a dropout_p > 0 model
+    like its dropout-free twin); the matmul precision (`tf32`, `autocast_dtype`) is read at construction and baked
+    into the graph; the weights are repacked once per `score()` when a parameter changed."""
+
+    def __init__(self, model, batch_size, constants=None, n_atom_types=None, n_formal_charge=None, n_imp_H=None,
+                 n_chirality=None, chunk_molecules=4096, device=None):
+        from .generation import action_layout
+        from ._lib import PP_STATUS_INTS, PPDims
+        C, A, CH, H, X = action_layout(model, constants, n_atom_types, n_formal_charge, n_imp_H, n_chirality)
+        if not hasattr(model, "dims"):
+            raise TypeError("RouteScorer runs this package's models (graphinvent_b200.gnn.mpnn) only")
+        self.model, self.constants = model, C
+        self.batch_size = int(batch_size)
+        if self.batch_size < 1:
+            raise ValueError(f"batch_size must be >= 1, got {batch_size}")
+        # the captured batch: from ROUTE_MIN_BATCH rows on, every GEMM of the forward whose kernel depends on its row
+        # count runs on the tensor-core kernel, so each state's logits do not depend on the batch size
+        self.B = B = max(self.batch_size, ROUTE_MIN_BATCH)
+        self.params = _static_dims(self, model, B, 1)
+        self.dev = dev = torch.device(device) if device is not None else self.params[0].device
+        self.N, self.F, self.Ef = N, F_, Ef = C.max_n_nodes, C.n_node_features, C.n_edge_features
+        self.apd = N * (C.len_f_add_per_node + C.len_f_conn_per_node) + 1
+        self.chunk = chunk = max(1, int(chunk_molecules))
+        self.pp = PPDims(N=N, F=F_, Ef=Ef, n_atom_types=A, n_formal_charge=CH, n_imp_H=H, n_chirality=X, batch_size=B)
+        pd = ctypes.byref(self.pp)
+        ws_bytes, max_states = lib.gib_route_plan_ws_bytes(pd, chunk), lib.gib_route_max_states(pd, chunk)
+        if ws_bytes == 0 or max_states < 0 or lib.gib_preprocess_apd_length(pd) != self.apd:
+            raise ValueError(f"RouteScorer: {lib.gib_last_error().decode()}")
+        i8, i32 = torch.int8, torch.int32
+        self.in_nodes = torch.zeros(chunk, N, F_, dtype=i8, device=dev)
+        self.in_edges = torch.zeros(chunk, N, N, Ef, dtype=i8, device=dev)
+        self.plan_ws = torch.empty(ws_bytes, dtype=_u8, device=dev)
+        self.offsets = torch.zeros(chunk + 1, dtype=i32, device=dev)
+        # [5] the chunk's state count, [6] the captured graph's batch index (gib_route_plan zeroes it)
+        self.status = torch.zeros(PP_STATUS_INTS, dtype=i32, device=dev)
+        self.slots = torch.zeros(2 * B, dtype=i32, device=dev)
+        self.ctl = torch.zeros(2, dtype=i32, device=dev)
+        self.lik = torch.zeros(max_states, dtype=torch.float32, device=dev)
+        self.nodes, self.edges, _ = _static_inputs(self.d, dev)
+        self.capacity = route_entry_capacity(B, N, Ef)
+        self.cws, self.gbuf, self.hdr_np, self.hdr, self.ws, self.workspace_bytes = _model_buffers(
+            self.d, self.edges, self.capacity)
+        self.packed = torch.empty(lib.gib_model_packed_bytes(ctypes.byref(self.d)), dtype=_u8, device=dev)
+        self.logits = torch.empty(B, self.apd, dtype=torch.float32, device=dev)
+        self._flags = torch.zeros(1, dtype=i32, device=dev)
+        self._hdr_flags = self.cws[: HDR_INTS * 4].view(torch.int32)[HDR_FLAGS:HDR_FLAGS + 1]
+        self._packed_key = None
+        self.graph = None
+        self.replays = 0
+
+    def _pack(self):
+        params = list(self.model.parameters())
+        key = F._weights_key(self.d.tf32, params)
+        if key == self._packed_key:
+            return
+        if len(params) != len(self.params) or any(p.shape != q.shape for p, q in zip(params, self.params)):
+            raise RuntimeError("the model's parameter table changed after the RouteScorer was built")
+        F._require_cuda(*params)
+        check(lib.gib_model_pack(ctypes.byref(self.d), F._ptr_table(params), F._ptr(self.packed), F._stream(self.dev)),
+              "gib_model_pack")
+        self.params = params
+        self._packed_key = key
+
+    def _enqueue(self):
+        st = F._stream(self.dev)
+        check(lib.gib_route_fill(ctypes.byref(self.pp), F._ptr(self.in_nodes), F._ptr(self.in_edges), self.chunk,
+                                 F._ptr(self.plan_ws), F._ptr(self.offsets), F._ptr(self.status), F._ptr(self.ctl),
+                                 F._ptr(self.slots), F._ptr(self.nodes), F._ptr(self.edges), st), "gib_route_fill")
+        _k0_forward(self, self.nodes, self.edges, [(self.packed, self.logits)], st)
+        self._flags.bitwise_or_(self._hdr_flags)
+        check(lib.gib_route_probs(self.B, self.apd, F._ptr(self.logits), F._ptr(self.slots), F._ptr(self.lik), st),
+              "gib_route_probs")
+        check(lib.gib_rl_next_round(F._ptr(self.status[6:7]), st), "gib_rl_next_round")
+
+    def capture(self):
+        """the warm-up runs on the zeroed plan (no state): it writes zero rows and no likelihood"""
+        self.graph, = _capture(self.dev, [self._enqueue])
+
+    @torch.no_grad()
+    def score(self, nodes, edges):
+        """`RouteScores` of the molecules nodes [M, N, F] / edges [M, N, N, Ef]: int8 numpy arrays or torch tensors on
+        the host or the device, padded graphs in decoding order (what `preprocess.stacks` makes of the reference's
+        `PreprocessingGraph`s, or a generator's generated_nodes / generated_edges `.to(torch.int8)`)"""
+        from .preprocess import refuse_bad
+        nodes, edges = _int8_stack(nodes, "nodes", 3), _int8_stack(edges, "edges", 4)
+        M = nodes.shape[0]
+        if tuple(nodes.shape[1:]) != (self.N, self.F) or tuple(edges.shape) != (M, self.N, self.N, self.Ef):
+            raise ValueError(f"nodes {tuple(nodes.shape)} / edges {tuple(edges.shape)} do not fit the scorer's "
+                             f"[M, {self.N}, {self.F}] / [M, {self.N}, {self.N}, {self.Ef}]")
+        dev, f32 = self.dev, torch.float32
+        nll, final = torch.empty(M, dtype=f32, device=dev), torch.empty(M, dtype=f32, device=dev)
+        pieces, offs, base = [], [], 0
+        if M:
+            self._pack()
+            if self.graph is None:
+                self.capture()
+        st = F._stream(self.dev)
+        pd = ctypes.byref(self.pp)
+        for pos in range(0, M, self.chunk):
+            stop = min(pos + self.chunk, M)
+            n = stop - pos
+            self.in_nodes[:n].copy_(nodes[pos:stop])
+            self.in_edges[:n].copy_(edges[pos:stop])
+            check(lib.gib_route_plan(pd, F._ptr(self.in_nodes), F._ptr(self.in_edges), n, self.chunk,
+                                     F._ptr(self.plan_ws), F._ptr(self.offsets), F._ptr(self.status), st),
+                  "gib_route_plan")
+            status = self.status.cpu().numpy()
+            refuse_bad(status, pos, stop)
+            S = int(status[5])
+            self._flags.zero_()
+            for _ in range(-(-S // self.B)):
+                self.graph.replay()
+            self.replays += -(-S // self.B)
+            check(lib.gib_route_reduce(n, F._ptr(self.offsets), F._ptr(self.lik), F._ptr(nll[pos:]),
+                                       F._ptr(final[pos:]), st), "gib_route_reduce")
+            pieces.append(self.lik[:S].clone())
+            offs.append(self.offsets[:n].to(torch.int64) + base)
+            base += S
+            _check_flags(int(self._flags.item()), self.d, f"a batch of route states held more than {self.capacity} "
+                         "bond entries: the static entry capacity is wrong, the scores are invalid")
+        offs.append(torch.full((1,), base, dtype=torch.int64, device=dev))
+        lik = torch.cat(pieces) if pieces else torch.zeros(0, dtype=f32, device=dev)
+        return RouteScores(lik, torch.cat(offs), nll, final)

@@ -45,6 +45,14 @@ _REASONS = ((PP_BAD_NODES, "a node row that is not one-hot per segment with 0/1 
             (PP_DISCONNECTED, "a decoding route that disconnects (the reference's truncate_graph raises)"))
 
 
+def refuse_bad(status, start, stop):
+    """raises the ValueError naming the first bad molecule of the chunk [start, stop) whose status words (GIB_PP_*
+    flags in [3], the molecule in [4]) are `status`"""
+    if status[3]:
+        why = "; ".join(r for bit, r in _REASONS if status[3] & bit)
+        raise ValueError(f"molecule {start + int(status[4])} (or a later one in molecules [{start}, {stop})): {why}")
+
+
 def _ptr(t):
     return ctypes.c_void_p(t.data_ptr())
 
@@ -130,9 +138,7 @@ def groups(nodes, edges, batch_size, n_atom_types, n_formal_charge, n_imp_H=0, n
                                                       ctypes.c_void_p(stream.cuda_stream)),
                   "gib_preprocess_group_statistics")
         st = status.cpu().numpy()
-        if st[3]:
-            why = "; ".join(r for bit, r in _REASONS if st[3] & bit)
-            raise ValueError(f"molecule {pos + int(st[4])} (or a later one in molecules [{pos}, {stop})): {why}")
+        refuse_bad(st, pos, stop)
         ng, nxt, rows = int(st[0]), int(st[1]), int(st[2])
         if ng == 0:
             raise RuntimeError("gib_preprocess_chunk completed no group")

@@ -608,6 +608,36 @@ int gib_preprocess_group_statistics(const gib_pp_dims* d, const signed char* nod
                                     int n_molecules, int max_molecules, const int* groups, const int* status,
                                     void* ws, int* out, gib_stream stream);
 
+/* ---- the likelihood of a molecule's decoding route (graphinvent_b200.graphed.RouteScorer): for every route state,
+ *      p(action | state) = softmax(model(state))[action], one chunk of molecules at a time.
+ * gib_route_plan: the decoding routes of a chunk, by the count / scan / route kernels of gib_preprocess_chunk (same
+ * input contract, dims and limits; d->batch_size is the scorer's batch B).  Writes offsets [n_molecules + 1] (the
+ * molecules' first state; offsets[n] = S, the chunk's states) and the per-state plan in ws, and status int32
+ * [GIB_PP_STATUS_INTS]: [3] GIB_PP_* flags, [4] first bad molecule (INT_MAX: none), [5] S, [6] = 0, the fill cursor;
+ * the other words are 0.  A chunk with a bad molecule has no valid plan.  ws: gib_route_plan_ws_bytes, may hold
+ * anything.  gib_route_max_states: the most states a chunk of max_molecules molecules can have (< 0: bad dims).
+ * gib_route_fill: states [c*B, c*B + B) of the chunk, c = status[6], into out_nodes [B, N, F] / out_edges [B, N, N, Ef]
+ * int8 (state k of a molecule: node rows below its node count, the bonds the route still holds at step k), zero rows
+ * past S; ctl->live = the states it wrote; slots int32 [2B]: each slot's action, then its place in the chunk's
+ * likelihood buffer (-1 / -1 for a zero row).  A molecule's places run offsets[m] .. offsets[m+1]-1 in BUILD order:
+ * the empty graph first, the full graph with the terminate action last.  Advance the cursor with
+ * gib_rl_next_round(status + 6).  Reads only what gib_route_plan wrote for this chunk, from the same nodes / edges;
+ * nodes, edges and both outputs 16-byte aligned.
+ * gib_route_probs: likelihoods[slots[B+b]] = softmax(logits[b])[slots[b]] for every slot with slots[B+b] >= 0, by
+ * the softmax reduction of the RL sampler (bit for bit the probability gib_rl_sample_round records for that row).
+ * gib_route_reduce: per molecule m < n_molecules, over likelihoods[offsets[m] .. offsets[m+1]) in order, in fp64:
+ * nll[m] = -sum log p and final[m] = log(sum p), each rounded once to fp32. */
+size_t gib_route_plan_ws_bytes(const gib_pp_dims* d, int max_molecules);
+long long gib_route_max_states(const gib_pp_dims* d, int max_molecules);
+int gib_route_plan(const gib_pp_dims* d, const signed char* nodes, const signed char* edges, int n_molecules,
+                   int max_molecules, void* ws, int* offsets, int* status, gib_stream stream);
+int gib_route_fill(const gib_pp_dims* d, const signed char* nodes, const signed char* edges, int max_molecules,
+                   const void* ws, const int* offsets, const int* status, gib_batch_ctl* ctl, int* slots,
+                   signed char* out_nodes, signed char* out_edges, gib_stream stream);
+int gib_route_probs(int B, int apd, const float* logits, const int* slots, float* likelihoods, gib_stream stream);
+int gib_route_reduce(int n_molecules, const int* offsets, const float* likelihoods, float* nll, float* final_,
+                     gib_stream stream);
+
 /* ---- measurement hooks: CUDA-event timing per kernel class on the launching stream.
  *      class 0 = forward/dX launches of the tensor-core kernel, 1 = its weight-gradient launches, 2 = scatter-aggregate (K2),
  *      3 / 4 = forward/dX and weight-gradient GEMMs on the fp32 SIMT kernels.  GIB_PROFILE_CLASSES entries per array.
