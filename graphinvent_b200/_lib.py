@@ -157,6 +157,8 @@ _PROTOS = {
     "gib_route_fill": (c_i, [c_p, c_p, c_p, c_i] + [c_p] * 8),
     "gib_route_probs": (c_i, [c_i, c_i, c_p, c_p, c_p, c_p]),
     "gib_route_reduce": (c_i, [c_i] + [c_p] * 5),
+    "gib_route_grad_coef": (c_i, [c_i] + [c_p] * 7),
+    "gib_route_dlogits": (c_i, [c_i, c_i] + [c_p] * 6),
     "gib_profile_enable": (None, [c_i]),
     "gib_launch_count": (c_ll, []),
     "gib_profile_collect": (c_i, [c_p, c_p, c_p]),

@@ -745,6 +745,34 @@ __global__ void route_reduce_kernel(int n, const int* __restrict__ off, const fl
   fin[m] = (float)log(s);
 }
 
+// the backward of route_probs + route_reduce in log p, one warp per molecule: coef[s] = dL/d log p_s =
+// g_lik[s] p_s - g_nll[m] + g_final[m] p_s / sum p, with sum p summed in fp64 in build order as route_reduce sums it
+// (lane 0), each coefficient evaluated in fp64 and rounded once.  A null gradient counts as zero.
+constexpr int kCoefWarps = 4;
+__global__ void __launch_bounds__(32 * kCoefWarps) route_grad_coef_kernel(int n, const int* __restrict__ off,
+                                                                          const float* __restrict__ lik,
+                                                                          const float* __restrict__ g_lik,
+                                                                          const float* __restrict__ g_nll,
+                                                                          const float* __restrict__ g_fin,
+                                                                          float* __restrict__ coef) {
+  const int m = blockIdx.x * kCoefWarps + threadIdx.x / 32, lane = threadIdx.x & 31;
+  if (m >= n) return;
+  const int a = off[m], e = off[m + 1];
+  const double gn = g_nll ? (double)g_nll[m] : 0.0;
+  const double gf = g_fin ? (double)g_fin[m] : 0.0;
+  double s = 0.0;
+  if (gf != 0.0 && lane == 0)
+    for (int i = a; i < e; ++i) s += (double)lik[i];
+  s = __shfl_sync(0xffffffffu, s, 0);
+  for (int i = a + lane; i < e; i += 32) {
+    const double p = (double)lik[i];
+    double c = -gn;
+    if (g_lik) c += (double)g_lik[i] * p;
+    if (gf != 0.0) c += gf * p / s;
+    coef[i] = (float)c;
+  }
+}
+
 bool aligned16(const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15) == 0; }
 
 int route_limits(const char* who, const gib_pp_dims* d, int max_molecules, PP* p) {
@@ -902,6 +930,19 @@ int gib_route_reduce(int n_molecules, const int* offsets, const float* likelihoo
   }
   route_reduce_kernel<<<ceil_div(n_molecules, 128), 128, 0, (cudaStream_t)stream>>>(n_molecules, offsets,
                                                                                     likelihoods, nll, final_);
+  GIB_LAUNCH_CHECK();
+  return 0;
+}
+
+int gib_route_grad_coef(int n_molecules, const int* offsets, const float* likelihoods, const float* g_lik,
+                        const float* g_nll, const float* g_final, float* coef, gib_stream stream) {
+  if (n_molecules < 1 || !offsets || !likelihoods || !coef) {
+    set_error("gib_route_grad_coef: need n_molecules >= 1, offsets, likelihoods and coef, got n_molecules = %d",
+              n_molecules);
+    return -1;
+  }
+  route_grad_coef_kernel<<<ceil_div(n_molecules, kCoefWarps), 32 * kCoefWarps, 0, (cudaStream_t)stream>>>(
+      n_molecules, offsets, likelihoods, g_lik, g_nll, g_final, coef);
   GIB_LAUNCH_CHECK();
   return 0;
 }

@@ -11,6 +11,8 @@
 // gib_rl_restore -> K0 -> forward -> gib_rl_dlogits -> gib_model_backward -> gib_rl_next_round, the round index in
 // device memory.  The kernels are deterministic and int8 inputs give the float inputs' logits bit for bit, so the
 // recomputed probabilities equal the rollout's.
+//
+// The route scorer's probabilities (gib_route_probs) and their backward (gib_route_dlogits) use the same softmax.
 #include <algorithm>
 
 #include "../../include/gib200.h"
@@ -84,6 +86,30 @@ __global__ void __launch_bounds__(kRowThreads) route_probs_kernel(const float* _
   row_softmax(o, apd, sm, mx, se);
   const float p = row_prob(o, apd, slots[b], mx, se);
   if (threadIdx.x == 0) lik[dst] = p;
+}
+
+// the route scorer's backward (graphed.RouteScorer): dlogits[b] = coef[dst] * (onehot(a) - softmax(logits[b])), the
+// gradient of coef * log p with the softmax of route_probs_kernel, so the recomputed p_out[dst] is the forward's p bit
+// for bit.  It never divides by p: an underflowed p = 0 (nll = inf) still gets a finite row.  Padding (dst < 0): zeros.
+__global__ void __launch_bounds__(kRowThreads) route_dlogits_kernel(const float* __restrict__ logits, int apd,
+                                                                    const int* __restrict__ slots,
+                                                                    const float* __restrict__ coef,
+                                                                    float* __restrict__ dlogits,
+                                                                    float* __restrict__ p_out) {
+  __shared__ float sm[kRowThreads / 32];
+  const int b = blockIdx.x, B = gridDim.x;
+  const int a = slots[b], dst = slots[B + b];
+  float* dl = dlogits + (size_t)b * apd;
+  if (dst < 0) {
+    for (int k = threadIdx.x; k < apd; k += kRowThreads) dl[k] = 0.f;
+    return;
+  }
+  const float* o = logits + (size_t)b * apd;
+  float mx, se;
+  row_softmax(o, apd, sm, mx, se);
+  const float g = coef[dst];
+  for (int k = threadIdx.x; k < apd; k += kRowThreads) dl[k] = g * ((k == a ? 1.f : 0.f) - expf(o[k] - mx) / se);
+  if (threadIdx.x == 0 && p_out) p_out[dst] = row_prob(o, apd, a, mx, se);
 }
 
 // one CTA per slot: float 0/1 state -> int8 model input and, for a running round, the record row state[0]
@@ -272,6 +298,17 @@ int gib_route_probs(int B, int apd, const float* logits, const int* slots, float
     return -1;
   }
   route_probs_kernel<<<B, kRowThreads, 0, ST(stream)>>>(logits, apd, slots, likelihoods);
+  GIB_LAUNCH_CHECK();
+  return 0;
+}
+
+int gib_route_dlogits(int B, int apd, const float* logits, const int* slots, const float* coef, float* dlogits,
+                      float* p_out, gib_stream stream) {
+  if (B <= 0 || apd <= 0 || !logits || !slots || !coef || !dlogits) {
+    set_error("gib_route_dlogits: bad arguments (B=%d apd=%d; logits, slots, coef and dlogits must be given)", B, apd);
+    return -1;
+  }
+  route_dlogits_kernel<<<B, kRowThreads, 0, ST(stream)>>>(logits, apd, slots, coef, dlogits, p_out);
   GIB_LAUNCH_CHECK();
   return 0;
 }

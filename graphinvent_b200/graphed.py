@@ -54,6 +54,9 @@ captured fill -> K0 -> forward -> probability graph per batch of route states (`
 
     lik, offsets, nll, final = graphinvent_b200.graphed.RouteScorer(model, batch_size=1000).score(nodes, edges)
 
+With `score(nodes, edges, requires_grad=True)` they are autograd tensors; the backward recomputes each batch's forward
+in a second captured graph, as the RL backward does.
+
 Matmul precision: each of these objects reads torch's float32 matmul precision once, at construction
 (`config.tf32_enabled`, exposed as its `tf32` attribute), and bakes it into its graphs -- single-pass TF32 GEMMs when
 the user allowed TF32, 3xTF32 otherwise -- as torch's own captured cuBLAS calls keep the math mode of their capture.
@@ -1040,6 +1043,31 @@ def route_entry_capacity(batch_size, max_n_nodes, n_edge_features):
     return max(1, min(B * N * (N - 1), B * N * N * Ef))
 
 
+class _RouteLikelihoods(torch.autograd.Function):
+    """RouteScores (likelihoods, offsets, nll, final) of one `score()` call as a function of the model's parameters;
+    the backward recomputes every batch of route states (RouteScorer._backward)"""
+
+    @staticmethod
+    def forward(ctx, scorer, nodes, edges, rec, *params):
+        ctx.set_materialize_grads(False)            # outputs the loss does not use come back as None
+        out = scorer._score(nodes, edges, rec)
+        ctx.scorer, ctx.rec = scorer, rec
+        ctx.ptrs = [p.data_ptr() for p in params]
+        ctx.save_for_backward(out.likelihoods, *params)
+        ctx.mark_non_differentiable(out.offsets)
+        return tuple(out)
+
+    @staticmethod
+    def backward(ctx, g_lik, g_off, g_nll, g_final):
+        lik, *params = ctx.saved_tensors    # autograd raises here if a parameter was modified in place since score()
+        if [p.data_ptr() for p in params] != ctx.ptrs:
+            raise RuntimeError("one of the variables needed for gradient computation has been modified by an inplace "
+                               "operation: a parameter's storage changed between RouteScorer.score() and its backward")
+        grads = ctx.scorer._backward(ctx.rec, lik, params, g_lik, g_nll, g_final)
+        return (None, None, None, None,
+                *(g if p.requires_grad else None for g, p in zip(grads, params)))
+
+
 def _int8_stack(x, name, ndim):
     t = torch.from_numpy(np.ascontiguousarray(x)) if isinstance(x, np.ndarray) else x
     if not isinstance(t, torch.Tensor) or t.dtype != torch.int8 or t.dim() != ndim:
@@ -1071,7 +1099,24 @@ class RouteScorer:
     The layout arguments are `GraphedGenerator`'s and are checked the same way.  Molecules the route cannot take raise
     `preprocess.groups`' ValueError, naming the first.  The model is scored as in eval mode (a dropout_p > 0 model
     like its dropout-free twin); the matmul precision (`tf32`, `autocast_dtype`) is read at construction and baked
-    into the graph; the weights are repacked once per `score()` when a parameter changed."""
+    into the graph; the weights are repacked once per `score()` when a parameter changed.
+
+    Training on the route likelihoods (fine-tuning on a set of molecules, or RL on molecules the agent did not just
+    sample):
+
+        out = scorer.score(nodes, edges, requires_grad=True)
+        (w * out.nll).sum().backward()                          # any function of likelihoods / nll / final
+
+    With grad enabled and a parameter requiring grad, `likelihoods`, `nll` and `final` are autograd tensors of the
+    model's parameters.  Each such call keeps a record -- a private copy of the int8 nodes / edges where they came
+    from, each chunk's state count and the forward's likelihoods -- and no activations, so several calls can wait for
+    one backward.  The backward repacks the weights, then per chunk: the upload, `gib_route_plan` again (deterministic,
+    no status read), `gib_route_grad_coef` (dL/d log p per state), and ceil(S / B) replays of ONE second captured
+    graph -- `gib_route_fill`, K0, the forward, `gib_route_dlogits`, `gib_model_backward` into one flat gradient bucket,
+    the batch index advanced.  The recomputed probabilities equal the forward's bit for bit (`lik` holds the last
+    chunk's after a backward).  It adds the backward scratch, one [B, apd] dlogits buffer, one coefficient per state
+    of a chunk and the bucket to the scorer's buffers.  A parameter modified in place, or moved, between `score()` and
+    the backward makes the backward raise, as autograd does."""
 
     def __init__(self, model, batch_size, constants=None, n_atom_types=None, n_formal_charge=None, n_imp_H=None,
                  n_chirality=None, chunk_molecules=4096, device=None):
@@ -1118,11 +1163,15 @@ class RouteScorer:
         self._packed_key = None
         self.graph = None
         self.replays = 0
+        self._bwd = None
+        self.backward_replays = 0
 
-    def _pack(self):
-        params = list(self.model.parameters())
+    def _pack(self, params=None):
+        """the model's parameters (or `params`, always repacked) into the arena when they changed"""
+        force = params is not None
+        params = list(self.model.parameters()) if params is None else list(params)
         key = F._weights_key(self.d.tf32, params)
-        if key == self._packed_key:
+        if key == self._packed_key and not force:
             return
         if len(params) != len(self.params) or any(p.shape != q.shape for p, q in zip(params, self.params)):
             raise RuntimeError("the model's parameter table changed after the RouteScorer was built")
@@ -1147,17 +1196,104 @@ class RouteScorer:
         """the warm-up runs on the zeroed plan (no state): it writes zero rows and no likelihood"""
         self.graph, = _capture(self.dev, [self._enqueue])
 
+    # ---- the captured backward batch ----------------------------------------------------------------------
+    def _enqueue_backward(self):
+        """batch status[6] of the planned chunk: fill, recompute the forward, dlogits from the coefficients (the
+        recomputed p into `lik`), accumulate the gradient into the bucket, advance the batch index"""
+        b, st = self._bwd, F._stream(self.dev)
+        check(lib.gib_route_fill(ctypes.byref(self.pp), F._ptr(self.in_nodes), F._ptr(self.in_edges), self.chunk,
+                                 F._ptr(self.plan_ws), F._ptr(self.offsets), F._ptr(self.status), F._ptr(self.ctl),
+                                 F._ptr(self.slots), F._ptr(self.nodes), F._ptr(self.edges), st), "gib_route_fill")
+        _k0_forward(self, self.nodes, self.edges, [(self.packed, self.logits)], st)
+        self._flags.bitwise_or_(self._hdr_flags)
+        check(lib.gib_route_dlogits(self.B, self.apd, F._ptr(self.logits), F._ptr(self.slots), F._ptr(b.coef),
+                                    F._ptr(b.dlogits), F._ptr(self.lik), st), "gib_route_dlogits")
+        check(lib.gib_model_backward(ctypes.byref(self.d), self.hdr, F._ptr(self.nodes), F._ptr(self.edges),
+                                     F._ptr(self.gbuf), F._ptr(self.packed), F._ptr(self.ws), F._ptr(self.logits),
+                                     F._ptr(b.dlogits), F._ptr_table(b.views), F._ptr(b.scratch), st),
+              "gib_model_backward")
+        check(lib.gib_rl_next_round(F._ptr(self.status[6:7]), st), "gib_rl_next_round")
+
+    def _ensure_backward(self):
+        """backward buffers and the captured backward batch, built by the first score() that needs gradients; the
+        warm-up runs on a zeroed status (no state): zero rows, no likelihood, a bucket the backward zeroes first"""
+        if self._bwd is not None:
+            return
+        dev = self.dev
+        b = types.SimpleNamespace()
+        b.scratch = torch.empty(lib.gib_model_bwd_scratch_bytes(ctypes.byref(self.d), self.hdr), dtype=_u8, device=dev)
+        b.dlogits = torch.empty(self.B, self.apd, dtype=torch.float32, device=dev)
+        b.coef = torch.zeros(self.lik.numel(), dtype=torch.float32, device=dev)
+        b.gflat = torch.zeros(sum(p.numel() for p in self.params), dtype=torch.float32, device=dev)
+        b.views = F._bucket_views(b.gflat, self.params)
+        self._bwd = b
+        self.status.zero_()
+        b.graph, = _capture(dev, [self._enqueue_backward])
+
+    def _backward_chunk(self, rec, c, lik, g_lik, g_nll, g_final, eager=False):
+        """chunk c of a record: upload, plan, coefficients, its batches (`eager`: the same calls without the graph)"""
+        pos, base, S = rec.chunks[c]
+        n = min(pos + self.chunk, rec.nodes.shape[0]) - pos
+        st = F._stream(self.dev)
+        self.in_nodes[:n].copy_(rec.nodes[pos:pos + n])
+        self.in_edges[:n].copy_(rec.edges[pos:pos + n])
+        check(lib.gib_route_plan(ctypes.byref(self.pp), F._ptr(self.in_nodes), F._ptr(self.in_edges), n, self.chunk,
+                                 F._ptr(self.plan_ws), F._ptr(self.offsets), F._ptr(self.status), st), "gib_route_plan")
+        part = lambda g, a, k: g[a:a + k] if g is not None else None
+        check(lib.gib_route_grad_coef(n, F._ptr(self.offsets), F._ptr(lik[base:base + S]),
+                                      F._ptr(part(g_lik, base, S)), F._ptr(part(g_nll, pos, n)),
+                                      F._ptr(part(g_final, pos, n)), F._ptr(self._bwd.coef), st), "gib_route_grad_coef")
+        for _ in range(-(-S // self.B)):
+            if eager:
+                self._enqueue_backward()
+            else:
+                self._bwd.graph.replay()
+        self.backward_replays += -(-S // self.B)
+
     @torch.no_grad()
-    def score(self, nodes, edges):
+    def _backward(self, rec, lik, params, g_lik, g_nll, g_final):
+        """gradients of sum(g_lik * likelihoods + g_nll * nll + g_final * final) of one record w.r.t. `params` (None
+        gradients count as zero), as views of a fresh bucket"""
+        b = self._bwd
+        if b is None:                               # M = 0: no state, no backward buffers
+            return F._bucket_views(torch.zeros(sum(p.numel() for p in params), device=self.dev), params)
+        g_lik, g_nll, g_final = (g.detach().contiguous().float() if g is not None else None
+                                 for g in (g_lik, g_nll, g_final))
+        self._pack(params)
+        b.gflat.zero_()
+        self._flags.zero_()
+        self.backward_replays = 0
+        for c in range(len(rec.chunks)):
+            self._backward_chunk(rec, c, lik, g_lik, g_nll, g_final)
+        self._packed_key = None                     # the next score() repacks the model's current parameters
+        _check_flags(int(self._flags.item()), self.d, f"a batch of route states held more than {self.capacity} bond "
+                     "entries: the static entry capacity is wrong, the gradients are invalid")
+        return F._bucket_views(b.gflat.clone(), params)     # a fresh bucket: autograd may keep it as .grad
+
+    def score(self, nodes, edges, requires_grad=False):
         """`RouteScores` of the molecules nodes [M, N, F] / edges [M, N, N, Ef]: int8 numpy arrays or torch tensors on
         the host or the device, padded graphs in decoding order (what `preprocess.stacks` makes of the reference's
-        `PreprocessingGraph`s, or a generator's generated_nodes / generated_edges `.to(torch.int8)`)"""
-        from .preprocess import refuse_bad
+        `PreprocessingGraph`s, or a generator's generated_nodes / generated_edges `.to(torch.int8)`).
+        `requires_grad=True`, with grad enabled and a parameter that requires grad: likelihoods, nll and final are
+        differentiable w.r.t. the model's parameters (offsets is not); otherwise plain tensors, as by default."""
         nodes, edges = _int8_stack(nodes, "nodes", 3), _int8_stack(edges, "edges", 4)
         M = nodes.shape[0]
         if tuple(nodes.shape[1:]) != (self.N, self.F) or tuple(edges.shape) != (M, self.N, self.N, self.Ef):
             raise ValueError(f"nodes {tuple(nodes.shape)} / edges {tuple(edges.shape)} do not fit the scorer's "
                              f"[M, {self.N}, {self.F}] / [M, {self.N}, {self.N}, {self.Ef}]")
+        params = list(self.model.parameters())
+        if not (requires_grad and torch.is_grad_enabled() and any(p.requires_grad for p in params)):
+            with torch.no_grad():
+                return self._score(nodes, edges)
+        # the record: private copies of the molecules where they came from, filled in with each chunk's states
+        rec = types.SimpleNamespace(nodes=nodes.clone(), edges=edges.clone(), chunks=[])
+        return RouteScores(*_RouteLikelihoods.apply(self, rec.nodes, rec.edges, rec, *params))
+
+    def _score(self, nodes, edges, rec=None):
+        """the forward of score(); `rec`: the backward record whose chunk list (first molecule, first state,
+        states) it fills, the backward graph captured"""
+        from .preprocess import refuse_bad
+        M = nodes.shape[0]
         dev, f32 = self.dev, torch.float32
         nll, final = torch.empty(M, dtype=f32, device=dev), torch.empty(M, dtype=f32, device=dev)
         pieces, offs, base = [], [], 0
@@ -1165,6 +1301,8 @@ class RouteScorer:
             self._pack()
             if self.graph is None:
                 self.capture()
+            if rec is not None:
+                self._ensure_backward()
         st = F._stream(self.dev)
         pd = ctypes.byref(self.pp)
         for pos in range(0, M, self.chunk):
@@ -1186,6 +1324,8 @@ class RouteScorer:
                                        F._ptr(final[pos:]), st), "gib_route_reduce")
             pieces.append(self.lik[:S].clone())
             offs.append(self.offsets[:n].to(torch.int64) + base)
+            if rec is not None:
+                rec.chunks.append((pos, base, S))
             base += S
             _check_flags(int(self._flags.item()), self.d, f"a batch of route states held more than {self.capacity} "
                          "bond entries: the static entry capacity is wrong, the scores are invalid")

@@ -626,7 +626,18 @@ int gib_preprocess_group_statistics(const gib_pp_dims* d, const signed char* nod
  * gib_route_probs: likelihoods[slots[B+b]] = softmax(logits[b])[slots[b]] for every slot with slots[B+b] >= 0, by
  * the softmax reduction of the RL sampler (bit for bit the probability gib_rl_sample_round records for that row).
  * gib_route_reduce: per molecule m < n_molecules, over likelihoods[offsets[m] .. offsets[m+1]) in order, in fp64:
- * nll[m] = -sum log p and final[m] = log(sum p), each rounded once to fp32. */
+ * nll[m] = -sum log p and final[m] = log(sum p), each rounded once to fp32.
+ * Backward (RouteScorer.score(..., requires_grad=True)), per chunk after a fresh gib_route_plan:
+ * gib_route_grad_coef: coef[s] = dL/d log p_s for every state s of molecule m < n_molecules,
+ *   coef[s] = g_lik[s] * p_s - g_nll[m] + g_final[m] * p_s / sum_{t in m} p_t   (p = likelihoods),
+ * the backward of gib_route_probs followed by gib_route_reduce.  sum p is taken in fp64 in build order as
+ * gib_route_reduce sums it, each coefficient in fp64 and rounded once.  Any of g_lik [S], g_nll [n], g_final [n] may
+ * be null (no gradient: zero); the g_final term is skipped for a molecule whose g_final is 0.  One warp per molecule.
+ * gib_route_dlogits: for every slot b of a gib_route_fill batch, a = slots[b], dst = slots[B + b]:
+ *   dlogits[b, :] = coef[dst] * (onehot(a) - softmax(logits[b])), and p_out[dst] = softmax(logits[b])[a] (p_out may be
+ * null); a zero row for dst < 0 (padding slots add exact zeros to the model backward).  The softmax is gib_route_probs',
+ * so p_out equals the forward's probability bit for bit.  It does not divide by p: a probability that underflows to 0
+ * in fp32 (nll = inf in the forward) still gets the finite row -g_nll * (onehot - softmax). */
 size_t gib_route_plan_ws_bytes(const gib_pp_dims* d, int max_molecules);
 long long gib_route_max_states(const gib_pp_dims* d, int max_molecules);
 int gib_route_plan(const gib_pp_dims* d, const signed char* nodes, const signed char* edges, int n_molecules,
@@ -637,6 +648,10 @@ int gib_route_fill(const gib_pp_dims* d, const signed char* nodes, const signed 
 int gib_route_probs(int B, int apd, const float* logits, const int* slots, float* likelihoods, gib_stream stream);
 int gib_route_reduce(int n_molecules, const int* offsets, const float* likelihoods, float* nll, float* final_,
                      gib_stream stream);
+int gib_route_grad_coef(int n_molecules, const int* offsets, const float* likelihoods, const float* g_lik,
+                        const float* g_nll, const float* g_final, float* coef, gib_stream stream);
+int gib_route_dlogits(int B, int apd, const float* logits, const int* slots, const float* coef, float* dlogits,
+                      float* p_out, gib_stream stream);
 
 /* ---- measurement hooks: CUDA-event timing per kernel class on the launching stream.
  *      class 0 = forward/dX launches of the tensor-core kernel, 1 = its weight-gradient launches, 2 = scatter-aggregate (K2),
