@@ -65,6 +65,12 @@ class PPDims(ctypes.Structure):
                                    "batch_size")]
 
 
+class Scaffolds(ctypes.Structure):
+    """mirror of `gib_scaffolds` (include/gib200.h): the scaffold table and the per-batch scaffold state"""
+    _fields_ = [(n, c_p) for n in ("nodes", "edges", "n_atoms", "protect", "slot_ids", "started", "gen_scaffolds")] + [
+        ("S", c_i), ("reserved", c_i)]
+
+
 PP_STATUS_INTS = 8                                                  # GIB_PP_* (include/gib200.h)
 PP_BAD_NODES, PP_BAD_EDGES, PP_EMPTY, PP_DISCONNECTED = 1, 2, 4, 8
 
@@ -134,6 +140,12 @@ _PROTOS = {
     "gib_generation_round_layout": (c_i, [c_i] * 9 + [c_p] * 11 + [c_i, c_p, c_p, c_p]),
     "gib_generation_sample_round": (c_i, [c_i] * 8 + [c_p, c_i] + [c_p] * 13 + [c_i, c_p, c_p, c_p]),
     "gib_rl_sample_round": (c_i, [c_i] * 8 + [c_p, c_p, c_i] + [c_p] * 17 + [c_i, c_p, c_p, c_p]),
+    "gib_generation_scaffold_init": (c_i, [c_i] * 4 + [c_p] * 6),
+    "gib_generation_round_scaffold": (c_i, [c_i] * 8 + [c_p, c_i] + [c_p] * 11 + [c_i, c_p, c_p, c_p]),
+    "gib_generation_sample_round_scaffold": (c_i, [c_i] * 8 + [c_p, c_p, c_i] + [c_p] * 13 + [c_i, c_p, c_p, c_p]),
+    "gib_rl_sample_round_scaffold": (c_i, [c_i] * 8 + [c_p, c_p, c_p, c_i] + [c_p] * 17 + [c_i, c_p, c_p, c_p]),
+    "gib_generation_mask_logits": (c_i, [c_i] * 4 + [c_p] * 8),
+    "gib_rl_snapshot_scaffold": (c_i, [c_i] * 2 + [c_p] * 7),
     "gib_rl_snapshot": (c_i, [c_i] * 5 + [c_p] * 9),
     "gib_rl_restore": (c_i, [c_i] * 4 + [c_p] * 6),
     "gib_rl_gather": (c_i, [c_i] * 3 + [c_p] * 6),

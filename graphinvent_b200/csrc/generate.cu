@@ -113,9 +113,9 @@ __global__ void __launch_bounds__(1024) gen_scan_kernel(int B, const int* __rest
                                                         int* __restrict__ counters,
                                                         signed char* __restrict__ properly_terminated, int cap,
                                                         const int* __restrict__ ctl, int* __restrict__ state,
-                                                        int rounds) {
-  __shared__ int s_cnt[2][1024];
-  __shared__ int s_tot[3];
+                                                        int rounds, gib_scaffolds sc) {
+  __shared__ int s_cnt[3][1024];
+  __shared__ int s_tot[4];
   if (ctl && ctl[0] < 0) return;
   const int L = ceil_div(B, 1024);
   const int lo = min(B, (int)threadIdx.x * L), hi = min(B, lo + L);
@@ -127,6 +127,8 @@ __global__ void __launch_bounds__(1024) gen_scan_kernel(int B, const int* __rest
   }
   s_cnt[0][threadIdx.x] = c_term;
   s_cnt[1][threadIdx.x] = c_inv;
+  // scaffolds: a third prefix, over every restarted slot (either class) in slot order -- its scaffold assignment
+  if (sc.slot_ids) s_cnt[2][threadIdx.x] = c_term + c_inv;
   __syncthreads();
   if (threadIdx.x == 0) {   // fixed-order serial prefix over 1024 partials (tiny)
     int run = 0;
@@ -136,6 +138,11 @@ __global__ void __launch_bounds__(1024) gen_scan_kernel(int B, const int* __rest
     for (int i = 0; i < 1024; ++i) { int v = s_cnt[1][i]; s_cnt[1][i] = run2; run2 += v; }
     s_tot[1] = run2;
     s_tot[2] = counters[0];
+    if (sc.slot_ids) {
+      int run3 = 0;
+      for (int i = 0; i < 1024; ++i) { int v = s_cnt[2][i]; s_cnt[2][i] = run3; run3 += v; }
+      s_tot[3] = sc.started[0];
+    }
   }
   __syncthreads();
   const int n_term = s_tot[0], n_inv = s_tot[1], k = s_tot[2];
@@ -148,6 +155,18 @@ __global__ void __launch_bounds__(1024) gen_scan_kernel(int B, const int* __rest
     }
     pos[b] = (p >= 0 && p < cap) ? p : (p >= 0 ? -2 : -1);   // -2: would overflow the output buffers
   }
+  if (sc.slot_ids) {
+    // each restarted slot: its old scaffold to its output row, then the next scaffold in round-robin order (each
+    // thread reads and writes only its own slots; gen_apply_kernel copies the new scaffold in)
+    int rs = s_cnt[2][threadIdx.x];
+    const int started = s_tot[3];
+    for (int b = max(lo, 1); b < hi; ++b) {
+      if (flags[b] == 0) continue;
+      const int p = pos[b];
+      if (p >= 0) sc.gen_scaffolds[p] = sc.slot_ids[b];
+      sc.slot_ids[b] = (int)(((long long)started + rs++) % sc.S);
+    }
+  }
   // properly_terminated[k : k + len(term)] = 1, where len(term) counts the dummy slot too (build_graphs :127)
   const int n_term_all = n_term + ((B > 0 && (flags[0] & 1)) ? 1 : 0);
   for (int i = threadIdx.x; i < n_term_all; i += 1024)
@@ -155,12 +174,21 @@ __global__ void __launch_bounds__(1024) gen_scan_kernel(int B, const int* __rest
   if (threadIdx.x == 0) {
     counters[1] = n_term + n_inv;
     counters[0] = k + n_term + n_inv;
+    if (sc.slot_ids) sc.started[0] = s_tot[3] + n_term + n_inv;
     if (ctl) {                        // build_graphs' loop rule: round 2N would be needed -> status 1 (round limit)
       const int next = ctl[0] + 1;
       state[0] = next;
       if (k + n_term + n_inv < B && next >= rounds) state[1] = 1;
     }
   }
+}
+
+// scaffold s of the table as float 0/1 into one slot's nodes / edges (all rows: the slot's old content is overwritten)
+__device__ __forceinline__ void load_scaffold(const gib_scaffolds& sc, int s, int NF, int NNE, float* nb, float* eb) {
+  const signed char* sn = sc.nodes + (size_t)s * NF;
+  const signed char* se = sc.edges + (size_t)s * NNE;
+  for (int i = threadIdx.x; i < NF; i += blockDim.x) nb[i] = (float)sn[i];
+  for (int i = threadIdx.x; i < NNE; i += blockDim.x) eb[i] = (float)se[i];
 }
 
 // one CTA per slot: copy-out (pre-action state), apply the action, reset, re-stamp the dummy graph
@@ -170,7 +198,8 @@ __global__ void __launch_bounds__(128) gen_apply_kernel(GenDims d, int round, co
                                                         int* __restrict__ n_nodes, float* __restrict__ likelihoods,
                                                         float* __restrict__ g_nodes, float* __restrict__ g_edges,
                                                         signed char* __restrict__ g_n_nodes,
-                                                        float* __restrict__ g_lik, const int* __restrict__ ctl) {
+                                                        float* __restrict__ g_lik, const int* __restrict__ ctl,
+                                                        gib_scaffolds sc) {
   if (ctl) {
     round = ctl[0];
     if (round < 0) return;
@@ -193,9 +222,15 @@ __global__ void __launch_bounds__(128) gen_apply_kernel(GenDims d, int round, co
       if (threadIdx.x == 0) g_n_nodes[p] = (signed char)n_nodes[b];
     }
     __syncthreads();
+    for (int i = threadIdx.x; i < d.Lw; i += 128) lb[i] = 0.f;
+    if (sc.slot_ids) {                                                // restart from the scaffold gen_scan assigned
+      const int s = sc.slot_ids[b];
+      load_scaffold(sc, s, NF, NNE, nb, eb);
+      if (threadIdx.x == 0) n_nodes[b] = sc.n_atoms[s];
+      return;
+    }
     for (int i = threadIdx.x; i < NF; i += 128) nb[i] = 0.f;          // reset_graphs :447-460
     for (int i = threadIdx.x; i < NNE; i += 128) eb[i] = 0.f;
-    for (int i = threadIdx.x; i < d.Lw; i += 128) lb[i] = 0.f;
     if (threadIdx.x == 0) n_nodes[b] = 0;
     return;
   }
@@ -223,6 +258,51 @@ __global__ void __launch_bounds__(128) gen_apply_kernel(GenDims d, int round, co
     for (int i = threadIdx.x; i < NF; i += 128) nb[i] = 1.f;
     if (threadIdx.x == 0) { eb[0] = 1.f; n_nodes[0] = 1; }
   }
+}
+
+// the scaffold start state: one CTA per slot b >= 1 (grid B - 1)
+__global__ void __launch_bounds__(128) gen_scaffold_init_kernel(int N, int F, int Ef, int Lw, gib_scaffolds sc,
+                                                                float* __restrict__ nodes, float* __restrict__ edges,
+                                                                int* __restrict__ n_nodes,
+                                                                float* __restrict__ likelihoods) {
+  const int b = blockIdx.x + 1, B = gridDim.x + 1;
+  const int NF = N * F, NNE = N * N * Ef;
+  const int s = (b - 1) % sc.S;
+  load_scaffold(sc, s, NF, NNE, nodes + (size_t)b * NF, edges + (size_t)b * NNE);
+  for (int i = threadIdx.x; i < Lw; i += 128) likelihoods[(size_t)b * Lw + i] = 0.f;
+  if (threadIdx.x == 0) {
+    n_nodes[b] = sc.n_atoms[s];
+    sc.slot_ids[b] = s;
+    if (b == 1) { sc.slot_ids[0] = -1; sc.started[0] = B - 1; }
+  }
+}
+
+// the attachment-point mask: one CTA per slot, -inf into the add blocks and connect entries whose bond_to is a
+// protected atom, and into every connect while bond_from = n - 1 is still a scaffold atom (n_nodes only grows from
+// k_s, so that is n == k_s).  Terminate is never touched, so a masked row keeps an action of non-zero probability.
+__global__ void __launch_bounds__(128) gen_mask_kernel(int N, int Ef, int apd, gib_scaffolds sc,
+                                                       const int* __restrict__ slot_ids,
+                                                       const int* __restrict__ n_nodes, const int* __restrict__ row,
+                                                       const int* __restrict__ state,
+                                                       const int* __restrict__ counters, float* __restrict__ logits) {
+  const int b = blockIdx.x, B = gridDim.x;
+  if (state && !(counters[0] < B && state[1] == 0 && state[0] >= 0 && state[0] < 2 * N)) return;
+  const size_t off = row ? (size_t)row[0] * B : 0;
+  const int s = slot_ids[off + b];
+  if (b == 0 || s < 0 || s >= sc.S) return;
+  const int k = sc.n_atoms[s], n = n_nodes[off + b];
+  const unsigned int* pm = sc.protect + (size_t)s * 4;
+  const int per_node = (apd - 1) / N - Ef, len_add = N * per_node;
+  float* o = logits + (size_t)b * apd;
+  const bool conn_all = n - 1 < k;
+  for (int i = 0; i < k; ++i) {
+    if (!((pm[i >> 5] >> (i & 31)) & 1u)) continue;
+    for (int t = threadIdx.x; t < per_node; t += 128) o[(size_t)i * per_node + t] = -INFINITY;
+    if (!conn_all)
+      for (int t = threadIdx.x; t < Ef; t += 128) o[len_add + i * Ef + t] = -INFINITY;
+  }
+  if (conn_all)
+    for (int t = threadIdx.x; t < N * Ef; t += 128) o[len_add + t] = -INFINITY;
 }
 
 }  // namespace gib
@@ -258,17 +338,19 @@ static int launch_round(const GenDims& d, int round, const int* ctl, int* state,
                         const float* likelihood, float* nodes, float* edges, int* n_nodes, float* likelihoods,
                         float* gen_nodes, float* gen_edges, signed char* gen_n_nodes, float* gen_likelihoods,
                         signed char* properly_terminated, int capacity, int* counters, void* scratch,
-                        cudaStream_t st) {
+                        cudaStream_t st, const gib_scaffolds* sc = nullptr) {
   const int B = d.B;
+  const gib_scaffolds scv = sc ? *sc : gib_scaffolds{};
   int4* rec = reinterpret_cast<int4*>(scratch);
   int* flags = reinterpret_cast<int*>(rec + B);
   int* pos = flags + B;
   gen_decode_kernel<<<ceil_div(B, 128), 128, 0, st>>>(d, action, edges, n_nodes, rec, flags, ctl);
   GIB_LAUNCH_CHECK();
-  gen_scan_kernel<<<1, 1024, 0, st>>>(B, flags, pos, counters, properly_terminated, capacity, ctl, state, d.Lw);
+  gen_scan_kernel<<<1, 1024, 0, st>>>(B, flags, pos, counters, properly_terminated, capacity, ctl, state, d.Lw,
+                                       scv);
   GIB_LAUNCH_CHECK();
   gen_apply_kernel<<<B, 128, 0, st>>>(d, round, rec, pos, likelihood, nodes, edges, n_nodes, likelihoods, gen_nodes,
-                                      gen_edges, gen_n_nodes, gen_likelihoods, ctl);
+                                      gen_edges, gen_n_nodes, gen_likelihoods, ctl, scv);
   GIB_LAUNCH_CHECK();
   return 0;
 }
@@ -277,29 +359,66 @@ static int* round_ctl(void* scratch, int B) {
   return reinterpret_cast<int*>(reinterpret_cast<int4*>(scratch) + B) + 2 * B;   // behind rec, flags and pos
 }
 
+// a scaffold table the round kernels can use; `who` names the entry point
+static int check_scaffolds(const char* who, const gib_scaffolds* sc) {
+  if (!sc || sc->S <= 0 || !sc->nodes || !sc->edges || !sc->n_atoms || !sc->slot_ids || !sc->started ||
+      !sc->gen_scaffolds) {
+    set_error("%s: the scaffold table needs S >= 1 and its nodes, edges, n_atoms, slot_ids, started and gen_scaffolds "
+              "buffers", who);
+    return -1;
+  }
+  return 0;
+}
+
+static int round_layout(int B, int N, int F, int Ef, int n_atom_types, int n_charges, int n_imp_H, int n_chirality,
+                        const gib_scaffolds* sc, int round, const int* action, const float* likelihood, float* nodes,
+                        float* edges, int* n_nodes, float* likelihoods, float* gen_nodes, float* gen_edges,
+                        signed char* gen_n_nodes, float* gen_likelihoods, signed char* properly_terminated,
+                        int capacity, int* counters, void* scratch, gib_stream stream) {
+  GIB_TRY(check_round_args(B, N, F, Ef, n_atom_types, n_charges, n_imp_H, n_chirality, round));
+  GenDims d{B, N, F, Ef, n_atom_types, n_charges, n_imp_H, n_chirality, 2 * N};
+  return launch_round(d, round, nullptr, nullptr, action, likelihood, nodes, edges, n_nodes, likelihoods, gen_nodes,
+                      gen_edges, gen_n_nodes, gen_likelihoods, properly_terminated, capacity, counters, scratch,
+                      reinterpret_cast<cudaStream_t>(stream), sc);
+}
+
 extern "C" int gib_generation_round_layout(int B, int N, int F, int Ef, int n_atom_types, int n_charges, int n_imp_H,
                                            int n_chirality, int round, const int* action, const float* likelihood,
                                            float* nodes, float* edges, int* n_nodes, float* likelihoods,
                                            float* gen_nodes, float* gen_edges, signed char* gen_n_nodes,
                                            float* gen_likelihoods, signed char* properly_terminated, int capacity,
                                            int* counters, void* scratch, gib_stream stream) {
-  GIB_TRY(check_round_args(B, N, F, Ef, n_atom_types, n_charges, n_imp_H, n_chirality, round));
-  GenDims d{B, N, F, Ef, n_atom_types, n_charges, n_imp_H, n_chirality, 2 * N};
-  return launch_round(d, round, nullptr, nullptr, action, likelihood, nodes, edges, n_nodes, likelihoods, gen_nodes,
-                      gen_edges, gen_n_nodes, gen_likelihoods, properly_terminated, capacity, counters, scratch,
-                      reinterpret_cast<cudaStream_t>(stream));
+  return round_layout(B, N, F, Ef, n_atom_types, n_charges, n_imp_H, n_chirality, nullptr, round, action, likelihood,
+                      nodes, edges, n_nodes, likelihoods, gen_nodes, gen_edges, gen_n_nodes, gen_likelihoods,
+                      properly_terminated, capacity, counters, scratch, stream);
 }
 
-extern "C" int gib_generation_sample_round(int B, int N, int F, int Ef, int n_atom_types, int n_charges, int n_imp_H,
-                                           int n_chirality, const float* logits, int apd, const float* uniforms,
-                                           int* state, int* action, float* likelihood, float* nodes, float* edges,
-                                           int* n_nodes, float* likelihoods, float* gen_nodes, float* gen_edges,
-                                           signed char* gen_n_nodes, float* gen_likelihoods,
-                                           signed char* properly_terminated, int capacity, int* counters,
-                                           void* scratch, gib_stream stream) {
+extern "C" int gib_generation_round_scaffold(int B, int N, int F, int Ef, int n_atom_types, int n_charges,
+                                             int n_imp_H, int n_chirality, const gib_scaffolds* sc, int round,
+                                             const int* action, const float* likelihood, float* nodes, float* edges,
+                                             int* n_nodes, float* likelihoods, float* gen_nodes, float* gen_edges,
+                                             signed char* gen_n_nodes, float* gen_likelihoods,
+                                             signed char* properly_terminated, int capacity, int* counters,
+                                             void* scratch, gib_stream stream) {
+  GIB_TRY(check_scaffolds("gib_generation_round_scaffold", sc));
+  return round_layout(B, N, F, Ef, n_atom_types, n_charges, n_imp_H, n_chirality, sc, round, action, likelihood,
+                      nodes, edges, n_nodes, likelihoods, gen_nodes, gen_edges, gen_n_nodes, gen_likelihoods,
+                      properly_terminated, capacity, counters, scratch, stream);
+}
+
+static long long layout_apd(int N, int Ef, int n_atom_types, int n_charges, int n_imp_H, int n_chirality) {
+  return (long long)N * n_atom_types * n_charges * (n_imp_H ? n_imp_H : 1) * (n_chirality ? n_chirality : 1) * Ef +
+         (long long)N * Ef + 1;
+}
+
+static int sample_round(int B, int N, int F, int Ef, int n_atom_types, int n_charges, int n_imp_H, int n_chirality,
+                        const gib_scaffolds* sc, const float* logits, int apd, const float* uniforms, int* state,
+                        int* action, float* likelihood, float* nodes, float* edges, int* n_nodes, float* likelihoods,
+                        float* gen_nodes, float* gen_edges, signed char* gen_n_nodes, float* gen_likelihoods,
+                        signed char* properly_terminated, int capacity, int* counters, void* scratch,
+                        gib_stream stream) {
   GIB_TRY(check_round_args(B, N, F, Ef, n_atom_types, n_charges, n_imp_H, n_chirality, 0));
-  const long long want = (long long)N * n_atom_types * n_charges * (n_imp_H ? n_imp_H : 1) *
-                         (n_chirality ? n_chirality : 1) * Ef + (long long)N * Ef + 1;
+  const long long want = layout_apd(N, Ef, n_atom_types, n_charges, n_imp_H, n_chirality);
   if (apd != want) {
     set_error("gib_generation_round: apd=%d, the action layout (N=%d A=%d CH=%d H=%d C=%d Ef=%d) has %lld actions",
               apd, N, n_atom_types, n_charges, n_imp_H, n_chirality, Ef, want);
@@ -311,19 +430,44 @@ extern "C" int gib_generation_sample_round(int B, int N, int F, int Ef, int n_at
   const RoundGate gate{state, counters, ctl, 2 * N};
   GIB_TRY(sample_actions_launch(logits, B, apd, uniforms, action, likelihood, &gate, st));
   return launch_round(d, 0, ctl, state, action, likelihood, nodes, edges, n_nodes, likelihoods, gen_nodes, gen_edges,
-                      gen_n_nodes, gen_likelihoods, properly_terminated, capacity, counters, scratch, st);
+                      gen_n_nodes, gen_likelihoods, properly_terminated, capacity, counters, scratch, st, sc);
 }
 
-extern "C" int gib_rl_sample_round(int B, int N, int F, int Ef, int n_atom_types, int n_charges, int n_imp_H,
-                                   int n_chirality, const float* logits_a, const float* logits_b, int apd,
-                                   const float* uniforms, const int* actions, int* state, int* act_rec, float* p_a,
-                                   float* p_b, int* action, float* tags, float* nodes, float* edges, int* n_nodes,
-                                   float* likelihoods, float* gen_nodes, float* gen_edges, signed char* gen_n_nodes,
-                                   float* gen_likelihoods, signed char* properly_terminated, int capacity,
-                                   int* counters, void* scratch, gib_stream stream) {
+extern "C" int gib_generation_sample_round(int B, int N, int F, int Ef, int n_atom_types, int n_charges, int n_imp_H,
+                                           int n_chirality, const float* logits, int apd, const float* uniforms,
+                                           int* state, int* action, float* likelihood, float* nodes, float* edges,
+                                           int* n_nodes, float* likelihoods, float* gen_nodes, float* gen_edges,
+                                           signed char* gen_n_nodes, float* gen_likelihoods,
+                                           signed char* properly_terminated, int capacity, int* counters,
+                                           void* scratch, gib_stream stream) {
+  return sample_round(B, N, F, Ef, n_atom_types, n_charges, n_imp_H, n_chirality, nullptr, logits, apd, uniforms,
+                      state, action, likelihood, nodes, edges, n_nodes, likelihoods, gen_nodes, gen_edges,
+                      gen_n_nodes, gen_likelihoods, properly_terminated, capacity, counters, scratch, stream);
+}
+
+extern "C" int gib_generation_sample_round_scaffold(int B, int N, int F, int Ef, int n_atom_types, int n_charges,
+                                                    int n_imp_H, int n_chirality, const gib_scaffolds* sc,
+                                                    const float* logits, int apd, const float* uniforms, int* state,
+                                                    int* action, float* likelihood, float* nodes, float* edges,
+                                                    int* n_nodes, float* likelihoods, float* gen_nodes,
+                                                    float* gen_edges, signed char* gen_n_nodes,
+                                                    float* gen_likelihoods, signed char* properly_terminated,
+                                                    int capacity, int* counters, void* scratch, gib_stream stream) {
+  GIB_TRY(check_scaffolds("gib_generation_sample_round_scaffold", sc));
+  return sample_round(B, N, F, Ef, n_atom_types, n_charges, n_imp_H, n_chirality, sc, logits, apd, uniforms, state,
+                      action, likelihood, nodes, edges, n_nodes, likelihoods, gen_nodes, gen_edges, gen_n_nodes,
+                      gen_likelihoods, properly_terminated, capacity, counters, scratch, stream);
+}
+
+static int rl_sample_round(int B, int N, int F, int Ef, int n_atom_types, int n_charges, int n_imp_H, int n_chirality,
+                           const gib_scaffolds* sc, const float* logits_a, const float* logits_b, int apd,
+                           const float* uniforms, const int* actions, int* state, int* act_rec, float* p_a,
+                           float* p_b, int* action, float* tags, float* nodes, float* edges, int* n_nodes,
+                           float* likelihoods, float* gen_nodes, float* gen_edges, signed char* gen_n_nodes,
+                           float* gen_likelihoods, signed char* properly_terminated, int capacity, int* counters,
+                           void* scratch, gib_stream stream) {
   GIB_TRY(check_round_args(B, N, F, Ef, n_atom_types, n_charges, n_imp_H, n_chirality, 0));
-  const long long want = (long long)N * n_atom_types * n_charges * (n_imp_H ? n_imp_H : 1) *
-                         (n_chirality ? n_chirality : 1) * Ef + (long long)N * Ef + 1;
+  const long long want = layout_apd(N, Ef, n_atom_types, n_charges, n_imp_H, n_chirality);
   if (apd != want || B + 1 >= (1 << 24) || !logits_a || !logits_b || (!uniforms && !actions) || !act_rec || !p_a ||
       !p_b) {
     set_error("gib_rl_sample_round: apd=%d (the action layout N=%d A=%d CH=%d H=%d C=%d Ef=%d has %lld actions), "
@@ -338,7 +482,73 @@ extern "C" int gib_rl_sample_round(int B, int N, int F, int Ef, int n_atom_types
   GIB_TRY(sample_actions_launch(logits_a, B, apd, uniforms, action, tags, &gate, st));
   GIB_TRY(rl_probs_launch(logits_a, logits_b, B, apd, action, ctl, act_rec, p_a, p_b, tags, st));
   return launch_round(d, 0, ctl, state, action, tags, nodes, edges, n_nodes, likelihoods, gen_nodes, gen_edges,
-                      gen_n_nodes, gen_likelihoods, properly_terminated, capacity, counters, scratch, st);
+                      gen_n_nodes, gen_likelihoods, properly_terminated, capacity, counters, scratch, st, sc);
+}
+
+extern "C" int gib_rl_sample_round(int B, int N, int F, int Ef, int n_atom_types, int n_charges, int n_imp_H,
+                                   int n_chirality, const float* logits_a, const float* logits_b, int apd,
+                                   const float* uniforms, const int* actions, int* state, int* act_rec, float* p_a,
+                                   float* p_b, int* action, float* tags, float* nodes, float* edges, int* n_nodes,
+                                   float* likelihoods, float* gen_nodes, float* gen_edges, signed char* gen_n_nodes,
+                                   float* gen_likelihoods, signed char* properly_terminated, int capacity,
+                                   int* counters, void* scratch, gib_stream stream) {
+  return rl_sample_round(B, N, F, Ef, n_atom_types, n_charges, n_imp_H, n_chirality, nullptr, logits_a, logits_b, apd,
+                         uniforms, actions, state, act_rec, p_a, p_b, action, tags, nodes, edges, n_nodes, likelihoods,
+                         gen_nodes, gen_edges, gen_n_nodes, gen_likelihoods, properly_terminated, capacity, counters,
+                         scratch, stream);
+}
+
+extern "C" int gib_rl_sample_round_scaffold(int B, int N, int F, int Ef, int n_atom_types, int n_charges, int n_imp_H,
+                                            int n_chirality, const gib_scaffolds* sc, const float* logits_a,
+                                            const float* logits_b, int apd, const float* uniforms, const int* actions,
+                                            int* state, int* act_rec, float* p_a, float* p_b, int* action,
+                                            float* tags, float* nodes, float* edges, int* n_nodes,
+                                            float* likelihoods, float* gen_nodes, float* gen_edges,
+                                            signed char* gen_n_nodes, float* gen_likelihoods,
+                                            signed char* properly_terminated, int capacity, int* counters,
+                                            void* scratch, gib_stream stream) {
+  GIB_TRY(check_scaffolds("gib_rl_sample_round_scaffold", sc));
+  return rl_sample_round(B, N, F, Ef, n_atom_types, n_charges, n_imp_H, n_chirality, sc, logits_a, logits_b, apd,
+                         uniforms, actions, state, act_rec, p_a, p_b, action, tags, nodes, edges, n_nodes, likelihoods,
+                         gen_nodes, gen_edges, gen_n_nodes, gen_likelihoods, properly_terminated, capacity, counters,
+                         scratch, stream);
+}
+
+extern "C" int gib_generation_scaffold_init(int B, int N, int F, int Ef, const gib_scaffolds* sc, float* nodes,
+                                            float* edges, int* n_nodes, float* likelihoods, gib_stream stream) {
+  GIB_TRY(check_scaffolds("gib_generation_scaffold_init", sc));
+  if (B <= 0 || N <= 0 || N > 127 || F <= 0 || Ef <= 0 || !nodes || !edges || !n_nodes || !likelihoods) {
+    set_error("gib_generation_scaffold_init: unsupported arguments (B=%d N=%d F=%d Ef=%d; the state buffers must be "
+              "given)", B, N, F, Ef);
+    return -1;
+  }
+  if (B == 1) {                      // only the dummy slot: started = B - 1 = 0, slot_ids[0] = -1 (all bits set)
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    GIB_CUDA_TRY(cudaMemsetAsync(sc->started, 0, sizeof(int), st));
+    GIB_CUDA_TRY(cudaMemsetAsync(sc->slot_ids, 0xff, sizeof(int), st));
+    return 0;
+  }
+  gen_scaffold_init_kernel<<<B - 1, 128, 0, reinterpret_cast<cudaStream_t>(stream)>>>(N, F, Ef, 2 * N, *sc, nodes,
+                                                                                      edges, n_nodes, likelihoods);
+  GIB_LAUNCH_CHECK();
+  return 0;
+}
+
+extern "C" int gib_generation_mask_logits(int B, int N, int Ef, int apd, const gib_scaffolds* sc, const int* slot_ids,
+                                          const int* n_nodes, const int* row, const int* state, const int* counters,
+                                          float* logits, gib_stream stream) {
+  if (!sc || sc->S <= 0 || !sc->n_atoms || B <= 0 || N <= 0 || N > 127 || Ef <= 0 || apd < 1 ||
+      (apd - 1) % N != 0 || (apd - 1) / N <= Ef || !slot_ids || !n_nodes || !logits || (!state != !counters)) {
+    set_error("gib_generation_mask_logits: bad arguments (B=%d N=%d Ef=%d apd=%d; apd - 1 must be N times the "
+              "per-node add and connect lengths, the table, slot_ids, n_nodes and logits must be given, and state "
+              "and counters together or neither)", B, N, Ef, apd);
+    return -1;
+  }
+  if (!sc->protect) return 0;       // no attachment points: nothing is masked
+  gen_mask_kernel<<<B, 128, 0, reinterpret_cast<cudaStream_t>(stream)>>>(N, Ef, apd, *sc, slot_ids, n_nodes, row,
+                                                                         state, counters, logits);
+  GIB_LAUNCH_CHECK();
+  return 0;
 }
 
 extern "C" int gib_generation_round(int B, int N, int F, int Ef, int n_atom_types, int n_charges, int round,

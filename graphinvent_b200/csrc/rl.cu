@@ -150,6 +150,18 @@ __global__ void __launch_bounds__(128) rl_snapshot_kernel(int N, int F, int Ef, 
   }
 }
 
+// the scaffold mask inputs of a running round into row state[0] of the record (gib_rl_snapshot's gate)
+__global__ void rl_snapshot_scaffold_kernel(int B, int N, const int* __restrict__ slot_ids,
+                                            const int* __restrict__ n_nodes, const int* __restrict__ state,
+                                            const int* __restrict__ counters, int* __restrict__ rec_ids,
+                                            int* __restrict__ rec_n) {
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  const int r = state[0];
+  if (b >= B || !(counters[0] < B && state[1] == 0 && r >= 0 && r < 2 * N)) return;
+  rec_ids[(size_t)r * B + b] = slot_ids[b];
+  rec_n[(size_t)r * B + b] = n_nodes[b];
+}
+
 __global__ void rl_restore_kernel(const signed char* __restrict__ rec, signed char* __restrict__ in, long long n,
                                   const int* __restrict__ ctl) {
   const signed char* src = rec + (long long)ctl[0] * n;
@@ -234,6 +246,18 @@ int gib_rl_snapshot(int B, int N, int F, int Ef, int att_view, const float* node
   }
   rl_snapshot_kernel<<<B, 128, 0, ST(stream)>>>(N, F, Ef, att_view, nodes, edges, state, counters, rec_nodes,
                                                 rec_edges, in_nodes, in_edges);
+  GIB_LAUNCH_CHECK();
+  return 0;
+}
+
+int gib_rl_snapshot_scaffold(int B, int N, const int* slot_ids, const int* n_nodes, const int* state,
+                             const int* counters, int* rec_ids, int* rec_n, gib_stream stream) {
+  if (B <= 0 || N <= 0 || N > 127 || !slot_ids || !n_nodes || !state || !counters || !rec_ids || !rec_n) {
+    set_error("gib_rl_snapshot_scaffold: bad arguments (B=%d N=%d; every buffer must be given)", B, N);
+    return -1;
+  }
+  rl_snapshot_scaffold_kernel<<<(unsigned)ceil_div(B, 256), 256, 0, ST(stream)>>>(B, N, slot_ids, n_nodes, state,
+                                                                                   counters, rec_ids, rec_n);
   GIB_LAUNCH_CHECK();
   return 0;
 }

@@ -19,6 +19,13 @@ The sampler draws with inverse-CDF on `torch.rand` uniforms (same distribution a
 RNG stream); `build_graphs(replay=...)` replays recorded draws instead, which is how the parity tests pin the state
 machine bit-exactly against a trace of the unmodified reference.
 
+Scaffold decoration (`scaffolds=(nodes, edges)`, `attachment=`, `set_scaffolds`): every slot but the dummy one starts
+from a given partial graph instead of the empty one and restarts from the next scaffold in round-robin order when its
+molecule terminates; `generated_scaffolds` says which scaffold each molecule grew from.  The action space only ever
+appends, so the model, the sampler, the validity rules and the likelihood bookkeeping are unchanged: the likelihoods
+cover the decoration actions.  With attachment points, adds and connects onto the other scaffold atoms, and connects
+while the newest atom is still a scaffold atom, get logit -inf before the softmax (`ScaffoldTable`).
+
 `GraphGeneratorRL` is the twin used by the reinforcement-learning loop (reference GraphGeneratorRL.py:25-172):
 two models are evaluated on every round -- the sampling "agent" and a second model whose probability of the SAME
 action is recorded -- and, unlike plain generation, autograd runs through the whole rollout
@@ -26,10 +33,11 @@ action is recorded -- and, unlike plain generation, autograd runs through the wh
 """
 import ctypes
 
+import numpy as np
 import torch
 
 from . import functional as Fn
-from ._lib import check, lib
+from ._lib import Scaffolds, check, lib
 
 
 def _ptr(t):
@@ -57,9 +65,107 @@ def action_layout(model, constants=None, n_atom_types=None, n_formal_charge=None
     return C, A, CH, H, X
 
 
+class ScaffoldTable:
+    """The scaffolds a generator decorates, as the device table of `gib_scaffolds` (include/gib200.h).
+
+    nodes int8 [S, N', F] / edges int8 [S, N', N', Ef]: scaffold s holds k_s >= 1 atoms in rows 0..k_s-1 (N' rows, the
+    rows past the generator's N must be empty), in the format `preprocess.stacks` makes from `PreprocessingGraph`s.
+    They are checked by the training-set construction's own kernels (`preprocess.groups`), which refuse, naming the
+    first bad scaffold, a node row that is not one-hot per segment, a gap between atom rows, an edge entry that is not
+    a symmetric single-type bond, no atoms, and a graph whose decoding route disconnects -- a disconnected graph, or
+    one whose atom order the generator could not have produced, since every add bonds the new atom to an existing one.
+    The whole pass runs, not only its count stage: the count kernel's status words are read back once per chunk, after
+    the route stage, and that route stage is the check of the atom order.  For a scaffold set it is one chunk of a few
+    route states per scaffold, so it costs one small launch sequence and one read when the scaffolds are set.
+
+    attachment: None (nothing is masked; the scaffold may gain bonds anywhere), a bool [S, N'] array (True = an
+    attachment point), or one list of atom indices per scaffold.  The other atoms of scaffold s are protected: bit i
+    of `protect[s]` (4 x 32 bits, N <= 127)."""
+
+    def __init__(self, nodes, edges, attachment, N, F, Ef, layout, device):
+        from . import preprocess
+        nodes = np.ascontiguousarray(torch.as_tensor(nodes).cpu().numpy())
+        edges = np.ascontiguousarray(torch.as_tensor(edges).cpu().numpy())
+        if (nodes.ndim != 3 or edges.ndim != 4 or nodes.shape[0] < 1 or nodes.shape[2] != F or edges.shape[3] != Ef
+                or edges.shape[:3] != (nodes.shape[0], nodes.shape[1], nodes.shape[1])):
+            raise ValueError(f"scaffolds must be int8 stacks nodes [S, N, {F}] / edges [S, N, N, {Ef}] with S >= 1, "
+                             f"got {nodes.shape} / {edges.shape}")
+        if nodes.dtype != np.int8 or edges.dtype != np.int8:
+            if not (np.array_equal(nodes, nodes.astype(np.int8)) and np.array_equal(edges, edges.astype(np.int8))):
+                raise ValueError("scaffold features are not int8-exact")
+            nodes, edges = nodes.astype(np.int8), edges.astype(np.int8)
+        S, rows = nodes.shape[:2]
+        try:
+            for _ in preprocess.groups(nodes, edges, 64, *layout, device=device):
+                pass
+        except ValueError as e:
+            raise ValueError(f"invalid scaffold (molecule i below is scaffold i): {e}") from None
+        k = (nodes != 0).any(-1).sum(-1).astype(np.int32)
+        if int(k.max()) > N:
+            s = int(np.argmax(k > N))
+            raise ValueError(f"scaffold {s} holds {int(k[s])} atoms, the generator's max_n_nodes is {N}")
+        if rows > N:
+            nodes, edges = nodes[:, :N], edges[:, :N, :N]
+        elif rows < N:
+            nodes = np.pad(nodes, ((0, 0), (0, N - rows), (0, 0)))
+            edges = np.pad(edges, ((0, 0), (0, N - rows), (0, N - rows), (0, 0)))
+        self.S, self.N = S, N
+        self.n_atoms = k
+        self.n_bonds = (edges.reshape(S, -1).astype(np.int64).sum(1) // 2)
+        self.m_max = int(self.n_bonds.max())
+        self.protect_mask = None
+        if attachment is not None:
+            attach = np.zeros((S, N), bool)
+            if isinstance(attachment, (list, tuple)):
+                if len(attachment) != S:
+                    raise ValueError(f"attachment lists {len(attachment)} scaffolds, there are {S}")
+                for s, idx in enumerate(attachment):
+                    idx = np.asarray(list(idx), np.int64)
+                    if idx.size and (idx.min() < 0 or idx.max() >= k[s]):
+                        raise ValueError(f"attachment point of scaffold {s} outside its atoms 0..{int(k[s]) - 1}")
+                    attach[s, idx] = True
+            else:
+                a = np.asarray(torch.as_tensor(attachment).cpu().numpy(), bool)
+                if a.ndim != 2 or a.shape[0] != S or a.shape[1] < min(rows, N):
+                    raise ValueError(f"attachment must be a bool [S, N] array, got shape {a.shape}")
+                attach[:, :min(a.shape[1], N)] = a[:, :N]
+            self.protect_mask = (np.arange(N)[None] < k[:, None]) & ~attach
+        dev = torch.device(device)
+        self.nodes = torch.from_numpy(nodes).to(dev)
+        self.edges = torch.from_numpy(edges).to(dev)
+        self.n_atoms_dev = torch.from_numpy(k).to(dev)
+        self.protect = None
+        if self.protect_mask is not None:
+            bits = np.zeros((S, 128), bool)
+            bits[:, :N] = self.protect_mask
+            words = (bits.reshape(S, 4, 32).astype(np.uint64) << np.arange(32, dtype=np.uint64)).sum(-1)
+            self.protect = torch.from_numpy(words.astype(np.uint32).view(np.int32)).to(dev)
+
+    def copy_(self, other):
+        """`other`'s scaffolds into this table's buffers, in place (same S, attachment points given in both or in
+        neither)"""
+        self.nodes.copy_(other.nodes)
+        self.edges.copy_(other.edges)
+        self.n_atoms_dev.copy_(other.n_atoms_dev)
+        if self.protect is not None:
+            self.protect.copy_(other.protect)
+        self.n_atoms, self.n_bonds, self.protect_mask = other.n_atoms, other.n_bonds, other.protect_mask
+
+    def struct(self, slot_ids, started, gen_scaffolds):
+        """the `gib_scaffolds` of this table and the per-batch state buffers"""
+        return Scaffolds(nodes=_ptr(self.nodes).value, edges=_ptr(self.edges).value,
+                         n_atoms=_ptr(self.n_atoms_dev).value,
+                         protect=_ptr(self.protect).value if self.protect is not None else None,
+                         slot_ids=_ptr(slot_ids).value, started=_ptr(started).value,
+                         gen_scaffolds=_ptr(gen_scaffolds).value, S=self.S)
+
+
 class GraphGenerator:
+    """`scaffolds=(nodes, edges)` / `attachment=`: decorate those scaffolds instead of growing molecules from the empty
+    graph (`ScaffoldTable`; `set_scaffolds` changes them).  None (the default) keeps the reference's behaviour."""
+
     def __init__(self, model, batch_size, constants=None, n_atom_types=None, n_formal_charge=None, n_imp_H=None,
-                 n_chirality=None, device="cuda"):
+                 n_chirality=None, device="cuda", scaffolds=None, attachment=None):
         C, self.A, self.CH, self.n_imp_H, self.n_chirality = action_layout(
             model, constants, n_atom_types, n_formal_charge, n_imp_H, n_chirality)
         self.constants = C
@@ -67,7 +173,49 @@ class GraphGenerator:
         self.N, self.F, self.Ef = C.max_n_nodes, C.n_node_features, C.n_edge_features
         self.apd = self.N * (C.len_f_add_per_node + C.len_f_conn_per_node) + 1
         self.rounds = 0
+        self.scaffolds = None
+        self.generated_scaffolds = None
         self._allocate()
+        if scaffolds is not None:
+            self.set_scaffolds(scaffolds, attachment)
+
+    def _table(self, scaffolds, attachment):
+        """the ScaffoldTable of set_scaffolds' arguments (None for None)"""
+        if scaffolds is None:
+            if attachment is not None:
+                raise ValueError("attachment points need scaffolds")
+            return None
+        nodes, edges = scaffolds
+        return ScaffoldTable(nodes, edges, attachment, self.N, self.F, self.Ef,
+                             (self.A, self.CH, self.n_imp_H, self.n_chirality), self.device)
+
+    def set_scaffolds(self, scaffolds, attachment=None):
+        """decorate `scaffolds` = (nodes, edges) from the next batch on (None: grow from the empty graph again)"""
+        self.scaffolds = self._table(scaffolds, attachment)
+        self._allocate()
+
+    def _scaffold_struct(self):
+        return self.scaffolds.struct(self._slot_ids, self._started, self._gen_scaffolds)
+
+    def _scaffold_init(self, stream):
+        """the scaffold start state of slots 1..B-1 (gib_generation_scaffold_init)"""
+        self._sc = self._scaffold_struct()
+        check(lib.gib_generation_scaffold_init(self.batch_size, self.N, self.F, self.Ef, ctypes.byref(self._sc),
+                                               _ptr(self.nodes), _ptr(self.edges), _ptr(self.n_nodes),
+                                               _ptr(self.likelihoods), stream), "gib_generation_scaffold_init")
+
+    def _mask(self, logits, stream, slot_ids=None, n_nodes=None):
+        """-inf into the logits [B, apd] (in place) of the actions the attachment points forbid in this round's state"""
+        check(lib.gib_generation_mask_logits(
+            self.batch_size, self.N, self.Ef, self.apd, ctypes.byref(self._sc),
+            _ptr(slot_ids if slot_ids is not None else self._slot_ids),
+            _ptr(n_nodes if n_nodes is not None else self.n_nodes), None, None, None, _ptr(logits), stream),
+            "gib_generation_mask_logits")
+
+    @property
+    def masked(self):
+        """True when attachment points restrict the actions"""
+        return self.scaffolds is not None and self.scaffolds.protect is not None
 
     def _allocate(self):
         B, N, F, Ef, dev = self.batch_size, self.N, self.F, self.Ef, self.device
@@ -87,6 +235,10 @@ class GraphGenerator:
         self.properly_terminated = z(cap, dt=torch.int8)     # must start zeroed: the rounds only set flags to 1
         self._counters = z(2, dt=torch.int32)
         self._scratch = torch.empty(lib.gib_generation_scratch_bytes(B), dtype=torch.uint8, device=dev)
+        if getattr(self, "scaffolds", None) is not None:
+            self._slot_ids, self._started = z(B, dt=torch.int32), z(1, dt=torch.int32)
+            self._gen_scaffolds = torch.full((cap,), -1, dtype=torch.int32, device=dev)
+            self._scaffold_init(torch.cuda.current_stream(dev).cuda_stream)
 
     def _round(self, rnd, action, lik, stream):
         """one round of the device state machine; the gdb13 layout goes through `gib_generation_round`"""
@@ -94,7 +246,11 @@ class GraphGenerator:
                  _ptr(self.generated_nodes), _ptr(self.generated_edges), _ptr(self.generated_n_nodes),
                  _ptr(self.generated_likelihoods), _ptr(self.properly_terminated), self.capacity, _ptr(self._counters),
                  _ptr(self._scratch), stream)
-        if self.n_imp_H == 0 and self.n_chirality == 0:
+        if self.scaffolds is not None:
+            check(lib.gib_generation_round_scaffold(self.batch_size, self.N, self.F, self.Ef, self.A, self.CH,
+                                                    self.n_imp_H, self.n_chirality, ctypes.byref(self._sc), rnd,
+                                                    *state), "gib_generation_round_scaffold")
+        elif self.n_imp_H == 0 and self.n_chirality == 0:
             check(lib.gib_generation_round(self.batch_size, self.N, self.F, self.Ef, self.A, self.CH, rnd, *state),
                   "gib_generation_round")
         else:
@@ -141,12 +297,20 @@ class GraphGenerator:
                 lik = lik.to(self.device, torch.float32).contiguous()
             else:
                 out = self.model(*self._model_inputs(self.model))    # GraphGenerator.py:121
+                if self.masked:
+                    out = out.contiguous()
+                    self._mask(out, st)
                 action, lik = Fn.sample_actions(out, generator=generator)
             self._round(rnd, action, lik, st)
             n_generated = int(self._counters[0].item())           # the loop condition lives on the host (:118)
             rnd += 1
         self.rounds = rnd
+        self._keep_scaffold_ids()
         return n_generated
+
+    def _keep_scaffold_ids(self):
+        self.generated_scaffolds = (self._gen_scaffolds[:self.batch_size].clone() if self.scaffolds is not None
+                                    else None)
 
     def sample(self, generator=None):
         """returns (generated_nodes, generated_edges, generated_n_nodes) of the first batch_size finished molecules,
@@ -187,6 +351,7 @@ class GraphGeneratorRL(GraphGenerator):
 
     def __init__(self, model, batch_size, **kw):
         super().__init__(model, batch_size, **kw)
+        self.generated_scaffolds = None
         self.generated_agent_likelihoods = None
         self.generated_prior_likelihoods = None
 
@@ -217,6 +382,10 @@ class GraphGeneratorRL(GraphGenerator):
             graph = Fn.build_graph(agent, edges_in) if share else None
             out_a = agent(nodes_in, edges_in, graph=graph) if share else agent(nodes_in, edges_in)   # GraphGeneratorRL.py:131-132
             out_p = prior(nodes_in, edges_in, graph=graph) if share else prior(nodes_in, edges_in)
+            if self.masked:                      # the attachment mask as a detached 0 / -inf bias: softmax renormalises
+                bias = torch.zeros(B, self.apd, dtype=torch.float32, device=self.device)
+                self._mask(bias, st)
+                out_a, out_p = out_a + bias, out_p + bias
             if replay is not None:
                 try:
                     action = next(replay)
@@ -241,6 +410,7 @@ class GraphGeneratorRL(GraphGenerator):
             per_round = torch.stack(rounds_l)                                           # [rounds, B], differentiable
             g = per_round.gather(1, slot).t() * mask                                    # [2B, rounds]
             setattr(self, name, torch.nn.functional.pad(g, (0, pad)))                   # [2B, 2N] like the reference
+        self._keep_scaffold_ids()
         return n_generated
 
     def sample(self, agent_model, prior_model, generator=None, replay=None):

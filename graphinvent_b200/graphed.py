@@ -610,6 +610,17 @@ def entry_capacity(batch_size, max_n_nodes, n_edge_features):
     return min(1 + 4 * B * N, B * N * N * Ef)
 
 
+def scaffold_entry_capacity(batch_size, max_n_nodes, n_edge_features, max_scaffold_bonds):
+    """`entry_capacity` of a batch that decorates scaffolds of at most m_max = `max_scaffold_bonds` bonds: a slot
+    b >= 1 starts, and restarts after each molecule it finishes, from a scaffold of 2 * m_s <= 2 * m_max entries; from
+    then on each round adds at most two (an add into a non-empty graph or a connect; terminate and invalid actions add
+    none), and a batch runs at most 2N rounds, so it never holds more than 2 * m_max + 4N.  Slot 0 keeps its bound of
+    1 + 4N.  In all, 1 + 4N + (B - 1) * (2 * m_max + 4N) = 1 + 4 * B * N + 2 * (B - 1) * m_max, and never more than
+    `edges` has elements."""
+    B, N, Ef, m = int(batch_size), int(max_n_nodes), int(n_edge_features), int(max_scaffold_bonds)
+    return min(1 + 4 * B * N + 2 * (B - 1) * m, B * N * N * Ef)
+
+
 class GraphedGenerator(GraphGenerator):
     """`GraphGenerator` with each round a replay of one captured CUDA graph:
 
@@ -631,10 +642,17 @@ class GraphedGenerator(GraphGenerator):
     The weights are re-packed into the arena (one launch per batch, not per round) whenever a parameter's storage,
     in-place version or `functional.invalidate_packed_weights` epoch changed; the graph reads only the arena, so no
     recapture is needed for that.  Generation with recorded actions (`replay=`) stays with the eager generator; the
-    RL rollout has its own captured form, `GraphedGeneratorRL`."""
+    RL rollout has its own captured form, `GraphedGeneratorRL`.
+
+    Scaffolds (`scaffolds=`, `attachment=`, `set_scaffolds`, see `generation.ScaffoldTable`): the table is a static
+    buffer the captured round reads; each batch starts with `gib_generation_scaffold_init`, and with attachment points
+    the round masks the logits (`gib_generation_mask_logits`) between the forward and the sampler.  The entry
+    capacity is then `scaffold_entry_capacity(B, N, Ef, m_max)`.  `set_scaffolds` copies a new set into the table in
+    place when it has the same number of scaffolds, at most the bonds the capacity was sized for and attachment points
+    given in both or in neither; otherwise it reallocates and the next batch recaptures."""
 
     def __init__(self, model, batch_size, constants=None, n_atom_types=None, n_formal_charge=None, n_imp_H=None,
-                 n_chirality=None, device="cuda"):
+                 n_chirality=None, device="cuda", scaffolds=None, attachment=None):
         super().__init__(model, batch_size, constants=constants, n_atom_types=n_atom_types,
                          n_formal_charge=n_formal_charge, n_imp_H=n_imp_H, n_chirality=n_chirality, device=device)
         if not hasattr(model, "dims"):
@@ -660,6 +678,48 @@ class GraphedGenerator(GraphGenerator):
         self._packed_key = None
         self.graph = None
         self.inert_rounds = 0
+        self._scaffold_m, self.scaffold_version = 0, 0
+        if scaffolds is not None:
+            self.set_scaffolds(scaffolds, attachment)
+
+    # ---- scaffolds --------------------------------------------------------------------------------------------
+    def _set_capacity(self, capacity):
+        """K0 / forward buffers for `capacity` bond entries (the captured graphs must be captured again)"""
+        self.entry_capacity = capacity
+        self.cws, self.gbuf, self.hdr_np, self.hdr, self.ws, self.workspace_bytes = _model_buffers(
+            self.d, self._k0_edges(), capacity)
+        self._hdr_flags = self.cws[: HDR_INTS * 4].view(torch.int32)[HDR_FLAGS:HDR_FLAGS + 1]
+
+    def _k0_edges(self):
+        return self._edges_in
+
+    def _invalidate_graphs(self):
+        self.graph = None
+
+    def set_scaffolds(self, scaffolds, attachment=None):
+        """decorate `scaffolds` = (nodes, edges) from the next batch on (None: the empty graph again).  In place when
+        the new set fits the static table; otherwise the table is reallocated and the round captured again."""
+        new = self._table(scaffolds, attachment)
+        old = self.scaffolds
+        if (new is not None and old is not None and new.S == old.S and new.m_max <= self._scaffold_m
+                and (new.protect is None) == (old.protect is None)):
+            old.copy_(new)
+            self.scaffold_version += 1
+            return
+        self.scaffolds = new
+        self.scaffold_version += 1
+        self._invalidate_graphs()
+        B, N, dev = self.batch_size, self.N, self.device
+        if new is None:
+            self._scaffold_m = 0
+            self._set_capacity(entry_capacity(B, N, self.Ef))
+            return
+        self._slot_ids = torch.zeros(B, dtype=torch.int32, device=dev)
+        self._started = torch.zeros(1, dtype=torch.int32, device=dev)
+        self._gen_scaffolds = torch.full((self.capacity,), -1, dtype=torch.int32, device=dev)
+        self._sc = self._scaffold_struct()
+        self._scaffold_m = new.m_max
+        self._set_capacity(scaffold_entry_capacity(B, N, self.Ef, new.m_max))
 
     def _allocate(self):
         super()._allocate()
@@ -675,6 +735,15 @@ class GraphedGenerator(GraphGenerator):
         self.nodes[0].fill_(1.0)                    # fill_, not __setitem__: no host scalar is copied to the device
         self.edges[0, 0, 0, 0].fill_(1.0)
         self.n_nodes[0].fill_(1)
+        if self.scaffolds is not None:
+            self._gen_scaffolds.fill_(-1)
+            self._scaffold_init(F._stream(self.device))
+
+    def _mask_round(self, logits, st):
+        """the attachment mask on a captured round's logits, gated by the round state"""
+        check(lib.gib_generation_mask_logits(self.batch_size, self.N, self.Ef, self.apd, ctypes.byref(self._sc),
+                                             F._ptr(self._slot_ids), F._ptr(self.n_nodes), None, F._ptr(self._state),
+                                             F._ptr(self._counters), F._ptr(logits), st), "gib_generation_mask_logits")
 
     def _pack(self):
         self.model._check_dropout()
@@ -704,13 +773,20 @@ class GraphedGenerator(GraphGenerator):
             self._edges_in[0].copy_(e0 * (nz & (nz.to(torch.int32).cumsum(-1) == 1)).to(e0.dtype))
         _k0_forward(self, self.nodes, self._edges_in, [(self.packed, self.logits)], st)
         self._flags.bitwise_or_(self._hdr_flags)
-        check(lib.gib_generation_sample_round(
-            self.batch_size, self.N, self.F, self.Ef, self.A, self.CH, self.n_imp_H, self.n_chirality,
+        if self.scaffolds is None:
+            fn, name, sc = lib.gib_generation_sample_round, "gib_generation_sample_round", ()
+        else:
+            if self.masked:
+                self._mask_round(self.logits, st)
+            fn, name, sc = (lib.gib_generation_sample_round_scaffold, "gib_generation_sample_round_scaffold",
+                            (ctypes.byref(self._sc),))
+        check(fn(
+            self.batch_size, self.N, self.F, self.Ef, self.A, self.CH, self.n_imp_H, self.n_chirality, *sc,
             F._ptr(self.logits), self.apd, F._ptr(self.uniforms), F._ptr(self._state), F._ptr(self.action),
             F._ptr(self.lik), F._ptr(self.nodes), F._ptr(self.edges), F._ptr(self.n_nodes), F._ptr(self.likelihoods),
             F._ptr(self.generated_nodes), F._ptr(self.generated_edges), F._ptr(self.generated_n_nodes),
             F._ptr(self.generated_likelihoods), F._ptr(self.properly_terminated), self.capacity,
-            F._ptr(self._counters), F._ptr(self._scratch), st), "gib_generation_sample_round")
+            F._ptr(self._counters), F._ptr(self._scratch), st), name)
 
     def capture(self):
         self.graph, = _capture(self.device, [self._enqueue_round])
@@ -752,6 +828,7 @@ class GraphedGenerator(GraphGenerator):
         if status != 0:
             raise RuntimeError("generation needs more than 2*max_n_nodes rounds: the per-slot likelihood buffer "
                                "(GraphGenerator.py:173, 'the 2 is arbitrary') would overflow, as in the reference")
+        self._keep_scaffold_ids()
         return n_generated
 
     def sample(self, generator=None, uniforms=None):
@@ -765,12 +842,13 @@ class GraphedGenerator(GraphGenerator):
 
 
 # ---- the RL rollout -------------------------------------------------------------------------------------------
-def rl_record_bytes(batch_size, max_n_nodes, n_node_features, n_edge_features):
+def rl_record_bytes(batch_size, max_n_nodes, n_node_features, n_edge_features, masked=False):
     """device bytes one `GraphedGeneratorRL.sample()` keeps for its backward at the 2N-round limit (a rollout of R
     rounds keeps R / 2N of the per-round part): the int8 model input of every round, the action and both models'
-    probabilities per (round, slot), and the (molecule, round) -> slot map [2B, 2N] in fp32"""
+    probabilities per (round, slot), and the (molecule, round) -> slot map [2B, 2N] in fp32.  masked=True (scaffolds
+    with attachment points): also each (round, slot)'s scaffold id and atom count, int32 each"""
     B, N, F_, Ef = int(batch_size), int(max_n_nodes), int(n_node_features), int(n_edge_features)
-    per_round = B * (N * F_ + N * N * Ef) + B * (4 + 4 + 4)
+    per_round = B * (N * F_ + N * N * Ef) + B * (4 + 4 + 4) + (B * 8 if masked else 0)
     return 2 * N * per_round + 2 * B * 2 * N * 4
 
 
@@ -821,10 +899,15 @@ class GraphedGeneratorRL(GraphedGenerator):
 
     The agent and the prior must be this package's models of the generator's family with equal dims (in
     `learning_step` they are deep copies of one model); other pairs raise ValueError.  A parameter modified in place,
-    or moved, between a rollout and its backward makes the backward raise, as autograd does."""
+    or moved, between a rollout and its backward makes the backward raise, as autograd does.
+
+    With scaffolds and attachment points both models' logits are masked before `gib_rl_sample_round_scaffold`, and
+    the record also keeps each (round, slot)'s scaffold id and atom count (`gib_rl_snapshot_scaffold`), from which the
+    backward round masks the recomputed logits the same way before `gib_rl_dlogits`: the recomputed probabilities
+    still equal the rollout's.  A `set_scaffolds` between a rollout and its backward makes that backward raise."""
 
     def __init__(self, model, batch_size, constants=None, n_atom_types=None, n_formal_charge=None, n_imp_H=None,
-                 n_chirality=None, device="cuda"):
+                 n_chirality=None, device="cuda", scaffolds=None, attachment=None):
         GraphGenerator.__init__(self, model, batch_size, constants=constants, n_atom_types=n_atom_types,
                                 n_formal_charge=n_formal_charge, n_imp_H=n_imp_H, n_chirality=n_chirality,
                                 device=device)
@@ -868,6 +951,22 @@ class GraphedGeneratorRL(GraphedGenerator):
         self._bwd = None
         self.inert_rounds = 0
         self.backward_rounds = [0, 0]
+        self._scaffold_m, self.scaffold_version = 0, 0
+        if scaffolds is not None:
+            self.set_scaffolds(scaffolds, attachment)
+
+    def _k0_edges(self):
+        return self.in_edges
+
+    def _invalidate_graphs(self):
+        self.graph, self._graphs, self._bwd = None, {}, None
+
+    def set_scaffolds(self, scaffolds, attachment=None):
+        GraphedGenerator.set_scaffolds(self, scaffolds, attachment)
+        if self.masked and getattr(self, "rec_ids", None) is None:
+            B, N, dev = self.batch_size, self.N, self.device
+            self.rec_ids = torch.full((2 * N, B), -1, dtype=torch.int32, device=dev)
+            self.rec_n = torch.zeros(2 * N, B, dtype=torch.int32, device=dev)
 
     def _check_pair(self, agent, prior):
         for m in (agent, prior):
@@ -895,16 +994,27 @@ class GraphedGeneratorRL(GraphedGenerator):
                                   F._ptr(self._state), F._ptr(self._counters), F._ptr(self.rec_nodes),
                                   F._ptr(self.rec_edges), F._ptr(self.in_nodes), F._ptr(self.in_edges), st),
               "gib_rl_snapshot")
+        if self.masked:
+            check(lib.gib_rl_snapshot_scaffold(B, N, F._ptr(self._slot_ids), F._ptr(self.n_nodes), F._ptr(self._state),
+                                               F._ptr(self._counters), F._ptr(self.rec_ids), F._ptr(self.rec_n), st),
+                  "gib_rl_snapshot_scaffold")
         _k0_forward(self, self.in_nodes, self.in_edges, list(zip(self.packed, self.logits)), st)
         self._flags.bitwise_or_(self._hdr_flags)
-        check(lib.gib_rl_sample_round(
-            B, N, self.F, self.Ef, self.A, self.CH, self.n_imp_H, self.n_chirality, F._ptr(self.logits[0]),
+        if self.scaffolds is None:
+            fn, name, sc = lib.gib_rl_sample_round, "gib_rl_sample_round", ()
+        else:
+            if self.masked:
+                for logits in self.logits:
+                    self._mask_round(logits, st)
+            fn, name, sc = lib.gib_rl_sample_round_scaffold, "gib_rl_sample_round_scaffold", (ctypes.byref(self._sc),)
+        check(fn(
+            B, N, self.F, self.Ef, self.A, self.CH, self.n_imp_H, self.n_chirality, *sc, F._ptr(self.logits[0]),
             F._ptr(self.logits[1]), self.apd, F._ptr(self.uniforms), F._ptr(self.actions if self._replay else None),
             F._ptr(self._state), F._ptr(self.act_rec), F._ptr(self.p_a), F._ptr(self.p_b), F._ptr(self.action),
             F._ptr(self.lik), F._ptr(self.nodes), F._ptr(self.edges), F._ptr(self.n_nodes), F._ptr(self.likelihoods),
             F._ptr(self.generated_nodes), F._ptr(self.generated_edges), F._ptr(self.generated_n_nodes),
             F._ptr(self.generated_likelihoods), F._ptr(self.properly_terminated), self.capacity,
-            F._ptr(self._counters), F._ptr(self._scratch), st), "gib_rl_sample_round")
+            F._ptr(self._counters), F._ptr(self._scratch), st), name)
 
     # ---- the captured backward round ----------------------------------------------------------------------
     def _enqueue_backward_round(self, slot):
@@ -913,7 +1023,16 @@ class GraphedGeneratorRL(GraphedGenerator):
         check(lib.gib_rl_restore(B, self.N, self.F, self.Ef, F._ptr(self.rec_nodes), F._ptr(self.rec_edges),
                                  F._ptr(b.ctl), F._ptr(self.in_nodes), F._ptr(self.in_edges), st), "gib_rl_restore")
         _k0_forward(self, self.in_nodes, self.in_edges, [(self.packed[slot], self.logits[0])], st)
-        check(lib.gib_rl_dlogits(B, self.apd, F._ptr(self.logits[0]), F._ptr(self.act_rec), F._ptr(b.dp[slot]),
+        sampled = self.logits[0]
+        if self.masked:
+            # the rollout's mask, from the round's recorded scaffold ids and atom counts, on a copy: the model backward
+            # reads the unmasked output
+            sampled = self.logits[1]
+            sampled.copy_(self.logits[0])
+            check(lib.gib_generation_mask_logits(B, self.N, self.Ef, self.apd, ctypes.byref(self._sc),
+                                                 F._ptr(self.rec_ids), F._ptr(self.rec_n), F._ptr(b.ctl), None, None,
+                                                 F._ptr(sampled), st), "gib_generation_mask_logits")
+        check(lib.gib_rl_dlogits(B, self.apd, F._ptr(sampled), F._ptr(self.act_rec), F._ptr(b.dp[slot]),
                                  F._ptr(b.ctl), F._ptr(b.dlogits), F._ptr(self.recomputed_p[slot]), st), "gib_rl_dlogits")
         check(lib.gib_model_backward(ctypes.byref(self.d), self.hdr, F._ptr(self.in_nodes), F._ptr(self.in_edges),
                                      F._ptr(self.gbuf), F._ptr(self.packed[slot]), F._ptr(self.ws),
@@ -950,11 +1069,18 @@ class GraphedGeneratorRL(GraphedGenerator):
     def _backward(self, rec, d_a, d_b, params_a, params_b):
         """gradients of sum(d_a * agent table + d_b * prior table) w.r.t. the models given (None: frozen, skipped)"""
         B, N, R, st = self.batch_size, self.N, rec.rounds, F._stream(self.device)
+        if rec.scaffold_version != self.scaffold_version:
+            raise RuntimeError("set_scaffolds was called between an RL rollout and its backward: the backward would "
+                               "mask the recomputed logits with other scaffolds")
+        self._ensure_backward()
         b = self._bwd
         self.backward_rounds = [0, 0]
         self.rec_nodes[:R].copy_(rec.nodes)
         self.rec_edges[:R].copy_(rec.edges)
         self.act_rec[:R].copy_(rec.act)
+        if self.masked:
+            self.rec_ids[:R].copy_(rec.ids)
+            self.rec_n[:R].copy_(rec.n)
         grads = [d.contiguous().float() if ps is not None else None
                  for d, ps in ((d_a, params_a), (d_b, params_b))]
         check(lib.gib_rl_scatter_grad(B, 2 * B, 2 * N, F._ptr(rec.owner), F._ptr(grads[0]), F._ptr(grads[1]),
@@ -1008,10 +1134,12 @@ class GraphedGeneratorRL(GraphedGenerator):
         B, R = self.batch_size, self.rounds
         pa, pb = list(agent.parameters()), list(prior.parameters())
         rec = types.SimpleNamespace(owner=self.generated_likelihoods.clone(), p_a=self.p_a[:R].clone(),
-                                    p_b=self.p_b[:R].clone(), rounds=R)
+                                    p_b=self.p_b[:R].clone(), rounds=R, scaffold_version=self.scaffold_version)
         if torch.is_grad_enabled() and any(p.requires_grad for p in pa + pb):
             self._ensure_backward()
             rec.nodes, rec.edges, rec.act = self.rec_nodes[:R].clone(), self.rec_edges[:R].clone(), self.act_rec[:R].clone()
+            if self.masked:
+                rec.ids, rec.n = self.rec_ids[:R].clone(), self.rec_n[:R].clone()
             lik_a, lik_b = _RolloutLikelihoods.apply(self, rec, len(pa), *pa, *pb)
         else:
             lik_a, lik_b = self._gather(rec)

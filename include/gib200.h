@@ -475,6 +475,69 @@ int gib_generation_sample_round(int B, int N, int F, int Ef, int n_atom_types, i
                                 float* gen_likelihoods, signed char* properly_terminated, int capacity,
                                 int* counters, void* scratch, gib_stream stream);
 
+/* ---- scaffold decoration: every slot b >= 1 grows from a given partial graph instead of the empty one ----
+ * The table (device memory, read through this host struct; a captured round keeps the pointers it was captured with):
+ *   nodes int8 [S, N, F], edges int8 [S, N, N, Ef]: scaffold s holds n_atoms[s] = k_s >= 1 atoms in rows 0..k_s-1
+ *     (graphinvent_b200.generation validates them with the training-set construction's checks);
+ *   protect [S, 4]: bit i of word i / 32 set = atom i of scaffold s is a scaffold atom that is not an attachment point,
+ *     null = no attachment points (nothing is masked);
+ *   slot_ids int32 [B]: the scaffold each slot is growing from (-1 for the dummy slot 0); started int32 [1]: scaffolds
+ *     handed out so far; gen_scaffolds int32 [capacity]: the scaffold of the molecule copied out to each output row.
+ * Start: slot b >= 1 holds scaffold (b - 1) mod S, started = B - 1.  Reset: the slots that terminate in a round, in
+ * ascending slot order, restart from scaffolds (started + j) mod S, j = 0, 1, ...; started then grows by their number.
+ * Mask (gib_generation_mask_logits): an add whose bond_to is a protected atom, a connect whose bond_to is one, and
+ * every connect while bond_from = n_nodes - 1 is still a scaffold atom get logit -inf; terminate never does. */
+typedef struct gib_scaffolds {
+  const signed char* nodes;
+  const signed char* edges;
+  const int* n_atoms;
+  const unsigned int* protect;
+  int* slot_ids;
+  int* started;
+  int* gen_scaffolds;
+  int S;
+  int reserved;
+} gib_scaffolds;
+/* the start state: slots 1..B-1 of nodes / edges (float 0/1) from the table, n_nodes = k_s, likelihood rows [B, 2N]
+ * zeroed, slot_ids and started set.  Slot 0 is left as it is (slot_ids[0] = -1).  Reads nothing back: capturable. */
+int gib_generation_scaffold_init(int B, int N, int F, int Ef, const gib_scaffolds* sc, float* nodes, float* edges,
+                                 int* n_nodes, float* likelihoods, gib_stream stream);
+/* gib_generation_round_layout / gib_generation_sample_round / gib_rl_sample_round with the scaffold reset: a slot that
+ * terminates restarts from its assigned scaffold instead of the empty graph, and gen_scaffolds[p] records the scaffold
+ * of the molecule copied out to row p.  Every other output keeps its meaning. */
+int gib_generation_round_scaffold(int B, int N, int F, int Ef, int n_atom_types, int n_charges, int n_imp_H,
+                                  int n_chirality, const gib_scaffolds* sc, int round, const int* action,
+                                  const float* likelihood, float* nodes, float* edges, int* n_nodes,
+                                  float* likelihoods, float* gen_nodes, float* gen_edges, signed char* gen_n_nodes,
+                                  float* gen_likelihoods, signed char* properly_terminated, int capacity,
+                                  int* counters, void* scratch, gib_stream stream);
+int gib_generation_sample_round_scaffold(int B, int N, int F, int Ef, int n_atom_types, int n_charges, int n_imp_H,
+                                         int n_chirality, const gib_scaffolds* sc, const float* logits, int apd,
+                                         const float* uniforms, int* state, int* action, float* likelihood,
+                                         float* nodes, float* edges, int* n_nodes, float* likelihoods,
+                                         float* gen_nodes, float* gen_edges, signed char* gen_n_nodes,
+                                         float* gen_likelihoods, signed char* properly_terminated, int capacity,
+                                         int* counters, void* scratch, gib_stream stream);
+int gib_rl_sample_round_scaffold(int B, int N, int F, int Ef, int n_atom_types, int n_charges, int n_imp_H,
+                                 int n_chirality, const gib_scaffolds* sc, const float* logits_a,
+                                 const float* logits_b, int apd, const float* uniforms, const int* actions, int* state,
+                                 int* act_rec, float* p_a, float* p_b, int* action, float* tags, float* nodes,
+                                 float* edges, int* n_nodes, float* likelihoods, float* gen_nodes, float* gen_edges,
+                                 signed char* gen_n_nodes, float* gen_likelihoods, signed char* properly_terminated,
+                                 int capacity, int* counters, void* scratch, gib_stream stream);
+/* -inf in place into the forbidden entries of logits [B, apd] (apd = N * (per-node add length + Ef) + 1), from each
+ * slot's scaffold id slot_ids[b] and atom count n_nodes[b].  row != null (device int): slot_ids / n_nodes are tables
+ * [*, B] read at row row[0] (the RL backward's record).  state / counters != null: the round gate of
+ * gib_generation_sample_round -- nothing is written unless counters[0] < B, state[1] == 0 and 0 <= state[0] < 2N.
+ * A table without protect masks nothing. */
+int gib_generation_mask_logits(int B, int N, int Ef, int apd, const gib_scaffolds* sc, const int* slot_ids,
+                               const int* n_nodes, const int* row, const int* state, const int* counters,
+                               float* logits, gib_stream stream);
+/* row state[0] of rec_ids / rec_n [2N, B] = slot_ids / n_nodes [B] when the round runs (gib_rl_snapshot's rule): the
+ * per-round mask inputs the RL backward replays */
+int gib_rl_snapshot_scaffold(int B, int N, const int* slot_ids, const int* n_nodes, const int* state,
+                             const int* counters, int* rec_ids, int* rec_n, gib_stream stream);
+
 /* ---- the RL rollout (GraphGeneratorRL.py:109-172) as captured rounds, and its backward by recomputation
  *      (graphinvent_b200.graphed.GraphedGeneratorRL).  Tables indexed [round, slot] have 2N rows of B. ----
  * gib_rl_sample_round: gib_generation_sample_round with two models.  The draw comes from logits_a (row state[0] of
