@@ -73,6 +73,7 @@ class Scaffolds(ctypes.Structure):
 
 PP_STATUS_INTS = 8                                                  # GIB_PP_* (include/gib200.h)
 PP_BAD_NODES, PP_BAD_EDGES, PP_EMPTY, PP_DISCONNECTED = 1, 2, 4, 8
+ROUTE_NOT_PREFIX, ROUTE_MASKED, ROUTE_BAD_ID = 1, 2, 4                # GIB_ROUTE_* (status[1] of the conditional plan)
 
 MOL_HDR_WORDS, MOL_WORDS, MOL_ATOM_WORDS = 8, 6, 3                 # GIB_MOL_* (include/gib200.h)
 MOL_DECODES, MOL_KEY_ERROR, MOL_DUPLICATE_BOND = 1, 2, 4
@@ -171,6 +172,9 @@ _PROTOS = {
     "gib_route_reduce": (c_i, [c_i] + [c_p] * 5),
     "gib_route_grad_coef": (c_i, [c_i] + [c_p] * 7),
     "gib_route_dlogits": (c_i, [c_i, c_i] + [c_p] * 6),
+    "gib_route_plan_scaffold": (c_i, [c_p, c_p, c_p, c_i, c_i] + [c_p] * 6),
+    "gib_route_fill_scaffold": (c_i, [c_p, c_p, c_p, c_i] + [c_p] * 11),
+    "gib_route_mask_logits": (c_i, [c_i] * 4 + [c_p] * 5),
     "gib_profile_enable": (None, [c_i]),
     "gib_launch_count": (c_ll, []),
     "gib_profile_collect": (c_i, [c_p, c_p, c_p]),

@@ -32,6 +32,7 @@
 #include "../../include/gib200.h"
 #include "common.cuh"
 #include "ops.cuh"
+#include "scaffold_mask.cuh"
 
 namespace gib {
 
@@ -277,26 +278,29 @@ __global__ void __launch_bounds__(128) gen_scaffold_init_kernel(int N, int F, in
   }
 }
 
-// the attachment-point mask: one CTA per slot, -inf into the add blocks and connect entries whose bond_to is a
-// protected atom, and into every connect while bond_from = n - 1 is still a scaffold atom (n_nodes only grows from
-// k_s, so that is n == k_s).  Terminate is never touched, so a masked row keeps an action of non-zero probability.
+// the attachment-point mask (scaffold_mask.cuh): one CTA per slot, -inf into the add blocks and connect entries whose
+// bond_to is a protected atom, and into every connect while bond_from = n - 1 is still a scaffold atom (n_nodes only
+// grows from k_s, so that is n == k_s).  Terminate is never touched, so a masked row keeps an action of non-zero
+// probability.  Slots below first_slot are left alone: 1 skips the generator's dummy slot 0, 0 masks a route batch,
+// where slot 0 carries a real state.
 __global__ void __launch_bounds__(128) gen_mask_kernel(int N, int Ef, int apd, gib_scaffolds sc,
                                                        const int* __restrict__ slot_ids,
                                                        const int* __restrict__ n_nodes, const int* __restrict__ row,
                                                        const int* __restrict__ state,
-                                                       const int* __restrict__ counters, float* __restrict__ logits) {
+                                                       const int* __restrict__ counters, float* __restrict__ logits,
+                                                       int first_slot) {
   const int b = blockIdx.x, B = gridDim.x;
   if (state && !(counters[0] < B && state[1] == 0 && state[0] >= 0 && state[0] < 2 * N)) return;
   const size_t off = row ? (size_t)row[0] * B : 0;
   const int s = slot_ids[off + b];
-  if (b == 0 || s < 0 || s >= sc.S) return;
+  if (b < first_slot || s < 0 || s >= sc.S) return;
   const int k = sc.n_atoms[s], n = n_nodes[off + b];
   const unsigned int* pm = sc.protect + (size_t)s * 4;
   const int per_node = (apd - 1) / N - Ef, len_add = N * per_node;
   float* o = logits + (size_t)b * apd;
-  const bool conn_all = n - 1 < k;
+  const bool conn_all = scaffold_connects_closed(n, k);
   for (int i = 0; i < k; ++i) {
-    if (!((pm[i >> 5] >> (i & 31)) & 1u)) continue;
+    if (!scaffold_protected(pm, i)) continue;
     for (int t = threadIdx.x; t < per_node; t += 128) o[(size_t)i * per_node + t] = -INFINITY;
     if (!conn_all)
       for (int t = threadIdx.x; t < Ef; t += 128) o[len_add + i * Ef + t] = -INFINITY;
@@ -546,7 +550,22 @@ extern "C" int gib_generation_mask_logits(int B, int N, int Ef, int apd, const g
   }
   if (!sc->protect) return 0;       // no attachment points: nothing is masked
   gen_mask_kernel<<<B, 128, 0, reinterpret_cast<cudaStream_t>(stream)>>>(N, Ef, apd, *sc, slot_ids, n_nodes, row,
-                                                                         state, counters, logits);
+                                                                         state, counters, logits, 1);
+  GIB_LAUNCH_CHECK();
+  return 0;
+}
+
+extern "C" int gib_route_mask_logits(int B, int N, int Ef, int apd, const gib_scaffolds* sc, const int* slot_ids,
+                                     const int* n_nodes, float* logits, gib_stream stream) {
+  if (!sc || sc->S <= 0 || !sc->n_atoms || B <= 0 || N <= 0 || N > 127 || Ef <= 0 || apd < 1 ||
+      (apd - 1) % N != 0 || (apd - 1) / N <= Ef || !slot_ids || !n_nodes || !logits) {
+    set_error("gib_route_mask_logits: bad arguments (B=%d N=%d Ef=%d apd=%d; apd - 1 must be N times the per-node "
+              "add and connect lengths, and the table, slot_ids, n_nodes and logits must be given)", B, N, Ef, apd);
+    return -1;
+  }
+  if (!sc->protect) return 0;       // no attachment points: nothing is masked
+  gen_mask_kernel<<<B, 128, 0, reinterpret_cast<cudaStream_t>(stream)>>>(N, Ef, apd, *sc, slot_ids, n_nodes, nullptr,
+                                                                         nullptr, nullptr, logits, 0);
   GIB_LAUNCH_CHECK();
   return 0;
 }

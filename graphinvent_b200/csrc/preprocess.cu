@@ -22,6 +22,7 @@
 #include <climits>
 
 #include "common.cuh"
+#include "scaffold_mask.cuh"
 #include "../../include/gib200.h"
 
 namespace gib {
@@ -155,10 +156,12 @@ __device__ __forceinline__ void flag_bad(int* status, int flags, int m) {
   atomicMin(&status[4], m);
 }
 
-__global__ void pp_init_kernel(int* status, unsigned long long* keys, int* vals, long long table) {
+// scaffold != 0 (the conditional route plan): status[2] holds the first molecule with a GIB_ROUTE_* flag, INT_MAX
+__global__ void pp_init_kernel(int* status, unsigned long long* keys, int* vals, long long table, int scaffold) {
   if (blockIdx.x == 0 && threadIdx.x == 0) {
     status[0] = status[1] = status[2] = status[3] = status[5] = status[6] = status[7] = 0;
     status[4] = INT_MAX;
+    if (scaffold) status[2] = INT_MAX;
   }
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < table; i += (long long)gridDim.x * blockDim.x) {
     keys[i] = kEmpty;
@@ -166,10 +169,50 @@ __global__ void pp_init_kernel(int* status, unsigned long long* keys, int* vals,
   }
 }
 
+__device__ __forceinline__ void flag_scaffold(int* status, int flags, int m) {
+  atomicOr(&status[1], flags);
+  atomicMin(&status[2], m);
+}
+
+// the conditional route of molecule m decorating scaffold ids[m] (>= 0): its first k_s node rows and the edges among
+// them must equal the scaffold's (one warp, every lane gets the answer).  Returns the states kept, n_edges - m_k + 1
+// (m_k: the scaffold's bonds), or 0 with a GIB_ROUTE_* flag raised.  ids[m] = -1: the whole route, n_edges + 2.
+__device__ int conditional_length(const PP& p, const gib_scaffolds& sc, int sid, const signed char* X,
+                                  const signed char* E, int e, int m, int* status) {
+  const int lane = threadIdx.x & 31;
+  const int N = p.N, F = p.F, Ef = p.Ef;
+  if (sid < -1 || sid >= sc.S) {
+    if (lane == 0) flag_scaffold(status, GIB_ROUTE_BAD_ID, m);
+    return 0;
+  }
+  if (sid < 0) return e + 2;
+  const int k = sc.n_atoms[sid];
+  const signed char* SX = sc.nodes + (size_t)sid * N * F;
+  const signed char* SE = sc.edges + (size_t)sid * N * N * Ef;
+  bool diff = false;
+  int nnz = 0;
+  // rows 0..k-1 (a molecule of fewer atoms has a zero row there, the scaffold does not)
+  for (int q = lane; q < k * F; q += 32) diff |= X[q] != SX[q];
+  for (int q = lane; q < k * k; q += 32) {
+    const size_t ij = (size_t)(q / k) * N + q % k;
+    for (int t = 0; t < Ef; ++t) {
+      const signed char w = SE[ij * Ef + t];
+      diff |= E[ij * Ef + t] != w;
+      nnz += w != 0;
+    }
+  }
+  if (__any_sync(0xffffffffu, diff)) {
+    if (lane == 0) flag_scaffold(status, GIB_ROUTE_NOT_PREFIX, m);
+    return 0;
+  }
+  return e - warp_sum(nnz) / 2 + 1;
+}
+
 // ---- count: validation and route length (one warp per molecule) ------------------------------------------------
+// ids != null (the conditional route plan): the length is that of molecule m's conditional route
 __global__ void __launch_bounds__(32) pp_count_kernel(PP p, const signed char* __restrict__ nodes,
                                                       const signed char* __restrict__ edges, int* len, int* n0,
-                                                      int* status) {
+                                                      int* status, const int* __restrict__ ids, gib_scaffolds sc) {
   const int m = blockIdx.x, lane = threadIdx.x;
   const int N = p.N, F = p.F, Ef = p.Ef;
   const signed char* X = nodes + (size_t)m * N * F;
@@ -216,10 +259,11 @@ __global__ void __launch_bounds__(32) pp_count_kernel(PP p, const signed char* _
   nnz = warp_sum(nnz);
   bad = __reduce_or_sync(0xffffffffu, bad);
   if (n == 0) bad |= GIB_PP_EMPTY;
+  const int e = min(nnz / 2, p.s_max - 2);
+  const int kept = ids && !bad ? conditional_length(p, sc, ids[m], X, E, e, m, status) : e + 2;
   if (lane == 0) {
     if (bad) flag_bad(status, bad, m);
-    const int e = nnz / 2;
-    len[m] = bad ? 2 : min(e, p.s_max - 2) + 2;
+    len[m] = bad ? 2 : kept;
     n0[m] = n;
   }
 }
@@ -266,13 +310,21 @@ __global__ void __launch_bounds__(1024) pp_scan_kernel(int n, const int* len, in
 }
 
 // ---- route: one warp per molecule ------------------------------------------------------------------------------
+// ids != null (the conditional route plan): only the first off[m+1] - off[m] states (truncation order) are emitted --
+// the conditional route, from the full graph back to the scaffold's state -- each kept action is checked against the
+// attachment-point rule (GIB_ROUTE_MASKED), and the scaffold's bonds, which no kept step removes, get step SHRT_MAX
 __global__ void __launch_bounds__(32) pp_route_kernel(PP p, const signed char* __restrict__ nodes,
                                                       const signed char* __restrict__ edges, const int* off,
                                                       const int* n0, unsigned long long* hash, int* apd, int* nn,
-                                                      int* mol, short* rs_all, int* status) {
+                                                      int* mol, short* rs_all, int* status,
+                                                      const int* __restrict__ ids, gib_scaffolds sc) {
   extern __shared__ __align__(16) unsigned char smem[];
   if (status[3]) return;
   const int m = blockIdx.x, lane = threadIdx.x;
+  if (ids && off[m + 1] == off[m]) return;      // refused by the count stage (GIB_ROUTE_NOT_PREFIX / _BAD_ID)
+  const int sid = ids ? ids[m] : -1;
+  const unsigned int* pm = sid >= 0 && sc.protect ? sc.protect + (size_t)sid * 4 : nullptr;
+  const int ks = sid >= 0 ? sc.n_atoms[sid] : 0;
   const int N = p.N, F = p.F, Ef = p.Ef;
   const int nb = N * F, eb = N * N * Ef;
   int* sflat = reinterpret_cast<int*>(smem);
@@ -313,6 +365,7 @@ __global__ void __launch_bounds__(32) pp_route_kernel(PP p, const signed char* _
       apd[i] = a;
       nn[i] = n;
       mol[i] = m;
+      if (pm && scaffold_forbidden(a, n, ks, pm, N, Ef, p.f_add)) flag_scaffold(status, GIB_ROUTE_MASKED, m);
     }
   };
   emit(0, p.apd_len - 1);
@@ -357,6 +410,13 @@ __global__ void __launch_bounds__(32) pp_route_kernel(PP p, const signed char* _
     if (n == 1 || deg == 1) --n;
     __syncwarp();
     emit(k, a);
+  }
+  if (ids) {
+    for (int q = lane; q < N * N; q += 32) {
+      bool any = false;
+      for (int t = 0; t < Ef; ++t) any |= E[(size_t)q * Ef + t] != 0;
+      if (any) rs[q] = SHRT_MAX;
+    }
   }
 }
 
@@ -611,14 +671,17 @@ struct RouteBufs {
   int* mol;
 };
 
+// ids / sc (the conditional route plan): each molecule's route from its scaffold's state on, see pp_count_kernel
 int launch_route(const PP& p, const signed char* nodes, const signed char* edges, int n, const RouteBufs& r,
-                 int* status, cudaStream_t s) {
-  pp_count_kernel<<<n, 32, 0, s>>>(p, nodes, edges, r.len, r.n0, status);
+                 int* status, cudaStream_t s, const int* ids = nullptr, const gib_scaffolds* sc = nullptr) {
+  const gib_scaffolds scv = sc ? *sc : gib_scaffolds{};
+  pp_count_kernel<<<n, 32, 0, s>>>(p, nodes, edges, r.len, r.n0, status, ids, scv);
   GIB_LAUNCH_CHECK();
   pp_scan_kernel<<<1, 1024, 0, s>>>(n, r.len, r.off, status);
   GIB_LAUNCH_CHECK();
   const size_t smem = 4 * (size_t)p.N + (size_t)p.N * p.F + (size_t)p.N * p.N * p.Ef;
-  pp_route_kernel<<<n, 32, smem, s>>>(p, nodes, edges, r.off, r.n0, r.hash, r.apd, r.nn, r.mol, r.rs, status);
+  pp_route_kernel<<<n, 32, smem, s>>>(p, nodes, edges, r.off, r.n0, r.hash, r.apd, r.nn, r.mol, r.rs, status, ids,
+                                      scv);
   GIB_LAUNCH_CHECK();
   return 0;
 }
@@ -704,25 +767,37 @@ __device__ __forceinline__ void fill_chunk(const PP& p, const FillSrc& f, bool e
 }
 
 // states [s0, s0 + B) of the chunk, s0 = status[kCursor] * B, into the model's int8 inputs; per slot b its action and
-// its place in the likelihood buffer (build order: the molecule's empty graph first), -1 / -1 past the last state
+// its place in the likelihood buffer (build order: the molecule's empty graph first), -1 / -1 past the last state.
+// ids != null (the conditional route): also each slot's scaffold id and atom count, the mask's inputs (-1 / -1 for
+// a molecule scored whole and past the last state)
 __global__ void __launch_bounds__(kFillNT) route_fill_kernel(PP p, FillSrc f, const int* __restrict__ status,
                                                              gib_batch_ctl* ctl, int* __restrict__ slots,
                                                              signed char* __restrict__ out_nodes,
                                                              signed char* __restrict__ out_edges,
-                                                             long long node_chunks, long long edge_chunks) {
+                                                             long long node_chunks, long long edge_chunks,
+                                                             const int* __restrict__ ids, int* __restrict__ slot_ids,
+                                                             int* __restrict__ slot_n) {
   const int B = p.B, S = status[5], s0 = status[kCursor] * B;
   const long long tid = (long long)blockIdx.x * kFillNT + threadIdx.x, stride = (long long)gridDim.x * kFillNT;
   if (tid == 0) ctl->live = max(0, min(B, S - s0));
   for (long long b = tid; b < B; b += stride) {
     const int i = s0 + (int)b;
-    int a = -1, d = -1;
+    int a = -1, d = -1, sid = -1, n = -1;
     if (i < S) {
       const int m = f.mol[i];
       a = f.apd[i];
       d = f.off[m] + f.off[m + 1] - 1 - i;
+      if (ids && ids[m] >= 0) {
+        sid = ids[m];
+        n = f.nn[i];
+      }
     }
     slots[b] = a;
     slots[B + b] = d;
+    if (ids) {
+      slot_ids[b] = sid;
+      slot_n[b] = n;
+    }
   }
   for (long long c = tid; c < node_chunks + edge_chunks; c += stride) {
     if (c < node_chunks) fill_chunk(p, f, false, c, s0, S, out_nodes);
@@ -842,7 +917,7 @@ int gib_preprocess_chunk(const gib_pp_dims* d, const signed char* nodes, const s
   int* vals = (int*)(b + w.vals);
   cudaStream_t s = (cudaStream_t)stream;
   const int init_blocks = (int)(w.table / 256 < 1024 ? w.table / 256 : 1024);
-  pp_init_kernel<<<init_blocks, 256, 0, s>>>(status, keys, vals, w.table);
+  pp_init_kernel<<<init_blocks, 256, 0, s>>>(status, keys, vals, w.table, 0);
   GIB_LAUNCH_CHECK();
   GIB_TRY(launch_route(p, nodes, edges, n_molecules, RouteBufs{len, n0, off, rs, hash, apd, nn, mol}, status, s));
   const StateRef S{off, nn, mol, rs, nodes, edges};
@@ -886,7 +961,7 @@ int gib_route_plan(const gib_pp_dims* d, const signed char* nodes, const signed 
   const RouteWs w = route_ws_layout(p, max_molecules);
   char* b = static_cast<char*>(ws);
   cudaStream_t s = (cudaStream_t)stream;
-  pp_init_kernel<<<1, 32, 0, s>>>(status, nullptr, nullptr, 0);
+  pp_init_kernel<<<1, 32, 0, s>>>(status, nullptr, nullptr, 0, 0);
   GIB_LAUNCH_CHECK();
   return launch_route(p, nodes, edges, n_molecules,
                       RouteBufs{(int*)(b + w.len), (int*)(b + w.n0), offsets, (short*)(b + w.rs),
@@ -917,7 +992,65 @@ int gib_route_fill(const gib_pp_dims* d, const signed char* nodes, const signed 
   const long long need = std::max<long long>(ceil_div_ll(nc + ec, kFillNT), ceil_div_ll(p.B, kFillNT));
   const int blocks = (int)std::min<long long>(need, kFillMaxBlocks);
   route_fill_kernel<<<blocks, kFillNT, 0, (cudaStream_t)stream>>>(p, f, status, ctl, slots, out_nodes, out_edges, nc,
-                                                                  ec);
+                                                                  ec, nullptr, nullptr, nullptr);
+  GIB_LAUNCH_CHECK();
+  return 0;
+}
+
+int gib_route_plan_scaffold(const gib_pp_dims* d, const signed char* nodes, const signed char* edges, int n_molecules,
+                            int max_molecules, const gib_scaffolds* sc, const int* scaffold_ids, void* ws,
+                            int* offsets, int* status, gib_stream stream) {
+  PP p;
+  GIB_TRY(route_limits("gib_route_plan_scaffold", d, max_molecules, &p));
+  if (n_molecules < 1 || n_molecules > max_molecules) {
+    set_error("gib_route_plan_scaffold: n_molecules %d outside [1, max_molecules = %d]", n_molecules, max_molecules);
+    return -1;
+  }
+  if (!nodes || !edges || !ws || !offsets || !status || !scaffold_ids) {
+    set_error("gib_route_plan_scaffold: null argument");
+    return -1;
+  }
+  if (!sc || sc->S <= 0 || !sc->nodes || !sc->edges || !sc->n_atoms) {
+    set_error("gib_route_plan_scaffold: the scaffold table needs S >= 1 and its nodes, edges and n_atoms buffers");
+    return -1;
+  }
+  const RouteWs w = route_ws_layout(p, max_molecules);
+  char* b = static_cast<char*>(ws);
+  cudaStream_t s = (cudaStream_t)stream;
+  pp_init_kernel<<<1, 32, 0, s>>>(status, nullptr, nullptr, 0, 1);
+  GIB_LAUNCH_CHECK();
+  return launch_route(p, nodes, edges, n_molecules,
+                      RouteBufs{(int*)(b + w.len), (int*)(b + w.n0), offsets, (short*)(b + w.rs),
+                                (unsigned long long*)(b + w.hash), (int*)(b + w.apd), (int*)(b + w.nn),
+                                (int*)(b + w.mol)},
+                      status, s, scaffold_ids, sc);
+}
+
+int gib_route_fill_scaffold(const gib_pp_dims* d, const signed char* nodes, const signed char* edges,
+                            int max_molecules, const void* ws, const int* offsets, const int* status,
+                            const int* scaffold_ids, gib_batch_ctl* ctl, int* slots, int* slot_ids, int* slot_n,
+                            signed char* out_nodes, signed char* out_edges, gib_stream stream) {
+  PP p;
+  GIB_TRY(route_limits("gib_route_fill_scaffold", d, max_molecules, &p));
+  if (!nodes || !edges || !ws || !offsets || !status || !scaffold_ids || !ctl || !slots || !slot_ids || !slot_n ||
+      !out_nodes || !out_edges) {
+    set_error("gib_route_fill_scaffold: null argument");
+    return -1;
+  }
+  if (!aligned16(nodes) || !aligned16(edges) || !aligned16(out_nodes) || !aligned16(out_edges)) {
+    set_error("gib_route_fill_scaffold: nodes, edges, out_nodes and out_edges must be 16-byte aligned");
+    return -1;
+  }
+  const RouteWs w = route_ws_layout(p, max_molecules);
+  const char* b = static_cast<const char*>(ws);
+  const FillSrc f{nodes, edges, offsets, (const int*)(b + w.nn), (const int*)(b + w.mol), (const int*)(b + w.apd),
+                  (const short*)(b + w.rs)};
+  const long long nc = ceil_div_ll((long long)p.B * p.N * p.F, 16);
+  const long long ec = ceil_div_ll((long long)p.B * p.N * p.N * p.Ef, 16);
+  const long long need = std::max<long long>(ceil_div_ll(nc + ec, kFillNT), ceil_div_ll(p.B, kFillNT));
+  const int blocks = (int)std::min<long long>(need, kFillMaxBlocks);
+  route_fill_kernel<<<blocks, kFillNT, 0, (cudaStream_t)stream>>>(p, f, status, ctl, slots, out_nodes, out_edges, nc,
+                                                                  ec, scaffold_ids, slot_ids, slot_n);
   GIB_LAUNCH_CHECK();
   return 0;
 }

@@ -151,13 +151,23 @@ class ScaffoldTable:
             self.protect.copy_(other.protect)
         self.n_atoms, self.n_bonds, self.protect_mask = other.n_atoms, other.n_bonds, other.protect_mask
 
-    def struct(self, slot_ids, started, gen_scaffolds):
-        """the `gib_scaffolds` of this table and the per-batch state buffers"""
-        return Scaffolds(nodes=_ptr(self.nodes).value, edges=_ptr(self.edges).value,
-                         n_atoms=_ptr(self.n_atoms_dev).value,
-                         protect=_ptr(self.protect).value if self.protect is not None else None,
-                         slot_ids=_ptr(slot_ids).value, started=_ptr(started).value,
-                         gen_scaffolds=_ptr(gen_scaffolds).value, S=self.S)
+    def struct(self, slot_ids=None, started=None, gen_scaffolds=None):
+        """the `gib_scaffolds` of this table and the per-batch state buffers (None: null, for the route scorer's
+        entry points, which read only the table)"""
+        ptr = lambda t: _ptr(t).value if t is not None else None
+        return Scaffolds(nodes=ptr(self.nodes), edges=ptr(self.edges), n_atoms=ptr(self.n_atoms_dev),
+                         protect=ptr(self.protect), slot_ids=ptr(slot_ids), started=ptr(started),
+                         gen_scaffolds=ptr(gen_scaffolds), S=self.S)
+
+
+def scaffold_table(scaffolds, attachment, N, F, Ef, layout, device):
+    """the ScaffoldTable of `set_scaffolds`' arguments (None for None), for the generators and the route scorer"""
+    if scaffolds is None:
+        if attachment is not None:
+            raise ValueError("attachment points need scaffolds")
+        return None
+    nodes, edges = scaffolds
+    return ScaffoldTable(nodes, edges, attachment, N, F, Ef, layout, device)
 
 
 class GraphGenerator:
@@ -181,13 +191,8 @@ class GraphGenerator:
 
     def _table(self, scaffolds, attachment):
         """the ScaffoldTable of set_scaffolds' arguments (None for None)"""
-        if scaffolds is None:
-            if attachment is not None:
-                raise ValueError("attachment points need scaffolds")
-            return None
-        nodes, edges = scaffolds
-        return ScaffoldTable(nodes, edges, attachment, self.N, self.F, self.Ef,
-                             (self.A, self.CH, self.n_imp_H, self.n_chirality), self.device)
+        return scaffold_table(scaffolds, attachment, self.N, self.F, self.Ef,
+                              (self.A, self.CH, self.n_imp_H, self.n_chirality), self.device)
 
     def set_scaffolds(self, scaffolds, attachment=None):
         """decorate `scaffolds` = (nodes, edges) from the next batch on (None: grow from the empty graph again)"""

@@ -86,7 +86,8 @@ import torch
 
 from . import functional as F
 from .config import matmul_code
-from ._lib import FLAG_MULTITYPE, FLAG_OVERFLOW, HDR_FLAGS, HDR_INTS, EvalPass, check, lib
+from ._lib import (FLAG_MULTITYPE, FLAG_OVERFLOW, HDR_FLAGS, HDR_INTS, ROUTE_BAD_ID, ROUTE_MASKED, ROUTE_NOT_PREFIX,
+                   EvalPass, check, lib)
 from .generation import GraphGenerator
 
 _u8 = torch.uint8
@@ -1161,6 +1162,13 @@ nll float32 [M]: -sum(log p) over the molecule's states, accumulated in fp64 in 
 final float32 [M]: log(sum p), GraphGenerator.sample's `final` convention (GraphGenerator.py:81-83), in fp64 likewise"""
 
 
+_ROUTE_REASONS = (
+    (ROUTE_NOT_PREFIX, "the molecule does not begin with its scaffold (it has fewer atoms, another atom in the "
+                       "scaffold's rows, or another bond among the scaffold's atoms -- an extra bond between two "
+                       "scaffold atoms too: its canonical route does not pass through the scaffold's state)"),
+    (ROUTE_MASKED, "its conditional route takes an action the scaffold's attachment points forbid (probability 0)"),
+    (ROUTE_BAD_ID, "the scaffold id lies outside [-1, S)"))
+
 ROUTE_MIN_BATCH = 256        # rows from which the forward GEMMs take the tensor-core kernel (csrc/gemm_simt.cu)
 
 
@@ -1178,7 +1186,7 @@ class _RouteLikelihoods(torch.autograd.Function):
     @staticmethod
     def forward(ctx, scorer, nodes, edges, rec, *params):
         ctx.set_materialize_grads(False)            # outputs the loss does not use come back as None
-        out = scorer._score(nodes, edges, rec)
+        out = scorer._score(nodes, edges, rec, ids=rec.ids)
         ctx.scorer, ctx.rec = scorer, rec
         ctx.ptrs = [p.data_ptr() for p in params]
         ctx.save_for_backward(out.likelihoods, *params)
@@ -1244,13 +1252,42 @@ class RouteScorer:
     the batch index advanced.  The recomputed probabilities equal the forward's bit for bit (`lik` holds the last
     chunk's after a backward).  It adds the backward scratch, one [B, apd] dlogits buffer, one coefficient per state
     of a chunk and the bucket to the scorer's buffers.  A parameter modified in place, or moved, between `score()` and
-    the backward makes the backward raise, as autograd does."""
+    the backward makes the backward raise, as autograd does.
+
+    Conditional likelihoods p(molecule | scaffold), the probability a scaffold generator gives to a known decoration
+    (`scaffolds=(nodes, edges)`, `attachment=`, `set_scaffolds`: the generators' arguments and `generation.ScaffoldTable`):
+
+        scorer = RouteScorer(model, 1000, scaffolds=(sc_nodes, sc_edges), attachment=points)
+        out = scorer.score(nodes, edges, scaffold_ids=ids)          # ids int [M]: a scaffold, or -1 (the whole route)
+
+    Molecule m must begin, in decoding order, with scaffold s = ids[m]: its first k_s atoms, with every bond among
+    them, are exactly the scaffold (the state S_k).  The reference's canonical route removes the last atom's bonds one
+    at a time, so it passes through S_k, as state 1 + m_k in build order (m_k: the scaffold's bonds); the scored
+    states are the route's last n_bonds - m_k + 1, from S_k to the terminate action.  With attachment points each of
+    their logits rows goes through the generator's mask (`gib_route_mask_logits`) before the softmax.  `likelihoods`,
+    `offsets`, `nll` and `final` keep their meaning over these states, as the generator's likelihoods cover only the
+    decoration actions.  Molecules the rule cannot score are refused, naming the first, before any state of their
+    chunk is scored: one that does not begin with its scaffold (fewer atoms, another atom or another bond among the
+    scaffold's atoms -- an extra bond between two scaffold atoms too: the unmasked generator can make that molecule,
+    but its canonical route does not pass through S_k), and, with attachment points, one whose conditional route takes
+    a forbidden action (probability 0).  A generator's output scores as it is:
+
+        scorer.score(gen.generated_nodes[:n].to(torch.int8), gen.generated_edges[:n].to(torch.int8),
+                     scaffold_ids=gen.generated_scaffolds[:n])
+
+    which scores each molecule's canonical route from its scaffold -- not the order in which the generator happened to
+    place the bonds.  Per chunk the plan (`gib_route_plan_scaffold`) checks the prefixes and the masked actions with
+    its route kernels and reads the status words once; the captured graph is fill (`gib_route_fill_scaffold`), K0, the
+    forward, the mask (with attachment points), `gib_route_probs`.  The backward masks a copy of the recomputed logits
+    (the model backward reads the unmasked output), so masked entries get zero dlogits; a `set_scaffolds` between
+    `score()` and its backward makes the backward raise.  `scaffold_ids=None` runs the unconditional path unchanged."""
 
     def __init__(self, model, batch_size, constants=None, n_atom_types=None, n_formal_charge=None, n_imp_H=None,
-                 n_chirality=None, chunk_molecules=4096, device=None):
+                 n_chirality=None, chunk_molecules=4096, device=None, scaffolds=None, attachment=None):
         from .generation import action_layout
         from ._lib import PP_STATUS_INTS, PPDims
         C, A, CH, H, X = action_layout(model, constants, n_atom_types, n_formal_charge, n_imp_H, n_chirality)
+        self.layout = (A, CH, H, X)
         if not hasattr(model, "dims"):
             raise TypeError("RouteScorer runs this package's models (graphinvent_b200.gnn.mpnn) only")
         self.model, self.constants = model, C
@@ -1293,6 +1330,63 @@ class RouteScorer:
         self.replays = 0
         self._bwd = None
         self.backward_replays = 0
+        self.scaffolds, self.scaffold_version, self._sgraph = None, 0, None
+        if scaffolds is not None or attachment is not None:
+            self.set_scaffolds(scaffolds, attachment)
+
+    # ---- scaffolds ----------------------------------------------------------------------------------------------
+    def set_scaffolds(self, scaffolds, attachment=None):
+        """score conditional routes from `scaffolds` = (nodes, edges) with optional `attachment` points from the next
+        score() on (None: no table).  In place when the new set has as many scaffolds and attachment points given in
+        both or in neither; otherwise the table is reallocated and the conditional graphs are captured again."""
+        from .generation import scaffold_table
+        new = scaffold_table(scaffolds, attachment, self.N, self.F, self.Ef, self.layout, self.dev)
+        old = self.scaffolds
+        self.scaffold_version += 1
+        if new is not None and old is not None and new.S == old.S and (new.protect is None) == (old.protect is None):
+            old.copy_(new)
+            return
+        self.scaffolds = new
+        self._sgraph = None
+        if self._bwd is not None:
+            self._bwd.sgraph = None
+        if new is not None and not hasattr(self, "in_ids"):
+            i32 = torch.int32
+            self.in_ids = torch.zeros(self.chunk, dtype=i32, device=self.dev)
+            self.slot_ids = torch.full((self.B,), -1, dtype=i32, device=self.dev)
+            self.slot_n = torch.full((self.B,), -1, dtype=i32, device=self.dev)
+            self.masked_logits = torch.empty(self.B, self.apd, dtype=torch.float32, device=self.dev)
+
+    @property
+    def masked(self):
+        """True when the scaffolds' attachment points restrict the actions"""
+        return self.scaffolds is not None and self.scaffolds.protect is not None
+
+    def _scaffold_ids(self, ids, M):
+        """scaffold_ids as a contiguous int32 tensor where it came from, checked against the table"""
+        if self.scaffolds is None:
+            raise ValueError("scaffold_ids need a scaffold table: RouteScorer(..., scaffolds=) or set_scaffolds()")
+        t = torch.from_numpy(np.ascontiguousarray(ids)) if isinstance(ids, np.ndarray) else ids
+        if (not isinstance(t, torch.Tensor) or t.dtype.is_floating_point or t.dtype.is_complex or t.dtype == torch.bool
+                or t.dim() != 1 or t.shape[0] != M):
+            raise ValueError(f"scaffold_ids must be an integer numpy array or torch tensor of shape [M] = [{M}], got "
+                             f"{getattr(t, 'dtype', type(t).__name__)} {tuple(getattr(t, 'shape', ()))}")
+        S = self.scaffolds.S
+        bad = (t < -1) | (t >= S)
+        if M and bool(bad.any()):
+            m = int(bad.nonzero()[0, 0])
+            raise ValueError(f"scaffold_ids[{m}] = {int(t[m])} lies outside [-1, {S}): the table holds {S} scaffolds "
+                             "(-1 scores the whole route)")
+        return t.to(torch.int32).contiguous()
+
+    def _refuse_scaffold(self, status, ids, start, stop):
+        """the ValueError naming the first molecule of the chunk the conditional route cannot score (GIB_ROUTE_*
+        flags in status[1], the molecule in status[2])"""
+        if not status[1]:
+            return
+        m = start + int(status[2])
+        why = "; ".join(r for bit, r in _ROUTE_REASONS if status[1] & bit)
+        raise ValueError(f"molecule {m} (or a later one in molecules [{start}, {stop})), scaffold {int(ids[m])}: {why}")
 
     def _pack(self, params=None):
         """the model's parameters (or `params`, always repacked) into the arena when they changed"""
@@ -1309,32 +1403,62 @@ class RouteScorer:
         self.params = params
         self._packed_key = key
 
-    def _enqueue(self):
+    def _fill(self, st, scaffold):
+        """the next batch of the planned chunk into the static inputs (`scaffold`: of a conditional plan, with each
+        slot's scaffold id and atom count)"""
+        if not scaffold:
+            check(lib.gib_route_fill(ctypes.byref(self.pp), F._ptr(self.in_nodes), F._ptr(self.in_edges), self.chunk,
+                                     F._ptr(self.plan_ws), F._ptr(self.offsets), F._ptr(self.status),
+                                     F._ptr(self.ctl), F._ptr(self.slots), F._ptr(self.nodes), F._ptr(self.edges), st),
+                  "gib_route_fill")
+            return
+        check(lib.gib_route_fill_scaffold(ctypes.byref(self.pp), F._ptr(self.in_nodes), F._ptr(self.in_edges),
+                                          self.chunk, F._ptr(self.plan_ws), F._ptr(self.offsets), F._ptr(self.status),
+                                          F._ptr(self.in_ids), F._ptr(self.ctl), F._ptr(self.slots),
+                                          F._ptr(self.slot_ids), F._ptr(self.slot_n), F._ptr(self.nodes),
+                                          F._ptr(self.edges), st), "gib_route_fill_scaffold")
+
+    def _mask(self, logits, st):
+        """the attachment-point mask on every slot of a conditional batch, in place"""
+        self._sc = self.scaffolds.struct()
+        check(lib.gib_route_mask_logits(self.B, self.N, self.Ef, self.apd, ctypes.byref(self._sc),
+                                        F._ptr(self.slot_ids), F._ptr(self.slot_n), F._ptr(logits), st),
+              "gib_route_mask_logits")
+
+    def _enqueue(self, scaffold=False):
         st = F._stream(self.dev)
-        check(lib.gib_route_fill(ctypes.byref(self.pp), F._ptr(self.in_nodes), F._ptr(self.in_edges), self.chunk,
-                                 F._ptr(self.plan_ws), F._ptr(self.offsets), F._ptr(self.status), F._ptr(self.ctl),
-                                 F._ptr(self.slots), F._ptr(self.nodes), F._ptr(self.edges), st), "gib_route_fill")
+        self._fill(st, scaffold)
         _k0_forward(self, self.nodes, self.edges, [(self.packed, self.logits)], st)
         self._flags.bitwise_or_(self._hdr_flags)
+        if scaffold and self.masked:
+            self._mask(self.logits, st)
         check(lib.gib_route_probs(self.B, self.apd, F._ptr(self.logits), F._ptr(self.slots), F._ptr(self.lik), st),
               "gib_route_probs")
         check(lib.gib_rl_next_round(F._ptr(self.status[6:7]), st), "gib_rl_next_round")
 
-    def capture(self):
+    def capture(self, scaffold=False):
         """the warm-up runs on the zeroed plan (no state): it writes zero rows and no likelihood"""
-        self.graph, = _capture(self.dev, [self._enqueue])
+        if not scaffold:
+            self.graph, = _capture(self.dev, [self._enqueue])
+            return
+        self.status.zero_()
+        self._sgraph, = _capture(self.dev, [lambda: self._enqueue(True)])
 
     # ---- the captured backward batch ----------------------------------------------------------------------
-    def _enqueue_backward(self):
+    def _enqueue_backward(self, scaffold=False):
         """batch status[6] of the planned chunk: fill, recompute the forward, dlogits from the coefficients (the
-        recomputed p into `lik`), accumulate the gradient into the bucket, advance the batch index"""
+        recomputed p into `lik`), accumulate the gradient into the bucket, advance the batch index.  With attachment
+        points the mask goes on a copy of the logits: the model backward reads the unmasked output."""
         b, st = self._bwd, F._stream(self.dev)
-        check(lib.gib_route_fill(ctypes.byref(self.pp), F._ptr(self.in_nodes), F._ptr(self.in_edges), self.chunk,
-                                 F._ptr(self.plan_ws), F._ptr(self.offsets), F._ptr(self.status), F._ptr(self.ctl),
-                                 F._ptr(self.slots), F._ptr(self.nodes), F._ptr(self.edges), st), "gib_route_fill")
+        self._fill(st, scaffold)
         _k0_forward(self, self.nodes, self.edges, [(self.packed, self.logits)], st)
         self._flags.bitwise_or_(self._hdr_flags)
-        check(lib.gib_route_dlogits(self.B, self.apd, F._ptr(self.logits), F._ptr(self.slots), F._ptr(b.coef),
+        sampled = self.logits
+        if scaffold and self.masked:
+            sampled = self.masked_logits
+            sampled.copy_(self.logits)
+            self._mask(sampled, st)
+        check(lib.gib_route_dlogits(self.B, self.apd, F._ptr(sampled), F._ptr(self.slots), F._ptr(b.coef),
                                     F._ptr(b.dlogits), F._ptr(self.lik), st), "gib_route_dlogits")
         check(lib.gib_model_backward(ctypes.byref(self.d), self.hdr, F._ptr(self.nodes), F._ptr(self.edges),
                                      F._ptr(self.gbuf), F._ptr(self.packed), F._ptr(self.ws), F._ptr(self.logits),
@@ -1354,9 +1478,17 @@ class RouteScorer:
         b.coef = torch.zeros(self.lik.numel(), dtype=torch.float32, device=dev)
         b.gflat = torch.zeros(sum(p.numel() for p in self.params), dtype=torch.float32, device=dev)
         b.views = F._bucket_views(b.gflat, self.params)
+        b.sgraph = None
         self._bwd = b
         self.status.zero_()
         b.graph, = _capture(dev, [self._enqueue_backward])
+
+    def _ensure_backward_scaffold(self):
+        """the captured conditional backward batch (captured again after set_scaffolds reallocates the table)"""
+        self._ensure_backward()
+        if self._bwd.sgraph is None:
+            self.status.zero_()
+            self._bwd.sgraph, = _capture(self.dev, [lambda: self._enqueue_backward(True)])
 
     def _backward_chunk(self, rec, c, lik, g_lik, g_nll, g_final, eager=False):
         """chunk c of a record: upload, plan, coefficients, its batches (`eager`: the same calls without the graph)"""
@@ -1365,17 +1497,18 @@ class RouteScorer:
         st = F._stream(self.dev)
         self.in_nodes[:n].copy_(rec.nodes[pos:pos + n])
         self.in_edges[:n].copy_(rec.edges[pos:pos + n])
-        check(lib.gib_route_plan(ctypes.byref(self.pp), F._ptr(self.in_nodes), F._ptr(self.in_edges), n, self.chunk,
-                                 F._ptr(self.plan_ws), F._ptr(self.offsets), F._ptr(self.status), st), "gib_route_plan")
+        self._plan(n, rec.ids[pos:pos + n] if rec.ids is not None else None, st)
         part = lambda g, a, k: g[a:a + k] if g is not None else None
         check(lib.gib_route_grad_coef(n, F._ptr(self.offsets), F._ptr(lik[base:base + S]),
                                       F._ptr(part(g_lik, base, S)), F._ptr(part(g_nll, pos, n)),
                                       F._ptr(part(g_final, pos, n)), F._ptr(self._bwd.coef), st), "gib_route_grad_coef")
+        scaffold = rec.ids is not None
+        graph = self._bwd.sgraph if scaffold else self._bwd.graph
         for _ in range(-(-S // self.B)):
             if eager:
-                self._enqueue_backward()
+                self._enqueue_backward(scaffold)
             else:
-                self._bwd.graph.replay()
+                graph.replay()
         self.backward_replays += -(-S // self.B)
 
     @torch.no_grad()
@@ -1385,6 +1518,11 @@ class RouteScorer:
         b = self._bwd
         if b is None:                               # M = 0: no state, no backward buffers
             return F._bucket_views(torch.zeros(sum(p.numel() for p in params), device=self.dev), params)
+        if rec.ids is not None:
+            if rec.scaffold_version != self.scaffold_version:
+                raise RuntimeError("set_scaffolds was called between RouteScorer.score() and its backward: the "
+                                   "backward would plan and mask the recomputed states with other scaffolds")
+            self._ensure_backward_scaffold()
         g_lik, g_nll, g_final = (g.detach().contiguous().float() if g is not None else None
                                  for g in (g_lik, g_nll, g_final))
         self._pack(params)
@@ -1398,10 +1536,12 @@ class RouteScorer:
                      "entries: the static entry capacity is wrong, the gradients are invalid")
         return F._bucket_views(b.gflat.clone(), params)     # a fresh bucket: autograd may keep it as .grad
 
-    def score(self, nodes, edges, requires_grad=False):
+    def score(self, nodes, edges, scaffold_ids=None, requires_grad=False):
         """`RouteScores` of the molecules nodes [M, N, F] / edges [M, N, N, Ef]: int8 numpy arrays or torch tensors on
         the host or the device, padded graphs in decoding order (what `preprocess.stacks` makes of the reference's
         `PreprocessingGraph`s, or a generator's generated_nodes / generated_edges `.to(torch.int8)`).
+        `scaffold_ids`: int [M] (numpy or torch, host or device) -- molecule m's conditional route from scaffold
+        scaffold_ids[m] of the table, -1 for its whole route; None: every whole route.
         `requires_grad=True`, with grad enabled and a parameter that requires grad: likelihoods, nll and final are
         differentiable w.r.t. the model's parameters (offsets is not); otherwise plain tensors, as by default."""
         nodes, edges = _int8_stack(nodes, "nodes", 3), _int8_stack(edges, "edges", 4)
@@ -1409,44 +1549,66 @@ class RouteScorer:
         if tuple(nodes.shape[1:]) != (self.N, self.F) or tuple(edges.shape) != (M, self.N, self.N, self.Ef):
             raise ValueError(f"nodes {tuple(nodes.shape)} / edges {tuple(edges.shape)} do not fit the scorer's "
                              f"[M, {self.N}, {self.F}] / [M, {self.N}, {self.N}, {self.Ef}]")
+        ids = self._scaffold_ids(scaffold_ids, M) if scaffold_ids is not None else None
         params = list(self.model.parameters())
         if not (requires_grad and torch.is_grad_enabled() and any(p.requires_grad for p in params)):
             with torch.no_grad():
-                return self._score(nodes, edges)
-        # the record: private copies of the molecules where they came from, filled in with each chunk's states
-        rec = types.SimpleNamespace(nodes=nodes.clone(), edges=edges.clone(), chunks=[])
+                return self._score(nodes, edges, ids=ids)
+        # the record: private copies of the molecules (and scaffold ids) where they came from, filled in with each
+        # chunk's states
+        rec = types.SimpleNamespace(nodes=nodes.clone(), edges=edges.clone(), chunks=[],
+                                    ids=ids.clone() if ids is not None else None,
+                                    scaffold_version=self.scaffold_version)
         return RouteScores(*_RouteLikelihoods.apply(self, rec.nodes, rec.edges, rec, *params))
 
-    def _score(self, nodes, edges, rec=None):
+    def _plan(self, n, ids, st):
+        """the plan of the n molecules in in_nodes / in_edges: their whole routes, or (`ids`: the chunk's scaffold
+        ids, uploaded to in_ids) their conditional routes"""
+        pd = ctypes.byref(self.pp)
+        if ids is None:
+            check(lib.gib_route_plan(pd, F._ptr(self.in_nodes), F._ptr(self.in_edges), n, self.chunk,
+                                     F._ptr(self.plan_ws), F._ptr(self.offsets), F._ptr(self.status), st),
+                  "gib_route_plan")
+            return
+        self.in_ids[:n].copy_(ids)
+        self._sc = self.scaffolds.struct()
+        check(lib.gib_route_plan_scaffold(pd, F._ptr(self.in_nodes), F._ptr(self.in_edges), n, self.chunk,
+                                          ctypes.byref(self._sc), F._ptr(self.in_ids), F._ptr(self.plan_ws),
+                                          F._ptr(self.offsets), F._ptr(self.status), st), "gib_route_plan_scaffold")
+
+    def _score(self, nodes, edges, rec=None, ids=None):
         """the forward of score(); `rec`: the backward record whose chunk list (first molecule, first state,
-        states) it fills, the backward graph captured"""
+        states) it fills, the backward graph captured; `ids`: the scaffold ids (conditional routes)"""
         from .preprocess import refuse_bad
         M = nodes.shape[0]
         dev, f32 = self.dev, torch.float32
         nll, final = torch.empty(M, dtype=f32, device=dev), torch.empty(M, dtype=f32, device=dev)
         pieces, offs, base = [], [], 0
+        scaffold = ids is not None
         if M:
             self._pack()
-            if self.graph is None:
+            if scaffold and self._sgraph is None:
+                self.capture(scaffold=True)
+            elif not scaffold and self.graph is None:
                 self.capture()
             if rec is not None:
-                self._ensure_backward()
+                self._ensure_backward_scaffold() if scaffold else self._ensure_backward()
+        graph = self._sgraph if scaffold else self.graph
         st = F._stream(self.dev)
-        pd = ctypes.byref(self.pp)
         for pos in range(0, M, self.chunk):
             stop = min(pos + self.chunk, M)
             n = stop - pos
             self.in_nodes[:n].copy_(nodes[pos:stop])
             self.in_edges[:n].copy_(edges[pos:stop])
-            check(lib.gib_route_plan(pd, F._ptr(self.in_nodes), F._ptr(self.in_edges), n, self.chunk,
-                                     F._ptr(self.plan_ws), F._ptr(self.offsets), F._ptr(self.status), st),
-                  "gib_route_plan")
+            self._plan(n, ids[pos:stop] if scaffold else None, st)
             status = self.status.cpu().numpy()
             refuse_bad(status, pos, stop)
+            if scaffold:
+                self._refuse_scaffold(status, ids, pos, stop)
             S = int(status[5])
             self._flags.zero_()
             for _ in range(-(-S // self.B)):
-                self.graph.replay()
+                graph.replay()
             self.replays += -(-S // self.B)
             check(lib.gib_route_reduce(n, F._ptr(self.offsets), F._ptr(self.lik), F._ptr(nll[pos:]),
                                        F._ptr(final[pos:]), st), "gib_route_reduce")

@@ -716,6 +716,41 @@ int gib_route_grad_coef(int n_molecules, const int* offsets, const float* likeli
 int gib_route_dlogits(int B, int apd, const float* logits, const int* slots, const float* coef, float* dlogits,
                       float* p_out, gib_stream stream);
 
+/* ---- conditional route likelihoods p(molecule | scaffold) (RouteScorer.score(..., scaffold_ids=)): molecule m's
+ *      route from the state of its scaffold s = scaffold_ids[m] on.
+ * When the first k_s atoms of a molecule in decoding order, with every bond among them, are exactly scaffold s (the
+ * state S_k), the reference's canonical route (truncate_graph) passes through S_k: the last atom's bonds go one at a
+ * time, so once atom k_s is gone what is left is atoms 0..k_s-1 with all their bonds.  In build order S_k is state
+ * 1 + m_k (m_k: the scaffold's bonds), and the conditional route is the last n_edges - m_k + 1 states of the route,
+ * from S_k to the terminate action.  scaffold_ids[m] = -1: the whole route, as gib_route_plan plans it.
+ * gib_route_plan_scaffold: gib_route_plan over the conditional routes of a chunk, with the table `sc` (its nodes,
+ * edges, n_atoms and protect; the per-batch generator buffers are not read) and scaffold_ids int32 [n_molecules] on
+ * the device.  offsets and status[5] count the kept states only.  Besides status[3] / [4] (the molecule itself is
+ * invalid; no conditional state is then checked): status[1] GIB_ROUTE_* flags, status[2] the first molecule with one
+ * (INT_MAX: none):
+ *   GIB_ROUTE_NOT_PREFIX  the molecule does not begin with its scaffold: fewer atoms, another atom in rows 0..k_s-1,
+ *                         or another edge entry among them (an extra bond between two scaffold atoms too -- the
+ *                         unmasked generator can make such a molecule, but its canonical route misses S_k);
+ *   GIB_ROUTE_MASKED      with attachment points (protect != null), a kept state's action is one the generator's mask
+ *                         forbids (gib_generation_mask_logits' rule): its probability would be exactly 0;
+ *   GIB_ROUTE_BAD_ID      scaffold_ids[m] outside [-1, S).
+ * A chunk with any flag has no valid plan.
+ * gib_route_fill_scaffold: gib_route_fill of a gib_route_plan_scaffold plan (the same scaffold_ids), and per slot b
+ * the mask's inputs: slot_ids[b] = the state's scaffold id, slot_n[b] = its atom count (-1 / -1 for a molecule scored
+ * whole and past the last state).
+ * gib_route_mask_logits: gib_generation_mask_logits' rule on every slot of a route batch, slot 0 included (a route
+ * batch has no dummy slot); slots with slot_ids[b] < 0 are left alone; a table without protect masks nothing. */
+enum { GIB_ROUTE_NOT_PREFIX = 1, GIB_ROUTE_MASKED = 2, GIB_ROUTE_BAD_ID = 4 };
+int gib_route_plan_scaffold(const gib_pp_dims* d, const signed char* nodes, const signed char* edges, int n_molecules,
+                            int max_molecules, const gib_scaffolds* sc, const int* scaffold_ids, void* ws,
+                            int* offsets, int* status, gib_stream stream);
+int gib_route_fill_scaffold(const gib_pp_dims* d, const signed char* nodes, const signed char* edges,
+                            int max_molecules, const void* ws, const int* offsets, const int* status,
+                            const int* scaffold_ids, gib_batch_ctl* ctl, int* slots, int* slot_ids, int* slot_n,
+                            signed char* out_nodes, signed char* out_edges, gib_stream stream);
+int gib_route_mask_logits(int B, int N, int Ef, int apd, const gib_scaffolds* sc, const int* slot_ids,
+                          const int* n_nodes, float* logits, gib_stream stream);
+
 /* ---- measurement hooks: CUDA-event timing per kernel class on the launching stream.
  *      class 0 = forward/dX launches of the tensor-core kernel, 1 = its weight-gradient launches, 2 = scatter-aggregate (K2),
  *      3 / 4 = forward/dX and weight-gradient GEMMs on the fp32 SIMT kernels.  GIB_PROFILE_CLASSES entries per array.
