@@ -1014,6 +1014,10 @@ int gib_route_plan_scaffold(const gib_pp_dims* d, const signed char* nodes, cons
     set_error("gib_route_plan_scaffold: the scaffold table needs S >= 1 and its nodes, edges and n_atoms buffers");
     return -1;
   }
+  if (sc->protect && p.N > 127) {     // protect holds 4 x 32 bits per scaffold, as the generator's mask reads it
+    set_error("gib_route_plan_scaffold: attachment points need N <= 127 (4 protect words per scaffold), got N=%d", p.N);
+    return -1;
+  }
   const RouteWs w = route_ws_layout(p, max_molecules);
   char* b = static_cast<char*>(ws);
   cudaStream_t s = (cudaStream_t)stream;

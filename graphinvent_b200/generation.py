@@ -84,6 +84,9 @@ class ScaffoldTable:
 
     def __init__(self, nodes, edges, attachment, N, F, Ef, layout, device):
         from . import preprocess
+        if attachment is not None and N > 127:
+            raise ValueError(f"attachment points need max_n_nodes N <= 127 (4 x 32 protect bits per scaffold), "
+                             f"got N = {N}")
         nodes = np.ascontiguousarray(torch.as_tensor(nodes).cpu().numpy())
         edges = np.ascontiguousarray(torch.as_tensor(edges).cpu().numpy())
         if (nodes.ndim != 3 or edges.ndim != 4 or nodes.shape[0] < 1 or nodes.shape[2] != F or edges.shape[3] != Ef

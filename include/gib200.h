@@ -734,7 +734,8 @@ int gib_route_dlogits(int B, int apd, const float* logits, const int* slots, con
  *   GIB_ROUTE_MASKED      with attachment points (protect != null), a kept state's action is one the generator's mask
  *                         forbids (gib_generation_mask_logits' rule): its probability would be exactly 0;
  *   GIB_ROUTE_BAD_ID      scaffold_ids[m] outside [-1, S).
- * A chunk with any flag has no valid plan.
+ * A chunk with any flag has no valid plan.  A table with protect != null needs N <= 127 (its 4 protect words per
+ * scaffold, as the generator's mask); without attachment points any N gib_route_plan accepts is allowed.
  * gib_route_fill_scaffold: gib_route_fill of a gib_route_plan_scaffold plan (the same scaffold_ids), and per slot b
  * the mask's inputs: slot_ids[b] = the state's scaffold id, slot_n[b] = its atom count (-1 / -1 for a molecule scored
  * whole and past the last state).
