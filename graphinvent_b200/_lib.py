@@ -175,6 +175,7 @@ _PROTOS = {
     "gib_route_plan_scaffold": (c_i, [c_p, c_p, c_p, c_i, c_i] + [c_p] * 6),
     "gib_route_fill_scaffold": (c_i, [c_p, c_p, c_p, c_i] + [c_p] * 11),
     "gib_route_mask_logits": (c_i, [c_i] * 4 + [c_p] * 5),
+    "gib_test_route_plan_offsets": (c_i, [c_p, c_i, c_p]),
     "gib_profile_enable": (None, [c_i]),
     "gib_launch_count": (c_ll, []),
     "gib_profile_collect": (c_i, [c_p, c_p, c_p]),

@@ -970,6 +970,21 @@ int gib_route_plan(const gib_pp_dims* d, const signed char* nodes, const signed 
                       status, s);
 }
 
+int gib_test_route_plan_offsets(const gib_pp_dims* d, int max_molecules, long long* out) {
+  PP p;
+  GIB_TRY(route_limits("gib_test_route_plan_offsets", d, max_molecules, &p));
+  if (!out) {
+    set_error("gib_test_route_plan_offsets: null out");
+    return -1;
+  }
+  const RouteWs w = route_ws_layout(p, max_molecules);
+  out[0] = (long long)w.hash;
+  out[1] = (long long)w.apd;
+  out[2] = (long long)w.nn;
+  out[3] = (long long)w.mol;
+  return 0;
+}
+
 int gib_route_fill(const gib_pp_dims* d, const signed char* nodes, const signed char* edges, int max_molecules,
                    const void* ws, const int* offsets, const int* status, gib_batch_ctl* ctl, int* slots,
                    signed char* out_nodes, signed char* out_edges, gib_stream stream) {

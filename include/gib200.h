@@ -715,6 +715,13 @@ int gib_route_grad_coef(int n_molecules, const int* offsets, const float* likeli
                         const float* g_nll, const float* g_final, float* coef, gib_stream stream);
 int gib_route_dlogits(int B, int apd, const float* logits, const int* slots, const float* coef, float* dlogits,
                       float* p_out, gib_stream stream);
+/* host only, a test hook: the byte offsets of the per-state arrays in a gib_route_plan workspace for (d, max_molecules),
+ * out[4] = {hash (uint64), apd, nn, mol (int32)}, each of gib_route_max_states entries; molecule m's route state k
+ * (truncation order) is entry offsets[m] + k, numbered as gib_preprocess_chunk numbers a chunk's states.  hash is the
+ * key of gib_preprocess_chunk's dedup table: the sum mod 2^64 over the state's non-zero bytes (node bytes at positions
+ * [0, N*F), then edge bytes) of splitmix64's finaliser of (position << 8 | byte), with 2^64 - 1 (the empty-slot key)
+ * stored as 2^64 - 2.  Returns 0, < 0 for dims or max_molecules gib_route_plan refuses. */
+int gib_test_route_plan_offsets(const gib_pp_dims* d, int max_molecules, long long* out);
 
 /* ---- conditional route likelihoods p(molecule | scaffold) (RouteScorer.score(..., scaffold_ids=)): molecule m's
  *      route from the state of its scaffold s = scaffold_ids[m] on.

@@ -7,6 +7,9 @@ Numpy restatement of the reference's training-set construction -- the decoding r
 Groups are deduplicated with a dict on the state's bytes instead of the reference's quadratic scan; the reference's
 append rule is kept: a state is appended as a new row when it matches no row, or when its first match is the LAST row
 (its APD is then added to that row and the new row carries it too).
+
+`state_hash` restates the device's 64-bit state hash, the key of its dedup table, so that tests can build and check
+inputs whose states collide in it (tests/golden/make_preprocess_collisions.py).
 """
 import numpy as np
 
@@ -119,6 +122,47 @@ def groups(nodes, edges, batch_size, segs):
                    apds=np.array(apds, np.int64).reshape(-1, apd_len),
                    resume_idx=resume, dataset_size=size)
         g += 1
+
+
+# ---- the group kernel's state hash (csrc/preprocess.cu), restated: the device keys its dedup table by it and compares
+# the bytes of hash-equal states, so two states of one hash are one row only when their bytes are equal ------------
+_U = np.uint64
+RESERVED = _U(0xFFFFFFFFFFFFFFFF)          # the table's empty-slot key: a state of this hash is stored as RESERVED - 1
+
+
+def mix64(x):
+    """splitmix64's finaliser of uint64 x (array or scalar), wrapping mod 2^64"""
+    x = np.asarray(x, _U)
+    with np.errstate(over="ignore"):
+        x = x + _U(0x9E3779B97F4A7C15)
+        x = (x ^ (x >> _U(30))) * _U(0xBF58476D1CE4E5B9)
+        x = (x ^ (x >> _U(27))) * _U(0x94D049BB133111EB)
+        return x ^ (x >> _U(31))
+
+
+def byte_hash(pos, v):
+    """the mix of byte v (int8, read as unsigned) at flat position pos; 0 for a zero byte"""
+    pos, v = np.asarray(pos, np.int64), np.asarray(v, np.int8)
+    h = mix64((pos.astype(_U) << _U(8)) | v.view(np.uint8).astype(_U))
+    return np.where(v != 0, h, _U(0))
+
+
+def state_hash(X, E):
+    """the sum mod 2^64 of byte_hash over the state's bytes: node bytes at positions [0, N*F), then edge bytes"""
+    flat = np.concatenate([np.ravel(X), np.ravel(E)]).astype(np.int8)
+    nz = np.flatnonzero(flat)
+    return _U(byte_hash(nz, flat[nz]).sum(dtype=_U))
+
+
+def stored_hash(h):
+    """the key the route kernel stores for a state of hash h: RESERVED is remapped to RESERVED - 1"""
+    h = np.asarray(h, _U)
+    return np.where(h == RESERVED, RESERVED - _U(1), h)
+
+
+def route_hashes(nodes, edges, segs):
+    """state_hash of every state of route(nodes, edges), in truncation order (uint64, not remapped)"""
+    return np.array([state_hash(X, E) for X, E, _ in route(nodes, edges, segs)], _U)
 
 
 def total_subgraphs(edges):

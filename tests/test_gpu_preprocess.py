@@ -35,6 +35,21 @@ def graphs(M, N, layout, Ef=3, seed=0, min_atoms=1):
     return np.concatenate([nodes] + extra, axis=2), edges
 
 
+def complete_graph(n, N, layout, Ef, seed):
+    """one molecule of n atoms (a random one-hot per segment of the layout), every pair bonded with a random type"""
+    rng = np.random.default_rng(seed)
+    segs = P.segments(*layout)
+    X = np.zeros((N, sum(segs)), np.int8)
+    for i in range(n):
+        X[i, np.cumsum([0] + segs[:-1]) + rng.integers(0, segs)] = 1
+    E = np.zeros((N, N, Ef), np.int8)
+    for i in range(1, n):
+        for j in range(i):
+            t = int(rng.integers(Ef))
+            E[i, j, t] = E[j, i, t] = 1
+    return X, E
+
+
 def device_groups(nodes, edges, B, layout, **kw):
     from graphinvent_b200 import preprocess as PP
     return list(PP.groups(nodes, edges, B, *layout, **kw))
@@ -80,11 +95,18 @@ def test_gdb13_files_rebuilt_byte_for_byte(key, chunk):
     (38, 120, 30, 40, 4, "imp_H+chirality"),
     (90, 24, 200, 4096, 3, "gdb13"),
     (90, 24, 64, 64, 1, "gdb13"),
+    (127, 12, 1060, 1060, 2, "imp_H"),       # beyond N = 90: a complete graph of 47 atoms first (1083 states),
+    (181, 8, 1030, 4096, 1, "gdb13"),        # of 46 atoms (1037 states); the cut at B falls in its second tile
 ])
 def test_matches_restatement(N, M, B, chunk, Ef, layout):
     L = LAYOUTS[layout]
     nodes, edges = graphs(M, N, L, Ef=Ef, seed=N * 1000 + B)
+    if N > 90:
+        X, E = complete_graph(47 if N < 150 else 46, N, L, Ef, seed=N)
+        nodes, edges = np.concatenate([X[None], nodes]), np.concatenate([E[None], edges])
     ref = list(P.groups(nodes, edges, B, segs_of(L)))
+    if N > 90:                                # one route spans tiles of 1024 states and the group is cut inside it
+        assert int(edges[0].sum()) // 2 > B > 1024 and ref[0]["full"] and ref[0]["stop"] == 1
     assert_same(device_groups(nodes, edges, B, L, chunk_molecules=chunk), ref)
 
 
