@@ -564,9 +564,8 @@ static GemmDW to_gemm_dw(const gib_dw_problem& s) {
   q.m_dev = s.m_dev; q.base_dev = s.base_dev; q.tf32 = s.tf32;
   return q;
 }
-// both scratch halves, sized as make_bwd sizes them: the largest group (with the same plan rows) and member
-static size_t test_dw_scratch_floats(const gib_dw_problem* qs, const int* group_sizes, int n_groups,
-                                     long long plan_rows) {
+// both scratch halves, sized as make_bwd sizes them: the largest group and member
+static size_t test_dw_scratch_floats(const gib_dw_problem* qs, const int* group_sizes, int n_groups) {
   size_t f = 0;
   int k = 0;
   for (int g = 0; g < n_groups; ++g) {
@@ -574,7 +573,7 @@ static size_t test_dw_scratch_floats(const gib_dw_problem* qs, const int* group_
     const int n = group_sizes[g];
     if (n < 1 || n > kTc3MaxProblems) return 0;
     for (int i = 0; i < n; ++i) grp[i] = to_gemm_dw(qs[k + i]);
-    f = std::max(f, 2 * gemm_dw_group_half_floats(grp, n, plan_rows));
+    f = std::max(f, 2 * gemm_dw_group_half_floats(grp, n));
     k += n;
   }
   return f;
@@ -603,11 +602,13 @@ int gib_test_gemm_nt(const gib_gemm_problem* ps, int n, const int* dep, int* fla
   return gemm_nt_chain(p, dep, n, flags, ST(stream));
 }
 size_t gib_test_dw_scratch_bytes(const gib_dw_problem* qs, const int* group_sizes, int n_groups, long long plan_rows) {
-  return test_dw_scratch_floats(qs, group_sizes, n_groups, plan_rows) * sizeof(float);
+  (void)plan_rows;
+  return test_dw_scratch_floats(qs, group_sizes, n_groups) * sizeof(float);
 }
 int gib_test_dw_groups(const gib_dw_problem* qs, const int* group_sizes, int n_groups, long long plan_rows,
                        void* scratch, gib_stream stream) {
-  const size_t floats = test_dw_scratch_floats(qs, group_sizes, n_groups, plan_rows);
+  (void)plan_rows;
+  const size_t floats = test_dw_scratch_floats(qs, group_sizes, n_groups);
   if (n_groups < 1 || floats == 0) { set_error("gib_test_dw_groups: bad group sizes"); return -2; }
   GIB_TRY(dw_begin());
   int rc = 0;
@@ -618,10 +619,14 @@ int gib_test_dw_groups(const gib_dw_problem* qs, const int* group_sizes, int n_g
       grp[i].scratch = reinterpret_cast<float*>(scratch);
       grp[i].half_floats = floats / 2;
     }
-    rc = group_sizes[g] == 1 ? gemm_dw(grp[0], ST(stream)) : gemm_dw_group(grp, group_sizes[g], plan_rows, ST(stream));
+    rc = group_sizes[g] == 1 ? gemm_dw(grp[0], ST(stream)) : gemm_dw_group(grp, group_sizes[g], ST(stream));
   }
   const int rj = dw_join(ST(stream));
   return rc ? rc : rj;
+}
+int gib_test_dw_schedule(const int* rows, const int* Nn, const int* Kk, int n, int sms, int* segs, int max_segs,
+                         int* tile_ctas, int* G) {
+  return tc3_dw_schedule(rows, Nn, Kk, n, sms, segs, max_segs, tile_ctas, G);
 }
 int gib_test_scatter_bwd(float* G, const float* dM, const float* Y, int ld, const int* dst, const float* w, int act,
                          long long P, gib_stream stream) {

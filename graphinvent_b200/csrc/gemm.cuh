@@ -66,12 +66,10 @@ struct GemmDW {
 
 constexpr int kTc3MaxProblems = 16;   // problems per launch of the tensor-core kernel
 
-// scratch layout of one grouped weight-gradient launch of the tensor-core kernel (gemm_tc3.cu)
+// scratch layout of one grouped weight-gradient launch of the tensor-core kernel (gemm_tc3.cu): [slots][128][128]
+// partial tiles, then [slots][128] bias partials; slots = min(SMs, ceil(k-blocks / 8)) + the group's output tiles
 struct Dw3Layout {
-  int chunk_rows;                          // reduction rows per work item
-  int cap_splits[kTc3MaxProblems];         // split capacity per problem (the live count may be smaller: device-side row counts)
-  size_t part_off[kTc3MaxProblems];        // float offsets of [cap_splits][Nn][Kk] partial products
-  size_t bias_off[kTc3MaxProblems];        // float offsets of [cap_splits][Nn] partial column sums
+  int slots;
   size_t floats;                           // total
 };
 
@@ -93,10 +91,11 @@ int gemm_nt_tc3_group(const GemmNT* ps, int n, cudaStream_t st);
 size_t tc3_chain_flag_ints(const GemmNT* ps, int n);
 int gemm_nt_tc3_chain(const GemmNT* ps, const int* dep, int n, int* flags, cudaStream_t st);
 bool tc3_dw_eligible(const GemmDW& q);
-int tc3_dw_chunk_rows(const GemmDW* qs, int n, long long plan_rows);   // from ALL members of a group (sizing == run time)
-void tc3_dw_layout(const GemmDW* qs, int n, int chunk_rows, Dw3Layout* L);
+void tc3_dw_layout(const GemmDW* qs, int n, Dw3Layout* L);
 int gemm_dw_tc3_partials(const GemmDW* qs, int n, const Dw3Layout& L, float* scratch, cudaStream_t st);
 int gemm_dw_tc3_reduce(const GemmDW* qs, int n, const Dw3Layout& L, const float* scratch, cudaStream_t st);
+int tc3_dw_schedule(const int* rows, const int* Nn, const int* Kk, int n, int sms, int* segs, int max_segs,
+                    int* tile_ctas, int* G_out);   // test hook (gib_test_dw_schedule)
 int device_sm_count();     // SMs of the current device (cached per device)
 void tc3_set_trace(long long* buf, int tiles);   // diagnosis: per-tile clock64 stamps of CTA 0
 extern bool g_use_tc;
@@ -107,15 +106,11 @@ int check_precision(int prec, const char* who);
 
 int gemm_dw(const GemmDW& q, cudaStream_t st);
 // n <= 16 weight-gradient problems that may run as ONE grouped tensor-core launch + ONE reduction launch (siblings of a
-// layer: the per-bond-type message MLPs, the readout heads, the two GRU projections).  plan_rows: expected total
-// reduction rows of the group (0: the sum of q.M), used to size the split so that the group fills the machine once.
-int gemm_dw_group(const GemmDW* qs, int n, long long plan_rows, cudaStream_t st);
-size_t gemm_dw_group_half_floats(const GemmDW* qs, int n, long long plan_rows);
+// layer: the per-bond-type message MLPs, the readout heads, the two GRU projections)
+int gemm_dw_group(const GemmDW* qs, int n, cudaStream_t st);
+size_t gemm_dw_group_half_floats(const GemmDW* qs, int n);
 int dw_begin();            // start of a C-ABI call that uses gemm_dw: forget the previous call's side-stream jobs
 void gemm_dw_plan(int M, int Nn, int Kk, int* splits, int* chunk);
-void tc_dw_plan(int M, int Nn, int Kk, int* splits, int* chunk);
-bool tc_dw_eligible(const GemmDW& q);
-int gemm_dw_tc_partials(const GemmDW& q, int* splits_out, cudaStream_t st);
 size_t gemm_dw_scratch_floats(int M, int Nn, int Kk);   // both halves
 size_t gemm_dw_half_floats(int M, int Nn, int Kk);
 int dw_join(cudaStream_t st);                            // drain the helper side stream into `st`

@@ -18,7 +18,6 @@
 namespace gib {
 
 constexpr int BK = 16;
-constexpr int kColsumSplits = 296;  // row chunks (one block each) of the two-stage bias-gradient column sum
 
 // ------------------------------------------------------------------------------------
 // C[M,N] = epilogue( A[M,K] * B[N,K]^T )       (both operands K-contiguous)
@@ -444,58 +443,14 @@ static int launch_reduce(const float* ws, int splits, const GemmDW& q, const flo
   return 0;
 }
 
-// part[z][n] = sum over the z-th row chunk of G[m, n]  (fixed order inside the chunk; chunks reduced in order).
-// One block per row chunk, whole rows read with float4 (fully coalesced); thread t owns float4 column t % (Nn/4) and
-// every (256 / (Nn/4))-th row of the chunk, partial sums meet in shared memory in a fixed order.
-__global__ void __launch_bounds__(256) colsum_partial_kernel(float* __restrict__ part, const float* __restrict__ G,
-                                                             int ldg, int M, int Nn) {
-  __shared__ float4 sm[256];
-  const int n4 = Nn >> 2;                       // float4 columns per row (Nn is a multiple of 16)
-  const int rows = ceil_div(M, (int)gridDim.x);
-  const int m0 = blockIdx.x * rows, m1 = min(M, m0 + rows);
-  for (int c0 = 0; c0 < n4; c0 += 256) {        // Nn <= 1024 handled in one sweep per 256 float4 columns
-    const int width = min(256, n4 - c0);        // active float4 columns in this sweep
-    const int lanes = 256 / width;              // row lanes sharing the sweep
-    const int col = threadIdx.x % width, rl = threadIdx.x / width;
-    float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
-    if (rl < lanes) {
-      int m = m0 + rl;
-      for (; m + 3 * lanes < m1; m += 4 * lanes) {      // four row loads in flight, summed in ascending row order
-        float4 v[4];
-#pragma unroll
-        for (int u = 0; u < 4; ++u)
-          v[u] = __ldg(reinterpret_cast<const float4*>(G + (size_t)(m + u * lanes) * ldg) + c0 + col);
-#pragma unroll
-        for (int u = 0; u < 4; ++u) { acc.x += v[u].x; acc.y += v[u].y; acc.z += v[u].z; acc.w += v[u].w; }
-      }
-      for (; m < m1; m += lanes) {
-        const float4 v = __ldg(reinterpret_cast<const float4*>(G + (size_t)m * ldg) + c0 + col);
-        acc.x += v.x; acc.y += v.y; acc.z += v.z; acc.w += v.w;
-      }
-    }
-    sm[threadIdx.x] = acc;
-    __syncthreads();
-    if (rl == 0) {
-      float4 t = sm[col];
-      for (int k = 1; k < lanes; ++k) {
-        const float4 u = sm[k * width + col];
-        t.x += u.x; t.y += u.y; t.z += u.z; t.w += u.w;
-      }
-      reinterpret_cast<float4*>(part + (size_t)blockIdx.x * Nn)[c0 + col] = t;
-    }
-    __syncthreads();
-  }
-}
-
 // ---- helper side stream ------------------------------------------------------------------------------------
 // A tensor-core GEMM CTA leaves ~16K registers and some shared memory free on every SM -- room for a 256-thread block
 // of the split reduction.  The reductions therefore run on a library-owned side stream (one per device),
 // concurrently with the NEXT tensor-core launches of the main stream, instead of serialising ~10 us per layer:
 //   job i (scratch half i&1):  main: [wait done(i-2)] partial products (+ bias partials) -> record tn(i)
 //                              side: wait tn(i); fixed-order reduction into the gradients; record done(i)
-// Second-generation kernel: the side job reads only the scratch half (bias column sums come out of the GEMM), so the
-// only hazard is the reuse of that half by job i+2.  First-generation kernel: the side job also reads the G operand
-// (column sums), hence the extra wait before the caller's next dX GEMM (g_pending).  dw_join() drains the side stream
+// The side job reads only the scratch half (bias column sums come out of the GEMM), so the only hazard is the reuse
+// of that half by job i+2.  dw_join() drains the side stream
 // into the caller's stream; every C-ABI entry that uses gemm_dw calls dw_begin() first and dw_join() before
 // returning, so the pattern is self-contained per call (fork / join: capturable in a CUDA graph).
 // One thread per device at a time (the C-ABI contract: one host thread drives a device's model).
@@ -504,7 +459,6 @@ struct DwSide {
   cudaEvent_t ev_tn[2], ev_done[2];
   bool done_valid[2] = {false, false};
   long long calls = 0;
-  int pending = -1;      // first generation: job whose completion the main stream has not waited for yet
   int last = -1;         // half of the most recent job
 };
 static DwSide g_dw[64];
@@ -531,7 +485,7 @@ int dw_begin() {
   DwSide* d;
   GIB_TRY(dw_side(&d));
   d->done_valid[0] = d->done_valid[1] = false;   // the previous call joined its jobs into its stream
-  d->calls = 0; d->pending = -1; d->last = -1;
+  d->calls = 0; d->last = -1;
   return 0;
 }
 
@@ -540,20 +494,18 @@ int dw_join(cudaStream_t st) {
   GIB_TRY(dw_side(&d));
   if (d->last >= 0) {       // the side stream is in order: the last job's event covers all of them
     GIB_CUDA_TRY(cudaStreamWaitEvent(st, d->ev_done[d->last], 0));
-    d->last = -1; d->pending = -1;
+    d->last = -1;
   }
   return 0;
 }
 
 size_t gemm_dw_half_floats(int M, int Nn, int Kk) {
-  int splits, chunk, s2, c2;
+  int splits, chunk;
   gemm_dw_plan(M, Nn, Kk, &splits, &chunk);
-  tc_dw_plan(M, Nn, Kk, &s2, &c2);       // the tensor-core path may pick a different split count
-  if (s2 > splits) splits = s2;
-  size_t f = (((size_t)splits * Nn * Kk + (size_t)(splits > kColsumSplits ? splits : kColsumSplits) * Nn) + 63) & ~(size_t)63;
+  const size_t f = ((size_t)splits * Nn * Kk + (size_t)splits * Nn + 63) & ~(size_t)63;
   GemmDW q; q.M = M; q.Nn = Nn; q.Kk = Kk;
   Dw3Layout L;
-  tc3_dw_layout(&q, 1, tc3_dw_chunk_rows(&q, 1, 0), &L);
+  tc3_dw_layout(&q, 1, &L);
   return std::max(f, (L.floats + 63) & ~(size_t)63);
 }
 
@@ -562,11 +514,11 @@ size_t gemm_dw_scratch_floats(int M, int Nn, int Kk) {
   return 2 * gemm_dw_half_floats(M, Nn, Kk);
 }
 
-size_t gemm_dw_group_half_floats(const GemmDW* qs, int n, long long plan_rows) {
+size_t gemm_dw_group_half_floats(const GemmDW* qs, int n) {
   size_t f = 0;
   for (int i = 0; i < n; ++i) f = std::max(f, gemm_dw_half_floats(qs[i].M, qs[i].Nn, qs[i].Kk));
   Dw3Layout L;
-  tc3_dw_layout(qs, n, tc3_dw_chunk_rows(qs, n, plan_rows), &L);
+  tc3_dw_layout(qs, n, &L);
   return std::max(f, (L.floats + 63) & ~(size_t)63);
 }
 
@@ -584,9 +536,33 @@ void gemm_dw_plan(int M, int Nn, int Kk, int* splits, int* chunk) {
   *chunk = c;
 }
 
-// grouped weight gradients: one tensor-core launch (partials + bias partials of every member) on the caller's stream and
-// one fixed-order reduction launch on the side stream; falls back to member-by-member when the group is not eligible
-int gemm_dw_group(const GemmDW* qs, int n, long long plan_rows, cudaStream_t st) {
+// one tensor-core launch (partials + bias partials of every member) on the caller's stream and one fixed-order
+// reduction launch on the side stream
+static int dw_tc_launch(const GemmDW* live, int nl, double work, const ProfRows* dyn_rows, int ndyn, cudaStream_t st) {
+  ProfScope prof(PROF_GEMM_DW, work, st, dyn_rows, ndyn);
+  DwSide* d;
+  GIB_TRY(dw_side(&d));
+  const int half = (int)(d->calls++ & 1);
+  float* const scratch = live[0].scratch + (size_t)half * live[0].half_floats;
+  Dw3Layout L;
+  tc3_dw_layout(live, nl, &L);
+  if (L.floats > live[0].half_floats) {
+    set_error("gemm_dw_group: scratch half of %zu floats is too small for %zu", live[0].half_floats, L.floats);
+    return -2;
+  }
+  if (d->done_valid[half]) GIB_CUDA_TRY(cudaStreamWaitEvent(st, d->ev_done[half], 0));   // job i-2 released this half
+  GIB_TRY(gemm_dw_tc3_partials(live, nl, L, scratch, st));
+  GIB_CUDA_TRY(cudaEventRecord(d->ev_tn[half], st));
+  GIB_CUDA_TRY(cudaStreamWaitEvent(d->side, d->ev_tn[half], 0));
+  GIB_TRY(gemm_dw_tc3_reduce(live, nl, L, scratch, d->side));
+  GIB_CUDA_TRY(cudaEventRecord(d->ev_done[half], d->side));
+  d->done_valid[half] = true;
+  d->last = half;
+  return 0;
+}
+
+// grouped weight gradients: one tensor-core launch + one reduction for the members that qualify, the others one by one
+int gemm_dw_group(const GemmDW* qs, int n, cudaStream_t st) {
   if (n < 1) return 0;
   if (n > kTc3MaxProblems) { set_error("gemm_dw_group: %d problems (max %d)", n, kTc3MaxProblems); return -2; }
   for (int i = 0; i < n; ++i) GIB_TRY(check_precision(qs[i].tf32, "gemm_dw_group"));
@@ -628,30 +604,7 @@ int gemm_dw_group(const GemmDW* qs, int n, long long plan_rows, cudaStream_t st)
   }
   for (int i = 0; i < nr; ++i) GIB_TRY(gemm_dw(rest[i], st));
   if (nl == 0) return 0;
-  ProfScope prof(PROF_GEMM_DW, work, st, dyn_rows, ndyn);
-  DwSide* d;
-  GIB_TRY(dw_side(&d));
-  const int half = (int)(d->calls++ & 1);
-  float* const scratch = live[0].scratch + (size_t)half * live[0].half_floats;
-  Dw3Layout L;       // chunk from ALL members (as the scratch was sized), offsets for the grouped ones
-  tc3_dw_layout(live, nl, tc3_dw_chunk_rows(qs, n, plan_rows), &L);
-  if (L.floats > live[0].half_floats) {
-    set_error("gemm_dw_group: scratch half of %zu floats is too small for %zu", live[0].half_floats, L.floats);
-    return -2;
-  }
-  if (d->pending >= 0) {      // a first-generation job still reads its G operand: finish it first
-    GIB_CUDA_TRY(cudaStreamWaitEvent(st, d->ev_done[d->pending], 0));
-    d->pending = -1;
-  }
-  if (d->done_valid[half]) GIB_CUDA_TRY(cudaStreamWaitEvent(st, d->ev_done[half], 0));   // job i-2 released this half
-  GIB_TRY(gemm_dw_tc3_partials(live, nl, L, scratch, st));
-  GIB_CUDA_TRY(cudaEventRecord(d->ev_tn[half], st));
-  GIB_CUDA_TRY(cudaStreamWaitEvent(d->side, d->ev_tn[half], 0));
-  GIB_TRY(gemm_dw_tc3_reduce(live, nl, L, scratch, d->side));
-  GIB_CUDA_TRY(cudaEventRecord(d->ev_done[half], d->side));
-  d->done_valid[half] = true;
-  d->last = half;
-  return 0;
+  return dw_tc_launch(live, nl, work, dyn_rows, ndyn, st);
 }
 
 int gemm_dw(const GemmDW& q, cudaStream_t st) {
@@ -661,39 +614,17 @@ int gemm_dw(const GemmDW& q, cudaStream_t st) {
     set_error("gemm_dw: ldg=%d ldx=%d Nn=%d Kk=%d violate the padded-layout contract", q.ldg, q.ldx, q.Nn, q.Kk);
     return -2;
   }
-  if (q.m_dev || (g_use_tc && use_tc3() && q.dW && q.M >= 2048 && q.Nn >= 32 && q.Kk >= 32 && tc3_dw_eligible(q) &&
-                  q.half_floats > 0))
-    return gemm_dw_group(&q, 1, 0, st);
-  const bool tc = g_use_tc && q.dW && tc_dw_eligible(q);
-  ProfScope prof(tc ? PROF_GEMM_DW : PROF_GEMM_DW_SIMT, q.work > 0 ? q.work : 2.0 * q.M * (double)q.R * q.C, st);
+  if (q.m_dev) return gemm_dw_group(&q, 1, st);
+  // the tensor-core launch as a group of one (also under gib_tc_debug bit 0, which groups no weight gradients)
+  const double work = q.work > 0 ? q.work : 2.0 * q.M * (double)q.R * q.C;
+  if (g_use_tc && q.dW && q.M >= 2048 && q.Nn >= 32 && q.Kk >= 32 && tc3_dw_eligible(q) && q.half_floats > 0)
+    return dw_tc_launch(&q, 1, work, nullptr, 0, st);
+  ProfScope prof(PROF_GEMM_DW_SIMT, work, st);
   DwSide* d;
   GIB_TRY(dw_side(&d));
   const int half = (int)(d->calls++ & 1);
   float* const scratch = q.scratch + (size_t)half * q.half_floats;
   if (d->done_valid[half]) GIB_CUDA_TRY(cudaStreamWaitEvent(st, d->ev_done[half], 0));   // job i-2 released this half
-  if (tc) {
-    // per-problem tensor-core partials (MN-major operands straight from the row-major activations) on the main
-    // stream; bias column sums + the fixed-order split reduction on the side stream
-    int tsplits = 0;
-    GemmDW q2 = q;
-    q2.scratch = scratch;
-    GIB_TRY(gemm_dw_tc_partials(q2, &tsplits, st));
-    GIB_CUDA_TRY(cudaEventRecord(d->ev_tn[half], st));
-    GIB_CUDA_TRY(cudaStreamWaitEvent(d->side, d->ev_tn[half], 0));
-    float* part = scratch + (size_t)tsplits * q.Nn * q.Kk;         // [kColsumSplits][Nn] partial column sums
-    if (q.dbias) {
-      colsum_partial_kernel<<<kColsumSplits, 256, 0, d->side>>>(part, q.G, q.ldg, q.M, q.Nn);
-      GIB_LAUNCH_CHECK();
-    }
-    GIB_TRY(launch_reduce(scratch, tsplits, q, part, kColsumSplits, d->side));
-    GIB_CUDA_TRY(cudaEventRecord(d->ev_done[half], d->side));
-    d->done_valid[half] = true;
-    const int prev = d->pending;      // the job before this one must be complete before the caller's next dX GEMM
-    d->pending = half;
-    d->last = half;
-    if (prev >= 0 && prev != half) GIB_CUDA_TRY(cudaStreamWaitEvent(st, d->ev_done[prev], 0));
-    return 0;
-  }
   GIB_TRY(dw_join(st));               // fp32 SIMT path: everything on the caller's stream, nothing left pending
   int splits, chunk;
   gemm_dw_plan(q.M, q.Nn, q.Kk, &splits, &chunk);

@@ -2,8 +2,9 @@
 //
 //   NT :  C[M, :N]   = epi( A[M,K] * W[N,K]^T )     A = fp32 activations (row-major, K contiguous), W = a packed weight,
 //                                                    given as its TF32 hi / lo planes (gib_model_pack) or raw fp32
-//   TN :  P[z][n][k] = sum_{m in chunk z} G[m,n] * X[m,k]   (weight-gradient partials; G, X fp32 row-major activations)
-//         pb[z][n]   = sum_{m in chunk z} G[m,n]            (bias-gradient partials, from the G fragments in registers)
+//   TN :  P[s][n][k] = sum_{m in segment s} G[m,n] * X[m,k]   (weight-gradient partial tiles; G, X fp32 row-major
+//         pb[s][n]   = sum_{m in segment s} G[m,n]            activations; bias-gradient partials from the G
+//                                                              fragments in registers; segments: see dw_plan)
 //
 // Why 3xTF32: the parity bar is 1e-4 on the logits; one TF32 pass is 1.8e-2 off (SURVEY.md §7).  Each operand x is
 // split into hi = tf32(x) and lo = x - hi; the product is accumulated as hi*hi + (lo*hi + hi*lo) (the dropped lo*lo term
@@ -25,8 +26,8 @@
 // transpose writes a 16-bit K-major plane; per k-block one group of 2 wgmma.m64n128k16 (A from registers).  No run-time
 // branch in the inner loop; the raw-W mma.sync kernel has no 16-bit instantiation.
 //
-// The kernels are persistent (one CTA per SM, work items = output tiles of up to 16 problems, or (tile, reduction
-// chunk) pairs in TN mode) and fed by one TMA lane through a ring of shared-memory stages (cp.async.bulk.tensor with
+// The kernels are persistent (one CTA per SM, work items = output tiles of up to 16 problems, or in TN mode the
+// segments of an even split of all k-blocks of the launch) and fed by one TMA lane through a ring of shared-memory stages (cp.async.bulk.tensor with
 // the 128-byte swizzle, mbarrier expect_tx per stage).
 //
 // tc3_wgmma_kernel: NT with W as pre-split (hi, lo) planes, the model's call pattern.  384 threads, 4-stage ring of
@@ -46,7 +47,7 @@
 //                   into a 4-stage ring of 32 KB raw stages;
 //                   warps 9-11: transpose X into X_hi^T / X_lo^T [128 x 32] K-major tiles with the 128-byte swizzle
 //                   (the layout TMA gives the W planes above) in a 3-stage ring of 32 KB plane stages, split with the
-//                   same round-to-nearest, reduction rows past the chunk / row count written as 0
+//                   same round-to-nearest, reduction rows past the segment / row count written as 0
 //   warpgroups 0-1  consumers      64 x 128 outputs each: G^T fragments read in transposed order from the raw boxes and
 //                                  split in registers (the bias-gradient partials are summed from them), X planes
 //                                  through descriptors; the same half-k-block wgmma pipeline as tc3_wgmma_kernel
@@ -140,7 +141,6 @@ constexpr int DW_OFF_SCHED = DW_OFF_BARS + 256;
 constexpr int DW_SMEM_BYTES = DW_OFF_SCHED + 512 + 1024 /*align slack*/;
 static_assert(DW_SMEM_BYTES <= 227 * 1024, "weight-gradient stages exceed the shared memory of an SM");
 
-constexpr int kMaxChunkRows = 4096;   // reduction rows per work item of the weight-gradient mode
 constexpr int MAXP = kTc3MaxProblems;   // 16: e.g. the 5 layers x 3 bond types of a message MLP as one dependent chain
 
 struct Maps {   // TMA descriptors in kernel-parameter space
@@ -151,13 +151,9 @@ struct Maps {   // TMA descriptors in kernel-parameter space
 };
 
 struct Params {
-  GemmNT g[MAXP];           // TN: A = G, B = X, M = rows (capacity when m_dev is set), C = partials of the problem,
-                            //     ldc = Kk, N = n_store = n_valid = Kk
-  int n_tiles[MAXP];        // column tiles of the output (NT: ceil(N / tile width), TN: ceil(Kk / DW_BN))
-  int k_blocks[MAXP];       // NT: ceil(K / 32)
-  int tn_mt[MAXP];          // TN: ceil(Nn / 128)
-  int tn_nn[MAXP];          // TN: Nn
-  float* bias_part[MAXP];   // TN: [splits][Nn] partial column sums of G (nullptr: not wanted)
+  GemmNT g[MAXP];
+  int n_tiles[MAXP];        // column tiles of the output: ceil(N / tile width)
+  int k_blocks[MAXP];       // ceil(K / 32)
   // dependent chains (NT): problem p reads as its A operand what problem dep[p] writes (the next layer of an MLP);
   // a tile of p at row block i may start once all n_tiles[dep[p]] tiles of row block i of dep[p] are stored.
   // flags[flag_off[p] + i] counts the stored tiles of row block i of problem p (zeroed by the host before the launch).
@@ -165,42 +161,132 @@ struct Params {
   int flag_off[MAXP];
   int* flags;
   int nprob;
-  int chunk_rows;           // TN: reduction rows per work item (multiple of 32)
   long long* trace;         // diagnosis: per-tile clock64 stamps of CTA 0 ([tile][16] int64, gib_tc_trace), else nullptr
   int trace_tiles;
 };
 
 struct Sched {              // computed once per CTA from host values or the device-side row counts
-  int M[MAXP], base[MAXP], begin[MAXP + 1], splits[MAXP];
+  int M[MAXP], base[MAXP], begin[MAXP + 1];
 };
 
 struct Item { int p, m0, n0, nkb, z, r0, rows; };
 
 // TBN: output tile width of the kernel
-template <bool TN, int TBN>
+template <int TBN>
 __device__ __forceinline__ Item decode_item(const Params& P, const Sched& S, int item) {
   Item it;
   int p = 0;
   while (p + 1 < P.nprob && item >= S.begin[p + 1]) ++p;
   const int local = item - S.begin[p];
   it.p = p;
-  if constexpr (TN) {
-    const int tiles_mn = P.tn_mt[p] * P.n_tiles[p];
-    const int tile = local % tiles_mn;
-    it.z = local / tiles_mn;
-    it.m0 = (tile / P.n_tiles[p]) * BM;
-    it.n0 = (tile % P.n_tiles[p]) * TBN;
-    it.r0 = it.z * P.chunk_rows;
-    it.rows = min(S.M[p], it.r0 + P.chunk_rows) - it.r0;
-    it.nkb = ceil_div(it.rows, BKF);
-  } else {
-    it.z = 0; it.r0 = 0; it.rows = 0;
-    it.m0 = (local / P.n_tiles[p]) * BM;
-    it.n0 = (local % P.n_tiles[p]) * TBN;
-    it.nkb = P.k_blocks[p];
-  }
+  it.z = 0; it.r0 = 0; it.rows = 0;
+  it.m0 = (local / P.n_tiles[p]) * BM;
+  it.n0 = (local % P.n_tiles[p]) * TBN;
+  it.nkb = P.k_blocks[p];
   return it;
 }
+
+// ---- schedule of a weight-gradient launch: an even split of its k-blocks (stream-K) -------------------------------
+// A work unit is one k-block (32 reduction rows) of one 128 x 128 output tile of one member; units are numbered
+// member-major, then tile, then k-block, U in all.  CTA b of G = min(SMs, ceil(U / 8)) takes the units
+// [floor(U b / G), floor(U (b + 1) / G)) -- at least one, about U / G -- and cuts them at tile boundaries into
+// segments.  The segment of CTA b in tile gt (tile index over the whole group) writes its partial tile to scratch slot
+// b + gt: the CTAs that cover one tile are consecutive and a CTA's tiles are consecutive, so no two segments share a
+// slot and every slot is below G + T (T: tiles of the group).  The reduction sums, for each tile, the slots of the
+// CTAs owner(first unit) .. owner(last unit) in that order.  The split depends on the live row counts, the member
+// shapes and the SM count only, never on a buffer's capacity: a launch on device-side row counts computes what the
+// same launch on host counts computes, bit for bit.
+constexpr int kDwMinUnits = 8;    // k-blocks per CTA at least: amortise the tile drain
+
+struct DwGroup {                  // the schedule inputs of a launch, shared by the GEMM and the reduction
+  const int* m_dev[MAXP];         // device-side row count inside a buffer of M rows (nullptr: M is the count)
+  const int* base_dev[MAXP];
+  int M[MAXP];
+  int mt[MAXP], nt[MAXP];         // tiles of the output: ceil(Nn / 128) x ceil(Kk / 128)
+  int n, sms;
+};
+
+struct DwPlan {
+  long long U;
+  long long ubegin[MAXP + 1];     // first unit of each member
+  int tbegin[MAXP + 1];           // first tile of each member
+  int M[MAXP], base[MAXP], kb[MAXP], nt[MAXP];   // live rows, first row, k-blocks per tile, column tiles
+  int n, G;
+};
+static_assert(sizeof(DwPlan) <= 512, "the plan lives in the 512-byte schedule area of the kernel's shared memory");
+
+// the plan from live row counts (host: the schedule test hook; device: dw_plan_dev)
+__host__ __device__ inline void dw_plan(DwPlan& S, const int* live, const int* base, const int* mt, const int* nt, int n,
+                                        int sms) {
+  long long u = 0;
+  int t = 0;
+  for (int p = 0; p < n; ++p) {
+    S.M[p] = live[p]; S.base[p] = base[p]; S.nt[p] = nt[p];
+    S.kb[p] = ceil_div(live[p], BKF);
+    S.ubegin[p] = u; S.tbegin[p] = t;
+    u += (long long)mt[p] * nt[p] * S.kb[p];
+    t += mt[p] * nt[p];
+  }
+  S.ubegin[n] = u; S.tbegin[n] = t;
+  S.n = n; S.U = u;
+  const long long g = ceil_div_ll(u, kDwMinUnits);
+  S.G = (int)(g < sms ? g : sms);
+}
+
+// the plan of a launch, from its host or device-side row counts (clamped to the buffer as init_sched clamps them)
+__device__ inline void dw_plan_dev(const DwGroup& g, DwPlan& S) {
+  for (int p = 0; p < g.n; ++p) {   // into S.M / S.base, which dw_plan keeps
+    const int base = g.base_dev[p] ? __ldg(g.base_dev[p]) : 0;
+    int M = g.M[p];
+    if (g.m_dev[p]) {
+      M = __ldg(g.m_dev[p]);
+      if (M > g.M[p] - base) M = g.M[p] - base;
+      if (M < 0) M = 0;
+    }
+    S.M[p] = M; S.base[p] = base;
+  }
+  dw_plan(S, S.M, S.base, g.mt, g.nt, g.n, g.sms);
+}
+
+// units [u0, u1) of CTA b (empty for b >= G)
+__host__ __device__ inline void dw_range(const DwPlan& S, int b, long long& u0, long long& u1) {
+  if (b >= S.G) { u0 = u1 = 0; return; }
+  u0 = S.U * b / S.G;
+  u1 = S.U * (b + 1) / S.G;
+}
+
+// the CTA whose range holds unit u < U
+__host__ __device__ inline int dw_owner(const DwPlan& S, long long u) { return (int)(((u + 1) * S.G - 1) / S.U); }
+
+// the segment of CTA b that starts at unit u < u1 (the end of its range): z = its scratch slot, r0 / rows = its
+// reduction rows relative to the member's first row
+__host__ __device__ inline Item dw_segment(const DwPlan& S, int b, long long u, long long u1) {
+  int p = 0;
+  while (p + 1 < S.n && u >= S.ubegin[p + 1]) ++p;
+  const long long local = u - S.ubegin[p];
+  const int t = (int)(local / S.kb[p]);
+  const int k = (int)(local - (long long)t * S.kb[p]);
+  const long long left = u1 - u;
+  Item it;
+  it.p = p;
+  it.m0 = (t / S.nt[p]) * BM;
+  it.n0 = (t % S.nt[p]) * DW_BN;
+  it.nkb = left < S.kb[p] - k ? (int)left : S.kb[p] - k;
+  it.z = b + S.tbegin[p] + t;
+  it.r0 = k * BKF;
+  it.rows = S.M[p] - it.r0 < it.nkb * BKF ? S.M[p] - it.r0 : it.nkb * BKF;
+  return it;
+}
+
+struct DwParams {
+  DwGroup grp;
+  int Nn[MAXP], Kk[MAXP];
+  unsigned bias_mask;             // bit p: member p wants the bias-gradient partials
+  float* part;                    // [slots][128][128] partial tiles (row: G column - m0, column: X column - n0)
+  float* part_bias;               // [slots][128] partial column sums of G (tiles with n0 == 0)
+  long long* trace;               // as Params::trace
+  int trace_tiles;
+};
 
 __device__ __forceinline__ float lds32(uint32_t saddr) {
   float v;
@@ -287,7 +373,6 @@ __device__ __forceinline__ float epi_one(float v, float b, float x, int mode, in
 }
 
 // Schedule of the launch from host values or the device-side row counts (thread 0 only).
-template <bool TN>
 __device__ __forceinline__ void init_sched(const Params& P, Sched& S) {
   int total = 0;
   for (int p = 0; p < P.nprob; ++p) {
@@ -300,14 +385,7 @@ __device__ __forceinline__ void init_sched(const Params& P, Sched& S) {
       if (M < 0) M = 0;
     }
     S.M[p] = M; S.base[p] = base; S.begin[p] = total;
-    if constexpr (TN) {
-      const int s = ceil_div(M, P.chunk_rows);
-      S.splits[p] = s;
-      total += P.tn_mt[p] * P.n_tiles[p] * s;
-    } else {
-      S.splits[p] = 1;
-      total += ceil_div(M, BM) * P.n_tiles[p];
-    }
+    total += ceil_div(M, BM) * P.n_tiles[p];
   }
   for (int p = P.nprob; p <= MAXP; ++p) S.begin[p] = total;
 }
@@ -412,7 +490,7 @@ tc3_gemm_kernel(const __grid_constant__ Maps maps, const Params P) {
       mbar_init(&empty[s], CONS_WARPS);     // one arrival per consumer warp (after __syncwarp)
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    init_sched<false>(P, S);
+    init_sched(P, S);
   }
   __syncthreads();
   const int num_items = S.begin[MAXP];
@@ -423,7 +501,7 @@ tc3_gemm_kernel(const __grid_constant__ Maps maps, const Params P) {
       int stage = 0;
       uint32_t phase = 0;
       for (int item = blockIdx.x; item < num_items; item += gridDim.x) {
-        const Item w = decode_item<false, BN>(P, S, item);
+        const Item w = decode_item<BN>(P, S, item);
         const int base = S.base[w.p];
         if (P.flags && P.dep[w.p] >= 0) wait_rows(P, w);
         for (int kb = 0; kb < w.nkb; ++kb) {
@@ -444,7 +522,7 @@ tc3_gemm_kernel(const __grid_constant__ Maps maps, const Params P) {
     uint32_t phase = 0;
     int it = 0;
     for (int item = blockIdx.x; item < num_items; item += gridDim.x, ++it) {
-      const Item w = decode_item<false, BN>(P, S, item);
+      const Item w = decode_item<BN>(P, S, item);
       const bool tr = P.trace && blockIdx.x == 0 && it < P.trace_tiles && threadIdx.x == 0;
       if (tr) P.trace[it * 16 + 0] = clock64();
       float acc[MI][NI][4], accx[MI][NI][4];
@@ -607,7 +685,7 @@ tc3_wgmma_kernel(const __grid_constant__ Maps maps, const Params P) {
       mbar_init(epi_empty, WG_STORE_WARPS);
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    init_sched<false>(P, S);
+    init_sched(P, S);
   }
   __syncthreads();
   const int num_items = S.begin[MAXP];
@@ -619,7 +697,7 @@ tc3_wgmma_kernel(const __grid_constant__ Maps maps, const Params P) {
       int stage = 0;
       uint32_t phase = 0;
       for (int item = blockIdx.x; item < num_items; item += gridDim.x) {
-        const Item w = decode_item<false, WG_BN>(P, S, item);
+        const Item w = decode_item<WG_BN>(P, S, item);
         const int base = S.base[w.p];
         if (P.flags && P.dep[w.p] >= 0) wait_rows(P, w);
         for (int kb = 0; kb < w.nkb; ++kb) {
@@ -635,7 +713,7 @@ tc3_wgmma_kernel(const __grid_constant__ Maps maps, const Params P) {
     } else if (SE && warp == CONS_WARPS + 1) {
       uint32_t phase = 0;
       for (int item = blockIdx.x; item < num_items; item += gridDim.x, phase ^= 1) {
-        const Item w = decode_item<false, WG_BN>(P, S, item);
+        const Item w = decode_item<WG_BN>(P, S, item);
         const GemmNT& g = P.g[w.p];
         mbar_wait(epi_empty, phase ^ 1);
         if constexpr (AUX) {
@@ -663,7 +741,7 @@ tc3_wgmma_kernel(const __grid_constant__ Maps maps, const Params P) {
       uint32_t phase = 0;
       int it = 0;
       for (int item = blockIdx.x; item < num_items; item += gridDim.x, phase ^= 1, ++it) {
-        const Item w = decode_item<false, WG_BN>(P, S, item);
+        const Item w = decode_item<WG_BN>(P, S, item);
         const GemmNT& g = P.g[w.p];
         const int rows = min(BM, S.M[w.p] - w.m0);
         const int chunks = min(WG_BN, g.n_store - w.n0) >> 2;    // 16-byte chunks per row (n_store % 4 == 0)
@@ -694,7 +772,7 @@ tc3_wgmma_kernel(const __grid_constant__ Maps maps, const Params P) {
     uint32_t phase = 0;
     int it = 0;
     for (int item = blockIdx.x; item < num_items; item += gridDim.x, ++it) {
-      const Item w = decode_item<false, WG_BN>(P, S, item);
+      const Item w = decode_item<WG_BN>(P, S, item);
       const bool tr = P.trace && blockIdx.x == 0 && it < P.trace_tiles && threadIdx.x == 0;
       if (tr) P.trace[it * 16 + 0] = clock64();
       float acc[64], accx[64];
@@ -879,7 +957,7 @@ __device__ __forceinline__ void dw_transpose_block16(uint32_t sx, uint32_t sp, i
 // of 2 k16 wgmma per k-block.
 template <bool TF1, int H16 = 0>
 __global__ void __launch_bounds__(WG_THREADS, 1)
-tc3_wgmma_dw_kernel(const __grid_constant__ Maps maps, const Params P) {
+tc3_wgmma_dw_kernel(const __grid_constant__ Maps maps, const DwParams P) {
   static_assert(H16 == 0 || TF1, "16-bit operands use the single accumulator");
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
@@ -888,7 +966,7 @@ tc3_wgmma_dw_kernel(const __grid_constant__ Maps maps, const Params P) {
   uint64_t* raw_empty = raw_full + DW_RAW_STAGES;       // [DW_RAW_STAGES] consumers + transposers -> TMA
   uint64_t* pl_full = raw_empty + DW_RAW_STAGES;        // [DW_PLANE_STAGES] transposers -> consumers
   uint64_t* pl_empty = pl_full + DW_PLANE_STAGES;       // [DW_PLANE_STAGES] consumers -> transposers
-  Sched& S = *reinterpret_cast<Sched*>(smem + DW_OFF_SCHED);
+  DwPlan& S = *reinterpret_cast<DwPlan*>(smem + DW_OFF_SCHED);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
@@ -902,10 +980,12 @@ tc3_wgmma_dw_kernel(const __grid_constant__ Maps maps, const Params P) {
       mbar_init(&pl_empty[s], CONS_WARPS);   // once the last wgmma group reading the planes has retired
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    init_sched<true>(P, S);
+    dw_plan_dev(P.grp, S);
   }
   __syncthreads();
-  const int num_items = S.begin[MAXP];
+  // every role walks the same segments: this CTA's units [u0, u1), cut at tile boundaries
+  long long u0, u1;
+  dw_range(S, blockIdx.x, u0, u1);
 
   if (warp >= CONS_WARPS) {
     asm volatile("setmaxnreg.dec.sync.aligned.u32 56;");
@@ -914,8 +994,9 @@ tc3_wgmma_dw_kernel(const __grid_constant__ Maps maps, const Params P) {
       if (lane == 0) {
         int stage = 0;
         uint32_t phase = 0;
-        for (int item = blockIdx.x; item < num_items; item += gridDim.x) {
-          const Item w = decode_item<true, DW_BN>(P, S, item);
+        for (long long u = u0; u < u1;) {
+          const Item w = dw_segment(S, blockIdx.x, u, u1);
+          u += w.nkb;
           const int row = S.base[w.p] + w.r0;
           for (int kb = 0; kb < w.nkb; ++kb) {
             mbar_wait(&raw_empty[stage], phase ^ 1);
@@ -936,8 +1017,9 @@ tc3_wgmma_dw_kernel(const __grid_constant__ Maps maps, const Params P) {
       const int tt = threadIdx.x - 32 * (CONS_WARPS + 1);
       int rs = 0, ps = 0;
       uint32_t rph = 0, pph = 0;
-      for (int item = blockIdx.x; item < num_items; item += gridDim.x) {
-        const Item w = decode_item<true, DW_BN>(P, S, item);
+      for (long long u = u0; u < u1;) {
+        const Item w = dw_segment(S, blockIdx.x, u, u1);
+        u += w.nkb;
         for (int kb = 0; kb < w.nkb; ++kb) {
           mbar_wait(&pl_empty[ps], pph ^ 1);
           mbar_wait(&raw_full[rs], rph);
@@ -969,15 +1051,16 @@ tc3_wgmma_dw_kernel(const __grid_constant__ Maps maps, const Params P) {
     int rs = 0, ps = 0;
     uint32_t rph = 0, pph = 0;
     int it = 0;
-    for (int item = blockIdx.x; item < num_items; item += gridDim.x, ++it) {
-      const Item w = decode_item<true, DW_BN>(P, S, item);
+    for (long long u = u0; u < u1; ++it) {
+      const Item w = dw_segment(S, blockIdx.x, u, u1);
+      u += w.nkb;
       const bool tr = P.trace && blockIdx.x == 0 && it < P.trace_tiles && threadIdx.x == 0;
       if (tr) P.trace[it * 16 + 0] = clock64();
       float acc[64], accx[64];
 #pragma unroll
       for (int e = 0; e < 64; ++e) { acc[e] = 0.f; accx[e] = 0.f; }
       float cs0 = 0.f, cs1 = 0.f;                // bias-gradient partials of this lane's G columns
-      const bool want_cs = P.bias_part[w.p] && w.n0 == 0;
+      const bool want_cs = ((P.bias_mask >> w.p) & 1u) && w.n0 == 0;
 
       // the pipeline of tc3_wgmma_kernel: half a k-block of fragments per buffer and wgmma group, wait_group 1; the
       // raw stage (G only) is released as soon as the fragments of its half 1 are in registers, the plane stage once
@@ -991,7 +1074,7 @@ tc3_wgmma_dw_kernel(const __grid_constant__ Maps maps, const Params P) {
           float a[4];
           a[0] = lds32(sg + go0 + swz(k0, c0)); a[1] = lds32(sg + go1 + swz(k0, c1));
           a[2] = lds32(sg + go0 + swz(k1, c0)); a[3] = lds32(sg + go1 + swz(k1, c1));
-          if (k0 >= valid) { a[0] = 0.f; a[1] = 0.f; }   // rows past the chunk / row count may hold anything
+          if (k0 >= valid) { a[0] = 0.f; a[1] = 0.f; }   // rows past the segment / row count may hold anything
           if (k1 >= valid) { a[2] = 0.f; a[3] = 0.f; }
           if (want_cs) { cs0 += a[0] + a[2]; cs1 += a[1] + a[3]; }
 #pragma unroll
@@ -1025,7 +1108,7 @@ tc3_wgmma_dw_kernel(const __grid_constant__ Maps maps, const Params P) {
             float a[4];
             a[0] = lds32(sg + go0 + swz(k, c0)); a[1] = lds32(sg + go0 + swz(k + 1, c0));
             a[2] = lds32(sg + go1 + swz(k, c1)); a[3] = lds32(sg + go1 + swz(k + 1, c1));
-            if (k >= valid) { a[0] = 0.f; a[2] = 0.f; }     // rows past the chunk / row count may hold anything
+            if (k >= valid) { a[0] = 0.f; a[2] = 0.f; }     // rows past the segment / row count may hold anything
             if (k + 1 >= valid) { a[1] = 0.f; a[3] = 0.f; }
             if (want_cs) { cs0 += a[0] + a[1]; cs1 += a[2] + a[3]; }
             f[s][2 * h] = pack16<H16 ? H16 : 1>(a[0], a[1]);
@@ -1064,32 +1147,31 @@ tc3_wgmma_dw_kernel(const __grid_constant__ Maps maps, const Params P) {
       __syncwarp();
       if (lane == 0) mbar_arrive(&pl_empty[prev]);
 
-      const int Nn = P.tn_nn[w.p];
+      // the partial tile into the segment's slot, at tile-local coordinates
+      const int Nn = P.Nn[w.p], Kk = P.Kk[w.p];
       if (want_cs) {
-        float* bp = P.bias_part[w.p] + (size_t)w.z * Nn;
+        float* bp = P.part_bias + (size_t)w.z * BM;
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
           float s = h ? cs1 : cs0;
           s += __shfl_xor_sync(0xffffffffu, s, 1);
           s += __shfl_xor_sync(0xffffffffu, s, 2);
-          const int n = w.m0 + r0 + h * 8;
-          if (t4 == 0 && n < Nn) bp[n] = s;
+          const int m = r0 + h * 8;
+          if (t4 == 0 && w.m0 + m < Nn) bp[m] = s;
         }
       }
-      const GemmNT& g = P.g[w.p];
-      const EpiArgs e = epi_args(g, g.C + (size_t)w.z * Nn * g.ldc, 0, Nn);
+      float* const out = P.part + (size_t)w.z * (BM * DW_BN);
 #pragma unroll
       for (int j = 0; j < DW_BN / 8; ++j) {
-        const int n = w.n0 + j * 8 + 2 * t4;      // this lane's column pair
-        if (n >= e.n_store) continue;
-        float b[2];
-        epi_bias<EPI_SPEC_LINEAR>(e, n, b);
+        const int n = j * 8 + 2 * t4;             // this lane's column pair (Kk % 4 == 0: both valid or neither)
+        if (w.n0 + n >= Kk) continue;
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
-          const int m = w.m0 + r0 + h * 8;
-          if (m >= Nn) continue;
-          epi_store<EPI_SPEC_LINEAR>(e, m, n, acc_total<TF1>(acc[4 * j + 2 * h], accx[4 * j + 2 * h]),
-                                     acc_total<TF1>(acc[4 * j + 2 * h + 1], accx[4 * j + 2 * h + 1]), b);
+          const int m = r0 + h * 8;
+          if (w.m0 + m >= Nn) continue;
+          *reinterpret_cast<float2*>(out + m * DW_BN + n) =
+              make_float2(acc_total<TF1>(acc[4 * j + 2 * h], accx[4 * j + 2 * h]),
+                          acc_total<TF1>(acc[4 * j + 2 * h + 1], accx[4 * j + 2 * h + 1]));
         }
       }
       if (tr) P.trace[it * 16 + 6] = clock64();
@@ -1097,65 +1179,50 @@ tc3_wgmma_dw_kernel(const __grid_constant__ Maps maps, const Params P) {
   }
 }
 
-// ---- fixed-order reduction of the split partials into the gradient tensors, all problems of a group in one launch.
-//      blocks [blk_w[p], blk_b[p]):    dW_p[r*rs + c*cs] += sum_z ws_p[z][prow(r)][c]   (one thread per element)
-//      blocks [blk_b[p], blk_w[p+1]):  db_p[r]           += sum_z wsb_p[z][prow(r)]     (32 rows per block)
-//      z runs over the problem's split count, recomputed here from the same host / device row count the GEMM used.
+// ---- fixed-order reduction of the partial tiles into the gradient tensors, all problems of a group in one launch.
+//      blocks [blk_w[p], blk_b[p]):    dW_p[r*rs + c*cs] += sum_b part[b + gt][prow(r) % 128][c % 128]   (one thread per
+//                                      element; gt: the tile of (prow(r), c), b: the CTAs that cover it, ascending)
+//      blocks [blk_b[p], blk_w[p+1]):  db_p[r]           += sum_b part_bias[b + gt][prow(r) % 128]  (gt: column tile 0)
+//      The segments are recomputed from the same host / device row counts the GEMM used (dw_plan_dev).
 struct ReduceProb {
-  const float* ws; const float* wsb; float* dW; float* db;
-  const int* m_dev; const int* base_dev; int M;
-  int Nn, Kk, R, C, Rb, Rbp;
+  float* dW; float* db;
+  int R, C, Rb, Rbp;
   long long rs, cs;
   int blk_w, blk_b;
 };
-struct ReduceTable { ReduceProb q[MAXP]; int n, total_blocks, chunk_rows; };
+struct ReduceTable { DwGroup grp; ReduceProb q[MAXP]; const float* part; const float* part_bias; };
 
 __global__ void __launch_bounds__(256) reduce_grads3_kernel(const ReduceTable T) {
+  __shared__ DwPlan S;
+  if (threadIdx.x == 0) dw_plan_dev(T.grp, S);
+  __syncthreads();
   int p = 0;
-  while (p + 1 < T.n && (int)blockIdx.x >= T.q[p + 1].blk_w) ++p;
+  while (p + 1 < T.grp.n && (int)blockIdx.x >= T.q[p + 1].blk_w) ++p;
   const ReduceProb& q = T.q[p];
-  int M = q.M;
-  if (q.m_dev) {
-    const int base = q.base_dev ? __ldg(q.base_dev) : 0;
-    M = __ldg(q.m_dev);
-    if (M > q.M - base) M = q.M - base;
-    if (M < 0) M = 0;
-  }
-  const int splits = ceil_div(M, T.chunk_rows);
+  const int kb = S.kb[p];
+  // the slots of tile t of problem p, in the order of the CTAs that cover it
+  auto sum_tile = [&](const float* src, int t, size_t slot_floats) {
+    float s = 0.f;
+    if (kb > 0) {
+      const long long u = S.ubegin[p] + (long long)t * kb;
+      const int b1 = dw_owner(S, u + kb - 1);
+      src += (size_t)(S.tbegin[p] + t) * slot_floats;
+      for (int b = dw_owner(S, u); b <= b1; ++b) s += src[(size_t)b * slot_floats];
+    }
+    return s;
+  };
   if ((int)blockIdx.x < q.blk_b) {
     const long long idx = (long long)((int)blockIdx.x - q.blk_w) * 256 + threadIdx.x;
     if (idx >= (long long)q.R * q.C) return;
     const int r = (int)(idx / q.C), c = (int)(idx % q.C);
     const int prow = (r / q.Rb) * q.Rbp + (r % q.Rb);
-    const float* src = q.ws + (size_t)prow * q.Kk + c;
-    const size_t stride = (size_t)q.Nn * q.Kk;
-    float s = 0.f;
-    int zi = 0;
-    for (; zi + 8 <= splits; zi += 8) {      // 8 independent loads in flight, summed in ascending z
-      float v[8];
-#pragma unroll
-      for (int u = 0; u < 8; ++u) v[u] = src[(size_t)(zi + u) * stride];
-#pragma unroll
-      for (int u = 0; u < 8; ++u) s += v[u];
-    }
-    for (; zi < splits; ++zi) s += src[(size_t)zi * stride];
-    q.dW[r * q.rs + c * q.cs] += s;
+    const int t = (prow / BM) * S.nt[p] + c / DW_BN;
+    q.dW[r * q.rs + c * q.cs] += sum_tile(T.part + (prow % BM) * DW_BN + c % DW_BN, t, (size_t)BM * DW_BN);
   } else {
-    __shared__ float sm[8][33];
-    const int r = ((int)blockIdx.x - q.blk_b) * 32 + (threadIdx.x & 31);
-    const int wy = threadIdx.x >> 5;
-    float s = 0.f;
-    if (r < q.R) {
-      const int prow = (r / q.Rb) * q.Rbp + (r % q.Rb);
-      for (int zi = wy; zi < splits; zi += 8) s += q.wsb[(size_t)zi * q.Nn + prow];
-    }
-    sm[wy][threadIdx.x & 31] = s;
-    __syncthreads();
-    if (wy == 0 && r < q.R) {
-      float t = 0.f;
-      for (int k = 0; k < 8; ++k) t += sm[k][threadIdx.x];
-      q.db[r] += t;
-    }
+    const int r = ((int)blockIdx.x - q.blk_b) * 256 + threadIdx.x;
+    if (r >= q.R) return;
+    const int prow = (r / q.Rb) * q.Rbp + (r % q.Rb);
+    q.db[r] += sum_tile(T.part_bias + prow % BM, (prow / BM) * S.nt[p], BM);
   }
 }
 
@@ -1485,61 +1552,42 @@ bool tc3_dw_eligible(const GemmDW& q) {
          (q.ldx % 4) == 0 && al(q.G) && al(q.X);
 }
 
-// Reduction rows per work item for a group: about one work item per SM, within [256, kMaxChunkRows].
-int tc3_dw_chunk_rows(const GemmDW* qs, int n, long long plan_rows) {
+// the schedule inputs of a launch (the members' host row counts, or their buffers' rows with m_dev)
+static void dw_group(const GemmDW* qs, int n, int sms, tc3::DwGroup& g) {
   using namespace tc3;
-  const int num_sms = device_sm_count();
-  int max_tiles = 1;
-  long long rows = 0;
+  memset(&g, 0, sizeof(g));
+  g.n = n; g.sms = sms;
   for (int i = 0; i < n; ++i) {
-    if (qs[i].M <= 0) continue;
-    max_tiles = std::max(max_tiles, ceil_div(qs[i].Nn, BM) * ceil_div(qs[i].Kk, DW_BN));
-    rows += qs[i].M;
+    g.m_dev[i] = qs[i].m_dev; g.base_dev[i] = qs[i].base_dev; g.M[i] = qs[i].M;
+    g.mt[i] = ceil_div(qs[i].Nn, BM); g.nt[i] = ceil_div(qs[i].Kk, DW_BN);
   }
-  if (plan_rows > 0) rows = plan_rows;
-  // whole rounds of work items: r rounds of num_sms items, the fewest rounds whose chunk respects the cap (a capped
-  // chunk that leaves a few items for an extra round would double the kernel time)
-  long long c = 8 * BKF;
-  for (int r = 1; r <= 64; ++r) {
-    c = ceil_div_ll(rows * max_tiles, (long long)r * num_sms);
-    c = ceil_div_ll(c, BKF) * BKF;
-    if (c <= kMaxChunkRows) break;                    // bounded accumulation chains per work item
-  }
-  if (c > kMaxChunkRows) c = kMaxChunkRows;
-  if (c < 8 * BKF) c = 8 * BKF;                       // >= 256 reduction rows per item: amortise the tile drain
-  return (int)c;
 }
 
-// Scratch layout of a group: per problem [cap_splits][Nn][Kk] partial products, then [cap_splits][Nn] bias partials.
-void tc3_dw_layout(const GemmDW* qs, int n, int chunk_rows, Dw3Layout* L) {
+// Scratch of a group: one partial tile [128][128] and one bias partial [128] per slot.  dw_plan needs at most G + T
+// slots; G = min(SMs, ceil(U / 8)) is bounded here with U from q.M (the capacity when the count is on the device).
+void tc3_dw_layout(const GemmDW* qs, int n, Dw3Layout* L) {
   using namespace tc3;
-  L->chunk_rows = chunk_rows;
-  size_t off = 0;
-  for (int i = 0; i < MAXP; ++i) {
-    if (i < n) {
-      const int s = std::max(1, ceil_div(qs[i].M, L->chunk_rows));
-      L->cap_splits[i] = s;
-      L->part_off[i] = off; off += (size_t)s * qs[i].Nn * qs[i].Kk;
-      L->bias_off[i] = off; off += (size_t)s * qs[i].Nn;
-      off = (off + 31) & ~(size_t)31;
-    } else {
-      L->cap_splits[i] = 0; L->part_off[i] = L->bias_off[i] = off;
-    }
+  int tiles = 0;
+  long long units = 0;
+  for (int i = 0; i < n; ++i) {
+    const int t = ceil_div(qs[i].Nn, BM) * ceil_div(qs[i].Kk, DW_BN);
+    tiles += t;
+    units += (long long)t * ceil_div(std::max(qs[i].M, 0), BKF);
   }
-  L->floats = off;
+  L->slots = (int)std::min<long long>(device_sm_count(), ceil_div_ll(units, kDwMinUnits)) + tiles;
+  L->floats = (size_t)L->slots * (BM * DW_BN + BM);
 }
 
-// partial products (+ bias partials where bias_part is set) of up to MAXP weight-gradient problems in one launch
-static int launch_tn(const GemmDW* qs, int n, int chunk_rows, float* const* part, float* const* bias_part,
-                     cudaStream_t st) {
+int gemm_dw_tc3_partials(const GemmDW* qs, int n, const Dw3Layout& L, float* scratch, cudaStream_t st) {
   using namespace tc3;
   if (n < 1 || n > MAXP) { set_error("gemm_dw_tc3_partials: %d problems (max %d)", n, MAXP); return -2; }
   int num_sms = 0;
   GIB_TRY(prepare(&num_sms));
   Maps maps;
-  Params P;
+  DwParams P;
   memset(&P, 0, sizeof(P));
-  long long items = 0;
+  dw_group(qs, n, num_sms, P.grp);
+  long long units = 0;        // upper bound when a row count lives on the device
   const int prec = qs[0].tf32;
   const bool tf32 = prec != 0;
   if (prec < 0 || prec > 3) { set_error("gemm_dw_tc3: unknown precision %d", prec); return -2; }
@@ -1549,22 +1597,16 @@ static int launch_tn(const GemmDW* qs, int n, int chunk_rows, float* const* part
     if (q.tf32 != prec) { set_error("gemm_dw_tc3: problems of one launch with different precisions"); return -2; }
     GIB_TRY(make_map(&maps.a[i], q.G, q.M, q.Nn, q.ldg, BKF));          // 32 x 32 boxes
     GIB_TRY(make_map(&maps.b[i], q.X, q.M, q.Kk, q.ldx, BKF));
-    GemmNT& g = P.g[i];
-    g = GemmNT();
-    g.A = q.G; g.lda = q.ldg; g.B = q.X; g.ldb = q.ldx;
-    g.M = q.M; g.m_dev = q.m_dev; g.base_dev = q.base_dev;
-    g.C = part[i]; g.ldc = q.Kk; g.N = q.Kk; g.n_store = q.Kk; g.n_valid = q.Kk;
-    g.mode = EPI_ACT; g.act = ACT_NONE; g.bias = nullptr;
-    P.n_tiles[i] = ceil_div(q.Kk, DW_BN);
-    P.tn_mt[i] = ceil_div(q.Nn, BM);
-    P.tn_nn[i] = q.Nn;
-    P.bias_part[i] = bias_part[i];
-    items += (long long)P.tn_mt[i] * P.n_tiles[i] * std::max(1, ceil_div(q.M, chunk_rows));
+    P.Nn[i] = q.Nn; P.Kk[i] = q.Kk;
+    if (q.dbias) P.bias_mask |= 1u << i;
+    units += (long long)P.grp.mt[i] * P.grp.nt[i] * ceil_div(q.M, BKF);
   }
-  P.nprob = n;
-  P.chunk_rows = chunk_rows;
+  P.part = scratch;
+  P.part_bias = scratch + (size_t)L.slots * BM * DW_BN;
   P.trace = g_trace; P.trace_tiles = g_trace_tiles;
-  const int grid = (int)(items < num_sms ? items : num_sms);
+  // the device plan's G = min(SMs, ceil(U / 8)) never exceeds this grid; CTAs past it find no units
+  const long long want = std::max(1LL, ceil_div_ll(units, kDwMinUnits));
+  const int grid = (int)std::min<long long>(want, num_sms);
   if (prec == 2) tc3_wgmma_dw_kernel<true, 1><<<grid, WG_THREADS, DW_SMEM_BYTES, st>>>(maps, P);
   else if (prec == 3) tc3_wgmma_dw_kernel<true, 2><<<grid, WG_THREADS, DW_SMEM_BYTES, st>>>(maps, P);
   else if (tf32) tc3_wgmma_dw_kernel<true><<<grid, WG_THREADS, DW_SMEM_BYTES, st>>>(maps, P);
@@ -1573,63 +1615,67 @@ static int launch_tn(const GemmDW* qs, int n, int chunk_rows, float* const* part
   return 0;
 }
 
-int gemm_dw_tc3_partials(const GemmDW* qs, int n, const Dw3Layout& L, float* scratch, cudaStream_t st) {
-  if (n < 1 || n > tc3::MAXP) { set_error("gemm_dw_tc3_partials: %d problems (max %d)", n, tc3::MAXP); return -2; }
-  float* part[tc3::MAXP];
-  float* bias_part[tc3::MAXP];
-  for (int i = 0; i < n; ++i) {
-    part[i] = scratch + L.part_off[i];
-    bias_part[i] = qs[i].dbias ? scratch + L.bias_off[i] : nullptr;
-  }
-  return launch_tn(qs, n, L.chunk_rows, part, bias_part, st);
-}
-
-// ---- single weight-gradient problem, partials only ([splits][Nn][Kk] into q.scratch; the caller reduces them) ----
-void tc_dw_plan(int M, int Nn, int Kk, int* splits, int* chunk) {
-  const int tiles = ceil_div(Nn, tc3::BM) * ceil_div(Kk, tc3::DW_BN);
-  int s = ceil_div(device_sm_count(), tiles);         // about one work item per SM
-  int c = ceil_div(ceil_div(M, s), tc3::BKF) * tc3::BKF;
-  if (c < 8 * tc3::BKF) c = 8 * tc3::BKF;             // >= 256 reduction rows per item
-  s = ceil_div(M, c);
-  if (s < 1) s = 1;
-  *splits = s;
-  *chunk = c;
-}
-
-bool tc_dw_eligible(const GemmDW& q) {
-  return q.M >= 2048 && q.Nn >= 32 && q.Kk >= 32 && tc3_dw_eligible(q) && !q.m_dev;
-}
-
-int gemm_dw_tc_partials(const GemmDW& q, int* splits_out, cudaStream_t st) {
-  int splits, chunk;
-  tc_dw_plan(q.M, q.Nn, q.Kk, &splits, &chunk);
-  float* part[1] = {q.scratch};
-  float* bias_part[1] = {nullptr};
-  GIB_TRY(launch_tn(&q, 1, chunk, part, bias_part, st));
-  *splits_out = splits;
-  return 0;
-}
-
 // fixed-order reduction of the group's partials into the gradient tensors (any stream ordered after the partials)
 int gemm_dw_tc3_reduce(const GemmDW* qs, int n, const Dw3Layout& L, const float* scratch, cudaStream_t st) {
   using namespace tc3;
+  int num_sms = 0;
+  GIB_TRY(prepare(&num_sms));
   ReduceTable T;
   memset(&T, 0, sizeof(T));
+  dw_group(qs, n, num_sms, T.grp);
+  T.part = scratch;
+  T.part_bias = scratch + (size_t)L.slots * BM * DW_BN;
   int blk = 0;
   for (int i = 0; i < n; ++i) {
     const GemmDW& q = qs[i];
     ReduceProb& r = T.q[i];
-    r.ws = scratch + L.part_off[i]; r.wsb = scratch + L.bias_off[i]; r.dW = q.dW; r.db = q.dbias;
-    r.m_dev = q.m_dev; r.base_dev = q.base_dev; r.M = q.M;
-    r.Nn = q.Nn; r.Kk = q.Kk; r.R = q.R; r.C = q.C; r.Rb = q.Rb; r.Rbp = q.Rbp; r.rs = q.rs; r.cs = q.cs;
+    r.dW = q.dW; r.db = q.dbias;
+    r.R = q.R; r.C = q.C; r.Rb = q.Rb; r.Rbp = q.Rbp; r.rs = q.rs; r.cs = q.cs;
     r.blk_w = blk; blk += q.dW ? (int)ceil_div_ll((long long)q.R * q.C, 256) : 0;
-    r.blk_b = blk; blk += q.dbias ? ceil_div(q.R, 32) : 0;
+    r.blk_b = blk; blk += q.dbias ? ceil_div(q.R, 256) : 0;
   }
-  T.n = n; T.total_blocks = blk; T.chunk_rows = L.chunk_rows;
   if (blk == 0) return 0;
   reduce_grads3_kernel<<<blk, 256, 0, st>>>(T);
   GIB_LAUNCH_CHECK();
   return 0;
+}
+
+// the segments dw_plan gives a group with host row counts (test hook): per segment (CTA, member, tile, first row,
+// rows, slot), per tile the first and last CTA the reduction reads (-1, -1: no rows)
+int tc3_dw_schedule(const int* rows, const int* Nn, const int* Kk, int n, int sms, int* segs, int max_segs,
+                    int* tile_ctas, int* G_out) {
+  using namespace tc3;
+  if (n < 1 || n > MAXP || sms < 1) { set_error("tc3_dw_schedule: n=%d sms=%d", n, sms); return -2; }
+  int mt[MAXP], nt[MAXP], base[MAXP] = {0};
+  for (int i = 0; i < n; ++i) {
+    if (rows[i] < 0) { set_error("tc3_dw_schedule: negative row count"); return -2; }
+    mt[i] = ceil_div(Nn[i], BM); nt[i] = ceil_div(Kk[i], DW_BN);
+  }
+  DwPlan S;
+  dw_plan(S, rows, base, mt, nt, n, sms);
+  *G_out = S.G;
+  int ns = 0;
+  for (int b = 0; b < S.G; ++b) {
+    long long u0, u1;
+    dw_range(S, b, u0, u1);
+    for (long long u = u0; u < u1;) {
+      const Item w = dw_segment(S, b, u, u1);
+      u += w.nkb;
+      if (ns == max_segs) { set_error("tc3_dw_schedule: more than %d segments", max_segs); return -3; }
+      int* o = segs + 6 * ns++;
+      o[0] = b; o[1] = w.p; o[2] = (w.m0 / BM) * nt[w.p] + w.n0 / DW_BN; o[3] = w.r0; o[4] = w.rows; o[5] = w.z;
+    }
+  }
+  for (int p = 0; p < n; ++p)
+    for (int t = 0; t < mt[p] * nt[p]; ++t) {
+      int* o = tile_ctas + 2 * (S.tbegin[p] + t);
+      o[0] = o[1] = -1;
+      if (S.kb[p] > 0) {
+        const long long u = S.ubegin[p] + (long long)t * S.kb[p];
+        o[0] = dw_owner(S, u); o[1] = dw_owner(S, u + S.kb[p] - 1);
+      }
+    }
+  return ns;
 }
 
 }  // namespace gib

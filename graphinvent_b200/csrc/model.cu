@@ -570,25 +570,22 @@ static int sub_group(const Mlp* const* ms, int n, int i) {
 //       every G_l kept in its own buffer;
 //   (B) the weight gradients of ALL layers and members (dW_l = G_l^T X_{l-1}) as ONE grouped launch + ONE reduction;
 //   (C) the first layer's input gradient (if wanted).
-// plan_rows: expected total rows of the members of ONE layer (capacity mode: the entry capacity the bond-type groups
-// share, or n x the capacity for the EMN's siblings, which each span it), 0 = their sum.
 // same_rows (capacity mode): the members run on the SAME device row range (the EMN's siblings) and keep one gradient
 // slice each; otherwise members with device row ranges are the disjoint bond-type groups of ONE buffer of `rows` rows
 // and share one slice.
-static int mlp_backward_multi(const Run& r, const BwdBufs& bb, const MlpBwdJob* jobs, int n, long long plan_rows = 0,
-                              bool same_rows = false) {
+static int mlp_backward_multi(const Run& r, const BwdBufs& bb, const MlpBwdJob* jobs, int n, bool same_rows = false) {
   bool same = n <= 4;
   for (int i = 1; i < n && same; ++i) same = jobs[i].m->n == jobs[0].m->n;
   const int depth = jobs[0].m->n;
   if (!same || depth * n > kTc3MaxProblems) {
     if (jobs[0].m_dev) {
-      // device-side row counts need the grouped call pattern: sub-groups that fit one launch, each planned with the
-      // whole group's plan rows (make_bwd sizes the same split through group_extent)
+      // device-side row counts need the grouped call pattern: sub-groups that fit one launch (make_bwd sizes their
+      // scratch through group_extent)
       const Mlp* ms[4];
       for (int i = 0; i < n; ++i) ms[i] = jobs[i].m;
       for (int i = 0, k; i < n; i += k) {
         k = sub_group(ms, n, i);
-        GIB_TRY(mlp_backward_multi(r, bb, jobs + i, k, plan_rows, same_rows));
+        GIB_TRY(mlp_backward_multi(r, bb, jobs + i, k, same_rows));
       }
       return 0;
     }
@@ -664,11 +661,7 @@ static int mlp_backward_multi(const Run& r, const BwdBufs& bb, const MlpBwdJob* 
       const float* Xin = x_in(j, l, &ldxin);
       qs[nq++] = lin_dw(r, bb, L, G[l][i], Xin, ldxin, j.rows, j.m_dev, j.base_dev);
     }
-  GIB_TRY(gemm_dw_group(qs, nq, plan_rows * depth, r.st));
-  // the side-stream reduction reads only its scratch half; a first-generation / SIMT fallback job may still read
-  // the caller's Gtop buffer: finish it before returning
-  if (!(g_use_tc && (g_tc_debug & 1) == 0)) GIB_TRY(dw_join(r.st));
-  return 0;
+  return gemm_dw_group(qs, nq, r.st);   // the side-stream reduction reads only its scratch half
 }
 
 // ------------------------------------------------------------------------------------
@@ -865,7 +858,7 @@ static int node_model_backward(const Run& r, const BwdBufs& bb, const float* out
     {   // weight gradients of the two GRU projections: one grouped launch
       const GemmDW qs[2] = {lin_dw(r, bb, ih, sc + bb.dgi, r.ws + L.msum[t], Mp, (int)S),
                             lin_dw(r, bb, hh, sc + bb.dgh, h, Hp, (int)S)};
-      GIB_TRY(gemm_dw_group(qs, 2, 0, r.st));
+      GIB_TRY(gemm_dw_group(qs, 2, r.st));
     }
     {   // dMsum = dgi W_ih  and  dh[t] = dgh W_hh + direct  (dh[t+1] is dead after gru_bwd): one grouped launch
       GemmNT ps[2] = {lin_dx(r, ih, sc + bb.dgi, (int)S, sc + bb.dmsum, Mp), lin_dx(r, hh, sc + bb.dgh, (int)S, dh, Hp)};
@@ -900,7 +893,7 @@ static int node_model_backward(const Run& r, const BwdBufs& bb, const float* out
         jobs[g] = MlpBwdJob{&pl.msg[g], r.ws + L.x0[t], &L.msg[t], rr.row0, rr.rows, T1 + ro * Mp,
                             t == 0 ? nullptr : dx0 + ro * Hp, Hp, nullptr, rr.m_dev, rr.base_dev};
       }
-      GIB_TRY(mlp_backward_multi(r, bb, jobs, r.ngroups, msg_dev(r) ? r.P : 0));
+      GIB_TRY(mlp_backward_multi(r, bb, jobs, r.ngroups));
       if (d.model == GIB_ATTGGNN) {
         for (int g = 0; g < r.ngroups; ++g) {
           const size_t ro = (size_t)r.tb[g];
@@ -908,7 +901,7 @@ static int node_model_backward(const Run& r, const BwdBufs& bb, const float* out
                               t == 0 ? nullptr : dx0 + ro * Hp, Hp, dx0 + ro * Hp, type_count_dev(r, g),
                               type_base_dev(r, g)};
         }
-        GIB_TRY(mlp_backward_multi(r, bb, jobs, r.ngroups, r.cap ? r.P : 0));
+        GIB_TRY(mlp_backward_multi(r, bb, jobs, r.ngroups));
       }
     }
     // dh[t][src] += (w) dX0   -- deterministic gather-reduce over the by-source CSR (of message rows or of entries; the
@@ -975,9 +968,9 @@ static int emn_forward(const Run& r, float* out) {
 // att_depth) run one after the other, each still on the device row range.
 static int emn_siblings_backward(const Run& r, const BwdBufs& bb, const MlpBwdJob* j) {
   if (!r.cap) return mlp_backward_multi(r, bb, j, 2);
-  if (j[0].m->n == j[1].m->n) return mlp_backward_multi(r, bb, j, 2, 2LL * r.E, /*same_rows=*/true);
-  GIB_TRY(mlp_backward_multi(r, bb, j, 1, r.E));
-  return mlp_backward_multi(r, bb, j + 1, 1, r.E);
+  if (j[0].m->n == j[1].m->n) return mlp_backward_multi(r, bb, j, 2, /*same_rows=*/true);
+  GIB_TRY(mlp_backward_multi(r, bb, j, 1));
+  return mlp_backward_multi(r, bb, j + 1, 1);
 }
 
 static int emn_backward(const Run& r, const BwdBufs& bb, const float* out, const float* dout, int part) {
@@ -1029,7 +1022,7 @@ static int emn_backward(const Run& r, const BwdBufs& bb, const float* out, const
   GIB_TRY(tanh_selu_bwd(T1, dmem, r.ws + L.xt, r.ws + L.embnn.y[pl.embnn.n], E, Hp, live, r.st));
   {
     MlpBwdJob j[1] = {{&pl.embnn, r.ws + L.xin, &L.embnn, 0, E, T1, nullptr, 0, nullptr, live, base}};
-    GIB_TRY(mlp_backward_multi(r, bb, j, 1, r.cap ? r.E : 0));
+    GIB_TRY(mlp_backward_multi(r, bb, j, 1));
   }
   return 0;
 }
@@ -1047,8 +1040,7 @@ static void mlp_extent(const Plan& pl, const Mlp& m, size_t rows, size_t& big, s
 }
 // the same for sibling MLPs of equal depth whose weight gradients run as one grouped launch per layer; split: siblings
 // that do not fit one launch run in the sub-groups of mlp_backward_multi (capacity mode), else one by one (mlp_extent)
-static void group_extent(const Plan& pl, const Mlp* const* ms, const size_t* rows, int n, long long plan_rows, size_t& dw,
-                         bool split = false) {
+static void group_extent(const Plan& pl, const Mlp* const* ms, const size_t* rows, int n, size_t& dw, bool split = false) {
   bool same = true;
   for (int i = 1; i < n; ++i) same = same && ms[i]->n == ms[0]->n;
   const int depth = ms[0]->n;
@@ -1056,7 +1048,7 @@ static void group_extent(const Plan& pl, const Mlp* const* ms, const size_t* row
     if (split)
       for (int i = 0, k; i < n; i += k) {
         k = sub_group(ms, n, i);
-        group_extent(pl, ms + i, rows + i, k, plan_rows, dw);
+        group_extent(pl, ms + i, rows + i, k, dw);
       }
     return;
   }
@@ -1069,7 +1061,7 @@ static void group_extent(const Plan& pl, const Mlp* const* ms, const size_t* row
       qs[nq].M = (int)rows[i]; qs[nq].Nn = L.Rp; qs[nq].Kk = L.Cp;
       ++nq;
     }
-  if (nq) dw = std::max(dw, 2 * gemm_dw_group_half_floats(qs, nq, plan_rows * depth));
+  if (nq) dw = std::max(dw, 2 * gemm_dw_group_half_floats(qs, nq));
 }
 
 void make_bwd(const Run& r, BwdBufs& bb) {
@@ -1093,24 +1085,23 @@ void make_bwd(const Run& r, BwdBufs& bb) {
     {
       const Mlp* ms[4];
       for (int g = 0; g < r.ngroups; ++g) ms[g] = &pl.msg[g];
-      group_extent(pl, ms, mrows, r.ngroups, dev ? r.P : 0, dw, dev);
+      group_extent(pl, ms, mrows, r.ngroups, dw, dev);
       if (d.model == GIB_ATTGGNN) {
         for (int g = 0; g < r.ngroups; ++g) ms[g] = &pl.att[g];
-        group_extent(pl, ms, mrows, r.ngroups, dev ? r.P : 0, dw, dev);
+        group_extent(pl, ms, mrows, r.ngroups, dw, dev);
       }
     }
   } else {
     mlp_extent(pl, pl.embnn, E, big, dw);
     mlp_extent(pl, pl.emsg, E, big, dw);
     mlp_extent(pl, pl.eatt, E, big, dw);
-    // the same plan rows as emn_backward / emn_siblings_backward (the split of a grouped weight gradient depends on them)
     const Mlp* one[1] = {&pl.embnn}; const size_t re[2] = {E, E};
-    group_extent(pl, one, re, 1, r.cap ? (long long)E : 0, dw);
+    group_extent(pl, one, re, 1, dw);
     const Mlp* two[2] = {&pl.emsg, &pl.eatt};
-    group_extent(pl, two, re, 2, r.cap ? 2LL * (long long)E : 0, dw);
+    group_extent(pl, two, re, 2, dw);
     if (r.cap && pl.emsg.n != pl.eatt.n) {
-      group_extent(pl, two, re, 1, (long long)E, dw);
-      group_extent(pl, two + 1, re, 1, (long long)E, dw);
+      group_extent(pl, two, re, 1, dw);
+      group_extent(pl, two + 1, re, 1, dw);
     }
     big = std::max(big, E * (mlp_max_ld(pl, pl.emsg) + mlp_max_ld(pl, pl.eatt)) + 64);
   }
@@ -1125,18 +1116,18 @@ void make_bwd(const Run& r, BwdBufs& bb) {
   mlp_extent(pl, pl.fterm2, B, big, dw);
   {
     const Mlp* t2[3] = {&pl.fadd2, &pl.fconn2, &pl.fterm2}; const size_t r2[3] = {B, B, B};
-    group_extent(pl, t2, r2, 3, 0, dw);
+    group_extent(pl, t2, r2, 3, dw);
     const Mlp* t1[2] = {&pl.fadd1, &pl.fconn1}; const size_t r1[2] = {S, S};
-    group_extent(pl, t1, r1, 2, 0, dw);
+    group_extent(pl, t1, r1, 2, dw);
     if (d.model != GIB_MNN) {
       const Mlp* ga[2] = {&pl.gemb, &pl.gatt};
-      group_extent(pl, ga, r1, 2, 0, dw);
+      group_extent(pl, ga, r1, 2, dw);
     }
     GemmDW qs[2];
     qs[0].M = qs[1].M = (int)gru_rows;
     qs[0].Nn = pl.lins[pl.gru_ih].Rp; qs[0].Kk = pl.lins[pl.gru_ih].Cp;
     qs[1].Nn = pl.lins[pl.gru_hh].Rp; qs[1].Kk = pl.lins[pl.gru_hh].Cp;
-    dw = std::max(dw, 2 * gemm_dw_group_half_floats(qs, 2, 0));
+    dw = std::max(dw, 2 * gemm_dw_group_half_floats(qs, 2));
   }
   // grouped backward passes keep one ping/pong slice per member inside GA / GB
   {

@@ -346,11 +346,18 @@ typedef struct gib_dw_problem {
 } gib_dw_problem;
 /* n_groups consecutive groups of group_sizes[g] (<= 16) problems, each run as the model runs the weight gradients of one
  * layer (one grouped tensor-core launch + one side-stream reduction when it qualifies), all on ONE scratch whose two
- * halves alternate between groups; plan_rows: the expected reduction rows of a group (0: the sum of its M).  The
- * members of one group write disjoint destinations; different groups may add into the same ones. */
+ * halves alternate between groups.  plan_rows is ignored: the split of a launch depends on its live row counts only.
+ * The members of one group write disjoint destinations; different groups may add into the same ones. */
 size_t gib_test_dw_scratch_bytes(const gib_dw_problem* qs, const int* group_sizes, int n_groups, long long plan_rows);
 int gib_test_dw_groups(const gib_dw_problem* qs, const int* group_sizes, int n_groups, long long plan_rows,
                        void* scratch, gib_stream stream);
+/* The schedule of one grouped tensor-core weight-gradient launch of n (<= 16) members with host row counts rows[p] and
+ * padded shapes Nn[p] x Kk[p] on sms SMs (host arithmetic, no device): writes G (the CTAs with work), per segment 6
+ * ints (CTA, member, tile of the member, first reduction row, rows, scratch slot) into segs, and per tile of the group
+ * (member-major) the first and last CTA whose slots the reduction sums into tile_ctas [tiles][2] (-1, -1: no rows).
+ * Returns the segment count, or < 0 (more than max_segs segments, bad arguments). */
+int gib_test_dw_schedule(const int* rows, const int* Nn, const int* Kk, int n, int sms, int* segs, int max_segs,
+                         int* tile_ctas, int* G);
 /* G[p] = w[p] * dM[dst[p]] * act'(Y[p]) (rows with dst[p] < 0: zeros) */
 int gib_test_scatter_bwd(float* G, const float* dM, const float* Y, int ld, const int* dst, const float* w, int act,
                          long long P, gib_stream stream);
