@@ -860,6 +860,228 @@ int route_limits(const char* who, const gib_pp_dims* d, int max_molecules, PP* p
   return 0;
 }
 
+// ---- node_remap (MolecularGraph.py:435-461, 328-433, 592-614): one warp per molecule -------------------------------
+// The BFS / DFS of the reference from atom ranking[0], then reorder_nodes.  Adjacency bitsets and the ranking live in
+// shared memory; the search runs on lane 0 and the reordered bytes are written by the whole warp.
+constexpr int kReorderMaxN = 181;                           // N*N*Ef <= 32768
+constexpr int kReorderWords = (kReorderMaxN + 31) / 32;
+constexpr int kSetMaxSlots = 512;                           // the table of a set of <= 306 small ints (CPython 3.12)
+constexpr int kSetLinearProbes = 9, kSetPerturbShift = 5;   // Objects/setobject.c
+
+// CPython 3.12's set table for small non-negative ints (hash = value, no deletions): set_add_entry's probe sequence
+// (LINEAR_PROBES slots after the home slot while they fit, then perturbation), set_table_resize on the fill rule
+// (fill * 5 >= mask * 3 -> the smallest power of two above used * 4) re-inserting in old-table order.  Iterating the
+// table in slot order is list(set(...)).
+struct PySet {
+  short* slot;   // [kSetMaxSlots], -1 = empty
+  short* tmp;    // [kReorderMaxN]
+  int mask, used;
+
+  __device__ void clear() {
+    mask = 7;
+    used = 0;
+    for (int i = 0; i <= mask; ++i) slot[i] = -1;
+  }
+  // set_insert_clean / the probe of set_add_entry; returns the slot holding `key` or the empty slot for it
+  __device__ int find(int key) const {
+    size_t perturb = (size_t)key, i = (size_t)key & mask;
+    while (true) {
+      const int probes = i + kSetLinearProbes <= (size_t)mask ? kSetLinearProbes : 0;
+      for (int j = 0; j <= probes; ++j)
+        if (slot[i + j] < 0 || slot[i + j] == key) return (int)(i + j);
+      perturb >>= kSetPerturbShift;
+      i = (i * 5 + 1 + perturb) & mask;
+    }
+  }
+  __device__ void add(int key) {
+    const int s = find(key);
+    if (slot[s] == key) return;
+    slot[s] = (short)key;
+    ++used;                                                 // fill == used: nothing is ever deleted
+    if ((size_t)used * 5 < (size_t)mask * 3) return;
+    int n = 0;
+    for (int i = 0; i <= mask; ++i)
+      if (slot[i] >= 0) tmp[n++] = slot[i];
+    int size = 8;
+    while (size <= used * 4) size <<= 1;
+    mask = size - 1;
+    for (int i = 0; i <= mask; ++i) slot[i] = -1;
+    for (int k = 0; k < n; ++k) slot[find(tmp[k])] = tmp[k];
+  }
+};
+
+// the highest-ranked atom of bitset `cand` (-1: empty)
+__device__ __forceinline__ int best_of(const unsigned* cand, const int* rank, int W) {
+  int best = -1, br = -1;
+  for (int w = 0; w < W; ++w)
+    for (unsigned b = cand[w]; b; b &= b - 1) {
+      const int a = w * 32 + __ffs(b) - 1;
+      if (rank[a] > br) br = rank[a], best = a;
+    }
+  return best;
+}
+
+// a uniformly random permutation of 0..n-1 per molecule, a function of (seed, epoch, molecule) only: atom i's rank is
+// its place among the counter-based keys mix64(seed, epoch, molecule, i), ties broken by atom index
+__device__ void draw_ranking(unsigned long long seed, long long epoch, long long molecule, int n, int* rank,
+                             unsigned long long* key) {
+  const int lane = threadIdx.x & 31;
+  const unsigned long long h = mix64(mix64(mix64(seed) ^ (unsigned long long)epoch) ^ (unsigned long long)molecule);
+  for (int i = lane; i < n; i += 32) key[i] = mix64(h ^ (unsigned long long)i);
+  __syncwarp();
+  for (int i = lane; i < n; i += 32) {
+    const unsigned long long k = key[i];
+    int r = 0;
+    for (int j = 0; j < n; ++j) r += key[j] < k || (key[j] == k && j < i);
+    rank[i] = r;
+  }
+  __syncwarp();
+}
+
+__global__ void __launch_bounds__(32) rank_draw_kernel(int N, const int* __restrict__ n_atoms, unsigned long long seed,
+                                                       long long epoch, long long first, int* rankings) {
+  __shared__ int rank[kReorderMaxN];
+  __shared__ unsigned long long key[kReorderMaxN];
+  const int m = blockIdx.x, lane = threadIdx.x;
+  const int n = min(max(n_atoms[m], 0), N);
+  draw_ranking(seed, epoch, first + m, n, rank, key);
+  for (int i = lane; i < N; i += 32) rankings[(size_t)m * N + i] = i < n ? rank[i] : -1;
+}
+
+// route: 0 = BFS, 1 = DFS.  draw != 0: the ranking is drawn (draw_ranking) and written to `rankings`, else read from it
+__global__ void __launch_bounds__(32) reorder_kernel(PP p, const signed char* __restrict__ nodes,
+                                                     const signed char* __restrict__ edges, const int* __restrict__ n0,
+                                                     int route, int draw, unsigned long long seed, long long epoch,
+                                                     long long first, int* rankings, int* order,
+                                                     signed char* out_nodes, signed char* out_edges, int* status) {
+  __shared__ unsigned adj[kReorderMaxN][kReorderWords];
+  __shared__ unsigned seen[kReorderWords];
+  __shared__ int rank[kReorderMaxN], ord[kReorderMaxN], pos[kReorderMaxN];
+  __shared__ unsigned long long key[kReorderMaxN];
+  __shared__ short table[kSetMaxSlots], tmp[kReorderMaxN];
+  __shared__ int ok;
+  const int m = blockIdx.x, lane = threadIdx.x;
+  const int N = p.N, F = p.F, Ef = p.Ef, W = (N + 31) / 32;
+  const int n = n0[m];
+  const signed char* X = nodes + (size_t)m * N * F;
+  const signed char* E = edges + (size_t)m * N * N * Ef;
+  int* R = rankings + (size_t)m * N;
+  for (int q = lane; q < N * W; q += 32) adj[q / W][q % W] = 0;
+  if (lane < W) seen[lane] = 0;
+  if (lane == 0) ok = n > 0;
+  __syncwarp();
+  for (int q = lane; q < n * n; q += 32) {
+    const int i = q / n, j = q % n;
+    bool any = false;
+    for (int t = 0; t < Ef; ++t) any |= E[((size_t)i * N + j) * Ef + t] != 0;
+    if (any) atomicOr(&adj[i][j >> 5], 1u << (j & 31));
+  }
+  // the ranking: a permutation of 0..n-1 over the molecule's atoms
+  if (draw) {
+    draw_ranking(seed, epoch, first + m, n, rank, key);
+    for (int i = lane; i < N; i += 32) R[i] = i < n ? rank[i] : -1;
+  } else {
+    for (int i = lane; i < n; i += 32) rank[i] = R[i];
+  }
+  __syncwarp();
+  bool bad_rank = false;
+  for (int i = lane; i < n; i += 32) {
+    const int r = rank[i];
+    if (r < 0 || r >= n || (atomicOr(&seen[r >> 5], 1u << (r & 31)) >> (r & 31) & 1u)) bad_rank = true;
+  }
+  if (__any_sync(0xffffffffu, bad_rank)) {
+    if (lane == 0) {
+      flag_bad(status, GIB_PP_BAD_RANKING, m);
+      ok = 0;
+    }
+  }
+  __syncwarp();
+  if (lane == 0 && ok) {
+    unsigned* vis = seen;                                   // reused: the visited set
+    for (int w = 0; w < W; ++w) vis[w] = 0;
+    const int start = rank[0];                              // node_init = atom_ranking[0]
+    // connectivity first: both reference searches loop forever on a disconnected graph
+    int count = 1;
+    ord[0] = start;
+    vis[start >> 5] |= 1u << (start & 31);
+    for (int k = 0; k < count; ++k)
+      for (int w = 0; w < W; ++w)
+        for (unsigned b = adj[ord[k]][w] & ~vis[w]; b; b &= b - 1) {
+          const int a = w * 32 + __ffs(b) - 1;
+          vis[w] |= 1u << (a & 31);
+          ord[count++] = a;
+        }
+    if (count != n) {
+      flag_bad(status, GIB_PP_DISCONNECTED, m);
+      ok = 0;
+    } else {
+      for (int w = 0; w < W; ++w) vis[w] = 0;
+      vis[start >> 5] |= 1u << (start & 31);
+      ord[0] = start;
+      pos[start] = 0;
+      count = 1;
+      unsigned cand[kReorderWords];
+      if (route == 0) {
+        // breadth_first_search: per layer, each last-layer atom's unvisited neighbours by falling rank into one set;
+        // the set's iteration order is the layer's order (nodes_visited.extend(set(...)), last_nodes_visited = set(...))
+        PySet set{table, tmp, 0, 0};
+        int lo = 0, hi = 1;
+        while (count < n) {
+          set.clear();
+          for (int k = lo; k < hi; ++k) {
+            for (int w = 0; w < W; ++w) cand[w] = adj[ord[k]][w] & ~vis[w];
+            for (int a = best_of(cand, rank, W); a >= 0; a = best_of(cand, rank, W)) {
+              set.add(a);
+              cand[a >> 5] &= ~(1u << (a & 31));
+            }
+          }
+          lo = hi;
+          for (int i = 0; i <= set.mask; ++i)
+            if (table[i] >= 0) {
+              const int a = table[i];
+              vis[a >> 5] |= 1u << (a & 31);
+              ord[count++] = a;
+            }
+          hi = count;
+        }
+      } else {
+        // depth_first_search: the highest-ranked unvisited neighbour of the last atom; none -> back to the atom
+        // before it in visit order (nodes_visited[idx - 1], index -1 = the last one)
+        int last = start;
+        while (count < n) {
+          for (int w = 0; w < W; ++w) cand[w] = adj[last][w] & ~vis[w];
+          const int a = best_of(cand, rank, W);
+          if (a < 0) {
+            const int idx = pos[last];
+            last = ord[idx ? idx - 1 : count - 1];
+            continue;
+          }
+          vis[a >> 5] |= 1u << (a & 31);
+          pos[a] = count;
+          ord[count++] = a;
+          last = a;
+        }
+      }
+    }
+  }
+  __syncwarp();
+  const bool good = ok;
+  int* O = order + (size_t)m * N;
+  for (int i = lane; i < N; i += 32) O[i] = good && i < n ? ord[i] : -1;
+  // reorder_nodes; a refused molecule's outputs are zero
+  signed char* OX = out_nodes + (size_t)m * N * F;
+  signed char* OE = out_edges + (size_t)m * N * N * Ef;
+  const int nk = good ? n : 0;
+  for (int q = lane; q < N * F; q += 32) {
+    const int k = q / F;
+    OX[q] = k < nk ? X[(size_t)ord[k] * F + q % F] : 0;
+  }
+  for (int q = lane; q < N * N * Ef; q += 32) {
+    const int k = q / (N * Ef), l = q / Ef % N, t = q % Ef;
+    OE[q] = k < nk && l < nk ? E[((size_t)ord[k] * N + ord[l]) * Ef + t] : 0;
+  }
+}
+
 }  // namespace
 }  // namespace gib
 
@@ -1095,6 +1317,47 @@ int gib_route_grad_coef(int n_molecules, const int* offsets, const float* likeli
   }
   route_grad_coef_kernel<<<ceil_div(n_molecules, kCoefWarps), 32 * kCoefWarps, 0, (cudaStream_t)stream>>>(
       n_molecules, offsets, likelihoods, g_lik, g_nll, g_final, coef);
+  GIB_LAUNCH_CHECK();
+  return 0;
+}
+
+size_t gib_reorder_ws_bytes(int n_molecules) { return n_molecules < 1 ? 0 : 2 * align256(4ull * n_molecules); }
+
+int gib_draw_rankings(int n_molecules, int N, const int* n_atoms, unsigned long long seed, long long epoch,
+                      long long first_molecule, int* rankings, gib_stream stream) {
+  if (n_molecules < 1 || N < 1 || N > kReorderMaxN || first_molecule < 0 || !n_atoms || !rankings) {
+    set_error("gib_draw_rankings: need n_molecules >= 1, 1 <= N <= %d, first_molecule >= 0 and non-null buffers "
+              "(got %d, %d, %lld)", kReorderMaxN, n_molecules, N, first_molecule);
+    return -1;
+  }
+  rank_draw_kernel<<<n_molecules, 32, 0, (cudaStream_t)stream>>>(N, n_atoms, seed, epoch, first_molecule, rankings);
+  GIB_LAUNCH_CHECK();
+  return 0;
+}
+
+int gib_reorder(const gib_pp_dims* d, const signed char* nodes, const signed char* edges, int n_molecules, int route,
+                int draw, unsigned long long seed, long long epoch, long long first_molecule, int* rankings,
+                int* order, signed char* out_nodes, signed char* out_edges, void* ws, int* status, gib_stream stream) {
+  PP p;
+  GIB_TRY(make_pp("gib_reorder", d, &p));
+  if (n_molecules < 1 || (route != GIB_ROUTE_BFS && route != GIB_ROUTE_DFS) || first_molecule < 0) {
+    set_error("gib_reorder: need n_molecules >= 1, route GIB_ROUTE_BFS or GIB_ROUTE_DFS and first_molecule >= 0 "
+              "(got %d, %d, %lld)", n_molecules, route, first_molecule);
+    return -1;
+  }
+  if (!nodes || !edges || !rankings || !order || !out_nodes || !out_edges || !ws || !status) {
+    set_error("gib_reorder: null argument");
+    return -1;
+  }
+  cudaStream_t s = (cudaStream_t)stream;
+  int* len = static_cast<int*>(ws);
+  int* n0 = (int*)(static_cast<char*>(ws) + align256(4ull * n_molecules));
+  pp_init_kernel<<<1, 32, 0, s>>>(status, nullptr, nullptr, 0, 0);
+  GIB_LAUNCH_CHECK();
+  pp_count_kernel<<<n_molecules, 32, 0, s>>>(p, nodes, edges, len, n0, status, nullptr, gib_scaffolds{});
+  GIB_LAUNCH_CHECK();
+  reorder_kernel<<<n_molecules, 32, 0, s>>>(p, nodes, edges, n0, route, draw, seed, epoch, first_molecule, rankings,
+                                            order, out_nodes, out_edges, status);
   GIB_LAUNCH_CHECK();
   return 0;
 }

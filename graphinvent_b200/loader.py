@@ -23,6 +23,8 @@ Deviation: when the last block holds one row, the reference's `torch.squeeze` dr
 its ShuffleBlockWrapper then indexes atoms as molecules; here that block is a batch of one molecule (INTEGRATION.md
 section 2).  Its draws are the reference's.
 """
+import ctypes
+import types
 from concurrent.futures import ThreadPoolExecutor
 
 import numpy as np
@@ -31,7 +33,7 @@ import torch
 from . import functional as F
 from ._lib import check, lib
 
-__all__ = ["DeviceBlockLoader"]
+__all__ = ["DeviceBlockLoader", "RandomRouteLoader"]
 
 
 class _Batch:
@@ -47,7 +49,8 @@ class DeviceBlockLoader:
                  device=None):
         """the reference's BlockDataLoader arguments; n_workers and pin_memory are accepted and have no effect.
         `dataset`: the reference's HDFDataset or any object with int8 `nodes` [n, N, F], `edges` [n, N, N, Ef] and
-        `apds` [n, apd] array-likes that can be sliced by rows (h5py datasets, numpy arrays)."""
+        `apds` [n, apd] array-likes that can be sliced by rows (h5py datasets, numpy arrays), or three contiguous int8
+        tensors on the loader's device, whose rows are gathered in place."""
         self.batch_size, self.block_size = int(batch_size), int(block_size)
         self.shuffle, self.n_workers, self.pin_memory = bool(shuffle), n_workers, pin_memory
         if self.batch_size < 1:
@@ -55,6 +58,15 @@ class DeviceBlockLoader:
         if self.block_size < self.batch_size:
             raise ValueError(f"block_size ({self.block_size}) must be >= batch_size ({self.batch_size}), as the "
                              "reference's BlockDataset asserts")
+        self.device = torch.device(device if device is not None else "cuda")
+        if self.device.index is None and torch.cuda.is_available():
+            self.device = torch.device("cuda", torch.cuda.current_device())
+        self._bind(dataset)
+
+    def _bind(self, dataset):
+        """takes `dataset`'s rows: checks them and sets up the pass state.  Rows held as int8 device tensors on the
+        loader's device are gathered in place (both slots are the whole set, a batch's rows are indices into it): no
+        staging or uploads."""
         self.dataset = dataset
         arrays = (dataset.nodes, dataset.edges, dataset.apds)
         shapes = [tuple(a.shape) for a in arrays]
@@ -65,8 +77,14 @@ class DeviceBlockLoader:
         if shapes[1][1] != shapes[0][1] or shapes[1][2] != shapes[0][1]:
             raise ValueError(f"edges {shapes[1]} do not match nodes {shapes[0]}: need [n, N, N, Ef] with N = "
                              f"{shapes[0][1]}")
+        self._on_device = all(isinstance(a, torch.Tensor) and a.is_cuda for a in arrays)
         for name, a in zip(("nodes", "edges", "apds"), arrays):
-            if np.dtype(a.dtype) != np.int8:
+            if isinstance(a, torch.Tensor):
+                if a.dtype != torch.int8 or not a.is_contiguous() or (a.is_cuda and (not self._on_device
+                                                                                     or a.device != self.device)):
+                    raise ValueError(f"{name}: a tensor must be contiguous int8 on {self.device} (device rows) or a "
+                                     f"host array, got {a.dtype} on {a.device}")
+            elif np.dtype(a.dtype) != np.int8:
                 raise ValueError(f"{name} must be int8 (the reference's preprocessed HDF5 layout), got {a.dtype}")
         self.n_rows = shapes[0][0]
         if self.n_rows < 1:
@@ -74,9 +92,6 @@ class DeviceBlockLoader:
         _, self.N, self.F = shapes[0]
         self.Ef, self.apd = shapes[1][3], shapes[2][1]
         self.row_bytes = (self.N * self.F, self.N * self.N * self.Ef, self.apd)
-        self.device = torch.device(device if device is not None else "cuda")
-        if self.device.index is None and torch.cuda.is_available():
-            self.device = torch.device("cuda", torch.cuda.current_device())
         self.n_blocks = -(-self.n_rows // self.block_size)
         # the reference's drop_last expression, evaluated as Python does (with its precedence it is False unless there
         # are about block_size blocks or more)
@@ -97,7 +112,10 @@ class DeviceBlockLoader:
     # ---- the reference's BlockDataLoader protocol --------------------------------------------------------------
     def __len__(self):
         """the reference's BlockDataLoader.__len__"""
-        n_blocks, n_rem = divmod(self.n_rows, self.block_size)
+        return self._count(self.n_rows)
+
+    def _count(self, n_rows):
+        n_blocks, n_rem = divmod(n_rows, self.block_size)
         return -(-self.block_size // self.batch_size) * n_blocks + -(-n_rem // self.batch_size)
 
     def __iter__(self):
@@ -171,6 +189,13 @@ class DeviceBlockLoader:
                 return slot
         slot = 1 - avoid if avoid is not None else (0 if self._resident[0] is None else 1)
         self._wait(slot)
+        if self._on_device:        # device rows: the slot is the whole set (16-byte aligned), its rows offset by block
+            self._slots[slot] = (self.dataset.nodes, self.dataset.edges, self.dataset.apds)
+            self._resident[slot] = k
+            if self._ready[slot] is None:
+                self._ready[slot], self._free[slot] = torch.cuda.Event(), torch.cuda.Event()
+                self._ready[slot].record(torch.cuda.current_stream(self.device))
+            return slot
         self._allocate(slot)
         self._resident[slot] = k
         self._pending[slot] = self._reader.submit(self._read, k, slot)
@@ -203,7 +228,10 @@ class DeviceBlockLoader:
                 continue
             self._wait(slot)
             cur.wait_event(self._ready[slot])
-            rows = torch.cat(order).to(torch.int32).pin_memory().to(self.device, non_blocking=True)
+            rows = torch.cat(order)
+            if self._on_device:
+                rows += self._block_range(k)[0]
+            rows = rows.to(torch.int32).pin_memory().to(self.device, non_blocking=True)
             off = 0
             for idx in order:
                 b = idx.numel()
@@ -232,3 +260,93 @@ class DeviceBlockLoader:
                                   F._ptr(target), F._ptr(ctl),
                                   F._stream(self.device)), "gib_gather_rows")
         self._free[item.slot].record(torch.cuda.current_stream(self.device))
+
+
+class RandomRouteLoader(DeviceBlockLoader):
+    """Training passes over fresh random decoding routes: pass e is exactly `DeviceBlockLoader(ds_e, batch_size,
+    block_size, shuffle)`, where ds_e is the int8 file the reference's preprocessing writes for the molecules reordered
+    by `preprocess.reorder(nodes, edges, route, seed=seed, epoch=e)` -- the same batches and the same draws from
+    torch's default generator.  The reordering and the construction run on the device; the ranking draws depend on
+    (seed, e, molecule) only and take nothing from torch's generators.
+
+        loader = RandomRouteLoader(nodes, edges, batch_size=B, block_size=K, route="bfs", seed=0, constants=C)
+        scheduler = OneCycleLR(optimizer, ..., total_steps=loader.total_batches(start_epoch, n_epochs))
+        loader.set_epoch(start_epoch)                 # a restarted job
+        loss = step.train_epoch(loader, scheduler)    # graphed.TrainStep; one call per pass
+
+    `epoch` is the epoch of the upcoming pass: it starts at 0 (or `set_epoch`) and advances by one when a pass starts,
+    so `len(loader)` before a pass counts that pass's batches.  A pass's rows are built when the pass or its `len` is
+    first needed and stay on the device until the next pass's are built: about
+    `preprocess.file_rows`' sum over molecules of (bonds + 2) rows at N*F + N*N*Ef + apd bytes each (6.5 KB at N = 38
+    with gdb13's layout).  A set whose rows do not fit raises torch's out-of-memory error.  The molecule stacks stay on
+    the device too.  Building the next pass's rows (its `len`) while a pass is being consumed ends that pass."""
+
+    def __init__(self, nodes, edges, batch_size=100, block_size=10000, route="bfs", seed=0, n_atom_types=None,
+                 n_formal_charge=None, n_imp_H=0, n_chirality=0, constants=None, shuffle=True, chunk_molecules=4096,
+                 device=None):
+        """`nodes` [M, N, F] / `edges` [M, N, N, Ef]: int8 padded molecules (numpy or torch), in any atom order.  The
+        layout: `constants` (the reference's, through `preprocess.layout_of`) or the segment widths."""
+        from . import preprocess
+        if route not in ("bfs", "dfs"):
+            raise ValueError(f"route must be 'bfs' or 'dfs', got {route!r}")
+        if constants is not None:
+            self.layout = preprocess.layout_of(constants)
+        elif n_atom_types is None or n_formal_charge is None:
+            raise ValueError("give constants= or n_atom_types and n_formal_charge")
+        else:
+            self.layout = (int(n_atom_types), int(n_formal_charge), int(n_imp_H), int(n_chirality))
+        self.route, self.seed, self.chunk_molecules = route, int(seed), int(chunk_molecules)
+        self.batch_size, self.block_size, self.shuffle = int(batch_size), int(block_size), bool(shuffle)
+        if self.batch_size < 1 or self.block_size < self.batch_size:
+            raise ValueError(f"need 1 <= batch_size <= block_size, got {batch_size} and {block_size}")
+        self.n_workers, self.pin_memory = 0, False
+        self.device = torch.device(device if device is not None else "cuda")
+        if self.device.index is None and torch.cuda.is_available():
+            self.device = torch.device("cuda", torch.cuda.current_device())
+        self.M, self.N, self.F, self.Ef = preprocess._check_stacks(nodes, edges)
+        if self.M < 1:
+            raise ValueError("no molecules")
+        self.nodes = preprocess._on_device(nodes, self.device)
+        self.edges = preprocess._on_device(edges, self.device)
+        d = preprocess._pp_dims(self.N, self.F, self.Ef, self.layout, self.batch_size)
+        self.apd = preprocess.lib.gib_preprocess_apd_length(ctypes.byref(d))
+        self.row_bytes = (self.N * self.F, self.N * self.N * self.Ef, self.apd)
+        self.epoch = 0
+        self._built = None                  # the epoch whose rows are bound
+
+    def set_epoch(self, epoch):
+        """the next pass (and `len`) is epoch `epoch`: resumes a job or repeats a pass"""
+        self.epoch = int(epoch)
+
+    def _rows(self, epoch, keep):
+        from . import preprocess
+        nodes, edges, _ = preprocess.reorder(self.nodes, self.edges, self.route, seed=self.seed, epoch=epoch,
+                                             layout=self.layout, device=self.device)
+        return preprocess.file_rows(nodes, edges, self.batch_size, *self.layout, chunk_molecules=self.chunk_molecules,
+                                    keep=keep, device=self.device)
+
+    def _build(self):
+        if self._built == self.epoch:
+            return
+        self._built = None
+        self.dataset = self._slots = None                     # the last pass's rows go before the next pass's come
+        rows, _ = self._rows(self.epoch, keep=True)
+        self._bind(types.SimpleNamespace(nodes=rows[0], edges=rows[1], apds=rows[2]))
+        self._built = self.epoch
+
+    def __len__(self):
+        """batches of the upcoming pass (epoch `epoch`), building its rows"""
+        self._build()
+        return super().__len__()
+
+    def total_batches(self, first_epoch, n_epochs):
+        """sum of len() over passes first_epoch .. first_epoch + n_epochs - 1, counted without keeping their rows:
+        the total_steps of a OneCycleLR over those passes"""
+        return sum(self._count(self.n_rows if e == self._built else self._rows(e, keep=False)[1])
+                   for e in range(int(first_epoch), int(first_epoch) + int(n_epochs)))
+
+    def batches(self):
+        """the pass of epoch `epoch` (DeviceBlockLoader.batches over its rows); the epoch advances as it starts"""
+        self._build()
+        self.epoch += 1
+        yield from super().batches()

@@ -13,6 +13,11 @@ int8 conversion and the final resize / resave stay the reference's own methods. 
 reference's `get_ts_properties` per group, or, with `device_properties=True`, each group's integer statistics from
 `gib_preprocess_group_statistics` (`groups(..., statistics=True)`) turned into the dict `get_molecular_properties`
 returns and merged by the reference's own `combine_ts_properties`.
+
+`reorder()` is the reference's choice of decoding route, `PreprocessingGraph.node_remap`, on the device
+(`gib_reorder`): a BFS or DFS from a node ranking -- given, or drawn per (seed, epoch, molecule) -- and the reordered
+stacks.  `file_rows()` runs the construction of `groups()` with the rows left on the device, laid out as the file
+`run_data_processer` writes; `loader.RandomRouteLoader` builds every training pass from fresh routes with the two.
 """
 import ctypes
 import sys
@@ -21,7 +26,8 @@ from collections import namedtuple
 import numpy as np
 import torch
 
-from ._lib import (PP_BAD_EDGES, PP_BAD_NODES, PP_DISCONNECTED, PP_EMPTY, PP_STATUS_INTS, PPDims, check, lib)
+from ._lib import (PP_BAD_EDGES, PP_BAD_NODES, PP_BAD_RANKING, PP_DISCONNECTED, PP_EMPTY, PP_STATUS_INTS, ROUTE_BFS,
+                   ROUTE_DFS, PPDims, check, lib)
 
 Group = namedtuple("Group", "index init_idx start stop full nodes edges apds resume_idx dataset_size statistics",
                    defaults=(None,))
@@ -45,11 +51,11 @@ _REASONS = ((PP_BAD_NODES, "a node row that is not one-hot per segment with 0/1 
             (PP_DISCONNECTED, "a decoding route that disconnects (the reference's truncate_graph raises)"))
 
 
-def refuse_bad(status, start, stop):
+def refuse_bad(status, start, stop, reasons=_REASONS):
     """raises the ValueError naming the first bad molecule of the chunk [start, stop) whose status words (GIB_PP_*
     flags in [3], the molecule in [4]) are `status`"""
     if status[3]:
-        why = "; ".join(r for bit, r in _REASONS if status[3] & bit)
+        why = "; ".join(r for bit, r in reasons if status[3] & bit)
         raise ValueError(f"molecule {start + int(status[4])} (or a later one in molecules [{start}, {stop})): {why}")
 
 
@@ -102,15 +108,48 @@ def groups(nodes, edges, batch_size, n_atom_types, n_formal_charge, n_imp_H=0, n
     ws_bytes = lib.gib_preprocess_ws_bytes(ctypes.byref(d), chunk, max_rows)
     if ws_bytes == 0:
         raise ValueError(lib.gib_last_error().decode())
-    dev = torch.device(device)
-    if dev.type != "cuda":
-        raise RuntimeError("graphinvent_b200.preprocess runs on a CUDA device (no CPU fallback)")
-    ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
+    dev = _cuda(torch.device(device))
     in_nodes = torch.empty((chunk, N, F), dtype=torch.int8, device=dev)
     in_edges = torch.empty((chunk, N, N, Ef), dtype=torch.int8, device=dev)
-    out_nodes = torch.empty((max_rows, N, F), dtype=torch.int8, device=dev)
-    out_edges = torch.empty((max_rows, N, N, Ef), dtype=torch.int8, device=dev)
-    out_apds = torch.empty((max_rows, apd_len), dtype=torch.int32, device=dev)
+
+    def inputs(pos, stop):
+        in_nodes[:stop - pos].copy_(torch.from_numpy(nodes[pos:stop]))
+        in_edges[:stop - pos].copy_(torch.from_numpy(edges[pos:stop]))
+        return in_nodes, in_edges
+
+    if statistics:
+        splits = np.cumsum([N + 1, F, 10])
+    g, size = 0, 0
+    for pos, table, (out_nodes, out_edges, out_apds), rows in _chunks(d, M, chunk, max_rows, dev, inputs,
+                                                                      statistics):
+        on, oe, oa = out_nodes[:rows].cpu().numpy(), out_edges[:rows].cpu().numpy(), out_apds[:rows].cpu().numpy()
+        for row in table:
+            s, e, r0, r = row[:4].tolist()
+            full = r == B
+            size += B if full else e - s
+            stats = Statistics(*np.split(row[4:].astype(np.int64), splits)) if statistics else None
+            yield Group(g, g * B, pos + s, pos + e, full, on[r0:r0 + r], oe[r0:r0 + r], oa[r0:r0 + r], pos + e,
+                        size, stats)
+            g += 1
+
+
+def _cuda(dev):
+    if dev.type != "cuda":
+        raise RuntimeError("graphinvent_b200.preprocess runs on a CUDA device (no CPU fallback)")
+    return dev
+
+
+def _chunks(d, M, chunk, max_rows, dev, inputs, statistics=False):
+    """gib_preprocess_chunk over molecules [0, M) in chunks of at most `chunk`; inputs(pos, stop) gives the chunk's
+    molecules as int8 device tensors whose first stop - pos rows are molecules [pos, stop).  Yields per chunk the
+    first molecule, the host group table (int32 [groups, 4], or with statistics [groups, 4 + statistics words]) and the
+    device output buffers (out_nodes, out_edges, out_apds), valid until the next chunk runs, and the rows written."""
+    apd_len = lib.gib_preprocess_apd_length(ctypes.byref(d))
+    ws = torch.empty(lib.gib_preprocess_ws_bytes(ctypes.byref(d), chunk, max_rows), dtype=torch.uint8, device=dev)
+    N, F, Ef = d.N, d.F, d.Ef
+    out = (torch.empty((max_rows, N, F), dtype=torch.int8, device=dev),
+           torch.empty((max_rows, N, N, Ef), dtype=torch.int8, device=dev),
+           torch.empty((max_rows, apd_len), dtype=torch.int32, device=dev))
     out_groups = torch.empty((chunk, 4), dtype=torch.int32, device=dev)
     status = torch.empty(PP_STATUS_INTS, dtype=torch.int32, device=dev)
     if statistics:
@@ -120,17 +159,15 @@ def groups(nodes, edges, batch_size, n_atom_types, n_formal_charge, n_imp_H=0, n
         stats_ws = torch.empty(lib.gib_preprocess_group_statistics_ws_bytes(ctypes.byref(d), chunk),
                                dtype=torch.uint8, device=dev)
         stats_out = torch.empty((chunk, words), dtype=torch.int32, device=dev)
-        splits = np.cumsum([N + 1, F, 10])
     stream = torch.cuda.current_stream(dev)
-    pos, g, size = 0, 0, 0
+    pos = 0
     while pos < M:
         stop = min(pos + chunk, M)
         n = stop - pos
-        in_nodes[:n].copy_(torch.from_numpy(nodes[pos:stop]))
-        in_edges[:n].copy_(torch.from_numpy(edges[pos:stop]))
+        in_nodes, in_edges = inputs(pos, stop)
         check(lib.gib_preprocess_chunk(ctypes.byref(d), _ptr(in_nodes), _ptr(in_edges), n, int(stop == M), chunk,
-                                       max_rows, _ptr(ws), _ptr(out_nodes), _ptr(out_edges), _ptr(out_apds),
-                                       _ptr(out_groups), _ptr(status), ctypes.c_void_p(stream.cuda_stream)),
+                                       max_rows, _ptr(ws), *map(_ptr, out), _ptr(out_groups), _ptr(status),
+                                       ctypes.c_void_p(stream.cuda_stream)),
               "gib_preprocess_chunk")
         if statistics:
             check(lib.gib_preprocess_group_statistics(ctypes.byref(d), _ptr(in_nodes), _ptr(in_edges), n, chunk,
@@ -139,20 +176,146 @@ def groups(nodes, edges, batch_size, n_atom_types, n_formal_charge, n_imp_H=0, n
                   "gib_preprocess_group_statistics")
         st = status.cpu().numpy()
         refuse_bad(st, pos, stop)
-        ng, nxt, rows = int(st[0]), int(st[1]), int(st[2])
+        ng, nxt = int(st[0]), int(st[1])
         if ng == 0:
             raise RuntimeError("gib_preprocess_chunk completed no group")
-        gr = (stats_out if statistics else out_groups)[:ng].cpu().numpy()
-        on, oe, oa = out_nodes[:rows].cpu().numpy(), out_edges[:rows].cpu().numpy(), out_apds[:rows].cpu().numpy()
-        for row in gr:
-            s, e, r0, r = row[:4].tolist()
-            full = r == B
-            size += B if full else e - s
-            stats = Statistics(*np.split(row[4:].astype(np.int64), splits)) if statistics else None
-            yield Group(g, g * B, pos + s, pos + e, full, on[r0:r0 + r], oe[r0:r0 + r], oa[r0:r0 + r], pos + e,
-                        size, stats)
-            g += 1
+        yield pos, (stats_out if statistics else out_groups)[:ng].cpu().numpy(), out, int(st[2])
         pos += nxt
+
+
+def _check_stacks(nodes, edges):
+    """(M, N, F, Ef) of int8 stacks nodes [M, N, F] / edges [M, N, N, Ef]"""
+    if nodes.dtype not in (np.int8, torch.int8) or edges.dtype not in (np.int8, torch.int8) or nodes.ndim != 3 \
+            or edges.ndim != 4:
+        raise ValueError("nodes / edges must be int8 [M, N, F] / [M, N, N, Ef]")
+    M, N, F = nodes.shape
+    if tuple(edges.shape[:3]) != (M, N, N):
+        raise ValueError(f"edges {tuple(edges.shape)} do not match nodes {tuple(nodes.shape)}")
+    return M, N, F, edges.shape[3]
+
+
+def _on_device(x, device):
+    t = torch.from_numpy(np.ascontiguousarray(x)) if isinstance(x, np.ndarray) else x
+    return t.to(_cuda(torch.device(device))).contiguous()
+
+
+def _pp_dims(N, F, Ef, layout, batch_size=1):
+    d = PPDims(N=N, F=F, Ef=Ef, n_atom_types=layout[0], n_formal_charge=layout[1], n_imp_H=layout[2],
+               n_chirality=layout[3], batch_size=batch_size)
+    if lib.gib_preprocess_apd_length(ctypes.byref(d)) < 0:
+        raise ValueError(lib.gib_last_error().decode())
+    return d
+
+
+def file_rows(nodes, edges, batch_size, n_atom_types, n_formal_charge, n_imp_H=0, n_chirality=0,
+              chunk_molecules=4096, max_rows=None, keep=True, device="cuda"):
+    """The training-set construction of `groups` with its rows left on the device: (nodes, edges, apds), int8 device
+    tensors laid out as the file `run_data_processer` writes after its final resize -- each group's rows at
+    group * batch_size, APD counts clipped to int8 as h5py stores them, zero rows where no group wrote, and
+    `dataset_size` rows in all (the last group adds its molecule count, not its row count, so the file may cut rows
+    or end in zero rows).  `nodes` / `edges`: int8 [M, N, F] / [M, N, N, Ef] in decoding order, M >= 1 (device
+    tensors are used in place).
+    Returns (rows or None with keep=False, dataset_size).  The rows are views of buffers of the file's initial
+    length, sum over molecules of (bonds + 2) rows: at N*F + N*N*Ef + apd bytes a row."""
+    M, N, F, Ef = _check_stacks(nodes, edges)
+    if M == 0:
+        raise ValueError("no molecules")
+    layout = (n_atom_types, n_formal_charge, n_imp_H, n_chirality)
+    d = _pp_dims(N, F, Ef, layout, batch_size)
+    nodes, edges = _on_device(nodes, device), _on_device(edges, device)
+    B = batch_size
+    chunk = min(max(int(chunk_molecules), B), M)
+    max_rows = max(int(max_rows or 16 * chunk), B)
+    if lib.gib_preprocess_ws_bytes(ctypes.byref(d), chunk, max_rows) == 0:
+        raise ValueError(lib.gib_last_error().decode())
+    dev = nodes.device
+    rows = None
+    if keep:
+        total = int((torch.count_nonzero(edges.view(M, -1), dim=1) // 2 + 2).sum())
+        apd_len = lib.gib_preprocess_apd_length(ctypes.byref(d))
+        rows = (torch.zeros((total, N, F), dtype=torch.int8, device=dev),
+                torch.zeros((total, N, N, Ef), dtype=torch.int8, device=dev),
+                torch.zeros((total, apd_len), dtype=torch.int8, device=dev))
+    g, size = 0, 0
+    for _, table, out, _ in _chunks(d, M, chunk, max_rows, dev,
+                                    lambda pos, stop: (nodes[pos:stop], edges[pos:stop])):
+        if keep:
+            # one copy per run of groups whose rows follow each other both in `out` and in the file: [src, dst, rows]
+            runs = []
+            for i, (s, e, r0, r) in enumerate(table[:, :4].tolist()):
+                if runs and runs[-1][0] + runs[-1][2] == r0 and runs[-1][1] + runs[-1][2] == (g + i) * B:
+                    runs[-1][2] += r
+                else:
+                    runs.append([r0, (g + i) * B, r])
+            for src, dst, r in runs:
+                r = min(r, total - dst)        # past the file's initial length: cut by the final resize anyway
+                if r > 0:
+                    rows[0][dst:dst + r].copy_(out[0][src:src + r])
+                    rows[1][dst:dst + r].copy_(out[1][src:src + r])
+                    rows[2][dst:dst + r].copy_(out[2][src:src + r].clamp(-128, 127))
+        for s, e, r0, r in table[:, :4].tolist():
+            size += B if r == B else e - s
+        g += table.shape[0]
+    return (tuple(t[:size] for t in rows) if keep else None), size
+
+
+def rankings(n_atoms, N, seed=0, epoch=0, first=0, device="cuda"):
+    """int32 [M, N] device tensor: the node rankings `reorder` draws for molecules of n_atoms[m] atoms (-1 past
+    n_atoms[m]), uniform permutations that depend on (seed, epoch, first + m) only.  `first`: the index of molecule 0
+    in the whole set, so that a set drawn in pieces gets the rankings it gets drawn at once.  Draws nothing from
+    torch's generators."""
+    n = _on_device(torch.as_tensor(np.asarray(n_atoms, np.int32)), device)
+    M = n.numel()
+    out = torch.empty((M, N), dtype=torch.int32, device=n.device)
+    if M:
+        check(lib.gib_draw_rankings(M, N, _ptr(n), ctypes.c_ulonglong(seed % 2**64), epoch, first, _ptr(out),
+                                    ctypes.c_void_p(torch.cuda.current_stream(n.device).cuda_stream)),
+              "gib_draw_rankings")
+    return out
+
+
+_REORDER_REASONS = ((PP_BAD_NODES, "a node row that is not one-hot per segment with 0/1 entries, or a zero row "
+                     "between atoms"),
+                    (PP_BAD_EDGES, "edges that are not symmetric 0/1 single-type bonds between its atoms"),
+                    (PP_EMPTY, "no atoms"),
+                    (PP_DISCONNECTED, "a disconnected graph (the reference's searches do not terminate on it)"),
+                    (PP_BAD_RANKING, "a ranking that is not a permutation of 0..n-1 over its n atoms"))
+
+
+def reorder(nodes, edges, route="bfs", rankings=None, seed=0, epoch=0, *, layout, first=0, device="cuda"):
+    """`PreprocessingGraph.node_remap` (MolecularGraph.py:435-461) of every molecule of the int8 stacks `nodes`
+    [M, N, F] / `edges` [M, N, N, Ef] (numpy or torch, any atom order): `breadth_first_search` (route="bfs") or
+    `depth_first_search` ("dfs") from atom ranking[0], then `reorder_nodes`, atom for atom as the reference on
+    CPython 3.12.  `rankings`: int32 [M, N] (row m's first n entries a permutation of 0..n-1), or None to draw them on
+    the device from (seed, epoch, first + m) as `rankings()` does.  `layout`: the node-feature segment widths
+    (n_atom_types, n_formal_charge, n_imp_H, n_chirality), as `groups` takes them (`layout_of(constants)`).
+    Returns device tensors (nodes, edges, order): the reordered stacks and int32 [M, N] old atom indices in the new
+    order, -1 past the atom count.  Raises ValueError naming the first molecule that `groups` would refuse, that is
+    disconnected or empty, or whose ranking is not a permutation."""
+    if route not in ("bfs", "dfs"):
+        raise ValueError(f"route must be 'bfs' or 'dfs', got {route!r}")
+    M, N, F, Ef = _check_stacks(nodes, edges)
+    d = _pp_dims(N, F, Ef, tuple(layout))
+    nodes, edges = _on_device(nodes, device), _on_device(edges, device)
+    dev = nodes.device
+    if rankings is None:
+        rk = torch.empty((M, N), dtype=torch.int32, device=dev)
+    else:
+        rk = _on_device(torch.as_tensor(rankings), dev).to(torch.int32)
+        if tuple(rk.shape) != (M, N):
+            raise ValueError(f"rankings must be [M, N] = {(M, N)}, got {tuple(rk.shape)}")
+    out_nodes, out_edges = torch.empty_like(nodes), torch.empty_like(edges)
+    order = torch.empty((M, N), dtype=torch.int32, device=dev)
+    if M == 0:
+        return out_nodes, out_edges, order
+    ws = torch.empty(lib.gib_reorder_ws_bytes(M), dtype=torch.uint8, device=dev)
+    status = torch.empty(PP_STATUS_INTS, dtype=torch.int32, device=dev)
+    check(lib.gib_reorder(ctypes.byref(d), _ptr(nodes), _ptr(edges), M, ROUTE_BFS if route == "bfs" else ROUTE_DFS,
+                          int(rankings is None), ctypes.c_ulonglong(seed % 2**64), epoch, first, _ptr(rk), _ptr(order),
+                          _ptr(out_nodes), _ptr(out_edges), _ptr(ws), _ptr(status),
+                          ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)), "gib_reorder")
+    refuse_bad(status.cpu().numpy(), 0, M, _REORDER_REASONS)
+    return out_nodes, out_edges, order
 
 
 def ts_properties(stats, smiles, constants):

@@ -648,7 +648,8 @@ int gib_graph_statistics(int B, int N, int F, int Ef, const float* nodes, const 
  * segment is absent: the four action layouts), F their sum, batch_size >= 1, max_rows >= batch_size,
  * max_molecules * (N*(N-1)/2 + 2) < 2^30. */
 #define GIB_PP_STATUS_INTS 8
-enum { GIB_PP_BAD_NODES = 1, GIB_PP_BAD_EDGES = 2, GIB_PP_EMPTY = 4, GIB_PP_DISCONNECTED = 8 };
+enum { GIB_PP_BAD_NODES = 1, GIB_PP_BAD_EDGES = 2, GIB_PP_EMPTY = 4, GIB_PP_DISCONNECTED = 8,
+       GIB_PP_BAD_RANKING = 16 /* gib_reorder only */ };
 typedef struct gib_pp_dims {
   int N, F, Ef;                                             /* max_n_nodes, n_node_features, n_edge_features */
   int n_atom_types, n_formal_charge, n_imp_H, n_chirality;  /* node-feature segment widths, in order */
@@ -677,6 +678,29 @@ size_t gib_preprocess_group_statistics_ws_bytes(const gib_pp_dims* d, int max_mo
 int gib_preprocess_group_statistics(const gib_pp_dims* d, const signed char* nodes, const signed char* edges,
                                     int n_molecules, int max_molecules, const int* groups, const int* status,
                                     void* ws, int* out, gib_stream stream);
+
+/* ---- decoding routes: PreprocessingGraph.node_remap (MolecularGraph.py:435-461) per molecule -- breadth_first_search
+ *      or depth_first_search (MolecularGraph.py:328-433) from atom ranking[0], then reorder_nodes (graphinvent_b200.
+ *      preprocess.reorder).
+ * Input as gib_preprocess_chunk's, in any atom order (same dims and limits; d->batch_size is unused but must be >= 1).
+ * The atom count n is that of gib_preprocess_chunk (rows up to the last non-zero one).  rankings int32 [n_molecules, N]:
+ * entries [0, n) of row m a permutation of 0..n-1 (atom i's importance), read unless draw != 0; draw != 0: a uniform
+ * permutation per molecule is drawn from (seed, epoch, first_molecule + m) alone (as gib_draw_rankings) and written
+ * there, -1 past n.  BFS orders each layer as CPython 3.12's set of the layer's atoms iterates (DESIGN.md).
+ * Output: order int32 [n_molecules, N] (the old index of the atom at each new position, -1 past n), out_nodes /
+ * out_edges the reordered int8 stacks (zero past n).  status int32 [GIB_PP_STATUS_INTS]: [3] GIB_PP_* flags -- the
+ * input checks of gib_preprocess_chunk, GIB_PP_DISCONNECTED for a disconnected molecule, GIB_PP_BAD_RANKING -- and
+ * [4] the first flagged molecule (INT_MAX: none); a flagged molecule's order is -1 and its stacks zero.
+ * ws: gib_reorder_ws_bytes(n_molecules) bytes, may hold anything. */
+enum { GIB_ROUTE_BFS = 0, GIB_ROUTE_DFS = 1 };
+size_t gib_reorder_ws_bytes(int n_molecules);
+int gib_reorder(const gib_pp_dims* d, const signed char* nodes, const signed char* edges, int n_molecules, int route,
+                int draw, unsigned long long seed, long long epoch, long long first_molecule, int* rankings,
+                int* order, signed char* out_nodes, signed char* out_edges, void* ws, int* status, gib_stream stream);
+/* the rankings gib_reorder draws: row m of rankings [n_molecules, N] for a molecule of n_atoms[m] atoms (device int32),
+ * a function of (seed, epoch, first_molecule + m) only; N <= 181 */
+int gib_draw_rankings(int n_molecules, int N, const int* n_atoms, unsigned long long seed, long long epoch,
+                      long long first_molecule, int* rankings, gib_stream stream);
 
 /* ---- the likelihood of a molecule's decoding route (graphinvent_b200.graphed.RouteScorer): for every route state,
  *      p(action | state) = softmax(model(state))[action], one chunk of molecules at a time.
