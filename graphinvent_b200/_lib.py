@@ -74,7 +74,7 @@ class Scaffolds(ctypes.Structure):
 PP_STATUS_INTS = 8                                                  # GIB_PP_* (include/gib200.h)
 PP_BAD_NODES, PP_BAD_EDGES, PP_EMPTY, PP_DISCONNECTED, PP_BAD_RANKING = 1, 2, 4, 8, 16
 ROUTE_BFS, ROUTE_DFS = 0, 1                                         # GIB_ROUTE_BFS / GIB_ROUTE_DFS (gib_reorder)
-ROUTE_NOT_PREFIX, ROUTE_MASKED, ROUTE_BAD_ID = 1, 2, 4                # GIB_ROUTE_* (status[1] of the conditional plan)
+ROUTE_NOT_PREFIX, ROUTE_MASKED, ROUTE_BAD_ID, ROUTE_ACTION = 1, 2, 4, 8               # GIB_ROUTE_* (status[1] of the conditional plan)
 
 MOL_HDR_WORDS, MOL_WORDS, MOL_ATOM_WORDS = 8, 6, 3                 # GIB_MOL_* (include/gib200.h)
 MOL_DECODES, MOL_KEY_ERROR, MOL_DUPLICATE_BOND = 1, 2, 4
@@ -148,6 +148,7 @@ _PROTOS = {
     "gib_rl_sample_round_scaffold": (c_i, [c_i] * 8 + [c_p, c_p, c_p, c_i] + [c_p] * 17 + [c_i, c_p, c_p, c_p]),
     "gib_generation_mask_logits": (c_i, [c_i] * 4 + [c_p] * 8),
     "gib_rl_snapshot_scaffold": (c_i, [c_i] * 2 + [c_p] * 7),
+    "gib_action_mask_logits": (c_i, [c_i] * 10 + [c_p] * 12 + [c_i, c_p]),
     "gib_rl_snapshot": (c_i, [c_i] * 5 + [c_p] * 9),
     "gib_rl_restore": (c_i, [c_i] * 4 + [c_p] * 6),
     "gib_rl_gather": (c_i, [c_i] * 3 + [c_p] * 6),
@@ -179,6 +180,7 @@ _PROTOS = {
     "gib_route_plan_scaffold": (c_i, [c_p, c_p, c_p, c_i, c_i] + [c_p] * 6),
     "gib_route_fill_scaffold": (c_i, [c_p, c_p, c_p, c_i] + [c_p] * 11),
     "gib_route_mask_logits": (c_i, [c_i] * 4 + [c_p] * 5),
+    "gib_route_check_actions": (c_i, [c_p, c_p, c_p, c_i, c_i, c_p, c_p, c_i, c_p, c_p, c_p]),
     "gib_test_route_plan_offsets": (c_i, [c_p, c_i, c_p]),
     "gib_profile_enable": (None, [c_i]),
     "gib_launch_count": (c_ll, []),

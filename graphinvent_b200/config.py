@@ -6,6 +6,8 @@ any namedtuple/object with these attributes works -- the reference's own `consta
 """
 from collections import namedtuple
 
+import numpy as np
+
 DEFAULTS = dict(
     model="GGNN", device="cuda", big_positive=1e6, big_negative=-1e6,
     n_node_features=8, n_edge_features=3, max_n_nodes=13,          # gdb13: 5 atom types + 3 charges
@@ -82,6 +84,83 @@ def make_constants(model="GGNN", **overrides):
 
 def apd_length(C):
     return C.max_n_nodes * (C.len_f_add_per_node + C.len_f_conn_per_node) + 1
+
+
+# The action mask's valence limits (`action_mask="valence"`): the largest valence, in bonds counted by order (aromatic
+# 1.5) plus implicit hydrogens, that the mask lets an atom of that element and formal charge reach.  They are upper
+# bounds by design -- the mask removes only bonds that no valence state of the (element, charge) allows -- and this
+# package's own values, not checked against RDKit's valence model.
+DEFAULT_MAX_VALENCE = {
+    ("C", -1): 3, ("C", 0): 4, ("C", 1): 3,
+    ("N", -1): 2, ("N", 0): 3, ("N", 1): 4,
+    ("O", -1): 1, ("O", 0): 2, ("O", 1): 3,
+    ("S", -1): 5, ("S", 0): 6, ("S", 1): 7,
+    ("Cl", -1): 0, ("Cl", 0): 1, ("Cl", 1): 2,
+    ("H", 0): 1, ("B", 0): 3, ("F", 0): 1, ("Si", 0): 4, ("P", 0): 5, ("Br", 0): 1, ("I", 0): 1,
+}
+# bond orders in half-bond units, by the name of the reference's `int_to_bondtype` entries
+BOND_HALF_ORDERS = {"SINGLE": 2, "DOUBLE": 4, "TRIPLE": 6, "AROMATIC": 3}
+
+
+def _bond_name(bt):
+    """"SINGLE" for rdkit's BondType.SINGLE, its str() or the plain name"""
+    name = getattr(bt, "name", None) or str(bt)
+    return name.rsplit(".", 1)[-1].upper()
+
+
+def action_rule_table(n_atom_types, n_formal_charge, n_edge_features, n_imp_H=0, max_valence=None, constants=None):
+    """The action mask's rule table: (V int32 [A, CH], bond orders int32 [Ef] in half-bond units, implicit-H counts
+    int32 [H]).  Bond orders come from `constants.int_to_bondtype` (SINGLE / DOUBLE / TRIPLE / AROMATIC = 2 / 4 / 6 /
+    3), or in that order without it; implicit-H counts from `constants.imp_H`, or the index without it.
+
+    max_valence: None (DEFAULT_MAX_VALENCE), a dict keyed by element symbol (every charge of that element) or by
+    (symbol, charge), which overrides the defaults and is resolved through `constants.atom_types` /
+    `constants.formal_charge`, or an int array [A, CH] by index, which needs no constants.  A (type, charge) pair of
+    the layout that neither covers raises ValueError naming it."""
+    A, CH, Ef, H = int(n_atom_types), int(n_formal_charge), int(n_edge_features), int(n_imp_H)
+    itb = getattr(constants, "int_to_bondtype", None)
+    if itb is not None:
+        if len(itb) != Ef:
+            raise ValueError(f"constants.int_to_bondtype names {len(itb)} bond types, the layout has {Ef}")
+        names = [_bond_name(itb[i]) for i in range(Ef)]
+    elif Ef <= 4:
+        names = ["SINGLE", "DOUBLE", "TRIPLE", "AROMATIC"][:Ef]
+    else:
+        raise ValueError(f"{Ef} bond types need constants.int_to_bondtype to name their orders")
+    bad = [n for n in names if n not in BOND_HALF_ORDERS]
+    if bad:
+        raise ValueError(f"bond type {bad[0]} has no order here (known: {', '.join(BOND_HALF_ORDERS)})")
+    order = np.array([BOND_HALF_ORDERS[n] for n in names], np.int32)
+    imp = getattr(constants, "imp_H", None)
+    imp_h = np.array(list(imp) if imp is not None else range(H), np.int64) if H else np.zeros(0, np.int64)
+    if imp_h.size != H:
+        raise ValueError(f"constants.imp_H lists {imp_h.size} counts, the layout has {H} implicit-H indices")
+    if max_valence is not None and not isinstance(max_valence, dict):
+        V = np.asarray(max_valence)
+        if V.shape != (A, CH) or not np.issubdtype(V.dtype, np.integer):
+            raise ValueError(f"max_valence must be an int array [n_atom_types, n_formal_charge] = [{A}, {CH}] or a "
+                             f"dict, got {V.dtype} {V.shape}")
+    else:
+        atoms, charges = getattr(constants, "atom_types", None), getattr(constants, "formal_charge", None)
+        if atoms is None or charges is None:
+            raise ValueError("a valence table by element needs constants with atom_types and formal_charge; give "
+                             "max_valence as an int array [n_atom_types, n_formal_charge] instead")
+        if len(atoms) != A or len(charges) != CH:
+            raise ValueError(f"constants list {len(atoms)} atom types and {len(charges)} charges, the layout has "
+                             f"{A} and {CH}")
+        user = dict(max_valence or {})
+        V = np.zeros((A, CH), np.int64)
+        for t, sym in enumerate(atoms):
+            for c, q in enumerate(charges):
+                key = (sym, int(q))
+                v = user.get(key, user.get(sym, DEFAULT_MAX_VALENCE.get(key)))
+                if v is None:
+                    raise ValueError(f"no valence limit for atom type {sym!r} with formal charge {int(q):+d}: add "
+                                     f"max_valence={{({sym!r}, {int(q)}): ...}}")
+                V[t, c] = int(v)
+    if (V < 0).any() or (V > 1 << 20).any() or (imp_h < 0).any() or (imp_h > 1 << 20).any():
+        raise ValueError("valence limits and implicit-H counts must lie in [0, 2**20]")
+    return V.astype(np.int32), order, imp_h.astype(np.int32)
 
 
 def layout_dims(n_atom_types, n_formal_charge, n_edge_features=3, use_explicit_H=False, ignore_H=True,

@@ -32,14 +32,13 @@
 #include "../../include/gib200.h"
 #include "common.cuh"
 #include "ops.cuh"
+#include "action_mask.cuh"
 #include "scaffold_mask.cuh"
 
 namespace gib {
 
 // H / C = implicit-H / chirality index counts, 0 = segment absent; Lw = likelihood columns (2 * max_n_nodes)
 struct GenDims { int B, N, F, Ef, A, CH, H, C, Lw; };
-
-enum : int { ACT_ADD = 0, ACT_CONN = 1, ACT_TERM = 2 };
 
 // per slot: decoded action + validity  (one thread per slot)
 __global__ void gen_decode_kernel(GenDims d, const int* __restrict__ action, const float* __restrict__ edges,
@@ -49,59 +48,38 @@ __global__ void gen_decode_kernel(GenDims d, const int* __restrict__ action, con
   if (b >= d.B || (ctl && ctl[0] < 0)) return;
   const int a = action[b];
   const int n = n_nodes[b];
-  const int len_add = d.N * d.A * d.CH * max(d.H, 1) * max(d.C, 1) * d.Ef, len_conn = d.N * d.Ef;
-  int kind, bond_to = 0, atom = 0, charge = 0, imp_h = 0, chir = 0, btype = 0, bond_from = 0, invalid = 0;
+  const ActionLayout L{d.N, d.A, d.CH, d.H, d.C, d.Ef};
+  const int len_add = layout_len_add(L), len_conn = d.N * d.Ef;
+  Action x{ACT_TERM, 0, 0, 0, 0, 0, 0};
+  int bond_from = 0, invalid = 0;
   if (a < 0 || a > len_add + len_conn) {
     // not an APD index (a corrupted replay trace, or the sampler's NaN fallback): an invalid action that edits
     // nothing -- the slot terminates as "invalid" and is reset, no field of `rec` is out of range
-    kind = ACT_TERM;
     invalid = 1;
-  } else if (a < len_add) {
-    kind = ACT_ADD;
-    int r = a;
-    btype = r % d.Ef;
-    r /= d.Ef;
-    if (d.C) { chir = r % d.C; r /= d.C; }
-    if (d.H) { imp_h = r % d.H; r /= d.H; }
-    charge = r % d.CH;
-    r /= d.CH;
-    atom = r % d.A;
-    bond_to = r / d.A;
-    bond_from = n;
-    const bool empty = n == 0;
-    if (!empty && bond_to >= n) invalid = 1;          // bond to a non-existing atom          (:600-604)
-    if (empty && bond_to != 0) invalid = 1;           // first atom must use slot 0           (:606-610)
-    // f_add_idc[5]: bond_from (L0), bond_type (L1, L2) or chirality (L3)
-    const int e5_sel = (d.H == 0 && d.C == 0) ? 0 : (d.H && d.C) ? 2 : 1;
-    const int e5 = e5_sel == 0 ? bond_from : e5_sel == 2 ? chir : btype;
-    const bool madd = e5 >= d.N;
-    if (madd) invalid = 1;                            // "graph already holds max_n_nodes atoms" (:618)
-    if (madd || empty) {                              // get_actions: f_add_idc[5][max_node_idc] = 0   (:568)
-      if (e5_sel == 0) bond_from = 0;
-      else if (e5_sel == 2) chir = 0;
-      else btype = 0;
-    }
-    if (n >= d.N) { invalid = 1; bond_from = 0; }     // full graph: the L0 outcome in every layout (see above)
-  } else if (a < len_add + len_conn) {
-    kind = ACT_CONN;
-    const int c = a - len_add;
-    btype = c % d.Ef;
-    bond_to = c / d.Ef;
-    bond_from = n - 1;
-    if (bond_to >= n) invalid = 1;                    // (:616)
-    if (n == 0) invalid = 1;                          // (:619)
-    if (bond_to == bond_from) invalid = 1;            // self loop (:622)
-    const int bf = bond_from < 0 ? bond_from + d.N : bond_from;   // Python negative index
-    const float* e = edges + (((size_t)b * d.N + bond_to) * d.N + bf) * d.Ef;
-    float s = 0.f;
-    for (int t = 0; t < d.Ef; ++t) s += e[t];
-    if (s == 1.f) invalid = 1;                        // bond already present (:625-629)
-    bond_from = bf;
   } else {
-    kind = ACT_TERM;
+    // the rule of action_mask.cuh (GraphGenerator.py:573-657): the mask of gib_action_mask_logits forbids exactly
+    // the actions flagged invalid here
+    x = decode_action(a, L);
+    float psum = 0.f;
+    if (x.kind == ACT_CONN) psum = pair_sum(edges + (size_t)b * d.N * d.N * d.Ef, d.N, d.Ef, x.bond_to, n);
+    invalid = structure_forbidden(x, L, n, psum) ? 1 : 0;
+    if (x.kind == ACT_ADD) {
+      bond_from = n;
+      // get_actions: f_add_idc[5][max_node_idc] = 0 (:568) for adds past max_n_nodes and every add into an empty graph
+      if (add_e5(x, L, n) >= d.N || n == 0) {
+        const int e5_sel = layout_e5_sel(L);
+        if (e5_sel == 0) bond_from = 0;
+        else if (e5_sel == 2) x.chir = 0;
+        else x.btype = 0;
+      }
+      if (n >= d.N) bond_from = 0;                    // full graph: the L0 outcome in every layout (see above)
+    } else if (x.kind == ACT_CONN) {
+      bond_from = n - 1 < 0 ? n - 1 + d.N : n - 1;    // Python negative index
+    }
   }
-  rec[b] = make_int4(kind | (invalid << 4), bond_to | (bond_from << 8), atom | (charge << 8),
-                     btype | (imp_h << 8) | (chir << 16));
+  const int kind = x.kind;
+  rec[b] = make_int4(kind | (invalid << 4), x.bond_to | (bond_from << 8), x.atom | (x.charge << 8),
+                     x.btype | (x.imp_h << 8) | (x.chir << 16));
   // one class per slot: an index outside the APD decodes as kind TERM but counts once, as invalid (the scan gives every
   // flagged slot one output row; counting it in both classes left a row unwritten and over-counted n_generated)
   flags[b] = invalid ? 2 : (kind == ACT_TERM ? 1 : 0);
@@ -307,6 +285,67 @@ __global__ void __launch_bounds__(128) gen_mask_kernel(int N, int Ef, int apd, g
   }
   if (conn_all)
     for (int t = threadIdx.x; t < N * Ef; t += 128) o[len_add + t] = -INFINITY;
+}
+
+// the action mask (action_mask.cuh): one CTA per slot, -inf into every entry of the slot's logits row that the rule
+// forbids in its state (nodes [B, N, F] / edges [B, N, N, Ef], float in the generator, int8 in route batches), OR-ed
+// with the attachment-point rule of the slot's scaffold when sc.protect is given.  Terminate is never touched.  The
+// gate, `row` and first_slot mean what they mean for gen_mask_kernel; `row` selects the row of n_nodes and slot_ids
+// only, the state is always [B, ...].  table = V [A * CH] | bond orders [Ef] | implicit-H counts [H].
+template <typename T>
+__global__ void __launch_bounds__(128) gen_action_mask_kernel(ActionLayout L, int F, int apd, int valence,
+                                                              const int* __restrict__ table,
+                                                              const T* __restrict__ nodes, const T* __restrict__ edges,
+                                                              const int* __restrict__ n_nodes, gib_scaffolds sc,
+                                                              const int* __restrict__ slot_ids,
+                                                              const int* __restrict__ row,
+                                                              const int* __restrict__ state,
+                                                              const int* __restrict__ counters,
+                                                              float* __restrict__ logits, int first_slot) {
+  __shared__ int s_used[128], s_limit[128];
+  const int b = blockIdx.x, B = gridDim.x, N = L.N, Ef = L.Ef;
+  if (b < first_slot) return;
+  if (state && !(counters[0] < B && state[1] == 0 && state[0] >= 0 && state[0] < 2 * N)) return;
+  const size_t off = row ? (size_t)row[0] * B : 0;
+  int n;
+  if (n_nodes) {
+    n = min(max(n_nodes[off + b], 0), N);                  // a count outside [0, N] is read as the nearest bound
+  } else {                                                 // the number of non-empty node rows (N <= 127 < 128)
+    int live = 0;
+    if ((int)threadIdx.x < N) {
+      const T* nr = nodes + ((size_t)b * N + threadIdx.x) * F;
+      for (int f = 0; f < F; ++f) live |= nr[f] != T(0);
+    }
+    n = __syncthreads_count(live);
+  }
+  const T* e = edges + (size_t)b * N * N * Ef;
+  const int* V = valence ? table : nullptr;
+  const int* order = valence ? table + L.A * L.CH : nullptr;
+  const int* imp_h = valence ? order + Ef : nullptr;
+  if (valence) {
+    for (int i = threadIdx.x; i < n; i += 128) {
+      const int2 u = atom_usage(nodes + ((size_t)b * N + i) * F, e + (size_t)i * N * Ef, L, V, order, imp_h);
+      s_used[i] = u.x;
+      s_limit[i] = u.y;
+    }
+    __syncthreads();
+  }
+  const Valence v{s_used, s_limit, V, order, imp_h};
+  const unsigned int* pm = nullptr;
+  int k = 0;
+  if (sc.protect) {
+    const int s = slot_ids[off + b];
+    if (s >= 0 && s < sc.S) {
+      pm = sc.protect + (size_t)s * 4;
+      k = sc.n_atoms[s];
+    }
+  }
+  const int per_node = (apd - 1) / N - Ef;
+  float* o = logits + (size_t)b * apd;
+  for (int a = threadIdx.x; a < apd - 1; a += 128)
+    if (action_forbidden(a, L, n, e, valence != 0, v) ||
+        (pm && scaffold_forbidden(a, n, k, pm, N, Ef, per_node)))
+      o[a] = -INFINITY;
 }
 
 }  // namespace gib
@@ -566,6 +605,58 @@ extern "C" int gib_route_mask_logits(int B, int N, int Ef, int apd, const gib_sc
   if (!sc->protect) return 0;       // no attachment points: nothing is masked
   gen_mask_kernel<<<B, 128, 0, reinterpret_cast<cudaStream_t>(stream)>>>(N, Ef, apd, *sc, slot_ids, n_nodes, nullptr,
                                                                          nullptr, nullptr, logits, 0);
+  GIB_LAUNCH_CHECK();
+  return 0;
+}
+
+extern "C" int gib_action_mask_logits(int B, int N, int F, int Ef, int n_atom_types, int n_charges, int n_imp_H,
+                                      int n_chirality, int apd, int mode, const int* table, const float* nodes,
+                                      const float* edges, const signed char* nodes_i8, const signed char* edges_i8,
+                                      const int* n_nodes, const gib_scaffolds* sc, const int* slot_ids,
+                                      const int* row, const int* state, const int* counters, float* logits,
+                                      int first_slot, gib_stream stream) {
+  const bool counts_ok = n_atom_types > 0 && n_charges > 0 && Ef > 0 && n_imp_H >= 0 && n_chirality >= 0 &&
+                         n_atom_types <= 255 && n_charges <= 255 && Ef <= 255 && n_imp_H <= 255 && n_chirality <= 255;
+  if (!counts_ok || B <= 0 || N <= 0 || N > 127 || n_atom_types + n_charges + n_imp_H + n_chirality != F) {
+    set_error("gib_action_mask_logits: unsupported dims (B=%d N=%d F=%d A=%d CH=%d H=%d C=%d Ef=%d; N <= 127, the "
+              "counts lie in 1..255 (0..255 for implicit H / chirality) and F = A + CH + H + C)", B, N, F,
+              n_atom_types, n_charges, n_imp_H, n_chirality, Ef);
+    return -1;
+  }
+  const long long want = layout_apd(N, Ef, n_atom_types, n_charges, n_imp_H, n_chirality);
+  if (apd != want || want >= (1ll << 31)) {
+    set_error("gib_action_mask_logits: apd=%d, the action layout (N=%d A=%d CH=%d H=%d C=%d Ef=%d) has %lld actions",
+              apd, N, n_atom_types, n_charges, n_imp_H, n_chirality, Ef, want);
+    return -1;
+  }
+  const bool as_float = nodes && edges, as_i8 = nodes_i8 && edges_i8;
+  const int n_state = !!nodes + !!edges + !!nodes_i8 + !!edges_i8;
+  if ((mode != GIB_ACTION_MASK_STRUCTURE && mode != GIB_ACTION_MASK_VALENCE) || n_state != 2 ||
+      !(as_float || as_i8) || !logits ||
+      (mode == GIB_ACTION_MASK_VALENCE && !table) || (!state != !counters) || (first_slot != 0 && first_slot != 1)) {
+    set_error("gib_action_mask_logits: bad arguments (mode=%d first_slot=%d; mode is GIB_ACTION_MASK_STRUCTURE or "
+              "GIB_ACTION_MASK_VALENCE, the valence mode needs the table, the state is given as float nodes and edges "
+              "or as int8 nodes and edges, logits must be given, state and counters together or neither, "
+              "first_slot is 0 or 1)", mode, first_slot);
+    return -1;
+  }
+  gib_scaffolds scv{};
+  if (sc && sc->protect) {
+    if (sc->S <= 0 || !sc->n_atoms || !slot_ids) {
+      set_error("gib_action_mask_logits: a scaffold table with attachment points needs S >= 1, n_atoms and slot_ids");
+      return -1;
+    }
+    scv = *sc;
+  }
+  const ActionLayout L{N, n_atom_types, n_charges, n_imp_H, n_chirality, Ef};
+  const int valence = mode == GIB_ACTION_MASK_VALENCE;
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  if (as_float)
+    gen_action_mask_kernel<float><<<B, 128, 0, st>>>(L, F, apd, valence, table, nodes, edges, n_nodes, scv, slot_ids,
+                                                     row, state, counters, logits, first_slot);
+  else
+    gen_action_mask_kernel<signed char><<<B, 128, 0, st>>>(L, F, apd, valence, table, nodes_i8, edges_i8, n_nodes,
+                                                           scv, slot_ids, row, state, counters, logits, first_slot);
   GIB_LAUNCH_CHECK();
   return 0;
 }

@@ -22,6 +22,7 @@
 #include <climits>
 
 #include "common.cuh"
+#include "action_mask.cuh"
 #include "scaffold_mask.cuh"
 #include "../../include/gib200.h"
 
@@ -1292,6 +1293,61 @@ int gib_route_fill_scaffold(const gib_pp_dims* d, const signed char* nodes, cons
   const int blocks = (int)std::min<long long>(need, kFillMaxBlocks);
   route_fill_kernel<<<blocks, kFillNT, 0, (cudaStream_t)stream>>>(p, f, status, ctl, slots, out_nodes, out_edges, nc,
                                                                   ec, scaffold_ids, slot_ids, slot_n);
+  GIB_LAUNCH_CHECK();
+  return 0;
+}
+
+// the action mask's rule on the planned routes: one warp per molecule.  Every kept state's action against the structural
+// rule with its state's atom count -- a route state never holds the bond its connect adds, so the duplicate-bond test
+// has nothing to find -- and, with valence, every atom of the whole molecule (state 0 of the plan: valences only grow
+// along a route, so its states are all within the table exactly when the molecule is)
+__global__ void __launch_bounds__(32) route_action_check_kernel(ActionLayout L, int F, const int* __restrict__ off,
+                                                                const int* __restrict__ apd,
+                                                                const int* __restrict__ nn,
+                                                                const signed char* __restrict__ nodes,
+                                                                const signed char* __restrict__ edges, int valence,
+                                                                const int* __restrict__ table, int* result) {
+  const int m = blockIdx.x, lane = threadIdx.x, N = L.N;
+  const int s0 = off[m], s1 = off[m + 1];
+  if (s1 == s0) return;                       // refused by the plan (GIB_ROUTE_NOT_PREFIX / _BAD_ID)
+  bool bad = false;
+  for (int s = s0 + lane; s < s1; s += 32) bad |= structure_forbidden(decode_action(apd[s], L), L, nn[s], 0.f);
+  if (valence) {
+    const int* order = table + L.A * L.CH;
+    const int n = min(max(nn[s0], 0), N);
+    for (int i = lane; i < n; i += 32) {
+      const int2 u = atom_usage(nodes + ((size_t)m * N + i) * F, edges + (((size_t)m * N + i) * N) * L.Ef, L, table,
+                                order, order + L.Ef);
+      bad |= u.x > u.y;
+    }
+  }
+  if (__any_sync(0xffffffffu, bad) && lane == 0) {
+    atomicOr(&result[0], GIB_ROUTE_ACTION);
+    atomicMin(&result[1], m);
+  }
+}
+
+int gib_route_check_actions(const gib_pp_dims* d, const signed char* nodes, const signed char* edges, int n_molecules,
+                            int max_molecules, const void* ws, const int* offsets, int mode, const int* table,
+                            int* result, gib_stream stream) {
+  PP p;
+  GIB_TRY(route_limits("gib_route_check_actions", d, max_molecules, &p));
+  if (n_molecules < 1 || n_molecules > max_molecules || p.N > 127 || !nodes || !edges || !ws || !offsets ||
+      !result || (mode != GIB_ACTION_MASK_STRUCTURE && mode != GIB_ACTION_MASK_VALENCE) ||
+      (mode == GIB_ACTION_MASK_VALENCE && !table)) {
+    set_error("gib_route_check_actions: bad arguments (n_molecules=%d max_molecules=%d N=%d mode=%d; N <= 127, the "
+              "buffers must be given, the valence mode needs the table)", n_molecules, max_molecules, p.N, mode);
+    return -1;
+  }
+  const ActionLayout L{p.N, d->n_atom_types, d->n_formal_charge, d->n_imp_H, d->n_chirality, p.Ef};
+  const RouteWs w = route_ws_layout(p, max_molecules);
+  const char* b = static_cast<const char*>(ws);
+  cudaStream_t s = (cudaStream_t)stream;
+  GIB_CUDA_TRY(cudaMemsetAsync(result, 0, sizeof(int), s));
+  GIB_CUDA_TRY(cudaMemsetAsync(result + 1, 0x7f, sizeof(int), s));     // 0x7f7f7f7f: no molecule yet
+  route_action_check_kernel<<<n_molecules, 32, 0, s>>>(L, p.F, offsets, (const int*)(b + w.apd),
+                                                       (const int*)(b + w.nn), nodes, edges,
+                                                       mode == GIB_ACTION_MASK_VALENCE, table, result);
   GIB_LAUNCH_CHECK();
   return 0;
 }

@@ -158,7 +158,7 @@ __global__ void rl_snapshot_scaffold_kernel(int B, int N, const int* __restrict_
   const int b = blockIdx.x * blockDim.x + threadIdx.x;
   const int r = state[0];
   if (b >= B || !(counters[0] < B && state[1] == 0 && r >= 0 && r < 2 * N)) return;
-  rec_ids[(size_t)r * B + b] = slot_ids[b];
+  if (rec_ids) rec_ids[(size_t)r * B + b] = slot_ids[b];
   rec_n[(size_t)r * B + b] = n_nodes[b];
 }
 
@@ -252,8 +252,9 @@ int gib_rl_snapshot(int B, int N, int F, int Ef, int att_view, const float* node
 
 int gib_rl_snapshot_scaffold(int B, int N, const int* slot_ids, const int* n_nodes, const int* state,
                              const int* counters, int* rec_ids, int* rec_n, gib_stream stream) {
-  if (B <= 0 || N <= 0 || N > 127 || !slot_ids || !n_nodes || !state || !counters || !rec_ids || !rec_n) {
-    set_error("gib_rl_snapshot_scaffold: bad arguments (B=%d N=%d; every buffer must be given)", B, N);
+  if (B <= 0 || N <= 0 || N > 127 || !slot_ids != !rec_ids || !n_nodes || !state || !counters || !rec_n) {
+    set_error("gib_rl_snapshot_scaffold: bad arguments (B=%d N=%d; every buffer must be given, slot_ids and rec_ids "
+              "both or neither)", B, N);
     return -1;
   }
   rl_snapshot_scaffold_kernel<<<(unsigned)ceil_div(B, 256), 256, 0, ST(stream)>>>(B, N, slot_ids, n_nodes, state,

@@ -163,6 +163,55 @@ class ScaffoldTable:
                          gen_scaffolds=ptr(gen_scaffolds), S=self.S)
 
 
+ACTION_MASK_MODES = {"structure": 1, "valence": 2}          # GIB_ACTION_MASK_* (include/gib200.h)
+
+
+class ActionMask:
+    """The action mask of a generator or route scorer (`action_mask=`, `gib_action_mask_logits`): logit -inf for
+    every action the round would reject as invalid in the slot's state ("structure": a bond to an atom that does not
+    exist, a self loop, a bond that exists, an add into a full graph, ...), and with "valence" also every bond that
+    takes an atom past its limit in the table of `config.action_rule_table(max_valence=...)`.  Terminate is never
+    masked.  The rule is graphinvent_b200/csrc/action_mask.cuh, the one the round's decode kernel flags invalid
+    actions with."""
+
+    def __init__(self, mode, max_valence, constants, layout, N, F, Ef, apd, device):
+        if mode not in ACTION_MASK_MODES:
+            raise ValueError(f"action_mask must be None, 'structure' or 'valence', got {mode!r}")
+        if max_valence is not None and mode != "valence":
+            raise ValueError("max_valence is read by action_mask='valence' only")
+        if N > 127:
+            raise ValueError(f"the action mask needs max_n_nodes N <= 127, got N = {N}")
+        from .config import action_rule_table
+        self.mode, self.code = mode, ACTION_MASK_MODES[mode]
+        self.layout, self.N, self.F, self.Ef, self.apd = tuple(layout), N, F, Ef, apd
+        self.valence, self.bond_orders, self.imp_h, self.table = None, None, None, None
+        if mode == "valence":
+            A, CH, H, _ = layout
+            self.valence, self.bond_orders, self.imp_h = action_rule_table(A, CH, Ef, H, max_valence, constants)
+            flat = np.concatenate([self.valence.ravel(), self.bond_orders, self.imp_h]).astype(np.int32)
+            self.table = torch.from_numpy(flat).to(torch.device(device))
+
+    def apply(self, B, logits, n_nodes, stream, nodes=None, edges=None, int8=False, sc=None, slot_ids=None, row=None,
+              state=None, counters=None, first_slot=1):
+        """-inf in place into logits [B, apd]; nodes / edges float (int8=False) or int8 [B, ...]; sc (a gib_scaffolds
+        with attachment points) and slot_ids: that rule too, in the same launch"""
+        p = lambda t: _ptr(t) if t is not None else None
+        fl = (p(nodes), p(edges), None, None) if not int8 else (None, None, p(nodes), p(edges))
+        check(lib.gib_action_mask_logits(
+            B, self.N, self.F, self.Ef, *self.layout, self.apd, self.code, p(self.table), *fl, p(n_nodes),
+            ctypes.byref(sc) if sc is not None else None, p(slot_ids), p(row), p(state), p(counters), _ptr(logits),
+            first_slot, stream), "gib_action_mask_logits")
+
+
+def make_action_mask(mode, max_valence, constants, layout, N, F, Ef, apd, device):
+    """the ActionMask of a constructor's `action_mask=` / `max_valence=` (None for None)"""
+    if mode is None:
+        if max_valence is not None:
+            raise ValueError("max_valence needs action_mask='valence'")
+        return None
+    return ActionMask(mode, max_valence, constants, layout, N, F, Ef, apd, device)
+
+
 def scaffold_table(scaffolds, attachment, N, F, Ef, layout, device):
     """the ScaffoldTable of `set_scaffolds`' arguments (None for None), for the generators and the route scorer"""
     if scaffolds is None:
@@ -175,10 +224,15 @@ def scaffold_table(scaffolds, attachment, N, F, Ef, layout, device):
 
 class GraphGenerator:
     """`scaffolds=(nodes, edges)` / `attachment=`: decorate those scaffolds instead of growing molecules from the empty
-    graph (`ScaffoldTable`; `set_scaffolds` changes them).  None (the default) keeps the reference's behaviour."""
+    graph (`ScaffoldTable`; `set_scaffolds` changes them).  None (the default) keeps the reference's behaviour.
+
+    `action_mask="structure"` / `"valence"` (`ActionMask`): sample only actions the round accepts, from the model's
+    softmax renormalised over them; `max_valence=` overrides the valence table (`config.action_rule_table`).  With
+    attachment points too, one launch applies both rules."""
 
     def __init__(self, model, batch_size, constants=None, n_atom_types=None, n_formal_charge=None, n_imp_H=None,
-                 n_chirality=None, device="cuda", scaffolds=None, attachment=None):
+                 n_chirality=None, device="cuda", scaffolds=None, attachment=None, action_mask=None,
+                 max_valence=None):
         C, self.A, self.CH, self.n_imp_H, self.n_chirality = action_layout(
             model, constants, n_atom_types, n_formal_charge, n_imp_H, n_chirality)
         self.constants = C
@@ -188,14 +242,19 @@ class GraphGenerator:
         self.rounds = 0
         self.scaffolds = None
         self.generated_scaffolds = None
+        self.action_mask = make_action_mask(action_mask, max_valence, C, self.layout, self.N, self.F, self.Ef, self.apd,
+                                            self.device)
         self._allocate()
         if scaffolds is not None:
             self.set_scaffolds(scaffolds, attachment)
 
+    @property
+    def layout(self):
+        return (self.A, self.CH, self.n_imp_H, self.n_chirality)
+
     def _table(self, scaffolds, attachment):
         """the ScaffoldTable of set_scaffolds' arguments (None for None)"""
-        return scaffold_table(scaffolds, attachment, self.N, self.F, self.Ef,
-                              (self.A, self.CH, self.n_imp_H, self.n_chirality), self.device)
+        return scaffold_table(scaffolds, attachment, self.N, self.F, self.Ef, self.layout, self.device)
 
     def set_scaffolds(self, scaffolds, attachment=None):
         """decorate `scaffolds` = (nodes, edges) from the next batch on (None: grow from the empty graph again)"""
@@ -213,7 +272,13 @@ class GraphGenerator:
                                                _ptr(self.likelihoods), stream), "gib_generation_scaffold_init")
 
     def _mask(self, logits, stream, slot_ids=None, n_nodes=None):
-        """-inf into the logits [B, apd] (in place) of the actions the attachment points forbid in this round's state"""
+        """-inf into the logits [B, apd] (in place) of the actions the attachment points and the action mask forbid in
+        this round's state"""
+        if self.action_mask is not None:
+            self.action_mask.apply(self.batch_size, logits, self.n_nodes, stream, self.nodes, self.edges,
+                                   sc=self._sc if self.masked else None,
+                                   slot_ids=self._slot_ids if self.masked else None)
+            return
         check(lib.gib_generation_mask_logits(
             self.batch_size, self.N, self.Ef, self.apd, ctypes.byref(self._sc),
             _ptr(slot_ids if slot_ids is not None else self._slot_ids),
@@ -224,6 +289,11 @@ class GraphGenerator:
     def masked(self):
         """True when attachment points restrict the actions"""
         return self.scaffolds is not None and self.scaffolds.protect is not None
+
+    @property
+    def masks_logits(self):
+        """True when the round's logits are masked: attachment points or the action mask"""
+        return self.masked or self.action_mask is not None
 
     def _allocate(self):
         B, N, F, Ef, dev = self.batch_size, self.N, self.F, self.Ef, self.device
@@ -305,7 +375,7 @@ class GraphGenerator:
                 lik = lik.to(self.device, torch.float32).contiguous()
             else:
                 out = self.model(*self._model_inputs(self.model))    # GraphGenerator.py:121
-                if self.masked:
+                if self.masks_logits:
                     out = out.contiguous()
                     self._mask(out, st)
                 action, lik = Fn.sample_actions(out, generator=generator)
@@ -390,7 +460,7 @@ class GraphGeneratorRL(GraphGenerator):
             graph = Fn.build_graph(agent, edges_in) if share else None
             out_a = agent(nodes_in, edges_in, graph=graph) if share else agent(nodes_in, edges_in)   # GraphGeneratorRL.py:131-132
             out_p = prior(nodes_in, edges_in, graph=graph) if share else prior(nodes_in, edges_in)
-            if self.masked:                      # the attachment mask as a detached 0 / -inf bias: softmax renormalises
+            if self.masks_logits:                # the masks as a detached 0 / -inf bias: both softmaxes renormalise
                 bias = torch.zeros(B, self.apd, dtype=torch.float32, device=self.device)
                 self._mask(bias, st)
                 out_a, out_p = out_a + bias, out_p + bias

@@ -86,8 +86,8 @@ import torch
 
 from . import functional as F
 from .config import matmul_code
-from ._lib import (FLAG_MULTITYPE, FLAG_OVERFLOW, HDR_FLAGS, HDR_INTS, ROUTE_BAD_ID, ROUTE_MASKED, ROUTE_NOT_PREFIX,
-                   EvalPass, check, lib)
+from ._lib import (FLAG_MULTITYPE, FLAG_OVERFLOW, HDR_FLAGS, HDR_INTS, PP_STATUS_INTS, ROUTE_ACTION, ROUTE_BAD_ID,
+                   ROUTE_MASKED, ROUTE_NOT_PREFIX, EvalPass, check, lib)
 from .generation import GraphGenerator
 
 _u8 = torch.uint8
@@ -653,9 +653,11 @@ class GraphedGenerator(GraphGenerator):
     given in both or in neither; otherwise it reallocates and the next batch recaptures."""
 
     def __init__(self, model, batch_size, constants=None, n_atom_types=None, n_formal_charge=None, n_imp_H=None,
-                 n_chirality=None, device="cuda", scaffolds=None, attachment=None):
+                 n_chirality=None, device="cuda", scaffolds=None, attachment=None, action_mask=None,
+                 max_valence=None):
         super().__init__(model, batch_size, constants=constants, n_atom_types=n_atom_types,
-                         n_formal_charge=n_formal_charge, n_imp_H=n_imp_H, n_chirality=n_chirality, device=device)
+                         n_formal_charge=n_formal_charge, n_imp_H=n_imp_H, n_chirality=n_chirality, device=device,
+                         action_mask=action_mask, max_valence=max_valence)
         if not hasattr(model, "dims"):
             raise TypeError("GraphedGenerator runs this package's models (graphinvent_b200.gnn.mpnn) only")
         B, N, dev = self.batch_size, self.N, self.device
@@ -741,7 +743,13 @@ class GraphedGenerator(GraphGenerator):
             self._scaffold_init(F._stream(self.device))
 
     def _mask_round(self, logits, st):
-        """the attachment mask on a captured round's logits, gated by the round state"""
+        """the attachment and action masks on a captured round's logits, gated by the round state"""
+        if self.action_mask is not None:
+            self.action_mask.apply(self.batch_size, logits, self.n_nodes, st, self.nodes, self.edges,
+                                   sc=self._sc if self.masked else None,
+                                   slot_ids=self._slot_ids if self.masked else None, state=self._state,
+                                   counters=self._counters)
+            return
         check(lib.gib_generation_mask_logits(self.batch_size, self.N, self.Ef, self.apd, ctypes.byref(self._sc),
                                              F._ptr(self._slot_ids), F._ptr(self.n_nodes), None, F._ptr(self._state),
                                              F._ptr(self._counters), F._ptr(logits), st), "gib_generation_mask_logits")
@@ -774,11 +782,11 @@ class GraphedGenerator(GraphGenerator):
             self._edges_in[0].copy_(e0 * (nz & (nz.to(torch.int32).cumsum(-1) == 1)).to(e0.dtype))
         _k0_forward(self, self.nodes, self._edges_in, [(self.packed, self.logits)], st)
         self._flags.bitwise_or_(self._hdr_flags)
+        if self.masks_logits:
+            self._mask_round(self.logits, st)
         if self.scaffolds is None:
             fn, name, sc = lib.gib_generation_sample_round, "gib_generation_sample_round", ()
         else:
-            if self.masked:
-                self._mask_round(self.logits, st)
             fn, name, sc = (lib.gib_generation_sample_round_scaffold, "gib_generation_sample_round_scaffold",
                             (ctypes.byref(self._sc),))
         check(fn(
@@ -843,13 +851,14 @@ class GraphedGenerator(GraphGenerator):
 
 
 # ---- the RL rollout -------------------------------------------------------------------------------------------
-def rl_record_bytes(batch_size, max_n_nodes, n_node_features, n_edge_features, masked=False):
+def rl_record_bytes(batch_size, max_n_nodes, n_node_features, n_edge_features, masked=False, action_mask=False):
     """device bytes one `GraphedGeneratorRL.sample()` keeps for its backward at the 2N-round limit (a rollout of R
     rounds keeps R / 2N of the per-round part): the int8 model input of every round, the action and both models'
     probabilities per (round, slot), and the (molecule, round) -> slot map [2B, 2N] in fp32.  masked=True (scaffolds
-    with attachment points): also each (round, slot)'s scaffold id and atom count, int32 each"""
+    with attachment points): also each (round, slot)'s scaffold id and atom count, int32 each; action_mask=True
+    without attachment points: the atom count alone"""
     B, N, F_, Ef = int(batch_size), int(max_n_nodes), int(n_node_features), int(n_edge_features)
-    per_round = B * (N * F_ + N * N * Ef) + B * (4 + 4 + 4) + (B * 8 if masked else 0)
+    per_round = B * (N * F_ + N * N * Ef) + B * (4 + 4 + 4) + (B * 8 if masked else B * 4 if action_mask else 0)
     return 2 * N * per_round + 2 * B * 2 * N * 4
 
 
@@ -905,13 +914,18 @@ class GraphedGeneratorRL(GraphedGenerator):
     With scaffolds and attachment points both models' logits are masked before `gib_rl_sample_round_scaffold`, and
     the record also keeps each (round, slot)'s scaffold id and atom count (`gib_rl_snapshot_scaffold`), from which the
     backward round masks the recomputed logits the same way before `gib_rl_dlogits`: the recomputed probabilities
-    still equal the rollout's.  A `set_scaffolds` between a rollout and its backward makes that backward raise."""
+    still equal the rollout's.  A `set_scaffolds` between a rollout and its backward makes that backward raise.
+
+    With `action_mask=` both models' logits go through the action mask (with attachment points too, in the same
+    launch) and the record keeps each (round, slot)'s atom count; the backward round rebuilds the mask from the
+    restored int8 state and those counts."""
 
     def __init__(self, model, batch_size, constants=None, n_atom_types=None, n_formal_charge=None, n_imp_H=None,
-                 n_chirality=None, device="cuda", scaffolds=None, attachment=None):
+                 n_chirality=None, device="cuda", scaffolds=None, attachment=None, action_mask=None,
+                 max_valence=None):
         GraphGenerator.__init__(self, model, batch_size, constants=constants, n_atom_types=n_atom_types,
                                 n_formal_charge=n_formal_charge, n_imp_H=n_imp_H, n_chirality=n_chirality,
-                                device=device)
+                                device=device, action_mask=action_mask, max_valence=max_valence)
         if not hasattr(model, "dims"):
             raise TypeError("GraphedGeneratorRL runs this package's models (graphinvent_b200.gnn.mpnn) only")
         B, N, dev = self.batch_size, self.N, self.device
@@ -953,6 +967,8 @@ class GraphedGeneratorRL(GraphedGenerator):
         self.inert_rounds = 0
         self.backward_rounds = [0, 0]
         self._scaffold_m, self.scaffold_version = 0, 0
+        self.rec_ids = None
+        self.rec_n = torch.zeros(2 * N, B, dtype=torch.int32, device=dev) if self.action_mask is not None else None
         if scaffolds is not None:
             self.set_scaffolds(scaffolds, attachment)
 
@@ -967,7 +983,8 @@ class GraphedGeneratorRL(GraphedGenerator):
         if self.masked and getattr(self, "rec_ids", None) is None:
             B, N, dev = self.batch_size, self.N, self.device
             self.rec_ids = torch.full((2 * N, B), -1, dtype=torch.int32, device=dev)
-            self.rec_n = torch.zeros(2 * N, B, dtype=torch.int32, device=dev)
+            if getattr(self, "rec_n", None) is None:
+                self.rec_n = torch.zeros(2 * N, B, dtype=torch.int32, device=dev)
 
     def _check_pair(self, agent, prior):
         for m in (agent, prior):
@@ -995,18 +1012,19 @@ class GraphedGeneratorRL(GraphedGenerator):
                                   F._ptr(self._state), F._ptr(self._counters), F._ptr(self.rec_nodes),
                                   F._ptr(self.rec_edges), F._ptr(self.in_nodes), F._ptr(self.in_edges), st),
               "gib_rl_snapshot")
-        if self.masked:
-            check(lib.gib_rl_snapshot_scaffold(B, N, F._ptr(self._slot_ids), F._ptr(self.n_nodes), F._ptr(self._state),
-                                               F._ptr(self._counters), F._ptr(self.rec_ids), F._ptr(self.rec_n), st),
+        if self.masks_logits:
+            ids = (self._slot_ids, self.rec_ids) if self.masked else (None, None)
+            check(lib.gib_rl_snapshot_scaffold(B, N, F._ptr(ids[0]), F._ptr(self.n_nodes), F._ptr(self._state),
+                                               F._ptr(self._counters), F._ptr(ids[1]), F._ptr(self.rec_n), st),
                   "gib_rl_snapshot_scaffold")
         _k0_forward(self, self.in_nodes, self.in_edges, list(zip(self.packed, self.logits)), st)
         self._flags.bitwise_or_(self._hdr_flags)
+        if self.masks_logits:
+            for logits in self.logits:
+                self._mask_round(logits, st)
         if self.scaffolds is None:
             fn, name, sc = lib.gib_rl_sample_round, "gib_rl_sample_round", ()
         else:
-            if self.masked:
-                for logits in self.logits:
-                    self._mask_round(logits, st)
             fn, name, sc = lib.gib_rl_sample_round_scaffold, "gib_rl_sample_round_scaffold", (ctypes.byref(self._sc),)
         check(fn(
             B, N, self.F, self.Ef, self.A, self.CH, self.n_imp_H, self.n_chirality, *sc, F._ptr(self.logits[0]),
@@ -1025,7 +1043,15 @@ class GraphedGeneratorRL(GraphedGenerator):
                                  F._ptr(b.ctl), F._ptr(self.in_nodes), F._ptr(self.in_edges), st), "gib_rl_restore")
         _k0_forward(self, self.in_nodes, self.in_edges, [(self.packed[slot], self.logits[0])], st)
         sampled = self.logits[0]
-        if self.masked:
+        if self.action_mask is not None:
+            # the rollout's masks, from the restored state and the round's recorded atom counts (and scaffold ids), on
+            # a copy: the model backward reads the unmasked output
+            sampled = self.logits[1]
+            sampled.copy_(self.logits[0])
+            self.action_mask.apply(B, sampled, self.rec_n, st, self.in_nodes, self.in_edges, int8=True,
+                                   sc=self._sc if self.masked else None,
+                                   slot_ids=self.rec_ids if self.masked else None, row=b.ctl)
+        elif self.masked:
             # the rollout's mask, from the round's recorded scaffold ids and atom counts, on a copy: the model backward
             # reads the unmasked output
             sampled = self.logits[1]
@@ -1081,6 +1107,7 @@ class GraphedGeneratorRL(GraphedGenerator):
         self.act_rec[:R].copy_(rec.act)
         if self.masked:
             self.rec_ids[:R].copy_(rec.ids)
+        if self.masks_logits:
             self.rec_n[:R].copy_(rec.n)
         grads = [d.contiguous().float() if ps is not None else None
                  for d, ps in ((d_a, params_a), (d_b, params_b))]
@@ -1140,7 +1167,9 @@ class GraphedGeneratorRL(GraphedGenerator):
             self._ensure_backward()
             rec.nodes, rec.edges, rec.act = self.rec_nodes[:R].clone(), self.rec_edges[:R].clone(), self.act_rec[:R].clone()
             if self.masked:
-                rec.ids, rec.n = self.rec_ids[:R].clone(), self.rec_n[:R].clone()
+                rec.ids = self.rec_ids[:R].clone()
+            if self.masks_logits:
+                rec.n = self.rec_n[:R].clone()
             lik_a, lik_b = _RolloutLikelihoods.apply(self, rec, len(pa), *pa, *pb)
         else:
             lik_a, lik_b = self._gather(rec)
@@ -1167,7 +1196,9 @@ _ROUTE_REASONS = (
                        "scaffold's rows, or another bond among the scaffold's atoms -- an extra bond between two "
                        "scaffold atoms too: its canonical route does not pass through the scaffold's state)"),
     (ROUTE_MASKED, "its conditional route takes an action the scaffold's attachment points forbid (probability 0)"),
-    (ROUTE_BAD_ID, "the scaffold id lies outside [-1, S)"))
+    (ROUTE_BAD_ID, "the scaffold id lies outside [-1, S)"),
+    (ROUTE_ACTION, "its route takes an action the action mask forbids (probability 0): with 'valence', an atom of the "
+                   "molecule is over its limit in the valence table"))
 
 ROUTE_MIN_BATCH = 256        # rows from which the forward GEMMs take the tensor-core kernel (csrc/gemm_simt.cu)
 
@@ -1280,12 +1311,21 @@ class RouteScorer:
     its route kernels and reads the status words once; the captured graph is fill (`gib_route_fill_scaffold`), K0, the
     forward, the mask (with attachment points), `gib_route_probs`.  The backward masks a copy of the recomputed logits
     (the model backward reads the unmasked output), so masked entries get zero dlogits; a `set_scaffolds` between
-    `score()` and its backward makes the backward raise.  `scaffold_ids=None` runs the unconditional path unchanged."""
+    `score()` and its backward makes the backward raise.  `scaffold_ids=None` runs the unconditional path unchanged.
+
+    `action_mask="structure"` / `"valence"` and `max_valence=` (the generators' arguments, `generation.ActionMask`):
+    p(molecule) under the masked generator.  Every logits row of a route batch goes through `gib_action_mask_logits`
+    before the softmax (slot 0 too: a route batch has no dummy slot; each state's atom count is its number of
+    non-empty node rows), with the attachment points in the same launch; the backward masks the
+    recomputed logits the same way.  Per chunk the plan is checked by `gib_route_check_actions`, and a molecule whose
+    route takes a forbidden action -- with "valence", any molecule with an atom over its limit -- is refused by name
+    before its chunk is scored."""
 
     def __init__(self, model, batch_size, constants=None, n_atom_types=None, n_formal_charge=None, n_imp_H=None,
-                 n_chirality=None, chunk_molecules=4096, device=None, scaffolds=None, attachment=None):
+                 n_chirality=None, chunk_molecules=4096, device=None, scaffolds=None, attachment=None,
+                 action_mask=None, max_valence=None):
         from .generation import action_layout
-        from ._lib import PP_STATUS_INTS, PPDims
+        from ._lib import PPDims
         C, A, CH, H, X = action_layout(model, constants, n_atom_types, n_formal_charge, n_imp_H, n_chirality)
         self.layout = (A, CH, H, X)
         if not hasattr(model, "dims"):
@@ -1302,6 +1342,8 @@ class RouteScorer:
         self.N, self.F, self.Ef = N, F_, Ef = C.max_n_nodes, C.n_node_features, C.n_edge_features
         self.apd = N * (C.len_f_add_per_node + C.len_f_conn_per_node) + 1
         self.chunk = chunk = max(1, int(chunk_molecules))
+        from .generation import make_action_mask
+        self.action_mask = make_action_mask(action_mask, max_valence, C, self.layout, N, F_, Ef, self.apd, dev)
         self.pp = PPDims(N=N, F=F_, Ef=Ef, n_atom_types=A, n_formal_charge=CH, n_imp_H=H, n_chirality=X, batch_size=B)
         pd = ctypes.byref(self.pp)
         ws_bytes, max_states = lib.gib_route_plan_ws_bytes(pd, chunk), lib.gib_route_max_states(pd, chunk)
@@ -1312,8 +1354,9 @@ class RouteScorer:
         self.in_edges = torch.zeros(chunk, N, N, Ef, dtype=i8, device=dev)
         self.plan_ws = torch.empty(ws_bytes, dtype=_u8, device=dev)
         self.offsets = torch.zeros(chunk + 1, dtype=i32, device=dev)
-        # [5] the chunk's state count, [6] the captured graph's batch index (gib_route_plan zeroes it)
-        self.status = torch.zeros(PP_STATUS_INTS, dtype=i32, device=dev)
+        # [5] the chunk's state count, [6] the captured graph's batch index (gib_route_plan zeroes it); with the
+        # action mask [PP_STATUS_INTS:] the result of gib_route_check_actions, read back with the rest
+        self.status = torch.zeros(PP_STATUS_INTS + 2, dtype=i32, device=dev)
         self.slots = torch.zeros(2 * B, dtype=i32, device=dev)
         self.ctl = torch.zeros(2, dtype=i32, device=dev)
         self.lik = torch.zeros(max_states, dtype=torch.float32, device=dev)
@@ -1331,6 +1374,8 @@ class RouteScorer:
         self._bwd = None
         self.backward_replays = 0
         self.scaffolds, self.scaffold_version, self._sgraph = None, 0, None
+        # the masked copy of the logits the backward reads (attachment points or the action mask)
+        self.masked_logits = torch.empty(B, self.apd, dtype=torch.float32, device=dev)
         if scaffolds is not None or attachment is not None:
             self.set_scaffolds(scaffolds, attachment)
 
@@ -1355,7 +1400,6 @@ class RouteScorer:
             self.in_ids = torch.zeros(self.chunk, dtype=i32, device=self.dev)
             self.slot_ids = torch.full((self.B,), -1, dtype=i32, device=self.dev)
             self.slot_n = torch.full((self.B,), -1, dtype=i32, device=self.dev)
-            self.masked_logits = torch.empty(self.B, self.apd, dtype=torch.float32, device=self.dev)
 
     @property
     def masked(self):
@@ -1418,8 +1462,16 @@ class RouteScorer:
                                           F._ptr(self.slot_ids), F._ptr(self.slot_n), F._ptr(self.nodes),
                                           F._ptr(self.edges), st), "gib_route_fill_scaffold")
 
-    def _mask(self, logits, st):
-        """the attachment-point mask on every slot of a conditional batch, in place"""
+    def _mask(self, logits, st, scaffold=True):
+        """the action mask (with the attachment points of a conditional batch, in the same launch) or the
+        attachment-point mask alone on every slot of the batch, in place"""
+        if self.action_mask is not None:
+            masked = scaffold and self.masked
+            self._sc = self.scaffolds.struct() if masked else None
+            # the atom counts are the states' non-empty node rows: slot_n is -1 for molecules scored whole
+            self.action_mask.apply(self.B, logits, None, st, self.nodes, self.edges,
+                                   int8=True, sc=self._sc, slot_ids=self.slot_ids if masked else None, first_slot=0)
+            return
         self._sc = self.scaffolds.struct()
         check(lib.gib_route_mask_logits(self.B, self.N, self.Ef, self.apd, ctypes.byref(self._sc),
                                         F._ptr(self.slot_ids), F._ptr(self.slot_n), F._ptr(logits), st),
@@ -1430,8 +1482,8 @@ class RouteScorer:
         self._fill(st, scaffold)
         _k0_forward(self, self.nodes, self.edges, [(self.packed, self.logits)], st)
         self._flags.bitwise_or_(self._hdr_flags)
-        if scaffold and self.masked:
-            self._mask(self.logits, st)
+        if self.action_mask is not None or (scaffold and self.masked):
+            self._mask(self.logits, st, scaffold)
         check(lib.gib_route_probs(self.B, self.apd, F._ptr(self.logits), F._ptr(self.slots), F._ptr(self.lik), st),
               "gib_route_probs")
         check(lib.gib_rl_next_round(F._ptr(self.status[6:7]), st), "gib_rl_next_round")
@@ -1454,10 +1506,10 @@ class RouteScorer:
         _k0_forward(self, self.nodes, self.edges, [(self.packed, self.logits)], st)
         self._flags.bitwise_or_(self._hdr_flags)
         sampled = self.logits
-        if scaffold and self.masked:
+        if self.action_mask is not None or (scaffold and self.masked):
             sampled = self.masked_logits
             sampled.copy_(self.logits)
-            self._mask(sampled, st)
+            self._mask(sampled, st, scaffold)
         check(lib.gib_route_dlogits(self.B, self.apd, F._ptr(sampled), F._ptr(self.slots), F._ptr(b.coef),
                                     F._ptr(b.dlogits), F._ptr(self.lik), st), "gib_route_dlogits")
         check(lib.gib_model_backward(ctypes.byref(self.d), self.hdr, F._ptr(self.nodes), F._ptr(self.edges),
@@ -1569,12 +1621,19 @@ class RouteScorer:
             check(lib.gib_route_plan(pd, F._ptr(self.in_nodes), F._ptr(self.in_edges), n, self.chunk,
                                      F._ptr(self.plan_ws), F._ptr(self.offsets), F._ptr(self.status), st),
                   "gib_route_plan")
-            return
-        self.in_ids[:n].copy_(ids)
-        self._sc = self.scaffolds.struct()
-        check(lib.gib_route_plan_scaffold(pd, F._ptr(self.in_nodes), F._ptr(self.in_edges), n, self.chunk,
-                                          ctypes.byref(self._sc), F._ptr(self.in_ids), F._ptr(self.plan_ws),
-                                          F._ptr(self.offsets), F._ptr(self.status), st), "gib_route_plan_scaffold")
+        else:
+            self.in_ids[:n].copy_(ids)
+            self._sc = self.scaffolds.struct()
+            check(lib.gib_route_plan_scaffold(pd, F._ptr(self.in_nodes), F._ptr(self.in_edges), n, self.chunk,
+                                              ctypes.byref(self._sc), F._ptr(self.in_ids), F._ptr(self.plan_ws),
+                                              F._ptr(self.offsets), F._ptr(self.status), st),
+                  "gib_route_plan_scaffold")
+        if self.action_mask is not None:
+            m = self.action_mask
+            check(lib.gib_route_check_actions(pd, F._ptr(self.in_nodes), F._ptr(self.in_edges), n, self.chunk,
+                                              F._ptr(self.plan_ws), F._ptr(self.offsets), m.code,
+                                              F._ptr(m.table) if m.table is not None else None,
+                                              F._ptr(self.status[PP_STATUS_INTS:]), st), "gib_route_check_actions")
 
     def _score(self, nodes, edges, rec=None, ids=None):
         """the forward of score(); `rec`: the backward record whose chunk list (first molecule, first state,
@@ -1605,6 +1664,10 @@ class RouteScorer:
             refuse_bad(status, pos, stop)
             if scaffold:
                 self._refuse_scaffold(status, ids, pos, stop)
+            if self.action_mask is not None and status[PP_STATUS_INTS]:
+                m = pos + int(status[PP_STATUS_INTS + 1])
+                raise ValueError(f"molecule {m} (or a later one in molecules [{pos}, {stop})): "
+                                 + dict(_ROUTE_REASONS)[ROUTE_ACTION])
             S = int(status[5])
             self._flags.zero_()
             for _ in range(-(-S // self.B)):

@@ -541,9 +541,30 @@ int gib_generation_mask_logits(int B, int N, int Ef, int apd, const gib_scaffold
                                const int* n_nodes, const int* row, const int* state, const int* counters,
                                float* logits, gib_stream stream);
 /* row state[0] of rec_ids / rec_n [2N, B] = slot_ids / n_nodes [B] when the round runs (gib_rl_snapshot's rule): the
- * per-round mask inputs the RL backward replays */
+ * per-round mask inputs the RL backward replays.  slot_ids = rec_ids = null: the atom counts only (the action mask
+ * without scaffolds). */
 int gib_rl_snapshot_scaffold(int B, int N, const int* slot_ids, const int* n_nodes, const int* state,
                              const int* counters, int* rec_ids, int* rec_n, gib_stream stream);
+
+/* ---- the action mask: sample only actions the state machine accepts (graphinvent_b200/csrc/action_mask.cuh) ----
+ * -inf in place into every entry of logits [B, apd] that the rule forbids in slot b's state, terminate never:
+ *   GIB_ACTION_MASK_STRUCTURE  exactly the actions the round's decode flags invalid (a bond to an atom that does not
+ *                              exist, a self loop, a bond that exists, an add into a full graph, ...);
+ *   GIB_ACTION_MASK_VALENCE    those, and every bond that takes an atom past its valence limit, from the device table
+ *                              int32 [A * CH + Ef + H] = V[atom type][charge] | bond orders in half-bond units (single
+ *                              2, double 4, triple 6, aromatic 3) | implicit-H count of each index.
+ * The state is nodes [B, N, F] / edges [B, N, N, Ef], either float (give nodes / edges, null the int8 pair) or int8
+ * (the other way round), with atom counts n_nodes [B], or n_nodes = null: each slot's count is its number of
+ * non-empty node rows (route batches, whose rows past the count are zero).  row != null: n_nodes and slot_ids are tables [*, B] read at
+ * row row[0] (the RL backward's record); state / counters: the round gate of gib_generation_mask_logits.  sc with
+ * protect != null: the attachment-point rule of slot b's scaffold slot_ids[b] is applied in the same launch (forbidden
+ * = either rule).  Slots below first_slot (0 or 1; 1 skips the generator's dummy slot 0) are left alone.  N <= 127. */
+enum { GIB_ACTION_MASK_STRUCTURE = 1, GIB_ACTION_MASK_VALENCE = 2 };
+int gib_action_mask_logits(int B, int N, int F, int Ef, int n_atom_types, int n_charges, int n_imp_H, int n_chirality,
+                           int apd, int mode, const int* table, const float* nodes, const float* edges,
+                           const signed char* nodes_i8, const signed char* edges_i8, const int* n_nodes,
+                           const gib_scaffolds* sc, const int* slot_ids, const int* row, const int* state,
+                           const int* counters, float* logits, int first_slot, gib_stream stream);
 
 /* ---- the RL rollout (GraphGeneratorRL.py:109-172) as captured rounds, and its backward by recomputation
  *      (graphinvent_b200.graphed.GraphedGeneratorRL).  Tables indexed [round, slot] have 2N rows of B. ----
@@ -779,7 +800,7 @@ int gib_test_route_plan_offsets(const gib_pp_dims* d, int max_molecules, long lo
  * whole and past the last state).
  * gib_route_mask_logits: gib_generation_mask_logits' rule on every slot of a route batch, slot 0 included (a route
  * batch has no dummy slot); slots with slot_ids[b] < 0 are left alone; a table without protect masks nothing. */
-enum { GIB_ROUTE_NOT_PREFIX = 1, GIB_ROUTE_MASKED = 2, GIB_ROUTE_BAD_ID = 4 };
+enum { GIB_ROUTE_NOT_PREFIX = 1, GIB_ROUTE_MASKED = 2, GIB_ROUTE_BAD_ID = 4, GIB_ROUTE_ACTION = 8 };
 int gib_route_plan_scaffold(const gib_pp_dims* d, const signed char* nodes, const signed char* edges, int n_molecules,
                             int max_molecules, const gib_scaffolds* sc, const int* scaffold_ids, void* ws,
                             int* offsets, int* status, gib_stream stream);
@@ -789,6 +810,15 @@ int gib_route_fill_scaffold(const gib_pp_dims* d, const signed char* nodes, cons
                             signed char* out_nodes, signed char* out_edges, gib_stream stream);
 int gib_route_mask_logits(int B, int N, int Ef, int apd, const gib_scaffolds* sc, const int* slot_ids,
                           const int* n_nodes, float* logits, gib_stream stream);
+/* gib_route_check_actions: the action mask's rule (gib_action_mask_logits, mode GIB_ACTION_MASK_*) on a plan of
+ * gib_route_plan / gib_route_plan_scaffold over the same n_molecules molecules: every kept state's action against the
+ * structural rule, and with GIB_ACTION_MASK_VALENCE (table as for gib_action_mask_logits) every atom of each molecule
+ * within its limit -- valences only grow along a route, so its states all are exactly when the molecule is.  result
+ * int32 [2] (written here): [0] GIB_ROUTE_ACTION when some molecule's route takes a forbidden action (probability 0
+ * under the mask), [1] the first such molecule (0x7f7f7f7f: none).  N <= 127. */
+int gib_route_check_actions(const gib_pp_dims* d, const signed char* nodes, const signed char* edges, int n_molecules,
+                            int max_molecules, const void* ws, const int* offsets, int mode, const int* table,
+                            int* result, gib_stream stream);
 
 /* ---- measurement hooks: CUDA-event timing per kernel class on the launching stream.
  *      class 0 = forward/dX launches of the tensor-core kernel, 1 = its weight-gradient launches, 2 = scatter-aggregate (K2),
