@@ -72,7 +72,7 @@ class Scaffolds(ctypes.Structure):
 
 
 PP_STATUS_INTS = 8                                                  # GIB_PP_* (include/gib200.h)
-PP_BAD_NODES, PP_BAD_EDGES, PP_EMPTY, PP_DISCONNECTED, PP_BAD_RANKING = 1, 2, 4, 8, 16
+PP_BAD_NODES, PP_BAD_EDGES, PP_EMPTY, PP_DISCONNECTED, PP_BAD_RANKING, PP_MATCH_BUDGET = 1, 2, 4, 8, 16, 32
 ROUTE_BFS, ROUTE_DFS = 0, 1                                         # GIB_ROUTE_BFS / GIB_ROUTE_DFS (gib_reorder)
 ROUTE_NOT_PREFIX, ROUTE_MASKED, ROUTE_BAD_ID, ROUTE_ACTION = 1, 2, 4, 8               # GIB_ROUTE_* (status[1] of the conditional plan)
 
@@ -169,6 +169,9 @@ _PROTOS = {
     "gib_reorder_ws_bytes": (c_sz, [c_i]),
     "gib_reorder": (c_i, [c_p, c_p, c_p, c_i, c_i, c_i, ctypes.c_ulonglong, c_ll, c_ll] + [c_p] * 7),
     "gib_draw_rankings": (c_i, [c_i, c_i, c_p, ctypes.c_ulonglong, c_ll, c_ll, c_p, c_p]),
+    "gib_scaffold_first_ws_bytes": (c_sz, [c_p, c_i, c_i]),
+    "gib_scaffold_first": (c_i, [c_p, c_p, c_p, c_i, c_p, c_p, c_i, ctypes.c_ulonglong, c_ll, c_ll, c_p, c_ll]
+                           + [c_p] * 7),
     "gib_route_plan_ws_bytes": (c_sz, [c_p, c_i]),
     "gib_route_max_states": (c_ll, [c_p, c_i]),
     "gib_route_plan": (c_i, [c_p, c_p, c_p, c_i, c_i] + [c_p] * 4),

@@ -175,6 +175,35 @@ __device__ __forceinline__ void flag_scaffold(int* status, int flags, int m) {
   atomicMin(&status[2], m);
 }
 
+// The comparison that defines "molecule atoms phi(0..k-1) are scaffold s": node row phi(i) equals scaffold row i in
+// all F bytes and, for every i, j < k, edge cell (phi(i), phi(j)) equals scaffold cell (i, j) in all Ef bytes (an
+// induced match: an extra bond among the image differs).  phi = null is the identity, the prefix rule of the
+// conditional route plan; scaffold_first_kernel confirms every embedding its search finds with it.  One warp, every
+// lane gets the answer; *nnz (per lane, summed by the caller) counts the scaffold's non-zero edge bytes.
+__device__ bool scaffold_differs(const PP& p, const signed char* X, const signed char* E, const signed char* SX,
+                                 const signed char* SE, int k, const short* phi, int* nnz) {
+  const int lane = threadIdx.x & 31;
+  const int N = p.N, F = p.F, Ef = p.Ef;
+  bool diff = false;
+  int z = 0;
+  // a molecule of fewer atoms has a zero row there, the scaffold does not
+  for (int q = lane; q < k * F; q += 32) {
+    const int i = q / F, a = phi ? phi[i] : i;
+    diff |= X[(size_t)a * F + q % F] != SX[q];
+  }
+  for (int q = lane; q < k * k; q += 32) {
+    const int i = q / k, j = q % k;
+    const size_t ij = (size_t)i * N + j, ab = (size_t)(phi ? phi[i] : i) * N + (phi ? phi[j] : j);
+    for (int t = 0; t < Ef; ++t) {
+      const signed char w = SE[ij * Ef + t];
+      diff |= E[ab * Ef + t] != w;
+      z += w != 0;
+    }
+  }
+  *nnz = z;
+  return __any_sync(0xffffffffu, diff);
+}
+
 // the conditional route of molecule m decorating scaffold ids[m] (>= 0): its first k_s node rows and the edges among
 // them must equal the scaffold's (one warp, every lane gets the answer).  Returns the states kept, n_edges - m_k + 1
 // (m_k: the scaffold's bonds), or 0 with a GIB_ROUTE_* flag raised.  ids[m] = -1: the whole route, n_edges + 2.
@@ -188,21 +217,9 @@ __device__ int conditional_length(const PP& p, const gib_scaffolds& sc, int sid,
   }
   if (sid < 0) return e + 2;
   const int k = sc.n_atoms[sid];
-  const signed char* SX = sc.nodes + (size_t)sid * N * F;
-  const signed char* SE = sc.edges + (size_t)sid * N * N * Ef;
-  bool diff = false;
-  int nnz = 0;
-  // rows 0..k-1 (a molecule of fewer atoms has a zero row there, the scaffold does not)
-  for (int q = lane; q < k * F; q += 32) diff |= X[q] != SX[q];
-  for (int q = lane; q < k * k; q += 32) {
-    const size_t ij = (size_t)(q / k) * N + q % k;
-    for (int t = 0; t < Ef; ++t) {
-      const signed char w = SE[ij * Ef + t];
-      diff |= E[ij * Ef + t] != w;
-      nnz += w != 0;
-    }
-  }
-  if (__any_sync(0xffffffffu, diff)) {
+  int nnz;
+  if (scaffold_differs(p, X, E, sc.nodes + (size_t)sid * N * F, sc.edges + (size_t)sid * N * N * Ef, k, nullptr,
+                       &nnz)) {
     if (lane == 0) flag_scaffold(status, GIB_ROUTE_NOT_PREFIX, m);
     return 0;
   }
@@ -210,10 +227,12 @@ __device__ int conditional_length(const PP& p, const gib_scaffolds& sc, int sid,
 }
 
 // ---- count: validation and route length (one warp per molecule) ------------------------------------------------
-// ids != null (the conditional route plan): the length is that of molecule m's conditional route
+// ids != null (the conditional route plan): the length is that of molecule m's conditional route.  bad_out != null:
+// each molecule's GIB_PP_* input flags (0: it passed), for a later kernel that must leave refused molecules alone
 __global__ void __launch_bounds__(32) pp_count_kernel(PP p, const signed char* __restrict__ nodes,
                                                       const signed char* __restrict__ edges, int* len, int* n0,
-                                                      int* status, const int* __restrict__ ids, gib_scaffolds sc) {
+                                                      int* status, const int* __restrict__ ids, gib_scaffolds sc,
+                                                      int* bad_out = nullptr) {
   const int m = blockIdx.x, lane = threadIdx.x;
   const int N = p.N, F = p.F, Ef = p.Ef;
   const signed char* X = nodes + (size_t)m * N * F;
@@ -266,6 +285,7 @@ __global__ void __launch_bounds__(32) pp_count_kernel(PP p, const signed char* _
     if (bad) flag_bad(status, bad, m);
     len[m] = bad ? 2 : kept;
     n0[m] = n;
+    if (bad_out) bad_out[m] = bad;
   }
 }
 
@@ -949,6 +969,46 @@ __global__ void __launch_bounds__(32) rank_draw_kernel(int N, const int* __restr
   for (int i = lane; i < N; i += 32) rankings[(size_t)m * N + i] = i < n ? rank[i] : -1;
 }
 
+// molecule m's ranking into rank[0, n) (one warp): drawn from (seed, epoch, first + m) and written to R (-1 past n),
+// or read from R.  seen [kReorderWords] must be zero on entry.  False, with GIB_PP_BAD_RANKING raised, when it is not
+// a permutation of 0..n-1.
+__device__ bool load_ranking(int N, int n, int draw, unsigned long long seed, long long epoch, long long first, int m,
+                             int* R, int* rank, unsigned long long* key, unsigned* seen, int* status) {
+  const int lane = threadIdx.x & 31;
+  if (draw) {
+    draw_ranking(seed, epoch, first + m, n, rank, key);
+    for (int i = lane; i < N; i += 32) R[i] = i < n ? rank[i] : -1;
+  } else {
+    for (int i = lane; i < n; i += 32) rank[i] = R[i];
+  }
+  __syncwarp();
+  bool bad_rank = false;
+  for (int i = lane; i < n; i += 32) {
+    const int r = rank[i];
+    if (r < 0 || r >= n || (atomicOr(&seen[r >> 5], 1u << (r & 31)) >> (r & 31) & 1u)) bad_rank = true;
+  }
+  bad_rank = __any_sync(0xffffffffu, bad_rank);
+  if (bad_rank && lane == 0) flag_bad(status, GIB_PP_BAD_RANKING, m);
+  return !bad_rank;
+}
+
+// reorder_nodes (one warp): the atom at new position k is old atom ord[k] for k < nk; order row O = ord, -1 past nk,
+// node rows / edge rows and columns of the molecule (X, E) into OX / OE, zero past nk
+__device__ void write_reordered(const PP& p, const signed char* X, const signed char* E, const int* ord, int nk,
+                                int* O, signed char* OX, signed char* OE) {
+  const int lane = threadIdx.x & 31;
+  const int N = p.N, F = p.F, Ef = p.Ef;
+  for (int i = lane; i < N; i += 32) O[i] = i < nk ? ord[i] : -1;
+  for (int q = lane; q < N * F; q += 32) {
+    const int k = q / F;
+    OX[q] = k < nk ? X[(size_t)ord[k] * F + q % F] : 0;
+  }
+  for (int q = lane; q < N * N * Ef; q += 32) {
+    const int k = q / (N * Ef), l = q / Ef % N, t = q % Ef;
+    OE[q] = k < nk && l < nk ? E[((size_t)ord[k] * N + ord[l]) * Ef + t] : 0;
+  }
+}
+
 // route: 0 = BFS, 1 = DFS.  draw != 0: the ranking is drawn (draw_ranking) and written to `rankings`, else read from it
 __global__ void __launch_bounds__(32) reorder_kernel(PP p, const signed char* __restrict__ nodes,
                                                      const signed char* __restrict__ edges, const int* __restrict__ n0,
@@ -977,25 +1037,7 @@ __global__ void __launch_bounds__(32) reorder_kernel(PP p, const signed char* __
     for (int t = 0; t < Ef; ++t) any |= E[((size_t)i * N + j) * Ef + t] != 0;
     if (any) atomicOr(&adj[i][j >> 5], 1u << (j & 31));
   }
-  // the ranking: a permutation of 0..n-1 over the molecule's atoms
-  if (draw) {
-    draw_ranking(seed, epoch, first + m, n, rank, key);
-    for (int i = lane; i < N; i += 32) R[i] = i < n ? rank[i] : -1;
-  } else {
-    for (int i = lane; i < n; i += 32) rank[i] = R[i];
-  }
-  __syncwarp();
-  bool bad_rank = false;
-  for (int i = lane; i < n; i += 32) {
-    const int r = rank[i];
-    if (r < 0 || r >= n || (atomicOr(&seen[r >> 5], 1u << (r & 31)) >> (r & 31) & 1u)) bad_rank = true;
-  }
-  if (__any_sync(0xffffffffu, bad_rank)) {
-    if (lane == 0) {
-      flag_bad(status, GIB_PP_BAD_RANKING, m);
-      ok = 0;
-    }
-  }
+  if (!load_ranking(N, n, draw, seed, epoch, first, m, R, rank, key, seen, status) && lane == 0) ok = 0;
   __syncwarp();
   if (lane == 0 && ok) {
     unsigned* vis = seen;                                   // reused: the visited set
@@ -1066,21 +1108,245 @@ __global__ void __launch_bounds__(32) reorder_kernel(PP p, const signed char* __
     }
   }
   __syncwarp();
-  const bool good = ok;
-  int* O = order + (size_t)m * N;
-  for (int i = lane; i < N; i += 32) O[i] = good && i < n ? ord[i] : -1;
-  // reorder_nodes; a refused molecule's outputs are zero
-  signed char* OX = out_nodes + (size_t)m * N * F;
-  signed char* OE = out_edges + (size_t)m * N * N * Ef;
-  const int nk = good ? n : 0;
-  for (int q = lane; q < N * F; q += 32) {
-    const int k = q / F;
-    OX[q] = k < nk ? X[(size_t)ord[k] * F + q % F] : 0;
+  // a refused molecule's outputs are zero
+  write_reordered(p, X, E, ord, ok ? n : 0, order + (size_t)m * N, out_nodes + (size_t)m * N * F,
+                  out_edges + (size_t)m * N * N * Ef);
+}
+
+// ---- scaffold-first decoding order (gib_scaffold_first): one warp per molecule -------------------------------------
+// The embedding search is a depth-first search over scaffold atoms 0..k-1 with the candidate sets as bitsets in shared
+// memory: depth i's candidates are label(i) (molecule atoms whose node row is scaffold row i, of a degree that fits)
+// minus the atoms in use, intersected, for every assigned j < i, with the bond-type-t neighbours of phi(j) when
+// scaffold atoms i, j share a type-t bond and with the non-neighbours of phi(j) when they share none.  The lanes
+// compute that over the words, lane 0 moves the search; candidates are taken lowest index first, so the first leaf is
+// the lexicographically smallest embedding.
+constexpr int kMatchAdjWords = 2048;     // Ef * N * ceil(N / 32) words of per-bond-type adjacency
+
+// per scaffold s (one warp each): deg[s, i] = scaffold atom i's bonds (0 past k_s), bonds[s] = its bonds in all
+__global__ void __launch_bounds__(32) scaffold_degree_kernel(PP p, gib_scaffolds sc, short* deg, int* bonds) {
+  const int s = blockIdx.x, lane = threadIdx.x, N = p.N, Ef = p.Ef;
+  const int k = min(max(sc.n_atoms[s], 0), N);
+  const signed char* SE = sc.edges + (size_t)s * N * N * Ef;
+  int total = 0;
+  for (int i = lane; i < N; i += 32) {
+    int d = 0;
+    for (int j = 0; j < k && i < k; ++j) {
+      bool any = false;
+      for (int t = 0; t < Ef; ++t) any |= SE[((size_t)i * N + j) * Ef + t] != 0;
+      d += any;
+    }
+    deg[(size_t)s * N + i] = (short)d;
+    total += d;
   }
-  for (int q = lane; q < N * N * Ef; q += 32) {
-    const int k = q / (N * Ef), l = q / Ef % N, t = q % Ef;
-    OE[q] = k < nk && l < nk ? E[((size_t)ord[k] * N + ord[l]) * Ef + t] : 0;
+  total = warp_sum(total);
+  if (lane == 0) bonds[s] = total / 2;
+}
+
+// lane 0: the layered breadth-first search from ord[0, c) (marked in vis): layer L + 1 is the unvisited neighbours of
+// layer L, appended highest-ranked first (best_of).  Returns the atoms reached.
+__device__ int layered_bfs(const unsigned (*adj)[kReorderWords], int W, const int* rank, unsigned* vis, int* ord,
+                           int c) {
+  unsigned next[kReorderWords];
+  for (int lo = 0, hi = c; lo < hi; lo = hi, hi = c) {
+    for (int w = 0; w < W; ++w) next[w] = 0;
+    for (int k = lo; k < hi; ++k)
+      for (int w = 0; w < W; ++w) next[w] |= adj[ord[k]][w];
+    for (int w = 0; w < W; ++w) {
+      next[w] &= ~vis[w];
+      vis[w] |= next[w];
+    }
+    for (int a = best_of(next, rank, W); a >= 0; a = best_of(next, rank, W)) {
+      ord[c++] = a;
+      next[a >> 5] &= ~(1u << (a & 31));
+    }
   }
+  return c;
+}
+
+struct MatchSmem {
+  unsigned adj[kMatchAdjWords];                       // [Ef][N][W]: bit b of (t, a) = a bond of type t between a, b
+  unsigned any[kReorderMaxN][kReorderWords];          // a bond of any type
+  unsigned label[kReorderMaxN][kReorderWords];        // per scaffold atom: the molecule atoms it may map to
+  unsigned cand[kReorderMaxN][kReorderWords];         // the search stack: depth i's untried candidates
+  unsigned used[kReorderWords];                       // the atoms phi(0..depth-1)
+  short phi[kReorderMaxN], mdeg[kReorderMaxN];
+};
+
+// depth i's candidate set into S.cand[i] (phi(0..i-1) assigned)
+__device__ void match_candidates(const PP& p, MatchSmem& S, const signed char* SE, int i, int W) {
+  const int lane = threadIdx.x & 31, N = p.N, Ef = p.Ef;
+  unsigned acc[kReorderWords];
+#pragma unroll
+  for (int w = 0; w < kReorderWords; ++w) acc[w] = ~0u;
+  for (int j = lane; j < i; j += 32) {
+    int t = -1;
+    for (int u = Ef - 1; u >= 0; --u)
+      if (SE[((size_t)i * N + j) * Ef + u]) t = u;
+    const int a = S.phi[j];
+    const unsigned* nb = t >= 0 ? S.adj + ((size_t)t * N + a) * W : S.any[a];
+#pragma unroll
+    for (int w = 0; w < kReorderWords; ++w)
+      if (w < W) acc[w] &= t >= 0 ? nb[w] : ~nb[w];
+  }
+#pragma unroll
+  for (int w = 0; w < kReorderWords; ++w) acc[w] = __reduce_and_sync(0xffffffffu, acc[w]);
+  if (lane == 0)
+    for (int w = 0; w < W; ++w) S.cand[i][w] = S.label[i][w] & ~S.used[w] & acc[w];
+  __syncwarp();
+}
+
+// the smallest embedding of scaffold s (k atoms) in the molecule (X, E, n atoms) into S.phi: 1 found, 0 none, -1 the
+// search would take more than `budget` assignments.  Every lane gets the answer.
+__device__ int match_scaffold(const PP& p, MatchSmem& S, const signed char* X, const signed char* E, int n,
+                              const gib_scaffolds& sc, const short* sdeg, int s, int k, long long budget) {
+  const int lane = threadIdx.x & 31, N = p.N, F = p.F, W = (N + 31) / 32;
+  const signed char* SX = sc.nodes + (size_t)s * N * F;
+  const signed char* SE = sc.edges + (size_t)s * N * N * p.Ef;
+  const unsigned* pm = sc.protect ? sc.protect + (size_t)s * 4 : nullptr;
+  const short* sd = sdeg + (size_t)s * N;
+  for (int q = lane; q < k * W; q += 32) S.label[q / W][q % W] = 0;
+  if (lane < W) S.used[lane] = 0;
+  __syncwarp();
+  // labels: the node row equals scaffold row i (all F bytes, as scaffold_differs compares it), the degree is at least
+  // scaffold atom i's, and exactly its for a protected atom (no bond may leave the image there)
+  for (int q = lane; q < k * n; q += 32) {
+    const int i = q / n, a = q % n;
+    bool eq = S.mdeg[a] == sd[i] || (S.mdeg[a] > sd[i] && !(pm && scaffold_protected(pm, i)));
+    for (int f = 0; f < F && eq; ++f) eq = X[(size_t)a * F + f] == SX[(size_t)i * F + f];
+    if (eq) atomicOr(&S.label[i][a >> 5], 1u << (a & 31));
+  }
+  __syncwarp();
+  match_candidates(p, S, SE, 0, W);
+  long long nodes = 0;
+  int d = 0;
+  while (true) {
+    int a = -1;
+    for (int w = 0; w < W && a < 0; ++w)
+      if (S.cand[d][w]) a = w * 32 + __ffs(S.cand[d][w]) - 1;
+    __syncwarp();
+    if (a < 0) {                                            // depth d exhausted: back to depth d - 1
+      if (d == 0) return 0;
+      --d;
+      if (lane == 0) S.used[S.phi[d] >> 5] &= ~(1u << (S.phi[d] & 31));
+      __syncwarp();
+      continue;
+    }
+    if (++nodes > budget) return -1;
+    if (lane == 0) {
+      S.cand[d][a >> 5] &= ~(1u << (a & 31));
+      S.phi[d] = (short)a;
+      S.used[a >> 5] |= 1u << (a & 31);
+    }
+    __syncwarp();
+    if (d + 1 < k) {
+      match_candidates(p, S, SE, ++d, W);
+      continue;
+    }
+    int nnz;
+    if (!scaffold_differs(p, X, E, SX, SE, k, S.phi, &nnz)) return 1;
+    if (lane == 0) S.used[a >> 5] &= ~(1u << (a & 31));  // a leaf the byte comparison rejects: the next candidate
+    __syncwarp();
+  }
+}
+
+// ids != null: molecule m tries scaffold ids[m] only (-1, or an id outside [0, S): none); null: scaffolds 0..S-1 in
+// order until one embeds.  draw / rankings as in reorder_kernel.  bad: pp_count_kernel's per-molecule flags.
+__global__ void __launch_bounds__(32) scaffold_first_kernel(
+    PP p, const signed char* __restrict__ nodes, const signed char* __restrict__ edges, const int* __restrict__ n0,
+    const int* __restrict__ bad, gib_scaffolds sc, const short* __restrict__ sdeg, const int* __restrict__ sbonds,
+    const int* __restrict__ ids, int draw, unsigned long long seed, long long epoch, long long first, int* rankings,
+    long long budget, int* order, int* out_ids, signed char* out_nodes, signed char* out_edges, int* status) {
+  __shared__ MatchSmem S;
+  __shared__ int rank[kReorderMaxN], ord[kReorderMaxN];
+  __shared__ unsigned long long key[kReorderMaxN];
+  __shared__ unsigned seen[kReorderWords];
+  __shared__ int ok;
+  const int m = blockIdx.x, lane = threadIdx.x;
+  const int N = p.N, F = p.F, Ef = p.Ef, W = (N + 31) / 32;
+  const int n = n0[m];
+  const signed char* X = nodes + (size_t)m * N * F;
+  const signed char* E = edges + (size_t)m * N * N * Ef;
+  for (int q = lane; q < Ef * N * W; q += 32) S.adj[q] = 0;
+  for (int q = lane; q < N * W; q += 32) S.any[q / W][q % W] = 0;
+  if (lane < W) seen[lane] = 0;
+  if (lane == 0) ok = n > 0 && !bad[m];                     // refused by the input checks: left alone, outputs zero
+  __syncwarp();
+  for (int q = lane; q < n * n; q += 32) {
+    const int i = q / n, j = q % n;
+    bool any = false;
+    for (int t = 0; t < Ef; ++t)
+      if (E[((size_t)i * N + j) * Ef + t]) {
+        atomicOr(&S.adj[((size_t)t * N + i) * W + (j >> 5)], 1u << (j & 31));
+        any = true;
+      }
+    if (any) atomicOr(&S.any[i][j >> 5], 1u << (j & 31));
+  }
+  if (!load_ranking(N, n, draw, seed, epoch, first, m, rankings + (size_t)m * N, rank, key, seen, status) && lane == 0)
+    ok = 0;
+  __syncwarp();
+  int deg_sum = 0;
+  for (int i = lane; i < n; i += 32) {
+    int d = 0;
+    for (int w = 0; w < W; ++w) d += __popc(S.any[i][w]);
+    S.mdeg[i] = (short)d;
+    deg_sum += d;
+  }
+  deg_sum = warp_sum(deg_sum);
+  // connectivity first, as gib_reorder checks it: the layers from atom 0 must reach every atom
+  if (lane == 0 && ok) {
+    for (int w = 0; w < W; ++w) seen[w] = 0;
+    seen[0] = 1u;
+    ord[0] = 0;
+    if (layered_bfs(S.any, W, rank, seen, ord, 1) != n) {
+      flag_bad(status, GIB_PP_DISCONNECTED, m);
+      ok = 0;
+    }
+  }
+  __syncwarp();
+  int sid = -1;
+  if (ok) {
+    int s0 = 0, s1 = sc.S;
+    if (ids) {
+      s0 = ids[m];
+      s1 = s0 >= 0 && s0 < sc.S ? s0 + 1 : s0;
+    }
+    for (int s = s0; s < s1; ++s) {
+      const int k = sc.n_atoms[s];
+      if (k < 1 || k > n || 2 * sbonds[s] > deg_sum) continue;     // cheap rejects before any search
+      const int r = match_scaffold(p, S, X, E, n, sc, sdeg, s, k, budget);
+      if (r < 0) {
+        if (lane == 0) {
+          flag_bad(status, GIB_PP_MATCH_BUDGET, m);
+          ok = 0;
+        }
+        __syncwarp();
+        break;
+      }
+      if (r > 0) {
+        sid = s;
+        break;
+      }
+    }
+  }
+  // the order: phi's image, then its layers; the identity without an embedding
+  if (lane == 0 && ok) {
+    if (sid >= 0) {
+      const int k = sc.n_atoms[sid];
+      for (int w = 0; w < W; ++w) seen[w] = 0;
+      for (int i = 0; i < k; ++i) {
+        ord[i] = S.phi[i];
+        seen[S.phi[i] >> 5] |= 1u << (S.phi[i] & 31);
+      }
+      layered_bfs(S.any, W, rank, seen, ord, k);
+    } else {
+      for (int i = 0; i < n; ++i) ord[i] = i;
+    }
+  }
+  __syncwarp();
+  if (lane == 0) out_ids[m] = ok ? sid : -1;
+  // a refused molecule's outputs are zero
+  write_reordered(p, X, E, ord, ok ? n : 0, order + (size_t)m * N, out_nodes + (size_t)m * N * F,
+                  out_edges + (size_t)m * N * N * Ef);
 }
 
 }  // namespace
@@ -1414,6 +1680,69 @@ int gib_reorder(const gib_pp_dims* d, const signed char* nodes, const signed cha
   GIB_LAUNCH_CHECK();
   reorder_kernel<<<n_molecules, 32, 0, s>>>(p, nodes, edges, n0, route, draw, seed, epoch, first_molecule, rankings,
                                             order, out_nodes, out_edges, status);
+  GIB_LAUNCH_CHECK();
+  return 0;
+}
+
+// workspace: len, n0, bad [n_molecules] (the count stage), scaffold degrees short [S, N], scaffold bonds [S]
+size_t gib_scaffold_first_ws_bytes(const gib_pp_dims* d, int n_molecules, int n_scaffolds) {
+  PP p;
+  if (make_pp("gib_scaffold_first_ws_bytes", d, &p)) return 0;
+  if (n_molecules < 1 || n_scaffolds < 1) {
+    set_error("gib_scaffold_first_ws_bytes: need n_molecules >= 1 and n_scaffolds >= 1, got %d and %d", n_molecules,
+              n_scaffolds);
+    return 0;
+  }
+  return 3 * align256(4ull * n_molecules) + align256(2ull * n_scaffolds * p.N) + align256(4ull * n_scaffolds);
+}
+
+int gib_scaffold_first(const gib_pp_dims* d, const signed char* nodes, const signed char* edges, int n_molecules,
+                       const gib_scaffolds* sc, const int* scaffold_ids, int draw, unsigned long long seed,
+                       long long epoch, long long first_molecule, int* rankings, long long budget, int* order,
+                       int* ids, signed char* out_nodes, signed char* out_edges, void* ws, int* status,
+                       gib_stream stream) {
+  PP p;
+  GIB_TRY(make_pp("gib_scaffold_first", d, &p));
+  const int W = (p.N + 31) / 32;
+  if (p.N > kReorderMaxN || (long long)p.Ef * p.N * W > kMatchAdjWords) {
+    set_error("gib_scaffold_first: need N <= %d and Ef * N * ceil(N / 32) <= %d, got N=%d Ef=%d", kReorderMaxN,
+              kMatchAdjWords, p.N, p.Ef);
+    return -1;
+  }
+  if (n_molecules < 1 || first_molecule < 0 || budget < 1) {
+    set_error("gib_scaffold_first: need n_molecules >= 1, first_molecule >= 0 and budget >= 1 (got %d, %lld, %lld)",
+              n_molecules, first_molecule, budget);
+    return -1;
+  }
+  if (!nodes || !edges || !rankings || !order || !ids || !out_nodes || !out_edges || !ws || !status) {
+    set_error("gib_scaffold_first: null argument");
+    return -1;
+  }
+  if (!sc || sc->S <= 0 || !sc->nodes || !sc->edges || !sc->n_atoms) {
+    set_error("gib_scaffold_first: the scaffold table needs S >= 1 and its nodes, edges and n_atoms buffers");
+    return -1;
+  }
+  if (sc->protect && p.N > 127) {
+    set_error("gib_scaffold_first: attachment points need N <= 127 (4 protect words per scaffold), got N=%d", p.N);
+    return -1;
+  }
+  cudaStream_t s = (cudaStream_t)stream;
+  char* b = static_cast<char*>(ws);
+  int* len = (int*)b;
+  const size_t per_mol = align256(4ull * n_molecules);
+  int* n0 = (int*)(b + per_mol);
+  int* bad = (int*)(b + 2 * per_mol);
+  short* sdeg = (short*)(b + 3 * per_mol);
+  int* sbonds = (int*)(b + 3 * per_mol + align256(2ull * sc->S * p.N));
+  pp_init_kernel<<<1, 32, 0, s>>>(status, nullptr, nullptr, 0, 0);
+  GIB_LAUNCH_CHECK();
+  pp_count_kernel<<<n_molecules, 32, 0, s>>>(p, nodes, edges, len, n0, status, nullptr, gib_scaffolds{}, bad);
+  GIB_LAUNCH_CHECK();
+  scaffold_degree_kernel<<<sc->S, 32, 0, s>>>(p, *sc, sdeg, sbonds);
+  GIB_LAUNCH_CHECK();
+  scaffold_first_kernel<<<n_molecules, 32, 0, s>>>(p, nodes, edges, n0, bad, *sc, sdeg, sbonds, scaffold_ids, draw,
+                                                   seed, epoch, first_molecule, rankings, budget, order, ids,
+                                                   out_nodes, out_edges, status);
   GIB_LAUNCH_CHECK();
   return 0;
 }

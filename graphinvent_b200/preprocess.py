@@ -18,6 +18,9 @@ returns and merged by the reference's own `combine_ts_properties`.
 (`gib_reorder`): a BFS or DFS from a node ranking -- given, or drawn per (seed, epoch, molecule) -- and the reordered
 stacks.  `file_rows()` runs the construction of `groups()` with the rows left on the device, laid out as the file
 `run_data_processer` writes; `loader.RandomRouteLoader` builds every training pass from fresh routes with the two.
+
+`scaffold_first()` finds each molecule's scaffold (`gib_scaffold_first`) and puts it first in decoding order, the
+order the conditional route scorer and the scaffold decorators need.
 """
 import ctypes
 import sys
@@ -26,8 +29,8 @@ from collections import namedtuple
 import numpy as np
 import torch
 
-from ._lib import (PP_BAD_EDGES, PP_BAD_NODES, PP_BAD_RANKING, PP_DISCONNECTED, PP_EMPTY, PP_STATUS_INTS, ROUTE_BFS,
-                   ROUTE_DFS, PPDims, check, lib)
+from ._lib import (PP_BAD_EDGES, PP_BAD_NODES, PP_BAD_RANKING, PP_DISCONNECTED, PP_EMPTY, PP_MATCH_BUDGET,
+                   PP_STATUS_INTS, ROUTE_BFS, ROUTE_DFS, PPDims, check, lib)
 
 Group = namedtuple("Group", "index init_idx start stop full nodes edges apds resume_idx dataset_size statistics",
                    defaults=(None,))
@@ -316,6 +319,88 @@ def reorder(nodes, edges, route="bfs", rankings=None, seed=0, epoch=0, *, layout
                           ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)), "gib_reorder")
     refuse_bad(status.cpu().numpy(), 0, M, _REORDER_REASONS)
     return out_nodes, out_edges, order
+
+
+_MATCH_REASONS = _REORDER_REASONS + ((PP_MATCH_BUDGET, "the scaffold search ran out of its budget of search-tree nodes "
+                                      "(raise `budget`)"),)
+
+
+def scaffold_first(nodes, edges, scaffolds, attachment=None, scaffold_ids=None, rankings=None, seed=0, epoch=0, *,
+                   layout, first=0, budget=1 << 20, chunk_molecules=65536, device="cuda"):
+    """Scaffold-first decoding order (`gib_scaffold_first`, csrc/preprocess.cu): find each molecule's scaffold and
+    renumber its atoms so that its first k_s atoms, with every bond among them, are byte for byte scaffold s -- the
+    order `RouteScorer.score(..., scaffold_ids=)` and the scaffold decorators need.
+
+    nodes [M, N, F] / edges [M, N, N, Ef]: int8 stacks (numpy or torch, any atom order), validated and refused as
+    `reorder` refuses them.  scaffolds: a `generation.ScaffoldTable` (its attachment points are used), or a pair of
+    int8 stacks (nodes [S, N', F], edges [S, N', N', Ef]) checked once by `ScaffoldTable` with `attachment`.
+    An embedding of scaffold s maps its atom i to a molecule atom phi(i) whose node row equals scaffold row i (all F
+    bytes), with edge cell (phi(i), phi(j)) equal to scaffold cell (i, j) for every pair (an induced match of the same
+    bond types) and, with attachment points, no bond from a protected scaffold atom to an atom outside the image.  The
+    chosen one is the lexicographically smallest (phi(0), ..., phi(k-1)).
+    scaffold_ids: int [M] (-1: do not match), or None: the first scaffold in table order that embeds (order the table
+    by priority, larger scaffolds first for example).
+    The order: phi(0..k-1), then breadth-first layers out of the image, each layer highest-ranked atom first, rankings
+    as `reorder` takes or draws them (seed, epoch, first + m): a fresh epoch redraws the decoration order.
+    Returns device tensors (nodes, edges, order int32 [M, N] (old index per new position, -1 past the atom count),
+    ids int32 [M] (the scaffold used)).  A molecule without an embedding keeps its bytes, the identity order and id -1,
+    so `score(nodes, edges, scaffold_ids=ids)` scores it whole.
+    budget: search-tree nodes per (molecule, scaffold); a search that needs more raises ValueError naming the molecule,
+    as do the refusals of `reorder`.  Molecules go to the device chunk_molecules at a time."""
+    from .generation import ScaffoldTable
+    M, N, F, Ef = _check_stacks(nodes, edges)
+    d = _pp_dims(N, F, Ef, tuple(layout))
+    if isinstance(scaffolds, ScaffoldTable):
+        if attachment is not None:
+            raise ValueError("attachment is given with the ScaffoldTable, not here")
+        table = scaffolds
+        if table.N != N or tuple(table.nodes.shape[1:]) != (N, F) or table.edges.shape[3] != Ef:
+            raise ValueError(f"the scaffold table holds [S, {table.N}, {table.nodes.shape[2]}] graphs, the molecules "
+                             f"[M, {N}, {F}] with Ef = {Ef}")
+    else:
+        table = ScaffoldTable(scaffolds[0], scaffolds[1], attachment, N, F, Ef, tuple(layout), device)
+    if int(budget) < 1:
+        raise ValueError(f"budget must be >= 1, got {budget}")
+    dev = _cuda(torch.device(device))
+    if scaffold_ids is not None:
+        ids_in = torch.as_tensor(np.asarray(torch.as_tensor(scaffold_ids).cpu(), np.int64))
+        if tuple(ids_in.shape) != (M,):
+            raise ValueError(f"scaffold_ids must be [M] = [{M}], got {tuple(ids_in.shape)}")
+        bad = (ids_in < -1) | (ids_in >= table.S)
+        if bool(bad.any()):
+            m = int(torch.nonzero(bad)[0])
+            raise ValueError(f"molecule {m}: scaffold id {int(ids_in[m])} outside [-1, {table.S})")
+        ids_in = ids_in.to(torch.int32).to(dev)
+    if rankings is not None:
+        rk_in = torch.as_tensor(rankings)
+        if tuple(rk_in.shape) != (M, N):
+            raise ValueError(f"rankings must be [M, N] = {(M, N)}, got {tuple(rk_in.shape)}")
+    out_nodes = torch.empty((M, N, F), dtype=torch.int8, device=dev)
+    out_edges = torch.empty((M, N, N, Ef), dtype=torch.int8, device=dev)
+    order = torch.empty((M, N), dtype=torch.int32, device=dev)
+    ids = torch.empty(M, dtype=torch.int32, device=dev)
+    if M == 0:
+        return out_nodes, out_edges, order, ids
+    chunk = min(max(int(chunk_molecules), 1), M)
+    ws = torch.empty(lib.gib_scaffold_first_ws_bytes(ctypes.byref(d), chunk, table.S), dtype=torch.uint8, device=dev)
+    status = torch.empty(PP_STATUS_INTS, dtype=torch.int32, device=dev)
+    rk = torch.empty((chunk, N), dtype=torch.int32, device=dev)
+    sc = table.struct()
+    stream = ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+    for pos in range(0, M, chunk):
+        stop = min(pos + chunk, M)
+        n = stop - pos
+        x, e = _on_device(nodes[pos:stop], dev), _on_device(edges[pos:stop], dev)
+        if rankings is not None:
+            rk[:n].copy_(_on_device(rk_in[pos:stop], dev))
+        check(lib.gib_scaffold_first(ctypes.byref(d), _ptr(x), _ptr(e), n, ctypes.byref(sc),
+                                     _ptr(ids_in[pos:stop]) if scaffold_ids is not None else None,
+                                     int(rankings is None), ctypes.c_ulonglong(seed % 2**64), epoch, first + pos,
+                                     _ptr(rk), int(budget), _ptr(order[pos:stop]), _ptr(ids[pos:stop]),
+                                     _ptr(out_nodes[pos:stop]), _ptr(out_edges[pos:stop]), _ptr(ws), _ptr(status),
+                                     stream), "gib_scaffold_first")
+        refuse_bad(status.cpu().numpy(), pos, stop, _MATCH_REASONS)
+    return out_nodes, out_edges, order, ids
 
 
 def ts_properties(stats, smiles, constants):

@@ -670,7 +670,7 @@ int gib_graph_statistics(int B, int N, int F, int Ef, const float* nodes, const 
  * max_molecules * (N*(N-1)/2 + 2) < 2^30. */
 #define GIB_PP_STATUS_INTS 8
 enum { GIB_PP_BAD_NODES = 1, GIB_PP_BAD_EDGES = 2, GIB_PP_EMPTY = 4, GIB_PP_DISCONNECTED = 8,
-       GIB_PP_BAD_RANKING = 16 /* gib_reorder only */ };
+       GIB_PP_BAD_RANKING = 16 /* gib_reorder, gib_scaffold_first */, GIB_PP_MATCH_BUDGET = 32 /* gib_scaffold_first */ };
 typedef struct gib_pp_dims {
   int N, F, Ef;                                             /* max_n_nodes, n_node_features, n_edge_features */
   int n_atom_types, n_formal_charge, n_imp_H, n_chirality;  /* node-feature segment widths, in order */
@@ -711,7 +711,9 @@ int gib_preprocess_group_statistics(const gib_pp_dims* d, const signed char* nod
  * Output: order int32 [n_molecules, N] (the old index of the atom at each new position, -1 past n), out_nodes /
  * out_edges the reordered int8 stacks (zero past n).  status int32 [GIB_PP_STATUS_INTS]: [3] GIB_PP_* flags -- the
  * input checks of gib_preprocess_chunk, GIB_PP_DISCONNECTED for a disconnected molecule, GIB_PP_BAD_RANKING -- and
- * [4] the first flagged molecule (INT_MAX: none); a flagged molecule's order is -1 and its stacks zero.
+ * [4] the first flagged molecule (INT_MAX: none).  A molecule flagged GIB_PP_EMPTY, GIB_PP_DISCONNECTED or
+ * GIB_PP_BAD_RANKING gets order -1 and zero stacks; the outputs of one that only the input checks refuse
+ * (GIB_PP_BAD_NODES / GIB_PP_BAD_EDGES) are unspecified.
  * ws: gib_reorder_ws_bytes(n_molecules) bytes, may hold anything. */
 enum { GIB_ROUTE_BFS = 0, GIB_ROUTE_DFS = 1 };
 size_t gib_reorder_ws_bytes(int n_molecules);
@@ -722,6 +724,41 @@ int gib_reorder(const gib_pp_dims* d, const signed char* nodes, const signed cha
  * a function of (seed, epoch, first_molecule + m) only; N <= 181 */
 int gib_draw_rankings(int n_molecules, int N, const int* n_atoms, unsigned long long seed, long long epoch,
                       long long first_molecule, int* rankings, gib_stream stream);
+
+/* ---- scaffold-first decoding order (graphinvent_b200.preprocess.scaffold_first): find each molecule's scaffold and
+ *      renumber its atoms so that the scaffold comes first, the order gib_route_plan_scaffold and the scaffold
+ *      decorators need (the molecule's first k_s atoms, with every bond among them, byte for byte scaffold s).
+ * Input as gib_reorder's (any atom order, the same validation and refusals: status[3] / [4]), and the table `sc` (its
+ * nodes, edges, n_atoms and protect, with the molecules' N, F and Ef; the per-batch generator buffers are not read).
+ * Embedding of scaffold s (k atoms) in molecule m (n atoms): an injective phi: {0..k-1} -> {0..n-1} with
+ *   1. node row phi(i) equal to scaffold row i, all F bytes (implicit-H and chirality segments too);
+ *   2. for all i != j < k, edge cell (phi(i), phi(j)) equal to scaffold cell (i, j), all Ef bytes: an induced match of
+ *      the same bond types (an extra bond between two image atoms is no embedding);
+ *   3. with attachment points (protect != null), no bond from a protected scaffold atom to an atom outside the image.
+ * The chosen embedding is the lexicographically smallest (phi(0), ..., phi(k-1)): a depth-first search that assigns
+ * scaffold atom i at depth i, candidates in ascending atom index, pruned by 1-3 against the atoms assigned so far and by
+ * degree (molecule degree >= the scaffold atom's, equal for a protected atom).  Each assignment is one node of the
+ * search tree; a search of (molecule, scaffold) that would take more than `budget` nodes stops and raises
+ * GIB_PP_MATCH_BUDGET for the molecule (never a guess).
+ * Which scaffold: scaffold_ids int32 [n_molecules] (device) given: scaffold_ids[m] only (-1, or an id outside [0, S):
+ * none); null: the first scaffold in table order that embeds, after the cheap rejects k > n and fewer bonds than it.
+ * Order: new positions 0..k-1 are phi(0..k-1); the other atoms follow by layers, layer 0 being phi's image and layer
+ * L + 1 the unvisited neighbours of layer L, each layer highest-ranked atom first.  Rankings as gib_reorder's (read
+ * from `rankings`, or drawn from (seed, epoch, first_molecule + m) and written there when draw != 0).
+ * Output: order int32 [n_molecules, N] (old index per new position, -1 past n), out_nodes / out_edges the reordered
+ * stacks (zero past n), ids int32 [n_molecules] the scaffold used.  A molecule without an embedding keeps its bytes
+ * unchanged, the identity order and id -1; a flagged molecule (any GIB_PP_* flag, the input checks' included: it is
+ * not searched) gets order -1, zero stacks and id -1.
+ * status int32 [GIB_PP_STATUS_INTS]: [3] GIB_PP_* flags (gib_reorder's, and GIB_PP_MATCH_BUDGET), [4] the first flagged
+ * molecule (INT_MAX: none).  Limits: N <= 181 and Ef * N * ceil(N / 32) <= 2048 (Ef <= 4 always fits); N <= 127 with
+ * protect.  ws: gib_scaffold_first_ws_bytes(d, n_molecules, sc->S) bytes, may hold anything.  One warp per molecule;
+ * no allocation and no host read. */
+size_t gib_scaffold_first_ws_bytes(const gib_pp_dims* d, int n_molecules, int n_scaffolds);
+int gib_scaffold_first(const gib_pp_dims* d, const signed char* nodes, const signed char* edges, int n_molecules,
+                       const gib_scaffolds* sc, const int* scaffold_ids, int draw, unsigned long long seed,
+                       long long epoch, long long first_molecule, int* rankings, long long budget, int* order,
+                       int* ids, signed char* out_nodes, signed char* out_edges, void* ws, int* status,
+                       gib_stream stream);
 
 /* ---- the likelihood of a molecule's decoding route (graphinvent_b200.graphed.RouteScorer): for every route state,
  *      p(action | state) = softmax(model(state))[action], one chunk of molecules at a time.
