@@ -75,6 +75,11 @@ struct Dw3Layout {
 
 int gemm_nt(const GemmNT& p, cudaStream_t st);      // dispatches to the tensor-core path when enabled and eligible
 int gemm_nt_simt(const GemmNT& p, cudaStream_t st);
+// n <= 4 independent host-row problems with max(N, n_store) <= 48 in one launch of the narrow fp32 SIMT kernel
+// (bit-identical to gemm_nt_simt)
+int gemm_nt_narrow(const GemmNT* ps, int n, cudaStream_t st);
+// n <= 4 independent problems writing disjoint outputs, bit-identical to gemm_nt on each, in as few launches as that allows
+int gemm_nt_batch(const GemmNT* ps, int n, cudaStream_t st);
 int gemm_nt_tc(const GemmNT& p, cudaStream_t st);
 int gemm_nt_tc_group(const GemmNT* ps, int n, cudaStream_t st);   // n <= 4 independent problems, raw or pre-split W
 int gemm_nt_group(const GemmNT* ps, int n, cudaStream_t st);      // dispatcher: grouped tensor-core launch or per-problem

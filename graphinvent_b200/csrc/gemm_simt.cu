@@ -19,6 +19,51 @@ namespace gib {
 
 constexpr int BK = 16;
 
+// Epilogue of the fp32 SIMT NT kernels: the sums v of row m, columns [n, n + 4) -> C (columns >= n_store untouched).
+// vec_c / vec_x: C / aux rows may be read and written as float4.
+__device__ __forceinline__ void sgemm_nt_epilogue4(const GemmNT& p, int m, int n, const float (&acc)[4], bool vec_c,
+                                                   bool vec_x) {
+  float v[4] = {acc[0], acc[1], acc[2], acc[3]};
+  float x[4] = {0.f, 0.f, 0.f, 0.f};
+  if (p.mode != EPI_ACT) {
+    if (vec_x && n + 3 < p.n_store) {
+      float4 t4 = *reinterpret_cast<const float4*>(p.aux + (size_t)m * p.ldaux + n);
+      x[0] = t4.x; x[1] = t4.y; x[2] = t4.z; x[3] = t4.w;
+    } else {
+#pragma unroll
+      for (int j = 0; j < 4; ++j)
+        if (n + j < p.n_store) x[j] = p.aux[(size_t)m * p.ldaux + n + j];
+    }
+  }
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    if (p.mode == EPI_ACT) {
+      float bj = (p.bias && n + j < p.N) ? p.bias[n + j] : 0.f;
+      v[j] = act_f(v[j] + bj, p.act);
+    } else if (p.mode == EPI_MUL_DACT) {
+      v[j] = v[j] * dact_from_out(x[j], p.act);
+    } else {
+      v[j] = v[j] + x[j];
+    }
+    if (n + j >= p.n_valid) v[j] = 0.f;
+  }
+  float* dst = p.C + (size_t)m * p.ldc + n;
+  if (vec_c && n + 3 < p.n_store) {
+    *reinterpret_cast<float4*>(dst) = make_float4(v[0], v[1], v[2], v[3]);
+  } else {
+#pragma unroll
+    for (int j = 0; j < 4; ++j)
+      if (n + j < p.n_store) dst[j] = v[j];
+  }
+}
+
+__device__ __forceinline__ bool sgemm_vec_c(const GemmNT& p) {
+  return (p.ldc & 3) == 0 && ((reinterpret_cast<uintptr_t>(p.C) & 15) == 0);
+}
+__device__ __forceinline__ bool sgemm_vec_x(const GemmNT& p) {
+  return p.aux && (p.ldaux & 3) == 0 && ((reinterpret_cast<uintptr_t>(p.aux) & 15) == 0);
+}
+
 // ------------------------------------------------------------------------------------
 // C[M,N] = epilogue( A[M,K] * B[N,K]^T )       (both operands K-contiguous)
 // ------------------------------------------------------------------------------------
@@ -118,8 +163,7 @@ __global__ void __launch_bounds__(256, 2) sgemm_nt_kernel(const GemmNT p) {
   }
 
   // ---- epilogue -------------------------------------------------------------------
-  const bool vec_c = (p.ldc & 3) == 0 && ((reinterpret_cast<uintptr_t>(p.C) & 15) == 0);
-  const bool vec_x = p.aux && (p.ldaux & 3) == 0 && ((reinterpret_cast<uintptr_t>(p.aux) & 15) == 0);
+  const bool vec_c = sgemm_vec_c(p), vec_x = sgemm_vec_x(p);
 #pragma unroll
   for (int a = 0; a < RM; ++a)
 #pragma unroll
@@ -130,40 +174,118 @@ __global__ void __launch_bounds__(256, 2) sgemm_nt_kernel(const GemmNT p) {
       for (int b = 0; b < RN; ++b) {
         const int n = n0 + tx * 4 + b * (BN / RN);
         if (n >= p.n_store) continue;
-        float v[4] = {acc[a][i][b][0], acc[a][i][b][1], acc[a][i][b][2], acc[a][i][b][3]};
-        float x[4] = {0.f, 0.f, 0.f, 0.f};
-        if (p.mode != EPI_ACT) {
-          if (vec_x && n + 3 < p.n_store) {
-            float4 t4 = *reinterpret_cast<const float4*>(p.aux + (size_t)m * p.ldaux + n);
-            x[0] = t4.x; x[1] = t4.y; x[2] = t4.z; x[3] = t4.w;
-          } else {
-#pragma unroll
-            for (int j = 0; j < 4; ++j)
-              if (n + j < p.n_store) x[j] = p.aux[(size_t)m * p.ldaux + n + j];
-          }
-        }
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          if (p.mode == EPI_ACT) {
-            float bj = (p.bias && n + j < p.N) ? p.bias[n + j] : 0.f;
-            v[j] = act_f(v[j] + bj, p.act);
-          } else if (p.mode == EPI_MUL_DACT) {
-            v[j] = v[j] * dact_from_out(x[j], p.act);
-          } else {
-            v[j] = v[j] + x[j];
-          }
-          if (n + j >= p.n_valid) v[j] = 0.f;
-        }
-        float* dst = p.C + (size_t)m * p.ldc + n;
-        if (vec_c && n + 3 < p.n_store) {
-          *reinterpret_cast<float4*>(dst) = make_float4(v[0], v[1], v[2], v[3]);
-        } else {
-#pragma unroll
-          for (int j = 0; j < 4; ++j)
-            if (n + j < p.n_store) dst[j] = v[j];
-        }
+        const float v[4] = {acc[a][i][b][0], acc[a][i][b][1], acc[a][i][b][2], acc[a][i][b][3]};
+        sgemm_nt_epilogue4(p, m, n, v, vec_c, vec_x);
       }
     }
+}
+
+// ------------------------------------------------------------------------------------
+// Narrow outputs (max(N, n_store) <= 48: the APD heads' output layers), up to kNarrowMax independent problems per
+// launch.  One column tile per problem, 16, 32 or 48 wide; 192 threads, each owning TM rows x 4 columns, so a CTA covers
+// (192 / (bn / 4)) * TM rows.  Every output is the same fmaf chain over k = 0 .. K-1 as in sgemm_nt_kernel and goes
+// through the same epilogue: the results are bit-identical to it.
+// ------------------------------------------------------------------------------------
+constexpr int kNarrowThreads = 192;
+constexpr int kNarrowMaxN = 48;
+constexpr int kNarrowMax = 4;
+struct NarrowGroup {
+  GemmNT p[kNarrowMax];
+  int bn[kNarrowMax];          // column tile of each problem
+  int cta0[kNarrowMax + 1];    // first CTA of each problem
+  int n;
+};
+
+template <int TM>
+__global__ void __launch_bounds__(kNarrowThreads) sgemm_nt_narrow_kernel(const __grid_constant__ NarrowGroup g) {
+  __shared__ __align__(16) float As[2][BK][kNarrowThreads / 4 * TM + 4];   // rows of a 16-wide tile, the tallest
+  __shared__ __align__(16) float Bs[2][BK][kNarrowMaxN + 4];
+  int pi = 0;
+  while (pi + 1 < g.n && (int)blockIdx.x >= g.cta0[pi + 1]) ++pi;
+  const GemmNT& p = g.p[pi];
+  const int bn = g.bn[pi], nt = bn / 4;
+  const int tid = threadIdx.x;
+  const int cg = tid % nt, rg = tid / nt;
+  const int bm = (kNarrowThreads / nt) * TM;
+  const int m0 = ((int)blockIdx.x - g.cta0[pi]) * bm;
+
+  float4 ra[TM], rb;
+  const float* a_ptr[TM];
+  bool a_ok[TM];
+#pragma unroll
+  for (int i = 0; i < TM; ++i) {
+    const int q = tid + i * kNarrowThreads, row = q >> 2;
+    a_ok[i] = q < bm * 4 && (m0 + row) < p.M;
+    a_ptr[i] = p.A + (size_t)(m0 + row) * p.lda + (q & 3) * 4;
+  }
+  const bool b_ok = tid < bn * 4 && (tid >> 2) < p.N;
+  const float* b_ptr = p.B + (size_t)(tid >> 2) * p.ldb + (tid & 3) * 4;
+  auto gload = [&](int k0) {
+#pragma unroll
+    for (int i = 0; i < TM; ++i)
+      ra[i] = a_ok[i] ? __ldg(reinterpret_cast<const float4*>(a_ptr[i] + k0)) : make_float4(0, 0, 0, 0);
+    rb = b_ok ? __ldg(reinterpret_cast<const float4*>(b_ptr + k0)) : make_float4(0, 0, 0, 0);
+  };
+  auto sstore = [&](int buf) {
+#pragma unroll
+    for (int i = 0; i < TM; ++i) {
+      const int q = tid + i * kNarrowThreads, row = q >> 2, kq = (q & 3) * 4;
+      if (q < bm * 4) {
+        As[buf][kq + 0][row] = ra[i].x; As[buf][kq + 1][row] = ra[i].y;
+        As[buf][kq + 2][row] = ra[i].z; As[buf][kq + 3][row] = ra[i].w;
+      }
+    }
+    if (tid < bn * 4) {
+      const int row = tid >> 2, kq = (tid & 3) * 4;
+      Bs[buf][kq + 0][row] = rb.x; Bs[buf][kq + 1][row] = rb.y;
+      Bs[buf][kq + 2][row] = rb.z; Bs[buf][kq + 3][row] = rb.w;
+    }
+  };
+
+  float acc[TM][4];
+#pragma unroll
+  for (int i = 0; i < TM; ++i)
+#pragma unroll
+    for (int j = 0; j < 4; ++j) acc[i][j] = 0.f;
+
+  const int ntiles = p.K / BK;
+  gload(0);
+  sstore(0);
+  __syncthreads();
+  for (int t = 0; t < ntiles; ++t) {
+    const int buf = t & 1;
+    if (t + 1 < ntiles) gload((t + 1) * BK);
+#pragma unroll
+    for (int kk = 0; kk < BK; ++kk) {
+      float av[TM];
+      if constexpr (TM == 4) {
+        const float4 f = *reinterpret_cast<const float4*>(&As[buf][kk][rg * 4]);
+        av[0] = f.x; av[1] = f.y; av[2] = f.z; av[3] = f.w;
+      } else if constexpr (TM == 2) {
+        const float2 f = *reinterpret_cast<const float2*>(&As[buf][kk][rg * 2]);
+        av[0] = f.x; av[1] = f.y;
+      } else {
+        av[0] = As[buf][kk][rg];
+      }
+      const float4 fb = *reinterpret_cast<const float4*>(&Bs[buf][kk][cg * 4]);
+      const float bv[4] = {fb.x, fb.y, fb.z, fb.w};
+#pragma unroll
+      for (int i = 0; i < TM; ++i)
+#pragma unroll
+        for (int j = 0; j < 4; ++j) acc[i][j] = fmaf(av[i], bv[j], acc[i][j]);
+    }
+    if (t + 1 < ntiles) sstore(buf ^ 1);
+    __syncthreads();
+  }
+
+  const bool vec_c = sgemm_vec_c(p), vec_x = sgemm_vec_x(p);
+  const int n = cg * 4;
+  if (n >= p.n_store) return;
+#pragma unroll
+  for (int i = 0; i < TM; ++i) {
+    const int m = m0 + rg * TM + i;
+    if (m < p.M) sgemm_nt_epilogue4(p, m, n, acc[i], vec_c, vec_x);
+  }
 }
 
 // gib_tc_debug bit 0: the per-problem call pattern (no grouped / chained launches, W split in the kernel)
@@ -180,32 +302,70 @@ int check_precision(int prec, const char* who) {
   return 0;
 }
 
-int gemm_nt(const GemmNT& p, cudaStream_t st) {
-  GIB_TRY(check_precision(p.tf32, "gemm_nt"));
-  // tensor-core path for all but the tiny / skinny GEMMs (those stay on the SIMT kernel); a problem whose row count
-  // lives on the device (capacity mode) needs the grouped call pattern
-  if (p.m_dev) {
-    if (!g_use_tc || !use_tc3() || !tc3_eligible(p)) {
-      set_error("gemm_nt: device-side row counts need the tensor-core path (tensor cores on, pre-split weights)");
-      return -2;
-    }
-    return gemm_nt_tc3_group(&p, 1, st);
-  }
+// gib_tc_debug bit 4: the dispatch before the narrow kernel -- narrow problems on sgemm_nt_kernel, mixed groups and the
+// first-layer input gradients of sibling MLPs problem by problem (A/B comparisons, and the reference of the tests)
+static inline bool narrow_dispatch() { return (g_tc_debug & 16) == 0; }
+
+// Where gemm_nt sends one problem
+enum NtRoute { NT_TC3, NT_TC, NT_NARROW, NT_SIMT };
+static NtRoute nt_route(const GemmNT& p) {
+  // tensor-core path for all but the tiny / skinny GEMMs (those stay on the SIMT kernels); a problem whose row count
+  // lives on the device (capacity mode) runs there only (gemm_nt refuses it when that path is off or not eligible)
+  if (p.m_dev) return NT_TC3;
   if (g_use_tc && p.N >= 48 && p.K >= 32) {
-    if (use_tc3() && p.M >= 256 && tc3_eligible(p)) return gemm_nt_tc3_group(&p, 1, st);
-    if (p.M >= 1024 && tc_eligible(p)) return gemm_nt_tc(p, st);
+    if (use_tc3() && p.M >= 256 && tc3_eligible(p)) return NT_TC3;
+    if (p.M >= 1024 && tc_eligible(p)) return NT_TC;
   }
-  // Narrow outputs (the APD heads: 1024 x 500 -> 39 / 3 / 1) stay on the fp32 SIMT kernel unless debug bit 2 is set:
+  // Narrow outputs (the APD heads: 1024 x 500 -> 39 / 3 / 1) stay on the fp32 SIMT kernels unless debug bit 2 is set:
   // a handful of tensor-core tiles would be faster, but the output layer's 3xTF32 error lands on the logits
   // unattenuated, and on the shipped checkpoint x 256 gdb13 rows the logit error is already close to the 1e-4 contract
   // with this layer in fp32 (tests/test_gpu_parity.py::test_pretrained_checkpoint_on_real_gdb13_rows).
   if (g_use_tc && use_tc3() && (g_tc_debug & 4) && p.N < 48 && p.K >= 128 && p.M >= 256 && tc3_eligible(p))
-    return gemm_nt_tc3_group(&p, 1, st);
-  return gemm_nt_simt(p, st);
+    return NT_TC3;
+  if (narrow_dispatch() && std::max(p.N, p.n_store) <= kNarrowMaxN) return NT_NARROW;
+  return NT_SIMT;
+}
+
+int gemm_nt(const GemmNT& p, cudaStream_t st) {
+  GIB_TRY(check_precision(p.tf32, "gemm_nt"));
+  if (p.m_dev && (!g_use_tc || !use_tc3() || !tc3_eligible(p))) {
+    set_error("gemm_nt: device-side row counts need the tensor-core path (tensor cores on, pre-split weights)");
+    return -2;
+  }
+  switch (nt_route(p)) {
+    case NT_TC3: return gemm_nt_tc3_group(&p, 1, st);
+    case NT_TC: return gemm_nt_tc(p, st);
+    case NT_NARROW: return gemm_nt_narrow(&p, 1, st);
+    default: return gemm_nt_simt(p, st);
+  }
+}
+
+// n <= 4 independent problems that write disjoint outputs, with the results gemm_nt gives each of them: the members
+// gemm_nt sends to the wgmma kernel as one grouped launch, the narrow ones as one narrow launch, the rest one by one
+int gemm_nt_batch(const GemmNT* ps, int n, cudaStream_t st) {
+  if (n > kNarrowMax) { set_error("gemm_nt_batch: %d problems (max %d)", n, kNarrowMax); return -2; }
+  if (n == 1 || !narrow_dispatch()) {
+    for (int i = 0; i < n; ++i) GIB_TRY(gemm_nt(ps[i], st));
+    return 0;
+  }
+  GemmNT tc3[kNarrowMax], narrow[kNarrowMax];
+  int n3 = 0, nn = 0;
+  for (int i = 0; i < n; ++i) {
+    const GemmNT& p = ps[i];
+    const NtRoute rt = nt_route(p);
+    const bool refused = p.m_dev && (!g_use_tc || !use_tc3() || !tc3_eligible(p));
+    if (refused || (rt != NT_TC3 && rt != NT_NARROW)) { GIB_TRY(gemm_nt(p, st)); continue; }
+    GIB_TRY(check_precision(p.tf32, "gemm_nt_batch"));
+    if (p.M <= 0 || p.N <= 0) continue;
+    if (rt == NT_TC3) tc3[n3++] = p; else narrow[nn++] = p;
+  }
+  if (n3) GIB_TRY(gemm_nt_tc3_group(tc3, n3, st));
+  if (nn) GIB_TRY(gemm_nt_narrow(narrow, nn, st));
+  return 0;
 }
 
 // Several independent problems (sibling MLPs, the per-bond-type message MLPs): one grouped tensor-core launch when
-// together they fill the machine reasonably, else problem by problem.
+// together they fill the machine reasonably, else as gemm_nt_batch
 int gemm_nt_group(const GemmNT* ps, int n, cudaStream_t st) {
   if (n == 1) return gemm_nt(ps[0], st);
   for (int i = 0; i < n; ++i) GIB_TRY(check_precision(ps[i].tf32, "gemm_nt_group"));
@@ -220,8 +380,7 @@ int gemm_nt_group(const GemmNT* ps, int n, cudaStream_t st) {
   }
   if (ok3 && (tiles >= 4 || dyn)) return gemm_nt_tc3_group(ps, n, st);
   if (ok && !dyn && tiles >= 16) return gemm_nt_tc_group(ps, n, st);
-  for (int i = 0; i < n; ++i) GIB_TRY(gemm_nt(ps[i], st));
-  return 0;
+  return gemm_nt_batch(ps, n, st);
 }
 
 // Dependent chain (the layers of sibling MLPs): ONE persistent tensor-core launch when every member qualifies,
@@ -263,6 +422,42 @@ int gemm_nt_simt(const GemmNT& p, cudaStream_t st) {
     dim3 grid(ceil_div(ncols, 64), ceil_div(p.M, 64));
     sgemm_nt_kernel<64, 64, 1, 1><<<grid, 256, 0, st>>>(p);
   }
+  GIB_LAUNCH_CHECK();
+  return 0;
+}
+
+int gemm_nt_narrow(const GemmNT* ps, int n, cudaStream_t st) {
+  NarrowGroup g;
+  g.n = 0;
+  double work = 0;
+  for (int i = 0; i < n; ++i) {
+    const GemmNT& p = ps[i];
+    if (p.M <= 0 || p.N <= 0) continue;
+    if (p.K % BK != 0 || (p.lda & 3) || (p.ldb & 3) || p.K <= 0 || p.m_dev || std::max(p.N, p.n_store) > kNarrowMaxN ||
+        g.n == kNarrowMax) {
+      set_error("gemm_nt_narrow: K=%d lda=%d ldb=%d N=%d n_store=%d (problem %d of %d) violate the narrow-kernel "
+                "contract", p.K, p.lda, p.ldb, p.N, p.n_store, i, n);
+      return -2;
+    }
+    g.p[g.n] = p;
+    g.bn[g.n] = ceil_div(std::max(p.N, p.n_store), 16) * 16;
+    ++g.n;
+    work += p.work > 0 ? p.work : 2.0 * p.M * (double)p.N * p.K;
+  }
+  if (g.n == 0) return 0;
+  // the most rows per thread that still gives every SM a CTA
+  const int num_sms = device_sm_count();
+  int tm = 4;
+  for (;; tm >>= 1) {
+    g.cta0[0] = 0;
+    for (int i = 0; i < g.n; ++i) g.cta0[i + 1] = g.cta0[i] + ceil_div(g.p[i].M, kNarrowThreads / (g.bn[i] / 4) * tm);
+    if (tm == 1 || g.cta0[g.n] >= num_sms) break;
+  }
+  ProfScope prof(PROF_GEMM_NT_SIMT, work, st);
+  const int grid = g.cta0[g.n];
+  if (tm == 4) sgemm_nt_narrow_kernel<4><<<grid, kNarrowThreads, 0, st>>>(g);
+  else if (tm == 2) sgemm_nt_narrow_kernel<2><<<grid, kNarrowThreads, 0, st>>>(g);
+  else sgemm_nt_narrow_kernel<1><<<grid, kNarrowThreads, 0, st>>>(g);
   GIB_LAUNCH_CHECK();
   return 0;
 }

@@ -641,13 +641,22 @@ static int mlp_backward_multi(const Run& r, const BwdBufs& bb, const MlpBwdJob* 
       k0 = k1;
     }
   }
-  // ---- (C) input gradient of the first layer (may chain through a shared buffer via aux: keep the members in order)
-  for (int i = 0; i < n; ++i) {
-    const MlpBwdJob& j = jobs[i];
-    if (j.rows <= 0 || !j.dX0) continue;
-    GemmNT p1 = lin_dx(r, r.pl.lins[j.m->first], G[1][i], j.rows, j.dX0, j.ld_dx, j.m_dev, j.base_dev);
-    if (j.dx_aux) { p1.mode = EPI_ADD; p1.aux = j.dx_aux; p1.ldaux = j.ld_dx; }
-    GIB_TRY(gemm_nt(p1, r.st));
+  // ---- (C) input gradient of the first layer: consecutive members without aux write disjoint outputs and run as one
+  //      batch; a member that adds into a shared buffer through aux keeps its place in the order
+  {
+    GemmNT batch[4];
+    int nb = 0;
+    for (int i = 0; i < n; ++i) {
+      const MlpBwdJob& j = jobs[i];
+      if (j.rows <= 0 || !j.dX0) continue;
+      GemmNT p1 = lin_dx(r, r.pl.lins[j.m->first], G[1][i], j.rows, j.dX0, j.ld_dx, j.m_dev, j.base_dev);
+      if (!j.dx_aux) { batch[nb++] = p1; continue; }
+      p1.mode = EPI_ADD; p1.aux = j.dx_aux; p1.ldaux = j.ld_dx;
+      GIB_TRY(gemm_nt_batch(batch, nb, r.st));
+      nb = 0;
+      GIB_TRY(gemm_nt(p1, r.st));
+    }
+    GIB_TRY(gemm_nt_batch(batch, nb, r.st));
   }
   // ---- (B) weight gradients of every layer and member: one grouped launch + one reduction -----------------------
   GemmDW qs[kTc3MaxProblems];

@@ -98,7 +98,10 @@ int gib_version(void);
 /* tensor-core 3xTF32 GEMM path on (default) / off (fp32 SIMT GEMMs only); process-wide switch */
 void gib_set_tensor_cores(int on);
 int gib_get_tensor_cores(void);
-/* bit 3: GGNN / MNN message MLPs on one row per bond entry (the AttentionGGNN's layout) instead of one per message row.
+/* bit 4: the GEMM dispatch before the narrow fp32 kernel: narrow outputs (max(N, n_store) <= 48) on the general SIMT
+ * kernel, groups that do not all qualify for one tensor-core launch and the first-layer input gradients of sibling MLPs
+ * problem by problem.  The results are bit-identical either way; only the launches differ.
+ * bit 3: GGNN / MNN message MLPs on one row per bond entry (the AttentionGGNN's layout) instead of one per message row.
  * bit 2: narrow outputs (N < 48, the APD heads) on the tensor-core kernel too (default: fp32 SIMT, see gemm_simt.cu).
  * bit 1: no dependent-chain launches (every MLP layer its own launch).
  * bit 0: per-problem call pattern: no grouped or chained tensor-core launches, raw weights split inside the kernel,
