@@ -172,6 +172,8 @@ _PROTOS = {
     "gib_scaffold_first_ws_bytes": (c_sz, [c_p, c_i, c_i]),
     "gib_scaffold_first": (c_i, [c_p, c_p, c_p, c_i, c_p, c_p, c_i, ctypes.c_ulonglong, c_ll, c_ll, c_p, c_ll]
                            + [c_p] * 7),
+    "gib_murcko_ws_bytes": (c_sz, [c_p, c_i, c_i]),
+    "gib_murcko": (c_i, [c_p, c_p, c_p, c_i, c_i] + [c_p] * 4 + [c_ll] + [c_p] * 5),
     "gib_route_plan_ws_bytes": (c_sz, [c_p, c_i]),
     "gib_route_max_states": (c_ll, [c_p, c_i]),
     "gib_route_plan": (c_i, [c_p, c_p, c_p, c_i, c_i] + [c_p] * 4),

@@ -1195,6 +1195,35 @@ __device__ void match_candidates(const PP& p, MatchSmem& S, const signed char* S
   __syncwarp();
 }
 
+// the molecule side of match_scaffold for the graph E of n atoms: S.adj, S.any and S.mdeg.  Returns the degree sum
+// (every lane).
+__device__ int match_load(const PP& p, MatchSmem& S, const signed char* E, int n) {
+  const int lane = threadIdx.x & 31, N = p.N, Ef = p.Ef, W = (N + 31) / 32;
+  for (int q = lane; q < Ef * N * W; q += 32) S.adj[q] = 0;
+  for (int q = lane; q < N * W; q += 32) S.any[q / W][q % W] = 0;
+  __syncwarp();
+  for (int q = lane; q < n * n; q += 32) {
+    const int i = q / n, j = q % n;
+    bool any = false;
+    for (int t = 0; t < Ef; ++t)
+      if (E[((size_t)i * N + j) * Ef + t]) {
+        atomicOr(&S.adj[((size_t)t * N + i) * W + (j >> 5)], 1u << (j & 31));
+        any = true;
+      }
+    if (any) atomicOr(&S.any[i][j >> 5], 1u << (j & 31));
+  }
+  __syncwarp();
+  int deg_sum = 0;
+  for (int i = lane; i < n; i += 32) {
+    int d = 0;
+    for (int w = 0; w < W; ++w) d += __popc(S.any[i][w]);
+    S.mdeg[i] = (short)d;
+    deg_sum += d;
+  }
+  __syncwarp();
+  return warp_sum(deg_sum);
+}
+
 // the smallest embedding of scaffold s (k atoms) in the molecule (X, E, n atoms) into S.phi: 1 found, 0 none, -1 the
 // search would take more than `budget` assignments.  Every lane gets the answer.
 __device__ int match_scaffold(const PP& p, MatchSmem& S, const signed char* X, const signed char* E, int n,
@@ -1266,32 +1295,12 @@ __global__ void __launch_bounds__(32) scaffold_first_kernel(
   const int n = n0[m];
   const signed char* X = nodes + (size_t)m * N * F;
   const signed char* E = edges + (size_t)m * N * N * Ef;
-  for (int q = lane; q < Ef * N * W; q += 32) S.adj[q] = 0;
-  for (int q = lane; q < N * W; q += 32) S.any[q / W][q % W] = 0;
   if (lane < W) seen[lane] = 0;
   if (lane == 0) ok = n > 0 && !bad[m];                     // refused by the input checks: left alone, outputs zero
-  __syncwarp();
-  for (int q = lane; q < n * n; q += 32) {
-    const int i = q / n, j = q % n;
-    bool any = false;
-    for (int t = 0; t < Ef; ++t)
-      if (E[((size_t)i * N + j) * Ef + t]) {
-        atomicOr(&S.adj[((size_t)t * N + i) * W + (j >> 5)], 1u << (j & 31));
-        any = true;
-      }
-    if (any) atomicOr(&S.any[i][j >> 5], 1u << (j & 31));
-  }
+  const int deg_sum = match_load(p, S, E, n);
   if (!load_ranking(N, n, draw, seed, epoch, first, m, rankings + (size_t)m * N, rank, key, seen, status) && lane == 0)
     ok = 0;
   __syncwarp();
-  int deg_sum = 0;
-  for (int i = lane; i < n; i += 32) {
-    int d = 0;
-    for (int w = 0; w < W; ++w) d += __popc(S.any[i][w]);
-    S.mdeg[i] = (short)d;
-    deg_sum += d;
-  }
-  deg_sum = warp_sum(deg_sum);
   // connectivity first, as gib_reorder checks it: the layers from atom 0 must reach every atom
   if (lane == 0 && ok) {
     for (int w = 0; w < W; ++w) seen[w] = 0;
@@ -1347,6 +1356,349 @@ __global__ void __launch_bounds__(32) scaffold_first_kernel(
   // a refused molecule's outputs are zero
   write_reordered(p, X, E, ord, ok ? n : 0, order + (size_t)m * N, out_nodes + (size_t)m * N * F,
                   out_edges + (size_t)m * N * N * Ef);
+}
+
+// ---- Murcko scaffolds (gib_murcko) ---------------------------------------------------------------------------------
+// The items of one call: the known table's entries 0..K-1, then the scaffolds of the chunk's molecules K..K+n-1.
+// rep[i]: the item whose class item i belongs to (the first item of that class), kItemNone (no scaffold, or refused)
+// or kItemOpen (not yet assigned).
+constexpr int kItemNone = -1, kItemOpen = -2;
+
+struct MurckoItems {
+  const signed char* known_nodes;   // [K, N, F]
+  const signed char* known_edges;   // [K, N, N, Ef]
+  const signed char* nodes;         // [n, N, F]: the chunk's scaffolds, canonical order
+  const signed char* edges;
+  int K;
+  __device__ const signed char* X(const PP& p, int i) const {
+    return i < K ? known_nodes + (size_t)i * p.N * p.F : nodes + (size_t)(i - K) * p.N * p.F;
+  }
+  __device__ const signed char* E(const PP& p, int i) const {
+    const size_t eb = (size_t)p.N * p.N * p.Ef;
+    return i < K ? known_edges + (size_t)i * eb : edges + (size_t)(i - K) * eb;
+  }
+};
+
+// one warp per molecule: keep = the 2-core (atoms of degree <= 1 removed, all at once, until none is left) plus the
+// atoms outside it with a double bond (edge feature 1) to it; the scaffold is the molecule's induced subgraph on them,
+// written in canonical order (breadth-first from the lowest kept index, each layer in increasing index) with its
+// order row (molecule atom per scaffold position, -1 past k).  No ring: nothing kept, k = 0, zero bytes.
+__global__ void __launch_bounds__(32) murcko_kernel(PP p, const signed char* __restrict__ nodes,
+                                                    const signed char* __restrict__ edges,
+                                                    const int* __restrict__ n0, const int* __restrict__ bad,
+                                                    unsigned char* keep_out, int* sorder, signed char* sc_nodes,
+                                                    signed char* sc_edges, int* status) {
+  __shared__ unsigned adj[kReorderMaxN][kReorderWords], dbl[kReorderMaxN][kReorderWords];
+  __shared__ unsigned alive[kReorderWords], keep[kReorderWords], vis[kReorderWords];
+  __shared__ int rank[kReorderMaxN], ord[kReorderMaxN];
+  __shared__ int ok, k;
+  const int m = blockIdx.x, lane = threadIdx.x;
+  const int N = p.N, F = p.F, Ef = p.Ef, W = (N + 31) / 32;
+  const int n = n0[m];
+  const signed char* X = nodes + (size_t)m * N * F;
+  const signed char* E = edges + (size_t)m * N * N * Ef;
+  for (int q = lane; q < N * W; q += 32) adj[q / W][q % W] = dbl[q / W][q % W] = 0;
+  for (int i = lane; i < N; i += 32) rank[i] = N - i;      // layered_bfs takes the highest rank first
+  if (lane < W) alive[lane] = keep[lane] = 0;
+  if (lane == 0) {
+    ok = n > 0 && !bad[m];
+    k = 0;
+  }
+  __syncwarp();
+  for (int q = lane; q < n * n; q += 32) {
+    const int i = q / n, j = q % n;
+    bool any = false;
+    for (int t = 0; t < Ef; ++t) any |= E[((size_t)i * N + j) * Ef + t] != 0;
+    if (any) atomicOr(&adj[i][j >> 5], 1u << (j & 31));
+    if (Ef > 1 && E[((size_t)i * N + j) * Ef + 1]) atomicOr(&dbl[i][j >> 5], 1u << (j & 31));
+  }
+  for (int a = lane; a < n; a += 32) atomicOr(&alive[a >> 5], 1u << (a & 31));
+  __syncwarp();
+  if (lane == 0 && ok) {                                    // connectivity, as gib_reorder checks it
+    for (int w = 0; w < W; ++w) vis[w] = 0;
+    vis[0] = 1u;
+    ord[0] = 0;
+    if (layered_bfs(adj, W, rank, vis, ord, 1) != n) {
+      flag_bad(status, GIB_PP_DISCONNECTED, m);
+      ok = 0;
+    }
+  }
+  __syncwarp();
+  if (ok) {
+    // atom w * 32 + lane is bit `lane` of word w: one ballot per word gives the atoms that go
+    for (bool again = true; again;) {
+      unsigned gone[kReorderWords];
+      again = false;
+#pragma unroll
+      for (int w = 0; w < kReorderWords; ++w) {
+        bool go = false;
+        const int a = w * 32 + lane;
+        if (w < W && a < n && (alive[w] >> lane & 1u)) {
+          int d = 0;
+          for (int v = 0; v < W; ++v) d += __popc(adj[a][v] & alive[v]);
+          go = d <= 1;
+        }
+        gone[w] = __ballot_sync(0xffffffffu, go);
+        again |= gone[w] != 0;
+      }
+      __syncwarp();
+      if (lane == 0) {
+#pragma unroll
+        for (int w = 0; w < kReorderWords; ++w)
+          if (w < W) alive[w] &= ~gone[w];
+      }
+      __syncwarp();
+    }
+#pragma unroll
+    for (int w = 0; w < kReorderWords; ++w) {
+      const int a = w * 32 + lane;
+      bool kp = false;
+      if (w < W && a < n) {
+        kp = alive[w] >> lane & 1u;
+        for (int v = 0; v < W && !kp; ++v) kp = (dbl[a][v] & alive[v]) != 0;
+      }
+      const unsigned kw = __ballot_sync(0xffffffffu, kp);
+      if (lane == 0 && w < W) keep[w] = kw;
+    }
+    __syncwarp();
+    if (lane == 0) {
+      int start = -1;
+      for (int w = 0; w < W && start < 0; ++w)
+        if (keep[w]) start = w * 32 + __ffs(keep[w]) - 1;
+      if (start >= 0) {
+        for (int w = 0; w < W; ++w) vis[w] = ~keep[w];     // only kept atoms are reached
+        vis[start >> 5] |= 1u << (start & 31);
+        ord[0] = start;
+        k = layered_bfs(adj, W, rank, vis, ord, 1);
+      }
+    }
+    __syncwarp();
+  }
+  for (int a = lane; a < N; a += 32) keep_out[(size_t)m * N + a] = ok && (keep[a >> 5] >> (a & 31) & 1u);
+  write_reordered(p, X, E, ord, k, sorder + (size_t)m * N, sc_nodes + (size_t)m * N * F,
+                  sc_edges + (size_t)m * N * N * Ef);
+}
+
+// one warp per item: its atom count k (rows up to the last non-zero one), bonds, and a colour-refinement (1-WL) hash
+//   c_0(a) = mix64(sum_f byte_hash(f, X[a][f])),
+//   c_r(a) = mix64(c_{r-1}(a) + sum over bonds (a, b) of type t of mix64(c_{r-1}(b) ^ (t + 1) << 56)), r = 1..k,
+//   hash   = mix64(sum_a mix64(c_k(a)) ^ (k << 32 | bonds))   (kEmpty -> kEmpty - 1),
+// the type being the bond's first non-zero edge byte.  Isomorphic graphs hash equal; equal hashes prove nothing.
+// An item with k >= 1 is inserted into the hash table (slot) and left open.
+__global__ void __launch_bounds__(32) murcko_hash_kernel(PP p, MurckoItems it, int* item_k, int* item_bonds,
+                                                         unsigned long long* keys, long long mask, int* slot,
+                                                         int* rep) {
+  __shared__ unsigned adj[kMatchAdjWords];
+  __shared__ unsigned long long col[2][kReorderMaxN];
+  const int i = blockIdx.x, lane = threadIdx.x;
+  const int N = p.N, F = p.F, Ef = p.Ef, W = (N + 31) / 32;
+  const signed char* X = it.X(p, i);
+  const signed char* E = it.E(p, i);
+  int last = -1;
+  for (int r = lane; r < N; r += 32) {
+    bool any = false;
+    for (int f = 0; f < F; ++f) any |= X[(size_t)r * F + f] != 0;
+    if (any) last = r;
+  }
+  const int k = warp_max(last) + 1;
+  for (int q = lane; q < Ef * N * W; q += 32) adj[q] = 0;
+  __syncwarp();
+  int nnz = 0;
+  for (int q = lane; q < k * k; q += 32) {
+    const int a = q / k, b = q % k;
+    for (int t = 0; t < Ef; ++t)
+      if (E[((size_t)a * N + b) * Ef + t]) {
+        atomicOr(&adj[((size_t)t * N + a) * W + (b >> 5)], 1u << (b & 31));
+        ++nnz;
+        break;
+      }
+  }
+  const int bonds = warp_sum(nnz) / 2;
+  for (int a = lane; a < k; a += 32) {
+    unsigned long long h = 0;
+    for (int f = 0; f < F; ++f) h += byte_hash(f, X[(size_t)a * F + f]);
+    col[0][a] = mix64(h);
+  }
+  __syncwarp();
+  for (int r = 0; r < k; ++r) {
+    const unsigned long long* src = col[r & 1];
+    unsigned long long* dst = col[(r + 1) & 1];
+    for (int a = lane; a < k; a += 32) {
+      unsigned long long s = src[a];
+      for (int t = 0; t < Ef; ++t)
+        for (int w = 0; w < W; ++w)
+          for (unsigned bits = adj[((size_t)t * N + a) * W + w]; bits; bits &= bits - 1)
+            s += mix64(src[w * 32 + __ffs(bits) - 1] ^ ((unsigned long long)(t + 1) << 56));
+      dst[a] = mix64(s);
+    }
+    __syncwarp();
+  }
+  unsigned long long sum = 0;
+  for (int a = lane; a < k; a += 32) sum += mix64(col[k & 1][a]);
+  sum = warp_sum_u64(sum);
+  unsigned long long h = mix64(sum ^ ((unsigned long long)k << 32 | (unsigned)bonds));
+  if (h == kEmpty) h = kEmpty - 1;
+  if (lane == 0) {
+    item_k[i] = k;
+    item_bonds[i] = bonds;
+    slot[i] = k > 0 ? tbl_insert(keys, h, mask) : -1;
+    rep[i] = k > 0 ? kItemOpen : kItemNone;
+  }
+}
+
+// one dedup round, part 1: each hash bucket's smallest open item becomes its representative this round (atomicMax of
+// (round, ~item): buckets need no reset between rounds).  Clears the round's open counter, status[0].
+__global__ void murcko_select_kernel(int items, int round, const int* __restrict__ rep, const int* __restrict__ slot,
+                                     unsigned long long* bucket, int* status) {
+  const int t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t == 0) status[0] = 0;
+  for (int i = t; i < items; i += gridDim.x * blockDim.x)
+    if (rep[i] == kItemOpen)
+      atomicMax(&bucket[slot[i]], (unsigned long long)round << 32 | (0xffffffffu - (unsigned)i));
+}
+
+// part 2, one warp per open item: the representative joins its own class (phi = the identity); a chunk item of the same
+// atom and bond counts joins it when match_scaffold embeds the representative in it -- an induced embedding between
+// graphs of equal counts is an isomorphism -- with that smallest embedding as phi (representative atom -> item atom).
+// A known item never joins another (the known entries are distinct).  The others stay open and are counted.
+__global__ void __launch_bounds__(32) murcko_match_kernel(PP p, MurckoItems it, const int* __restrict__ item_k,
+                                                          const int* __restrict__ item_bonds,
+                                                          const int* __restrict__ slot,
+                                                          const unsigned long long* __restrict__ bucket,
+                                                          long long budget, int* rep, short* phi, int* status) {
+  __shared__ MatchSmem S;
+  __shared__ short rdeg[kReorderMaxN];
+  const int i = blockIdx.x, lane = threadIdx.x, N = p.N, Ef = p.Ef;
+  if (rep[i] != kItemOpen) return;
+  const int r = (int)(0xffffffffu - (unsigned)bucket[slot[i]]);
+  const int k = item_k[i];
+  short* ph = i >= it.K ? phi + (size_t)(i - it.K) * N : nullptr;
+  int res = 0;
+  if (r == i) {
+    res = 1;
+    if (ph)
+      for (int a = lane; a < k; a += 32) ph[a] = (short)a;
+  } else if (ph && item_k[r] == k && item_bonds[r] == item_bonds[i]) {
+    const signed char* RE = it.E(p, r);
+    match_load(p, S, it.E(p, i), k);
+    for (int a = lane; a < N; a += 32) {
+      int d = 0;
+      for (int b = 0; b < k && a < k; ++b) {
+        bool any = false;
+        for (int t = 0; t < Ef; ++t) any |= RE[((size_t)a * N + b) * Ef + t] != 0;
+        d += any;
+      }
+      rdeg[a] = (short)d;
+    }
+    __syncwarp();
+    gib_scaffolds view{};
+    view.nodes = it.X(p, r);
+    view.edges = RE;
+    res = match_scaffold(p, S, it.X(p, i), it.E(p, i), k, view, rdeg, 0, k, budget);
+    if (res > 0)
+      for (int a = lane; a < k; a += 32) ph[a] = S.phi[a];
+  }
+  if (lane == 0) {
+    if (res > 0) {
+      rep[i] = r;
+    } else if (res < 0) {
+      rep[i] = kItemNone;
+      flag_bad(status, GIB_PP_MATCH_BUDGET, i - it.K);
+    } else {
+      atomicAdd(&status[0], 1);
+    }
+  }
+}
+
+__global__ void murcko_new_kernel(int n, int K, const int* __restrict__ rep, int* is_new) {
+  const int m = blockIdx.x * blockDim.x + threadIdx.x;
+  if (m < n) is_new[m] = rep[K + m] == K + m;
+}
+
+// one warp per molecule: its entry id (a new entry's id is K + its rank among the chunk's new representatives, off),
+// the count, a new entry's bytes into the table, and the attachment points: entry atom i is one when the molecule atom
+// it maps to (through phi and the scaffold's order row) has a bond to an atom outside the scaffold
+__global__ void __launch_bounds__(32) murcko_emit_kernel(PP p, MurckoItems it, const signed char* __restrict__ edges,
+                                                         const int* __restrict__ n0,
+                                                         const unsigned char* __restrict__ keep,
+                                                         const int* __restrict__ sorder, const int* __restrict__ rep,
+                                                         const int* __restrict__ off, const short* __restrict__ phi,
+                                                         const int* __restrict__ item_k, int* ids,
+                                                         signed char* table_nodes, signed char* table_edges,
+                                                         unsigned long long* counts, unsigned char* attach) {
+  const int m = blockIdx.x, lane = threadIdx.x, K = it.K;
+  const int N = p.N, F = p.F, Ef = p.Ef;
+  const int r = rep[K + m];
+  const int id = r < 0 ? -1 : r < K ? r : K + off[r - K];
+  if (lane == 0) {
+    ids[m] = id;
+    if (id >= 0) atomicAdd(&counts[id], 1ull);
+  }
+  if (id < 0) return;
+  if (r == K + m) {
+    const signed char* X = it.X(p, r);
+    const signed char* E = it.E(p, r);
+    for (int q = lane; q < N * F; q += 32) table_nodes[(size_t)id * N * F + q] = X[q];
+    for (int q = lane; q < N * N * Ef; q += 32) table_edges[(size_t)id * N * N * Ef + q] = E[q];
+  }
+  const int k = item_k[K + m], n = n0[m];
+  const signed char* E = edges + (size_t)m * N * N * Ef;
+  const unsigned char* kp = keep + (size_t)m * N;
+  const int* o = sorder + (size_t)m * N;
+  const short* ph = phi + (size_t)m * N;
+  for (int q = lane; q < k * n; q += 32) {
+    const int i = q / n, b = q % n, a = o[ph[i]];
+    if (kp[b]) continue;
+    bool any = false;
+    for (int t = 0; t < Ef; ++t) any |= E[((size_t)a * N + b) * Ef + t] != 0;
+    if (any) attach[(size_t)id * N + i] = 1;
+  }
+}
+
+struct MurckoWs {
+  size_t len, n0, bad, off, sorder, phi, sc_nodes, sc_edges, item_k, item_bonds, slot, rep, keys, bucket, total;
+  long long table;
+};
+
+MurckoWs murcko_ws_layout(const PP& p, int n, int K) {
+  MurckoWs w{};
+  const long long items = (long long)n + K;
+  w.table = 1024;
+  while (w.table < 2 * items) w.table <<= 1;
+  size_t o = 0;
+  auto take = [&](size_t bytes) { size_t r = o; o = align256(o + bytes); return r; };
+  w.len = take(4ull * n);
+  w.n0 = take(4ull * n);
+  w.bad = take(4ull * n);
+  w.off = take(4ull * (n + 1));
+  w.sorder = take(4ull * n * p.N);
+  w.phi = take(2ull * n * p.N);
+  w.sc_nodes = take((size_t)n * p.N * p.F);
+  w.sc_edges = take((size_t)n * p.N * p.N * p.Ef);
+  w.item_k = take(4ull * items);
+  w.item_bonds = take(4ull * items);
+  w.slot = take(4ull * items);
+  w.rep = take(4ull * items);
+  w.keys = take(8ull * w.table);
+  w.bucket = take(8ull * w.table);
+  w.total = o;
+  return w;
+}
+
+int murcko_limits(const char* who, const gib_pp_dims* d, int n_molecules, int n_known, PP* p) {
+  GIB_TRY(make_pp(who, d, p));
+  const int W = (p->N + 31) / 32;
+  if (p->N > kReorderMaxN || (long long)p->Ef * p->N * W > kMatchAdjWords) {
+    set_error("%s: need N <= %d and Ef * N * ceil(N / 32) <= %d, got N=%d Ef=%d", who, kReorderMaxN, kMatchAdjWords,
+              p->N, p->Ef);
+    return -1;
+  }
+  if (n_molecules < 1 || n_known < 0 || (long long)n_molecules + n_known > INT_MAX / 4) {
+    set_error("%s: need n_molecules >= 1, n_known >= 0 and n_molecules + n_known <= %d, got %d and %d", who,
+              INT_MAX / 4, n_molecules, n_known);
+    return -1;
+  }
+  return 0;
 }
 
 }  // namespace
@@ -1743,6 +2095,79 @@ int gib_scaffold_first(const gib_pp_dims* d, const signed char* nodes, const sig
   scaffold_first_kernel<<<n_molecules, 32, 0, s>>>(p, nodes, edges, n0, bad, *sc, sdeg, sbonds, scaffold_ids, draw,
                                                    seed, epoch, first_molecule, rankings, budget, order, ids,
                                                    out_nodes, out_edges, status);
+  GIB_LAUNCH_CHECK();
+  return 0;
+}
+
+size_t gib_murcko_ws_bytes(const gib_pp_dims* d, int n_molecules, int n_known) {
+  PP p;
+  if (murcko_limits("gib_murcko_ws_bytes", d, n_molecules, n_known, &p)) return 0;
+  return murcko_ws_layout(p, n_molecules, n_known).total;
+}
+
+int gib_murcko(const gib_pp_dims* d, const signed char* nodes, const signed char* edges, int n_molecules, int n_known,
+               signed char* table_nodes, signed char* table_edges, long long* counts, unsigned char* attachment,
+               long long budget, unsigned char* keep, int* ids, void* ws, int* status, gib_stream stream) {
+  PP p;
+  GIB_TRY(murcko_limits("gib_murcko", d, n_molecules, n_known, &p));
+  if (budget < 1) {
+    set_error("gib_murcko: need budget >= 1, got %lld", budget);
+    return -1;
+  }
+  if (!nodes || !edges || !table_nodes || !table_edges || !counts || !attachment || !keep || !ids || !ws || !status) {
+    set_error("gib_murcko: null argument");
+    return -1;
+  }
+  const MurckoWs w = murcko_ws_layout(p, n_molecules, n_known);
+  char* b = static_cast<char*>(ws);
+  int* len = (int*)(b + w.len);
+  int* n0 = (int*)(b + w.n0);
+  int* bad = (int*)(b + w.bad);
+  int* off = (int*)(b + w.off);
+  int* sorder = (int*)(b + w.sorder);
+  short* phi = (short*)(b + w.phi);
+  int* item_k = (int*)(b + w.item_k);
+  int* item_bonds = (int*)(b + w.item_bonds);
+  int* slot = (int*)(b + w.slot);
+  int* rep = (int*)(b + w.rep);
+  unsigned long long* keys = (unsigned long long*)(b + w.keys);
+  unsigned long long* bucket = (unsigned long long*)(b + w.bucket);
+  const MurckoItems it{table_nodes, table_edges, (const signed char*)(b + w.sc_nodes),
+                       (const signed char*)(b + w.sc_edges), n_known};
+  const int n = n_molecules, items = n + n_known;
+  cudaStream_t s = (cudaStream_t)stream;
+  pp_init_kernel<<<1, 32, 0, s>>>(status, nullptr, nullptr, 0, 0);
+  GIB_LAUNCH_CHECK();
+  GIB_CUDA_TRY(cudaMemsetAsync(keys, 0xff, 8ull * w.table, s));      // kEmpty
+  GIB_CUDA_TRY(cudaMemsetAsync(bucket, 0, 8ull * w.table, s));
+  pp_count_kernel<<<n, 32, 0, s>>>(p, nodes, edges, len, n0, status, nullptr, gib_scaffolds{}, bad);
+  GIB_LAUNCH_CHECK();
+  murcko_kernel<<<n, 32, 0, s>>>(p, nodes, edges, n0, bad, keep, sorder, (signed char*)(b + w.sc_nodes),
+                                 (signed char*)(b + w.sc_edges), status);
+  GIB_LAUNCH_CHECK();
+  murcko_hash_kernel<<<items, 32, 0, s>>>(p, it, item_k, item_bonds, keys, w.table - 1, slot, rep);
+  GIB_LAUNCH_CHECK();
+  // every round closes at least one item per bucket with an open item (its representative): at most `items` rounds
+  for (int round = 1;; ++round) {
+    if (round > items) {
+      set_error("gib_murcko: the deduplication did not finish in %d rounds", items);
+      return -1;
+    }
+    murcko_select_kernel<<<std::min(ceil_div(items, 256), 1024), 256, 0, s>>>(items, round, rep, slot, bucket, status);
+    GIB_LAUNCH_CHECK();
+    murcko_match_kernel<<<items, 32, 0, s>>>(p, it, item_k, item_bonds, slot, bucket, budget, rep, phi, status);
+    GIB_LAUNCH_CHECK();
+    int open = 0;
+    GIB_CUDA_TRY(cudaMemcpyAsync(&open, status, sizeof(int), cudaMemcpyDeviceToHost, s));
+    GIB_CUDA_TRY(cudaStreamSynchronize(s));
+    if (!open) break;
+  }
+  murcko_new_kernel<<<ceil_div(n, 256), 256, 0, s>>>(n, n_known, rep, len);
+  GIB_LAUNCH_CHECK();
+  pp_scan_kernel<<<1, 1024, 0, s>>>(n, len, off, status);
+  GIB_LAUNCH_CHECK();
+  murcko_emit_kernel<<<n, 32, 0, s>>>(p, it, edges, n0, keep, sorder, rep, off, phi, item_k, ids, table_nodes,
+                                      table_edges, (unsigned long long*)counts, attachment);
   GIB_LAUNCH_CHECK();
   return 0;
 }

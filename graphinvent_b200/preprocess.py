@@ -21,6 +21,9 @@ stacks.  `file_rows()` runs the construction of `groups()` with the rows left on
 
 `scaffold_first()` finds each molecule's scaffold (`gib_scaffold_first`) and puts it first in decoding order, the
 order the conditional route scorer and the scaffold decorators need.
+
+`murcko_scaffolds()` extracts each molecule's Bemis-Murcko scaffold (`gib_murcko`) and deduplicates them into the
+scaffold table, with counts and observed attachment points, that `scaffold_first` and the decorators take.
 """
 import ctypes
 import sys
@@ -401,6 +404,85 @@ def scaffold_first(nodes, edges, scaffolds, attachment=None, scaffold_ids=None, 
                                      stream), "gib_scaffold_first")
         refuse_bad(status.cpu().numpy(), pos, stop, _MATCH_REASONS)
     return out_nodes, out_edges, order, ids
+
+
+Murcko = namedtuple("Murcko", "nodes edges ids counts attachment keep")
+Murcko.__doc__ = """The Murcko scaffolds of a set (`murcko_scaffolds`), all device tensors:
+nodes int8 [S, N, F] / edges int8 [S, N, N, Ef]: the distinct scaffolds, in order of first occurrence
+ids int32 [M]: each molecule's entry, -1 without a ring;  counts int64 [S]: molecules per entry
+attachment bool [S, N]: entry atoms where some molecule of the entry carries a substituent
+keep bool [M, N]: the kept atoms, in each molecule's own numbering"""
+
+_MURCKO_REASONS = _REORDER_REASONS[:3] + ((PP_DISCONNECTED, "a disconnected graph"),
+                                         (PP_MATCH_BUDGET, "the scaffold isomorphism search ran out of its budget of "
+                                          "search-tree nodes (raise `budget`)"))
+
+
+def murcko_scaffolds(nodes, edges, *, layout, known=None, budget=1 << 20, chunk_molecules=65536, device="cuda"):
+    """Each molecule's Bemis-Murcko scaffold and the distinct scaffolds of the set (`gib_murcko`, csrc/preprocess.cu).
+
+    nodes [M, N, F] / edges [M, N, N, Ef]: int8 stacks (numpy or torch, any atom order), validated and refused as
+    `reorder` refuses them (ValueError naming the first bad molecule).  `layout` as `reorder` takes it.
+    The rule is RDKit's `MurckoScaffold.GetScaffoldForMol`: an atom is kept when it lies on a ring or on the shortest
+    path between two rings, or when it has a double bond (edge feature 1) to such an atom.  The scaffold keeps every
+    bond among its atoms and copies their node rows byte for byte, implicit-H and chirality bytes included -- unlike
+    RDKit's standalone scaffold molecule, whose hydrogens are recomputed -- so that `scaffold_first` finds each
+    molecule's own scaffold in it.  Its atoms are in breadth-first order from the lowest kept index, each layer in
+    increasing index.  A molecule without a ring has no scaffold (id -1).
+    Two molecules share an entry when their scaffolds are isomorphic (checked by an exact search, never by a hash
+    alone); entries come in order of first occurrence, each as its first molecule's scaffold.  An entry atom is an
+    attachment point when, in some molecule of the entry, the atom it maps to (the smallest isomorphism) carries a
+    bond out of the scaffold.
+    known: an earlier result whose entries come first and keep their ids; new scaffolds follow, counts and attachment
+    accumulate (ids >= known.nodes.shape[0] are novel scaffolds).  Calls chained over the pieces of a set give what
+    one call over the whole set gives.  budget: search-tree nodes per isomorphism test (ValueError naming the molecule
+    beyond it).  Molecules go to the device chunk_molecules at a time.  Returns a `Murcko`."""
+    M, N, F, Ef = _check_stacks(nodes, edges)
+    d = _pp_dims(N, F, Ef, tuple(layout))
+    if int(budget) < 1:
+        raise ValueError(f"budget must be >= 1, got {budget}")
+    dev = _cuda(torch.device(device))
+    if known is None:
+        S = 0
+        t_nodes = torch.zeros((0, N, F), dtype=torch.int8, device=dev)
+        t_edges = torch.zeros((0, N, N, Ef), dtype=torch.int8, device=dev)
+        counts = torch.zeros(0, dtype=torch.int64, device=dev)
+        attach = torch.zeros((0, N), dtype=torch.uint8, device=dev)
+    else:
+        S = known.nodes.shape[0]
+        if tuple(known.nodes.shape) != (S, N, F) or tuple(known.edges.shape) != (S, N, N, Ef) \
+                or tuple(known.counts.shape) != (S,) or tuple(known.attachment.shape) != (S, N):
+            raise ValueError(f"known holds [S, {N}, {F}] / Ef = {Ef} scaffolds with counts [S] and attachment "
+                             f"[S, {N}], got {tuple(known.nodes.shape)} / {tuple(known.edges.shape)}")
+        t_nodes, t_edges = _on_device(known.nodes, dev).to(torch.int8), _on_device(known.edges, dev).to(torch.int8)
+        counts = _on_device(known.counts, dev).to(torch.int64)
+        attach = _on_device(known.attachment, dev).to(torch.uint8)
+    ids = torch.empty(M, dtype=torch.int32, device=dev)
+    keep = torch.zeros((M, N), dtype=torch.uint8, device=dev)
+    status = torch.empty(PP_STATUS_INTS, dtype=torch.int32, device=dev)
+    stream = ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+    chunk = min(max(int(chunk_molecules), 1), max(M, 1))
+    for pos in range(0, M, chunk):
+        stop = min(pos + chunk, M)
+        n = stop - pos
+        x, e = _on_device(nodes[pos:stop], dev), _on_device(edges[pos:stop], dev)
+        # room for n new entries after the S known ones; the call appends status[5] of them
+        t_nodes = torch.cat([t_nodes, t_nodes.new_zeros((n, N, F))])
+        t_edges = torch.cat([t_edges, t_edges.new_zeros((n, N, N, Ef))])
+        counts = torch.cat([counts, counts.new_zeros(n)])
+        attach = torch.cat([attach, attach.new_zeros((n, N))])
+        ws_bytes = lib.gib_murcko_ws_bytes(ctypes.byref(d), n, S)
+        if ws_bytes == 0:
+            raise ValueError(lib.gib_last_error().decode())
+        ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
+        check(lib.gib_murcko(ctypes.byref(d), _ptr(x), _ptr(e), n, S, _ptr(t_nodes), _ptr(t_edges), _ptr(counts),
+                             _ptr(attach), int(budget), _ptr(keep[pos:stop]), _ptr(ids[pos:stop]), _ptr(ws),
+                             _ptr(status), stream), "gib_murcko")
+        st = status.cpu().numpy()
+        refuse_bad(st, pos, stop, _MURCKO_REASONS)
+        S += int(st[5])
+        t_nodes, t_edges, counts, attach = t_nodes[:S], t_edges[:S], counts[:S], attach[:S]
+    return Murcko(t_nodes, t_edges, ids, counts, attach.bool(), keep.bool())
 
 
 def ts_properties(stats, smiles, constants):

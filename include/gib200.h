@@ -763,6 +763,35 @@ int gib_scaffold_first(const gib_pp_dims* d, const signed char* nodes, const sig
                        int* ids, signed char* out_nodes, signed char* out_edges, void* ws, int* status,
                        gib_stream stream);
 
+/* ---- Murcko scaffolds (graphinvent_b200.preprocess.murcko_scaffolds): each molecule's Bemis-Murcko scaffold, the
+ *      distinct scaffolds as a table with counts, and the attachment points their molecules use.
+ * Input as gib_reorder's (any atom order, the same validation and refusals: status[3] / [4]; d->batch_size unused).
+ * Rule (RDKit's MurckoScaffold.GetScaffoldForMol on these graphs): molecule atom a is kept when it lies in the 2-core
+ * (atoms of degree <= 1 removed until none is left: the ring atoms and the linkers between rings), or when it is
+ * outside the core with a double bond (edge feature 1; none when Ef == 1) to a core atom.  The scaffold is the
+ * induced subgraph on the kept atoms, node rows byte for byte (implicit-H and chirality bytes as the molecule has
+ * them), in canonical order: breadth-first from the lowest kept index, each layer in increasing index (every prefix
+ * is connected).  A molecule without a ring keeps nothing and gets id -1.
+ * Table: rows [0, n_known) of table_nodes [n_known + n_molecules, N, F] / table_edges [.., N, N, Ef] are the known
+ * entries (distinct scaffolds, as an earlier call wrote them); the call appends the chunk's new scaffolds at rows
+ * [n_known, n_known + status[5]) in order of first occurrence, each as its first molecule's scaffold.  Two scaffolds
+ * are one entry when they are isomorphic (node rows and edge cells preserved); candidates are grouped by a 64-bit
+ * colour-refinement hash and every match is confirmed by gib_scaffold_first's embedding search (same atom and bond
+ * counts), never by the hash.  A search needing more than `budget` nodes raises GIB_PP_MATCH_BUDGET.
+ * Output: ids int32 [n_molecules] (entry, -1 without a ring), keep uint8 [n_molecules, N] (kept atoms, molecule
+ * numbering); counts int64 [n_known + n_molecules] += molecules per entry; attachment uint8 [n_known + n_molecules, N]:
+ * entry atom i set to 1 when the molecule atom it maps to (the lexicographically smallest isomorphism from the entry
+ * to the molecule's scaffold) has a bond leaving the scaffold (never cleared).  status int32 [GIB_PP_STATUS_INTS]:
+ * [3] GIB_PP_* flags, [4] the first flagged molecule (INT_MAX: none), [5] new entries.  A flagged molecule's outputs
+ * are unspecified.  Limits: N <= 181, Ef * N * ceil(N / 32) <= 2048.  ws: gib_murcko_ws_bytes(d, n_molecules,
+ * n_known) bytes, may hold anything.  One warp per molecule and per table entry; the deduplication runs in rounds (each
+ * hash group's first open scaffold is compared with the group's other open ones) and reads one status word back per
+ * round: the call synchronises the stream and cannot be captured. */
+size_t gib_murcko_ws_bytes(const gib_pp_dims* d, int n_molecules, int n_known);
+int gib_murcko(const gib_pp_dims* d, const signed char* nodes, const signed char* edges, int n_molecules, int n_known,
+               signed char* table_nodes, signed char* table_edges, long long* counts, unsigned char* attachment,
+               long long budget, unsigned char* keep, int* ids, void* ws, int* status, gib_stream stream);
+
 /* ---- the likelihood of a molecule's decoding route (graphinvent_b200.graphed.RouteScorer): for every route state,
  *      p(action | state) = softmax(model(state))[action], one chunk of molecules at a time.
  * gib_route_plan: the decoding routes of a chunk, by the count / scan / route kernels of gib_preprocess_chunk (same
