@@ -35,6 +35,18 @@ constexpr int kEmitNT = 128;
 constexpr int kMaxNodeBytes = 8192;
 constexpr unsigned long long kEmpty = ~0ull;
 
+// status words (int32 [GIB_PP_STATUS_INTS], documented per entry point in gib200.h)
+constexpr int kStGroups = 0;       // gib_preprocess_chunk: groups written
+constexpr int kStOpen = 0;         // gib_murcko: items left open by the dedup round
+constexpr int kStNext = 1;         // gib_preprocess_chunk: the molecule after the last one visited
+constexpr int kStRouteFlags = 1;   // the conditional route plan: GIB_ROUTE_* flags
+constexpr int kStRows = 2;         // gib_preprocess_chunk: rows written
+constexpr int kStRouteFirst = 2;   // the conditional route plan: the first molecule with a GIB_ROUTE_* flag
+constexpr int kStFlags = 3;        // GIB_PP_* flags
+constexpr int kStFirstBad = 4;     // the first molecule with a GIB_PP_* flag
+constexpr int kStTotal = 5;        // the scan's total: the chunk's states, gib_murcko's new entries
+constexpr int kCursor = 6;         // the route fill: replays of the chunk done so far (its batch index)
+
 struct PP {
   int N, F, Ef, B;
   int nseg, seg[4];
@@ -50,30 +62,39 @@ struct WsLayout {
 
 __host__ __device__ inline size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
 
+// a workspace cut into consecutive 256-byte-aligned pieces: take(bytes) is the next piece's offset, end the total
+struct Carve {
+  size_t end = 0;
+  size_t take(size_t bytes) {
+    const size_t r = end;
+    end = align256(end + bytes);
+    return r;
+  }
+};
+
 WsLayout ws_layout(const PP& p, int max_mols, int max_rows) {
   WsLayout w{};
   w.states = (long long)max_mols * p.s_max;
   const long long window = (long long)(max_mols < p.B ? max_mols : p.B) * p.s_max;
   w.table = 1024;
   while (w.table < 2 * window) w.table <<= 1;
-  size_t o = 0;
-  auto take = [&](size_t bytes) { size_t r = o; o = align256(o + bytes); return r; };
-  w.len = take(4ull * max_mols);
-  w.n0 = take(4ull * max_mols);
-  w.off = take(4ull * (max_mols + 1));
-  w.rs = take(2ull * max_mols * p.N * p.N);
-  w.hash = take(8ull * w.states);
-  w.apd = take(4ull * w.states);
-  w.nn = take(4ull * w.states);
-  w.mol = take(4ull * w.states);
-  w.slot = take(4ull * w.states);
-  w.row_of = take(4ull * w.states);
-  w.dst = take(4ull * w.states);
-  w.own = take(4ull * w.states);
-  w.row_state = take(4ull * max_rows);
-  w.keys = take(8ull * w.table);
-  w.vals = take(4ull * w.table);
-  w.total = o;
+  Carve c;
+  w.len = c.take(4ull * max_mols);
+  w.n0 = c.take(4ull * max_mols);
+  w.off = c.take(4ull * (max_mols + 1));
+  w.rs = c.take(2ull * max_mols * p.N * p.N);
+  w.hash = c.take(8ull * w.states);
+  w.apd = c.take(4ull * w.states);
+  w.nn = c.take(4ull * w.states);
+  w.mol = c.take(4ull * w.states);
+  w.slot = c.take(4ull * w.states);
+  w.row_of = c.take(4ull * w.states);
+  w.dst = c.take(4ull * w.states);
+  w.own = c.take(4ull * w.states);
+  w.row_state = c.take(4ull * max_rows);
+  w.keys = c.take(8ull * w.table);
+  w.vals = c.take(4ull * w.table);
+  w.total = c.end;
   return w;
 }
 
@@ -152,17 +173,33 @@ __device__ __forceinline__ int warp_max(int v) {
   return v;
 }
 
-__device__ __forceinline__ void flag_bad(int* status, int flags, int m) {
-  atomicOr(&status[3], flags);
-  atomicMin(&status[4], m);
+// ---- bond cell (i, j) of the dense edges E [N, N, Ef] ---------------------------------------------------------------
+// a bond: any non-zero byte
+__device__ __forceinline__ bool has_bond(const signed char* E, int N, int Ef, int i, int j) {
+  const signed char* c = E + ((size_t)i * N + j) * Ef;
+  bool any = false;
+  for (int t = 0; t < Ef; ++t) any |= c[t] != 0;
+  return any;
+}
+// its type: the first non-zero byte's index, -1 without a bond
+__device__ __forceinline__ int bond_type(const signed char* E, int N, int Ef, int i, int j) {
+  const signed char* c = E + ((size_t)i * N + j) * Ef;
+  for (int t = 0; t < Ef; ++t)
+    if (c[t]) return t;
+  return -1;
 }
 
-// scaffold != 0 (the conditional route plan): status[2] holds the first molecule with a GIB_ROUTE_* flag, INT_MAX
+__device__ __forceinline__ void flag_bad(int* status, int flags, int m) {
+  atomicOr(&status[kStFlags], flags);
+  atomicMin(&status[kStFirstBad], m);
+}
+
+// scaffold != 0 (the conditional route plan): the first molecule with a GIB_ROUTE_* flag starts at INT_MAX
 __global__ void pp_init_kernel(int* status, unsigned long long* keys, int* vals, long long table, int scaffold) {
   if (blockIdx.x == 0 && threadIdx.x == 0) {
-    status[0] = status[1] = status[2] = status[3] = status[5] = status[6] = status[7] = 0;
-    status[4] = INT_MAX;
-    if (scaffold) status[2] = INT_MAX;
+    for (int i = 0; i < GIB_PP_STATUS_INTS; ++i) status[i] = 0;
+    status[kStFirstBad] = INT_MAX;
+    if (scaffold) status[kStRouteFirst] = INT_MAX;
   }
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < table; i += (long long)gridDim.x * blockDim.x) {
     keys[i] = kEmpty;
@@ -171,8 +208,8 @@ __global__ void pp_init_kernel(int* status, unsigned long long* keys, int* vals,
 }
 
 __device__ __forceinline__ void flag_scaffold(int* status, int flags, int m) {
-  atomicOr(&status[1], flags);
-  atomicMin(&status[2], m);
+  atomicOr(&status[kStRouteFlags], flags);
+  atomicMin(&status[kStRouteFirst], m);
 }
 
 // The comparison that defines "molecule atoms phi(0..k-1) are scaffold s": node row phi(i) equals scaffold row i in
@@ -326,7 +363,7 @@ __global__ void __launch_bounds__(1024) pp_scan_kernel(int n, const int* len, in
   }
   if (threadIdx.x == 0) {
     off[n] = carry;
-    status[5] = carry;
+    status[kStTotal] = carry;
   }
 }
 
@@ -340,7 +377,7 @@ __global__ void __launch_bounds__(32) pp_route_kernel(PP p, const signed char* _
                                                       int* mol, short* rs_all, int* status,
                                                       const int* __restrict__ ids, gib_scaffolds sc) {
   extern __shared__ __align__(16) unsigned char smem[];
-  if (status[3]) return;
+  if (status[kStFlags]) return;
   const int m = blockIdx.x, lane = threadIdx.x;
   if (ids && off[m + 1] == off[m]) return;      // refused by the count stage (GIB_ROUTE_NOT_PREFIX / _BAD_ID)
   const int sid = ids ? ids[m] : -1;
@@ -432,13 +469,9 @@ __global__ void __launch_bounds__(32) pp_route_kernel(PP p, const signed char* _
     __syncwarp();
     emit(k, a);
   }
-  if (ids) {
-    for (int q = lane; q < N * N; q += 32) {
-      bool any = false;
-      for (int t = 0; t < Ef; ++t) any |= E[(size_t)q * Ef + t] != 0;
-      if (any) rs[q] = SHRT_MAX;
-    }
-  }
+  if (ids)
+    for (int q = lane; q < N * N; q += 32)
+      if (has_bond(E, N, Ef, q / N, q % N)) rs[q] = SHRT_MAX;
 }
 
 // ---- exact comparison of two states (one warp; every lane gets the answer) --------------------------------------
@@ -540,9 +573,9 @@ __global__ void __launch_bounds__(kGroupNT) pp_group_kernel(PP p, StateRef S, in
   __shared__ int prev[kGroupNT];
   __shared__ int cut_sm;
   const int tid = threadIdx.x, lane = tid & 31;
-  if (status[3]) {
+  if (status[kStFlags]) {
     __syncthreads();
-    if (tid == 0) status[0] = status[1] = status[2] = 0;
+    if (tid == 0) status[kStGroups] = status[kStNext] = status[kStRows] = 0;
     return;
   }
   const int B = p.B;
@@ -642,9 +675,9 @@ __global__ void __launch_bounds__(kGroupNT) pp_group_kernel(PP p, StateRef S, in
     __syncthreads();
   }
   if (tid == 0) {
-    status[0] = ng;
-    status[1] = s;
-    status[2] = rows_used;
+    status[kStGroups] = ng;
+    status[kStNext] = s;
+    status[kStRows] = rows_used;
   }
 }
 
@@ -652,7 +685,7 @@ __global__ void __launch_bounds__(kGroupNT) pp_group_kernel(PP p, StateRef S, in
 __global__ void __launch_bounds__(kEmitNT) pp_emit_kernel(PP p, StateRef S, const int* row_state, const int* status,
                                                           signed char* out_nodes, signed char* out_edges,
                                                           int* out_apds) {
-  const int rows = status[2];
+  const int rows = status[kStRows];
   const int N = p.N, F = p.F, Ef = p.Ef;
   for (int r = blockIdx.x; r < rows; r += gridDim.x) {
     const int i = row_state[r];
@@ -671,7 +704,7 @@ __global__ void __launch_bounds__(kEmitNT) pp_emit_kernel(PP p, StateRef S, cons
 
 __global__ void pp_scatter_kernel(PP p, const int* off, const int* apd, const int* dst, const int* own,
                                   const int* status, int* out_apds) {
-  const int n = off[status[1]];
+  const int n = off[status[kStNext]];
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
     const int a = apd[i], d = dst[i], o = own[i];
     if (d >= 0) atomicAdd(&out_apds[(size_t)d * p.apd_len + a], 1);
@@ -711,7 +744,6 @@ int launch_route(const PP& p, const signed char* nodes, const signed char* edges
 // states into the model's static int8 inputs, the per-molecule reduction ----------------------------------------
 constexpr int kFillNT = 256;
 constexpr int kFillMaxBlocks = 4096;
-constexpr int kCursor = 6;      // status word: replays of the chunk done so far (the fill's batch index)
 
 struct RouteWs {
   size_t len, n0, rs, hash, apd, nn, mol, total;
@@ -720,16 +752,15 @@ struct RouteWs {
 RouteWs route_ws_layout(const PP& p, int max_mols) {
   RouteWs w{};
   const long long states = (long long)max_mols * p.s_max;
-  size_t o = 0;
-  auto take = [&](size_t bytes) { size_t r = o; o = align256(o + bytes); return r; };
-  w.len = take(4ull * max_mols);
-  w.n0 = take(4ull * max_mols);
-  w.rs = take(2ull * max_mols * p.N * p.N);
-  w.hash = take(8ull * states);
-  w.apd = take(4ull * states);
-  w.nn = take(4ull * states);
-  w.mol = take(4ull * states);
-  w.total = o;
+  Carve c;
+  w.len = c.take(4ull * max_mols);
+  w.n0 = c.take(4ull * max_mols);
+  w.rs = c.take(2ull * max_mols * p.N * p.N);
+  w.hash = c.take(8ull * states);
+  w.apd = c.take(4ull * states);
+  w.nn = c.take(4ull * states);
+  w.mol = c.take(4ull * states);
+  w.total = c.end;
   return w;
 }
 
@@ -798,7 +829,7 @@ __global__ void __launch_bounds__(kFillNT) route_fill_kernel(PP p, FillSrc f, co
                                                              long long node_chunks, long long edge_chunks,
                                                              const int* __restrict__ ids, int* __restrict__ slot_ids,
                                                              int* __restrict__ slot_n) {
-  const int B = p.B, S = status[5], s0 = status[kCursor] * B;
+  const int B = p.B, S = status[kStTotal], s0 = status[kCursor] * B;
   const long long tid = (long long)blockIdx.x * kFillNT + threadIdx.x, stride = (long long)gridDim.x * kFillNT;
   if (tid == 0) ctl->live = max(0, min(B, S - s0));
   for (long long b = tid; b < B; b += stride) {
@@ -869,6 +900,36 @@ __global__ void __launch_bounds__(32 * kCoefWarps) route_grad_coef_kernel(int n,
   }
 }
 
+// the action mask's rule on the planned routes: one warp per molecule.  Every kept state's action against the structural
+// rule with its state's atom count -- a route state never holds the bond its connect adds, so the duplicate-bond test
+// has nothing to find -- and, with valence, every atom of the whole molecule (state 0 of the plan: valences only grow
+// along a route, so its states are all within the table exactly when the molecule is)
+__global__ void __launch_bounds__(32) route_action_check_kernel(ActionLayout L, int F, const int* __restrict__ off,
+                                                                const int* __restrict__ apd,
+                                                                const int* __restrict__ nn,
+                                                                const signed char* __restrict__ nodes,
+                                                                const signed char* __restrict__ edges, int valence,
+                                                                const int* __restrict__ table, int* result) {
+  const int m = blockIdx.x, lane = threadIdx.x, N = L.N;
+  const int s0 = off[m], s1 = off[m + 1];
+  if (s1 == s0) return;                       // refused by the plan (GIB_ROUTE_NOT_PREFIX / _BAD_ID)
+  bool bad = false;
+  for (int s = s0 + lane; s < s1; s += 32) bad |= structure_forbidden(decode_action(apd[s], L), L, nn[s], 0.f);
+  if (valence) {
+    const int* order = table + L.A * L.CH;
+    const int n = min(max(nn[s0], 0), N);
+    for (int i = lane; i < n; i += 32) {
+      const int2 u = atom_usage(nodes + ((size_t)m * N + i) * F, edges + (((size_t)m * N + i) * N) * L.Ef, L, table,
+                                order, order + L.Ef);
+      bad |= u.x > u.y;
+    }
+  }
+  if (__any_sync(0xffffffffu, bad) && lane == 0) {
+    atomicOr(&result[0], GIB_ROUTE_ACTION);
+    atomicMin(&result[1], m);
+  }
+}
+
 bool aligned16(const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15) == 0; }
 
 int route_limits(const char* who, const gib_pp_dims* d, int max_molecules, PP* p) {
@@ -881,6 +942,76 @@ int route_limits(const char* who, const gib_pp_dims* d, int max_molecules, PP* p
   return 0;
 }
 
+// the scaffold table of the conditional route plan and of gib_scaffold_first
+int check_scaffolds(const char* who, const gib_scaffolds* sc, const PP& p) {
+  if (!sc || sc->S <= 0 || !sc->nodes || !sc->edges || !sc->n_atoms) {
+    set_error("%s: the scaffold table needs S >= 1 and its nodes, edges and n_atoms buffers", who);
+    return -1;
+  }
+  if (sc->protect && p.N > 127) {     // protect holds 4 x 32 bits per scaffold, as the generator's mask reads it
+    set_error("%s: attachment points need N <= 127 (4 protect words per scaffold), got N=%d", who, p.N);
+    return -1;
+  }
+  return 0;
+}
+
+// gib_route_plan (sc, ids null), and with conditional set gib_route_plan_scaffold
+int route_plan(const char* who, const gib_pp_dims* d, const signed char* nodes, const signed char* edges,
+               int n_molecules, int max_molecules, bool conditional, const gib_scaffolds* sc, const int* ids,
+               void* ws, int* offsets, int* status, gib_stream stream) {
+  PP p;
+  GIB_TRY(route_limits(who, d, max_molecules, &p));
+  if (n_molecules < 1 || n_molecules > max_molecules) {
+    set_error("%s: n_molecules %d outside [1, max_molecules = %d]", who, n_molecules, max_molecules);
+    return -1;
+  }
+  if (!nodes || !edges || !ws || !offsets || !status || (conditional && !ids)) {
+    set_error("%s: null argument", who);
+    return -1;
+  }
+  if (conditional) GIB_TRY(check_scaffolds(who, sc, p));
+  const RouteWs w = route_ws_layout(p, max_molecules);
+  char* b = static_cast<char*>(ws);
+  cudaStream_t s = (cudaStream_t)stream;
+  pp_init_kernel<<<1, 32, 0, s>>>(status, nullptr, nullptr, 0, conditional);
+  GIB_LAUNCH_CHECK();
+  return launch_route(p, nodes, edges, n_molecules,
+                      RouteBufs{(int*)(b + w.len), (int*)(b + w.n0), offsets, (short*)(b + w.rs),
+                                (unsigned long long*)(b + w.hash), (int*)(b + w.apd), (int*)(b + w.nn),
+                                (int*)(b + w.mol)},
+                      status, s, ids, sc);
+}
+
+// gib_route_fill (ids, slot_ids, slot_n null), and with conditional set gib_route_fill_scaffold
+int route_fill(const char* who, const gib_pp_dims* d, const signed char* nodes, const signed char* edges,
+               int max_molecules, const void* ws, const int* offsets, const int* status, bool conditional,
+               const int* ids, gib_batch_ctl* ctl, int* slots, int* slot_ids, int* slot_n, signed char* out_nodes,
+               signed char* out_edges, gib_stream stream) {
+  PP p;
+  GIB_TRY(route_limits(who, d, max_molecules, &p));
+  if (!nodes || !edges || !ws || !offsets || !status || !ctl || !slots || !out_nodes || !out_edges ||
+      (conditional && (!ids || !slot_ids || !slot_n))) {
+    set_error("%s: null argument", who);
+    return -1;
+  }
+  if (!aligned16(nodes) || !aligned16(edges) || !aligned16(out_nodes) || !aligned16(out_edges)) {
+    set_error("%s: nodes, edges, out_nodes and out_edges must be 16-byte aligned", who);
+    return -1;
+  }
+  const RouteWs w = route_ws_layout(p, max_molecules);
+  const char* b = static_cast<const char*>(ws);
+  const FillSrc f{nodes, edges, offsets, (const int*)(b + w.nn), (const int*)(b + w.mol), (const int*)(b + w.apd),
+                  (const short*)(b + w.rs)};
+  const long long nc = ceil_div_ll((long long)p.B * p.N * p.F, 16);
+  const long long ec = ceil_div_ll((long long)p.B * p.N * p.N * p.Ef, 16);
+  const long long need = std::max<long long>(ceil_div_ll(nc + ec, kFillNT), ceil_div_ll(p.B, kFillNT));
+  const int blocks = (int)std::min<long long>(need, kFillMaxBlocks);
+  route_fill_kernel<<<blocks, kFillNT, 0, (cudaStream_t)stream>>>(
+      p, f, status, ctl, slots, out_nodes, out_edges, nc, ec, ids, slot_ids, slot_n);
+  GIB_LAUNCH_CHECK();
+  return 0;
+}
+
 // ---- node_remap (MolecularGraph.py:435-461, 328-433, 592-614): one warp per molecule -------------------------------
 // The BFS / DFS of the reference from atom ranking[0], then reorder_nodes.  Adjacency bitsets and the ranking live in
 // shared memory; the search runs on lane 0 and the reordered bytes are written by the whole warp.
@@ -888,6 +1019,70 @@ constexpr int kReorderMaxN = 181;                           // N*N*Ef <= 32768
 constexpr int kReorderWords = (kReorderMaxN + 31) / 32;
 constexpr int kSetMaxSlots = 512;                           // the table of a set of <= 306 small ints (CPython 3.12)
 constexpr int kSetLinearProbes = 9, kSetPerturbShift = 5;   // Objects/setobject.c
+
+// ---- per-molecule graph helpers of the one-warp-per-molecule kernels below -------------------------------------------
+// The bonds among atoms 0..n-1 of E as bitsets, bit j of row i (one warp): `any` [N][kReorderWords] every bond, and
+// `typed` [Ef][N][ceil(N / 32)] each bond under its bond_type; either may be null.  The N atoms' rows are cleared
+// first.  Returns this lane's count of bonded cells (i, j).
+__device__ int load_adjacency(const signed char* E, int N, int Ef, int n, unsigned (*any)[kReorderWords],
+                              unsigned* typed) {
+  const int lane = threadIdx.x & 31, W = (N + 31) / 32;
+  if (any)
+    for (int q = lane; q < N * W; q += 32) any[q / W][q % W] = 0;
+  if (typed)
+    for (int q = lane; q < Ef * N * W; q += 32) typed[q] = 0;
+  __syncwarp();
+  int cells = 0;
+  for (int q = lane; q < n * n; q += 32) {
+    const int i = q / n, j = q % n, t = bond_type(E, N, Ef, i, j);
+    if (t < 0) continue;
+    ++cells;
+    if (any) atomicOr(&any[i][j >> 5], 1u << (j & 31));
+    if (typed) atomicOr(&typed[((size_t)t * N + i) * W + (j >> 5)], 1u << (j & 31));
+  }
+  __syncwarp();
+  return cells;
+}
+
+// deg[i] = atom i's bonds among atoms 0..k-1 (0 for i >= k), i < N (one warp); returns their bonds (every lane)
+__device__ int prefix_degrees(const signed char* E, int N, int Ef, int k, short* deg) {
+  int total = 0;
+  for (int i = threadIdx.x & 31; i < N; i += 32) {
+    int d = 0;
+    for (int j = 0; j < k && i < k; ++j) d += has_bond(E, N, Ef, i, j);
+    deg[i] = (short)d;
+    total += d;
+  }
+  return warp_sum(total) / 2;
+}
+
+// lane 0: how many atoms the bitset rows adj reach from `start` (start included), frontier by frontier
+__device__ int reach(const unsigned (*adj)[kReorderWords], int W, int start) {
+  unsigned vis[kReorderWords], front[kReorderWords];
+#pragma unroll
+  for (int w = 0; w < kReorderWords; ++w) vis[w] = front[w] = w == start >> 5 ? 1u << (start & 31) : 0u;
+  int count = 1;
+  for (bool grew = true; grew;) {
+    unsigned next[kReorderWords] = {};
+#pragma unroll
+    for (int w = 0; w < kReorderWords; ++w)
+      for (unsigned b = front[w]; b; b &= b - 1) {
+        const int a = w * 32 + __ffs(b) - 1;
+#pragma unroll
+        for (int v = 0; v < kReorderWords; ++v)
+          if (v < W) next[v] |= adj[a][v];
+      }
+    grew = false;
+#pragma unroll
+    for (int w = 0; w < kReorderWords; ++w) {
+      front[w] = next[w] & ~vis[w];
+      vis[w] |= front[w];
+      count += __popc(front[w]);
+      grew |= front[w] != 0;
+    }
+  }
+  return count;
+}
 
 // CPython 3.12's set table for small non-negative ints (hash = value, no deletions): set_add_entry's probe sequence
 // (LINEAR_PROBES slots after the home slot while they fit, then perturbation), set_table_resize on the fill rule
@@ -1027,42 +1222,24 @@ __global__ void __launch_bounds__(32) reorder_kernel(PP p, const signed char* __
   const signed char* X = nodes + (size_t)m * N * F;
   const signed char* E = edges + (size_t)m * N * N * Ef;
   int* R = rankings + (size_t)m * N;
-  for (int q = lane; q < N * W; q += 32) adj[q / W][q % W] = 0;
   if (lane < W) seen[lane] = 0;
   if (lane == 0) ok = n > 0;
-  __syncwarp();
-  for (int q = lane; q < n * n; q += 32) {
-    const int i = q / n, j = q % n;
-    bool any = false;
-    for (int t = 0; t < Ef; ++t) any |= E[((size_t)i * N + j) * Ef + t] != 0;
-    if (any) atomicOr(&adj[i][j >> 5], 1u << (j & 31));
-  }
+  load_adjacency(E, N, Ef, n, adj, nullptr);
   if (!load_ranking(N, n, draw, seed, epoch, first, m, R, rank, key, seen, status) && lane == 0) ok = 0;
   __syncwarp();
   if (lane == 0 && ok) {
-    unsigned* vis = seen;                                   // reused: the visited set
-    for (int w = 0; w < W; ++w) vis[w] = 0;
     const int start = rank[0];                              // node_init = atom_ranking[0]
     // connectivity first: both reference searches loop forever on a disconnected graph
-    int count = 1;
-    ord[0] = start;
-    vis[start >> 5] |= 1u << (start & 31);
-    for (int k = 0; k < count; ++k)
-      for (int w = 0; w < W; ++w)
-        for (unsigned b = adj[ord[k]][w] & ~vis[w]; b; b &= b - 1) {
-          const int a = w * 32 + __ffs(b) - 1;
-          vis[w] |= 1u << (a & 31);
-          ord[count++] = a;
-        }
-    if (count != n) {
+    if (reach(adj, W, start) != n) {
       flag_bad(status, GIB_PP_DISCONNECTED, m);
       ok = 0;
     } else {
+      unsigned* vis = seen;                                 // reused: the visited set
       for (int w = 0; w < W; ++w) vis[w] = 0;
       vis[start >> 5] |= 1u << (start & 31);
       ord[0] = start;
       pos[start] = 0;
-      count = 1;
+      int count = 1;
       unsigned cand[kReorderWords];
       if (route == 0) {
         // breadth_first_search: per layer, each last-layer atom's unvisited neighbours by falling rank into one set;
@@ -1124,22 +1301,10 @@ constexpr int kMatchAdjWords = 2048;     // Ef * N * ceil(N / 32) words of per-b
 
 // per scaffold s (one warp each): deg[s, i] = scaffold atom i's bonds (0 past k_s), bonds[s] = its bonds in all
 __global__ void __launch_bounds__(32) scaffold_degree_kernel(PP p, gib_scaffolds sc, short* deg, int* bonds) {
-  const int s = blockIdx.x, lane = threadIdx.x, N = p.N, Ef = p.Ef;
+  const int s = blockIdx.x, N = p.N, Ef = p.Ef;
   const int k = min(max(sc.n_atoms[s], 0), N);
-  const signed char* SE = sc.edges + (size_t)s * N * N * Ef;
-  int total = 0;
-  for (int i = lane; i < N; i += 32) {
-    int d = 0;
-    for (int j = 0; j < k && i < k; ++j) {
-      bool any = false;
-      for (int t = 0; t < Ef; ++t) any |= SE[((size_t)i * N + j) * Ef + t] != 0;
-      d += any;
-    }
-    deg[(size_t)s * N + i] = (short)d;
-    total += d;
-  }
-  total = warp_sum(total);
-  if (lane == 0) bonds[s] = total / 2;
+  const int b = prefix_degrees(sc.edges + (size_t)s * N * N * Ef, N, Ef, k, deg + (size_t)s * N);
+  if (threadIdx.x == 0) bonds[s] = b;
 }
 
 // lane 0: the layered breadth-first search from ord[0, c) (marked in vis): layer L + 1 is the unvisited neighbours of
@@ -1179,9 +1344,7 @@ __device__ void match_candidates(const PP& p, MatchSmem& S, const signed char* S
 #pragma unroll
   for (int w = 0; w < kReorderWords; ++w) acc[w] = ~0u;
   for (int j = lane; j < i; j += 32) {
-    int t = -1;
-    for (int u = Ef - 1; u >= 0; --u)
-      if (SE[((size_t)i * N + j) * Ef + u]) t = u;
+    const int t = bond_type(SE, N, Ef, i, j);
     const int a = S.phi[j];
     const unsigned* nb = t >= 0 ? S.adj + ((size_t)t * N + a) * W : S.any[a];
 #pragma unroll
@@ -1198,30 +1361,15 @@ __device__ void match_candidates(const PP& p, MatchSmem& S, const signed char* S
 // the molecule side of match_scaffold for the graph E of n atoms: S.adj, S.any and S.mdeg.  Returns the degree sum
 // (every lane).
 __device__ int match_load(const PP& p, MatchSmem& S, const signed char* E, int n) {
-  const int lane = threadIdx.x & 31, N = p.N, Ef = p.Ef, W = (N + 31) / 32;
-  for (int q = lane; q < Ef * N * W; q += 32) S.adj[q] = 0;
-  for (int q = lane; q < N * W; q += 32) S.any[q / W][q % W] = 0;
-  __syncwarp();
-  for (int q = lane; q < n * n; q += 32) {
-    const int i = q / n, j = q % n;
-    bool any = false;
-    for (int t = 0; t < Ef; ++t)
-      if (E[((size_t)i * N + j) * Ef + t]) {
-        atomicOr(&S.adj[((size_t)t * N + i) * W + (j >> 5)], 1u << (j & 31));
-        any = true;
-      }
-    if (any) atomicOr(&S.any[i][j >> 5], 1u << (j & 31));
-  }
-  __syncwarp();
-  int deg_sum = 0;
+  const int lane = threadIdx.x & 31, W = (p.N + 31) / 32;
+  const int deg_sum = warp_sum(load_adjacency(E, p.N, p.Ef, n, S.any, S.adj));
   for (int i = lane; i < n; i += 32) {
     int d = 0;
     for (int w = 0; w < W; ++w) d += __popc(S.any[i][w]);
     S.mdeg[i] = (short)d;
-    deg_sum += d;
   }
   __syncwarp();
-  return warp_sum(deg_sum);
+  return deg_sum;
 }
 
 // the smallest embedding of scaffold s (k atoms) in the molecule (X, E, n atoms) into S.phi: 1 found, 0 none, -1 the
@@ -1301,15 +1449,10 @@ __global__ void __launch_bounds__(32) scaffold_first_kernel(
   if (!load_ranking(N, n, draw, seed, epoch, first, m, rankings + (size_t)m * N, rank, key, seen, status) && lane == 0)
     ok = 0;
   __syncwarp();
-  // connectivity first, as gib_reorder checks it: the layers from atom 0 must reach every atom
-  if (lane == 0 && ok) {
-    for (int w = 0; w < W; ++w) seen[w] = 0;
-    seen[0] = 1u;
-    ord[0] = 0;
-    if (layered_bfs(S.any, W, rank, seen, ord, 1) != n) {
-      flag_bad(status, GIB_PP_DISCONNECTED, m);
-      ok = 0;
-    }
+  // connectivity first, as gib_reorder checks it: atom 0 must reach every atom
+  if (lane == 0 && ok && reach(S.any, W, 0) != n) {
+    flag_bad(status, GIB_PP_DISCONNECTED, m);
+    ok = 0;
   }
   __syncwarp();
   int sid = -1;
@@ -1397,31 +1540,24 @@ __global__ void __launch_bounds__(32) murcko_kernel(PP p, const signed char* __r
   const int n = n0[m];
   const signed char* X = nodes + (size_t)m * N * F;
   const signed char* E = edges + (size_t)m * N * N * Ef;
-  for (int q = lane; q < N * W; q += 32) adj[q / W][q % W] = dbl[q / W][q % W] = 0;
+  for (int q = lane; q < N * W; q += 32) dbl[q / W][q % W] = 0;
   for (int i = lane; i < N; i += 32) rank[i] = N - i;      // layered_bfs takes the highest rank first
   if (lane < W) alive[lane] = keep[lane] = 0;
   if (lane == 0) {
     ok = n > 0 && !bad[m];
     k = 0;
   }
-  __syncwarp();
-  for (int q = lane; q < n * n; q += 32) {
-    const int i = q / n, j = q % n;
-    bool any = false;
-    for (int t = 0; t < Ef; ++t) any |= E[((size_t)i * N + j) * Ef + t] != 0;
-    if (any) atomicOr(&adj[i][j >> 5], 1u << (j & 31));
-    if (Ef > 1 && E[((size_t)i * N + j) * Ef + 1]) atomicOr(&dbl[i][j >> 5], 1u << (j & 31));
-  }
+  load_adjacency(E, N, Ef, n, adj, nullptr);
+  if (Ef > 1)
+    for (int q = lane; q < n * n; q += 32) {
+      const int i = q / n, j = q % n;
+      if (E[((size_t)i * N + j) * Ef + 1]) atomicOr(&dbl[i][j >> 5], 1u << (j & 31));
+    }
   for (int a = lane; a < n; a += 32) atomicOr(&alive[a >> 5], 1u << (a & 31));
   __syncwarp();
-  if (lane == 0 && ok) {                                    // connectivity, as gib_reorder checks it
-    for (int w = 0; w < W; ++w) vis[w] = 0;
-    vis[0] = 1u;
-    ord[0] = 0;
-    if (layered_bfs(adj, W, rank, vis, ord, 1) != n) {
-      flag_bad(status, GIB_PP_DISCONNECTED, m);
-      ok = 0;
-    }
+  if (lane == 0 && ok && reach(adj, W, 0) != n) {          // connectivity, as gib_reorder checks it
+    flag_bad(status, GIB_PP_DISCONNECTED, m);
+    ok = 0;
   }
   __syncwarp();
   if (ok) {
@@ -1501,19 +1637,7 @@ __global__ void __launch_bounds__(32) murcko_hash_kernel(PP p, MurckoItems it, i
     if (any) last = r;
   }
   const int k = warp_max(last) + 1;
-  for (int q = lane; q < Ef * N * W; q += 32) adj[q] = 0;
-  __syncwarp();
-  int nnz = 0;
-  for (int q = lane; q < k * k; q += 32) {
-    const int a = q / k, b = q % k;
-    for (int t = 0; t < Ef; ++t)
-      if (E[((size_t)a * N + b) * Ef + t]) {
-        atomicOr(&adj[((size_t)t * N + a) * W + (b >> 5)], 1u << (b & 31));
-        ++nnz;
-        break;
-      }
-  }
-  const int bonds = warp_sum(nnz) / 2;
+  const int bonds = warp_sum(load_adjacency(E, N, Ef, k, nullptr, adj)) / 2;
   for (int a = lane; a < k; a += 32) {
     unsigned long long h = 0;
     for (int f = 0; f < F; ++f) h += byte_hash(f, X[(size_t)a * F + f]);
@@ -1547,11 +1671,11 @@ __global__ void __launch_bounds__(32) murcko_hash_kernel(PP p, MurckoItems it, i
 }
 
 // one dedup round, part 1: each hash bucket's smallest open item becomes its representative this round (atomicMax of
-// (round, ~item): buckets need no reset between rounds).  Clears the round's open counter, status[0].
+// (round, ~item): buckets need no reset between rounds).  Clears the round's open counter.
 __global__ void murcko_select_kernel(int items, int round, const int* __restrict__ rep, const int* __restrict__ slot,
                                      unsigned long long* bucket, int* status) {
   const int t = blockIdx.x * blockDim.x + threadIdx.x;
-  if (t == 0) status[0] = 0;
+  if (t == 0) status[kStOpen] = 0;
   for (int i = t; i < items; i += gridDim.x * blockDim.x)
     if (rep[i] == kItemOpen)
       atomicMax(&bucket[slot[i]], (unsigned long long)round << 32 | (0xffffffffu - (unsigned)i));
@@ -1581,15 +1705,7 @@ __global__ void __launch_bounds__(32) murcko_match_kernel(PP p, MurckoItems it, 
   } else if (ph && item_k[r] == k && item_bonds[r] == item_bonds[i]) {
     const signed char* RE = it.E(p, r);
     match_load(p, S, it.E(p, i), k);
-    for (int a = lane; a < N; a += 32) {
-      int d = 0;
-      for (int b = 0; b < k && a < k; ++b) {
-        bool any = false;
-        for (int t = 0; t < Ef; ++t) any |= RE[((size_t)a * N + b) * Ef + t] != 0;
-        d += any;
-      }
-      rdeg[a] = (short)d;
-    }
+    prefix_degrees(RE, N, Ef, k, rdeg);
     __syncwarp();
     gib_scaffolds view{};
     view.nodes = it.X(p, r);
@@ -1605,7 +1721,7 @@ __global__ void __launch_bounds__(32) murcko_match_kernel(PP p, MurckoItems it, 
       rep[i] = kItemNone;
       flag_bad(status, GIB_PP_MATCH_BUDGET, i - it.K);
     } else {
-      atomicAdd(&status[0], 1);
+      atomicAdd(&status[kStOpen], 1);
     }
   }
 }
@@ -1648,10 +1764,7 @@ __global__ void __launch_bounds__(32) murcko_emit_kernel(PP p, MurckoItems it, c
   const short* ph = phi + (size_t)m * N;
   for (int q = lane; q < k * n; q += 32) {
     const int i = q / n, b = q % n, a = o[ph[i]];
-    if (kp[b]) continue;
-    bool any = false;
-    for (int t = 0; t < Ef; ++t) any |= E[((size_t)a * N + b) * Ef + t] != 0;
-    if (any) attach[(size_t)id * N + i] = 1;
+    if (!kp[b] && has_bond(E, N, Ef, a, b)) attach[(size_t)id * N + i] = 1;
   }
 }
 
@@ -1665,39 +1778,85 @@ MurckoWs murcko_ws_layout(const PP& p, int n, int K) {
   const long long items = (long long)n + K;
   w.table = 1024;
   while (w.table < 2 * items) w.table <<= 1;
-  size_t o = 0;
-  auto take = [&](size_t bytes) { size_t r = o; o = align256(o + bytes); return r; };
-  w.len = take(4ull * n);
-  w.n0 = take(4ull * n);
-  w.bad = take(4ull * n);
-  w.off = take(4ull * (n + 1));
-  w.sorder = take(4ull * n * p.N);
-  w.phi = take(2ull * n * p.N);
-  w.sc_nodes = take((size_t)n * p.N * p.F);
-  w.sc_edges = take((size_t)n * p.N * p.N * p.Ef);
-  w.item_k = take(4ull * items);
-  w.item_bonds = take(4ull * items);
-  w.slot = take(4ull * items);
-  w.rep = take(4ull * items);
-  w.keys = take(8ull * w.table);
-  w.bucket = take(8ull * w.table);
-  w.total = o;
+  Carve c;
+  w.len = c.take(4ull * n);
+  w.n0 = c.take(4ull * n);
+  w.bad = c.take(4ull * n);
+  w.off = c.take(4ull * (n + 1));
+  w.sorder = c.take(4ull * n * p.N);
+  w.phi = c.take(2ull * n * p.N);
+  w.sc_nodes = c.take((size_t)n * p.N * p.F);
+  w.sc_edges = c.take((size_t)n * p.N * p.N * p.Ef);
+  w.item_k = c.take(4ull * items);
+  w.item_bonds = c.take(4ull * items);
+  w.slot = c.take(4ull * items);
+  w.rep = c.take(4ull * items);
+  w.keys = c.take(8ull * w.table);
+  w.bucket = c.take(8ull * w.table);
+  w.total = c.end;
   return w;
+}
+
+// the shared-memory shapes of match_scaffold (MatchSmem), for gib_scaffold_first and gib_murcko
+int match_limits(const char* who, const PP& p) {
+  if (p.N > kReorderMaxN || (long long)p.Ef * p.N * ((p.N + 31) / 32) > kMatchAdjWords) {
+    set_error("%s: need N <= %d and Ef * N * ceil(N / 32) <= %d, got N=%d Ef=%d", who, kReorderMaxN, kMatchAdjWords,
+              p.N, p.Ef);
+    return -1;
+  }
+  return 0;
 }
 
 int murcko_limits(const char* who, const gib_pp_dims* d, int n_molecules, int n_known, PP* p) {
   GIB_TRY(make_pp(who, d, p));
-  const int W = (p->N + 31) / 32;
-  if (p->N > kReorderMaxN || (long long)p->Ef * p->N * W > kMatchAdjWords) {
-    set_error("%s: need N <= %d and Ef * N * ceil(N / 32) <= %d, got N=%d Ef=%d", who, kReorderMaxN, kMatchAdjWords,
-              p->N, p->Ef);
-    return -1;
-  }
+  GIB_TRY(match_limits(who, *p));
   if (n_molecules < 1 || n_known < 0 || (long long)n_molecules + n_known > INT_MAX / 4) {
     set_error("%s: need n_molecules >= 1, n_known >= 0 and n_molecules + n_known <= %d, got %d and %d", who,
               INT_MAX / 4, n_molecules, n_known);
     return -1;
   }
+  return 0;
+}
+
+// gib_reorder's workspace: the count stage's len and n0 [n]
+struct ReorderWs {
+  size_t len, n0, total;
+};
+
+ReorderWs reorder_ws_layout(int n) {
+  ReorderWs w{};
+  Carve c;
+  w.len = c.take(4ull * n);
+  w.n0 = c.take(4ull * n);
+  w.total = c.end;
+  return w;
+}
+
+// gib_scaffold_first's workspace: the count stage's len, n0 and bad [n], the scaffold degrees short [S, N] and bonds [S]
+struct ScaffoldFirstWs {
+  size_t len, n0, bad, sdeg, sbonds, total;
+};
+
+ScaffoldFirstWs scaffold_first_ws_layout(const PP& p, int n, int S) {
+  ScaffoldFirstWs w{};
+  Carve c;
+  w.len = c.take(4ull * n);
+  w.n0 = c.take(4ull * n);
+  w.bad = c.take(4ull * n);
+  w.sdeg = c.take(2ull * S * p.N);
+  w.sbonds = c.take(4ull * S);
+  w.total = c.end;
+  return w;
+}
+
+// the status words reset, then pp_count_kernel's validation of n molecules: len, n0 and, when bad != null, each
+// molecule's GIB_PP_* flags
+int launch_count(const PP& p, const signed char* nodes, const signed char* edges, int n, int* len, int* n0, int* bad,
+                 int* status, cudaStream_t s) {
+  pp_init_kernel<<<1, 32, 0, s>>>(status, nullptr, nullptr, 0, 0);
+  GIB_LAUNCH_CHECK();
+  pp_count_kernel<<<n, 32, 0, s>>>(p, nodes, edges, len, n0, status, nullptr, gib_scaffolds{}, bad);
+  GIB_LAUNCH_CHECK();
   return 0;
 }
 
@@ -1789,26 +1948,8 @@ long long gib_route_max_states(const gib_pp_dims* d, int max_molecules) {
 
 int gib_route_plan(const gib_pp_dims* d, const signed char* nodes, const signed char* edges, int n_molecules,
                    int max_molecules, void* ws, int* offsets, int* status, gib_stream stream) {
-  PP p;
-  GIB_TRY(route_limits("gib_route_plan", d, max_molecules, &p));
-  if (n_molecules < 1 || n_molecules > max_molecules) {
-    set_error("gib_route_plan: n_molecules %d outside [1, max_molecules = %d]", n_molecules, max_molecules);
-    return -1;
-  }
-  if (!nodes || !edges || !ws || !offsets || !status) {
-    set_error("gib_route_plan: null argument");
-    return -1;
-  }
-  const RouteWs w = route_ws_layout(p, max_molecules);
-  char* b = static_cast<char*>(ws);
-  cudaStream_t s = (cudaStream_t)stream;
-  pp_init_kernel<<<1, 32, 0, s>>>(status, nullptr, nullptr, 0, 0);
-  GIB_LAUNCH_CHECK();
-  return launch_route(p, nodes, edges, n_molecules,
-                      RouteBufs{(int*)(b + w.len), (int*)(b + w.n0), offsets, (short*)(b + w.rs),
-                                (unsigned long long*)(b + w.hash), (int*)(b + w.apd), (int*)(b + w.nn),
-                                (int*)(b + w.mol)},
-                      status, s);
+  return route_plan("gib_route_plan", d, nodes, edges, n_molecules, max_molecules, false, nullptr, nullptr, ws, offsets,
+                    status, stream);
 }
 
 int gib_test_route_plan_offsets(const gib_pp_dims* d, int max_molecules, long long* out) {
@@ -1829,120 +1970,23 @@ int gib_test_route_plan_offsets(const gib_pp_dims* d, int max_molecules, long lo
 int gib_route_fill(const gib_pp_dims* d, const signed char* nodes, const signed char* edges, int max_molecules,
                    const void* ws, const int* offsets, const int* status, gib_batch_ctl* ctl, int* slots,
                    signed char* out_nodes, signed char* out_edges, gib_stream stream) {
-  PP p;
-  GIB_TRY(route_limits("gib_route_fill", d, max_molecules, &p));
-  if (!nodes || !edges || !ws || !offsets || !status || !ctl || !slots || !out_nodes || !out_edges) {
-    set_error("gib_route_fill: null argument");
-    return -1;
-  }
-  if (!aligned16(nodes) || !aligned16(edges) || !aligned16(out_nodes) || !aligned16(out_edges)) {
-    set_error("gib_route_fill: nodes, edges, out_nodes and out_edges must be 16-byte aligned");
-    return -1;
-  }
-  const RouteWs w = route_ws_layout(p, max_molecules);
-  const char* b = static_cast<const char*>(ws);
-  const FillSrc f{nodes, edges, offsets, (const int*)(b + w.nn), (const int*)(b + w.mol), (const int*)(b + w.apd),
-                  (const short*)(b + w.rs)};
-  const long long nc = ceil_div_ll((long long)p.B * p.N * p.F, 16);
-  const long long ec = ceil_div_ll((long long)p.B * p.N * p.N * p.Ef, 16);
-  const long long need = std::max<long long>(ceil_div_ll(nc + ec, kFillNT), ceil_div_ll(p.B, kFillNT));
-  const int blocks = (int)std::min<long long>(need, kFillMaxBlocks);
-  route_fill_kernel<<<blocks, kFillNT, 0, (cudaStream_t)stream>>>(p, f, status, ctl, slots, out_nodes, out_edges, nc,
-                                                                  ec, nullptr, nullptr, nullptr);
-  GIB_LAUNCH_CHECK();
-  return 0;
+  return route_fill("gib_route_fill", d, nodes, edges, max_molecules, ws, offsets, status, false, nullptr, ctl, slots,
+                    nullptr, nullptr, out_nodes, out_edges, stream);
 }
 
 int gib_route_plan_scaffold(const gib_pp_dims* d, const signed char* nodes, const signed char* edges, int n_molecules,
                             int max_molecules, const gib_scaffolds* sc, const int* scaffold_ids, void* ws,
                             int* offsets, int* status, gib_stream stream) {
-  PP p;
-  GIB_TRY(route_limits("gib_route_plan_scaffold", d, max_molecules, &p));
-  if (n_molecules < 1 || n_molecules > max_molecules) {
-    set_error("gib_route_plan_scaffold: n_molecules %d outside [1, max_molecules = %d]", n_molecules, max_molecules);
-    return -1;
-  }
-  if (!nodes || !edges || !ws || !offsets || !status || !scaffold_ids) {
-    set_error("gib_route_plan_scaffold: null argument");
-    return -1;
-  }
-  if (!sc || sc->S <= 0 || !sc->nodes || !sc->edges || !sc->n_atoms) {
-    set_error("gib_route_plan_scaffold: the scaffold table needs S >= 1 and its nodes, edges and n_atoms buffers");
-    return -1;
-  }
-  if (sc->protect && p.N > 127) {     // protect holds 4 x 32 bits per scaffold, as the generator's mask reads it
-    set_error("gib_route_plan_scaffold: attachment points need N <= 127 (4 protect words per scaffold), got N=%d", p.N);
-    return -1;
-  }
-  const RouteWs w = route_ws_layout(p, max_molecules);
-  char* b = static_cast<char*>(ws);
-  cudaStream_t s = (cudaStream_t)stream;
-  pp_init_kernel<<<1, 32, 0, s>>>(status, nullptr, nullptr, 0, 1);
-  GIB_LAUNCH_CHECK();
-  return launch_route(p, nodes, edges, n_molecules,
-                      RouteBufs{(int*)(b + w.len), (int*)(b + w.n0), offsets, (short*)(b + w.rs),
-                                (unsigned long long*)(b + w.hash), (int*)(b + w.apd), (int*)(b + w.nn),
-                                (int*)(b + w.mol)},
-                      status, s, scaffold_ids, sc);
+  return route_plan("gib_route_plan_scaffold", d, nodes, edges, n_molecules, max_molecules, true, sc, scaffold_ids, ws,
+                    offsets, status, stream);
 }
 
 int gib_route_fill_scaffold(const gib_pp_dims* d, const signed char* nodes, const signed char* edges,
                             int max_molecules, const void* ws, const int* offsets, const int* status,
                             const int* scaffold_ids, gib_batch_ctl* ctl, int* slots, int* slot_ids, int* slot_n,
                             signed char* out_nodes, signed char* out_edges, gib_stream stream) {
-  PP p;
-  GIB_TRY(route_limits("gib_route_fill_scaffold", d, max_molecules, &p));
-  if (!nodes || !edges || !ws || !offsets || !status || !scaffold_ids || !ctl || !slots || !slot_ids || !slot_n ||
-      !out_nodes || !out_edges) {
-    set_error("gib_route_fill_scaffold: null argument");
-    return -1;
-  }
-  if (!aligned16(nodes) || !aligned16(edges) || !aligned16(out_nodes) || !aligned16(out_edges)) {
-    set_error("gib_route_fill_scaffold: nodes, edges, out_nodes and out_edges must be 16-byte aligned");
-    return -1;
-  }
-  const RouteWs w = route_ws_layout(p, max_molecules);
-  const char* b = static_cast<const char*>(ws);
-  const FillSrc f{nodes, edges, offsets, (const int*)(b + w.nn), (const int*)(b + w.mol), (const int*)(b + w.apd),
-                  (const short*)(b + w.rs)};
-  const long long nc = ceil_div_ll((long long)p.B * p.N * p.F, 16);
-  const long long ec = ceil_div_ll((long long)p.B * p.N * p.N * p.Ef, 16);
-  const long long need = std::max<long long>(ceil_div_ll(nc + ec, kFillNT), ceil_div_ll(p.B, kFillNT));
-  const int blocks = (int)std::min<long long>(need, kFillMaxBlocks);
-  route_fill_kernel<<<blocks, kFillNT, 0, (cudaStream_t)stream>>>(p, f, status, ctl, slots, out_nodes, out_edges, nc,
-                                                                  ec, scaffold_ids, slot_ids, slot_n);
-  GIB_LAUNCH_CHECK();
-  return 0;
-}
-
-// the action mask's rule on the planned routes: one warp per molecule.  Every kept state's action against the structural
-// rule with its state's atom count -- a route state never holds the bond its connect adds, so the duplicate-bond test
-// has nothing to find -- and, with valence, every atom of the whole molecule (state 0 of the plan: valences only grow
-// along a route, so its states are all within the table exactly when the molecule is)
-__global__ void __launch_bounds__(32) route_action_check_kernel(ActionLayout L, int F, const int* __restrict__ off,
-                                                                const int* __restrict__ apd,
-                                                                const int* __restrict__ nn,
-                                                                const signed char* __restrict__ nodes,
-                                                                const signed char* __restrict__ edges, int valence,
-                                                                const int* __restrict__ table, int* result) {
-  const int m = blockIdx.x, lane = threadIdx.x, N = L.N;
-  const int s0 = off[m], s1 = off[m + 1];
-  if (s1 == s0) return;                       // refused by the plan (GIB_ROUTE_NOT_PREFIX / _BAD_ID)
-  bool bad = false;
-  for (int s = s0 + lane; s < s1; s += 32) bad |= structure_forbidden(decode_action(apd[s], L), L, nn[s], 0.f);
-  if (valence) {
-    const int* order = table + L.A * L.CH;
-    const int n = min(max(nn[s0], 0), N);
-    for (int i = lane; i < n; i += 32) {
-      const int2 u = atom_usage(nodes + ((size_t)m * N + i) * F, edges + (((size_t)m * N + i) * N) * L.Ef, L, table,
-                                order, order + L.Ef);
-      bad |= u.x > u.y;
-    }
-  }
-  if (__any_sync(0xffffffffu, bad) && lane == 0) {
-    atomicOr(&result[0], GIB_ROUTE_ACTION);
-    atomicMin(&result[1], m);
-  }
+  return route_fill("gib_route_fill_scaffold", d, nodes, edges, max_molecules, ws, offsets, status, true, scaffold_ids,
+                    ctl, slots, slot_ids, slot_n, out_nodes, out_edges, stream);
 }
 
 int gib_route_check_actions(const gib_pp_dims* d, const signed char* nodes, const signed char* edges, int n_molecules,
@@ -1995,7 +2039,7 @@ int gib_route_grad_coef(int n_molecules, const int* offsets, const float* likeli
   return 0;
 }
 
-size_t gib_reorder_ws_bytes(int n_molecules) { return n_molecules < 1 ? 0 : 2 * align256(4ull * n_molecules); }
+size_t gib_reorder_ws_bytes(int n_molecules) { return n_molecules < 1 ? 0 : reorder_ws_layout(n_molecules).total; }
 
 int gib_draw_rankings(int n_molecules, int N, const int* n_atoms, unsigned long long seed, long long epoch,
                       long long first_molecule, int* rankings, gib_stream stream) {
@@ -2023,20 +2067,17 @@ int gib_reorder(const gib_pp_dims* d, const signed char* nodes, const signed cha
     set_error("gib_reorder: null argument");
     return -1;
   }
+  const ReorderWs w = reorder_ws_layout(n_molecules);
+  char* b = static_cast<char*>(ws);
+  int* n0 = (int*)(b + w.n0);
   cudaStream_t s = (cudaStream_t)stream;
-  int* len = static_cast<int*>(ws);
-  int* n0 = (int*)(static_cast<char*>(ws) + align256(4ull * n_molecules));
-  pp_init_kernel<<<1, 32, 0, s>>>(status, nullptr, nullptr, 0, 0);
-  GIB_LAUNCH_CHECK();
-  pp_count_kernel<<<n_molecules, 32, 0, s>>>(p, nodes, edges, len, n0, status, nullptr, gib_scaffolds{});
-  GIB_LAUNCH_CHECK();
+  GIB_TRY(launch_count(p, nodes, edges, n_molecules, (int*)(b + w.len), n0, nullptr, status, s));
   reorder_kernel<<<n_molecules, 32, 0, s>>>(p, nodes, edges, n0, route, draw, seed, epoch, first_molecule, rankings,
                                             order, out_nodes, out_edges, status);
   GIB_LAUNCH_CHECK();
   return 0;
 }
 
-// workspace: len, n0, bad [n_molecules] (the count stage), scaffold degrees short [S, N], scaffold bonds [S]
 size_t gib_scaffold_first_ws_bytes(const gib_pp_dims* d, int n_molecules, int n_scaffolds) {
   PP p;
   if (make_pp("gib_scaffold_first_ws_bytes", d, &p)) return 0;
@@ -2045,7 +2086,7 @@ size_t gib_scaffold_first_ws_bytes(const gib_pp_dims* d, int n_molecules, int n_
               n_scaffolds);
     return 0;
   }
-  return 3 * align256(4ull * n_molecules) + align256(2ull * n_scaffolds * p.N) + align256(4ull * n_scaffolds);
+  return scaffold_first_ws_layout(p, n_molecules, n_scaffolds).total;
 }
 
 int gib_scaffold_first(const gib_pp_dims* d, const signed char* nodes, const signed char* edges, int n_molecules,
@@ -2055,12 +2096,7 @@ int gib_scaffold_first(const gib_pp_dims* d, const signed char* nodes, const sig
                        gib_stream stream) {
   PP p;
   GIB_TRY(make_pp("gib_scaffold_first", d, &p));
-  const int W = (p.N + 31) / 32;
-  if (p.N > kReorderMaxN || (long long)p.Ef * p.N * W > kMatchAdjWords) {
-    set_error("gib_scaffold_first: need N <= %d and Ef * N * ceil(N / 32) <= %d, got N=%d Ef=%d", kReorderMaxN,
-              kMatchAdjWords, p.N, p.Ef);
-    return -1;
-  }
+  GIB_TRY(match_limits("gib_scaffold_first", p));
   if (n_molecules < 1 || first_molecule < 0 || budget < 1) {
     set_error("gib_scaffold_first: need n_molecules >= 1, first_molecule >= 0 and budget >= 1 (got %d, %lld, %lld)",
               n_molecules, first_molecule, budget);
@@ -2070,26 +2106,15 @@ int gib_scaffold_first(const gib_pp_dims* d, const signed char* nodes, const sig
     set_error("gib_scaffold_first: null argument");
     return -1;
   }
-  if (!sc || sc->S <= 0 || !sc->nodes || !sc->edges || !sc->n_atoms) {
-    set_error("gib_scaffold_first: the scaffold table needs S >= 1 and its nodes, edges and n_atoms buffers");
-    return -1;
-  }
-  if (sc->protect && p.N > 127) {
-    set_error("gib_scaffold_first: attachment points need N <= 127 (4 protect words per scaffold), got N=%d", p.N);
-    return -1;
-  }
-  cudaStream_t s = (cudaStream_t)stream;
+  GIB_TRY(check_scaffolds("gib_scaffold_first", sc, p));
+  const ScaffoldFirstWs w = scaffold_first_ws_layout(p, n_molecules, sc->S);
   char* b = static_cast<char*>(ws);
-  int* len = (int*)b;
-  const size_t per_mol = align256(4ull * n_molecules);
-  int* n0 = (int*)(b + per_mol);
-  int* bad = (int*)(b + 2 * per_mol);
-  short* sdeg = (short*)(b + 3 * per_mol);
-  int* sbonds = (int*)(b + 3 * per_mol + align256(2ull * sc->S * p.N));
-  pp_init_kernel<<<1, 32, 0, s>>>(status, nullptr, nullptr, 0, 0);
-  GIB_LAUNCH_CHECK();
-  pp_count_kernel<<<n_molecules, 32, 0, s>>>(p, nodes, edges, len, n0, status, nullptr, gib_scaffolds{}, bad);
-  GIB_LAUNCH_CHECK();
+  int* n0 = (int*)(b + w.n0);
+  int* bad = (int*)(b + w.bad);
+  short* sdeg = (short*)(b + w.sdeg);
+  int* sbonds = (int*)(b + w.sbonds);
+  cudaStream_t s = (cudaStream_t)stream;
+  GIB_TRY(launch_count(p, nodes, edges, n_molecules, (int*)(b + w.len), n0, bad, status, s));
   scaffold_degree_kernel<<<sc->S, 32, 0, s>>>(p, *sc, sdeg, sbonds);
   GIB_LAUNCH_CHECK();
   scaffold_first_kernel<<<n_molecules, 32, 0, s>>>(p, nodes, edges, n0, bad, *sc, sdeg, sbonds, scaffold_ids, draw,
@@ -2136,12 +2161,9 @@ int gib_murcko(const gib_pp_dims* d, const signed char* nodes, const signed char
                        (const signed char*)(b + w.sc_edges), n_known};
   const int n = n_molecules, items = n + n_known;
   cudaStream_t s = (cudaStream_t)stream;
-  pp_init_kernel<<<1, 32, 0, s>>>(status, nullptr, nullptr, 0, 0);
-  GIB_LAUNCH_CHECK();
   GIB_CUDA_TRY(cudaMemsetAsync(keys, 0xff, 8ull * w.table, s));      // kEmpty
   GIB_CUDA_TRY(cudaMemsetAsync(bucket, 0, 8ull * w.table, s));
-  pp_count_kernel<<<n, 32, 0, s>>>(p, nodes, edges, len, n0, status, nullptr, gib_scaffolds{}, bad);
-  GIB_LAUNCH_CHECK();
+  GIB_TRY(launch_count(p, nodes, edges, n, len, n0, bad, status, s));
   murcko_kernel<<<n, 32, 0, s>>>(p, nodes, edges, n0, bad, keep, sorder, (signed char*)(b + w.sc_nodes),
                                  (signed char*)(b + w.sc_edges), status);
   GIB_LAUNCH_CHECK();
@@ -2158,7 +2180,7 @@ int gib_murcko(const gib_pp_dims* d, const signed char* nodes, const signed char
     murcko_match_kernel<<<items, 32, 0, s>>>(p, it, item_k, item_bonds, slot, bucket, budget, rep, phi, status);
     GIB_LAUNCH_CHECK();
     int open = 0;
-    GIB_CUDA_TRY(cudaMemcpyAsync(&open, status, sizeof(int), cudaMemcpyDeviceToHost, s));
+    GIB_CUDA_TRY(cudaMemcpyAsync(&open, status + kStOpen, sizeof(int), cudaMemcpyDeviceToHost, s));
     GIB_CUDA_TRY(cudaStreamSynchronize(s));
     if (!open) break;
   }

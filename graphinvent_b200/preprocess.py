@@ -95,25 +95,12 @@ def groups(nodes, edges, batch_size, n_atom_types, n_formal_charge, n_imp_H=0, n
     computed on the device after each chunk and copied back with the group table."""
     nodes = np.ascontiguousarray(nodes)
     edges = np.ascontiguousarray(edges)
-    if nodes.dtype != np.int8 or edges.dtype != np.int8 or nodes.ndim != 3 or edges.ndim != 4:
-        raise ValueError("nodes / edges must be int8 [M, N, F] / [M, N, N, Ef]")
-    M, N, F = nodes.shape
-    Ef = edges.shape[3]
-    if edges.shape[:3] != (M, N, N):
-        raise ValueError(f"edges {edges.shape} do not match nodes {nodes.shape}")
-    d = PPDims(N=N, F=F, Ef=Ef, n_atom_types=n_atom_types, n_formal_charge=n_formal_charge, n_imp_H=n_imp_H,
-               n_chirality=n_chirality, batch_size=batch_size)
-    apd_len = lib.gib_preprocess_apd_length(ctypes.byref(d))
-    if apd_len < 0:
-        raise ValueError(lib.gib_last_error().decode())
+    M, N, F, Ef = _check_stacks(nodes, edges)
+    d = _pp_dims(N, F, Ef, (n_atom_types, n_formal_charge, n_imp_H, n_chirality), batch_size)
     if M == 0:
         return
     B = batch_size
-    chunk = min(max(int(chunk_molecules), B), M)
-    max_rows = max(int(max_rows or 16 * chunk), B)
-    ws_bytes = lib.gib_preprocess_ws_bytes(ctypes.byref(d), chunk, max_rows)
-    if ws_bytes == 0:
-        raise ValueError(lib.gib_last_error().decode())
+    chunk, max_rows = _chunk_sizes(d, M, chunk_molecules, max_rows)
     dev = _cuda(torch.device(device))
     in_nodes = torch.empty((chunk, N, F), dtype=torch.int8, device=dev)
     in_edges = torch.empty((chunk, N, N, Ef), dtype=torch.int8, device=dev)
@@ -213,6 +200,17 @@ def _pp_dims(N, F, Ef, layout, batch_size=1):
     return d
 
 
+def _chunk_sizes(d, M, chunk_molecules, max_rows):
+    """(chunk, max_rows) of the training-set construction over M >= 1 molecules: chunks of at least batch_size
+    molecules, max_rows at least batch_size (default 16 * chunk), checked by gib_preprocess_ws_bytes"""
+    B = d.batch_size
+    chunk = min(max(int(chunk_molecules), B), M)
+    max_rows = max(int(max_rows or 16 * chunk), B)
+    if lib.gib_preprocess_ws_bytes(ctypes.byref(d), chunk, max_rows) == 0:
+        raise ValueError(lib.gib_last_error().decode())
+    return chunk, max_rows
+
+
 def file_rows(nodes, edges, batch_size, n_atom_types, n_formal_charge, n_imp_H=0, n_chirality=0,
               chunk_molecules=4096, max_rows=None, keep=True, device="cuda"):
     """The training-set construction of `groups` with its rows left on the device: (nodes, edges, apds), int8 device
@@ -230,10 +228,7 @@ def file_rows(nodes, edges, batch_size, n_atom_types, n_formal_charge, n_imp_H=0
     d = _pp_dims(N, F, Ef, layout, batch_size)
     nodes, edges = _on_device(nodes, device), _on_device(edges, device)
     B = batch_size
-    chunk = min(max(int(chunk_molecules), B), M)
-    max_rows = max(int(max_rows or 16 * chunk), B)
-    if lib.gib_preprocess_ws_bytes(ctypes.byref(d), chunk, max_rows) == 0:
-        raise ValueError(lib.gib_last_error().decode())
+    chunk, max_rows = _chunk_sizes(d, M, chunk_molecules, max_rows)
     dev = nodes.device
     rows = None
     if keep:
