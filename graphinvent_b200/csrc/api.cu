@@ -626,7 +626,11 @@ int gib_test_dw_groups(const gib_dw_problem* qs, const int* group_sizes, int n_g
 }
 int gib_test_dw_schedule(const int* rows, const int* Nn, const int* Kk, int n, int sms, int* segs, int max_segs,
                          int* tile_ctas, int* G) {
-  return tc3_dw_schedule(rows, Nn, Kk, n, sms, segs, max_segs, tile_ctas, G);
+  return tc3_dw_schedule(rows, nullptr, Nn, Kk, n, sms, segs, 6, max_segs, tile_ctas, G);
+}
+int gib_test_dw_schedule_passes(const int* rows, const int* passes, const int* Nn, const int* Kk, int n, int sms,
+                                int* segs, int max_segs, int* tile_ctas, int* G) {
+  return tc3_dw_schedule(rows, passes, Nn, Kk, n, sms, segs, 7, max_segs, tile_ctas, G);
 }
 int gib_test_scatter_bwd(float* G, const float* dM, const float* Y, int ld, const int* dst, const float* w, int act,
                          long long P, gib_stream stream) {

@@ -62,9 +62,14 @@ struct GemmDW {
   const int* m_dev = nullptr;                         // device-side row range inside buffers of M rows (see GemmNT)
   const int* base_dev = nullptr;
   int tf32 = 0;                                       // tensor-core precision (see GemmNT)
+  // Pass extent: the reduction runs over the same row range of `passes` slices, slice t of G / X at G + t * pass_g /
+  // X + t * pass_x (elements) -- the message passes of a weight shared by every pass.  work covers all of them.
+  int passes = 1;
+  long long pass_g = 0, pass_x = 0;
 };
 
 constexpr int kTc3MaxProblems = 16;   // problems per launch of the tensor-core kernel
+constexpr int kDwMaxProblems = 32;    // members per launch of the weight-gradient tensor-core kernel
 
 // scratch layout of one grouped weight-gradient launch of the tensor-core kernel (gemm_tc3.cu): [slots][128][128]
 // partial tiles, then [slots][128] bias partials; slots = min(SMs, ceil(k-blocks / 8)) + the group's output tiles
@@ -99,8 +104,9 @@ bool tc3_dw_eligible(const GemmDW& q);
 void tc3_dw_layout(const GemmDW* qs, int n, Dw3Layout* L);
 int gemm_dw_tc3_partials(const GemmDW* qs, int n, const Dw3Layout& L, float* scratch, cudaStream_t st);
 int gemm_dw_tc3_reduce(const GemmDW* qs, int n, const Dw3Layout& L, const float* scratch, cudaStream_t st);
-int tc3_dw_schedule(const int* rows, const int* Nn, const int* Kk, int n, int sms, int* segs, int max_segs,
-                    int* tile_ctas, int* G_out);   // test hook (gib_test_dw_schedule)
+// test hook (gib_test_dw_schedule, gib_test_dw_schedule_passes): passes may be null (one pass each); seg_ints 6 or 7
+int tc3_dw_schedule(const int* rows, const int* passes, const int* Nn, const int* Kk, int n, int sms, int* segs,
+                    int seg_ints, int max_segs, int* tile_ctas, int* G_out);
 int device_sm_count();     // SMs of the current device (cached per device)
 void tc3_set_trace(long long* buf, int tiles);   // diagnosis: per-tile clock64 stamps of CTA 0
 extern bool g_use_tc;
@@ -110,8 +116,8 @@ extern int g_tc_debug;
 int check_precision(int prec, const char* who);
 
 int gemm_dw(const GemmDW& q, cudaStream_t st);
-// n <= 16 weight-gradient problems that may run as ONE grouped tensor-core launch + ONE reduction launch (siblings of a
-// layer: the per-bond-type message MLPs, the readout heads, the two GRU projections)
+// n <= kDwMaxProblems weight-gradient problems that may run as ONE grouped tensor-core launch + ONE reduction launch
+// (siblings of a layer: the per-bond-type message MLPs, the readout heads, the two GRU projections)
 int gemm_dw_group(const GemmDW* qs, int n, cudaStream_t st);
 size_t gemm_dw_group_half_floats(const GemmDW* qs, int n);
 int dw_begin();            // start of a C-ABI call that uses gemm_dw: forget the previous call's side-stream jobs

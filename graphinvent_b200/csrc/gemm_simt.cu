@@ -759,16 +759,16 @@ static int dw_tc_launch(const GemmDW* live, int nl, double work, const ProfRows*
 // grouped weight gradients: one tensor-core launch + one reduction for the members that qualify, the others one by one
 int gemm_dw_group(const GemmDW* qs, int n, cudaStream_t st) {
   if (n < 1) return 0;
-  if (n > kTc3MaxProblems) { set_error("gemm_dw_group: %d problems (max %d)", n, kTc3MaxProblems); return -2; }
+  if (n > kDwMaxProblems) { set_error("gemm_dw_group: %d problems (max %d)", n, kDwMaxProblems); return -2; }
   for (int i = 0; i < n; ++i) GIB_TRY(check_precision(qs[i].tf32, "gemm_dw_group"));
   const bool tc3 = g_use_tc && use_tc3();
   bool dyn = false;
   long long rows = 0;
   double work = 0;
-  ProfRows dyn_rows[kTc3MaxProblems];
+  ProfRows dyn_rows[kDwMaxProblems];
   int ndyn = 0;
-  GemmDW live[kTc3MaxProblems];      // members that run in the grouped tensor-core launch
-  GemmDW rest[kTc3MaxProblems];      // too small / unaligned for it: one by one
+  GemmDW live[kDwMaxProblems];       // members that run in the grouped tensor-core launch
+  GemmDW rest[kDwMaxProblems];       // too small / unaligned for it: one by one
   int nl = 0, nr = 0;
   for (int i = 0; i < n; ++i) {
     const GemmDW& q = qs[i];
@@ -784,8 +784,8 @@ int gemm_dw_group(const GemmDW* qs, int n, cudaStream_t st) {
       }
     }
     if (good) {
-      rows += q.M;
-      const double qw = q.work > 0 ? q.work : 2.0 * q.M * (double)q.R * q.C;
+      rows += (long long)q.M * q.passes;
+      const double qw = q.work > 0 ? q.work : 2.0 * q.M * (double)q.R * q.C * q.passes;
       if (q.m_dev) dyn_rows[ndyn++] = ProfRows{q.m_dev, q.base_dev, q.M, qw / q.M};   // the rows launched
       else work += qw;
       live[nl++] = q;
@@ -811,9 +811,20 @@ int gemm_dw(const GemmDW& q, cudaStream_t st) {
   }
   if (q.m_dev) return gemm_dw_group(&q, 1, st);
   // the tensor-core launch as a group of one (also under gib_tc_debug bit 0, which groups no weight gradients)
-  const double work = q.work > 0 ? q.work : 2.0 * q.M * (double)q.R * q.C;
-  if (g_use_tc && q.dW && q.M >= 2048 && q.Nn >= 32 && q.Kk >= 32 && tc3_dw_eligible(q) && q.half_floats > 0)
+  const double work = q.work > 0 ? q.work : 2.0 * q.M * (double)q.R * q.C * q.passes;
+  if (g_use_tc && q.dW && (long long)q.M * q.passes >= 2048 && q.Nn >= 32 && q.Kk >= 32 && tc3_dw_eligible(q) &&
+      q.half_floats > 0)
     return dw_tc_launch(&q, 1, work, nullptr, 0, st);
+  if (q.passes > 1) {   // the SIMT kernel has no pass extent: one call per pass, last pass first as the backward runs
+    for (int t = q.passes - 1; t >= 0; --t) {
+      GemmDW s = q;
+      s.passes = 1;
+      s.G += t * q.pass_g; s.X += t * q.pass_x;
+      s.work = work / q.passes;
+      GIB_TRY(gemm_dw(s, st));
+    }
+    return 0;
+  }
   ProfScope prof(PROF_GEMM_DW_SIMT, work, st);
   DwSide* d;
   GIB_TRY(dw_side(&d));

@@ -138,7 +138,8 @@ constexpr int DW_TR_WARPS = 3;                                 // warps 9-11
 constexpr int DW_OFF_PLANES = DW_RAW_STAGES * DW_RAW_BYTES;
 constexpr int DW_OFF_BARS = DW_OFF_PLANES + DW_PLANE_STAGES * DW_PLANE_BYTES;
 constexpr int DW_OFF_SCHED = DW_OFF_BARS + 256;
-constexpr int DW_SMEM_BYTES = DW_OFF_SCHED + 512 + 1024 /*align slack*/;
+constexpr int DW_SCHED_BYTES = 1536;
+constexpr int DW_SMEM_BYTES = DW_OFF_SCHED + DW_SCHED_BYTES + 1024 /*align slack*/;
 static_assert(DW_SMEM_BYTES <= 227 * 1024, "weight-gradient stages exceed the shared memory of an SM");
 
 constexpr int MAXP = kTc3MaxProblems;   // 16: e.g. the 5 layers x 3 bond types of a message MLP as one dependent chain
@@ -169,7 +170,7 @@ struct Sched {              // computed once per CTA from host values or the dev
   int M[MAXP], base[MAXP], begin[MAXP + 1];
 };
 
-struct Item { int p, m0, n0, nkb, z, r0, rows; };
+struct Item { int p, m0, n0, nkb, z, r0, rows, ps; };
 
 // TBN: output tile width of the kernel
 template <int TBN>
@@ -179,7 +180,7 @@ __device__ __forceinline__ Item decode_item(const Params& P, const Sched& S, int
   while (p + 1 < P.nprob && item >= S.begin[p + 1]) ++p;
   const int local = item - S.begin[p];
   it.p = p;
-  it.z = 0; it.r0 = 0; it.rows = 0;
+  it.z = 0; it.r0 = 0; it.rows = 0; it.ps = 0;
   it.m0 = (local / P.n_tiles[p]) * BM;
   it.n0 = (local % P.n_tiles[p]) * TBN;
   it.nkb = P.k_blocks[p];
@@ -187,8 +188,9 @@ __device__ __forceinline__ Item decode_item(const Params& P, const Sched& S, int
 }
 
 // ---- schedule of a weight-gradient launch: an even split of its k-blocks (stream-K) -------------------------------
-// A work unit is one k-block (32 reduction rows) of one 128 x 128 output tile of one member; units are numbered
-// member-major, then tile, then k-block, U in all.  CTA b of G = min(SMs, ceil(U / 8)) takes the units
+// A work unit is one k-block (32 reduction rows) of one pass of one 128 x 128 output tile of one member; units are
+// numbered member-major, then tile, then pass, then k-block, U in all (a member with a pass extent reduces over the same
+// rows of each of its passes' slices; a segment may cross a pass boundary and keeps one accumulator across it).  CTA b of G = min(SMs, ceil(U / 8)) takes the units
 // [floor(U b / G), floor(U (b + 1) / G)) -- at least one, about U / G -- and cuts them at tile boundaries into
 // segments.  The segment of CTA b in tile gt (tile index over the whole group) writes its partial tile to scratch slot
 // b + gt: the CTAs that cover one tile are consecutive and a CTA's tiles are consecutive, so no two segments share a
@@ -197,34 +199,42 @@ __device__ __forceinline__ Item decode_item(const Params& P, const Sched& S, int
 // shapes and the SM count only, never on a buffer's capacity: a launch on device-side row counts computes what the
 // same launch on host counts computes, bit for bit.
 constexpr int kDwMinUnits = 8;    // k-blocks per CTA at least: amortise the tile drain
+constexpr int DW_MAXP = kDwMaxProblems;   // members of one launch (the 15 message-MLP layers and the GRU pair at C2)
+
+struct DwMaps {                   // TMA descriptors of the weight-gradient kernel: G and X, boxes 32 x 32 (x 1)
+  CUtensorMap g[DW_MAXP];
+  CUtensorMap x[DW_MAXP];
+};
 
 struct DwGroup {                  // the schedule inputs of a launch, shared by the GEMM and the reduction
-  const int* m_dev[MAXP];         // device-side row count inside a buffer of M rows (nullptr: M is the count)
-  const int* base_dev[MAXP];
-  int M[MAXP];
-  int mt[MAXP], nt[MAXP];         // tiles of the output: ceil(Nn / 128) x ceil(Kk / 128)
+  const int* m_dev[DW_MAXP];         // device-side row count inside a buffer of M rows (nullptr: M is the count)
+  const int* base_dev[DW_MAXP];
+  int M[DW_MAXP];
+  int mt[DW_MAXP], nt[DW_MAXP];         // tiles of the output: ceil(Nn / 128) x ceil(Kk / 128)
+  int passes[DW_MAXP];               // slices reduced over (GemmDW::passes)
   int n, sms;
 };
 
 struct DwPlan {
   long long U;
-  long long ubegin[MAXP + 1];     // first unit of each member
-  int tbegin[MAXP + 1];           // first tile of each member
-  int M[MAXP], base[MAXP], kb[MAXP], nt[MAXP];   // live rows, first row, k-blocks per tile, column tiles
+  long long ubegin[DW_MAXP + 1];     // first unit of each member
+  int tbegin[DW_MAXP + 1];           // first tile of each member
+  int M[DW_MAXP], base[DW_MAXP], kb[DW_MAXP], nt[DW_MAXP];   // live rows, first row, k-blocks per pass, column tiles
+  int np[DW_MAXP];                   // passes
   int n, G;
 };
-static_assert(sizeof(DwPlan) <= 512, "the plan lives in the 512-byte schedule area of the kernel's shared memory");
+static_assert(sizeof(DwPlan) <= DW_SCHED_BYTES, "the plan lives in the schedule area of the kernel's shared memory");
 
 // the plan from live row counts (host: the schedule test hook; device: dw_plan_dev)
-__host__ __device__ inline void dw_plan(DwPlan& S, const int* live, const int* base, const int* mt, const int* nt, int n,
-                                        int sms) {
+__host__ __device__ inline void dw_plan(DwPlan& S, const int* live, const int* base, const int* mt, const int* nt,
+                                        const int* passes, int n, int sms) {
   long long u = 0;
   int t = 0;
   for (int p = 0; p < n; ++p) {
-    S.M[p] = live[p]; S.base[p] = base[p]; S.nt[p] = nt[p];
+    S.M[p] = live[p]; S.base[p] = base[p]; S.nt[p] = nt[p]; S.np[p] = passes[p];
     S.kb[p] = ceil_div(live[p], BKF);
     S.ubegin[p] = u; S.tbegin[p] = t;
-    u += (long long)mt[p] * nt[p] * S.kb[p];
+    u += (long long)mt[p] * nt[p] * S.kb[p] * passes[p];
     t += mt[p] * nt[p];
   }
   S.ubegin[n] = u; S.tbegin[n] = t;
@@ -245,7 +255,7 @@ __device__ inline void dw_plan_dev(const DwGroup& g, DwPlan& S) {
     }
     S.M[p] = M; S.base[p] = base;
   }
-  dw_plan(S, S.M, S.base, g.mt, g.nt, g.n, g.sms);
+  dw_plan(S, S.M, S.base, g.mt, g.nt, g.passes, g.n, g.sms);
 }
 
 // units [u0, u1) of CTA b (empty for b >= G)
@@ -258,35 +268,44 @@ __host__ __device__ inline void dw_range(const DwPlan& S, int b, long long& u0, 
 // the CTA whose range holds unit u < U
 __host__ __device__ inline int dw_owner(const DwPlan& S, long long u) { return (int)(((u + 1) * S.G - 1) / S.U); }
 
-// the segment of CTA b that starts at unit u < u1 (the end of its range): z = its scratch slot, r0 / rows = its
-// reduction rows relative to the member's first row
+// k-blocks of one output tile of member p over all its passes
+__host__ __device__ inline long long dw_tile_units(const DwPlan& S, int p) { return (long long)S.kb[p] * S.np[p]; }
+
+// the segment of CTA b that starts at unit u < u1 (the end of its range): z = its scratch slot, ps / r0 = the pass and
+// the reduction row (relative to the member's first row) of its first k-block, nkb its k-blocks (which continue into
+// the next pass at row 0); rows = its reduction rows when it stays inside one pass
 __host__ __device__ inline Item dw_segment(const DwPlan& S, int b, long long u, long long u1) {
   int p = 0;
   while (p + 1 < S.n && u >= S.ubegin[p + 1]) ++p;
   const long long local = u - S.ubegin[p];
-  const int t = (int)(local / S.kb[p]);
-  const int k = (int)(local - (long long)t * S.kb[p]);
+  const long long tu = dw_tile_units(S, p);
+  const int t = (int)(local / tu);
+  const int k = (int)(local - (long long)t * tu);   // pass * kb + k-block
   const long long left = u1 - u;
   Item it;
   it.p = p;
   it.m0 = (t / S.nt[p]) * BM;
   it.n0 = (t % S.nt[p]) * DW_BN;
-  it.nkb = left < S.kb[p] - k ? (int)left : S.kb[p] - k;
+  it.nkb = left < tu - k ? (int)left : (int)(tu - k);
   it.z = b + S.tbegin[p] + t;
-  it.r0 = k * BKF;
+  it.ps = k / S.kb[p];
+  it.r0 = (k - it.ps * S.kb[p]) * BKF;
   it.rows = S.M[p] - it.r0 < it.nkb * BKF ? S.M[p] - it.r0 : it.nkb * BKF;
   return it;
 }
 
 struct DwParams {
   DwGroup grp;
-  int Nn[MAXP], Kk[MAXP];
+  int Nn[DW_MAXP], Kk[DW_MAXP];
   unsigned bias_mask;             // bit p: member p wants the bias-gradient partials
   float* part;                    // [slots][128][128] partial tiles (row: G column - m0, column: X column - n0)
   float* part_bias;               // [slots][128] partial column sums of G (tiles with n0 == 0)
   long long* trace;               // as Params::trace
   int trace_tiles;
 };
+
+// kernel parameters beyond 4 KB: Hopper with CUDA >= 12.1 takes up to 32 764 bytes
+static_assert(sizeof(DwMaps) + sizeof(DwParams) <= 32764, "weight-gradient kernel parameters exceed 32 764 bytes");
 
 __device__ __forceinline__ float lds32(uint32_t saddr) {
   float v;
@@ -957,7 +976,7 @@ __device__ __forceinline__ void dw_transpose_block16(uint32_t sx, uint32_t sp, i
 // of 2 k16 wgmma per k-block.
 template <bool TF1, int H16 = 0>
 __global__ void __launch_bounds__(WG_THREADS, 1)
-tc3_wgmma_dw_kernel(const __grid_constant__ Maps maps, const DwParams P) {
+tc3_wgmma_dw_kernel(const __grid_constant__ DwMaps maps, const DwParams P) {
   static_assert(H16 == 0 || TF1, "16-bit operands use the single accumulator");
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
@@ -997,18 +1016,21 @@ tc3_wgmma_dw_kernel(const __grid_constant__ Maps maps, const DwParams P) {
         for (long long u = u0; u < u1;) {
           const Item w = dw_segment(S, blockIdx.x, u, u1);
           u += w.nkb;
-          const int row = S.base[w.p] + w.r0;
+          int row = S.base[w.p] + w.r0, pass = w.ps;
+          const int row_end = S.base[w.p] + S.kb[w.p] * BKF;
           for (int kb = 0; kb < w.nkb; ++kb) {
             mbar_wait(&raw_empty[stage], phase ^ 1);
             uint8_t* st = smem + stage * DW_RAW_BYTES;
             mbar_arrive_expect_tx(&raw_full[stage], DW_RAW_BYTES);
 #pragma unroll
             for (int j = 0; j < BM / 32; ++j)          // 32-float column groups of G
-              tma_load_2d(&maps.a[w.p], &raw_full[stage], st + j * 4096, w.m0 + 32 * j, row + kb * BKF);
+              tma_load_3d(&maps.g[w.p], &raw_full[stage], st + j * 4096, w.m0 + 32 * j, row, pass);
 #pragma unroll
             for (int j = 0; j < DW_BN / 32; ++j)       // and of X
-              tma_load_2d(&maps.b[w.p], &raw_full[stage], st + A_BYTES + j * 4096, w.n0 + 32 * j, row + kb * BKF);
+              tma_load_3d(&maps.x[w.p], &raw_full[stage], st + A_BYTES + j * 4096, w.n0 + 32 * j, row, pass);
             if (++stage == DW_RAW_STAGES) { stage = 0; phase ^= 1; }
+            row += BKF;
+            if (row == row_end) { row = S.base[w.p]; ++pass; }   // the next pass's slice, same rows
           }
         }
       }
@@ -1020,15 +1042,18 @@ tc3_wgmma_dw_kernel(const __grid_constant__ Maps maps, const DwParams P) {
       for (long long u = u0; u < u1;) {
         const Item w = dw_segment(S, blockIdx.x, u, u1);
         u += w.nkb;
+        int valid = S.M[w.p] - w.r0;                // live rows from the k-block's first row on
         for (int kb = 0; kb < w.nkb; ++kb) {
           mbar_wait(&pl_empty[ps], pph ^ 1);
           mbar_wait(&raw_full[rs], rph);
           const uint32_t sx = smem_u32(smem + rs * DW_RAW_BYTES + A_BYTES);
           const uint32_t sp = smem_u32(smem + DW_OFF_PLANES + ps * DW_PLANE_BYTES);
           for (int t = tt; t < 256; t += 32 * DW_TR_WARPS) {
-            if constexpr (H16) dw_transpose_block16<H16>(sx, sp, t, w.rows - kb * BKF);
-            else dw_transpose_block<TF1>(sx, sp, t, w.rows - kb * BKF);
+            if constexpr (H16) dw_transpose_block16<H16>(sx, sp, t, valid);
+            else dw_transpose_block<TF1>(sx, sp, t, valid);
           }
+          valid -= BKF;
+          if (valid <= 0) valid = S.M[w.p];        // next pass (a segment's k-blocks all hold live rows)
           asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy stores -> wgmma reads
           __syncwarp();
           if (lane == 0) {
@@ -1120,12 +1145,12 @@ tc3_wgmma_dw_kernel(const __grid_constant__ Maps maps, const DwParams P) {
         wgmma_commit();
         wgmma_wait<1>();
       };
+      int valid = S.M[w.p] - w.r0;                // live rows from the k-block's first row on (as the transposers)
       for (int kb = 0; kb < w.nkb; ++kb) {
         mbar_wait(&raw_full[rs], rph);
         mbar_wait(&pl_full[ps], pph);
         const uint32_t sg = smem_u32(smem + rs * DW_RAW_BYTES);
         const uint32_t sp = smem_u32(smem + DW_OFF_PLANES + ps * DW_PLANE_BYTES);
-        const int valid = w.rows - kb * BKF;
         if constexpr (H16) {
           if (kb & 1) kblock16(sg, sp, valid, f1);
           else kblock16(sg, sp, valid, f0);
@@ -1142,6 +1167,8 @@ tc3_wgmma_dw_kernel(const __grid_constant__ Maps maps, const DwParams P) {
         prev = ps;
         if (++rs == DW_RAW_STAGES) { rs = 0; rph ^= 1; }
         if (++ps == DW_PLANE_STAGES) { ps = 0; pph ^= 1; }
+        valid -= BKF;
+        if (valid <= 0) valid = S.M[w.p];
       }
       wgmma_wait<0>();
       __syncwarp();
@@ -1190,7 +1217,7 @@ struct ReduceProb {
   long long rs, cs;
   int blk_w, blk_b;
 };
-struct ReduceTable { DwGroup grp; ReduceProb q[MAXP]; const float* part; const float* part_bias; };
+struct ReduceTable { DwGroup grp; ReduceProb q[DW_MAXP]; const float* part; const float* part_bias; };
 
 __global__ void __launch_bounds__(256) reduce_grads3_kernel(const ReduceTable T) {
   __shared__ DwPlan S;
@@ -1199,13 +1226,13 @@ __global__ void __launch_bounds__(256) reduce_grads3_kernel(const ReduceTable T)
   int p = 0;
   while (p + 1 < T.grp.n && (int)blockIdx.x >= T.q[p + 1].blk_w) ++p;
   const ReduceProb& q = T.q[p];
-  const int kb = S.kb[p];
+  const long long tu = dw_tile_units(S, p);
   // the slots of tile t of problem p, in the order of the CTAs that cover it
   auto sum_tile = [&](const float* src, int t, size_t slot_floats) {
     float s = 0.f;
-    if (kb > 0) {
-      const long long u = S.ubegin[p] + (long long)t * kb;
-      const int b1 = dw_owner(S, u + kb - 1);
+    if (tu > 0) {
+      const long long u = S.ubegin[p] + (long long)t * tu;
+      const int b1 = dw_owner(S, u + tu - 1);
       src += (size_t)(S.tbegin[p] + t) * slot_floats;
       for (int b = dw_owner(S, u); b <= b1; ++b) s += src[(size_t)b * slot_floats];
     }
@@ -1248,10 +1275,12 @@ static EncodeTiledFn encode_fn() {
 // hundred operands every iteration, so they are memoised (an encode costs ~1 us of host time, 3-12 per launch).
 // Every tile is a [box_rows x 32 fp32] box with the 128-byte swizzle the consumers decode (swz()), or (kind 1 / 2: a
 // bf16 / fp16 plane, ld in 16-bit elements) a [box_rows x 32] box of 16-bit values with the 64-byte swizzle (swz64()).
+// passes > 0: a 3-D map of `passes` such [rows x cols] slices pstride elements apart, boxes [box_rows x 32 x 1].
 struct MapKey {
-  const void* base; int rows, cols, ld, box_rows, kind;
+  const void* base; int rows, cols, ld, box_rows, kind, passes; long long pstride;
   bool operator==(const MapKey& o) const {
-    return base == o.base && rows == o.rows && cols == o.cols && ld == o.ld && box_rows == o.box_rows && kind == o.kind;
+    return base == o.base && rows == o.rows && cols == o.cols && ld == o.ld && box_rows == o.box_rows &&
+           kind == o.kind && passes == o.passes && pstride == o.pstride;
   }
 };
 struct MapKeyHash {
@@ -1262,14 +1291,17 @@ struct MapKeyHash {
     h = h * 1000003u ^ (size_t)k.ld;
     h = h * 1000003u ^ (size_t)k.box_rows;
     h = h * 1000003u ^ (size_t)k.kind;
+    h = h * 1000003u ^ (size_t)k.passes;
+    h = h * 1000003u ^ (size_t)k.pstride;
     return h;
   }
 };
 static std::mutex g_map_mu;
 static std::unordered_map<MapKey, CUtensorMap, MapKeyHash> g_map_cache;
 
-static int make_map(CUtensorMap* map, const float* base, int rows, int cols, int ld, int box_rows, int kind = 0) {
-  const MapKey key{base, rows, cols, ld, box_rows, kind};
+static int make_map(CUtensorMap* map, const float* base, int rows, int cols, int ld, int box_rows, int kind = 0,
+                    int passes = 0, long long pstride = 0) {
+  const MapKey key{base, rows, cols, ld, box_rows, kind, passes, pstride};
   {
     std::lock_guard<std::mutex> lk(g_map_mu);
     auto it = g_map_cache.find(key);
@@ -1277,19 +1309,20 @@ static int make_map(CUtensorMap* map, const float* base, int rows, int cols, int
   }
   EncodeTiledFn fn = encode_fn();
   if (!fn) { set_error("cuTensorMapEncodeTiled entry point unavailable"); return -4; }
-  cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
-  cuuint64_t strides[1] = {(cuuint64_t)ld * (kind ? 2 : 4)};
-  cuuint32_t box[2] = {(cuuint32_t)BKF, (cuuint32_t)box_rows};
-  cuuint32_t estr[2] = {1, 1};
+  const size_t esz = kind ? 2 : 4;
+  cuuint64_t dims[3] = {(cuuint64_t)cols, (cuuint64_t)rows, (cuuint64_t)passes};
+  cuuint64_t strides[2] = {(cuuint64_t)ld * esz, (cuuint64_t)pstride * esz};
+  cuuint32_t box[3] = {(cuuint32_t)BKF, (cuuint32_t)box_rows, 1};
+  cuuint32_t estr[3] = {1, 1, 1};
   const CUtensorMapDataType dt = kind == 1   ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16
                                  : kind == 2 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16
                                              : CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
-  CUresult r = fn(map, dt, 2, const_cast<float*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+  CUresult r = fn(map, dt, passes > 0 ? 3 : 2, const_cast<float*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                   kind ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
-    set_error("cuTensorMapEncodeTiled failed (%d) rows=%d cols=%d ld=%d box_rows=%d kind=%d", (int)r, rows, cols, ld,
-              box_rows, kind);
+    set_error("cuTensorMapEncodeTiled failed (%d) rows=%d cols=%d ld=%d box_rows=%d kind=%d passes=%d pstride=%lld",
+              (int)r, rows, cols, ld, box_rows, kind, passes, pstride);
     return -4;
   }
   std::lock_guard<std::mutex> lk(g_map_mu);
@@ -1549,7 +1582,8 @@ int gemm_nt_tc3_chain(const GemmNT* ps, const int* dep, int n, int* flags, cudaS
 bool tc3_dw_eligible(const GemmDW& q) {
   auto al = [](const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; };
   return q.dW && q.M >= 1 && q.Nn >= 16 && q.Kk >= 16 && (q.Nn % 4) == 0 && (q.Kk % 4) == 0 && (q.ldg % 4) == 0 &&
-         (q.ldx % 4) == 0 && al(q.G) && al(q.X);
+         (q.ldx % 4) == 0 && al(q.G) && al(q.X) &&
+         (q.passes == 1 || (q.passes > 1 && (q.pass_g % 4) == 0 && (q.pass_x % 4) == 0 && q.pass_g > 0 && q.pass_x > 0));
 }
 
 // the schedule inputs of a launch (the members' host row counts, or their buffers' rows with m_dev)
@@ -1560,6 +1594,7 @@ static void dw_group(const GemmDW* qs, int n, int sms, tc3::DwGroup& g) {
   for (int i = 0; i < n; ++i) {
     g.m_dev[i] = qs[i].m_dev; g.base_dev[i] = qs[i].base_dev; g.M[i] = qs[i].M;
     g.mt[i] = ceil_div(qs[i].Nn, BM); g.nt[i] = ceil_div(qs[i].Kk, DW_BN);
+    g.passes[i] = std::max(qs[i].passes, 1);
   }
 }
 
@@ -1572,7 +1607,7 @@ void tc3_dw_layout(const GemmDW* qs, int n, Dw3Layout* L) {
   for (int i = 0; i < n; ++i) {
     const int t = ceil_div(qs[i].Nn, BM) * ceil_div(qs[i].Kk, DW_BN);
     tiles += t;
-    units += (long long)t * ceil_div(std::max(qs[i].M, 0), BKF);
+    units += (long long)t * ceil_div(std::max(qs[i].M, 0), BKF) * std::max(qs[i].passes, 1);
   }
   L->slots = (int)std::min<long long>(device_sm_count(), ceil_div_ll(units, kDwMinUnits)) + tiles;
   L->floats = (size_t)L->slots * (BM * DW_BN + BM);
@@ -1580,10 +1615,10 @@ void tc3_dw_layout(const GemmDW* qs, int n, Dw3Layout* L) {
 
 int gemm_dw_tc3_partials(const GemmDW* qs, int n, const Dw3Layout& L, float* scratch, cudaStream_t st) {
   using namespace tc3;
-  if (n < 1 || n > MAXP) { set_error("gemm_dw_tc3_partials: %d problems (max %d)", n, MAXP); return -2; }
+  if (n < 1 || n > DW_MAXP) { set_error("gemm_dw_tc3_partials: %d problems (max %d)", n, DW_MAXP); return -2; }
   int num_sms = 0;
   GIB_TRY(prepare(&num_sms));
-  Maps maps;
+  DwMaps maps;
   DwParams P;
   memset(&P, 0, sizeof(P));
   dw_group(qs, n, num_sms, P.grp);
@@ -1595,11 +1630,13 @@ int gemm_dw_tc3_partials(const GemmDW* qs, int n, const Dw3Layout& L, float* scr
     const GemmDW& q = qs[i];
     if (!tc3_dw_eligible(q)) { set_error("gemm_dw_tc3: operands violate the TMA alignment contract"); return -2; }
     if (q.tf32 != prec) { set_error("gemm_dw_tc3: problems of one launch with different precisions"); return -2; }
-    GIB_TRY(make_map(&maps.a[i], q.G, q.M, q.Nn, q.ldg, BKF));          // 32 x 32 boxes
-    GIB_TRY(make_map(&maps.b[i], q.X, q.M, q.Kk, q.ldx, BKF));
+    // 3-D maps, the pass outermost (one pass: a stride past the slice, never stepped over): 32 x 32 x 1 boxes
+    const int np = P.grp.passes[i];
+    GIB_TRY(make_map(&maps.g[i], q.G, q.M, q.Nn, q.ldg, BKF, 0, np, np > 1 ? q.pass_g : (long long)q.M * q.ldg));
+    GIB_TRY(make_map(&maps.x[i], q.X, q.M, q.Kk, q.ldx, BKF, 0, np, np > 1 ? q.pass_x : (long long)q.M * q.ldx));
     P.Nn[i] = q.Nn; P.Kk[i] = q.Kk;
     if (q.dbias) P.bias_mask |= 1u << i;
-    units += (long long)P.grp.mt[i] * P.grp.nt[i] * ceil_div(q.M, BKF);
+    units += (long long)P.grp.mt[i] * P.grp.nt[i] * ceil_div(q.M, BKF) * np;
   }
   P.part = scratch;
   P.part_bias = scratch + (size_t)L.slots * BM * DW_BN;
@@ -1641,18 +1678,23 @@ int gemm_dw_tc3_reduce(const GemmDW* qs, int n, const Dw3Layout& L, const float*
 }
 
 // the segments dw_plan gives a group with host row counts (test hook): per segment (CTA, member, tile, first row,
-// rows, slot), per tile the first and last CTA the reduction reads (-1, -1: no rows)
-int tc3_dw_schedule(const int* rows, const int* Nn, const int* Kk, int n, int sms, int* segs, int max_segs,
-                    int* tile_ctas, int* G_out) {
+// rows, slot), or with seg_ints == 7 (CTA, member, tile, first pass, first row in it, k-blocks, slot); per tile the
+// first and last CTA the reduction reads (-1, -1: no rows)
+int tc3_dw_schedule(const int* rows, const int* passes, const int* Nn, const int* Kk, int n, int sms, int* segs,
+                    int seg_ints, int max_segs, int* tile_ctas, int* G_out) {
   using namespace tc3;
-  if (n < 1 || n > MAXP || sms < 1) { set_error("tc3_dw_schedule: n=%d sms=%d", n, sms); return -2; }
-  int mt[MAXP], nt[MAXP], base[MAXP] = {0};
+  if (n < 1 || n > DW_MAXP || sms < 1 || (seg_ints != 6 && seg_ints != 7)) {
+    set_error("tc3_dw_schedule: n=%d sms=%d seg_ints=%d", n, sms, seg_ints);
+    return -2;
+  }
+  int mt[DW_MAXP], nt[DW_MAXP], np[DW_MAXP], base[DW_MAXP] = {0};
   for (int i = 0; i < n; ++i) {
-    if (rows[i] < 0) { set_error("tc3_dw_schedule: negative row count"); return -2; }
+    np[i] = passes ? passes[i] : 1;
+    if (rows[i] < 0 || np[i] < 1) { set_error("tc3_dw_schedule: negative row count or pass count < 1"); return -2; }
     mt[i] = ceil_div(Nn[i], BM); nt[i] = ceil_div(Kk[i], DW_BN);
   }
   DwPlan S;
-  dw_plan(S, rows, base, mt, nt, n, sms);
+  dw_plan(S, rows, base, mt, nt, np, n, sms);
   *G_out = S.G;
   int ns = 0;
   for (int b = 0; b < S.G; ++b) {
@@ -1662,17 +1704,20 @@ int tc3_dw_schedule(const int* rows, const int* Nn, const int* Kk, int n, int sm
       const Item w = dw_segment(S, b, u, u1);
       u += w.nkb;
       if (ns == max_segs) { set_error("tc3_dw_schedule: more than %d segments", max_segs); return -3; }
-      int* o = segs + 6 * ns++;
-      o[0] = b; o[1] = w.p; o[2] = (w.m0 / BM) * nt[w.p] + w.n0 / DW_BN; o[3] = w.r0; o[4] = w.rows; o[5] = w.z;
+      int* o = segs + seg_ints * ns++;
+      o[0] = b; o[1] = w.p; o[2] = (w.m0 / BM) * nt[w.p] + w.n0 / DW_BN;
+      if (seg_ints == 6) { o[3] = w.r0; o[4] = w.rows; o[5] = w.z; }
+      else { o[3] = w.ps; o[4] = w.r0; o[5] = w.nkb; o[6] = w.z; }
     }
   }
   for (int p = 0; p < n; ++p)
     for (int t = 0; t < mt[p] * nt[p]; ++t) {
       int* o = tile_ctas + 2 * (S.tbegin[p] + t);
       o[0] = o[1] = -1;
-      if (S.kb[p] > 0) {
-        const long long u = S.ubegin[p] + (long long)t * S.kb[p];
-        o[0] = dw_owner(S, u); o[1] = dw_owner(S, u + S.kb[p] - 1);
+      const long long tu = dw_tile_units(S, p);
+      if (tu > 0) {
+        const long long u = S.ubegin[p] + (long long)t * tu;
+        o[0] = dw_owner(S, u); o[1] = dw_owner(S, u + tu - 1);
       }
     }
   return ns;

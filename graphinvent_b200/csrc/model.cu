@@ -573,10 +573,18 @@ static int sub_group(const Mlp* const* ms, int n, int i) {
 // same_rows (capacity mode): the members run on the SAME device row range (the EMN's siblings) and keep one gradient
 // slice each; otherwise members with device row ranges are the disjoint bond-type groups of ONE buffer of `rows` rows
 // and share one slice.
-static int mlp_backward_multi(const Run& r, const BwdBufs& bb, const MlpBwdJob* jobs, int n, bool same_rows = false) {
+// gl: offsets of the per-layer gradient buffers (default bb.Gl).  defer: (B) is not launched; its problems are written
+// to defer[0 .. *ndefer) instead (needs the grouped path: equal depths, at most kTc3MaxProblems layers in all).
+static int mlp_backward_multi(const Run& r, const BwdBufs& bb, const MlpBwdJob* jobs, int n, bool same_rows = false,
+                              const size_t* gl = nullptr, GemmDW* defer = nullptr, int* ndefer = nullptr) {
   bool same = n <= 4;
   for (int i = 1; i < n && same; ++i) same = jobs[i].m->n == jobs[0].m->n;
   const int depth = jobs[0].m->n;
+  if (!gl) gl = bb.Gl;
+  if (defer && (!same || depth * n > kTc3MaxProblems)) {
+    set_error("mlp_backward_multi: deferred weight gradients need one grouped launch");
+    return -2;
+  }
   if (!same || depth * n > kTc3MaxProblems) {
     if (jobs[0].m_dev) {
       // device-side row counts need the grouped call pattern: sub-groups that fit one launch (make_bwd sizes their
@@ -599,7 +607,7 @@ static int mlp_backward_multi(const Run& r, const BwdBufs& bb, const MlpBwdJob* 
   size_t off = 0;
   for (int i = 0; i < n; ++i) {
     G[depth][i] = jobs[i].Gtop;
-    for (int l = 1; l < depth; ++l) G[l][i] = r.scratch + bb.Gl[l] + off;
+    for (int l = 1; l < depth; ++l) G[l][i] = r.scratch + gl[l] + off;
     if (!jobs[i].m_dev || same_rows)
       off += ((size_t)std::max(jobs[i].rows, 0) * mlp_max_ld(r.pl, *jobs[i].m) + 31) & ~(size_t)31;
   }
@@ -670,6 +678,11 @@ static int mlp_backward_multi(const Run& r, const BwdBufs& bb, const MlpBwdJob* 
       const float* Xin = x_in(j, l, &ldxin);
       qs[nq++] = lin_dw(r, bb, L, G[l][i], Xin, ldxin, j.rows, j.m_dev, j.base_dev);
     }
+  if (defer) {
+    std::copy(qs, qs + nq, defer);
+    *ndefer = nq;
+    return 0;
+  }
   return gemm_dw_group(qs, nq, r.st);   // the side-stream reduction reads only its scratch half
 }
 
@@ -841,6 +854,15 @@ static int node_model_forward(const Run& r, float* out) {
   return readout_forward(r, out);
 }
 
+// GGNN / MNN: the message MLPs and the GRU are the same weights in every pass.  With per-pass gradient slices
+// (make_bwd) and the grouped tensor-core weight-gradient launch, their weight gradients are reduced once over all
+// passes after the pass loop -- one launch of all their layers with a pass extent instead of two per pass.  The
+// per-pass launches stay for the SIMT path, for message MLPs too deep for one launch and under gib_tc_debug bit 5.
+static bool defer_pass_dw(const Run& r, const BwdBufs& bb) {
+  return bb.pass_floats > 0 && g_use_tc && (g_tc_debug & (1 | 32)) == 0 &&
+         r.pl.msg[0].n * r.ngroups <= kTc3MaxProblems;
+}
+
 // part 0: everything; part 1: the readout only (leaves d h_final in scratch[bb.dh]; the gradients of the gather /
 // APDReadout parameters -- the tail of the gradient bucket, 79 % of it -- are final afterwards); part 2: the message
 // passes only (continues from scratch[bb.dh]).  Splitting lets a data-parallel caller start the all-reduce of the
@@ -860,24 +882,34 @@ static int node_model_backward(const Run& r, const BwdBufs& bb, const float* out
   float* dh_dir = sc + bb.dh2;   // direct path through the GRU
   const MsgRows mr = r.msg_rows ? msg_rows_of(r) : MsgRows{};   // built by the forward
   const float* row_w = r.unit_bonds ? nullptr : mr.u_w;
+  // deferred weight gradients: members 0 .. nmq - 1 the message-MLP layers, kTc3MaxProblems and the next the two GRU
+  // projections; dq holds the problems of the pass processed last (t = 0), gp / xp every pass's G and X
+  const bool defer = defer_pass_dw(r, bb);
+  constexpr int kDefer = kTc3MaxProblems + 2;
+  GemmDW dq[kDefer];
+  const float* gp[kMaxPasses][kDefer];
+  const float* xp[kMaxPasses][kDefer];
+  int nmq = 0;
   for (int t = d.T - 1; t >= 0; --t) {
     const float* h = r.ws + L.h[t];
-    GIB_TRY(gru_bwd(sc + bb.dgi, sc + bb.dgh, dh_dir, dh, r.ws + L.gi[t], r.ws + L.gh[t], h, Hp, r.ga.dst_ptr, S,
-                    nullptr, r.st));
+    const size_t slice = bb.pass_base + (size_t)t * bb.pass_floats;
+    float* dgi = sc + (defer ? slice + bb.p_dgi : bb.dgi);
+    float* dgh = sc + (defer ? slice + bb.p_dgh : bb.dgh);
+    GIB_TRY(gru_bwd(dgi, dgh, dh_dir, dh, r.ws + L.gi[t], r.ws + L.gh[t], h, Hp, r.ga.dst_ptr, S, nullptr, r.st));
     {   // weight gradients of the two GRU projections: one grouped launch
-      const GemmDW qs[2] = {lin_dw(r, bb, ih, sc + bb.dgi, r.ws + L.msum[t], Mp, (int)S),
-                            lin_dw(r, bb, hh, sc + bb.dgh, h, Hp, (int)S)};
-      GIB_TRY(gemm_dw_group(qs, 2, r.st));
+      const GemmDW qs[2] = {lin_dw(r, bb, ih, dgi, r.ws + L.msum[t], Mp, (int)S), lin_dw(r, bb, hh, dgh, h, Hp, (int)S)};
+      if (defer) std::copy(qs, qs + 2, dq + kTc3MaxProblems);
+      else GIB_TRY(gemm_dw_group(qs, 2, r.st));
     }
     {   // dMsum = dgi W_ih  and  dh[t] = dgh W_hh + direct  (dh[t+1] is dead after gru_bwd): one grouped launch
-      GemmNT ps[2] = {lin_dx(r, ih, sc + bb.dgi, (int)S, sc + bb.dmsum, Mp), lin_dx(r, hh, sc + bb.dgh, (int)S, dh, Hp)};
+      GemmNT ps[2] = {lin_dx(r, ih, dgi, (int)S, sc + bb.dmsum, Mp), lin_dx(r, hh, dgh, (int)S, dh, Hp)};
       ps[1].mode = EPI_ADD; ps[1].aux = dh_dir; ps[1].ldaux = Hp;
       // h[0] is the zero-padded input (summation_mpnn.py:121-125): nothing consumes d h[0], so at t == 0 the dh GEMM,
       // the first-layer input gradients of the message MLPs and their scatter are skipped
       GIB_TRY(gemm_nt_group(ps, t == 0 ? 1 : 2, r.st));
     }
     // through the aggregation into the per-bond message MLPs
-    float* T1 = sc + bb.T1;
+    float* T1 = sc + (defer ? slice + bb.p_T1 : bb.T1);
     float* T2 = sc + bb.T2;
     float* dx0 = sc + bb.dx0;
     const int nm = pl.msg[0].n;
@@ -902,7 +934,10 @@ static int node_model_backward(const Run& r, const BwdBufs& bb, const float* out
         jobs[g] = MlpBwdJob{&pl.msg[g], r.ws + L.x0[t], &L.msg[t], rr.row0, rr.rows, T1 + ro * Mp,
                             t == 0 ? nullptr : dx0 + ro * Hp, Hp, nullptr, rr.m_dev, rr.base_dev};
       }
-      GIB_TRY(mlp_backward_multi(r, bb, jobs, r.ngroups));
+      size_t gl[8] = {0};
+      for (int l = 1; l < nm; ++l) gl[l] = slice + bb.p_Gl[l];
+      if (defer) GIB_TRY(mlp_backward_multi(r, bb, jobs, r.ngroups, false, gl, dq, &nmq));
+      else GIB_TRY(mlp_backward_multi(r, bb, jobs, r.ngroups));
       if (d.model == GIB_ATTGGNN) {
         for (int g = 0; g < r.ngroups; ++g) {
           const size_t ro = (size_t)r.tb[g];
@@ -922,6 +957,31 @@ static int node_model_backward(const Run& r, const BwdBufs& bb, const float* out
         GIB_TRY(scatter_sum(dh, dx0, Hp, r.ga.src_ptr, r.ga.src_ent, d.model == GIB_GGNN ? r.w() : nullptr, 1, S,
                             r.st, r.cap ? 0.0 : 4.0 * ((double)r.E * d.H + 2.0 * S * d.H + (double)(S + 1))));
     }
+    if (defer)
+      for (int k = 0; k < kDefer; ++k) {
+        gp[t][k] = dq[k].G;
+        xp[t][k] = dq[k].X;
+      }
+  }
+  if (defer) {
+    // one reduction over all passes per member: the slices of pass t lie t strides past those of pass 0
+    auto extend = [&](int k) -> int {
+      GemmDW& q = dq[k];
+      q.passes = d.T;
+      q.pass_g = gp[1][k] - gp[0][k];
+      q.pass_x = xp[1][k] - xp[0][k];
+      q.work *= d.T;
+      for (int t = 2; t < d.T; ++t)
+        if (gp[t][k] - gp[0][k] != t * q.pass_g || xp[t][k] - xp[0][k] != t * q.pass_x) {
+          set_error("node_model_backward: pass slices of a shared weight are not evenly spaced");
+          return -2;
+        }
+      return 0;
+    };
+    for (int k = 0; k < nmq; ++k) GIB_TRY(extend(k));
+    for (int k = kTc3MaxProblems; k < kDefer; ++k) GIB_TRY(extend(k));
+    std::copy(dq + kTc3MaxProblems, dq + kDefer, dq + nmq);   // the GRU pair after the message-MLP layers
+    GIB_TRY(gemm_dw_group(dq, nmq + 2, r.st));
   }
   return 0;
 }
@@ -1138,6 +1198,26 @@ void make_bwd(const Run& r, BwdBufs& bb) {
     qs[1].Nn = pl.lins[pl.gru_hh].Rp; qs[1].Kk = pl.lins[pl.gru_hh].Cp;
     dw = std::max(dw, 2 * gemm_dw_group_half_floats(qs, 2));
   }
+  // GGNN / MNN with several passes: the pass-shared weight gradients reduced over all passes (defer_pass_dw) -- the
+  // per-pass gradient slices, and the scratch of their one launch
+  const bool pass_slices = (d.model == GIB_GGNN || d.model == GIB_MNN) && d.T > 1;
+  if (pass_slices) {
+    GemmDW qs[kTc3MaxProblems + 2];
+    int nq = 0;
+    const int depth = pl.msg[0].n;
+    for (int l = 0; l < depth && depth * r.ngroups <= kTc3MaxProblems; ++l)
+      for (int g = 0; g < r.ngroups; ++g) {
+        if (mrows[g] == 0) continue;
+        const Lin& L = pl.lins[pl.msg[g].first + l];
+        qs[nq].M = (int)mrows[g]; qs[nq].Nn = L.Rp; qs[nq].Kk = L.Cp; qs[nq].passes = d.T;
+        ++nq;
+      }
+    for (int k = 0; k < 2; ++k, ++nq) {
+      const Lin& L = pl.lins[k ? pl.gru_hh : pl.gru_ih];
+      qs[nq].M = (int)S; qs[nq].Nn = L.Rp; qs[nq].Kk = L.Cp; qs[nq].passes = d.T;
+    }
+    dw = std::max(dw, 2 * gemm_dw_group_half_floats(qs, nq));
+  }
   // grouped backward passes keep one ping/pong slice per member inside GA / GB
   {
     size_t types = 64;
@@ -1178,6 +1258,20 @@ void make_bwd(const Run& r, BwdBufs& bb) {
     bb.dmem = bp.take(E * Hp); bb.dmem2 = bp.take(E * Hp);
     bb.dEMx = bp.take(E * Hp); bb.dENx = bp.take(E * Hp); bb.dEMm = bp.take(E * Hp); bb.dENm = bp.take(E * Hp);
     bb.st3 = bp.take(3 * E * Hp);
+  }
+  bb.pass_base = bb.pass_floats = bb.p_T1 = bb.p_dgi = bb.p_dgh = 0;
+  for (int l = 0; l < 8; ++l) bb.p_Gl[l] = 0;
+  if (pass_slices) {
+    // one slice per pass: the top gradient of the message MLPs ([P, Mp], rows as T1), their per-layer gradients (the
+    // bond-type groups' slices side by side, as mlp_backward_multi lays them out in Gl), dgi and dgh
+    Bump pp;
+    const size_t w = mlp_max_ld(pl, pl.msg[0]);
+    bb.p_T1 = pp.take(P * Mp);
+    for (int l = 1; l < pl.msg[0].n; ++l) bb.p_Gl[l] = pp.take(P * w + 32 * 4);
+    bb.p_dgi = pp.take(S * 3 * Hp);
+    bb.p_dgh = pp.take(S * 3 * Hp);
+    bb.pass_floats = pp.off;
+    bb.pass_base = bp.take((size_t)d.T * pp.off);
   }
   bb.total = bp.off;
 }

@@ -68,6 +68,10 @@ struct BwdBufs {
   size_t GA, GB, T1, T2, dw, dh, dh2, dmsum, dgi, dgh, dx0, dcat_att, dcat_add, dcat_conn, dgterm, dg;
   size_t dmem, dmem2, dEMx, dENx, dEMm, dENm, st3;
   size_t Gl[8];     // per-layer gradient buffers of a chained MLP backward (Gl[0] unused)
+  // GGNN / MNN with several passes: one slice per pass, pass_floats apart from pass_base, of the gradients the weight
+  // gradients of the pass-shared weights read (message MLPs: top gradient and per-layer G_l; GRU: dgi, dgh), so that
+  // they are reduced once over all passes after the pass loop.  Offsets inside a slice; pass_floats = 0: none.
+  size_t pass_base, pass_floats, p_T1, p_dgi, p_dgh, p_Gl[8];
   size_t flags;
   size_t total;
 };

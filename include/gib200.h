@@ -98,7 +98,10 @@ int gib_version(void);
 /* tensor-core 3xTF32 GEMM path on (default) / off (fp32 SIMT GEMMs only); process-wide switch */
 void gib_set_tensor_cores(int on);
 int gib_get_tensor_cores(void);
-/* bit 4: the GEMM dispatch before the narrow fp32 kernel: narrow outputs (max(N, n_store) <= 48) on the general SIMT
+/* bit 5: the weight gradients of the GGNN / MNN message MLPs and GRU pass by pass (two grouped launches per message
+ * pass) instead of once over all passes after the pass loop.  Logits, loss and the other weights' gradients are
+ * bit-identical either way; the pass-shared weights' gradients differ in fp32 summation order only.
+ * bit 4: the GEMM dispatch before the narrow fp32 kernel: narrow outputs (max(N, n_store) <= 48) on the general SIMT
  * kernel, groups that do not all qualify for one tensor-core launch and the first-layer input gradients of sibling MLPs
  * problem by problem.  The results are bit-identical either way; only the launches differ.
  * bit 3: GGNN / MNN message MLPs on one row per bond entry (the AttentionGGNN's layout) instead of one per message row.
@@ -354,13 +357,18 @@ typedef struct gib_dw_problem {
 size_t gib_test_dw_scratch_bytes(const gib_dw_problem* qs, const int* group_sizes, int n_groups, long long plan_rows);
 int gib_test_dw_groups(const gib_dw_problem* qs, const int* group_sizes, int n_groups, long long plan_rows,
                        void* scratch, gib_stream stream);
-/* The schedule of one grouped tensor-core weight-gradient launch of n (<= 16) members with host row counts rows[p] and
+/* The schedule of one grouped tensor-core weight-gradient launch of n (<= 32) members with host row counts rows[p] and
  * padded shapes Nn[p] x Kk[p] on sms SMs (host arithmetic, no device): writes G (the CTAs with work), per segment 6
  * ints (CTA, member, tile of the member, first reduction row, rows, scratch slot) into segs, and per tile of the group
  * (member-major) the first and last CTA whose slots the reduction sums into tile_ctas [tiles][2] (-1, -1: no rows).
  * Returns the segment count, or < 0 (more than max_segs segments, bad arguments). */
 int gib_test_dw_schedule(const int* rows, const int* Nn, const int* Kk, int n, int sms, int* segs, int max_segs,
                          int* tile_ctas, int* G);
+/* The same with a pass extent: member p reduces over the same rows[p] rows of passes[p] slices (its units are
+ * numbered tile, then pass, then k-block).  Per segment 7 ints: CTA, member, tile of the member, first pass, first
+ * reduction row in that pass, k-blocks (continuing into the next pass at row 0), scratch slot. */
+int gib_test_dw_schedule_passes(const int* rows, const int* passes, const int* Nn, const int* Kk, int n, int sms,
+                                int* segs, int max_segs, int* tile_ctas, int* G);
 /* G[p] = w[p] * dM[dst[p]] * act'(Y[p]) (rows with dst[p] < 0: zeros) */
 int gib_test_scatter_bwd(float* G, const float* dM, const float* Y, int ld, const int* dst, const float* w, int act,
                          long long P, gib_stream stream);

@@ -1,7 +1,9 @@
 """Host model of the tensor-core weight-gradient launches of one C2 training step (bench.py --config C2: GGNN, hidden
 128, message 128, 4 passes, batch 1024 of 13-atom graphs): the makespan of each grouped dW launch under the former
 schedule (one chunk length per launch from rows x the largest member's tiles, chunks dealt to CTAs round-robin) and
-under the even k-block split of csrc/gemm_tc3.cu (dw_plan), both from the plan's shapes.  CPU only, no library:
+under the even k-block split of csrc/gemm_tc3.cu (dw_plan), both from the plan's shapes; and for the pass-shared
+weights (GRU, message rows) the even split of one launch over all 4 passes (GemmDW::passes) against 4 per-pass
+launches.  CPU only, no library:
 
     python tools/dw_schedule.py [--sms 132]
 
@@ -43,11 +45,12 @@ def former(members, sms, plan_rows=0):
     return c, len(items), max(per)
 
 
-def even(members, sms):
-    """per-CTA clocks of the even split: CTA b takes units [U b / G, U (b + 1) / G), one drain per tile it touches"""
+def even(members, sms, passes=1):
+    """per-CTA clocks of the even split: CTA b takes units [U b / G, U (b + 1) / G), one drain per tile it touches;
+    passes: every member reduces over that many slices (a tile holds kb * passes units)"""
     bounds, u = [], 0
     for nn, kk, _, live in members:
-        kb = cdiv(live, BKF)
+        kb = cdiv(live, BKF) * passes
         for _ in range(tiles(nn, kk)):
             if kb:
                 bounds.append((u, u + kb))
@@ -100,6 +103,18 @@ def main():
         print(f"{name:34s} {c:6d} {items:6d} {mf / 1e3:12.1f} {G:4d} {segs:5d} {me / 1e3:10.1f} {mf / me:12.2f} {n:6d}")
     print(f"step: former {tot_f / 1e3:.0f} k clk, even {tot_e / 1e3:.0f} k clk: "
           f"{(tot_f - tot_e) / (args.ghz * 1e9) * 1e3:.3f} ms at {args.ghz} GHz")
+    tot_p = tot_a = 0
+    for name, members, _, n in c2_launches():
+        if n == 1:
+            continue
+        _, _, per = even(members, args.sms)
+        G, segs, once = even(members, args.sms, passes=n)
+        tot_p += per * n
+        tot_a += once
+        print(f"{name:34s} per pass {n} x {per / 1e3:.1f} k clk, all passes in one launch {once / 1e3:.1f} k clk "
+              f"(G {G}, {segs} segments)")
+    print(f"pass-shared weights: {(tot_p - tot_a) / (args.ghz * 1e9) * 1e3:.3f} ms at {args.ghz} GHz, plus "
+          f"{2 * (4 - 1)} launch ramps and tails")
 
 
 if __name__ == "__main__":
