@@ -65,6 +65,11 @@ class PPDims(ctypes.Structure):
                                    "batch_size")]
 
 
+class SamplingPolicy(ctypes.Structure):
+    """mirror of `gib_sampling_policy` (include/gib200.h): the temperature / top-k / top-p policy of the samplers"""
+    _fields_ = [("temperature", c_f), ("top_k", c_i), ("top_p", c_f), ("reserved", c_i)]
+
+
 class Scaffolds(ctypes.Structure):
     """mirror of `gib_scaffolds` (include/gib200.h): the scaffold table and the per-batch scaffold state"""
     _fields_ = [(n, c_p) for n in ("nodes", "edges", "n_atoms", "protect", "slot_ids", "started", "gen_scaffolds")] + [
@@ -137,6 +142,14 @@ _PROTOS = {
     "gib_adam_step_scaled": (c_i, [c_p, c_p, c_p, c_p, c_ll, c_p, c_p, c_p, c_d, c_d, c_d, c_d, c_d, c_d, c_p]),
     "gib_amp_update_scale": (c_i, [c_p, c_p, c_p, c_d, c_d, c_i, c_p, c_i, c_p]),
     "gib_sample_actions": (c_i, [c_p, c_i, c_i, c_p, c_p, c_p, c_p]),
+    "gib_sampling_policy_set": (c_i, [c_p, c_f, c_i, c_f, c_p]),
+    "gib_sample_actions_policy": (c_i, [c_p, c_i, c_i, c_p, c_p, c_p, c_p, c_p, c_p]),
+    "gib_generation_sample_round_policy": (c_i, [c_i] * 8 + [c_p, c_i] + [c_p] * 13 + [c_i, c_p, c_p, c_p, c_p]),
+    "gib_generation_sample_round_scaffold_policy": (c_i, [c_i] * 8 + [c_p, c_p, c_i] + [c_p] * 13
+                                                    + [c_i, c_p, c_p, c_p, c_p]),
+    "gib_rl_sample_round_policy": (c_i, [c_i] * 8 + [c_p, c_p, c_i] + [c_p] * 17 + [c_i, c_p, c_p, c_p, c_p]),
+    "gib_rl_sample_round_scaffold_policy": (c_i, [c_i] * 8 + [c_p, c_p, c_p, c_i] + [c_p] * 17
+                                            + [c_i, c_p, c_p, c_p, c_p]),
     "gib_generation_scratch_bytes": (c_sz, [c_i]),
     "gib_generation_round": (c_i, [c_i] * 7 + [c_p] * 11 + [c_i, c_p, c_p, c_p]),
     "gib_generation_round_layout": (c_i, [c_i] * 9 + [c_p] * 11 + [c_i, c_p, c_p, c_p]),

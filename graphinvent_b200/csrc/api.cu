@@ -99,16 +99,8 @@ __global__ void __launch_bounds__(256) sample_actions_kernel(const float* __rest
   __shared__ float pre[257];
   const int b = blockIdx.x;
   if (g.state) {
-    // every CTA reads the same words before any of them is written (state[0] / counters advance in gen_scan_kernel,
-    // which runs after this kernel); only CTA 0 writes, and a status it sets cannot change another CTA's decision
-    const int r = g.state[0], B = gridDim.x;
-    const bool live = g.counters[0] < B && g.state[1] == 0;
-    const bool go = live && r >= 0 && r < g.rounds;
-    if (b == 0 && threadIdx.x == 0) {
-      g.ctl[0] = go ? r : -1;
-      if (live && !go) g.state[1] = 1;
-    }
-    if (!go) return;
+    const int r = gate_round(g), B = gridDim.x;
+    if (r < 0) return;
     if (g.actions) {                  // recorded actions: row r is the draw, the caller computes the likelihoods
       if (threadIdx.x == 0) action[b] = g.actions[(size_t)r * B + b];
       return;

@@ -459,7 +459,7 @@ static int sample_round(int B, int N, int F, int Ef, int n_atom_types, int n_cha
                         int* action, float* likelihood, float* nodes, float* edges, int* n_nodes, float* likelihoods,
                         float* gen_nodes, float* gen_edges, signed char* gen_n_nodes, float* gen_likelihoods,
                         signed char* properly_terminated, int capacity, int* counters, void* scratch,
-                        gib_stream stream) {
+                        gib_stream stream, const gib_sampling_policy* policy) {
   GIB_TRY(check_round_args(B, N, F, Ef, n_atom_types, n_charges, n_imp_H, n_chirality, 0));
   const long long want = layout_apd(N, Ef, n_atom_types, n_charges, n_imp_H, n_chirality);
   if (apd != want) {
@@ -471,7 +471,10 @@ static int sample_round(int B, int N, int F, int Ef, int n_atom_types, int n_cha
   GenDims d{B, N, F, Ef, n_atom_types, n_charges, n_imp_H, n_chirality, 2 * N};
   int* ctl = round_ctl(scratch, B);
   const RoundGate gate{state, counters, ctl, 2 * N};
-  GIB_TRY(sample_actions_launch(logits, B, apd, uniforms, action, likelihood, &gate, st));
+  if (policy)
+    GIB_TRY(policy_sample_launch(logits, B, apd, uniforms, policy, action, likelihood, nullptr, &gate, st));
+  else
+    GIB_TRY(sample_actions_launch(logits, B, apd, uniforms, action, likelihood, &gate, st));
   return launch_round(d, 0, ctl, state, action, likelihood, nodes, edges, n_nodes, likelihoods, gen_nodes, gen_edges,
                       gen_n_nodes, gen_likelihoods, properly_terminated, capacity, counters, scratch, st, sc);
 }
@@ -485,7 +488,7 @@ extern "C" int gib_generation_sample_round(int B, int N, int F, int Ef, int n_at
                                            void* scratch, gib_stream stream) {
   return sample_round(B, N, F, Ef, n_atom_types, n_charges, n_imp_H, n_chirality, nullptr, logits, apd, uniforms,
                       state, action, likelihood, nodes, edges, n_nodes, likelihoods, gen_nodes, gen_edges,
-                      gen_n_nodes, gen_likelihoods, properly_terminated, capacity, counters, scratch, stream);
+                      gen_n_nodes, gen_likelihoods, properly_terminated, capacity, counters, scratch, stream, nullptr);
 }
 
 extern "C" int gib_generation_sample_round_scaffold(int B, int N, int F, int Ef, int n_atom_types, int n_charges,
@@ -499,7 +502,7 @@ extern "C" int gib_generation_sample_round_scaffold(int B, int N, int F, int Ef,
   GIB_TRY(check_scaffolds("gib_generation_sample_round_scaffold", sc));
   return sample_round(B, N, F, Ef, n_atom_types, n_charges, n_imp_H, n_chirality, sc, logits, apd, uniforms, state,
                       action, likelihood, nodes, edges, n_nodes, likelihoods, gen_nodes, gen_edges, gen_n_nodes,
-                      gen_likelihoods, properly_terminated, capacity, counters, scratch, stream);
+                      gen_likelihoods, properly_terminated, capacity, counters, scratch, stream, nullptr);
 }
 
 static int rl_sample_round(int B, int N, int F, int Ef, int n_atom_types, int n_charges, int n_imp_H, int n_chirality,
@@ -508,7 +511,7 @@ static int rl_sample_round(int B, int N, int F, int Ef, int n_atom_types, int n_
                            float* p_b, int* action, float* tags, float* nodes, float* edges, int* n_nodes,
                            float* likelihoods, float* gen_nodes, float* gen_edges, signed char* gen_n_nodes,
                            float* gen_likelihoods, signed char* properly_terminated, int capacity, int* counters,
-                           void* scratch, gib_stream stream) {
+                           void* scratch, gib_stream stream, const gib_sampling_policy* policy) {
   GIB_TRY(check_round_args(B, N, F, Ef, n_atom_types, n_charges, n_imp_H, n_chirality, 0));
   const long long want = layout_apd(N, Ef, n_atom_types, n_charges, n_imp_H, n_chirality);
   if (apd != want || B + 1 >= (1 << 24) || !logits_a || !logits_b || (!uniforms && !actions) || !act_rec || !p_a ||
@@ -522,7 +525,10 @@ static int rl_sample_round(int B, int N, int F, int Ef, int n_atom_types, int n_
   GenDims d{B, N, F, Ef, n_atom_types, n_charges, n_imp_H, n_chirality, 2 * N};
   int* ctl = round_ctl(scratch, B);
   const RoundGate gate{state, counters, ctl, 2 * N, actions};
-  GIB_TRY(sample_actions_launch(logits_a, B, apd, uniforms, action, tags, &gate, st));
+  if (policy && !actions)    // recorded actions are taken as they are
+    GIB_TRY(policy_sample_launch(logits_a, B, apd, uniforms, policy, action, tags, nullptr, &gate, st));
+  else
+    GIB_TRY(sample_actions_launch(logits_a, B, apd, uniforms, action, tags, &gate, st));
   GIB_TRY(rl_probs_launch(logits_a, logits_b, B, apd, action, ctl, act_rec, p_a, p_b, tags, st));
   return launch_round(d, 0, ctl, state, action, tags, nodes, edges, n_nodes, likelihoods, gen_nodes, gen_edges,
                       gen_n_nodes, gen_likelihoods, properly_terminated, capacity, counters, scratch, st, sc);
@@ -538,7 +544,7 @@ extern "C" int gib_rl_sample_round(int B, int N, int F, int Ef, int n_atom_types
   return rl_sample_round(B, N, F, Ef, n_atom_types, n_charges, n_imp_H, n_chirality, nullptr, logits_a, logits_b, apd,
                          uniforms, actions, state, act_rec, p_a, p_b, action, tags, nodes, edges, n_nodes, likelihoods,
                          gen_nodes, gen_edges, gen_n_nodes, gen_likelihoods, properly_terminated, capacity, counters,
-                         scratch, stream);
+                         scratch, stream, nullptr);
 }
 
 extern "C" int gib_rl_sample_round_scaffold(int B, int N, int F, int Ef, int n_atom_types, int n_charges, int n_imp_H,
@@ -554,7 +560,7 @@ extern "C" int gib_rl_sample_round_scaffold(int B, int N, int F, int Ef, int n_a
   return rl_sample_round(B, N, F, Ef, n_atom_types, n_charges, n_imp_H, n_chirality, sc, logits_a, logits_b, apd,
                          uniforms, actions, state, act_rec, p_a, p_b, action, tags, nodes, edges, n_nodes, likelihoods,
                          gen_nodes, gen_edges, gen_n_nodes, gen_likelihoods, properly_terminated, capacity, counters,
-                         scratch, stream);
+                         scratch, stream, nullptr);
 }
 
 extern "C" int gib_generation_scaffold_init(int B, int N, int F, int Ef, const gib_scaffolds* sc, float* nodes,
@@ -673,3 +679,57 @@ extern "C" int gib_generation_round(int B, int N, int F, int Ef, int n_atom_type
 }
 
 extern "C" size_t gib_generation_scratch_bytes(int B) { return (size_t)B * (sizeof(int4) + 2 * sizeof(int)) + 64; }
+
+// ---- the sample rounds under a sampling policy (sampling.cu); policy = null: the entry points above ----
+extern "C" int gib_generation_sample_round_policy(int B, int N, int F, int Ef, int n_atom_types, int n_charges,
+                                                  int n_imp_H, int n_chirality, const float* logits, int apd,
+                                                  const float* uniforms, int* state, int* action, float* likelihood,
+                                                  float* nodes, float* edges, int* n_nodes, float* likelihoods,
+                                                  float* gen_nodes, float* gen_edges, signed char* gen_n_nodes,
+                                                  float* gen_likelihoods, signed char* properly_terminated,
+                                                  int capacity, int* counters, void* scratch, gib_stream stream,
+                                                  const gib_sampling_policy* policy) {
+  return sample_round(B, N, F, Ef, n_atom_types, n_charges, n_imp_H, n_chirality, nullptr, logits, apd, uniforms,
+                      state, action, likelihood, nodes, edges, n_nodes, likelihoods, gen_nodes, gen_edges,
+                      gen_n_nodes, gen_likelihoods, properly_terminated, capacity, counters, scratch, stream, policy);
+}
+
+extern "C" int gib_generation_sample_round_scaffold_policy(
+    int B, int N, int F, int Ef, int n_atom_types, int n_charges, int n_imp_H, int n_chirality,
+    const gib_scaffolds* sc, const float* logits, int apd, const float* uniforms, int* state, int* action,
+    float* likelihood, float* nodes, float* edges, int* n_nodes, float* likelihoods, float* gen_nodes,
+    float* gen_edges, signed char* gen_n_nodes, float* gen_likelihoods, signed char* properly_terminated,
+    int capacity, int* counters, void* scratch, gib_stream stream, const gib_sampling_policy* policy) {
+  GIB_TRY(check_scaffolds("gib_generation_sample_round_scaffold_policy", sc));
+  return sample_round(B, N, F, Ef, n_atom_types, n_charges, n_imp_H, n_chirality, sc, logits, apd, uniforms, state,
+                      action, likelihood, nodes, edges, n_nodes, likelihoods, gen_nodes, gen_edges, gen_n_nodes,
+                      gen_likelihoods, properly_terminated, capacity, counters, scratch, stream, policy);
+}
+
+extern "C" int gib_rl_sample_round_policy(int B, int N, int F, int Ef, int n_atom_types, int n_charges, int n_imp_H,
+                                          int n_chirality, const float* logits_a, const float* logits_b, int apd,
+                                          const float* uniforms, const int* actions, int* state, int* act_rec,
+                                          float* p_a, float* p_b, int* action, float* tags, float* nodes,
+                                          float* edges, int* n_nodes, float* likelihoods, float* gen_nodes,
+                                          float* gen_edges, signed char* gen_n_nodes, float* gen_likelihoods,
+                                          signed char* properly_terminated, int capacity, int* counters,
+                                          void* scratch, gib_stream stream, const gib_sampling_policy* policy) {
+  return rl_sample_round(B, N, F, Ef, n_atom_types, n_charges, n_imp_H, n_chirality, nullptr, logits_a, logits_b, apd,
+                         uniforms, actions, state, act_rec, p_a, p_b, action, tags, nodes, edges, n_nodes, likelihoods,
+                         gen_nodes, gen_edges, gen_n_nodes, gen_likelihoods, properly_terminated, capacity, counters,
+                         scratch, stream, policy);
+}
+
+extern "C" int gib_rl_sample_round_scaffold_policy(
+    int B, int N, int F, int Ef, int n_atom_types, int n_charges, int n_imp_H, int n_chirality,
+    const gib_scaffolds* sc, const float* logits_a, const float* logits_b, int apd, const float* uniforms,
+    const int* actions, int* state, int* act_rec, float* p_a, float* p_b, int* action, float* tags, float* nodes,
+    float* edges, int* n_nodes, float* likelihoods, float* gen_nodes, float* gen_edges, signed char* gen_n_nodes,
+    float* gen_likelihoods, signed char* properly_terminated, int capacity, int* counters, void* scratch,
+    gib_stream stream, const gib_sampling_policy* policy) {
+  GIB_TRY(check_scaffolds("gib_rl_sample_round_scaffold_policy", sc));
+  return rl_sample_round(B, N, F, Ef, n_atom_types, n_charges, n_imp_H, n_chirality, sc, logits_a, logits_b, apd,
+                         uniforms, actions, state, act_rec, p_a, p_b, action, tags, nodes, edges, n_nodes, likelihoods,
+                         gen_nodes, gen_edges, gen_n_nodes, gen_likelihoods, properly_terminated, capacity, counters,
+                         scratch, stream, policy);
+}

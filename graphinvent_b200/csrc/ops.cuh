@@ -1,5 +1,6 @@
 // Host launch wrappers of the HBM-bound kernels (graph_ops.cu).  All return 0 / cudaError_t.
 #pragma once
+#include "../../include/gib200.h"
 #include "common.cuh"
 #include "graph.cuh"
 
@@ -59,6 +60,26 @@ int pack_weight(float* Wp, float* WTp, float* bp, const float* W, const float* b
 struct RoundGate { int* state; const int* counters; int* ctl; int rounds; const int* actions; };
 int sample_actions_launch(const float* out, int B, int apd, const float* uniforms, int* action, float* lik,
                           const RoundGate* gate, cudaStream_t st);
+
+// The gate's decision in a one-CTA-per-slot sampler: the round index to sample, or -1.  Every CTA reads the same words
+// before any of them is written (state[0] / counters advance in gen_scan_kernel, which runs after the sampler); only
+// CTA 0 writes, and a status it sets cannot change another CTA's decision.
+__device__ __forceinline__ int gate_round(const RoundGate& g) {
+  const int r = g.state[0], B = gridDim.x;
+  const bool live = g.counters[0] < B && g.state[1] == 0;
+  const bool go = live && r >= 0 && r < g.rounds;
+  if (blockIdx.x == 0 && threadIdx.x == 0) {
+    g.ctl[0] = go ? r : -1;
+    if (live && !go) g.state[1] = 1;
+  }
+  return go ? r : -1;
+}
+
+// The policy sampler (sampling.cu, include/gib200.h: gib_sample_actions_policy): the draw of sample_actions_launch
+// under the temperature / top-k / top-p policy read from device memory, the model's probability of the drawn action
+// into `lik` and, when q != null, the policy's into q.  gate: as above, with gate->actions == null.
+int policy_sample_launch(const float* out, int B, int apd, const float* uniforms, const gib_sampling_policy* policy,
+                         int* action, float* lik, float* q, const RoundGate* gate, cudaStream_t st);
 
 // RL rollout (rl.cu): for every slot b of a running round r = ctl[0] (ctl[0] < 0: nothing), the softmax
 // probability of action[b] under logits_a / logits_b [B, apd] into p_a / p_b[r, b], action[b] into act_rec[r, b], and

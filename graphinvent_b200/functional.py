@@ -7,6 +7,7 @@ No computation of the hot path happens in ATen, and there is no CPU path: CPU te
 """
 import ctypes
 import math
+from collections import namedtuple
 
 import numpy as np
 import torch
@@ -331,15 +332,57 @@ def validation_nll(output, target):
     return nll
 
 
-def sample_actions(output, uniforms=None, generator=None):
+SamplingPolicy = namedtuple("SamplingPolicy", "temperature top_k top_p")
+SamplingPolicy.__doc__ = """The sampling policy of `sample_actions` and the generators (include/gib200.h: gib_sampling_policy):
+temperature >= 0 (0 = greedy), top_k >= 0 (0 = no cut), top_p in (0, 1] (1 = no cut)."""
+SAMPLING_OFF = SamplingPolicy(1.0, 0, 1.0)
+
+
+def sampling_policy(temperature=1.0, top_k=0, top_p=1.0):
+    """the SamplingPolicy of these values as the device reads them (fp32 / int32); raises ValueError naming the
+    argument that is out of range"""
+    try:
+        with np.errstate(over="ignore"):          # a value past the fp32 range becomes inf and is refused below
+            t = float(np.float32(temperature))
+            p = float(np.float32(top_p))
+    except (TypeError, ValueError):
+        raise ValueError(f"temperature and top_p must be numbers, got {temperature!r} and {top_p!r}") from None
+    if not (math.isfinite(t) and t >= 0.0):
+        raise ValueError(f"temperature must be finite and >= 0 (0 = greedy), got {temperature!r}")
+    if isinstance(top_k, bool) or not isinstance(top_k, (int, np.integer)) or not 0 <= int(top_k) < 1 << 31:
+        raise ValueError(f"top_k must be an integer in [0, 2**31) (0 = no top-k cut), got {top_k!r}")
+    if not 0.0 < p <= 1.0:
+        raise ValueError(f"top_p must lie in (0, 1] (1 = no nucleus cut), got {top_p!r}")
+    return SamplingPolicy(t, int(top_k), p)
+
+
+def set_policy(buf, policy):
+    """`policy` (a SamplingPolicy) into the device struct `buf` (int32 [4]), in stream order"""
+    check(lib.gib_sampling_policy_set(_ptr(buf), *policy, _stream(buf.device)), "gib_sampling_policy_set")
+
+
+def sample_actions(output, uniforms=None, generator=None, temperature=1.0, top_k=0, top_p=1.0, return_policy=False):
     """softmax + one categorical draw per molecule from APD logits (GraphGenerator.py:121,535-542),
-    inverse-CDF on uniforms in [0,1).  Returns (flat action index int32 [B], likelihood [B])."""
+    inverse-CDF on uniforms in [0,1).  Returns (flat action index int32 [B], likelihood [B]).
+
+    temperature / top_k / top_p: the sampling policy (`SamplingPolicy`, include/gib200.h), which changes only which
+    action is drawn: the likelihood stays the model's softmax probability of that action.  return_policy=True also
+    returns q [B], the policy's probability of the drawn action.  The default policy runs today's sampler."""
     _require_cuda(output)
+    pol = sampling_policy(temperature, top_k, top_p)
     B, apd = output.shape
     if uniforms is None:
         uniforms = torch.rand(B, device=output.device, generator=generator)
     action = torch.empty(B, dtype=torch.int32, device=output.device)
     lik = torch.empty(B, dtype=torch.float32, device=output.device)
-    check(lib.gib_sample_actions(_ptr(output.contiguous()), B, apd, _ptr(uniforms.contiguous().float()),
-                                 _ptr(action), _ptr(lik), _stream(output.device)), "gib_sample_actions")
-    return action, lik
+    if pol == SAMPLING_OFF and not return_policy:
+        check(lib.gib_sample_actions(_ptr(output.contiguous()), B, apd, _ptr(uniforms.contiguous().float()),
+                                     _ptr(action), _ptr(lik), _stream(output.device)), "gib_sample_actions")
+        return action, lik
+    buf = torch.empty(4, dtype=torch.int32, device=output.device)
+    set_policy(buf, pol)
+    q = torch.empty(B, dtype=torch.float32, device=output.device) if return_policy else None
+    check(lib.gib_sample_actions_policy(_ptr(output.contiguous()), B, apd, _ptr(uniforms.contiguous().float()),
+                                        _ptr(buf), _ptr(action), _ptr(lik), _ptr(q), _stream(output.device)),
+          "gib_sample_actions_policy")
+    return (action, lik, q) if return_policy else (action, lik)

@@ -228,11 +228,18 @@ class GraphGenerator:
 
     `action_mask="structure"` / `"valence"` (`ActionMask`): sample only actions the round accepts, from the model's
     softmax renormalised over them; `max_valence=` overrides the valence table (`config.action_rule_table`).  With
-    attachment points too, one launch applies both rules."""
+    attachment points too, one launch applies both rules.
+
+    `temperature=`, `top_k=`, `top_p=` (`functional.SamplingPolicy`; `set_sampling` changes them, `sampling` reads
+    them): draw each action from the model's softmax at that temperature, cut to the top_k most likely actions and to
+    the smallest set of them holding top_p of their probability (after the masks).  Only the draw changes: the
+    recorded likelihoods stay the model's probabilities of the drawn actions.  The default (1, 0, 1) is the model's
+    softmax itself.  In `GraphGeneratorRL` the policy applies to the agent's draw."""
 
     def __init__(self, model, batch_size, constants=None, n_atom_types=None, n_formal_charge=None, n_imp_H=None,
                  n_chirality=None, device="cuda", scaffolds=None, attachment=None, action_mask=None,
-                 max_valence=None):
+                 max_valence=None, temperature=1.0, top_k=0, top_p=1.0):
+        self._sampling = Fn.sampling_policy(temperature, top_k, top_p)
         C, self.A, self.CH, self.n_imp_H, self.n_chirality = action_layout(
             model, constants, n_atom_types, n_formal_charge, n_imp_H, n_chirality)
         self.constants = C
@@ -251,6 +258,19 @@ class GraphGenerator:
     @property
     def layout(self):
         return (self.A, self.CH, self.n_imp_H, self.n_chirality)
+
+    @property
+    def sampling(self):
+        """the sampling policy of the draws (`functional.SamplingPolicy`)"""
+        return self._sampling
+
+    def set_sampling(self, temperature=1.0, top_k=0, top_p=1.0):
+        """the sampling policy of the following draws; raises ValueError naming an argument out of range"""
+        self._sampling = Fn.sampling_policy(temperature, top_k, top_p)
+
+    def _policy_kw(self):
+        """the policy arguments of the draw: none when it is off, so the draw is today's call"""
+        return {} if self._sampling == Fn.SAMPLING_OFF else self._sampling._asdict()
 
     def _table(self, scaffolds, attachment):
         """the ScaffoldTable of set_scaffolds' arguments (None for None)"""
@@ -378,7 +398,7 @@ class GraphGenerator:
                 if self.masks_logits:
                     out = out.contiguous()
                     self._mask(out, st)
-                action, lik = Fn.sample_actions(out, generator=generator)
+                action, lik = Fn.sample_actions(out, generator=generator, **self._policy_kw())
             self._round(rnd, action, lik, st)
             n_generated = int(self._counters[0].item())           # the loop condition lives on the host (:118)
             rnd += 1
@@ -471,7 +491,7 @@ class GraphGeneratorRL(GraphGenerator):
                     raise RuntimeError("replay trace ended before batch_size molecules were finished") from None
                 action = action.to(self.device, torch.int32).contiguous()
             else:
-                action, _ = Fn.sample_actions(out_a.detach(), generator=generator)
+                action, _ = Fn.sample_actions(out_a.detach(), generator=generator, **self._policy_kw())
             idx = action.long().unsqueeze(1)
             lik_a.append(torch.softmax(out_a, dim=1).gather(1, idx).squeeze(1))       # `apds[apd_one_hot == 1]` :547-548
             lik_p.append(torch.softmax(out_p, dim=1).gather(1, idx).squeeze(1))

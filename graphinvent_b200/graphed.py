@@ -650,14 +650,21 @@ class GraphedGenerator(GraphGenerator):
     the round masks the logits (`gib_generation_mask_logits`) between the forward and the sampler.  The entry
     capacity is then `scaffold_entry_capacity(B, N, Ef, m_max)`.  `set_scaffolds` copies a new set into the table in
     place when it has the same number of scaffolds, at most the bonds the capacity was sized for and attachment points
-    given in both or in neither; otherwise it reallocates and the next batch recaptures."""
+    given in both or in neither; otherwise it reallocates and the next batch recaptures.
+
+    The sampling policy (`temperature=`, `top_k=`, `top_p=`, `set_sampling`, see `generation.GraphGenerator`): built
+    with one, the round samples with `gib_generation_sample_round_policy`, which reads the policy from a device struct
+    on every replay, so `set_sampling` between batches only rewrites that struct.  Built without one (or with the
+    default (1, 0, 1)) the round keeps today's sampler; the first `set_sampling` to another policy makes the next batch
+    capture the round once more, and later ones reuse it.  The likelihoods stay the model's."""
 
     def __init__(self, model, batch_size, constants=None, n_atom_types=None, n_formal_charge=None, n_imp_H=None,
                  n_chirality=None, device="cuda", scaffolds=None, attachment=None, action_mask=None,
-                 max_valence=None):
+                 max_valence=None, temperature=1.0, top_k=0, top_p=1.0):
         super().__init__(model, batch_size, constants=constants, n_atom_types=n_atom_types,
                          n_formal_charge=n_formal_charge, n_imp_H=n_imp_H, n_chirality=n_chirality, device=device,
-                         action_mask=action_mask, max_valence=max_valence)
+                         action_mask=action_mask, max_valence=max_valence, temperature=temperature, top_k=top_k,
+                         top_p=top_p)
         if not hasattr(model, "dims"):
             raise TypeError("GraphedGenerator runs this package's models (graphinvent_b200.gnn.mpnn) only")
         B, N, dev = self.batch_size, self.N, self.device
@@ -682,8 +689,42 @@ class GraphedGenerator(GraphGenerator):
         self.graph = None
         self.inert_rounds = 0
         self._scaffold_m, self.scaffold_version = 0, 0
+        self._init_policy()
         if scaffolds is not None:
             self.set_scaffolds(scaffolds, attachment)
+
+    # ---- the sampling policy ------------------------------------------------------------------------------
+    def _init_policy(self):
+        """the device struct the captured round reads the policy from; without a policy the round keeps today's
+        sampler"""
+        self._policy = torch.zeros(4, dtype=torch.int32, device=self.device)
+        self._policy_round = False
+        self.set_sampling(*self._sampling)
+
+    def set_sampling(self, temperature=1.0, top_k=0, top_p=1.0):
+        """the sampling policy of the following batches.  A round captured with a policy reads it from device memory,
+        so this only rewrites that struct; the first policy other than (1, 0, 1) on a generator built without one
+        makes the next batch capture its round again, once."""
+        pol = F.sampling_policy(temperature, top_k, top_p)
+        self._sampling = pol
+        if pol != F.SAMPLING_OFF and not self._policy_round:
+            self._policy_round = True
+            self._invalidate_rounds()
+        if self._policy_round:
+            F.set_policy(self._policy, pol)
+
+    def _invalidate_rounds(self):
+        self.graph = None
+
+    def _sample_round_fn(self, plain, scaffold):
+        """(entry point, name, leading scaffold args, trailing policy args) of the round's sampler"""
+        if self.scaffolds is None:
+            name, sc = plain, ()
+        else:
+            name, sc = scaffold, (ctypes.byref(self._sc),)
+        if self._policy_round:
+            return getattr(lib, name + "_policy"), name + "_policy", sc, (F._ptr(self._policy),)
+        return getattr(lib, name), name, sc, ()
 
     # ---- scaffolds --------------------------------------------------------------------------------------------
     def _set_capacity(self, capacity):
@@ -784,18 +825,14 @@ class GraphedGenerator(GraphGenerator):
         self._flags.bitwise_or_(self._hdr_flags)
         if self.masks_logits:
             self._mask_round(self.logits, st)
-        if self.scaffolds is None:
-            fn, name, sc = lib.gib_generation_sample_round, "gib_generation_sample_round", ()
-        else:
-            fn, name, sc = (lib.gib_generation_sample_round_scaffold, "gib_generation_sample_round_scaffold",
-                            (ctypes.byref(self._sc),))
+        fn, name, sc, pol = self._sample_round_fn("gib_generation_sample_round", "gib_generation_sample_round_scaffold")
         check(fn(
             self.batch_size, self.N, self.F, self.Ef, self.A, self.CH, self.n_imp_H, self.n_chirality, *sc,
             F._ptr(self.logits), self.apd, F._ptr(self.uniforms), F._ptr(self._state), F._ptr(self.action),
             F._ptr(self.lik), F._ptr(self.nodes), F._ptr(self.edges), F._ptr(self.n_nodes), F._ptr(self.likelihoods),
             F._ptr(self.generated_nodes), F._ptr(self.generated_edges), F._ptr(self.generated_n_nodes),
             F._ptr(self.generated_likelihoods), F._ptr(self.properly_terminated), self.capacity,
-            F._ptr(self._counters), F._ptr(self._scratch), st), name)
+            F._ptr(self._counters), F._ptr(self._scratch), st, *pol), name)
 
     def capture(self):
         self.graph, = _capture(self.device, [self._enqueue_round])
@@ -918,14 +955,20 @@ class GraphedGeneratorRL(GraphedGenerator):
 
     With `action_mask=` both models' logits go through the action mask (with attachment points too, in the same
     launch) and the record keeps each (round, slot)'s atom count; the backward round rebuilds the mask from the
-    restored int8 state and those counts."""
+    restored int8 state and those counts.
+
+    The sampling policy (`temperature=`, `top_k=`, `top_p=`, `set_sampling`, as `GraphedGenerator`) applies to the
+    agent's draw only (`gib_rl_sample_round_policy`); p_a / p_b stay the two models' probabilities of the drawn action,
+    so the log-likelihoods, the loss and the recomputing backward are unchanged.  Recorded `actions=` are replayed as
+    they are."""
 
     def __init__(self, model, batch_size, constants=None, n_atom_types=None, n_formal_charge=None, n_imp_H=None,
                  n_chirality=None, device="cuda", scaffolds=None, attachment=None, action_mask=None,
-                 max_valence=None):
+                 max_valence=None, temperature=1.0, top_k=0, top_p=1.0):
         GraphGenerator.__init__(self, model, batch_size, constants=constants, n_atom_types=n_atom_types,
                                 n_formal_charge=n_formal_charge, n_imp_H=n_imp_H, n_chirality=n_chirality,
-                                device=device, action_mask=action_mask, max_valence=max_valence)
+                                device=device, action_mask=action_mask, max_valence=max_valence,
+                                temperature=temperature, top_k=top_k, top_p=top_p)
         if not hasattr(model, "dims"):
             raise TypeError("GraphedGeneratorRL runs this package's models (graphinvent_b200.gnn.mpnn) only")
         B, N, dev = self.batch_size, self.N, self.device
@@ -969,6 +1012,7 @@ class GraphedGeneratorRL(GraphedGenerator):
         self._scaffold_m, self.scaffold_version = 0, 0
         self.rec_ids = None
         self.rec_n = torch.zeros(2 * N, B, dtype=torch.int32, device=dev) if self.action_mask is not None else None
+        self._init_policy()
         if scaffolds is not None:
             self.set_scaffolds(scaffolds, attachment)
 
@@ -977,6 +1021,9 @@ class GraphedGeneratorRL(GraphedGenerator):
 
     def _invalidate_graphs(self):
         self.graph, self._graphs, self._bwd = None, {}, None
+
+    def _invalidate_rounds(self):
+        self.graph, self._graphs = None, {}
 
     def set_scaffolds(self, scaffolds, attachment=None):
         GraphedGenerator.set_scaffolds(self, scaffolds, attachment)
@@ -1022,10 +1069,7 @@ class GraphedGeneratorRL(GraphedGenerator):
         if self.masks_logits:
             for logits in self.logits:
                 self._mask_round(logits, st)
-        if self.scaffolds is None:
-            fn, name, sc = lib.gib_rl_sample_round, "gib_rl_sample_round", ()
-        else:
-            fn, name, sc = lib.gib_rl_sample_round_scaffold, "gib_rl_sample_round_scaffold", (ctypes.byref(self._sc),)
+        fn, name, sc, pol = self._sample_round_fn("gib_rl_sample_round", "gib_rl_sample_round_scaffold")
         check(fn(
             B, N, self.F, self.Ef, self.A, self.CH, self.n_imp_H, self.n_chirality, *sc, F._ptr(self.logits[0]),
             F._ptr(self.logits[1]), self.apd, F._ptr(self.uniforms), F._ptr(self.actions if self._replay else None),
@@ -1033,7 +1077,7 @@ class GraphedGeneratorRL(GraphedGenerator):
             F._ptr(self.lik), F._ptr(self.nodes), F._ptr(self.edges), F._ptr(self.n_nodes), F._ptr(self.likelihoods),
             F._ptr(self.generated_nodes), F._ptr(self.generated_edges), F._ptr(self.generated_n_nodes),
             F._ptr(self.generated_likelihoods), F._ptr(self.properly_terminated), self.capacity,
-            F._ptr(self._counters), F._ptr(self._scratch), st), name)
+            F._ptr(self._counters), F._ptr(self._scratch), st, *pol), name)
 
     # ---- the captured backward round ----------------------------------------------------------------------
     def _enqueue_backward_round(self, slot):

@@ -450,6 +450,38 @@ int gib_test_plan_linear(const gib_dims* d, int i, long long* out);
 int gib_sample_actions(const float* out, int B, int apd, const float* uniforms, int* action,
                        float* likelihood, gib_stream stream);
 
+/* ---- the sampling policy: temperature, top-k and nucleus (top-p) sampling (graphinvent_b200/csrc/sampling.cu) ----
+ * The policy lives in device memory, so a captured round reads its current values on every replay.  On a row of
+ * logits o (after any mask; masked entries are -inf), with m = max(o):
+ *   ranking  the finite entries by o descending, ties to the lower index (independent of the temperature);
+ *   weights  w_j = expf((o_j - m) / temperature) for temperature > 0; temperature 0 is greedy (weight 1 on the first
+ *            entry of the ranking, 0 elsewhere);
+ *   top_k    > 0: keep the first top_k entries of the ranking (all finite ones if there are fewer);
+ *   top_p    < 1: of those, keep the shortest prefix of the ranking whose weight reaches top_p times their total (at
+ *            least one entry);
+ *   draw     inverse CDF over the kept weights in index order with the row's uniform u, target = u * total clamped
+ *            into [0, total), so an entry of weight 0 is never drawn.
+ * `likelihood` receives the MODEL's masked-softmax probability of the drawn action, bit for bit what
+ * gib_sample_actions writes for that action; `q` (optional) the policy's probability w_a / (kept total).  A row
+ * without a finite entry, with NaN or +inf, or with a NaN uniform gives action apd - 1 and NaN (q too), as
+ * gib_sample_actions does; so does a row read under a policy struct holding values gib_sampling_policy_set refuses.
+ * (1, 0, 1) is "off": the draw and the likelihood are those of gib_sample_actions. */
+typedef struct gib_sampling_policy {
+  float temperature;   /* >= 0 and finite; 0 = greedy */
+  int top_k;           /* >= 0; 0 = no top-k cut */
+  float top_p;         /* in (0, 1]; 1 = no nucleus cut */
+  int reserved;
+} gib_sampling_policy;
+/* writes {temperature, top_k, top_p} into the device struct `policy` in stream order; refuses temperature < 0 or not
+ * finite, top_k < 0, top_p outside (0, 1] and a null policy before any CUDA call */
+int gib_sampling_policy_set(gib_sampling_policy* policy, float temperature, int top_k, float top_p,
+                            gib_stream stream);
+/* gib_sample_actions under `policy` (device); q [B] may be null.  policy = null: gib_sample_actions itself (q must
+ * then be null).  apd < 2^31. */
+int gib_sample_actions_policy(const float* out, int B, int apd, const float* uniforms,
+                              const gib_sampling_policy* policy, int* action, float* likelihood, float* q,
+                              gib_stream stream);
+
 /* ---- one round of batched graph generation on the device (SURVEY.md §8f rank 1): decode the sampled flat APD
  *      index per slot, validity rules, copy terminated graphs out (pre-action state; terminate-sampled first, then
  *      invalid, ascending), apply add / connect, reset, re-stamp the dummy graph in slot 0.  Replaces
@@ -592,6 +624,41 @@ int gib_rl_sample_round(int B, int N, int F, int Ef, int n_atom_types, int n_cha
                         float* gen_edges, signed char* gen_n_nodes, float* gen_likelihoods,
                         signed char* properly_terminated, int capacity, int* counters, void* scratch,
                         gib_stream stream);
+/* The four sample-round entry points with a sampling policy (device, gib_sampling_policy_set): the draw of a running
+ * round is made under it, every other output keeps its meaning -- `likelihood`, p_a and p_b are the models'
+ * probabilities of the drawn action.  policy = null is the entry point without the suffix.  In the RL forms only the
+ * draw from `uniforms` uses the policy; recorded `actions` are taken as they are. */
+int gib_generation_sample_round_policy(int B, int N, int F, int Ef, int n_atom_types, int n_charges, int n_imp_H,
+                                       int n_chirality, const float* logits, int apd, const float* uniforms,
+                                       int* state, int* action, float* likelihood, float* nodes, float* edges,
+                                       int* n_nodes, float* likelihoods, float* gen_nodes, float* gen_edges,
+                                       signed char* gen_n_nodes, float* gen_likelihoods,
+                                       signed char* properly_terminated, int capacity, int* counters, void* scratch,
+                                       gib_stream stream, const gib_sampling_policy* policy);
+int gib_generation_sample_round_scaffold_policy(int B, int N, int F, int Ef, int n_atom_types, int n_charges,
+                                                int n_imp_H, int n_chirality, const gib_scaffolds* sc,
+                                                const float* logits, int apd, const float* uniforms, int* state,
+                                                int* action, float* likelihood, float* nodes, float* edges,
+                                                int* n_nodes, float* likelihoods, float* gen_nodes, float* gen_edges,
+                                                signed char* gen_n_nodes, float* gen_likelihoods,
+                                                signed char* properly_terminated, int capacity, int* counters,
+                                                void* scratch, gib_stream stream, const gib_sampling_policy* policy);
+int gib_rl_sample_round_policy(int B, int N, int F, int Ef, int n_atom_types, int n_charges, int n_imp_H,
+                               int n_chirality, const float* logits_a, const float* logits_b, int apd,
+                               const float* uniforms, const int* actions, int* state, int* act_rec, float* p_a,
+                               float* p_b, int* action, float* tags, float* nodes, float* edges, int* n_nodes,
+                               float* likelihoods, float* gen_nodes, float* gen_edges, signed char* gen_n_nodes,
+                               float* gen_likelihoods, signed char* properly_terminated, int capacity, int* counters,
+                               void* scratch, gib_stream stream, const gib_sampling_policy* policy);
+int gib_rl_sample_round_scaffold_policy(int B, int N, int F, int Ef, int n_atom_types, int n_charges, int n_imp_H,
+                                        int n_chirality, const gib_scaffolds* sc, const float* logits_a,
+                                        const float* logits_b, int apd, const float* uniforms, const int* actions,
+                                        int* state, int* act_rec, float* p_a, float* p_b, int* action, float* tags,
+                                        float* nodes, float* edges, int* n_nodes, float* likelihoods,
+                                        float* gen_nodes, float* gen_edges, signed char* gen_n_nodes,
+                                        float* gen_likelihoods, signed char* properly_terminated, int capacity,
+                                        int* counters, void* scratch, gib_stream stream,
+                                        const gib_sampling_policy* policy);
 /* the model input of a round: nodes [B,N,F] / edges [B,N,N,Ef] (float 0/1) as int8 into in_nodes / in_edges and, when
  * the round runs (gib_generation_sample_round's state / counters: 0 <= state[0] < 2N, state[1] == 0,
  * counters[0] < B), into row state[0] of rec_nodes [2N,B,N,F] / rec_edges [2N,B,N,N,Ef].  att_view != 0: slot 0's
