@@ -80,6 +80,8 @@ PP_STATUS_INTS = 8                                                  # GIB_PP_* (
 PP_BAD_NODES, PP_BAD_EDGES, PP_EMPTY, PP_DISCONNECTED, PP_BAD_RANKING, PP_MATCH_BUDGET = 1, 2, 4, 8, 16, 32
 ROUTE_BFS, ROUTE_DFS = 0, 1                                         # GIB_ROUTE_BFS / GIB_ROUTE_DFS (gib_reorder)
 ROUTE_NOT_PREFIX, ROUTE_MASKED, ROUTE_BAD_ID, ROUTE_ACTION = 1, 2, 4, 8               # GIB_ROUTE_* (status[1] of the conditional plan)
+CONS_HDR_INTS = 8                                                   # GIB_CONS_* (include/gib200.h)
+CONS_OVER_MAX, CONS_SMALL_RING, CONS_UNDER_MIN, CONS_DEAD_END = 1, 2, 4, 8
 
 MOL_HDR_WORDS, MOL_WORDS, MOL_ATOM_WORDS = 8, 6, 3                 # GIB_MOL_* (include/gib200.h)
 MOL_DECODES, MOL_KEY_ERROR, MOL_DUPLICATE_BOND = 1, 2, 4
@@ -162,6 +164,10 @@ _PROTOS = {
     "gib_generation_mask_logits": (c_i, [c_i] * 4 + [c_p] * 8),
     "gib_rl_snapshot_scaffold": (c_i, [c_i] * 2 + [c_p] * 7),
     "gib_action_mask_logits": (c_i, [c_i] * 10 + [c_p] * 12 + [c_i, c_p]),
+    "gib_action_mask_logits_constrained": (c_i, [c_i] * 10 + [c_p] * 12 + [c_i, c_p, c_p]),
+    "gib_constraints_ints": (c_sz, [c_i] * 3),
+    "gib_constraints_set": (c_i, [c_p, c_p, c_i, c_i, c_i, c_i, c_p]),
+    "gib_constraints_check": (c_i, [c_i] * 9 + [c_p] * 11),
     "gib_rl_snapshot": (c_i, [c_i] * 5 + [c_p] * 9),
     "gib_rl_restore": (c_i, [c_i] * 4 + [c_p] * 6),
     "gib_rl_gather": (c_i, [c_i] * 3 + [c_p] * 6),

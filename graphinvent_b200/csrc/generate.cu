@@ -34,6 +34,7 @@
 #include "ops.cuh"
 #include "action_mask.cuh"
 #include "scaffold_mask.cuh"
+#include "constraints.cuh"
 
 namespace gib {
 
@@ -348,6 +349,136 @@ __global__ void __launch_bounds__(128) gen_action_mask_kernel(ActionLayout L, in
       o[a] = -INFINITY;
 }
 
+// the inputs of the constrained rule that every CTA of the two kernels below sets up the same way: the atom count,
+// the valence table, the attachment-point mask of the slot's scaffold
+struct ConsSlot {
+  int n, k;
+  const unsigned int* pm;
+};
+
+template <typename T>
+__device__ __forceinline__ ConsSlot cons_slot(const ActionLayout& L, int F, int valence, const int* __restrict__ table,
+                                              const T* __restrict__ nb, const T* __restrict__ e,
+                                              const int* __restrict__ n_nodes, size_t idx, const gib_scaffolds& sc,
+                                              const int* __restrict__ slot_ids, int* s_used, int* s_limit) {
+  ConsSlot r{0, 0, nullptr};
+  const int N = L.N;
+  if (n_nodes) {
+    r.n = min(max(n_nodes[idx], 0), N);
+  } else {
+    int live = 0;
+    if ((int)threadIdx.x < N) {
+      const T* nr = nb + (size_t)threadIdx.x * F;
+      for (int f = 0; f < F; ++f) live |= nr[f] != T(0);
+    }
+    r.n = __syncthreads_count(live);
+  }
+  if (valence) {
+    const int* order = table + L.A * L.CH;
+    for (int i = threadIdx.x; i < r.n; i += 128) {
+      const int2 u = atom_usage(nb + (size_t)i * F, e + (size_t)i * N * L.Ef, L, table, order, order + L.Ef);
+      s_used[i] = u.x;
+      s_limit[i] = u.y;
+    }
+    __syncthreads();
+  }
+  if (sc.protect && slot_ids) {
+    const int s = slot_ids[idx];
+    if (s >= 0 && s < sc.S) {
+      r.pm = sc.protect + (size_t)s * 4;
+      r.k = sc.n_atoms[s];
+    }
+  }
+  return r;
+}
+
+// gen_action_mask_kernel with the constraint rule (constraints.cuh) in the same launch: -inf into every entry any of
+// the rules forbids, and into terminate while the state is under a minimum and some other entry survives (a
+// block-wide OR over the row).  Same arguments and gating, plus the constraint table.
+template <typename T>
+__global__ void __launch_bounds__(128) gen_constrained_mask_kernel(ActionLayout L, int F, int apd, int valence,
+                                                                   const int* __restrict__ table,
+                                                                   const T* __restrict__ nodes,
+                                                                   const T* __restrict__ edges,
+                                                                   const int* __restrict__ n_nodes, gib_scaffolds sc,
+                                                                   const int* __restrict__ slot_ids,
+                                                                   const int* __restrict__ row,
+                                                                   const int* __restrict__ state,
+                                                                   const int* __restrict__ counters,
+                                                                   float* __restrict__ logits, int first_slot,
+                                                                   const int* __restrict__ cons) {
+  __shared__ int s_used[128], s_limit[128];
+  __shared__ ConsState s;
+  const int b = blockIdx.x, B = gridDim.x, N = L.N, Ef = L.Ef;
+  if (b < first_slot) return;
+  if (state && !(counters[0] < B && state[1] == 0 && state[0] >= 0 && state[0] < 2 * N)) return;
+  const size_t off = row ? (size_t)row[0] * B : 0;
+  const T* nb = nodes + (size_t)b * N * F;
+  const T* e = edges + (size_t)b * N * N * Ef;
+  const ConsSlot cs = cons_slot(L, F, valence, table, nb, e, n_nodes ? n_nodes + off : nullptr, b, sc,
+                                slot_ids ? slot_ids + off : nullptr, s_used, s_limit);
+  const ConsTable ct{cons, L.A, L.CH};
+  cons_load(s, ct, L, F, nb, e, cs.n);
+  const int* order = valence ? table + L.A * L.CH : nullptr;
+  const Valence v{s_used, s_limit, valence ? table : nullptr, order, valence ? order + Ef : nullptr};
+  const int per_node = (apd - 1) / N - Ef;
+  float* o = logits + (size_t)b * apd;
+  int survives = 0;
+  for (int a = threadIdx.x; a < apd - 1; a += 128) {
+    if (action_forbidden(a, L, cs.n, e, valence != 0, v) ||
+        (cs.pm && scaffold_forbidden(a, cs.n, cs.k, cs.pm, N, Ef, per_node)) ||
+        cons_forbidden(decode_action(a, L), s, ct))
+      o[a] = -INFINITY;
+    else
+      survives = 1;
+  }
+  if (__syncthreads_or(survives) && s.below && threadIdx.x == 0) o[apd - 1] = -INFINITY;
+}
+
+// gib_constraints_check: one CTA per finished molecule, its flag bits (GIB_CONS_*)
+template <typename T>
+__global__ void __launch_bounds__(128) constraints_check_kernel(ActionLayout L, int F, int apd, int valence,
+                                                                const int* __restrict__ table,
+                                                                const T* __restrict__ nodes,
+                                                                const T* __restrict__ edges,
+                                                                const int* __restrict__ n_nodes, gib_scaffolds sc,
+                                                                const int* __restrict__ scaffold_ids,
+                                                                const int* __restrict__ cons, int* __restrict__ flags) {
+  __shared__ int s_used[128], s_limit[128];
+  __shared__ ConsState s;
+  const int g = blockIdx.x, N = L.N, Ef = L.Ef;
+  const T* nb = nodes + (size_t)g * N * F;
+  const T* e = edges + (size_t)g * N * N * Ef;
+  const ConsSlot cs = cons_slot(L, F, valence, table, nb, e, n_nodes, g, sc, scaffold_ids, s_used, s_limit);
+  const ConsTable ct{cons, L.A, L.CH};
+  cons_load(s, ct, L, F, nb, e, cs.n);
+  int f = cons_over_max(s, ct, L.A, L.CH, Ef) ? GIB_CONS_OVER_MAX : 0;
+  if (s.below) {                       // did its terminate have probability 0?
+    const int* order = valence ? table + L.A * L.CH : nullptr;
+    const Valence v{s_used, s_limit, valence ? table : nullptr, order, valence ? order + Ef : nullptr};
+    const int per_node = (apd - 1) / N - Ef;
+    int survives = 0;
+    for (int a = threadIdx.x; a < apd - 1 && !survives; a += 128)
+      survives = !(action_forbidden(a, L, cs.n, e, valence != 0, v) ||
+                   (cs.pm && scaffold_forbidden(a, cs.n, cs.k, cs.pm, N, Ef, per_node)) ||
+                   cons_forbidden(decode_action(a, L), s, ct));
+    f |= __syncthreads_or(survives) ? GIB_CONS_UNDER_MIN : GIB_CONS_DEAD_END;
+  }
+  // girth < m: some bond (u, v) whose ends are within m - 2 bonds of each other without it
+  const int m = cons[CONS_MIN_RING_SIZE];
+  if (m > 0 && s.rank > 0) {
+    bool small = false;
+    for (int u = 0; u < s.n && !small; ++u)
+      for (int w = u + 1; w < s.n && !small; ++w) {
+        if (!((s.adj[u][w >> 5] >> (w & 31)) & 1u)) continue;
+        cons_bfs(s, u, w, min(m - 2, s.n));
+        small = s.dist[w] <= m - 2;
+      }
+    if (small) f |= GIB_CONS_SMALL_RING;
+  }
+  if (threadIdx.x == 0) flags[g] = f;
+}
+
 }  // namespace gib
 
 using namespace gib;
@@ -615,58 +746,196 @@ extern "C" int gib_route_mask_logits(int B, int N, int Ef, int apd, const gib_sc
   return 0;
 }
 
+// the arguments of the action mask and of the constraint check (`who` names the entry point); *scv receives the
+// scaffold table to apply (empty without attachment points)
+static int check_mask_args(const char* who, int B, int N, int F, int Ef, int n_atom_types, int n_charges, int n_imp_H,
+                           int n_chirality, int apd, int mode, const int* table, const float* nodes,
+                           const float* edges, const signed char* nodes_i8, const signed char* edges_i8,
+                           const gib_scaffolds* sc, const int* slot_ids, gib_scaffolds* scv) {
+  const bool counts_ok = n_atom_types > 0 && n_charges > 0 && Ef > 0 && n_imp_H >= 0 && n_chirality >= 0 &&
+                         n_atom_types <= 255 && n_charges <= 255 && Ef <= 255 && n_imp_H <= 255 && n_chirality <= 255;
+  if (!counts_ok || B <= 0 || N <= 0 || N > 127 || n_atom_types + n_charges + n_imp_H + n_chirality != F) {
+    set_error("%s: unsupported dims (B=%d N=%d F=%d A=%d CH=%d H=%d C=%d Ef=%d; N <= 127, the "
+              "counts lie in 1..255 (0..255 for implicit H / chirality) and F = A + CH + H + C)", who, B, N, F,
+              n_atom_types, n_charges, n_imp_H, n_chirality, Ef);
+    return -1;
+  }
+  const long long want = layout_apd(N, Ef, n_atom_types, n_charges, n_imp_H, n_chirality);
+  if (apd != want || want >= (1ll << 31)) {
+    set_error("%s: apd=%d, the action layout (N=%d A=%d CH=%d H=%d C=%d Ef=%d) has %lld actions",
+              who, apd, N, n_atom_types, n_charges, n_imp_H, n_chirality, Ef, want);
+    return -1;
+  }
+  const bool as_float = nodes && edges, as_i8 = nodes_i8 && edges_i8;
+  const int n_state = !!nodes + !!edges + !!nodes_i8 + !!edges_i8;
+  if ((mode != GIB_ACTION_MASK_STRUCTURE && mode != GIB_ACTION_MASK_VALENCE) || n_state != 2 ||
+      !(as_float || as_i8) || (mode == GIB_ACTION_MASK_VALENCE && !table)) {
+    set_error("%s: bad arguments (mode=%d; mode is GIB_ACTION_MASK_STRUCTURE or GIB_ACTION_MASK_VALENCE, the "
+              "valence mode needs the table, the state is given as float nodes and edges or as int8 nodes and edges)",
+              who, mode);
+    return -1;
+  }
+  *scv = gib_scaffolds{};
+  if (sc && sc->protect) {
+    if (sc->S <= 0 || !sc->n_atoms || !slot_ids) {
+      set_error("%s: a scaffold table with attachment points needs S >= 1, n_atoms and slot_ids", who);
+      return -1;
+    }
+    *scv = *sc;
+  }
+  return 0;
+}
+
+static int action_mask_launch(const char* who, int B, int N, int F, int Ef, int n_atom_types, int n_charges,
+                              int n_imp_H, int n_chirality, int apd, int mode, const int* table, const float* nodes,
+                              const float* edges, const signed char* nodes_i8, const signed char* edges_i8,
+                              const int* n_nodes, const gib_scaffolds* sc, const int* slot_ids, const int* row,
+                              const int* state, const int* counters, float* logits, int first_slot,
+                              gib_stream stream, const int* cons) {
+  gib_scaffolds scv;
+  GIB_TRY(check_mask_args(who, B, N, F, Ef, n_atom_types, n_charges, n_imp_H, n_chirality, apd, mode, table, nodes,
+                          edges, nodes_i8, edges_i8, sc, slot_ids, &scv));
+  if (!logits || (!state != !counters) || (first_slot != 0 && first_slot != 1)) {
+    set_error("%s: bad arguments (first_slot=%d; logits must be given, state and counters together or neither, "
+              "first_slot is 0 or 1)", who, first_slot);
+    return -1;
+  }
+  const ActionLayout L{N, n_atom_types, n_charges, n_imp_H, n_chirality, Ef};
+  const int valence = mode == GIB_ACTION_MASK_VALENCE;
+  const bool as_float = nodes && edges;
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  if (cons) {
+    if (as_float)
+      gen_constrained_mask_kernel<float><<<B, 128, 0, st>>>(L, F, apd, valence, table, nodes, edges, n_nodes, scv,
+                                                            slot_ids, row, state, counters, logits, first_slot, cons);
+    else
+      gen_constrained_mask_kernel<signed char><<<B, 128, 0, st>>>(L, F, apd, valence, table, nodes_i8, edges_i8,
+                                                                  n_nodes, scv, slot_ids, row, state, counters,
+                                                                  logits, first_slot, cons);
+  } else if (as_float) {
+    gen_action_mask_kernel<float><<<B, 128, 0, st>>>(L, F, apd, valence, table, nodes, edges, n_nodes, scv, slot_ids,
+                                                     row, state, counters, logits, first_slot);
+  } else {
+    gen_action_mask_kernel<signed char><<<B, 128, 0, st>>>(L, F, apd, valence, table, nodes_i8, edges_i8, n_nodes,
+                                                           scv, slot_ids, row, state, counters, logits, first_slot);
+  }
+  GIB_LAUNCH_CHECK();
+  return 0;
+}
+
 extern "C" int gib_action_mask_logits(int B, int N, int F, int Ef, int n_atom_types, int n_charges, int n_imp_H,
                                       int n_chirality, int apd, int mode, const int* table, const float* nodes,
                                       const float* edges, const signed char* nodes_i8, const signed char* edges_i8,
                                       const int* n_nodes, const gib_scaffolds* sc, const int* slot_ids,
                                       const int* row, const int* state, const int* counters, float* logits,
                                       int first_slot, gib_stream stream) {
-  const bool counts_ok = n_atom_types > 0 && n_charges > 0 && Ef > 0 && n_imp_H >= 0 && n_chirality >= 0 &&
-                         n_atom_types <= 255 && n_charges <= 255 && Ef <= 255 && n_imp_H <= 255 && n_chirality <= 255;
-  if (!counts_ok || B <= 0 || N <= 0 || N > 127 || n_atom_types + n_charges + n_imp_H + n_chirality != F) {
-    set_error("gib_action_mask_logits: unsupported dims (B=%d N=%d F=%d A=%d CH=%d H=%d C=%d Ef=%d; N <= 127, the "
-              "counts lie in 1..255 (0..255 for implicit H / chirality) and F = A + CH + H + C)", B, N, F,
-              n_atom_types, n_charges, n_imp_H, n_chirality, Ef);
+  return action_mask_launch("gib_action_mask_logits", B, N, F, Ef, n_atom_types, n_charges, n_imp_H, n_chirality,
+                            apd, mode, table, nodes, edges, nodes_i8, edges_i8, n_nodes, sc, slot_ids, row, state,
+                            counters, logits, first_slot, stream, nullptr);
+}
+
+// ---- constraints (constraints.cuh) ----
+extern "C" int gib_action_mask_logits_constrained(int B, int N, int F, int Ef, int n_atom_types, int n_charges,
+                                                  int n_imp_H, int n_chirality, int apd, int mode, const int* table,
+                                                  const float* nodes, const float* edges,
+                                                  const signed char* nodes_i8, const signed char* edges_i8,
+                                                  const int* n_nodes, const gib_scaffolds* sc, const int* slot_ids,
+                                                  const int* row, const int* state, const int* counters,
+                                                  float* logits, int first_slot, gib_stream stream,
+                                                  const int* constraints) {
+  return action_mask_launch("gib_action_mask_logits_constrained", B, N, F, Ef, n_atom_types, n_charges, n_imp_H,
+                            n_chirality, apd, mode, table, nodes, edges, nodes_i8, edges_i8, n_nodes, sc, slot_ids,
+                            row, state, counters, logits, first_slot, stream, constraints);
+}
+
+extern "C" size_t gib_constraints_ints(int n_atom_types, int n_charges, int Ef) {
+  if (n_atom_types <= 0 || n_charges <= 0 || Ef <= 0 || n_atom_types > 255 || n_charges > 255 || Ef > 255) return 0;
+  return (size_t)GIB_CONS_HDR_INTS + 2 * n_atom_types + n_charges + Ef;
+}
+
+extern "C" int gib_constraints_set(int* table, const int* values, int N, int n_atom_types, int n_charges, int Ef,
+                                   gib_stream stream) {
+  const size_t len = gib_constraints_ints(n_atom_types, n_charges, Ef);
+  if (!table || !values || len == 0 || N <= 0 || N > 127) {
+    set_error("gib_constraints_set: refused (table %s, values %s, N=%d A=%d CH=%d Ef=%d; N <= 127 and the counts lie "
+              "in 1..255)", table ? "given" : "null", values ? "given" : "null", N, n_atom_types, n_charges, Ef);
     return -1;
   }
-  const long long want = layout_apd(N, Ef, n_atom_types, n_charges, n_imp_H, n_chirality);
-  if (apd != want || want >= (1ll << 31)) {
-    set_error("gib_action_mask_logits: apd=%d, the action layout (N=%d A=%d CH=%d H=%d C=%d Ef=%d) has %lld actions",
-              apd, N, n_atom_types, n_charges, n_imp_H, n_chirality, Ef, want);
+  const int A = n_atom_types, CH = n_charges;
+  const int* v = values;
+  const int min_atoms = v[GIB_CONS_MIN_ATOMS], max_atoms = v[GIB_CONS_MAX_ATOMS];
+  const int min_rings = v[GIB_CONS_MIN_RINGS], max_rings = v[GIB_CONS_MAX_RINGS], ring = v[GIB_CONS_MIN_RING_SIZE];
+  const int* min_type = v + GIB_CONS_HDR_INTS;
+  const int* max_type = min_type + A;
+  const int* rest = max_type + A;           // max_charge [CH], max_bond [Ef]
+  const char* why = nullptr;
+  int idx = -1;
+  long long sum_min = 0;
+  if (min_atoms < 0 || min_rings < 0 || ring < 0) why = "a minimum or min_ring_size is negative";
+  else if (max_atoms < -1 || max_rings < -1) why = "a maximum is below -1 (-1 = off)";
+  else if (max_atoms > N) why = "max_atoms is over max_n_nodes";
+  else if (min_atoms > N) why = "min_atoms is over max_n_nodes";
+  else if (max_atoms >= 0 && min_atoms > max_atoms) why = "min_atoms is over max_atoms";
+  else if (max_rings >= 0 && min_rings > max_rings) why = "min_rings is over max_rings";
+  else if (ring == 1 || ring == 2) why = "min_ring_size is 1 or 2 (0 = off, a ring has at least 3 atoms)";
+  for (int t = 0; t < A && !why; ++t) {
+    idx = t;
+    if (min_type[t] < 0) why = "min_type is negative";
+    else if (max_type[t] < -1) why = "max_type is below -1 (-1 = off)";
+    else if (max_type[t] >= 0 && min_type[t] > max_type[t]) why = "min_type is over max_type";
+    sum_min += min_type[t];
+  }
+  for (int c = 0; c < CH + Ef && !why; ++c) {
+    idx = c < CH ? c : c - CH;
+    if (rest[c] < -1) why = c < CH ? "max_charge is below -1 (-1 = off)" : "max_bond is below -1 (-1 = off)";
+  }
+  if (!why && sum_min > (max_atoms >= 0 ? max_atoms : N)) {
+    idx = -1;
+    why = "the per-type minima add up to more atoms than max_atoms (or max_n_nodes)";
+  }
+  if (why) {
+    set_error("gib_constraints_set: refused: %s (index %d; min_atoms=%d max_atoms=%d min_rings=%d max_rings=%d "
+              "min_ring_size=%d, N=%d)", why, idx, min_atoms, max_atoms, min_rings, max_rings, ring, N);
     return -1;
   }
-  const bool as_float = nodes && edges, as_i8 = nodes_i8 && edges_i8;
-  const int n_state = !!nodes + !!edges + !!nodes_i8 + !!edges_i8;
-  if ((mode != GIB_ACTION_MASK_STRUCTURE && mode != GIB_ACTION_MASK_VALENCE) || n_state != 2 ||
-      !(as_float || as_i8) || !logits ||
-      (mode == GIB_ACTION_MASK_VALENCE && !table) || (!state != !counters) || (first_slot != 0 && first_slot != 1)) {
-    set_error("gib_action_mask_logits: bad arguments (mode=%d first_slot=%d; mode is GIB_ACTION_MASK_STRUCTURE or "
-              "GIB_ACTION_MASK_VALENCE, the valence mode needs the table, the state is given as float nodes and edges "
-              "or as int8 nodes and edges, logits must be given, state and counters together or neither, "
-              "first_slot is 0 or 1)", mode, first_slot);
+  // staged copy with the layout words filled in; pageable source: the call returns once the value is staged
+  int staged[GIB_CONS_HDR_INTS + 2 * 255 + 255 + 255];
+  for (size_t i = 0; i < len; ++i) staged[i] = v[i];
+  staged[GIB_CONS_N_ATOM_TYPES] = A;
+  staged[GIB_CONS_N_CHARGES] = CH;
+  staged[GIB_CONS_N_BOND_TYPES] = Ef;
+  GIB_CUDA_TRY(cudaMemcpyAsync(table, staged, len * sizeof(int), cudaMemcpyHostToDevice,
+                               reinterpret_cast<cudaStream_t>(stream)));
+  return 0;
+}
+
+extern "C" int gib_constraints_check(int M, int N, int F, int Ef, int n_atom_types, int n_charges, int n_imp_H,
+                                     int n_chirality, int mode, const int* table, const float* nodes,
+                                     const float* edges, const signed char* nodes_i8, const signed char* edges_i8,
+                                     const int* n_nodes, const gib_scaffolds* sc, const int* scaffold_ids,
+                                     const int* constraints, int* flags, gib_stream stream) {
+  if (M == 0) return 0;
+  const long long apd = layout_apd(N, Ef, n_atom_types, n_charges, n_imp_H > 0 ? n_imp_H : 0,
+                                   n_chirality > 0 ? n_chirality : 0);
+  gib_scaffolds scv;
+  GIB_TRY(check_mask_args("gib_constraints_check", M, N, F, Ef, n_atom_types, n_charges, n_imp_H, n_chirality,
+                          (int)apd, mode, table, nodes, edges, nodes_i8, edges_i8, sc, scaffold_ids, &scv));
+  if (!constraints || !flags) {
+    set_error("gib_constraints_check: the constraint table and the flags must be given");
     return -1;
-  }
-  gib_scaffolds scv{};
-  if (sc && sc->protect) {
-    if (sc->S <= 0 || !sc->n_atoms || !slot_ids) {
-      set_error("gib_action_mask_logits: a scaffold table with attachment points needs S >= 1, n_atoms and slot_ids");
-      return -1;
-    }
-    scv = *sc;
   }
   const ActionLayout L{N, n_atom_types, n_charges, n_imp_H, n_chirality, Ef};
   const int valence = mode == GIB_ACTION_MASK_VALENCE;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  if (as_float)
-    gen_action_mask_kernel<float><<<B, 128, 0, st>>>(L, F, apd, valence, table, nodes, edges, n_nodes, scv, slot_ids,
-                                                     row, state, counters, logits, first_slot);
+  if (nodes && edges)
+    constraints_check_kernel<float><<<M, 128, 0, st>>>(L, F, (int)apd, valence, table, nodes, edges, n_nodes, scv,
+                                                       scaffold_ids, constraints, flags);
   else
-    gen_action_mask_kernel<signed char><<<B, 128, 0, st>>>(L, F, apd, valence, table, nodes_i8, edges_i8, n_nodes,
-                                                           scv, slot_ids, row, state, counters, logits, first_slot);
+    constraints_check_kernel<signed char><<<M, 128, 0, st>>>(L, F, (int)apd, valence, table, nodes_i8, edges_i8,
+                                                             n_nodes, scv, scaffold_ids, constraints, flags);
   GIB_LAUNCH_CHECK();
   return 0;
 }
-
 extern "C" int gib_generation_round(int B, int N, int F, int Ef, int n_atom_types, int n_charges, int round,
                                     const int* action, const float* likelihood, float* nodes, float* edges,
                                     int* n_nodes, float* likelihoods, float* gen_nodes, float* gen_edges,

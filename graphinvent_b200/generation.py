@@ -164,6 +164,160 @@ class ScaffoldTable:
 
 
 ACTION_MASK_MODES = {"structure": 1, "valence": 2}          # GIB_ACTION_MASK_* (include/gib200.h)
+CONS_OFF = -1                                                   # a maximum's "off" value in the constraint table
+
+
+def _bound(v, what, min_only=False, max_only=False):
+    """(min, max) of a bound given as (min, max) (None = off) or, for a maximum-only field, as an int"""
+    if v is None:
+        return 0, CONS_OFF
+    if isinstance(v, (int, np.integer)) and not isinstance(v, bool) and max_only:
+        v = (None, int(v))
+    try:
+        lo, hi = v
+    except (TypeError, ValueError):
+        raise ValueError(f"{what} must be a (min, max) pair (None = no bound), got {v!r}") from None
+    for x in (lo, hi):
+        if x is not None and (isinstance(x, bool) or not isinstance(x, (int, np.integer)) or x < 0):
+            raise ValueError(f"{what}: bounds are non-negative ints or None, got {v!r}")
+    if max_only and lo not in (None, 0):
+        raise ValueError(f"{what} has a maximum only, got a minimum of {lo}")
+    lo, hi = int(lo or 0), CONS_OFF if hi is None else int(hi)
+    if hi != CONS_OFF and lo > hi:
+        raise ValueError(f"{what}: the minimum {lo} is over the maximum {hi}")
+    return lo, hi
+
+
+class Constraints:
+    """What a generated molecule may contain, applied as a mask on the actions (`constraints=`; the rule is
+    graphinvent_b200/csrc/constraints.cuh).  Each argument is optional; None is no bound:
+
+        Constraints(atoms=(9, 13), atom_types={"N": (1, None), "S": (0, 0)}, charges={1: 0}, bonds={"TRIPLE": 0},
+                    rings=(0, 2), min_ring_size=5)
+
+    atoms / rings: (min, max) atom count / cycle rank (bonds - atoms + 1, the number of rings a route closes);
+    atom_types: {type: (min, max)}; charges: {formal charge: max} and bonds: {bond type: max} (maxima only);
+    min_ring_size: no ring shorter than this (>= 3), i.e. no connect that closes one.
+    Keys are resolved through the reference's constants (`atom_types`, `formal_charge`, `int_to_bondtype`, or the bond
+    names SINGLE / DOUBLE / TRIPLE / AROMATIC in that order without it); integer keys are indices when no constants
+    are given (charge keys are formal charges when `constants.formal_charge` is there).  Maxima forbid the adds and
+    connects that would pass them; minima forbid terminate while the molecule is below them, unless no other action
+    is allowed (a dead end: the molecule then ends under its minimum).  Bad values raise ValueError here or, for those
+    that depend on the layout (max_atoms over max_n_nodes, minima adding up past max_atoms), in `table`."""
+
+    def __init__(self, atoms=None, atom_types=None, charges=None, bonds=None, rings=None, min_ring_size=None,
+                 constants=None):
+        self.atoms, self.rings = _bound(atoms, "atoms"), _bound(rings, "rings")
+        self.atom_types = {k: _bound(v, f"atom_types[{k!r}]") for k, v in dict(atom_types or {}).items()}
+        self.charges = {k: _bound(v, f"charges[{k!r}]", max_only=True)[1] for k, v in dict(charges or {}).items()}
+        self.bonds = {k: _bound(v, f"bonds[{k!r}]", max_only=True)[1] for k, v in dict(bonds or {}).items()}
+        m = 0 if min_ring_size is None else min_ring_size
+        if isinstance(m, bool) or not isinstance(m, (int, np.integer)) or m < 0 or m in (1, 2):
+            raise ValueError(f"min_ring_size must be None / 0 (off) or an int >= 3, got {min_ring_size!r}")
+        self.min_ring_size = int(m)
+        self.constants = constants
+        self._mask = None                                   # the ActionMask this set is bound to (check())
+
+    def _key(self):
+        return (self.atoms, self.rings, sorted(self.atom_types.items(), key=repr),
+                sorted(self.charges.items(), key=repr), sorted(self.bonds.items(), key=repr), self.min_ring_size)
+
+    def __eq__(self, other):
+        return isinstance(other, Constraints) and self._key() == other._key()
+
+    def __repr__(self):
+        return (f"Constraints(atoms={self.atoms}, atom_types={self.atom_types}, charges={self.charges}, "
+                f"bonds={self.bonds}, rings={self.rings}, min_ring_size={self.min_ring_size})")
+
+    @property
+    def off(self):
+        """True when no field bounds anything (the mask is then the unconstrained one, bit for bit)"""
+        return (self.atoms == (0, CONS_OFF) and self.rings == (0, CONS_OFF) and not self.min_ring_size
+                and all(v == (0, CONS_OFF) for v in self.atom_types.values())
+                and all(v == CONS_OFF for v in self.charges.values())
+                and all(v == CONS_OFF for v in self.bonds.values()))
+
+    def values(self, layout, N, n_edge_features, constants=None):
+        """the table's words (int32 numpy, include/gib200.h GIB_CONS_*) for the layout (A, CH, H, C), max_n_nodes N and
+        Ef bond types"""
+        A, CH = int(layout[0]), int(layout[1])
+        Ef = int(n_edge_features)
+        C = self.constants if self.constants is not None else constants      # the set's own constants first
+        t = np.zeros(8 + 2 * A + CH + Ef, np.int32)
+        t[0], t[1] = self.atoms
+        t[2], t[3] = self.rings
+        t[4] = self.min_ring_size
+        t[8 + A:8 + 2 * A] = CONS_OFF
+        t[8 + 2 * A:] = CONS_OFF
+        for k, (lo, hi) in self.atom_types.items():
+            i = _index(k, "atom type", A, getattr(C, "atom_types", None))
+            t[8 + i], t[8 + A + i] = lo, hi
+        charges = getattr(C, "formal_charge", None)
+        for k, hi in self.charges.items():
+            t[8 + 2 * A + _index(k, "formal charge", CH, charges, by_value=charges is not None)] = hi
+        names = _bond_names(C, Ef)
+        for k, hi in self.bonds.items():
+            key = k.upper() if isinstance(k, str) else k
+            t[8 + 2 * A + CH + _index(key, "bond type", Ef, names)] = hi
+        if t[1] != CONS_OFF and t[1] > N:
+            raise ValueError(f"atoms: the maximum {int(t[1])} is over max_n_nodes = {N}")
+        if t[0] > N:
+            raise ValueError(f"atoms: the minimum {int(t[0])} is over max_n_nodes = {N}")
+        cap = N if t[1] == CONS_OFF else int(t[1])
+        if int(t[8:8 + A].sum()) > cap:
+            raise ValueError(f"atom_types: the minima add up to {int(t[8:8 + A].sum())} atoms, more than "
+                             f"{'max_n_nodes' if t[1] == CONS_OFF else 'the maximum atom count'} {cap}")
+        return t
+
+    def table(self, layout, N, device, n_edge_features=None, constants=None):
+        """the device table (int32, written by `gib_constraints_set`, which checks it again) for the layout (A, CH, H,
+        C), max_n_nodes N and n_edge_features bond types (default: `constants.n_edge_features`)"""
+        C = self.constants if self.constants is not None else constants      # the set's own constants first
+        Ef = n_edge_features if n_edge_features is not None else getattr(C, "n_edge_features", None)
+        if Ef is None:
+            raise ValueError("Constraints.table needs n_edge_features (or constants with n_edge_features)")
+        vals = self.values(layout, N, Ef, C)
+        out = torch.empty(vals.size, dtype=torch.int32, device=torch.device(device))
+        check(lib.gib_constraints_set(_ptr(out), vals.ctypes.data_as(ctypes.c_void_p), int(N), int(layout[0]),
+                                      int(layout[1]), int(Ef), torch.cuda.current_stream(out.device).cuda_stream),
+              "gib_constraints_set")
+        return out
+
+    def check(self, nodes, edges, n_nodes=None, scaffold_ids=None):
+        """int32 flags [M] on the device of finished molecules nodes [M, N, F] / edges [M, N, N, Ef] (float or int8,
+        device tensors) with atom counts n_nodes [M] (None: the non-empty node rows), judged with the action mask of
+        the generator or scorer this set belongs to (`gen.constraints.check(...)`): bit 1 over a maximum, 2 a ring
+        shorter than min_ring_size, 4 under a minimum while another action was allowed (probability 0), 8 under a
+        minimum at a dead end (allowed).  scaffold_ids [M]: the molecules' scaffolds, for the attachment points of a
+        scaffold generator."""
+        if self._mask is None:
+            raise ValueError("this Constraints is not bound to a generator or scorer: use gen.constraints.check(...) "
+                             "or make one with make_action_mask(..., constraints=)")
+        return self._mask.check(nodes, edges, n_nodes, scaffold_ids)
+
+
+def _index(k, what, n, names, by_value=False):
+    """index of key k among n entries: a name (or a value, by_value) looked up in `names`, or an int index"""
+    if names is not None and (by_value or isinstance(k, str)):
+        lst = [str(x) if isinstance(k, str) else x for x in names]
+        if k not in lst:
+            raise ValueError(f"unknown {what} {k!r} (the constants list {list(names)})")
+        i = lst.index(k)
+    elif isinstance(k, (int, np.integer)) and not isinstance(k, bool):
+        i = int(k)
+    else:
+        raise ValueError(f"{what} {k!r}: names need constants; give an integer index instead")
+    if not 0 <= i < n:
+        raise ValueError(f"{what} index {i} outside the layout's 0..{n - 1}")
+    return i
+
+
+def _bond_names(C, Ef):
+    from .config import _bond_name
+    itb = getattr(C, "int_to_bondtype", None)
+    if itb is not None and len(itb) == Ef:
+        return [_bond_name(itb[i]) for i in range(Ef)]
+    return ["SINGLE", "DOUBLE", "TRIPLE", "AROMATIC"][:Ef] if Ef <= 4 else None
 
 
 class ActionMask:
@@ -172,9 +326,13 @@ class ActionMask:
     exist, a self loop, a bond that exists, an add into a full graph, ...), and with "valence" also every bond that
     takes an atom past its limit in the table of `config.action_rule_table(max_valence=...)`.  Terminate is never
     masked.  The rule is graphinvent_b200/csrc/action_mask.cuh, the one the round's decode kernel flags invalid
-    actions with."""
+    actions with.
 
-    def __init__(self, mode, max_valence, constants, layout, N, F, Ef, apd, device):
+    With `constraints` (a `Constraints`) the constraint rule runs in the same launch
+    (`gib_action_mask_logits_constrained`), from a device table that `set_constraints` rewrites in place: its minima
+    are the only rule that masks terminate."""
+
+    def __init__(self, mode, max_valence, constants, layout, N, F, Ef, apd, device, constraints=None):
         if mode not in ACTION_MASK_MODES:
             raise ValueError(f"action_mask must be None, 'structure' or 'valence', got {mode!r}")
         if max_valence is not None and mode != "valence":
@@ -184,12 +342,33 @@ class ActionMask:
         from .config import action_rule_table
         self.mode, self.code = mode, ACTION_MASK_MODES[mode]
         self.layout, self.N, self.F, self.Ef, self.apd = tuple(layout), N, F, Ef, apd
+        self.constants, self.device = constants, torch.device(device)
         self.valence, self.bond_orders, self.imp_h, self.table = None, None, None, None
         if mode == "valence":
             A, CH, H, _ = layout
             self.valence, self.bond_orders, self.imp_h = action_rule_table(A, CH, Ef, H, max_valence, constants)
             flat = np.concatenate([self.valence.ravel(), self.bond_orders, self.imp_h]).astype(np.int32)
             self.table = torch.from_numpy(flat).to(torch.device(device))
+        self.constraints, self.cons_table = None, None
+        if constraints is not None:
+            self.set_constraints(constraints)
+
+    def set_constraints(self, constraints):
+        """`constraints` into the device table, in place (allocated by the first call)"""
+        if not isinstance(constraints, Constraints):
+            raise TypeError(f"constraints must be a generation.Constraints, got {type(constraints).__name__}")
+        vals = constraints.values(self.layout, self.N, self.Ef, self.constants)
+        if self.cons_table is None:
+            self.cons_table = torch.zeros(vals.size, dtype=torch.int32, device=self.device)
+        check(lib.gib_constraints_set(_ptr(self.cons_table), vals.ctypes.data_as(ctypes.c_void_p), self.N,
+                                      self.layout[0], self.layout[1], self.Ef,
+                                      torch.cuda.current_stream(self.device).cuda_stream), "gib_constraints_set")
+        bound = Constraints.__new__(Constraints)
+        bound.__dict__.update(constraints.__dict__)
+        bound._mask = self
+        if bound.constants is None:
+            bound.constants = self.constants
+        self.constraints = bound
 
     def apply(self, B, logits, n_nodes, stream, nodes=None, edges=None, int8=False, sc=None, slot_ids=None, row=None,
               state=None, counters=None, first_slot=1):
@@ -197,19 +376,56 @@ class ActionMask:
         with attachment points) and slot_ids: that rule too, in the same launch"""
         p = lambda t: _ptr(t) if t is not None else None
         fl = (p(nodes), p(edges), None, None) if not int8 else (None, None, p(nodes), p(edges))
-        check(lib.gib_action_mask_logits(
-            B, self.N, self.F, self.Ef, *self.layout, self.apd, self.code, p(self.table), *fl, p(n_nodes),
-            ctypes.byref(sc) if sc is not None else None, p(slot_ids), p(row), p(state), p(counters), _ptr(logits),
-            first_slot, stream), "gib_action_mask_logits")
+        args = (B, self.N, self.F, self.Ef, *self.layout, self.apd, self.code, p(self.table), *fl, p(n_nodes),
+                ctypes.byref(sc) if sc is not None else None, p(slot_ids), p(row), p(state), p(counters),
+                _ptr(logits), first_slot, stream)
+        if self.cons_table is not None:
+            check(lib.gib_action_mask_logits_constrained(*args, _ptr(self.cons_table)),
+                  "gib_action_mask_logits_constrained")
+        else:
+            check(lib.gib_action_mask_logits(*args), "gib_action_mask_logits")
+
+    def check(self, nodes, edges, n_nodes=None, scaffold_ids=None, sc=None, out=None, stream=None):
+        """`gib_constraints_check` of finished molecules: int32 flags [M] on the device (`Constraints.check`)"""
+        if self.cons_table is None:
+            raise ValueError("no constraints are set")
+        M = nodes.shape[0]
+        if (not (nodes.is_cuda and edges.is_cuda) or nodes.dtype != edges.dtype
+                or nodes.dtype not in (torch.float32, torch.int8)
+                or tuple(nodes.shape[1:]) != (self.N, self.F) or tuple(edges.shape) != (M, self.N, self.N, self.Ef)):
+            raise ValueError(f"nodes / edges must be float32 or int8 device tensors [M, {self.N}, {self.F}] / "
+                             f"[M, {self.N}, {self.N}, {self.Ef}], got {nodes.dtype} {tuple(nodes.shape)} / "
+                             f"{edges.dtype} {tuple(edges.shape)}")
+        nodes, edges = nodes.contiguous(), edges.contiguous()
+        cnt = n_nodes.to(device=nodes.device, dtype=torch.int32).contiguous() if n_nodes is not None else None
+        ids = None
+        if scaffold_ids is not None:
+            ids = torch.as_tensor(scaffold_ids).to(device=nodes.device, dtype=torch.int32).contiguous()
+        flags = out if out is not None else torch.zeros(M, dtype=torch.int32, device=nodes.device)
+        p = lambda t: _ptr(t) if t is not None else None
+        i8 = nodes.dtype == torch.int8
+        fl = (None, None, _ptr(nodes), _ptr(edges)) if i8 else (_ptr(nodes), _ptr(edges), None, None)
+        st = stream if stream is not None else torch.cuda.current_stream(nodes.device).cuda_stream
+        check(lib.gib_constraints_check(M, self.N, self.F, self.Ef, *self.layout, self.code, p(self.table), *fl,
+                                        p(cnt), ctypes.byref(sc) if sc is not None else None,
+                                        p(ids) if sc is not None else None, _ptr(self.cons_table), _ptr(flags), st),
+              "gib_constraints_check")
+        return flags
 
 
-def make_action_mask(mode, max_valence, constants, layout, N, F, Ef, apd, device):
-    """the ActionMask of a constructor's `action_mask=` / `max_valence=` (None for None)"""
+def make_action_mask(mode, max_valence, constants, layout, N, F, Ef, apd, device, constraints=None):
+    """the ActionMask of a constructor's `action_mask=` / `max_valence=` / `constraints=` (None when all are None).
+    Constraints without an action mask bring the structural rule with them: once a minimum masks terminate, the
+    probability has to go to actions the round accepts, not to ones it would end as invalid."""
+    if constraints is not None and not isinstance(constraints, Constraints):
+        raise TypeError(f"constraints must be a generation.Constraints, got {type(constraints).__name__}")
     if mode is None:
         if max_valence is not None:
             raise ValueError("max_valence needs action_mask='valence'")
-        return None
-    return ActionMask(mode, max_valence, constants, layout, N, F, Ef, apd, device)
+        if constraints is None:
+            return None
+        mode = "structure"
+    return ActionMask(mode, max_valence, constants, layout, N, F, Ef, apd, device, constraints)
 
 
 def scaffold_table(scaffolds, attachment, N, F, Ef, layout, device):
@@ -234,11 +450,17 @@ class GraphGenerator:
     them): draw each action from the model's softmax at that temperature, cut to the top_k most likely actions and to
     the smallest set of them holding top_p of their probability (after the masks).  Only the draw changes: the
     recorded likelihoods stay the model's probabilities of the drawn actions.  The default (1, 0, 1) is the model's
-    softmax itself.  In `GraphGeneratorRL` the policy applies to the agent's draw."""
+    softmax itself.  In `GraphGeneratorRL` the policy applies to the agent's draw.
+
+    `constraints=` (`Constraints`; `set_constraints` changes them, `constraints` reads them): sample only molecules
+    within atom-count, element, charge, bond-type and ring budgets -- the maxima mask the actions that would pass them,
+    the minima mask terminate while a molecule is below them, unless nothing else is allowed.  Without `action_mask=`
+    the structural rule comes with them.  The likelihoods stay the model's masked-softmax probabilities, and the
+    sampling policy acts after all masks.  `gen.constraints.check(nodes, edges, n_nodes)` flags finished molecules."""
 
     def __init__(self, model, batch_size, constants=None, n_atom_types=None, n_formal_charge=None, n_imp_H=None,
                  n_chirality=None, device="cuda", scaffolds=None, attachment=None, action_mask=None,
-                 max_valence=None, temperature=1.0, top_k=0, top_p=1.0):
+                 max_valence=None, temperature=1.0, top_k=0, top_p=1.0, constraints=None):
         self._sampling = Fn.sampling_policy(temperature, top_k, top_p)
         C, self.A, self.CH, self.n_imp_H, self.n_chirality = action_layout(
             model, constants, n_atom_types, n_formal_charge, n_imp_H, n_chirality)
@@ -249,8 +471,9 @@ class GraphGenerator:
         self.rounds = 0
         self.scaffolds = None
         self.generated_scaffolds = None
+        self._mask_args, self.constraints_version = (action_mask, max_valence), 0
         self.action_mask = make_action_mask(action_mask, max_valence, C, self.layout, self.N, self.F, self.Ef, self.apd,
-                                            self.device)
+                                            self.device, constraints)
         self._allocate()
         if scaffolds is not None:
             self.set_scaffolds(scaffolds, attachment)
@@ -258,6 +481,29 @@ class GraphGenerator:
     @property
     def layout(self):
         return (self.A, self.CH, self.n_imp_H, self.n_chirality)
+
+    @property
+    def constraints(self):
+        """the constraint set of the following batches (`Constraints`, bound to this generator's mask for `check`),
+        or None"""
+        return self.action_mask.constraints if self.action_mask is not None else None
+
+    def set_constraints(self, constraints=None):
+        """the constraint set of the following batches (None: none).  A generator that already has a constraint table
+        rewrites it in place; otherwise the mask is rebuilt (a captured generator captures its round again, once)."""
+        if constraints is not None and not isinstance(constraints, Constraints):
+            raise TypeError(f"constraints must be a generation.Constraints, got {type(constraints).__name__}")
+        m = self.action_mask
+        if constraints is not None and m is not None and m.cons_table is not None:
+            m.set_constraints(constraints)
+        else:
+            self.action_mask = make_action_mask(*self._mask_args, self.constants, self.layout, self.N, self.F, self.Ef,
+                                                self.apd, self.device, constraints)
+            self._masks_rebuilt()
+        self.constraints_version += 1
+
+    def _masks_rebuilt(self):
+        """the action mask object was replaced (captured subclasses capture again)"""
 
     @property
     def sampling(self):

@@ -86,8 +86,9 @@ import torch
 
 from . import functional as F
 from .config import matmul_code
-from ._lib import (FLAG_MULTITYPE, FLAG_OVERFLOW, HDR_FLAGS, HDR_INTS, PP_STATUS_INTS, ROUTE_ACTION, ROUTE_BAD_ID,
-                   ROUTE_MASKED, ROUTE_NOT_PREFIX, EvalPass, check, lib)
+from ._lib import (CONS_OVER_MAX, CONS_SMALL_RING, CONS_UNDER_MIN, FLAG_MULTITYPE, FLAG_OVERFLOW, HDR_FLAGS,
+                   HDR_INTS, PP_STATUS_INTS, ROUTE_ACTION, ROUTE_BAD_ID, ROUTE_MASKED, ROUTE_NOT_PREFIX, EvalPass, check,
+                   lib)
 from .generation import GraphGenerator
 
 _u8 = torch.uint8
@@ -656,15 +657,20 @@ class GraphedGenerator(GraphGenerator):
     with one, the round samples with `gib_generation_sample_round_policy`, which reads the policy from a device struct
     on every replay, so `set_sampling` between batches only rewrites that struct.  Built without one (or with the
     default (1, 0, 1)) the round keeps today's sampler; the first `set_sampling` to another policy makes the next batch
-    capture the round once more, and later ones reuse it.  The likelihoods stay the model's."""
+    capture the round once more, and later ones reuse it.  The likelihoods stay the model's.
+
+    Constraints (`constraints=`, `set_constraints`, see `generation.GraphGenerator`): the round's mask launch reads
+    the constraint table from device memory on every replay, so `set_constraints` on a generator built with
+    constraints rewrites that table only; on one built without them (or to None) it rebuilds the mask and the next
+    batch captures the round again, once."""
 
     def __init__(self, model, batch_size, constants=None, n_atom_types=None, n_formal_charge=None, n_imp_H=None,
                  n_chirality=None, device="cuda", scaffolds=None, attachment=None, action_mask=None,
-                 max_valence=None, temperature=1.0, top_k=0, top_p=1.0):
+                 max_valence=None, temperature=1.0, top_k=0, top_p=1.0, constraints=None):
         super().__init__(model, batch_size, constants=constants, n_atom_types=n_atom_types,
                          n_formal_charge=n_formal_charge, n_imp_H=n_imp_H, n_chirality=n_chirality, device=device,
                          action_mask=action_mask, max_valence=max_valence, temperature=temperature, top_k=top_k,
-                         top_p=top_p)
+                         top_p=top_p, constraints=constraints)
         if not hasattr(model, "dims"):
             raise TypeError("GraphedGenerator runs this package's models (graphinvent_b200.gnn.mpnn) only")
         B, N, dev = self.batch_size, self.N, self.device
@@ -715,6 +721,9 @@ class GraphedGenerator(GraphGenerator):
 
     def _invalidate_rounds(self):
         self.graph = None
+
+    def _masks_rebuilt(self):
+        self._invalidate_graphs()
 
     def _sample_round_fn(self, plain, scaffold):
         """(entry point, name, leading scaffold args, trailing policy args) of the round's sampler"""
@@ -960,15 +969,19 @@ class GraphedGeneratorRL(GraphedGenerator):
     The sampling policy (`temperature=`, `top_k=`, `top_p=`, `set_sampling`, as `GraphedGenerator`) applies to the
     agent's draw only (`gib_rl_sample_round_policy`); p_a / p_b stay the two models' probabilities of the drawn action,
     so the log-likelihoods, the loss and the recomputing backward are unchanged.  Recorded `actions=` are replayed as
-    they are."""
+    they are.
+
+    With `constraints=` the constraint rule runs in the action mask's launch, in the rollout and in the backward
+    round, which reads the constraint table as it is then: a `set_constraints` between a rollout and its backward
+    makes that backward raise."""
 
     def __init__(self, model, batch_size, constants=None, n_atom_types=None, n_formal_charge=None, n_imp_H=None,
                  n_chirality=None, device="cuda", scaffolds=None, attachment=None, action_mask=None,
-                 max_valence=None, temperature=1.0, top_k=0, top_p=1.0):
+                 max_valence=None, temperature=1.0, top_k=0, top_p=1.0, constraints=None):
         GraphGenerator.__init__(self, model, batch_size, constants=constants, n_atom_types=n_atom_types,
                                 n_formal_charge=n_formal_charge, n_imp_H=n_imp_H, n_chirality=n_chirality,
                                 device=device, action_mask=action_mask, max_valence=max_valence,
-                                temperature=temperature, top_k=top_k, top_p=top_p)
+                                temperature=temperature, top_k=top_k, top_p=top_p, constraints=constraints)
         if not hasattr(model, "dims"):
             raise TypeError("GraphedGeneratorRL runs this package's models (graphinvent_b200.gnn.mpnn) only")
         B, N, dev = self.batch_size, self.N, self.device
@@ -1024,6 +1037,11 @@ class GraphedGeneratorRL(GraphedGenerator):
 
     def _invalidate_rounds(self):
         self.graph, self._graphs = None, {}
+
+    def _masks_rebuilt(self):
+        self._invalidate_graphs()
+        if self.action_mask is not None and getattr(self, "rec_n", None) is None:
+            self.rec_n = torch.zeros(2 * self.N, self.batch_size, dtype=torch.int32, device=self.device)
 
     def set_scaffolds(self, scaffolds, attachment=None):
         GraphedGenerator.set_scaffolds(self, scaffolds, attachment)
@@ -1143,6 +1161,9 @@ class GraphedGeneratorRL(GraphedGenerator):
         if rec.scaffold_version != self.scaffold_version:
             raise RuntimeError("set_scaffolds was called between an RL rollout and its backward: the backward would "
                                "mask the recomputed logits with other scaffolds")
+        if rec.constraints_version != self.constraints_version:
+            raise RuntimeError("set_constraints was called between an RL rollout and its backward: the backward would "
+                               "mask the recomputed logits with other constraints")
         self._ensure_backward()
         b = self._bwd
         self.backward_rounds = [0, 0]
@@ -1206,7 +1227,8 @@ class GraphedGeneratorRL(GraphedGenerator):
         B, R = self.batch_size, self.rounds
         pa, pb = list(agent.parameters()), list(prior.parameters())
         rec = types.SimpleNamespace(owner=self.generated_likelihoods.clone(), p_a=self.p_a[:R].clone(),
-                                    p_b=self.p_b[:R].clone(), rounds=R, scaffold_version=self.scaffold_version)
+                                    p_b=self.p_b[:R].clone(), rounds=R, scaffold_version=self.scaffold_version,
+                                    constraints_version=self.constraints_version)
         if torch.is_grad_enabled() and any(p.requires_grad for p in pa + pb):
             self._ensure_backward()
             rec.nodes, rec.edges, rec.act = self.rec_nodes[:R].clone(), self.rec_edges[:R].clone(), self.act_rec[:R].clone()
@@ -1363,11 +1385,19 @@ class RouteScorer:
     non-empty node rows), with the attachment points in the same launch; the backward masks the
     recomputed logits the same way.  Per chunk the plan is checked by `gib_route_check_actions`, and a molecule whose
     route takes a forbidden action -- with "valence", any molecule with an atom over its limit -- is refused by name
-    before its chunk is scored."""
+    before its chunk is scored.
+
+    `constraints=` (`generation.Constraints`, `set_constraints`): p(molecule) under the constrained generator.  The
+    constraint rule runs in the action mask's launch (`gib_action_mask_logits_constrained`, forward and backward), and
+    per chunk `gib_constraints_check` judges the molecules: one over a maximum, with a ring shorter than
+    min_ring_size, or under a minimum while its last state allowed another action -- a route of probability 0 -- is
+    refused by name before its chunk is scored.  The maxima and the ring-size bound do not depend on the route
+    (graphinvent_b200/csrc/constraints.cuh), so the check needs only the molecule.  A scaffold's own atoms, bonds and
+    rings count toward the bounds.  A `set_constraints` between `score()` and its backward makes the backward raise."""
 
     def __init__(self, model, batch_size, constants=None, n_atom_types=None, n_formal_charge=None, n_imp_H=None,
                  n_chirality=None, chunk_molecules=4096, device=None, scaffolds=None, attachment=None,
-                 action_mask=None, max_valence=None):
+                 action_mask=None, max_valence=None, constraints=None):
         from .generation import action_layout
         from ._lib import PPDims
         C, A, CH, H, X = action_layout(model, constants, n_atom_types, n_formal_charge, n_imp_H, n_chirality)
@@ -1387,7 +1417,10 @@ class RouteScorer:
         self.apd = N * (C.len_f_add_per_node + C.len_f_conn_per_node) + 1
         self.chunk = chunk = max(1, int(chunk_molecules))
         from .generation import make_action_mask
-        self.action_mask = make_action_mask(action_mask, max_valence, C, self.layout, N, F_, Ef, self.apd, dev)
+        self._mask_args, self.constraints_version = (action_mask, max_valence), 0
+        self.action_mask = make_action_mask(action_mask, max_valence, C, self.layout, N, F_, Ef, self.apd, dev,
+                                            constraints)
+        self.cons_flags = torch.zeros(chunk, dtype=torch.int32, device=dev)
         self.pp = PPDims(N=N, F=F_, Ef=Ef, n_atom_types=A, n_formal_charge=CH, n_imp_H=H, n_chirality=X, batch_size=B)
         pd = ctypes.byref(self.pp)
         ws_bytes, max_states = lib.gib_route_plan_ws_bytes(pd, chunk), lib.gib_route_max_states(pd, chunk)
@@ -1449,6 +1482,41 @@ class RouteScorer:
     def masked(self):
         """True when the scaffolds' attachment points restrict the actions"""
         return self.scaffolds is not None and self.scaffolds.protect is not None
+
+    # ---- constraints ----------------------------------------------------------------------------------------
+    @property
+    def constraints(self):
+        """the constraint set the routes are scored under (`generation.Constraints`), or None"""
+        return self.action_mask.constraints if self.action_mask is not None else None
+
+    def set_constraints(self, constraints=None):
+        """score under `constraints` from the next score() on (None: none).  In place when the scorer already has a
+        constraint table; otherwise the mask is rebuilt and the graphs are captured again."""
+        from .generation import Constraints, make_action_mask
+        if constraints is not None and not isinstance(constraints, Constraints):
+            raise TypeError(f"constraints must be a generation.Constraints, got {type(constraints).__name__}")
+        m = self.action_mask
+        if constraints is not None and m is not None and m.cons_table is not None:
+            m.set_constraints(constraints)
+        else:
+            self.action_mask = make_action_mask(*self._mask_args, self.constants, self.layout, self.N, self.F,
+                                                self.Ef, self.apd, self.dev, constraints)
+            self.graph, self._sgraph, self._bwd = None, None, None
+        self.constraints_version += 1
+
+    def _refuse_constraints(self, n, pos, stop):
+        """the ValueError naming the first molecule of the chunk whose route has probability 0 under the constraints"""
+        flags = self.cons_flags[:n].cpu().numpy()
+        bad = np.flatnonzero(flags & (CONS_OVER_MAX | CONS_SMALL_RING | CONS_UNDER_MIN))
+        if not bad.size:
+            return
+        f = int(flags[bad[0]])
+        why = [w for bit, w in ((CONS_OVER_MAX, "it is over a maximum"),
+                                (CONS_SMALL_RING, "it has a ring shorter than min_ring_size"),
+                                (CONS_UNDER_MIN, "it is under a minimum while its last state allowed another action"))
+               if f & bit]
+        raise ValueError(f"molecule {pos + int(bad[0])} (of molecules [{pos}, {stop})): its route has probability 0 "
+                         f"under the constraints: {'; '.join(why)}")
 
     def _scaffold_ids(self, ids, M):
         """scaffold_ids as a contiguous int32 tensor where it came from, checked against the table"""
@@ -1611,6 +1679,9 @@ class RouteScorer:
     def _backward(self, rec, lik, params, g_lik, g_nll, g_final):
         """gradients of sum(g_lik * likelihoods + g_nll * nll + g_final * final) of one record w.r.t. `params` (None
         gradients count as zero), as views of a fresh bucket"""
+        if rec.constraints_version != self.constraints_version:
+            raise RuntimeError("set_constraints was called between RouteScorer.score() and its backward: the backward "
+                               "would mask the recomputed states with other constraints")
         b = self._bwd
         if b is None:                               # M = 0: no state, no backward buffers
             return F._bucket_views(torch.zeros(sum(p.numel() for p in params), device=self.dev), params)
@@ -1654,7 +1725,8 @@ class RouteScorer:
         # chunk's states
         rec = types.SimpleNamespace(nodes=nodes.clone(), edges=edges.clone(), chunks=[],
                                     ids=ids.clone() if ids is not None else None,
-                                    scaffold_version=self.scaffold_version)
+                                    scaffold_version=self.scaffold_version,
+                                    constraints_version=self.constraints_version)
         return RouteScores(*_RouteLikelihoods.apply(self, rec.nodes, rec.edges, rec, *params))
 
     def _plan(self, n, ids, st):
@@ -1678,6 +1750,10 @@ class RouteScorer:
                                               F._ptr(self.plan_ws), F._ptr(self.offsets), m.code,
                                               F._ptr(m.table) if m.table is not None else None,
                                               F._ptr(self.status[PP_STATUS_INTS:]), st), "gib_route_check_actions")
+            if m.cons_table is not None:
+                masked = ids is not None and self.masked
+                m.check(self.in_nodes[:n], self.in_edges[:n], None, self.in_ids[:n] if masked else None,
+                        sc=self.scaffolds.struct() if masked else None, out=self.cons_flags[:n], stream=st)
 
     def _score(self, nodes, edges, rec=None, ids=None):
         """the forward of score(); `rec`: the backward record whose chunk list (first molecule, first state,
@@ -1712,6 +1788,8 @@ class RouteScorer:
                 m = pos + int(status[PP_STATUS_INTS + 1])
                 raise ValueError(f"molecule {m} (or a later one in molecules [{pos}, {stop})): "
                                  + dict(_ROUTE_REASONS)[ROUTE_ACTION])
+            if self.action_mask is not None and self.action_mask.cons_table is not None:
+                self._refuse_constraints(n, pos, stop)
             S = int(status[5])
             self._flags.zero_()
             for _ in range(-(-S // self.B)):

@@ -609,6 +609,57 @@ int gib_action_mask_logits(int B, int N, int F, int Ef, int n_atom_types, int n_
                            const gib_scaffolds* sc, const int* slot_ids, const int* row, const int* state,
                            const int* counters, float* logits, int first_slot, gib_stream stream);
 
+/* ---- constraints: what a molecule may contain, as a mask (graphinvent_b200/csrc/constraints.cuh) ----
+ * The constraint table (device int32, written by gib_constraints_set; gib_constraints_ints words):
+ *   header [GIB_CONS_HDR_INTS]: min_atoms, max_atoms, min_rings, max_rings, min_ring_size, then the layout's A, CH, Ef
+ *   (written by the setter);
+ *   min_type [A], max_type [A], max_charge [CH], max_bond [Ef].
+ * Off values: 0 for a minimum and for min_ring_size, -1 for a maximum.  A table with every field off masks nothing.
+ * With n atoms in the state, count_t / count_c atoms of type t / charge index c, bonds_e upper-triangle entries of bond
+ * type e and rank = sum_e bonds_e - n + 1 (0 for n = 0), the rule forbids
+ *   an add when n >= max_atoms, count_t >= max_type[t], count_c >= max_charge[c], or (n > 0) bonds_e >= max_bond[e];
+ *   a connect when bonds_e >= max_bond[e], rank >= max_rings, or when the smallest ring it closes (the shortest-path
+ *   distance from n - 1 to bond_to, plus one) is shorter than min_ring_size;
+ *   terminate while n < min_atoms, count_t < min_type[t] or rank < min_rings, unless no other action survives every
+ *   rule of the launch (structure, valence, attachment points, the maxima): then terminate stays allowed (a dead end).
+ * A captured launch reads the table on every replay, so rewriting it needs no recapture. */
+enum {
+  GIB_CONS_MIN_ATOMS = 0, GIB_CONS_MAX_ATOMS = 1, GIB_CONS_MIN_RINGS = 2, GIB_CONS_MAX_RINGS = 3,
+  GIB_CONS_MIN_RING_SIZE = 4, GIB_CONS_N_ATOM_TYPES = 5, GIB_CONS_N_CHARGES = 6, GIB_CONS_N_BOND_TYPES = 7,
+  GIB_CONS_HDR_INTS = 8
+};
+/* words of a table for the layout (0 for counts outside 1..255) */
+size_t gib_constraints_ints(int n_atom_types, int n_charges, int Ef);
+/* validates the host table `values` (the layout above; header words 5..7 are filled from the arguments) and copies it
+ * into the device `table` in stream order.  Refuses, before any CUDA call: null pointers, N outside 1..127, a negative
+ * minimum or min_ring_size, a maximum below -1, min_ring_size 1 or 2, max_atoms or min_atoms over N, a minimum over
+ * its maximum, and per-type minima adding up to more than max_atoms (N when off). */
+int gib_constraints_set(int* table, const int* values, int N, int n_atom_types, int n_charges, int Ef,
+                        gib_stream stream);
+/* gib_action_mask_logits with the constraint rule in the same launch (the dead-end rule needs the other rules' verdicts
+ * on the whole row).  constraints = null: gib_action_mask_logits itself. */
+int gib_action_mask_logits_constrained(int B, int N, int F, int Ef, int n_atom_types, int n_charges, int n_imp_H,
+                                       int n_chirality, int apd, int mode, const int* table, const float* nodes,
+                                       const float* edges, const signed char* nodes_i8, const signed char* edges_i8,
+                                       const int* n_nodes, const gib_scaffolds* sc, const int* slot_ids,
+                                       const int* row, const int* state, const int* counters, float* logits,
+                                       int first_slot, gib_stream stream, const int* constraints);
+/* flags [M] (int32) of M finished molecules (nodes / edges float or int8 as for gib_action_mask_logits, n_nodes [M] or
+ * null = the non-empty node rows; mode / table: the mask's; sc with protect and scaffold_ids [M]: the attachment points
+ * of each molecule's scaffold, -1 = none):
+ *   GIB_CONS_OVER_MAX    a maximum is exceeded;
+ *   GIB_CONS_SMALL_RING  the molecule has a ring shorter than min_ring_size (its girth);
+ *   GIB_CONS_UNDER_MIN   under a minimum while another action was allowed: its terminate had probability 0;
+ *   GIB_CONS_DEAD_END    under a minimum with no other action allowed (terminate stayed allowed).
+ * The maxima and the ring-size bound hold for every route that builds the molecule (constraints.cuh), so a molecule
+ * with neither of the first three bits is one the constrained generator can make. */
+enum { GIB_CONS_OVER_MAX = 1, GIB_CONS_SMALL_RING = 2, GIB_CONS_UNDER_MIN = 4, GIB_CONS_DEAD_END = 8 };
+int gib_constraints_check(int M, int N, int F, int Ef, int n_atom_types, int n_charges, int n_imp_H, int n_chirality,
+                          int mode, const int* table, const float* nodes, const float* edges,
+                          const signed char* nodes_i8, const signed char* edges_i8, const int* n_nodes,
+                          const gib_scaffolds* sc, const int* scaffold_ids, const int* constraints, int* flags,
+                          gib_stream stream);
+
 /* ---- the RL rollout (GraphGeneratorRL.py:109-172) as captured rounds, and its backward by recomputation
  *      (graphinvent_b200.graphed.GraphedGeneratorRL).  Tables indexed [round, slot] have 2N rows of B. ----
  * gib_rl_sample_round: gib_generation_sample_round with two models.  The draw comes from logits_a (row state[0] of
