@@ -59,6 +59,12 @@ class MolLayout(ctypes.Structure):
                                    "len_atom_types", "len_formal_charge", "len_imp_H", "len_chirality")]
 
 
+class MolSet(ctypes.Structure):
+    """mirror of `gib_molset` (include/gib200.h): the buffers of a molecule set"""
+    _fields_ = [(n, c_p) for n in ("nodes", "edges", "hash", "n_atoms", "n_bonds", "counts", "next", "index_keys",
+                                   "index_first", "size")] + [("capacity", c_i), ("slots", c_i)]
+
+
 class PPDims(ctypes.Structure):
     """mirror of `gib_pp_dims` (include/gib200.h): dims and action layout of the training-set construction"""
     _fields_ = [(n, c_i) for n in ("N", "F", "Ef", "n_atom_types", "n_formal_charge", "n_imp_H", "n_chirality",
@@ -78,6 +84,7 @@ class Scaffolds(ctypes.Structure):
 
 PP_STATUS_INTS = 8                                                  # GIB_PP_* (include/gib200.h)
 PP_BAD_NODES, PP_BAD_EDGES, PP_EMPTY, PP_DISCONNECTED, PP_BAD_RANKING, PP_MATCH_BUDGET = 1, 2, 4, 8, 16, 32
+PP_CAPACITY = 64
 ROUTE_BFS, ROUTE_DFS = 0, 1                                         # GIB_ROUTE_BFS / GIB_ROUTE_DFS (gib_reorder)
 ROUTE_NOT_PREFIX, ROUTE_MASKED, ROUTE_BAD_ID, ROUTE_ACTION = 1, 2, 4, 8               # GIB_ROUTE_* (status[1] of the conditional plan)
 CONS_HDR_INTS = 8                                                   # GIB_CONS_* (include/gib200.h)
@@ -193,6 +200,12 @@ _PROTOS = {
                            + [c_p] * 7),
     "gib_murcko_ws_bytes": (c_sz, [c_p, c_i, c_i]),
     "gib_murcko": (c_i, [c_p, c_p, c_p, c_i, c_i] + [c_p] * 4 + [c_ll] + [c_p] * 5),
+    "gib_molset_bytes": (c_sz, [c_p, c_i]),
+    "gib_molset_slots": (c_i, [c_i]),
+    "gib_molset_init": (c_i, [c_p, c_p]),
+    "gib_molset_ws_bytes": (c_sz, [c_p, c_i]),
+    "gib_molset_identify": (c_i, [c_p, c_p, c_p, c_p, c_p, c_i, c_i, c_ll] + [c_p] * 6),
+    "gib_molset_from_float": (c_i, [c_p, c_p, c_ll, c_p]),
     "gib_route_plan_ws_bytes": (c_sz, [c_p, c_i]),
     "gib_route_max_states": (c_ll, [c_p, c_i]),
     "gib_route_plan": (c_i, [c_p, c_p, c_p, c_i, c_i] + [c_p] * 4),

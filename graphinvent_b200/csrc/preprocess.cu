@@ -21,6 +21,8 @@
 #include <algorithm>
 #include <climits>
 
+#include <cub/device/device_radix_sort.cuh>
+
 #include "common.cuh"
 #include "action_mask.cuh"
 #include "scaffold_mask.cuh"
@@ -37,7 +39,7 @@ constexpr unsigned long long kEmpty = ~0ull;
 
 // status words (int32 [GIB_PP_STATUS_INTS], documented per entry point in gib200.h)
 constexpr int kStGroups = 0;       // gib_preprocess_chunk: groups written
-constexpr int kStOpen = 0;         // gib_murcko: items left open by the dedup round
+constexpr int kStSetSize = 0;      // gib_molset_identify: the set's entries before the call
 constexpr int kStNext = 1;         // gib_preprocess_chunk: the molecule after the last one visited
 constexpr int kStRouteFlags = 1;   // the conditional route plan: GIB_ROUTE_* flags
 constexpr int kStRows = 2;         // gib_preprocess_chunk: rows written
@@ -263,17 +265,12 @@ __device__ int conditional_length(const PP& p, const gib_scaffolds& sc, int sid,
   return e - warp_sum(nnz) / 2 + 1;
 }
 
-// ---- count: validation and route length (one warp per molecule) ------------------------------------------------
-// ids != null (the conditional route plan): the length is that of molecule m's conditional route.  bad_out != null:
-// each molecule's GIB_PP_* input flags (0: it passed), for a later kernel that must leave refused molecules alone
-__global__ void __launch_bounds__(32) pp_count_kernel(PP p, const signed char* __restrict__ nodes,
-                                                      const signed char* __restrict__ edges, int* len, int* n0,
-                                                      int* status, const int* __restrict__ ids, gib_scaffolds sc,
-                                                      int* bad_out = nullptr) {
-  const int m = blockIdx.x, lane = threadIdx.x;
+// ---- the input checks of one padded graph (one warp, every lane gets the results) -------------------------------
+// Returns its GIB_PP_BAD_NODES / GIB_PP_BAD_EDGES / GIB_PP_EMPTY flags; *n = its atom count (rows up to the last
+// non-zero one), *nnz = its non-zero edge bytes.
+__device__ int validate_graph(const PP& p, const signed char* X, const signed char* E, int* n_out, int* nnz_out) {
+  const int lane = threadIdx.x & 31;
   const int N = p.N, F = p.F, Ef = p.Ef;
-  const signed char* X = nodes + (size_t)m * N * F;
-  const signed char* E = edges + (size_t)m * N * N * Ef;
   int last = -1, bad = 0;
   for (int r = lane; r < N; r += 32) {
     const signed char* row = X + (size_t)r * F;
@@ -316,9 +313,27 @@ __global__ void __launch_bounds__(32) pp_count_kernel(PP p, const signed char* _
   nnz = warp_sum(nnz);
   bad = __reduce_or_sync(0xffffffffu, bad);
   if (n == 0) bad |= GIB_PP_EMPTY;
+  *n_out = n;
+  *nnz_out = nnz;
+  return bad;
+}
+
+// ---- count: validation and route length (one warp per molecule) ------------------------------------------------
+// ids != null (the conditional route plan): the length is that of molecule m's conditional route.  bad_out != null:
+// each molecule's GIB_PP_* input flags (0: it passed), for a later kernel that must leave refused molecules alone
+__global__ void __launch_bounds__(32) pp_count_kernel(PP p, const signed char* __restrict__ nodes,
+                                                      const signed char* __restrict__ edges, int* len, int* n0,
+                                                      int* status, const int* __restrict__ ids, gib_scaffolds sc,
+                                                      int* bad_out = nullptr) {
+  const int m = blockIdx.x;
+  const int N = p.N, F = p.F, Ef = p.Ef;
+  const signed char* X = nodes + (size_t)m * N * F;
+  const signed char* E = edges + (size_t)m * N * N * Ef;
+  int n, nnz;
+  const int bad = validate_graph(p, X, E, &n, &nnz);
   const int e = min(nnz / 2, p.s_max - 2);
   const int kept = ids && !bad ? conditional_length(p, sc, ids[m], X, E, e, m, status) : e + 2;
-  if (lane == 0) {
+  if (threadIdx.x == 0) {
     if (bad) flag_bad(status, bad, m);
     len[m] = bad ? 2 : kept;
     n0[m] = n;
@@ -1187,13 +1202,14 @@ __device__ bool load_ranking(int N, int n, int draw, unsigned long long seed, lo
   return !bad_rank;
 }
 
-// reorder_nodes (one warp): the atom at new position k is old atom ord[k] for k < nk; order row O = ord, -1 past nk,
-// node rows / edge rows and columns of the molecule (X, E) into OX / OE, zero past nk
+// reorder_nodes (one warp): the atom at new position k is old atom ord[k] for k < nk; order row O = ord, -1 past nk
+// (O may be null), node rows / edge rows and columns of the molecule (X, E) into OX / OE, zero past nk
 __device__ void write_reordered(const PP& p, const signed char* X, const signed char* E, const int* ord, int nk,
                                 int* O, signed char* OX, signed char* OE) {
   const int lane = threadIdx.x & 31;
   const int N = p.N, F = p.F, Ef = p.Ef;
-  for (int i = lane; i < N; i += 32) O[i] = i < nk ? ord[i] : -1;
+  if (O)
+    for (int i = lane; i < N; i += 32) O[i] = i < nk ? ord[i] : -1;
   for (int q = lane; q < N * F; q += 32) {
     const int k = q / F;
     OX[q] = k < nk ? X[(size_t)ord[k] * F + q % F] : 0;
@@ -1501,16 +1517,17 @@ __global__ void __launch_bounds__(32) scaffold_first_kernel(
                   out_edges + (size_t)m * N * N * Ef);
 }
 
-// ---- Murcko scaffolds (gib_murcko) ---------------------------------------------------------------------------------
-// The items of one call: the known table's entries 0..K-1, then the scaffolds of the chunk's molecules K..K+n-1.
-// rep[i]: the item whose class item i belongs to (the first item of that class), kItemNone (no scaffold, or refused)
-// or kItemOpen (not yet assigned).
+// ---- graph identity: the 1-WL hash and the one-pass deduplication of gib_murcko and the molecule set ---------------
+// The items of one call are graphs in canonical order (every prefix connected, so the embedding search stays on
+// connected partial maps).  rep[i]: the item whose class item i belongs to, kItemNone (no graph, skipped or refused)
+// or kItemOpen (to be searched); an item that starts with rep[i] = i (a known table entry) is fixed.
 constexpr int kItemNone = -1, kItemOpen = -2;
 
-struct MurckoItems {
+// item i < K is row i of the known table, item K + m row m of the call's canonical graphs
+struct GraphItems {
   const signed char* known_nodes;   // [K, N, F]
   const signed char* known_edges;   // [K, N, N, Ef]
-  const signed char* nodes;         // [n, N, F]: the chunk's scaffolds, canonical order
+  const signed char* nodes;         // [n, N, F]
   const signed char* edges;
   int K;
   __device__ const signed char* X(const PP& p, int i) const {
@@ -1521,6 +1538,169 @@ struct MurckoItems {
     return i < K ? known_edges + (size_t)i * eb : edges + (size_t)(i - K) * eb;
   }
 };
+
+// one warp: the graph's atom count k (rows up to the last non-zero one), bonds, and its colour-refinement (1-WL) hash
+//   c_0(a) = mix64(sum_f byte_hash(f, X[a][f])),
+//   c_r(a) = mix64(c_{r-1}(a) + sum over bonds (a, b) of type t of mix64(c_{r-1}(b) ^ (t + 1) << 56)), r = 1..k,
+//   hash   = mix64(sum_a mix64(c_k(a)) ^ (k << 32 | bonds))   (kEmpty -> kEmpty - 1),
+// the type being the bond's first non-zero edge byte.  Isomorphic graphs hash equal; equal hashes prove nothing.
+// adj [kMatchAdjWords] and col [2][kReorderMaxN] are the warp's shared scratch.  Every lane gets the results.
+__device__ unsigned long long wl_hash(const PP& p, const signed char* X, const signed char* E, unsigned* adj,
+                                      unsigned long long (*col)[kReorderMaxN], int* k_out, int* bonds_out) {
+  const int lane = threadIdx.x & 31;
+  const int N = p.N, F = p.F, Ef = p.Ef, W = (N + 31) / 32;
+  int last = -1;
+  for (int r = lane; r < N; r += 32) {
+    bool any = false;
+    for (int f = 0; f < F; ++f) any |= X[(size_t)r * F + f] != 0;
+    if (any) last = r;
+  }
+  const int k = warp_max(last) + 1;
+  const int bonds = warp_sum(load_adjacency(E, N, Ef, k, nullptr, adj)) / 2;
+  for (int a = lane; a < k; a += 32) {
+    unsigned long long h = 0;
+    for (int f = 0; f < F; ++f) h += byte_hash(f, X[(size_t)a * F + f]);
+    col[0][a] = mix64(h);
+  }
+  __syncwarp();
+  for (int r = 0; r < k; ++r) {
+    const unsigned long long* src = col[r & 1];
+    unsigned long long* dst = col[(r + 1) & 1];
+    for (int a = lane; a < k; a += 32) {
+      unsigned long long s = src[a];
+      for (int t = 0; t < Ef; ++t)
+        for (int w = 0; w < W; ++w)
+          for (unsigned bits = adj[((size_t)t * N + a) * W + w]; bits; bits &= bits - 1)
+            s += mix64(src[w * 32 + __ffs(bits) - 1] ^ ((unsigned long long)(t + 1) << 56));
+      dst[a] = mix64(s);
+    }
+    __syncwarp();
+  }
+  unsigned long long sum = 0;
+  for (int a = lane; a < k; a += 32) sum += mix64(col[k & 1][a]);
+  sum = warp_sum_u64(sum);
+  unsigned long long h = mix64(sum ^ ((unsigned long long)k << 32 | (unsigned)bonds));
+  if (h == kEmpty) h = kEmpty - 1;
+  *k_out = k;
+  *bonds_out = bonds;
+  return h;
+}
+
+// does graph (RX, RE) of k atoms embed in the graph (X, E) of k atoms whose molecule side match_load put in S?  Between
+// graphs of equal atom and bond counts an induced embedding is an isomorphism (the smallest one lands in S.phi).  1 yes,
+// 0 no, -1 the search would take more than `budget` nodes; two empty graphs are isomorphic.  Every lane gets the answer.
+__device__ int match_graph(const PP& p, MatchSmem& S, short* rdeg, const signed char* X, const signed char* E,
+                           const signed char* RX, const signed char* RE, int k, long long budget) {
+  if (k == 0) return 1;
+  prefix_degrees(RE, p.N, p.Ef, k, rdeg);
+  __syncwarp();
+  gib_scaffolds view{};
+  view.nodes = RX;
+  view.edges = RE;
+  return match_scaffold(p, S, X, E, k, view, rdeg, 0, k, budget);
+}
+
+// Grouping: the items' (hash, index) pairs are radix-sorted by hash (stable: each group in ascending index), and
+// first[i] / pos[i] are the sorted positions of item i's group start and of item i itself (one CTA).
+__global__ void __launch_bounds__(kGroupNT) group_kernel(int n, const unsigned long long* __restrict__ skey,
+                                                         const int* __restrict__ sval, int* first, int* pos) {
+  __shared__ int sm[32];
+  int carry = 0;
+  for (int base = 0; base < n; base += kGroupNT) {
+    const int q = base + threadIdx.x;
+    const bool head = q < n && (q == 0 || skey[q] != skey[q - 1]);
+    int total;
+    const int start = max(carry, cta_scan(head ? q : 0, true, sm, &total));
+    if (q < n) {
+      first[sval[q]] = start;
+      pos[sval[q]] = q;
+    }
+    carry = max(carry, total);
+  }
+}
+
+// workspace of the radix sort: CUB's temporary storage is sized at call time and checked against this bound
+size_t sort_tmp_bytes(long long items) { return align256((1u << 20) + 8ull * items); }
+
+// sorts the pairs (k0[i], v0[i]) by key, stably; *skey / *sval: the buffers holding the sorted pairs
+int sort_groups(const char* who, unsigned long long* k0, unsigned long long* k1, int* v0, int* v1, int items,
+                void* tmp, size_t tmp_bytes, cudaStream_t s, const unsigned long long** skey, const int** sval) {
+  cub::DoubleBuffer<unsigned long long> k(k0, k1);
+  cub::DoubleBuffer<int> v(v0, v1);
+  size_t need = 0;
+  GIB_CUDA_TRY(cub::DeviceRadixSort::SortPairs(nullptr, need, k, v, items, 0, 64, s));
+  if (need > tmp_bytes) {
+    set_error("%s: the radix sort of %d items needs %zu bytes of workspace, %zu reserved", who, items, need, tmp_bytes);
+    return -1;
+  }
+  GIB_CUDA_TRY(cub::DeviceRadixSort::SortPairs(tmp, need, k, v, items, 0, 64, s));
+  *skey = k.Current();
+  *sval = v.Current();
+  return 0;
+}
+
+// The one-pass deduplication, one warp per open item i: its representative is the smallest item j <= i of its hash
+// group in its class.  Isomorphism is an equivalence, so that j is the first item of the class and i finds it alone:
+// it tests the earlier items of its group in ascending order and stops at the first match (no rounds, no dependency
+// between items).  Candidates must have i's atom and bond counts; the test is match_graph (j embedded in i), whose
+// smallest isomorphism goes to phi (when given; the identity for a representative).  cls (may be null): an item of
+// cls >= 0 is already known to be class cls (a set entry) and matches exactly the earlier items of the same cls; the
+// others skip those.  A search beyond `budget` refuses the item (GIB_PP_MATCH_BUDGET, molecule i - K).
+__global__ void __launch_bounds__(32) dedup_kernel(PP p, GraphItems it, const int* __restrict__ sval,
+                                                   const int* __restrict__ first, const int* __restrict__ pos,
+                                                   const int* __restrict__ item_k, const int* __restrict__ item_bonds,
+                                                   const int* __restrict__ cls, long long budget, int* rep, short* phi,
+                                                   int* status) {
+  __shared__ MatchSmem S;
+  __shared__ short rdeg[kReorderMaxN];
+  const int i = blockIdx.x, lane = threadIdx.x;
+  if (rep[i] != kItemOpen) return;                          // from here on rep[i] is written by this warp alone
+  const int k = item_k[i], bonds = item_bonds[i], c = cls ? cls[i] : -1;
+  const signed char* X = it.X(p, i);
+  const signed char* E = it.E(p, i);
+  bool loaded = false;
+  int res = 0, r = i;
+  for (int q = first[i], end = pos[i]; q < end; ++q) {
+    const int j = sval[q], cj = cls ? cls[j] : -1;
+    if (c >= 0 || cj >= 0) {
+      if (cj != c) continue;
+      res = 1;
+      r = j;
+      break;
+    }
+    if (item_k[j] != k || item_bonds[j] != bonds) continue;
+    if (!loaded) {
+      match_load(p, S, E, k);
+      loaded = true;
+    }
+    res = match_graph(p, S, rdeg, X, E, it.X(p, j), it.E(p, j), k, budget);
+    if (res) {
+      r = j;
+      break;
+    }
+  }
+  if (res < 0) {
+    if (lane == 0) {
+      rep[i] = kItemNone;
+      flag_bad(status, GIB_PP_MATCH_BUDGET, i - it.K);
+    }
+    return;
+  }
+  if (phi) {
+    short* ph = phi + (size_t)(i - it.K) * p.N;
+    for (int a = lane; a < k; a += 32) ph[a] = r == i ? (short)a : S.phi[a];
+  }
+  if (lane == 0) rep[i] = r;
+}
+
+// is_new[m] = 1 when item K + m represents a class that is not a known entry
+__global__ void new_class_kernel(int n, int K, const int* __restrict__ rep, const int* __restrict__ cls, int* is_new) {
+  const int m = blockIdx.x * blockDim.x + threadIdx.x;
+  if (m < n) is_new[m] = rep[K + m] == K + m && !(cls && cls[K + m] >= 0);
+}
+
+// ---- Murcko scaffolds (gib_murcko) ---------------------------------------------------------------------------------
+// Items: the known table's entries 0..K-1 (fixed), then the scaffolds of the chunk's molecules K..K+n-1.
 
 // one warp per molecule: keep = the 2-core (atoms of degree <= 1 removed, all at once, until none is left) plus the
 // atoms outside it with a double bond (edge feature 1) to it; the scaffold is the molecule's induced subgraph on them,
@@ -1615,126 +1795,27 @@ __global__ void __launch_bounds__(32) murcko_kernel(PP p, const signed char* __r
                   sc_edges + (size_t)m * N * N * Ef);
 }
 
-// one warp per item: its atom count k (rows up to the last non-zero one), bonds, and a colour-refinement (1-WL) hash
-//   c_0(a) = mix64(sum_f byte_hash(f, X[a][f])),
-//   c_r(a) = mix64(c_{r-1}(a) + sum over bonds (a, b) of type t of mix64(c_{r-1}(b) ^ (t + 1) << 56)), r = 1..k,
-//   hash   = mix64(sum_a mix64(c_k(a)) ^ (k << 32 | bonds))   (kEmpty -> kEmpty - 1),
-// the type being the bond's first non-zero edge byte.  Isomorphic graphs hash equal; equal hashes prove nothing.
-// An item with k >= 1 is inserted into the hash table (slot) and left open.
-__global__ void __launch_bounds__(32) murcko_hash_kernel(PP p, MurckoItems it, int* item_k, int* item_bonds,
-                                                         unsigned long long* keys, long long mask, int* slot,
-                                                         int* rep) {
+// one warp per item: its atom count, bonds and sort key (wl_hash; kEmpty without a scaffold, sorted past every group)
+__global__ void __launch_bounds__(32) murcko_hash_kernel(PP p, GraphItems it, int* item_k, int* item_bonds,
+                                                         unsigned long long* key, int* val, int* rep) {
   __shared__ unsigned adj[kMatchAdjWords];
   __shared__ unsigned long long col[2][kReorderMaxN];
-  const int i = blockIdx.x, lane = threadIdx.x;
-  const int N = p.N, F = p.F, Ef = p.Ef, W = (N + 31) / 32;
-  const signed char* X = it.X(p, i);
-  const signed char* E = it.E(p, i);
-  int last = -1;
-  for (int r = lane; r < N; r += 32) {
-    bool any = false;
-    for (int f = 0; f < F; ++f) any |= X[(size_t)r * F + f] != 0;
-    if (any) last = r;
-  }
-  const int k = warp_max(last) + 1;
-  const int bonds = warp_sum(load_adjacency(E, N, Ef, k, nullptr, adj)) / 2;
-  for (int a = lane; a < k; a += 32) {
-    unsigned long long h = 0;
-    for (int f = 0; f < F; ++f) h += byte_hash(f, X[(size_t)a * F + f]);
-    col[0][a] = mix64(h);
-  }
-  __syncwarp();
-  for (int r = 0; r < k; ++r) {
-    const unsigned long long* src = col[r & 1];
-    unsigned long long* dst = col[(r + 1) & 1];
-    for (int a = lane; a < k; a += 32) {
-      unsigned long long s = src[a];
-      for (int t = 0; t < Ef; ++t)
-        for (int w = 0; w < W; ++w)
-          for (unsigned bits = adj[((size_t)t * N + a) * W + w]; bits; bits &= bits - 1)
-            s += mix64(src[w * 32 + __ffs(bits) - 1] ^ ((unsigned long long)(t + 1) << 56));
-      dst[a] = mix64(s);
-    }
-    __syncwarp();
-  }
-  unsigned long long sum = 0;
-  for (int a = lane; a < k; a += 32) sum += mix64(col[k & 1][a]);
-  sum = warp_sum_u64(sum);
-  unsigned long long h = mix64(sum ^ ((unsigned long long)k << 32 | (unsigned)bonds));
-  if (h == kEmpty) h = kEmpty - 1;
-  if (lane == 0) {
+  const int i = blockIdx.x;
+  int k, bonds;
+  const unsigned long long h = wl_hash(p, it.X(p, i), it.E(p, i), adj, col, &k, &bonds);
+  if (threadIdx.x == 0) {
     item_k[i] = k;
     item_bonds[i] = bonds;
-    slot[i] = k > 0 ? tbl_insert(keys, h, mask) : -1;
-    rep[i] = k > 0 ? kItemOpen : kItemNone;
+    key[i] = k > 0 ? h : kEmpty;
+    val[i] = i;
+    rep[i] = k == 0 ? kItemNone : i < it.K ? i : kItemOpen;
   }
-}
-
-// one dedup round, part 1: each hash bucket's smallest open item becomes its representative this round (atomicMax of
-// (round, ~item): buckets need no reset between rounds).  Clears the round's open counter.
-__global__ void murcko_select_kernel(int items, int round, const int* __restrict__ rep, const int* __restrict__ slot,
-                                     unsigned long long* bucket, int* status) {
-  const int t = blockIdx.x * blockDim.x + threadIdx.x;
-  if (t == 0) status[kStOpen] = 0;
-  for (int i = t; i < items; i += gridDim.x * blockDim.x)
-    if (rep[i] == kItemOpen)
-      atomicMax(&bucket[slot[i]], (unsigned long long)round << 32 | (0xffffffffu - (unsigned)i));
-}
-
-// part 2, one warp per open item: the representative joins its own class (phi = the identity); a chunk item of the same
-// atom and bond counts joins it when match_scaffold embeds the representative in it -- an induced embedding between
-// graphs of equal counts is an isomorphism -- with that smallest embedding as phi (representative atom -> item atom).
-// A known item never joins another (the known entries are distinct).  The others stay open and are counted.
-__global__ void __launch_bounds__(32) murcko_match_kernel(PP p, MurckoItems it, const int* __restrict__ item_k,
-                                                          const int* __restrict__ item_bonds,
-                                                          const int* __restrict__ slot,
-                                                          const unsigned long long* __restrict__ bucket,
-                                                          long long budget, int* rep, short* phi, int* status) {
-  __shared__ MatchSmem S;
-  __shared__ short rdeg[kReorderMaxN];
-  const int i = blockIdx.x, lane = threadIdx.x, N = p.N, Ef = p.Ef;
-  if (rep[i] != kItemOpen) return;
-  const int r = (int)(0xffffffffu - (unsigned)bucket[slot[i]]);
-  const int k = item_k[i];
-  short* ph = i >= it.K ? phi + (size_t)(i - it.K) * N : nullptr;
-  int res = 0;
-  if (r == i) {
-    res = 1;
-    if (ph)
-      for (int a = lane; a < k; a += 32) ph[a] = (short)a;
-  } else if (ph && item_k[r] == k && item_bonds[r] == item_bonds[i]) {
-    const signed char* RE = it.E(p, r);
-    match_load(p, S, it.E(p, i), k);
-    prefix_degrees(RE, N, Ef, k, rdeg);
-    __syncwarp();
-    gib_scaffolds view{};
-    view.nodes = it.X(p, r);
-    view.edges = RE;
-    res = match_scaffold(p, S, it.X(p, i), it.E(p, i), k, view, rdeg, 0, k, budget);
-    if (res > 0)
-      for (int a = lane; a < k; a += 32) ph[a] = S.phi[a];
-  }
-  if (lane == 0) {
-    if (res > 0) {
-      rep[i] = r;
-    } else if (res < 0) {
-      rep[i] = kItemNone;
-      flag_bad(status, GIB_PP_MATCH_BUDGET, i - it.K);
-    } else {
-      atomicAdd(&status[kStOpen], 1);
-    }
-  }
-}
-
-__global__ void murcko_new_kernel(int n, int K, const int* __restrict__ rep, int* is_new) {
-  const int m = blockIdx.x * blockDim.x + threadIdx.x;
-  if (m < n) is_new[m] = rep[K + m] == K + m;
 }
 
 // one warp per molecule: its entry id (a new entry's id is K + its rank among the chunk's new representatives, off),
 // the count, a new entry's bytes into the table, and the attachment points: entry atom i is one when the molecule atom
 // it maps to (through phi and the scaffold's order row) has a bond to an atom outside the scaffold
-__global__ void __launch_bounds__(32) murcko_emit_kernel(PP p, MurckoItems it, const signed char* __restrict__ edges,
+__global__ void __launch_bounds__(32) murcko_emit_kernel(PP p, GraphItems it, const signed char* __restrict__ edges,
                                                          const int* __restrict__ n0,
                                                          const unsigned char* __restrict__ keep,
                                                          const int* __restrict__ sorder, const int* __restrict__ rep,
@@ -1769,15 +1850,13 @@ __global__ void __launch_bounds__(32) murcko_emit_kernel(PP p, MurckoItems it, c
 }
 
 struct MurckoWs {
-  size_t len, n0, bad, off, sorder, phi, sc_nodes, sc_edges, item_k, item_bonds, slot, rep, keys, bucket, total;
-  long long table;
+  size_t len, n0, bad, off, sorder, phi, sc_nodes, sc_edges, item_k, item_bonds, rep, key0, key1, val0, val1, first,
+      pos, sort_tmp, total;
 };
 
 MurckoWs murcko_ws_layout(const PP& p, int n, int K) {
   MurckoWs w{};
   const long long items = (long long)n + K;
-  w.table = 1024;
-  while (w.table < 2 * items) w.table <<= 1;
   Carve c;
   w.len = c.take(4ull * n);
   w.n0 = c.take(4ull * n);
@@ -1789,10 +1868,14 @@ MurckoWs murcko_ws_layout(const PP& p, int n, int K) {
   w.sc_edges = c.take((size_t)n * p.N * p.N * p.Ef);
   w.item_k = c.take(4ull * items);
   w.item_bonds = c.take(4ull * items);
-  w.slot = c.take(4ull * items);
   w.rep = c.take(4ull * items);
-  w.keys = c.take(8ull * w.table);
-  w.bucket = c.take(8ull * w.table);
+  w.key0 = c.take(8ull * items);
+  w.key1 = c.take(8ull * items);
+  w.val0 = c.take(4ull * items);
+  w.val1 = c.take(4ull * items);
+  w.first = c.take(4ull * items);
+  w.pos = c.take(4ull * items);
+  w.sort_tmp = c.take(sort_tmp_bytes(items));
   w.total = c.end;
   return w;
 }
@@ -1816,6 +1899,279 @@ int murcko_limits(const char* who, const gib_pp_dims* d, int n_molecules, int n_
     return -1;
   }
   return 0;
+}
+
+// ---- the molecule set (gib_molset_*): a persistent table of distinct molecules -------------------------------------
+// Items of a call: its n molecules, in canonical order in the workspace.  cls[i]: the set entry molecule i is (-1: none).
+
+// one warp per molecule: skipped (valid[m] == 0) or refused -> kItemNone; else the input checks (gib_preprocess_chunk's,
+// an empty graph allowed), connectivity, the canonical order (breadth-first from atom 0, each layer in increasing
+// index) into (CX, CE), and the item's atom count, bonds and hash (copied to its sort key)
+__global__ void __launch_bounds__(32) molset_prepare_kernel(PP p, const signed char* __restrict__ nodes,
+                                                            const signed char* __restrict__ edges,
+                                                            const unsigned char* __restrict__ valid, signed char* CX,
+                                                            signed char* CE, int* item_k, int* item_bonds,
+                                                            unsigned long long* hash, unsigned long long* key,
+                                                            int* val, int* rep, int* status) {
+  __shared__ unsigned any[kReorderMaxN][kReorderWords];
+  __shared__ unsigned typed[kMatchAdjWords];
+  __shared__ unsigned long long col[2][kReorderMaxN];
+  __shared__ int rank[kReorderMaxN], ord[kReorderMaxN];
+  __shared__ unsigned vis[kReorderWords];
+  __shared__ int bad_s;
+  const int m = blockIdx.x, lane = threadIdx.x;
+  const int N = p.N, F = p.F, Ef = p.Ef, W = (N + 31) / 32;
+  const signed char* X = nodes + (size_t)m * N * F;
+  const signed char* E = edges + (size_t)m * N * N * Ef;
+  const bool use = !valid || valid[m];
+  int n = 0, nnz, bad = 0;
+  if (use) {
+    bad = validate_graph(p, X, E, &n, &nnz) & ~GIB_PP_EMPTY;
+    if (!bad && n > 0) {
+      load_adjacency(E, N, Ef, n, any, nullptr);
+      for (int i = lane; i < N; i += 32) rank[i] = N - i;   // layered_bfs takes the highest rank first
+      if (lane < W) vis[lane] = 0;
+      __syncwarp();
+      if (lane == 0) {
+        bad_s = 0;
+        if (reach(any, W, 0) != n) {
+          bad_s = GIB_PP_DISCONNECTED;
+        } else {
+          vis[0] = 1u;
+          ord[0] = 0;
+          layered_bfs(any, W, rank, vis, ord, 1);
+        }
+      }
+      __syncwarp();
+      bad = bad_s;
+    }
+  }
+  const bool ok = use && !bad;
+  write_reordered(p, X, E, ord, ok ? n : 0, nullptr, CX + (size_t)m * N * F, CE + (size_t)m * N * N * Ef);
+  int k = 0, bonds = 0;
+  const unsigned long long h = ok ? wl_hash(p, X, E, typed, col, &k, &bonds) : kEmpty;
+  if (lane == 0) {
+    if (bad) flag_bad(status, bad, m);
+    item_k[m] = k;
+    item_bonds[m] = bonds;
+    hash[m] = key[m] = h;
+    val[m] = m;
+    rep[m] = ok ? kItemOpen : kItemNone;
+  }
+}
+
+// the index slot of hash h (-1: not in the set)
+__device__ __forceinline__ long long molset_slot(const gib_molset& set, unsigned long long h) {
+  const long long mask = (long long)set.slots - 1;
+  for (long long s = (long long)(h & (unsigned long long)mask);; s = (s + 1) & mask) {
+    const unsigned long long k = set.index_keys[s];
+    if (k == h) return s;
+    if (k == kEmpty) return -1;
+  }
+}
+
+// one warp per open item: the set entry it is (cls[i], -1: none), found along its hash's chain; entries are distinct,
+// so at most one matches.  A search beyond `budget` refuses the molecule.
+__global__ void __launch_bounds__(32) molset_lookup_kernel(PP p, gib_molset set, GraphItems it,
+                                                           const int* __restrict__ item_k,
+                                                           const int* __restrict__ item_bonds,
+                                                           const unsigned long long* __restrict__ hash, int* rep,
+                                                           long long budget, int* cls, int* status) {
+  __shared__ MatchSmem S;
+  __shared__ short rdeg[kReorderMaxN];
+  const int i = blockIdx.x, lane = threadIdx.x, N = p.N, F = p.F, Ef = p.Ef;
+  int found = -1, res = 0;
+  if (rep[i] == kItemOpen) {
+    const long long s = molset_slot(set, hash[i]);
+    const int k = item_k[i], bonds = item_bonds[i];
+    bool loaded = false;
+    for (int e = s < 0 ? -1 : set.index_first[s]; e >= 0; e = set.next[e]) {
+      if (set.n_atoms[e] != k || set.n_bonds[e] != bonds) continue;
+      if (!loaded) {
+        match_load(p, S, it.E(p, i), k);
+        loaded = true;
+      }
+      res = match_graph(p, S, rdeg, it.X(p, i), it.E(p, i), set.nodes + (size_t)e * N * F,
+                        set.edges + (size_t)e * N * N * Ef, k, budget);
+      if (res) {
+        found = res > 0 ? e : -1;
+        break;
+      }
+    }
+  }
+  if (lane == 0) {
+    cls[i] = found;
+    if (res < 0) {
+      rep[i] = kItemNone;
+      flag_bad(status, GIB_PP_MATCH_BUDGET, i);
+    }
+  }
+}
+
+// one thread, after the scan: refuses an insert that does not fit (GIB_PP_CAPACITY), records the entry count before
+// the call in status and, when the call inserts, the count after it in the set
+__global__ void molset_commit_kernel(gib_molset set, int insert, int* status) {
+  const int S = *set.size;
+  status[kStSetSize] = S;
+  if (!insert || status[kStFlags]) return;
+  if ((long long)S + status[kStTotal] > set.capacity) {
+    atomicOr(&status[kStFlags], GIB_PP_CAPACITY);           // the molecule is named by molset_emit_kernel
+    return;
+  }
+  *set.size = S + status[kStTotal];
+}
+
+// one warp per molecule: ids and flags; when the call inserts, counts and the new entries (canonical bytes, hash, atom
+// and bond counts, the end of a chain).  A refused call writes none of the set: ids -1 and no flags, and under
+// GIB_PP_CAPACITY the first molecule of the first class that does not fit is named.
+__global__ void __launch_bounds__(32) molset_emit_kernel(PP p, gib_molset set, GraphItems it,
+                                                         const int* __restrict__ item_k,
+                                                         const int* __restrict__ item_bonds,
+                                                         const unsigned long long* __restrict__ hash,
+                                                         const int* __restrict__ rep, const int* __restrict__ cls,
+                                                         const int* __restrict__ off, int insert, int* ids,
+                                                         unsigned char* is_new, unsigned char* is_first, int* status) {
+  const int i = blockIdx.x, lane = threadIdx.x, N = p.N, F = p.F, Ef = p.Ef;
+  const int flags = status[kStFlags], S = status[kStSetSize], r = rep[i];
+  const bool found = r >= 0 && cls[i] >= 0;
+  const int id = r < 0 ? -1 : found ? cls[i] : S + off[r];
+  if (flags) {
+    if (lane == 0) {
+      ids[i] = -1;
+      is_new[i] = is_first[i] = 0;
+      if (flags == GIB_PP_CAPACITY && r == i && !found && id == set.capacity) atomicMin(&status[kStFirstBad], i);
+    }
+    return;
+  }
+  if (lane == 0) {
+    ids[i] = found || insert ? id : -1;
+    is_new[i] = r >= 0 && !found;
+    is_first[i] = r == i;
+    if (insert && id >= 0) atomicAdd((unsigned long long*)&set.counts[id], 1ull);
+  }
+  if (!insert || found || r != i) return;
+  const signed char* X = it.X(p, i);
+  const signed char* E = it.E(p, i);
+  for (int q = lane; q < N * F; q += 32) set.nodes[(size_t)id * N * F + q] = X[q];
+  for (int q = lane; q < N * N * Ef; q += 32) set.edges[(size_t)id * N * N * Ef + q] = E[q];
+  if (lane == 0) {
+    set.hash[id] = hash[i];
+    set.n_atoms[id] = item_k[i];
+    set.n_bonds[id] = item_bonds[i];
+    set.next[id] = -1;
+  }
+}
+
+// one CTA, after molset_emit_kernel of an inserting call: links the new entries into the index.  Within a hash group
+// (sorted positions, ascending item index) the new entries follow each other in id order; the first one of a hash
+// either takes an empty index slot or is appended to the end of the chain already there.
+__global__ void __launch_bounds__(kGroupNT) molset_link_kernel(gib_molset set, int n,
+                                                               const unsigned long long* __restrict__ skey,
+                                                               const int* __restrict__ sval,
+                                                               const int* __restrict__ first,
+                                                               const int* __restrict__ rep,
+                                                               const int* __restrict__ cls,
+                                                               const int* __restrict__ off,
+                                                               const int* __restrict__ status) {
+  __shared__ int sm[32], incl[kGroupNT];
+  if (status[kStFlags]) return;
+  const int S = status[kStSetSize];
+  const long long mask = (long long)set.slots - 1;
+  int carry = -1;
+  for (int base = 0; base < n; base += kGroupNT) {
+    const int q = base + threadIdx.x;
+    const int j = q < n ? sval[q] : -1;
+    const bool fresh = j >= 0 && rep[j] == j && cls[j] < 0;
+    int total;
+    const int inc = max(carry, cta_scan(fresh ? q : -1, true, sm, &total));
+    incl[threadIdx.x] = inc;
+    __syncthreads();
+    const int prev = threadIdx.x ? incl[threadIdx.x - 1] : carry;    // the last new entry before position q
+    if (fresh) {
+      const int id = S + off[j];
+      if (prev >= first[j]) {
+        set.next[S + off[sval[prev]]] = id;
+      } else {
+        const unsigned long long h = skey[q];
+        for (long long s = (long long)(h & (unsigned long long)mask);; s = (s + 1) & mask) {
+          const unsigned long long k = atomicCAS(&set.index_keys[s], kEmpty, h);
+          if (k == kEmpty) {
+            set.index_first[s] = id;
+            break;
+          }
+          if (k == h) {
+            int e = set.index_first[s];
+            while (set.next[e] >= 0) e = set.next[e];
+            set.next[e] = id;
+            break;
+          }
+        }
+      }
+    }
+    carry = max(carry, total);
+    __syncthreads();
+  }
+}
+
+struct MolsetWs {
+  size_t cx, ce, item_k, item_bonds, hash, rep, cls, is_new, off, key0, key1, val0, val1, first, pos, sort_tmp, total;
+};
+
+MolsetWs molset_ws_layout(const PP& p, int n) {
+  MolsetWs w{};
+  Carve c;
+  w.cx = c.take((size_t)n * p.N * p.F);
+  w.ce = c.take((size_t)n * p.N * p.N * p.Ef);
+  w.item_k = c.take(4ull * n);
+  w.item_bonds = c.take(4ull * n);
+  w.hash = c.take(8ull * n);
+  w.rep = c.take(4ull * n);
+  w.cls = c.take(4ull * n);
+  w.is_new = c.take(4ull * n);
+  w.off = c.take(4ull * (n + 1));
+  w.key0 = c.take(8ull * n);
+  w.key1 = c.take(8ull * n);
+  w.val0 = c.take(4ull * n);
+  w.val1 = c.take(4ull * n);
+  w.first = c.take(4ull * n);
+  w.pos = c.take(4ull * n);
+  w.sort_tmp = c.take(sort_tmp_bytes(n));
+  w.total = c.end;
+  return w;
+}
+
+// the index slots of a set of `capacity` entries: the smallest power of two >= 2 * capacity (0: capacity out of range)
+long long molset_slots(int capacity) {
+  if (capacity < 1 || capacity > (1 << 29)) return 0;
+  long long s = 1;
+  while (s < 2ll * capacity) s <<= 1;
+  return s;
+}
+
+int molset_limits(const char* who, const gib_pp_dims* d, PP* p) {
+  GIB_TRY(make_pp(who, d, p));
+  return match_limits(who, *p);
+}
+
+int check_molset(const char* who, const gib_molset* set) {
+  if (!set || !set->nodes || !set->edges || !set->hash || !set->n_atoms || !set->n_bonds || !set->counts ||
+      !set->next || !set->index_keys || !set->index_first || !set->size) {
+    set_error("%s: null set or set buffer", who);
+    return -1;
+  }
+  if (set->slots != molset_slots(set->capacity)) {
+    set_error("%s: a set of capacity %d needs %lld index slots, got %d", who, set->capacity,
+              molset_slots(set->capacity), set->slots);
+    return -1;
+  }
+  return 0;
+}
+
+__global__ void molset_from_float_kernel(const float* __restrict__ x, signed char* out, long long count) {
+  for (long long q = blockIdx.x * (long long)blockDim.x + threadIdx.x; q < count; q += (long long)gridDim.x * blockDim.x) {
+    const float v = x[q];
+    out[q] = v == 0.f ? 0 : v == 1.f ? 1 : 2;
+  }
 }
 
 // gib_reorder's workspace: the count stage's len and n0 [n]
@@ -2153,38 +2509,30 @@ int gib_murcko(const gib_pp_dims* d, const signed char* nodes, const signed char
   short* phi = (short*)(b + w.phi);
   int* item_k = (int*)(b + w.item_k);
   int* item_bonds = (int*)(b + w.item_bonds);
-  int* slot = (int*)(b + w.slot);
   int* rep = (int*)(b + w.rep);
-  unsigned long long* keys = (unsigned long long*)(b + w.keys);
-  unsigned long long* bucket = (unsigned long long*)(b + w.bucket);
-  const MurckoItems it{table_nodes, table_edges, (const signed char*)(b + w.sc_nodes),
-                       (const signed char*)(b + w.sc_edges), n_known};
+  int* first = (int*)(b + w.first);
+  int* pos = (int*)(b + w.pos);
+  const GraphItems it{table_nodes, table_edges, (const signed char*)(b + w.sc_nodes),
+                      (const signed char*)(b + w.sc_edges), n_known};
   const int n = n_molecules, items = n + n_known;
   cudaStream_t s = (cudaStream_t)stream;
-  GIB_CUDA_TRY(cudaMemsetAsync(keys, 0xff, 8ull * w.table, s));      // kEmpty
-  GIB_CUDA_TRY(cudaMemsetAsync(bucket, 0, 8ull * w.table, s));
   GIB_TRY(launch_count(p, nodes, edges, n, len, n0, bad, status, s));
   murcko_kernel<<<n, 32, 0, s>>>(p, nodes, edges, n0, bad, keep, sorder, (signed char*)(b + w.sc_nodes),
                                  (signed char*)(b + w.sc_edges), status);
   GIB_LAUNCH_CHECK();
-  murcko_hash_kernel<<<items, 32, 0, s>>>(p, it, item_k, item_bonds, keys, w.table - 1, slot, rep);
+  murcko_hash_kernel<<<items, 32, 0, s>>>(p, it, item_k, item_bonds, (unsigned long long*)(b + w.key0),
+                                          (int*)(b + w.val0), rep);
   GIB_LAUNCH_CHECK();
-  // every round closes at least one item per bucket with an open item (its representative): at most `items` rounds
-  for (int round = 1;; ++round) {
-    if (round > items) {
-      set_error("gib_murcko: the deduplication did not finish in %d rounds", items);
-      return -1;
-    }
-    murcko_select_kernel<<<std::min(ceil_div(items, 256), 1024), 256, 0, s>>>(items, round, rep, slot, bucket, status);
-    GIB_LAUNCH_CHECK();
-    murcko_match_kernel<<<items, 32, 0, s>>>(p, it, item_k, item_bonds, slot, bucket, budget, rep, phi, status);
-    GIB_LAUNCH_CHECK();
-    int open = 0;
-    GIB_CUDA_TRY(cudaMemcpyAsync(&open, status + kStOpen, sizeof(int), cudaMemcpyDeviceToHost, s));
-    GIB_CUDA_TRY(cudaStreamSynchronize(s));
-    if (!open) break;
-  }
-  murcko_new_kernel<<<ceil_div(n, 256), 256, 0, s>>>(n, n_known, rep, len);
+  const unsigned long long* skey;
+  const int* sval;
+  GIB_TRY(sort_groups("gib_murcko", (unsigned long long*)(b + w.key0), (unsigned long long*)(b + w.key1),
+                      (int*)(b + w.val0), (int*)(b + w.val1), items, b + w.sort_tmp, sort_tmp_bytes(items), s,
+                      &skey, &sval));
+  group_kernel<<<1, kGroupNT, 0, s>>>(items, skey, sval, first, pos);
+  GIB_LAUNCH_CHECK();
+  dedup_kernel<<<items, 32, 0, s>>>(p, it, sval, first, pos, item_k, item_bonds, nullptr, budget, rep, phi, status);
+  GIB_LAUNCH_CHECK();
+  new_class_kernel<<<ceil_div(n, 256), 256, 0, s>>>(n, n_known, rep, nullptr, len);
   GIB_LAUNCH_CHECK();
   pp_scan_kernel<<<1, 1024, 0, s>>>(n, len, off, status);
   GIB_LAUNCH_CHECK();
@@ -2194,4 +2542,122 @@ int gib_murcko(const gib_pp_dims* d, const signed char* nodes, const signed char
   return 0;
 }
 
+size_t gib_molset_bytes(const gib_pp_dims* d, int capacity) {
+  PP p;
+  if (molset_limits("gib_molset_bytes", d, &p)) return 0;
+  const long long slots = molset_slots(capacity);
+  if (!slots) {
+    set_error("gib_molset_bytes: capacity %d outside [1, 2^29]", capacity);
+    return 0;
+  }
+  // per entry: node and edge bytes, hash, atom and bond counts, count, next; per slot: key and first entry; the size
+  const size_t entry = (size_t)p.N * p.F + (size_t)p.N * p.N * p.Ef + 8 + 4 + 4 + 8 + 4;
+  return entry * capacity + 12ull * slots + 4;
+}
+
+int gib_molset_slots(int capacity) {
+  const long long slots = molset_slots(capacity);
+  if (!slots) {
+    set_error("gib_molset_slots: capacity %d outside [1, 2^29]", capacity);
+    return -1;
+  }
+  return (int)slots;
+}
+
+int gib_molset_init(const gib_molset* set, gib_stream stream) {
+  GIB_TRY(check_molset("gib_molset_init", set));
+  cudaStream_t s = (cudaStream_t)stream;
+  GIB_CUDA_TRY(cudaMemsetAsync(set->index_keys, 0xff, 8ull * set->slots, s));      // kEmpty
+  GIB_CUDA_TRY(cudaMemsetAsync(set->counts, 0, 8ull * set->capacity, s));
+  GIB_CUDA_TRY(cudaMemsetAsync(set->size, 0, sizeof(int), s));
+  return 0;
+}
+
+size_t gib_molset_ws_bytes(const gib_pp_dims* d, int n_molecules) {
+  PP p;
+  if (molset_limits("gib_molset_ws_bytes", d, &p)) return 0;
+  if (n_molecules < 1 || n_molecules > INT_MAX / 4) {
+    set_error("gib_molset_ws_bytes: n_molecules %d outside [1, %d]", n_molecules, INT_MAX / 4);
+    return 0;
+  }
+  return molset_ws_layout(p, n_molecules).total;
+}
+
+int gib_molset_identify(const gib_pp_dims* d, const gib_molset* set, const signed char* nodes,
+                        const signed char* edges, const unsigned char* valid, int n_molecules, int insert,
+                        long long budget, int* ids, unsigned char* is_new, unsigned char* is_first, void* ws,
+                        int* status, gib_stream stream) {
+  PP p;
+  GIB_TRY(molset_limits("gib_molset_identify", d, &p));
+  GIB_TRY(check_molset("gib_molset_identify", set));
+  if (n_molecules < 1 || n_molecules > INT_MAX / 4 || budget < 1 || (insert != 0 && insert != 1)) {
+    set_error("gib_molset_identify: need 1 <= n_molecules <= %d, budget >= 1 and insert 0 or 1 (got %d, %lld, %d)",
+              INT_MAX / 4, n_molecules, budget, insert);
+    return -1;
+  }
+  if (!nodes || !edges || !ids || !is_new || !is_first || !ws || !status) {
+    set_error("gib_molset_identify: null argument");
+    return -1;
+  }
+  const int n = n_molecules;
+  const MolsetWs w = molset_ws_layout(p, n);
+  char* b = static_cast<char*>(ws);
+  signed char* cx = (signed char*)(b + w.cx);
+  signed char* ce = (signed char*)(b + w.ce);
+  int* item_k = (int*)(b + w.item_k);
+  int* item_bonds = (int*)(b + w.item_bonds);
+  int* rep = (int*)(b + w.rep);
+  int* cls = (int*)(b + w.cls);
+  int* fresh = (int*)(b + w.is_new);
+  int* off = (int*)(b + w.off);
+  int* first = (int*)(b + w.first);
+  int* pos = (int*)(b + w.pos);
+  unsigned long long* hash = (unsigned long long*)(b + w.hash);
+  unsigned long long* key = (unsigned long long*)(b + w.key0);
+  const GraphItems it{nullptr, nullptr, cx, ce, 0};
+  cudaStream_t s = (cudaStream_t)stream;
+  pp_init_kernel<<<1, 32, 0, s>>>(status, nullptr, nullptr, 0, 0);
+  GIB_LAUNCH_CHECK();
+  molset_prepare_kernel<<<n, 32, 0, s>>>(p, nodes, edges, valid, cx, ce, item_k, item_bonds, hash, key,
+                                         (int*)(b + w.val0), rep, status);
+  GIB_LAUNCH_CHECK();
+  molset_lookup_kernel<<<n, 32, 0, s>>>(p, *set, it, item_k, item_bonds, hash, rep, budget, cls, status);
+  GIB_LAUNCH_CHECK();
+  const unsigned long long* skey;
+  const int* sval;
+  GIB_TRY(sort_groups("gib_molset_identify", key, (unsigned long long*)(b + w.key1), (int*)(b + w.val0),
+                      (int*)(b + w.val1), n, b + w.sort_tmp, sort_tmp_bytes(n), s, &skey, &sval));
+  group_kernel<<<1, kGroupNT, 0, s>>>(n, skey, sval, first, pos);
+  GIB_LAUNCH_CHECK();
+  dedup_kernel<<<n, 32, 0, s>>>(p, it, sval, first, pos, item_k, item_bonds, cls, budget, rep, nullptr, status);
+  GIB_LAUNCH_CHECK();
+  new_class_kernel<<<ceil_div(n, 256), 256, 0, s>>>(n, 0, rep, cls, fresh);
+  GIB_LAUNCH_CHECK();
+  pp_scan_kernel<<<1, 1024, 0, s>>>(n, fresh, off, status);
+  GIB_LAUNCH_CHECK();
+  molset_commit_kernel<<<1, 1, 0, s>>>(*set, insert, status);
+  GIB_LAUNCH_CHECK();
+  molset_emit_kernel<<<n, 32, 0, s>>>(p, *set, it, item_k, item_bonds, hash, rep, cls, off, insert, ids, is_new,
+                                      is_first, status);
+  GIB_LAUNCH_CHECK();
+  if (insert) {
+    molset_link_kernel<<<1, kGroupNT, 0, s>>>(*set, n, skey, sval, first, rep, cls, off, status);
+    GIB_LAUNCH_CHECK();
+  }
+  return 0;
+}
+
+int gib_molset_from_float(const float* x, signed char* out, long long count, gib_stream stream) {
+  if (count < 0 || (count && (!x || !out))) {
+    set_error("gib_molset_from_float: need count >= 0 and both buffers, got count = %lld", count);
+    return -1;
+  }
+  if (!count) return 0;
+  const int blocks = (int)std::min<long long>(ceil_div_ll(count, 256), 4096);
+  molset_from_float_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(x, out, count);
+  GIB_LAUNCH_CHECK();
+  return 0;
+}
+
 }  // extern "C"
+

@@ -17,16 +17,28 @@ two copies (its header, then the used records) and keeps the statistics on the d
 
 `rdkit` and `MolecularGraph` are the modules of the caller's environment (the reference's Workflow imports them by
 these names); this package does not depend on them.
+
+`MoleculeSet` is a persistent device set of distinct molecules (`gib_molset_identify`, csrc/preprocess.cu) for
+uniqueness across a whole sample and novelty against a training set; `uniqueness` is the reference's per-batch
+uniqueness tensor from one call on a transient set.
 """
 import ctypes
+from collections import namedtuple
 
 import numpy as np
 import torch
 
 from ._lib import (MOL_ATOM_WORDS, MOL_DECODES, MOL_ERR_INDEX, MOL_ERR_OVERFLOW, MOL_ERR_VALUE, MOL_HDR_WORDS,
-                   MOL_WORDS, MolLayout, check, lib)
+                   MOL_WORDS, PP_BAD_EDGES, PP_BAD_NODES, PP_CAPACITY, PP_DISCONNECTED, PP_MATCH_BUDGET, PP_STATUS_INTS,
+                   MolLayout, MolSet, check, lib)
 
 N_EDGES_TO_BIN = 10      # Analyzer.py:557-560
+
+_SET_REASONS = ((PP_BAD_NODES, "a node row that is not one-hot per segment with 0/1 entries, or a zero row between "
+                 "atoms"),
+                (PP_BAD_EDGES, "edges that are not symmetric 0/1 single-type bonds between its atoms"),
+                (PP_DISCONNECTED, "a disconnected graph"),
+                (PP_MATCH_BUDGET, "the isomorphism search ran out of its budget of search-tree nodes (raise `budget`)"))
 
 
 def _ptr(t):
@@ -284,3 +296,150 @@ def _fraction_valid(graphs, termination):
         fraction_valid_pt = 0.0
     fraction_pt = torch.sum(termination) / len(termination)
     return fraction_valid, fraction_valid_pt, fraction_pt
+
+
+# ---- the molecule set ------------------------------------------------------------------------------------------------
+Identity = namedtuple("Identity", "ids new first")
+Identity.__doc__ = """What a `MoleculeSet` call says about each molecule of a batch, all device tensors [B]:
+ids int32: its entry (-1: not in the set after a `find`, or skipped by `valid`)
+new bool: its class was not in the set before the call;  first bool: the first molecule of its class in the call"""
+
+
+class MoleculeSet:
+    """A persistent set of distinct molecules on the device (`gib_molset_identify`, csrc/preprocess.cu): uniqueness
+    across batches, novelty against a training set, a run-long memory of what was generated.
+
+    Two molecules are the same when their graphs are isomorphic: every node row (atom type, charge and the implicit-H
+    and chirality bytes of the layout) and every edge cell equal under some renumbering of the atoms.  This is graph
+    identity, not RDKit's canonical-SMILES identity: two Kekule structures of one aromatic ring, or a group RDKit's
+    sanitisation rewrites, are two entries, so the number of distinct graphs bounds the number of distinct SMILES from
+    above (DESIGN.md).  All empty graphs are one entry.
+
+    max_n_nodes, n_node_features, n_edge_features: the graphs' N, F, Ef; capacity: entries the set can hold, fixed at
+    creation (its buffers take `nbytes`); layout: the node-feature segment widths (n_atom_types, n_formal_charge,
+    n_imp_H, n_chirality) as `preprocess.reorder` takes them; budget: search-tree nodes per isomorphism test.
+    Each entry holds its first molecule in canonical order (breadth-first from atom 0, each layer in increasing index)
+    and the number of molecules `add` gave it.
+
+    `add` and `find` take int8 stacks nodes [B, N, F] / edges [B, N, N, Ef] (numpy or torch, any atom order) or the
+    generators' float32 nodes / edges (0 / 1 entries, converted on the device), and valid (bool / uint8 [B], optional:
+    molecules with 0 are skipped).  A call's work does not depend on the set's size.  A refused call -- a bad node row,
+    a zero row between atoms, bad edges, a disconnected graph, a search beyond `budget`, or more new classes than the
+    set has room for -- raises ValueError naming the first such molecule and leaves the set exactly as it was."""
+
+    def __init__(self, max_n_nodes, n_node_features, n_edge_features, capacity, *, layout, budget=1 << 20,
+                 device="cuda"):
+        from . import preprocess as PP
+        N, F, Ef = int(max_n_nodes), int(n_node_features), int(n_edge_features)
+        self.d = PP._pp_dims(N, F, Ef, tuple(layout))
+        self.N, self.F, self.Ef = N, F, Ef
+        self.layout = tuple(layout)
+        if int(budget) < 1:
+            raise ValueError(f"budget must be >= 1, got {budget}")
+        self.budget = int(budget)
+        self.capacity = int(capacity)
+        self.nbytes = lib.gib_molset_bytes(ctypes.byref(self.d), self.capacity)
+        if self.nbytes == 0:
+            raise ValueError(lib.gib_last_error().decode())
+        slots = lib.gib_molset_slots(self.capacity)
+        dev = PP._cuda(torch.device(device))
+        C = self.capacity
+        self._nodes = torch.empty((C, N, F), dtype=torch.int8, device=dev)
+        self._edges = torch.empty((C, N, N, Ef), dtype=torch.int8, device=dev)
+        self._hash = torch.empty(C, dtype=torch.int64, device=dev)
+        self._n_atoms = torch.empty(C, dtype=torch.int32, device=dev)
+        self._n_bonds = torch.empty(C, dtype=torch.int32, device=dev)
+        self._counts = torch.empty(C, dtype=torch.int64, device=dev)
+        self._next = torch.empty(C, dtype=torch.int32, device=dev)
+        self._index_keys = torch.empty(slots, dtype=torch.int64, device=dev)
+        self._index_first = torch.empty(slots, dtype=torch.int32, device=dev)
+        self._size = torch.empty(1, dtype=torch.int32, device=dev)
+        self.device = self._nodes.device
+        self._status = torch.empty(PP_STATUS_INTS, dtype=torch.int32, device=self.device)
+        self._struct = MolSet(*(_ptr(t) for t in self.buffers()), C, slots)
+        check(lib.gib_molset_init(ctypes.byref(self._struct), self._stream()), "gib_molset_init")
+
+    def buffers(self):
+        """every device buffer of the set, in `gib_molset` order"""
+        return (self._nodes, self._edges, self._hash, self._n_atoms, self._n_bonds, self._counts, self._next,
+                self._index_keys, self._index_first, self._size)
+
+    def _stream(self):
+        return ctypes.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
+
+    def _int8(self, x, shape, what):
+        from . import preprocess as PP
+        t = torch.from_numpy(np.ascontiguousarray(x)) if isinstance(x, np.ndarray) else x
+        if not isinstance(t, torch.Tensor) or t.dtype not in (torch.int8, torch.float32) or tuple(t.shape[1:]) != shape:
+            raise ValueError(f"{what} must be int8 or float32 [B, {', '.join(map(str, shape))}], got "
+                             f"{getattr(t, 'dtype', type(t))} {tuple(getattr(t, 'shape', ()))}")
+        t = PP._on_device(t, self.device)
+        if t.dtype == torch.int8:
+            return t
+        out = torch.empty(t.shape, dtype=torch.int8, device=self.device)
+        check(lib.gib_molset_from_float(_ptr(t), _ptr(out), t.numel(), self._stream()), "gib_molset_from_float")
+        return out
+
+    def _call(self, nodes, edges, valid, insert):
+        from . import preprocess as PP
+        N, F, Ef = self.N, self.F, self.Ef
+        x = self._int8(nodes, (N, F), "nodes")
+        e = self._int8(edges, (N, N, Ef), "edges")
+        B = x.shape[0]
+        if e.shape[0] != B:
+            raise ValueError(f"{B} node graphs but {e.shape[0]} edge graphs")
+        v = None
+        if valid is not None:
+            v = torch.as_tensor(valid)
+            if tuple(v.shape) != (B,):
+                raise ValueError(f"valid must be [B] = [{B}], got {tuple(v.shape)}")
+            v = v.to(self.device).ne(0).to(torch.uint8).contiguous()
+        ids = torch.full((B,), -1, dtype=torch.int32, device=self.device)
+        new = torch.zeros(B, dtype=torch.uint8, device=self.device)
+        first = torch.zeros(B, dtype=torch.uint8, device=self.device)
+        if B:
+            ws = torch.empty(lib.gib_molset_ws_bytes(ctypes.byref(self.d), B), dtype=torch.uint8, device=self.device)
+            check(lib.gib_molset_identify(ctypes.byref(self.d), ctypes.byref(self._struct), _ptr(x), _ptr(e),
+                                          None if v is None else _ptr(v), B, int(insert), self.budget, _ptr(ids),
+                                          _ptr(new), _ptr(first), _ptr(ws), _ptr(self._status), self._stream()),
+                  "gib_molset_identify")
+            PP.refuse_bad(self._status.cpu().numpy(), 0, B, _SET_REASONS + (
+                (PP_CAPACITY, f"the set is full: its {self.capacity} entries cannot take this molecule's new class"),))
+        return Identity(ids, new.view(torch.bool), first.view(torch.bool))
+
+    def add(self, nodes, edges, valid=None):
+        """inserts the batch: new classes become entries in order of first occurrence, every molecule counts once for
+        its entry.  Returns an `Identity`."""
+        return self._call(nodes, edges, valid, True)
+
+    def find(self, nodes, edges, valid=None):
+        """looks the batch up without changing the set (ids -1 for molecules not in it).  Returns an `Identity`."""
+        return self._call(nodes, edges, valid, False)
+
+    def __len__(self):
+        return int(self._size.item())
+
+    @property
+    def counts(self):
+        """int64 [len(self)] device tensor: molecules added per entry"""
+        return self._counts[:len(self)]
+
+    def entries(self):
+        """(nodes int8 [S, N, F], edges int8 [S, N, N, Ef]): views of the entries, each its first molecule in
+        canonical order"""
+        S = len(self)
+        return self._nodes[:S], self._edges[:S]
+
+
+def uniqueness(nodes, edges, valid=None, *, layout):
+    """float32 [B] on the device: the reference's per-batch `uniqueness_tensor` (util.write_molecules, util.py:549-585)
+    with graph identity in place of SMILES equality: 1 for the first occurrence of a molecule or a molecule with
+    valid 0 (the reference's invalid molecules), 0 for a later duplicate of a valid one.  nodes / edges as
+    `MoleculeSet.add` takes them; one call on a transient set."""
+    t = nodes if isinstance(nodes, torch.Tensor) else torch.from_numpy(np.asarray(nodes))
+    B, N, F = t.shape
+    dev = t.device if t.is_cuda else torch.device("cuda")
+    s = MoleculeSet(N, F, edges.shape[-1], max(B, 1), layout=layout, device=dev)
+    ident = s.add(nodes, edges, valid)
+    keep = ident.first if valid is None else ident.first | ~torch.as_tensor(valid).to(dev).bool()
+    return keep.float()

@@ -799,7 +799,8 @@ int gib_graph_statistics(int B, int N, int F, int Ef, const float* nodes, const 
  * max_molecules * (N*(N-1)/2 + 2) < 2^30. */
 #define GIB_PP_STATUS_INTS 8
 enum { GIB_PP_BAD_NODES = 1, GIB_PP_BAD_EDGES = 2, GIB_PP_EMPTY = 4, GIB_PP_DISCONNECTED = 8,
-       GIB_PP_BAD_RANKING = 16 /* gib_reorder, gib_scaffold_first */, GIB_PP_MATCH_BUDGET = 32 /* gib_scaffold_first */ };
+       GIB_PP_BAD_RANKING = 16 /* gib_reorder, gib_scaffold_first */, GIB_PP_MATCH_BUDGET = 32 /* gib_scaffold_first */,
+       GIB_PP_CAPACITY = 64 /* gib_molset_identify */ };
 typedef struct gib_pp_dims {
   int N, F, Ef;                                             /* max_n_nodes, n_node_features, n_edge_features */
   int n_atom_types, n_formal_charge, n_imp_H, n_chirality;  /* node-feature segment widths, in order */
@@ -910,13 +911,70 @@ int gib_scaffold_first(const gib_pp_dims* d, const signed char* nodes, const sig
  * to the molecule's scaffold) has a bond leaving the scaffold (never cleared).  status int32 [GIB_PP_STATUS_INTS]:
  * [3] GIB_PP_* flags, [4] the first flagged molecule (INT_MAX: none), [5] new entries.  A flagged molecule's outputs
  * are unspecified.  Limits: N <= 181, Ef * N * ceil(N / 32) <= 2048.  ws: gib_murcko_ws_bytes(d, n_molecules,
- * n_known) bytes, may hold anything.  One warp per molecule and per table entry; the deduplication runs in rounds (each
- * hash group's first open scaffold is compared with the group's other open ones) and reads one status word back per
- * round: the call synchronises the stream and cannot be captured. */
+ * n_known) bytes, may hold anything.  One warp per molecule and per table entry.  The deduplication is one pass: the
+ * items (known entries, then the chunk's scaffolds) are radix-sorted by hash, and each scaffold tests the earlier items
+ * of its hash group in ascending order, stopping at the first isomorphic one, its entry (the engine of
+ * gib_molset_identify).  The call reads nothing back and does not synchronise the stream. */
 size_t gib_murcko_ws_bytes(const gib_pp_dims* d, int n_molecules, int n_known);
 int gib_murcko(const gib_pp_dims* d, const signed char* nodes, const signed char* edges, int n_molecules, int n_known,
                signed char* table_nodes, signed char* table_edges, long long* counts, unsigned char* attachment,
                long long budget, unsigned char* keep, int* ids, void* ws, int* status, gib_stream stream);
+
+/* ---- the molecule set (graphinvent_b200.molecules.MoleculeSet): a persistent device table of distinct molecules, for
+ *      uniqueness within and across batches and novelty against a training set.
+ * Identity: two molecules are the same when their graphs are isomorphic: every node row (all F bytes: atom type,
+ * charge, and the implicit-H and chirality bytes of the layout) and every edge cell (all Ef bytes) preserved.  This is
+ * graph identity, not canonical-SMILES identity (DESIGN.md).  A molecule with no atoms is a molecule: all empty graphs
+ * are one entry.
+ * Set (gib_molset, buffers sized for the call's dims and `capacity`, fixed at creation): entry e < *size holds its
+ * first molecule in canonical order (breadth-first from atom 0, each layer in increasing index) in nodes
+ * [capacity, N, F] / edges [capacity, N, N, Ef] int8, its 1-WL hash (gib_murcko's), atom and bond counts, its
+ * molecules counted by the calls that inserted (counts int64) and next, the next entry of the same hash (-1: none).  The
+ * open-addressing index, slots = gib_molset_slots(capacity) (the smallest power of two >= 2 * capacity), maps a hash
+ * (index_keys, ~0 = empty slot) to its first entry (index_first).  gib_molset_init empties a set: index keys ~0,
+ * counts 0, size 0 (the other buffers may hold anything).  gib_molset_bytes(d, capacity): the bytes of all its buffers.
+ * gib_molset_identify, one call for a batch of n molecules (input as gib_reorder's: int8, any atom order; d->batch_size
+ * unused): each molecule with valid[m] != 0 (valid uint8 [n] may be null: all) is checked as gib_preprocess_chunk
+ * checks its input (an empty graph allowed) and for connectivity, hashed, looked up along its hash's chain (entries are
+ * distinct, so at most one is isomorphic to it, confirmed by gib_scaffold_first's embedding search, never by the hash),
+ * and the molecules not found are deduplicated by gib_murcko's one-pass engine.  With insert = 1, new classes get ids
+ * *size, *size + 1, ... in order of first occurrence, their entries are written and indexed, and every molecule adds
+ * one to its entry's count.  insert = 0 (a lookup) writes nothing to the set.
+ * Output per molecule: ids int32 (the entry; -1 when it is not in the set and insert = 0, or skipped), is_new uint8 (its
+ * class was not in the set before the call), is_first uint8 (the first molecule of its class in this call); a skipped
+ * molecule gets -1, 0, 0.  status int32 [GIB_PP_STATUS_INTS]: [0] entries before the call, [3] GIB_PP_* flags, [4] the
+ * first flagged molecule (INT_MAX: none), [5] the classes not in the set.  Refusals: GIB_PP_BAD_NODES / BAD_EDGES
+ * (including a zero row between atoms), GIB_PP_DISCONNECTED, GIB_PP_MATCH_BUDGET (a search beyond `budget` nodes) and
+ * GIB_PP_CAPACITY (*size + new classes > capacity; [4] names the first molecule of the first class that does not fit).
+ * A refused call leaves every set buffer byte for byte as it was (its kernels read the status word on the device and
+ * write nothing) and returns ids -1 and no flags.
+ * Work per call is independent of the set's size (one index probe and a hash chain per molecule); the call reads
+ * nothing back.  Limits: N <= 181, Ef * N * ceil(N / 32) <= 2048.  ws: gib_molset_ws_bytes(d, n), may hold anything.
+ * gib_molset_from_float: float32 0 / 1 graphs (the generators' nodes / edges) to int8 on the device, any other value
+ * to 2, which the input checks refuse. */
+typedef struct gib_molset {
+  signed char* nodes;               /* [capacity, N, F] */
+  signed char* edges;               /* [capacity, N, N, Ef] */
+  unsigned long long* hash;         /* [capacity] */
+  int* n_atoms;                     /* [capacity] */
+  int* n_bonds;                     /* [capacity] */
+  long long* counts;                /* [capacity] */
+  int* next;                        /* [capacity] */
+  unsigned long long* index_keys;   /* [slots] */
+  int* index_first;                 /* [slots] */
+  int* size;                        /* [1]: entries */
+  int capacity;
+  int slots;
+} gib_molset;
+size_t gib_molset_bytes(const gib_pp_dims* d, int capacity);
+int gib_molset_slots(int capacity);
+int gib_molset_init(const gib_molset* set, gib_stream stream);
+size_t gib_molset_ws_bytes(const gib_pp_dims* d, int n_molecules);
+int gib_molset_identify(const gib_pp_dims* d, const gib_molset* set, const signed char* nodes,
+                        const signed char* edges, const unsigned char* valid, int n_molecules, int insert,
+                        long long budget, int* ids, unsigned char* is_new, unsigned char* is_first, void* ws,
+                        int* status, gib_stream stream);
+int gib_molset_from_float(const float* x, signed char* out, long long count, gib_stream stream);
 
 /* ---- the likelihood of a molecule's decoding route (graphinvent_b200.graphed.RouteScorer): for every route state,
  *      p(action | state) = softmax(model(state))[action], one chunk of molecules at a time.
