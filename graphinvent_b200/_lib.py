@@ -42,6 +42,11 @@ class DwProblem(ctypes.Structure):
                 ("cs", c_ll), ("m_dev", c_p), ("base_dev", c_p), ("tf32", c_i)]
 
 
+class DwExtent(ctypes.Structure):
+    """mirror of `gib_dw_extent` (include/gib200.h, test hooks): the pass extent of a DwProblem"""
+    _fields_ = [("passes", c_i), ("pass_g", c_ll), ("pass_x", c_ll)]
+
+
 class BatchCtl(ctypes.Structure):
     """mirror of `gib_batch_ctl` (include/gib200.h): the live molecule count and loss scale of a captured batch"""
     _fields_ = [("live", c_i), ("scale", c_f)]
@@ -227,6 +232,8 @@ _PROTOS = {
     "gib_test_gemm_nt": (c_i, [c_p, c_i, c_p, c_p, c_p]),
     "gib_test_dw_scratch_bytes": (c_sz, [c_p, c_p, c_i, c_ll]),
     "gib_test_dw_groups": (c_i, [c_p, c_p, c_i, c_ll, c_p, c_p]),
+    "gib_test_dw_scratch_bytes_passes": (c_sz, [c_p, c_p, c_p, c_i]),
+    "gib_test_dw_groups_passes": (c_i, [c_p, c_p, c_p, c_i, c_p, c_p]),
     "gib_test_dw_schedule": (c_i, [c_p, c_p, c_p, c_i, c_i, c_p, c_i, c_p, c_p]),
     "gib_test_dw_schedule_passes": (c_i, [c_p, c_p, c_p, c_p, c_i, c_i, c_p, c_i, c_p, c_p]),
     "gib_test_scatter_bwd": (c_i, [c_p, c_p, c_p, c_i, c_p, c_p, c_i, c_ll, c_p]),

@@ -514,6 +514,7 @@ int gib_linear_bwd_dw(const float* G, int ldg, int Nn, const float* X, int ldx, 
   q.R = R; q.C = C; q.Rb = R; q.Rbp = Nn; q.rs = C; q.cs = 1; q.scratch = reinterpret_cast<float*>(scratch);
   q.half_floats = gemm_dw_half_floats(M, Nn, Kk);
   q.m_dev = m_dev; q.base_dev = base_dev;
+  GIB_TRY(dw_check_operands(q, "gib_linear_bwd_dw"));
   GIB_TRY(dw_begin());
   const int rc = gemm_dw(q, ST(stream));
   const int rj = dw_join(ST(stream));
@@ -549,26 +550,77 @@ static GemmNT to_gemm_nt(const gib_gemm_problem& s) {
   if (s.tf32 >= 2) p.B_lo = nullptr;        // W_hi: the 16-bit plane; W_lo is not read
   return p;
 }
-static GemmDW to_gemm_dw(const gib_dw_problem& s) {
+// e == nullptr: one pass
+static GemmDW to_gemm_dw(const gib_dw_problem& s, const gib_dw_extent* e = nullptr) {
   GemmDW q;
   q.G = s.G; q.ldg = s.ldg; q.Nn = s.Nn; q.X = s.X; q.ldx = s.ldx; q.Kk = s.Kk; q.M = s.M; q.dW = s.dW;
   q.dbias = s.dbias; q.R = s.R; q.C = s.C; q.Rb = s.Rb; q.Rbp = s.Rbp; q.rs = s.rs; q.cs = s.cs;
   q.m_dev = s.m_dev; q.base_dev = s.base_dev; q.tf32 = s.tf32;
+  if (e) { q.passes = e->passes; q.pass_g = e->pass_g; q.pass_x = e->pass_x; }
   return q;
 }
-// both scratch halves, sized as make_bwd sizes them: the largest group and member
-static size_t test_dw_scratch_floats(const gib_dw_problem* qs, const int* group_sizes, int n_groups) {
+// both scratch halves, sized as make_bwd sizes them: the largest group and member (a pass extent counted as
+// tc3_dw_layout counts it); 0 for a group size outside 1..max_n
+static size_t test_dw_scratch_floats(const gib_dw_problem* qs, const gib_dw_extent* ext, const int* group_sizes,
+                                     int n_groups, int max_n) {
   size_t f = 0;
   int k = 0;
   for (int g = 0; g < n_groups; ++g) {
-    GemmDW grp[kTc3MaxProblems];
+    GemmDW grp[kDwMaxProblems];
     const int n = group_sizes[g];
-    if (n < 1 || n > kTc3MaxProblems) return 0;
-    for (int i = 0; i < n; ++i) grp[i] = to_gemm_dw(qs[k + i]);
+    if (n < 1 || n > max_n) return 0;
+    for (int i = 0; i < n; ++i) grp[i] = to_gemm_dw(qs[k + i], ext ? &ext[k + i] : nullptr);
     f = std::max(f, 2 * gemm_dw_group_half_floats(grp, n));
     k += n;
   }
   return f;
+}
+// the groups one after another on one scratch, as the model's backward runs them
+static int test_dw_run(const gib_dw_problem* qs, const gib_dw_extent* ext, const int* group_sizes, int n_groups,
+                       size_t floats, void* scratch, cudaStream_t st) {
+  GIB_TRY(dw_begin());
+  int rc = 0;
+  for (int g = 0, k = 0; g < n_groups && rc == 0; k += group_sizes[g++]) {
+    GemmDW grp[kDwMaxProblems];
+    for (int i = 0; i < group_sizes[g]; ++i) {
+      grp[i] = to_gemm_dw(qs[k + i], ext ? &ext[k + i] : nullptr);
+      grp[i].scratch = reinterpret_cast<float*>(scratch);
+      grp[i].half_floats = floats / 2;
+    }
+    rc = group_sizes[g] == 1 ? gemm_dw(grp[0], st) : gemm_dw_group(grp, group_sizes[g], st);
+  }
+  const int rj = dw_join(st);
+  return rc ? rc : rj;
+}
+// the refusals of gib_test_dw_groups_passes: host arithmetic only, before any CUDA call
+static int test_dw_check_passes(const gib_dw_problem* qs, const gib_dw_extent* ext, const int* group_sizes,
+                                int n_groups) {
+  const char* who = "gib_test_dw_groups_passes";
+  if (n_groups < 1 || !qs || !group_sizes) { set_error("%s: n_groups = %d (>= 1), qs and group_sizes", who, n_groups); return -2; }
+  int n = 0;
+  for (int g = 0; g < n_groups; ++g) {
+    if (group_sizes[g] < 1 || group_sizes[g] > kDwMaxProblems) {
+      set_error("%s: group_sizes[%d] = %d (1..%d)", who, g, group_sizes[g], kDwMaxProblems);
+      return -2;
+    }
+    n += group_sizes[g];
+  }
+  for (int k = 0; k < n; ++k) {
+    const GemmDW q = to_gemm_dw(qs[k], ext ? &ext[k] : nullptr);
+    if (q.passes < 1 || q.passes > kMaxPasses) {
+      set_error("%s: problem %d: passes = %d (1..%d)", who, k, q.passes, kMaxPasses);
+      return -2;
+    }
+    if (q.passes > 1 && (q.pass_g <= 0 || q.pass_x <= 0)) {
+      set_error("%s: problem %d: %s = %lld is not > 0", who, k, q.pass_g <= 0 ? "pass_g" : "pass_x",
+                q.pass_g <= 0 ? q.pass_g : q.pass_x);
+      return -2;
+    }
+    char where[64];
+    snprintf(where, sizeof(where), "%s: problem %d", who, k);
+    GIB_TRY(dw_check_operands(q, where));
+  }
+  return 0;
 }
 
 extern "C" {
@@ -595,26 +647,25 @@ int gib_test_gemm_nt(const gib_gemm_problem* ps, int n, const int* dep, int* fla
 }
 size_t gib_test_dw_scratch_bytes(const gib_dw_problem* qs, const int* group_sizes, int n_groups, long long plan_rows) {
   (void)plan_rows;
-  return test_dw_scratch_floats(qs, group_sizes, n_groups) * sizeof(float);
+  return test_dw_scratch_floats(qs, nullptr, group_sizes, n_groups, kTc3MaxProblems) * sizeof(float);
 }
 int gib_test_dw_groups(const gib_dw_problem* qs, const int* group_sizes, int n_groups, long long plan_rows,
                        void* scratch, gib_stream stream) {
   (void)plan_rows;
-  const size_t floats = test_dw_scratch_floats(qs, group_sizes, n_groups);
+  const size_t floats = test_dw_scratch_floats(qs, nullptr, group_sizes, n_groups, kTc3MaxProblems);
   if (n_groups < 1 || floats == 0) { set_error("gib_test_dw_groups: bad group sizes"); return -2; }
-  GIB_TRY(dw_begin());
-  int rc = 0;
-  for (int g = 0, k = 0; g < n_groups && rc == 0; k += group_sizes[g++]) {
-    GemmDW grp[kTc3MaxProblems];
-    for (int i = 0; i < group_sizes[g]; ++i) {
-      grp[i] = to_gemm_dw(qs[k + i]);
-      grp[i].scratch = reinterpret_cast<float*>(scratch);
-      grp[i].half_floats = floats / 2;
-    }
-    rc = group_sizes[g] == 1 ? gemm_dw(grp[0], ST(stream)) : gemm_dw_group(grp, group_sizes[g], ST(stream));
-  }
-  const int rj = dw_join(ST(stream));
-  return rc ? rc : rj;
+  return test_dw_run(qs, nullptr, group_sizes, n_groups, floats, scratch, ST(stream));
+}
+size_t gib_test_dw_scratch_bytes_passes(const gib_dw_problem* qs, const gib_dw_extent* ext, const int* group_sizes,
+                                        int n_groups) {
+  if (test_dw_check_passes(qs, ext, group_sizes, n_groups)) return 0;
+  return test_dw_scratch_floats(qs, ext, group_sizes, n_groups, kDwMaxProblems) * sizeof(float);
+}
+int gib_test_dw_groups_passes(const gib_dw_problem* qs, const gib_dw_extent* ext, const int* group_sizes,
+                              int n_groups, void* scratch, gib_stream stream) {
+  GIB_TRY(test_dw_check_passes(qs, ext, group_sizes, n_groups));
+  const size_t floats = test_dw_scratch_floats(qs, ext, group_sizes, n_groups, kDwMaxProblems);
+  return test_dw_run(qs, ext, group_sizes, n_groups, floats, scratch, ST(stream));
 }
 int gib_test_dw_schedule(const int* rows, const int* Nn, const int* Kk, int n, int sms, int* segs, int max_segs,
                          int* tile_ctas, int* G) {

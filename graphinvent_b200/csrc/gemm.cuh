@@ -116,6 +116,9 @@ extern int g_tc_debug;
 int check_precision(int prec, const char* who);
 
 int gemm_dw(const GemmDW& q, cudaStream_t st);
+// 0 when the fp32 SIMT kernel may read q's operands as float4 (16-byte aligned G / X bases and, with a pass extent,
+// pass strides that are multiples of 4), else -2 with the message set; host arithmetic only
+int dw_check_operands(const GemmDW& q, const char* who);
 // n <= kDwMaxProblems weight-gradient problems that may run as ONE grouped tensor-core launch + ONE reduction launch
 // (siblings of a layer: the per-bond-type message MLPs, the readout heads, the two GRU projections)
 int gemm_dw_group(const GemmDW* qs, int n, cudaStream_t st);

@@ -802,6 +802,17 @@ int gemm_dw_group(const GemmDW* qs, int n, cudaStream_t st) {
   return dw_tc_launch(live, nl, work, dyn_rows, ndyn, st);
 }
 
+int dw_check_operands(const GemmDW& q, const char* who) {
+  const char* bad = nullptr;
+  if (reinterpret_cast<uintptr_t>(q.G) & 15) bad = "G is not 16-byte aligned";
+  else if (reinterpret_cast<uintptr_t>(q.X) & 15) bad = "X is not 16-byte aligned";
+  else if (q.passes > 1 && (q.pass_g & 3)) bad = "pass_g is not a multiple of 4";
+  else if (q.passes > 1 && (q.pass_x & 3)) bad = "pass_x is not a multiple of 4";
+  if (!bad) return 0;
+  set_error("%s: %s", who, bad);
+  return -2;
+}
+
 int gemm_dw(const GemmDW& q, cudaStream_t st) {
   if (q.M <= 0) return 0;  // nothing to add
   GIB_TRY(check_precision(q.tf32, "gemm_dw"));
@@ -809,6 +820,7 @@ int gemm_dw(const GemmDW& q, cudaStream_t st) {
     set_error("gemm_dw: ldg=%d ldx=%d Nn=%d Kk=%d violate the padded-layout contract", q.ldg, q.ldx, q.Nn, q.Kk);
     return -2;
   }
+  GIB_TRY(dw_check_operands(q, "gemm_dw"));
   if (q.m_dev) return gemm_dw_group(&q, 1, st);
   // the tensor-core launch as a group of one (also under gib_tc_debug bit 0, which groups no weight gradients)
   const double work = q.work > 0 ? q.work : 2.0 * q.M * (double)q.R * q.C * q.passes;

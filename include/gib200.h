@@ -287,7 +287,8 @@ int gib_split_planes(const float* W, float* W_hi, float* W_lo, long long n, gib_
 /* the 16-bit plane of n fp32 values (kind 2 = bf16, 3 = fp16: the gib_dims.tf32 codes), rounded to nearest-even
  * as gib_model_pack rounds them, into n 16-bit values at out -- the W_hi of a 16-bit test-hook problem */
 int gib_round_plane16(const float* W, void* out, long long n, int kind, gib_stream stream);
-/* dW[R,C] += G^T X, dbias[R] += colsum(G); G [M, ldg], X [M, ldx]; scratch from gib_dw_scratch_bytes */
+/* dW[R,C] += G^T X, dbias[R] += colsum(G); G [M, ldg], X [M, ldx]; scratch from gib_dw_scratch_bytes; G and X must be
+ * 16-byte aligned (-2 before any CUDA call otherwise: the fp32 kernel reads them as float4) */
 size_t gib_dw_scratch_bytes(int M, int Nn, int Kk);
 int gib_linear_bwd_dw(const float* G, int ldg, int Nn, const float* X, int ldx, int Kk, int M, float* dW,
                       float* dbias, int R, int C, void* scratch, const int* m_dev, const int* base_dev,
@@ -357,6 +358,21 @@ typedef struct gib_dw_problem {
 size_t gib_test_dw_scratch_bytes(const gib_dw_problem* qs, const int* group_sizes, int n_groups, long long plan_rows);
 int gib_test_dw_groups(const gib_dw_problem* qs, const int* group_sizes, int n_groups, long long plan_rows,
                        void* scratch, gib_stream stream);
+/* The pass extent of one problem, as the backward gives the message-MLP and GRU weights it reduces over all message
+ * passes: the problem sums over the same rows of `passes` (1..16) slices, slice t of G at G + t * pass_g and of X at
+ * X + t * pass_x (strides in elements, > 0 and multiples of 4 when passes > 1). */
+typedef struct gib_dw_extent {
+  int passes;
+  long long pass_g, pass_x;
+} gib_dw_extent;
+/* gib_test_dw_scratch_bytes / gib_test_dw_groups with a pass extent ext[k] for problem k (ext == NULL: one pass each)
+ * and groups of up to 32 problems (the model's deferred launch of every message-MLP layer and the GRU pair).  Each
+ * group runs as there.  Returns -2 (0 bytes) before any CUDA call for a group size outside 1..32, passes outside
+ * 1..16, a pass stride that is <= 0 or not a multiple of 4, or a G / X base that is not 16-byte aligned. */
+size_t gib_test_dw_scratch_bytes_passes(const gib_dw_problem* qs, const gib_dw_extent* ext, const int* group_sizes,
+                                        int n_groups);
+int gib_test_dw_groups_passes(const gib_dw_problem* qs, const gib_dw_extent* ext, const int* group_sizes,
+                              int n_groups, void* scratch, gib_stream stream);
 /* The schedule of one grouped tensor-core weight-gradient launch of n (<= 32) members with host row counts rows[p] and
  * padded shapes Nn[p] x Kk[p] on sms SMs (host arithmetic, no device): writes G (the CTAs with work), per segment 6
  * ints (CTA, member, tile of the member, first reduction row, rows, scratch slot) into segs, and per tile of the group
