@@ -29,6 +29,7 @@
 // GraphGenerator.build_graphs in device memory (so a captured round can be replayed without reading anything back):
 // the sampler decides once per call whether the round runs and leaves the round index (or -1: inert) in `ctl`, which
 // the decode, scan and apply kernels read instead of their `round` argument.  The plain entry points pass ctl = null.
+#include <type_traits>
 #include "../../include/gib200.h"
 #include "common.cuh"
 #include "ops.cuh"
@@ -257,6 +258,13 @@ __global__ void __launch_bounds__(128) gen_scaffold_init_kernel(int N, int F, in
   }
 }
 
+// the round gate of a captured round's mask (state != null): the mask runs only when the sampler after it will run
+// the round -- fewer than B molecules finished, status 0, a round index in [0, 2N)
+__device__ __forceinline__ bool round_gated_off(const int* __restrict__ state, const int* __restrict__ counters, int B,
+                                                int N) {
+  return state && !(counters[0] < B && state[1] == 0 && state[0] >= 0 && state[0] < 2 * N);
+}
+
 // the attachment-point mask (scaffold_mask.cuh): one CTA per slot, -inf into the add blocks and connect entries whose
 // bond_to is a protected atom, and into every connect while bond_from = n - 1 is still a scaffold atom (n_nodes only
 // grows from k_s, so that is n == k_s).  Terminate is never touched, so a masked row keeps an action of non-zero
@@ -269,7 +277,7 @@ __global__ void __launch_bounds__(128) gen_mask_kernel(int N, int Ef, int apd, g
                                                        const int* __restrict__ counters, float* __restrict__ logits,
                                                        int first_slot) {
   const int b = blockIdx.x, B = gridDim.x;
-  if (state && !(counters[0] < B && state[1] == 0 && state[0] >= 0 && state[0] < 2 * N)) return;
+  if (round_gated_off(state, counters, B, N)) return;
   const size_t off = row ? (size_t)row[0] * B : 0;
   const int s = slot_ids[off + b];
   if (b < first_slot || s < 0 || s >= sc.S) return;
@@ -288,80 +296,22 @@ __global__ void __launch_bounds__(128) gen_mask_kernel(int N, int Ef, int apd, g
     for (int t = threadIdx.x; t < N * Ef; t += 128) o[len_add + t] = -INFINITY;
 }
 
-// the action mask (action_mask.cuh): one CTA per slot, -inf into every entry of the slot's logits row that the rule
-// forbids in its state (nodes [B, N, F] / edges [B, N, N, Ef], float in the generator, int8 in route batches), OR-ed
-// with the attachment-point rule of the slot's scaffold when sc.protect is given.  Terminate is never touched.  The
-// gate, `row` and first_slot mean what they mean for gen_mask_kernel; `row` selects the row of n_nodes and slot_ids
-// only, the state is always [B, ...].  table = V [A * CH] | bond orders [Ef] | implicit-H counts [H].
-template <typename T>
-__global__ void __launch_bounds__(128) gen_action_mask_kernel(ActionLayout L, int F, int apd, int valence,
-                                                              const int* __restrict__ table,
-                                                              const T* __restrict__ nodes, const T* __restrict__ edges,
-                                                              const int* __restrict__ n_nodes, gib_scaffolds sc,
-                                                              const int* __restrict__ slot_ids,
-                                                              const int* __restrict__ row,
-                                                              const int* __restrict__ state,
-                                                              const int* __restrict__ counters,
-                                                              float* __restrict__ logits, int first_slot) {
-  __shared__ int s_used[128], s_limit[128];
-  const int b = blockIdx.x, B = gridDim.x, N = L.N, Ef = L.Ef;
-  if (b < first_slot) return;
-  if (state && !(counters[0] < B && state[1] == 0 && state[0] >= 0 && state[0] < 2 * N)) return;
-  const size_t off = row ? (size_t)row[0] * B : 0;
-  int n;
-  if (n_nodes) {
-    n = min(max(n_nodes[off + b], 0), N);                  // a count outside [0, N] is read as the nearest bound
-  } else {                                                 // the number of non-empty node rows (N <= 127 < 128)
-    int live = 0;
-    if ((int)threadIdx.x < N) {
-      const T* nr = nodes + ((size_t)b * N + threadIdx.x) * F;
-      for (int f = 0; f < F; ++f) live |= nr[f] != T(0);
-    }
-    n = __syncthreads_count(live);
-  }
-  const T* e = edges + (size_t)b * N * N * Ef;
-  const int* V = valence ? table : nullptr;
-  const int* order = valence ? table + L.A * L.CH : nullptr;
-  const int* imp_h = valence ? order + Ef : nullptr;
-  if (valence) {
-    for (int i = threadIdx.x; i < n; i += 128) {
-      const int2 u = atom_usage(nodes + ((size_t)b * N + i) * F, e + (size_t)i * N * Ef, L, V, order, imp_h);
-      s_used[i] = u.x;
-      s_limit[i] = u.y;
-    }
-    __syncthreads();
-  }
-  const Valence v{s_used, s_limit, V, order, imp_h};
-  const unsigned int* pm = nullptr;
-  int k = 0;
-  if (sc.protect) {
-    const int s = slot_ids[off + b];
-    if (s >= 0 && s < sc.S) {
-      pm = sc.protect + (size_t)s * 4;
-      k = sc.n_atoms[s];
-    }
-  }
-  const int per_node = (apd - 1) / N - Ef;
-  float* o = logits + (size_t)b * apd;
-  for (int a = threadIdx.x; a < apd - 1; a += 128)
-    if (action_forbidden(a, L, n, e, valence != 0, v) ||
-        (pm && scaffold_forbidden(a, n, k, pm, N, Ef, per_node)))
-      o[a] = -INFINITY;
-}
-
-// the inputs of the constrained rule that every CTA of the two kernels below sets up the same way: the atom count,
-// the valence table, the attachment-point mask of the slot's scaffold
-struct ConsSlot {
+// what every CTA of the action mask and of the constraint check sets up the same way from one state (node rows nb
+// [N, F], edges e [N, N, Ef]): the atom count n (n_nodes[idx] read as the nearest bound of [0, N], or the number of
+// non-empty node rows when n_nodes is null; N <= 127 < 128), the valence usage of its atoms into s_used / s_limit
+// (valence mode) and the attachment-point mask pm of the scaffold slot_ids[idx] with its k atoms (null without
+// attachment points or for an id outside [0, S); slot_ids is given whenever sc.protect is)
+struct SlotRules {
   int n, k;
   const unsigned int* pm;
 };
 
 template <typename T>
-__device__ __forceinline__ ConsSlot cons_slot(const ActionLayout& L, int F, int valence, const int* __restrict__ table,
-                                              const T* __restrict__ nb, const T* __restrict__ e,
-                                              const int* __restrict__ n_nodes, size_t idx, const gib_scaffolds& sc,
-                                              const int* __restrict__ slot_ids, int* s_used, int* s_limit) {
-  ConsSlot r{0, 0, nullptr};
+__device__ __forceinline__ SlotRules slot_rules(const ActionLayout& L, int F, int valence, const int* __restrict__ table,
+                                                const T* __restrict__ nb, const T* __restrict__ e,
+                                                const int* __restrict__ n_nodes, const int* __restrict__ slot_ids,
+                                                size_t idx, const gib_scaffolds& sc, int* s_used, int* s_limit) {
+  SlotRules r{0, 0, nullptr};
   const int N = L.N;
   if (n_nodes) {
     r.n = min(max(n_nodes[idx], 0), N);
@@ -382,7 +332,7 @@ __device__ __forceinline__ ConsSlot cons_slot(const ActionLayout& L, int F, int 
     }
     __syncthreads();
   }
-  if (sc.protect && slot_ids) {
+  if (sc.protect) {
     const int s = slot_ids[idx];
     if (s >= 0 && s < sc.S) {
       r.pm = sc.protect + (size_t)s * 4;
@@ -392,47 +342,49 @@ __device__ __forceinline__ ConsSlot cons_slot(const ActionLayout& L, int F, int 
   return r;
 }
 
-// gen_action_mask_kernel with the constraint rule (constraints.cuh) in the same launch: -inf into every entry any of
-// the rules forbids, and into terminate while the state is under a minimum and some other entry survives (a
-// block-wide OR over the row).  Same arguments and gating, plus the constraint table.
-template <typename T>
-__global__ void __launch_bounds__(128) gen_constrained_mask_kernel(ActionLayout L, int F, int apd, int valence,
-                                                                   const int* __restrict__ table,
-                                                                   const T* __restrict__ nodes,
-                                                                   const T* __restrict__ edges,
-                                                                   const int* __restrict__ n_nodes, gib_scaffolds sc,
-                                                                   const int* __restrict__ slot_ids,
-                                                                   const int* __restrict__ row,
-                                                                   const int* __restrict__ state,
-                                                                   const int* __restrict__ counters,
-                                                                   float* __restrict__ logits, int first_slot,
-                                                                   const int* __restrict__ cons) {
+// the action mask (action_mask.cuh): one CTA per slot, -inf into every entry of the slot's logits row that the rule
+// forbids in its state (nodes [B, N, F] / edges [B, N, N, Ef], float in the generator, int8 in route batches), OR-ed
+// with the attachment-point rule of the slot's scaffold when sc.protect is given.  The gate, `row` and first_slot mean
+// what they mean for gen_mask_kernel; `row` selects the row of n_nodes and slot_ids only, the state is always
+// [B, ...].  table = V [A * CH] | bond orders [Ef] | implicit-H counts [H].  Terminate is never touched, except with
+// kCons: the constraint rule (constraints.cuh, table `cons`) joins the OR, and terminate gets -inf while the state is
+// under a minimum and some other entry survives (a block-wide OR over the row).
+template <typename T, bool kCons>
+__global__ void __launch_bounds__(128) gen_action_mask_kernel(ActionLayout L, int F, int apd, int valence,
+                                                              const int* __restrict__ table,
+                                                              const T* __restrict__ nodes, const T* __restrict__ edges,
+                                                              const int* __restrict__ n_nodes, gib_scaffolds sc,
+                                                              const int* __restrict__ slot_ids,
+                                                              const int* __restrict__ row,
+                                                              const int* __restrict__ state,
+                                                              const int* __restrict__ counters,
+                                                              float* __restrict__ logits, int first_slot,
+                                                              const int* __restrict__ cons) {
   __shared__ int s_used[128], s_limit[128];
-  __shared__ ConsState s;
+  __shared__ ConsState s;                                  // referenced, and so allocated, with kCons only
   const int b = blockIdx.x, B = gridDim.x, N = L.N, Ef = L.Ef;
-  if (b < first_slot) return;
-  if (state && !(counters[0] < B && state[1] == 0 && state[0] >= 0 && state[0] < 2 * N)) return;
+  if (b < first_slot || round_gated_off(state, counters, B, N)) return;
   const size_t off = row ? (size_t)row[0] * B : 0;
   const T* nb = nodes + (size_t)b * N * F;
   const T* e = edges + (size_t)b * N * N * Ef;
-  const ConsSlot cs = cons_slot(L, F, valence, table, nb, e, n_nodes ? n_nodes + off : nullptr, b, sc,
-                                slot_ids ? slot_ids + off : nullptr, s_used, s_limit);
+  const SlotRules r = slot_rules(L, F, valence, table, nb, e, n_nodes, slot_ids, off + b, sc, s_used, s_limit);
   const ConsTable ct{cons, L.A, L.CH};
-  cons_load(s, ct, L, F, nb, e, cs.n);
+  if constexpr (kCons) cons_load(s, ct, L, F, nb, e, r.n);
   const int* order = valence ? table + L.A * L.CH : nullptr;
   const Valence v{s_used, s_limit, valence ? table : nullptr, order, valence ? order + Ef : nullptr};
   const int per_node = (apd - 1) / N - Ef;
   float* o = logits + (size_t)b * apd;
   int survives = 0;
   for (int a = threadIdx.x; a < apd - 1; a += 128) {
-    if (action_forbidden(a, L, cs.n, e, valence != 0, v) ||
-        (cs.pm && scaffold_forbidden(a, cs.n, cs.k, cs.pm, N, Ef, per_node)) ||
-        cons_forbidden(decode_action(a, L), s, ct))
+    if (action_forbidden(a, L, r.n, e, valence != 0, v) ||
+        (r.pm && scaffold_forbidden(a, r.n, r.k, r.pm, N, Ef, per_node)) ||
+        (kCons && cons_forbidden(decode_action(a, L), s, ct)))
       o[a] = -INFINITY;
     else
       survives = 1;
   }
-  if (__syncthreads_or(survives) && s.below && threadIdx.x == 0) o[apd - 1] = -INFINITY;
+  if constexpr (kCons)
+    if (__syncthreads_or(survives) && s.below && threadIdx.x == 0) o[apd - 1] = -INFINITY;
 }
 
 // gib_constraints_check: one CTA per finished molecule, its flag bits (GIB_CONS_*)
@@ -449,7 +401,7 @@ __global__ void __launch_bounds__(128) constraints_check_kernel(ActionLayout L, 
   const int g = blockIdx.x, N = L.N, Ef = L.Ef;
   const T* nb = nodes + (size_t)g * N * F;
   const T* e = edges + (size_t)g * N * N * Ef;
-  const ConsSlot cs = cons_slot(L, F, valence, table, nb, e, n_nodes, g, sc, scaffold_ids, s_used, s_limit);
+  const SlotRules cs = slot_rules(L, F, valence, table, nb, e, n_nodes, scaffold_ids, g, sc, s_used, s_limit);
   const ConsTable ct{cons, L.A, L.CH};
   cons_load(s, ct, L, F, nb, e, cs.n);
   int f = cons_over_max(s, ct, L.A, L.CH, Ef) ? GIB_CONS_OVER_MAX : 0;
@@ -714,36 +666,35 @@ extern "C" int gib_generation_scaffold_init(int B, int N, int F, int Ef, const g
   return 0;
 }
 
-extern "C" int gib_generation_mask_logits(int B, int N, int Ef, int apd, const gib_scaffolds* sc, const int* slot_ids,
-                                          const int* n_nodes, const int* row, const int* state, const int* counters,
-                                          float* logits, gib_stream stream) {
+// the attachment-point mask alone (`who` names the entry point; first_slot and the gate as for gen_mask_kernel)
+static int attachment_mask_launch(const char* who, int B, int N, int Ef, int apd, const gib_scaffolds* sc,
+                                  const int* slot_ids, const int* n_nodes, const int* row, const int* state,
+                                  const int* counters, float* logits, int first_slot, gib_stream stream) {
   if (!sc || sc->S <= 0 || !sc->n_atoms || B <= 0 || N <= 0 || N > 127 || Ef <= 0 || apd < 1 ||
       (apd - 1) % N != 0 || (apd - 1) / N <= Ef || !slot_ids || !n_nodes || !logits || (!state != !counters)) {
-    set_error("gib_generation_mask_logits: bad arguments (B=%d N=%d Ef=%d apd=%d; apd - 1 must be N times the "
-              "per-node add and connect lengths, the table, slot_ids, n_nodes and logits must be given, and state "
-              "and counters together or neither)", B, N, Ef, apd);
+    set_error("%s: bad arguments (B=%d N=%d Ef=%d apd=%d; apd - 1 must be N times the per-node add and connect "
+              "lengths, the table, slot_ids, n_nodes and logits must be given, and state and counters together or "
+              "neither)", who, B, N, Ef, apd);
     return -1;
   }
   if (!sc->protect) return 0;       // no attachment points: nothing is masked
   gen_mask_kernel<<<B, 128, 0, reinterpret_cast<cudaStream_t>(stream)>>>(N, Ef, apd, *sc, slot_ids, n_nodes, row,
-                                                                         state, counters, logits, 1);
+                                                                         state, counters, logits, first_slot);
   GIB_LAUNCH_CHECK();
   return 0;
 }
 
+extern "C" int gib_generation_mask_logits(int B, int N, int Ef, int apd, const gib_scaffolds* sc, const int* slot_ids,
+                                          const int* n_nodes, const int* row, const int* state, const int* counters,
+                                          float* logits, gib_stream stream) {
+  return attachment_mask_launch("gib_generation_mask_logits", B, N, Ef, apd, sc, slot_ids, n_nodes, row, state,
+                                counters, logits, 1, stream);
+}
+
 extern "C" int gib_route_mask_logits(int B, int N, int Ef, int apd, const gib_scaffolds* sc, const int* slot_ids,
                                      const int* n_nodes, float* logits, gib_stream stream) {
-  if (!sc || sc->S <= 0 || !sc->n_atoms || B <= 0 || N <= 0 || N > 127 || Ef <= 0 || apd < 1 ||
-      (apd - 1) % N != 0 || (apd - 1) / N <= Ef || !slot_ids || !n_nodes || !logits) {
-    set_error("gib_route_mask_logits: bad arguments (B=%d N=%d Ef=%d apd=%d; apd - 1 must be N times the per-node "
-              "add and connect lengths, and the table, slot_ids, n_nodes and logits must be given)", B, N, Ef, apd);
-    return -1;
-  }
-  if (!sc->protect) return 0;       // no attachment points: nothing is masked
-  gen_mask_kernel<<<B, 128, 0, reinterpret_cast<cudaStream_t>(stream)>>>(N, Ef, apd, *sc, slot_ids, n_nodes, nullptr,
-                                                                         nullptr, nullptr, logits, 0);
-  GIB_LAUNCH_CHECK();
-  return 0;
+  return attachment_mask_launch("gib_route_mask_logits", B, N, Ef, apd, sc, slot_ids, n_nodes, nullptr, nullptr,
+                                nullptr, logits, 0, stream);
 }
 
 // the arguments of the action mask and of the constraint check (`who` names the entry point); *scv receives the
@@ -802,23 +753,15 @@ static int action_mask_launch(const char* who, int B, int N, int F, int Ef, int 
   }
   const ActionLayout L{N, n_atom_types, n_charges, n_imp_H, n_chirality, Ef};
   const int valence = mode == GIB_ACTION_MASK_VALENCE;
-  const bool as_float = nodes && edges;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  if (cons) {
-    if (as_float)
-      gen_constrained_mask_kernel<float><<<B, 128, 0, st>>>(L, F, apd, valence, table, nodes, edges, n_nodes, scv,
-                                                            slot_ids, row, state, counters, logits, first_slot, cons);
-    else
-      gen_constrained_mask_kernel<signed char><<<B, 128, 0, st>>>(L, F, apd, valence, table, nodes_i8, edges_i8,
-                                                                  n_nodes, scv, slot_ids, row, state, counters,
-                                                                  logits, first_slot, cons);
-  } else if (as_float) {
-    gen_action_mask_kernel<float><<<B, 128, 0, st>>>(L, F, apd, valence, table, nodes, edges, n_nodes, scv, slot_ids,
-                                                     row, state, counters, logits, first_slot);
-  } else {
-    gen_action_mask_kernel<signed char><<<B, 128, 0, st>>>(L, F, apd, valence, table, nodes_i8, edges_i8, n_nodes,
-                                                           scv, slot_ids, row, state, counters, logits, first_slot);
-  }
+  auto launch = [&](const auto* nodes_t, const auto* edges_t) {
+    using T = std::decay_t<decltype(*nodes_t)>;                     // float or signed char
+    const auto kernel = cons ? gen_action_mask_kernel<T, true> : gen_action_mask_kernel<T, false>;
+    kernel<<<B, 128, 0, st>>>(L, F, apd, valence, table, nodes_t, edges_t, n_nodes, scv, slot_ids, row, state,
+                              counters, logits, first_slot, cons);
+  };
+  if (nodes && edges) launch(nodes, edges);
+  else launch(nodes_i8, edges_i8);
   GIB_LAUNCH_CHECK();
   return 0;
 }

@@ -41,7 +41,7 @@ from ._lib import Scaffolds, check, lib
 
 
 def _ptr(t):
-    return ctypes.c_void_p(t.data_ptr())
+    return ctypes.c_void_p(t.data_ptr()) if t is not None else None
 
 
 def action_layout(model, constants=None, n_atom_types=None, n_formal_charge=None, n_imp_H=None, n_chirality=None):
@@ -157,10 +157,9 @@ class ScaffoldTable:
     def struct(self, slot_ids=None, started=None, gen_scaffolds=None):
         """the `gib_scaffolds` of this table and the per-batch state buffers (None: null, for the route scorer's
         entry points, which read only the table)"""
-        ptr = lambda t: _ptr(t).value if t is not None else None
-        return Scaffolds(nodes=ptr(self.nodes), edges=ptr(self.edges), n_atoms=ptr(self.n_atoms_dev),
-                         protect=ptr(self.protect), slot_ids=ptr(slot_ids), started=ptr(started),
-                         gen_scaffolds=ptr(gen_scaffolds), S=self.S)
+        return Scaffolds(nodes=_ptr(self.nodes), edges=_ptr(self.edges), n_atoms=_ptr(self.n_atoms_dev),
+                         protect=_ptr(self.protect), slot_ids=_ptr(slot_ids), started=_ptr(started),
+                         gen_scaffolds=_ptr(gen_scaffolds), S=self.S)
 
 
 ACTION_MASK_MODES = {"structure": 1, "valence": 2}          # GIB_ACTION_MASK_* (include/gib200.h)
@@ -374,10 +373,9 @@ class ActionMask:
               state=None, counters=None, first_slot=1):
         """-inf in place into logits [B, apd]; nodes / edges float (int8=False) or int8 [B, ...]; sc (a gib_scaffolds
         with attachment points) and slot_ids: that rule too, in the same launch"""
-        p = lambda t: _ptr(t) if t is not None else None
-        fl = (p(nodes), p(edges), None, None) if not int8 else (None, None, p(nodes), p(edges))
-        args = (B, self.N, self.F, self.Ef, *self.layout, self.apd, self.code, p(self.table), *fl, p(n_nodes),
-                ctypes.byref(sc) if sc is not None else None, p(slot_ids), p(row), p(state), p(counters),
+        fl = (_ptr(nodes), _ptr(edges), None, None) if not int8 else (None, None, _ptr(nodes), _ptr(edges))
+        args = (B, self.N, self.F, self.Ef, *self.layout, self.apd, self.code, _ptr(self.table), *fl, _ptr(n_nodes),
+                ctypes.byref(sc) if sc is not None else None, _ptr(slot_ids), _ptr(row), _ptr(state), _ptr(counters),
                 _ptr(logits), first_slot, stream)
         if self.cons_table is not None:
             check(lib.gib_action_mask_logits_constrained(*args, _ptr(self.cons_table)),
@@ -402,15 +400,27 @@ class ActionMask:
         if scaffold_ids is not None:
             ids = torch.as_tensor(scaffold_ids).to(device=nodes.device, dtype=torch.int32).contiguous()
         flags = out if out is not None else torch.zeros(M, dtype=torch.int32, device=nodes.device)
-        p = lambda t: _ptr(t) if t is not None else None
         i8 = nodes.dtype == torch.int8
         fl = (None, None, _ptr(nodes), _ptr(edges)) if i8 else (_ptr(nodes), _ptr(edges), None, None)
         st = stream if stream is not None else torch.cuda.current_stream(nodes.device).cuda_stream
-        check(lib.gib_constraints_check(M, self.N, self.F, self.Ef, *self.layout, self.code, p(self.table), *fl,
-                                        p(cnt), ctypes.byref(sc) if sc is not None else None,
-                                        p(ids) if sc is not None else None, _ptr(self.cons_table), _ptr(flags), st),
+        check(lib.gib_constraints_check(M, self.N, self.F, self.Ef, *self.layout, self.code, _ptr(self.table), *fl,
+                                        _ptr(cnt), ctypes.byref(sc) if sc is not None else None,
+                                        _ptr(ids) if sc is not None else None, _ptr(self.cons_table), _ptr(flags), st),
               "gib_constraints_check")
         return flags
+
+
+def _mask_logits(action_mask, logits, stream, nodes, edges, n_nodes, sc=None, slot_ids=None, int8=False, row=None,
+                 state=None, counters=None, first_slot=1):
+    """-inf in place into logits [B, apd]: `action_mask.apply`, or without one the attachment points of sc / slot_ids
+    alone by `gib_generation_mask_logits` (first_slot 1) or `gib_route_mask_logits` (0; no row or gate)"""
+    if action_mask is not None:
+        return action_mask.apply(logits.shape[0], logits, n_nodes, stream, nodes, edges, int8, sc, slot_ids, row,
+                                 state, counters, first_slot)
+    B, apd = logits.shape
+    name, gate = ("gib_generation_mask_logits", (row, state, counters)) if first_slot else ("gib_route_mask_logits", ())
+    check(getattr(lib, name)(B, edges.shape[1], edges.shape[3], apd, ctypes.byref(sc), _ptr(slot_ids), _ptr(n_nodes),
+                             *map(_ptr, gate), _ptr(logits), stream), name)
 
 
 def make_action_mask(mode, max_valence, constants, layout, N, F, Ef, apd, device, constraints=None):
@@ -428,6 +438,32 @@ def make_action_mask(mode, max_valence, constants, layout, N, F, Ef, apd, device
     return ActionMask(mode, max_valence, constants, layout, N, F, Ef, apd, device, constraints)
 
 
+class _LogitMasks:
+    """The logit masks of a generator or the route scorer: `action_mask` (rebuilt from `_mask_args`), `scaffolds`"""
+
+    @property
+    def constraints(self):
+        """the constraint set of the following batches or scores (`Constraints`, bound to the mask for `check`)"""
+        return self.action_mask.constraints if self.action_mask is not None else None
+
+    def set_constraints(self, constraints=None):
+        """the constraint set of the following batches or scores (None: none); rebuilds the mask if it has no table"""
+        if constraints is not None and self.action_mask is not None and self.action_mask.cons_table is not None:
+            self.action_mask.set_constraints(constraints)
+        else:
+            self.action_mask = make_action_mask(*self._mask_args, constraints)
+            self._masks_rebuilt()
+        self.constraints_version += 1
+
+    def _masks_rebuilt(self):
+        """the action mask object was replaced (captured objects capture again)"""
+
+    @property
+    def masked(self):
+        """True when the scaffolds' attachment points restrict the actions"""
+        return self.scaffolds is not None and self.scaffolds.protect is not None
+
+
 def scaffold_table(scaffolds, attachment, N, F, Ef, layout, device):
     """the ScaffoldTable of `set_scaffolds`' arguments (None for None), for the generators and the route scorer"""
     if scaffolds is None:
@@ -438,7 +474,7 @@ def scaffold_table(scaffolds, attachment, N, F, Ef, layout, device):
     return ScaffoldTable(nodes, edges, attachment, N, F, Ef, layout, device)
 
 
-class GraphGenerator:
+class GraphGenerator(_LogitMasks):
     """`scaffolds=(nodes, edges)` / `attachment=`: decorate those scaffolds instead of growing molecules from the empty
     graph (`ScaffoldTable`; `set_scaffolds` changes them).  None (the default) keeps the reference's behaviour.
 
@@ -471,9 +507,9 @@ class GraphGenerator:
         self.rounds = 0
         self.scaffolds = None
         self.generated_scaffolds = None
-        self._mask_args, self.constraints_version = (action_mask, max_valence), 0
-        self.action_mask = make_action_mask(action_mask, max_valence, C, self.layout, self.N, self.F, self.Ef, self.apd,
-                                            self.device, constraints)
+        self._mask_args = (action_mask, max_valence, C, self.layout, self.N, self.F, self.Ef, self.apd, self.device)
+        self.constraints_version = 0
+        self.action_mask = make_action_mask(*self._mask_args, constraints)
         self._allocate()
         if scaffolds is not None:
             self.set_scaffolds(scaffolds, attachment)
@@ -481,29 +517,6 @@ class GraphGenerator:
     @property
     def layout(self):
         return (self.A, self.CH, self.n_imp_H, self.n_chirality)
-
-    @property
-    def constraints(self):
-        """the constraint set of the following batches (`Constraints`, bound to this generator's mask for `check`),
-        or None"""
-        return self.action_mask.constraints if self.action_mask is not None else None
-
-    def set_constraints(self, constraints=None):
-        """the constraint set of the following batches (None: none).  A generator that already has a constraint table
-        rewrites it in place; otherwise the mask is rebuilt (a captured generator captures its round again, once)."""
-        if constraints is not None and not isinstance(constraints, Constraints):
-            raise TypeError(f"constraints must be a generation.Constraints, got {type(constraints).__name__}")
-        m = self.action_mask
-        if constraints is not None and m is not None and m.cons_table is not None:
-            m.set_constraints(constraints)
-        else:
-            self.action_mask = make_action_mask(*self._mask_args, self.constants, self.layout, self.N, self.F, self.Ef,
-                                                self.apd, self.device, constraints)
-            self._masks_rebuilt()
-        self.constraints_version += 1
-
-    def _masks_rebuilt(self):
-        """the action mask object was replaced (captured subclasses capture again)"""
 
     @property
     def sampling(self):
@@ -537,24 +550,10 @@ class GraphGenerator:
                                                _ptr(self.nodes), _ptr(self.edges), _ptr(self.n_nodes),
                                                _ptr(self.likelihoods), stream), "gib_generation_scaffold_init")
 
-    def _mask(self, logits, stream, slot_ids=None, n_nodes=None):
-        """-inf into the logits [B, apd] (in place) of the actions the attachment points and the action mask forbid in
-        this round's state"""
-        if self.action_mask is not None:
-            self.action_mask.apply(self.batch_size, logits, self.n_nodes, stream, self.nodes, self.edges,
-                                   sc=self._sc if self.masked else None,
-                                   slot_ids=self._slot_ids if self.masked else None)
-            return
-        check(lib.gib_generation_mask_logits(
-            self.batch_size, self.N, self.Ef, self.apd, ctypes.byref(self._sc),
-            _ptr(slot_ids if slot_ids is not None else self._slot_ids),
-            _ptr(n_nodes if n_nodes is not None else self.n_nodes), None, None, None, _ptr(logits), stream),
-            "gib_generation_mask_logits")
-
-    @property
-    def masked(self):
-        """True when attachment points restrict the actions"""
-        return self.scaffolds is not None and self.scaffolds.protect is not None
+    def _mask(self, logits, stream):
+        """-inf into logits [B, apd] (in place) where this round's state makes the masks forbid an action"""
+        sc, ids = (self._sc, self._slot_ids) if self.masked else (None, None)
+        _mask_logits(self.action_mask, logits, stream, self.nodes, self.edges, self.n_nodes, sc, ids)
 
     @property
     def masks_logits(self):

@@ -89,7 +89,7 @@ from .config import matmul_code
 from ._lib import (CONS_OVER_MAX, CONS_SMALL_RING, CONS_UNDER_MIN, FLAG_MULTITYPE, FLAG_OVERFLOW, HDR_FLAGS,
                    HDR_INTS, PP_STATUS_INTS, ROUTE_ACTION, ROUTE_BAD_ID, ROUTE_MASKED, ROUTE_NOT_PREFIX, EvalPass, check,
                    lib)
-from .generation import GraphGenerator
+from .generation import GraphGenerator, _LogitMasks, _mask_logits
 
 _u8 = torch.uint8
 
@@ -794,15 +794,9 @@ class GraphedGenerator(GraphGenerator):
 
     def _mask_round(self, logits, st):
         """the attachment and action masks on a captured round's logits, gated by the round state"""
-        if self.action_mask is not None:
-            self.action_mask.apply(self.batch_size, logits, self.n_nodes, st, self.nodes, self.edges,
-                                   sc=self._sc if self.masked else None,
-                                   slot_ids=self._slot_ids if self.masked else None, state=self._state,
-                                   counters=self._counters)
-            return
-        check(lib.gib_generation_mask_logits(self.batch_size, self.N, self.Ef, self.apd, ctypes.byref(self._sc),
-                                             F._ptr(self._slot_ids), F._ptr(self.n_nodes), None, F._ptr(self._state),
-                                             F._ptr(self._counters), F._ptr(logits), st), "gib_generation_mask_logits")
+        sc, ids = (self._sc, self._slot_ids) if self.masked else (None, None)
+        _mask_logits(self.action_mask, logits, st, self.nodes, self.edges, self.n_nodes, sc, ids, state=self._state,
+                     counters=self._counters)
 
     def _pack(self):
         self.model._check_dropout()
@@ -1105,22 +1099,14 @@ class GraphedGeneratorRL(GraphedGenerator):
                                  F._ptr(b.ctl), F._ptr(self.in_nodes), F._ptr(self.in_edges), st), "gib_rl_restore")
         _k0_forward(self, self.in_nodes, self.in_edges, [(self.packed[slot], self.logits[0])], st)
         sampled = self.logits[0]
-        if self.action_mask is not None:
+        if self.masks_logits:
             # the rollout's masks, from the restored state and the round's recorded atom counts (and scaffold ids), on
             # a copy: the model backward reads the unmasked output
             sampled = self.logits[1]
             sampled.copy_(self.logits[0])
-            self.action_mask.apply(B, sampled, self.rec_n, st, self.in_nodes, self.in_edges, int8=True,
-                                   sc=self._sc if self.masked else None,
-                                   slot_ids=self.rec_ids if self.masked else None, row=b.ctl)
-        elif self.masked:
-            # the rollout's mask, from the round's recorded scaffold ids and atom counts, on a copy: the model backward
-            # reads the unmasked output
-            sampled = self.logits[1]
-            sampled.copy_(self.logits[0])
-            check(lib.gib_generation_mask_logits(B, self.N, self.Ef, self.apd, ctypes.byref(self._sc),
-                                                 F._ptr(self.rec_ids), F._ptr(self.rec_n), F._ptr(b.ctl), None, None,
-                                                 F._ptr(sampled), st), "gib_generation_mask_logits")
+            sc, ids = (self._sc, self.rec_ids) if self.masked else (None, None)
+            _mask_logits(self.action_mask, sampled, st, self.in_nodes, self.in_edges, self.rec_n, sc, ids, int8=True,
+                         row=b.ctl)
         check(lib.gib_rl_dlogits(B, self.apd, F._ptr(sampled), F._ptr(self.act_rec), F._ptr(b.dp[slot]),
                                  F._ptr(b.ctl), F._ptr(b.dlogits), F._ptr(self.recomputed_p[slot]), st), "gib_rl_dlogits")
         check(lib.gib_model_backward(ctypes.byref(self.d), self.hdr, F._ptr(self.in_nodes), F._ptr(self.in_edges),
@@ -1310,7 +1296,7 @@ def _int8_stack(x, name, ndim):
     return t.contiguous()
 
 
-class RouteScorer:
+class RouteScorer(_LogitMasks):
     """The likelihood of molecules under a model: for every state of each molecule's decoding route (the states
     `PreprocessingGraph.get_decoding_route_state` walks, MolecularGraph.py:676-732), p(action | state) =
     softmax(model(state))[action], the probability the generator gives the action that rebuilds the molecule.
@@ -1417,9 +1403,9 @@ class RouteScorer:
         self.apd = N * (C.len_f_add_per_node + C.len_f_conn_per_node) + 1
         self.chunk = chunk = max(1, int(chunk_molecules))
         from .generation import make_action_mask
-        self._mask_args, self.constraints_version = (action_mask, max_valence), 0
-        self.action_mask = make_action_mask(action_mask, max_valence, C, self.layout, N, F_, Ef, self.apd, dev,
-                                            constraints)
+        self._mask_args = (action_mask, max_valence, C, self.layout, N, F_, Ef, self.apd, dev)
+        self.constraints_version = 0
+        self.action_mask = make_action_mask(*self._mask_args, constraints)
         self.cons_flags = torch.zeros(chunk, dtype=torch.int32, device=dev)
         self.pp = PPDims(N=N, F=F_, Ef=Ef, n_atom_types=A, n_formal_charge=CH, n_imp_H=H, n_chirality=X, batch_size=B)
         pd = ctypes.byref(self.pp)
@@ -1478,31 +1464,9 @@ class RouteScorer:
             self.slot_ids = torch.full((self.B,), -1, dtype=i32, device=self.dev)
             self.slot_n = torch.full((self.B,), -1, dtype=i32, device=self.dev)
 
-    @property
-    def masked(self):
-        """True when the scaffolds' attachment points restrict the actions"""
-        return self.scaffolds is not None and self.scaffolds.protect is not None
-
     # ---- constraints ----------------------------------------------------------------------------------------
-    @property
-    def constraints(self):
-        """the constraint set the routes are scored under (`generation.Constraints`), or None"""
-        return self.action_mask.constraints if self.action_mask is not None else None
-
-    def set_constraints(self, constraints=None):
-        """score under `constraints` from the next score() on (None: none).  In place when the scorer already has a
-        constraint table; otherwise the mask is rebuilt and the graphs are captured again."""
-        from .generation import Constraints, make_action_mask
-        if constraints is not None and not isinstance(constraints, Constraints):
-            raise TypeError(f"constraints must be a generation.Constraints, got {type(constraints).__name__}")
-        m = self.action_mask
-        if constraints is not None and m is not None and m.cons_table is not None:
-            m.set_constraints(constraints)
-        else:
-            self.action_mask = make_action_mask(*self._mask_args, self.constants, self.layout, self.N, self.F,
-                                                self.Ef, self.apd, self.dev, constraints)
-            self.graph, self._sgraph, self._bwd = None, None, None
-        self.constraints_version += 1
+    def _masks_rebuilt(self):
+        self.graph, self._sgraph, self._bwd = None, None, None
 
     def _refuse_constraints(self, n, pos, stop):
         """the ValueError naming the first molecule of the chunk whose route has probability 0 under the constraints"""
@@ -1577,17 +1541,13 @@ class RouteScorer:
     def _mask(self, logits, st, scaffold=True):
         """the action mask (with the attachment points of a conditional batch, in the same launch) or the
         attachment-point mask alone on every slot of the batch, in place"""
-        if self.action_mask is not None:
-            masked = scaffold and self.masked
-            self._sc = self.scaffolds.struct() if masked else None
-            # the atom counts are the states' non-empty node rows: slot_n is -1 for molecules scored whole
-            self.action_mask.apply(self.B, logits, None, st, self.nodes, self.edges,
-                                   int8=True, sc=self._sc, slot_ids=self.slot_ids if masked else None, first_slot=0)
-            return
-        self._sc = self.scaffolds.struct()
-        check(lib.gib_route_mask_logits(self.B, self.N, self.Ef, self.apd, ctypes.byref(self._sc),
-                                        F._ptr(self.slot_ids), F._ptr(self.slot_n), F._ptr(logits), st),
-              "gib_route_mask_logits")
+        masked = scaffold and self.masked
+        self._sc = self.scaffolds.struct() if masked else None
+        # with the action mask the atom counts are the states' non-empty node rows: slot_n is -1 for molecules scored
+        # whole
+        _mask_logits(self.action_mask, logits, st, self.nodes, self.edges,
+                     self.slot_n if self.action_mask is None else None, self._sc,
+                     self.slot_ids if masked else None, int8=True, first_slot=0)
 
     def _enqueue(self, scaffold=False):
         st = F._stream(self.dev)
